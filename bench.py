@@ -1,14 +1,16 @@
 #!/usr/bin/env python
 """bench.py — speaker-embeddings/sec of the ResCNN hot path (BASELINE.json metric).
 
-    python bench.py --gpus 1 --steps K --warmup W            # our arm, one B200
+    python bench.py --gpus 1 --steps K --warmup W            # our arm, one H100
     torchrun ... bench.py --gpus N --steps K --warmup W      # N ranks, one per GPU
     python bench.py --impl reference --steps K --warmup W    # the reference's CPU path (oracle port) on host cores
 
 Headline (the JSON line's own keys): a "step" is one forward of the hot path over one batch of 64 synthetic utterances
 (64 fbank x 160 frames -> 512-d), BASELINE.json configs[1]; N ranks = N utterance-sharded replicas, no collective.
-The K-step timed window is repeated (5..50 windows, >= 0.5 s of device time in total) and the MEDIAN window is
-reported (`windows` holds the spread), so the driver's 20-step runs are not 4-ms single samples.
+Every timed figure is one window of exactly --steps steps after --warmup untimed ones.  --dump-outputs DIR writes
+what the timed path computed in its last step (embeddings.npy; train_loss.npy and allpairs_*.npy when those workloads
+run, with a seeded sample of the parameters and gradients after the last training step) from seeded inputs, so two
+builds can be compared output for output.
 
 Sub-records of the same line (default --workload all):
   "train"    : the triplet training step of BASELINE configs[2] (N=1) / configs[4] (N=8: data parallel, ONE NCCL
@@ -30,7 +32,7 @@ sys.path.insert(0, ROOT)
 METRIC = "speaker-embeddings/sec (64-fbank x 160-frame -> 512-d)"
 FLOP_PER_EMB = 2306670592            # BASELINE.md §2 (forward)
 CONV_TC_FLOP_PER_EMB = 2296381440    # the 11 tensor-core convs: 8 x 3x3 (94,371,840 MAC) + 3 x 5x5 s2 (131,072,000 MAC)
-L2_BYTES = 126 * 1024 * 1024
+L2_BYTES = 50 * 1024 * 1024   # H100 SXM
 
 
 _REAL_STDOUT = None
@@ -52,8 +54,8 @@ def load_peaks():
         d = json.load(open(p))
         return {"tflops_burst": d.get("bf16_tflops"), "tflops_sustained": d.get("bf16_tflops_sustained"),
                 "hbm_gbs": d.get("hbm_gbs"), "source": "measured (MEASURED_PEAKS.json)"}
-    return {"tflops_burst": 1590.0, "tflops_sustained": 1400.0, "hbm_gbs": 6650.0,
-            "source": "fallback (B200_PROFILING.md)"}
+    return {"tflops_burst": 989.0, "tflops_sustained": None, "hbm_gbs": 3350.0,
+            "source": "NVIDIA H100 SXM data sheet (dense FP16, 700 W card; not measured)"}
 
 
 class ClockSampler:
@@ -159,7 +161,7 @@ def pick_cpu_threads(sd, T):
 
 
 def cpu_forward_timer(sd, B, T, budget_s, threads):
-    """Times the oracle's eval forward (restatement of /root/reference/model.py:185-218) on host cores."""
+    """Times the oracle's eval forward (restatement of the reference's model.py:185-218) on host cores."""
     import torch
 
     from oracle import rescnn_oracle as O
@@ -188,13 +190,13 @@ def workload_config(args, world, dtype_note=True):
     return {"workload": f"batch-{B} embedding inference, synthetic 64x{T} fbank, eval-mode BN, "
                         f"DeepSpeakerModel(512,1211) random init (BASELINE configs[1])",
             "batch_per_gpu": B, "frames": T, "parallelism": f"replicas x{world} (utterance-sharded, no collective)",
-            "l2": f"inputs rotate over {nbuf} buffers = {nbuf * in_bytes >> 20} MiB > 126 MiB L2; "
+            "l2": f"inputs rotate over {nbuf} buffers = {nbuf * in_bytes >> 20} MiB > {L2_BYTES >> 20} MiB L2; "
                   f"activations ({B * 1843200 >> 20} MiB/step) are rewritten every step"}
 
 
 def run_reference(args, rank, world):
-    """--impl reference: the reference's own CPU implementation of the path.  /root/reference does not exist
-    on the GPU box, so this runs the oracle port (same PyTorch CPU kernels the reference dispatches to)."""
+    """--impl reference: the reference's CPU implementation of the path, as the oracle port (same PyTorch CPU kernels
+    the reference dispatches to; the reference itself is not a dependency of this repository)."""
     if rank != 0:
         return
     import torch
@@ -270,46 +272,13 @@ class Dist:
         return t.tolist()
 
 
-def timed_windows(D, window, K, min_total_ms=500.0, r_min=5, r_max=50):
-    """Repeats the K-step timed window (each bracketed by barrier + synchronize on both sides, CUDA events on the
-    launching stream) until at least `min_total_ms` of device time has been measured (5..50 windows): a 20-step window
-    of a 0.2 ms step lasts 4 ms, too short for one sample to be trusted or for nvidia-smi to see the load.  Returns the
-    per-window milliseconds, max over ranks window by window."""
-    times = [window()]
-    pilot = D.max_over_ranks(times)[0]
-    R = int(min(r_max, max(r_min, -(-min_total_ms // max(pilot, 1e-3)))))
-    for _ in range(R - 1):
-        times.append(window())
-    return D.max_over_ranks(times)
+def timed_windows(D, window):
+    """Runs the timed window once (exactly --steps steps, bracketed by barrier + synchronize on both sides, CUDA events
+    on the launching stream).  Returns [milliseconds], max over ranks."""
+    return D.max_over_ranks([window()])
 
 
-def conv_kernel_hash():
-    """Content hash of the dominant kernel's sources: profiles/traffic.json stores the ncu DRAM traffic per build."""
-    import hashlib
-
-    h = hashlib.sha1()
-    for f in ("conv3x3_halo.cuh", "conv_umma.cuh", "dsk_ptx.cuh"):
-        with open(os.path.join(ROOT, "deepspeaker_pytorch_b200", "csrc", f), "rb") as fh:
-            h.update(fh.read())
-    return h.hexdigest()[:12]
-
-
-def measured_traffic(B, T):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the 11 tensor-core conv launches of one forward, from the
-    committed `ncu --set full` capture of THIS kernel build (profiles/traffic.json), else None."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            table = json.load(f)
-    except (OSError, ValueError):
-        return None, "profiles/traffic.json missing"
-    key = conv_kernel_hash()
-    for e in table.get("captures", []):
-        if e.get("kernel_hash") == key and e.get("batch") == B and e.get("frames") == T:
-            return e["dram_bytes_per_forward"], e.get("source")
-    return None, f"no ncu capture recorded for kernel build {key} at batch {B}"
-
-
-def bench_infer(args, D):
+def bench_infer(args, D, outputs):
     """The headline: batch-64 eval inference (BASELINE configs[1]) through EmbeddingPipeline."""
     import ctypes
 
@@ -330,6 +299,7 @@ def bench_infer(args, D):
     cur = torch.cuda.current_stream(dev)
     cnt = [0]
     host_ms = []
+    last_emb = [None]
     with torch.no_grad():
         sampler = ClockSampler(D.local_rank)
         if rank == 0:
@@ -349,7 +319,7 @@ def bench_infer(args, D):
             e0.record(cur)
             t_host = time.perf_counter()
             for _ in range(K):
-                pipe.embed_device(xs[cnt[0] % nbuf])
+                last_emb[0] = pipe.embed_device(xs[cnt[0] % nbuf])
                 cnt[0] += 1
             host_ms.append((time.perf_counter() - t_host) * 1e3 / K)
             for st in pipe.lanes:
@@ -361,10 +331,12 @@ def bench_infer(args, D):
         D.barrier()
         if rank == 0:
             sampler.mark()
-        ws = timed_windows(D, window, K)
+        ws = timed_windows(D, window)
         ms = median(ws)
         value = world * B * K / (ms * 1e-3)
         host_ms_value = median(host_ms)
+        pipe.synchronize()
+        outputs["embeddings"] = last_emb[0].cpu().numpy()
 
         # ---- e2e: host buffers through the public API, H2D + D2H inside the timed region -----------
         nhost = 8
@@ -388,7 +360,7 @@ def bench_infer(args, D):
             D.barrier()
             return e0.elapsed_time(e1)
 
-        ws2 = timed_windows(D, window_e2e, K)
+        ws2 = timed_windows(D, window_e2e)
         clocks = sampler.stop() if rank == 0 else None
         ms_e2e = median(ws2)
         e2e_value = world * B * K / (ms_e2e * 1e-3)
@@ -424,14 +396,13 @@ def bench_infer(args, D):
     # the conv chain is timed alone (one forward, two events): the burst figure of MEASURED_PEAKS is its denominator; the
     # sustained figure belongs to the in-production rate, which is measured inside a long back-to-back run
     peak = peaks["tflops_burst"]
-    traffic, traffic_src = measured_traffic(B, T)
     # the production step keeps `lanes` forwards in flight, so launches of different forwards overlap: the in-production
     # rate charges the conv FLOPs with the WHOLE measured step (conv1 and the tail run under other forwards' convs)
     share = conv_ms / step_ms_prof
     overlapped = B * CONV_TC_FLOP_PER_EMB / (ms / K * 1e-3) / 1e12
     roofline = {
         "bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-        "traffic": traffic, "traffic_source": traffic_src,
+        "traffic": None, "traffic_source": "not measured",
         "kernel": "conv3x3_halo_kernel: the 11 tensor-core conv launches of a step (8 x 3x3 s1 + 3 x parity-planar 5x5 s2), "
                   "timed back to back between two CUDA events on the forward's stream (one forward in flight)",
         "flop_per_launch_set": B * CONV_TC_FLOP_PER_EMB, "launch_set_ms": conv_ms,
@@ -450,7 +421,7 @@ def bench_infer(args, D):
         cpu_baseline = {"value": v, "unit": "emb/s", "cores": threads, "host_cpus": os.cpu_count(),
                         "kind": "port",
                         "sample": f"{n_it} forwards of the same batch-{B} workload in {el:.1f} s (oracle port of "
-                                  f"/root/reference/model.py:185-218, torch CPU fp32)"}
+                                  f"the reference's model.py:185-218, torch CPU fp32)"}
     cfg = workload_config(args, world)
     line = {
         "metric": METRIC, "value": value, "unit": "emb/s", "n_gpus": world, "steps": K, "warmup": W,
@@ -459,8 +430,8 @@ def bench_infer(args, D):
         "engine": {"forwards_in_flight": args.lanes,
                    "operands": f"{args.dtype} tensor-core operands (BASELINE names bf16: same width and tensor-pipe rate; bf16 "
                                f"misses the 1e-3 parity bar, --dtype bf16 runs it), fp32 accumulate/BN/fc/norm"},
-        "windows": {"n": len(ws), "timing": "median of n windows of exactly `steps` steps, each bracketed by barrier + "
-                                            "synchronize, CUDA events, max over ranks per window",
+        "windows": {"n": len(ws), "timing": "one window of exactly `steps` steps, bracketed by barrier + synchronize, "
+                                            "CUDA events, max over ranks",
                     "ms_per_step_min": min(ws) / K, "ms_per_step_max": max(ws) / K,
                     "e2e_n": len(ws2), "e2e_ms_per_step_min": min(ws2) / K, "e2e_ms_per_step_max": max(ws2) / K},
         "clocks": clocks,
@@ -512,13 +483,13 @@ def bench_other_dtype(args, D):
             D.barrier()
             return e0.elapsed_time(e1)
 
-        ws = timed_windows(D, window, K, min_total_ms=200.0, r_min=5, r_max=25)
+        ws = timed_windows(D, window)
     ms = median(ws)
     return {"dtype": other, "value": D.world * B * K / (ms * 1e-3), "unit": "emb/s", "ms_per_step": ms / K, "windows": len(ws),
-            "parity": "eval embeddings ~3e-3 vs the fp32 reference (bar 1e-3)" if other == "bf16" else "eval embeddings 4e-4 - 7e-4 (bar 1e-3)"}
+            "parity": "eval embeddings gated at 6e-3 vs the fp32 reference (misses the 1e-3 bar)" if other == "bf16" else "eval embeddings gated at 1e-3"}
 
 
-def bench_allpairs(args, D):
+def bench_allpairs(args, D, outputs):
     """BASELINE configs[3]: 1024-utterance all-pairs distance matrix + top-8 hard-negative select (single GPU,
     launch-latency bound: reported in microseconds).  No reference implementation exists (SURVEY §0 fact 3); the
     CPU figure beside it is the oracle's C restatement (oracle/dsk_oracle.c) on one core."""
@@ -534,7 +505,7 @@ def bench_allpairs(args, D):
         E = torch.randn(N, Dm, device=dev, generator=g)
         sets.append(10.0 * E / E.norm(dim=1, keepdim=True))
     labels = (torch.arange(N, device=dev) // 16).long()
-    K, W = max(20, min(args.steps, 200)), max(3, args.warmup)
+    K, W = args.steps, max(3, args.warmup)
     for i in range(W):
         allpairs_topk(sets[i % 8], labels, k)
     torch.cuda.synchronize()
@@ -544,12 +515,15 @@ def bench_allpairs(args, D):
         torch.cuda.synchronize()
         e0.record()
         for i in range(K):
-            allpairs_topk(sets[i % 8], labels, k)
+            last[0] = allpairs_topk(sets[i % 8], labels, k)
         e1.record()
         torch.cuda.synchronize()
         return e0.elapsed_time(e1)
 
-    ws = [window() for _ in range(5)]
+    last = [None]
+    ws = [window()]
+    outputs["allpairs_idx"] = last[0][0].cpu().numpy().astype("float64")
+    outputs["allpairs_val"] = last[0][1].cpu().numpy().astype("float32")
     us = median(ws) / K * 1e3
     # algorithmic bytes: read E (N x D fp32) + labels, write idx (int64) + val (fp32); flops: N*N*D MACs of the Gram
     alg_bytes = N * Dm * 4 + N * 8 + N * k * 12
@@ -586,7 +560,7 @@ def bench_allpairs(args, D):
 TRAIN_FLOP_PER_UTT = 6911819776     # BASELINE.md §2 (forward + backward)
 
 
-def bench_train(args, D):
+def bench_train(args, D, outputs):
     """BASELINE configs[2] (N=1) / configs[4] (N=8): triplet training step restating train_triplet.py:215-224 with the
     drop-in classes — three train-mode forwards of 128 utterances (issued together through forward_triplet: identical
     results, the three calls and their backwards overlap on three streams), TripletMarginLoss, backward, ONE gradient
@@ -598,8 +572,8 @@ def bench_train(args, D):
 
     dev, world, rank = D.dev, D.world, D.rank
     B, T = 128, args.frames
-    K = max(3, min(args.steps, 10))
-    W = 3
+    K = args.steps
+    W = args.warmup
     model = make_model(args.dtype, dev).train()
     broadcast_parameters(model)
     opt = FusedAdagrad(path_parameters(model), lr=0.1, lr_decay=1e-4, weight_decay=0.0)   # train_triplet.py:70-77,378-382
@@ -633,9 +607,15 @@ def bench_train(args, D):
         return e0.elapsed_time(e1)
 
     last = [None]
-    ws = timed_windows(D, window, K, min_total_ms=600.0, r_min=7, r_max=9)
+    ws = timed_windows(D, window)
     ms = median(ws) / K
     loss_value = float(last[0].item())    # loss of the last timed step (48 distinct batches: no memorisation)
+    outputs["train_loss"] = last[0].detach().double().cpu().numpy().reshape(1)
+    # what the step leaves to its caller beside the loss: the updated parameters and the step's gradients, as a fixed,
+    # seeded sample of 2^20 positions of the flat buckets (the whole bucket is 46.5 MB)
+    sample = torch.randperm(opt.numel, generator=torch.Generator().manual_seed(0))[:1 << 20].sort().values.to(dev)
+    outputs["train_params_sample"] = opt.flat_param[sample].cpu().numpy()
+    outputs["train_grads_sample"] = opt.flat_grad[sample].cpu().numpy()
     # e2e: pinned host inputs copied in (on a copy stream, one batch ahead of the step that consumes it - the prefetch any
     # input pipeline does; every step's 15.7 MB still crosses PCIe inside the timed region), loss read back, every step
     nh = 4
@@ -673,7 +653,7 @@ def bench_train(args, D):
         D.barrier()
         return e0.elapsed_time(e1)
 
-    ws2 = timed_windows(D, window_e2e, K, min_total_ms=300.0, r_min=3, r_max=5)
+    ws2 = timed_windows(D, window_e2e)
     ms2 = median(ws2) / K
     if rank != 0:
         return None
@@ -747,7 +727,11 @@ def main():
     ap.add_argument("--workload", default="all", choices=["all", "infer", "train", "allpairs"],
                     help="all (default): the headline line (batch-64 embedding inference, BASELINE configs[1]) carrying "
                          "`train` (configs[2]/[4]) and `allpairs` (configs[3]) sub-records; infer/train/allpairs: that workload alone")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path computed in its last step as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     args.warmup = max(args.warmup, 3)
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -777,10 +761,11 @@ def main():
         dist.init_process_group("nccl", device_id=D.dev)
 
     line = None
+    outputs = {}
     if args.workload in ("all", "infer"):
-        line = bench_infer(args, D)
+        line = bench_infer(args, D, outputs)
     if args.workload in ("all", "train"):
-        rec = bench_train(args, D)
+        rec = bench_train(args, D, outputs)
         if rank == 0:
             if line is None:
                 line = dict(rec, vs_baseline=None, data="synthetic")
@@ -789,13 +774,19 @@ def main():
     if args.workload == "all" and world == 1:
         line["other_operand_dtype"] = bench_other_dtype(args, D)
     if args.workload in ("all", "allpairs") and rank == 0:
-        rec = bench_allpairs(args, D)
+        rec = bench_allpairs(args, D, outputs)
         if line is None:
             line = dict(rec, n_gpus=1, ms_per_step=rec["value"] / 1e3, scaling="weak", vs_baseline=None, data="synthetic",
                         e2e={"value": rec["value"], "unit": "us", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0})
         else:
             line["allpairs"] = rec
     if rank == 0:
+        if args.dump_outputs:
+            import numpy as np
+
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for name, arr in outputs.items():
+                np.save(os.path.join(args.dump_outputs, f"{name}.npy"), arr)
         emit(line)
     if world > 1:
         dist.barrier()

@@ -1,5 +1,5 @@
-"""B200-native Deep Speaker hot path: drop-in for /root/reference/model.py's DeepSpeakerModel,
-TripletMarginLoss and PairwiseDistance, backed by hand-written sm_100a CUDA behind a C ABI
+"""H100-native Deep Speaker hot path: drop-in for reference model.py's DeepSpeakerModel,
+TripletMarginLoss and PairwiseDistance, backed by hand-written sm_90a CUDA behind a C ABI
 (include/dsk.h, lib/libdsk.so)."""
 from .model import (DeepSpeakerModel, PairwiseDistance, TripletMarginLoss, allpairs_topk,  # noqa: F401
                     select_hard_triplets)

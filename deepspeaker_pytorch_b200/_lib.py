@@ -22,7 +22,7 @@ DSK_F16, DSK_BF16 = 0, 1
 DSK_EVAL, DSK_TRAIN = 0, 1
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--shared", "-Xcompiler", "-fPIC",
 ]
 
@@ -61,7 +61,7 @@ def needs_build() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/*.cu for sm_100a into lib/libdsk.so (nvcc cross-compiles without a GPU).  Safe under concurrent
+    """Compile csrc/*.cu for sm_90a into lib/libdsk.so (nvcc cross-compiles without a GPU).  Safe under concurrent
     callers: an exclusive file lock serialises them and the library is renamed into place."""
     if not force and not needs_build():
         return LIB_PATH

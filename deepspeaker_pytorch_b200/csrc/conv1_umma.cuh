@@ -1,19 +1,19 @@
 // Stage-entry conv1 of the eval forward — 5x5 stride-2 pad-2, 1 -> 64 channels, + folded bn1 + clipped ReLU
-// (/root/reference/model.py:94-97 used at :187-189) — on the tcgen05 tensor cores at fp32-level accuracy.
+// (reference model.py:94-97 used at :187-189) — on the Hopper tensor cores (wgmma) at fp32-level accuracy.
 //
-// The SIMT form of this layer is FP32-issue bound (1600 FMAs per output pixel, 21.5 us per batch-64 forward on
-// B200, as long as a 12-GFLOP tensor-core conv).  Here a CTA builds the im2col operand of 128 output pixels in
-// shared memory (one thread = one pixel = one 128-byte K-major SWIZZLE_128B row) and lets six UMMAs do the math:
+// The SIMT form of this layer is FP32-issue bound (1600 FMAs per output pixel).  Here a CTA builds the im2col operand
+// of 128 output pixels in shared memory (one thread = one pixel = one 128-byte K-major SWIZZLE_128B row) and lets
+// wgmma do the math (each K16 step twice, rows 0-63 and 64-127):
 //   x = x_hi + x_lo, w = w_hi + w_lo (each half a 16-bit float);  x*w ~= x_hi*w_hi + x_lo*w_hi + x_hi*w_lo
 //   A row  = [ x_hi(taps 0..24), 0 x 7 | x_lo(taps 0..24), 0 x 7 ]                      (K = 64)
-//   B1 row = [ w_hi,             0 x 7 | w_hi,             0 x 7 ]  -> 4 UMMAs (K = 64): (x_hi + x_lo) * w_hi
-//   B2 row = [ w_lo,             0 x 7 |        unused            ]  -> 2 UMMAs (K = 32):  x_hi * w_lo
+//   B1 row = [ w_hi,             0 x 7 | w_hi,             0 x 7 ]  -> 4 K16 steps (K = 64): (x_hi + x_lo) * w_hi
+//   B2 row = [ w_lo,             0 x 7 |        unused            ]  -> 2 K16 steps (K = 32):  x_hi * w_lo
 // The dropped x_lo*w_lo term is 2^-22 relative (fp16 halves; 2^-16 with bf16 halves), far below the 16-bit
-// rounding of the activation this kernel stores.  Accumulation is fp32 in TMEM.
-// One tile per CTA, 128 threads, ~36 KB shared memory and 64 TMEM columns: several CTAs share an SM, so one CTA's
-// operand build overlaps another's MMA / epilogue without any intra-CTA pipeline.
+// rounding of the activation this kernel stores.  Accumulation is fp32 in registers.
+// 128 threads (one warpgroup) and ~55 KB of shared memory per CTA: several CTAs share an SM, so one CTA's operand
+// build overlaps another's MMA / epilogue.
 #pragma once
-#include "dsk_ptx.cuh"
+#include "conv_umma.cuh"
 
 namespace dsk {
 
@@ -42,11 +42,10 @@ __global__ void pack_conv1_umma_kernel(const float* __restrict__ w, uint16_t* __
 // out: zero-padded NHWC 16-bit activation (rows n*(T/2+1)+h+1, 33 pixels per row, 64 channels).
 // Tiles: 4 output rows x 32 pixels; n_tiles = B * (T/2) / 4 (T/2 must be a multiple of 4).
 //
-// Persistent, software-pipelined over the CTA's tiles t_0, t_1, ... (tile = blockIdx.x + k * gridDim.x):
-//     iteration i :  wait patch(t_i)  ->  build A[i&1]  ->  prefetch patch(t_{i+2})  ->  issue MMA(t_i)  ->  epilogue(t_{i-1})
-// so the tensor core works on tile i while the threads write tile i-1 out, and the fbank rows of tile i+2 are in
-// flight.  The weight image, the TMEM allocation (2 x 64 columns) and the barriers are set up once per CTA instead of
-// once per tile (round 1: one tile per CTA, 1280 CTAs, 16 KB of weights re-read by each).
+// Persistent over the CTA's tiles t_0, t_1, ... (tile = blockIdx.x + k * gridDim.x):
+//     iteration i :  wait patch(t_i)  ->  build A[i&1]  ->  prefetch patch(t_{i+2})  ->  MMA(t_i)  ->  epilogue(t_i)
+// so the fbank rows of tile i+2 are in flight while tile i is computed.  The weight image and the barriers are set up
+// once per CTA instead of once per tile.
 constexpr int kConv1Threads = 128;
 constexpr int kConv1PatchRows = 11;
 constexpr int kConv1SmemBytes = 2 * 128 * 128 /*A*/ + 2 * 64 * 128 /*B*/ + 2 * kConv1PatchRows * 64 * 4 /*patch*/ + 1024 /*align*/;
@@ -62,22 +61,15 @@ conv1_umma_kernel(const __grid_constant__ CUtensorMap tmX, const uint4* __restri
   uint8_t* sB = sA + 2 * 128 * 128;                     // B1 | B2
   float* patch = reinterpret_cast<float*>(sB + 2 * 64 * 128);   // [2][11][64]
   __shared__ float s_scale[64], s_bias[64];
-  __shared__ __align__(8) uint64_t patch_full[2], mma_done[2];
-  __shared__ uint32_t tmem_ptr;
+  __shared__ __align__(8) uint64_t patch_full[2];
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int hout = T / 2, tiles_h = hout / ROWS;
   pdl_launch_dependents();
-  if (warp == 0) {
-    tmem_alloc(&tmem_ptr, 128);
-    tmem_relinquish();
-  }
   if (tid == 32) {
     tma_prefetch_desc(&tmX);
     mbar_init(&patch_full[0], 1);
     mbar_init(&patch_full[1], 1);
-    mbar_init(&mma_done[0], 1);
-    mbar_init(&mma_done[1], 1);
     fence_barrier_init();
   }
   // parameters are safe to read before the dependency wait; the input batch may come from the preceding kernel of
@@ -89,10 +81,7 @@ conv1_umma_kernel(const __grid_constant__ CUtensorMap tmX, const uint4* __restri
     s_bias[tid] = bias[tid];
   }
   fence_proxy_async_smem();  // B image: generic-proxy writes -> visible to the tensor core's async proxy
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_ptr;
   pdl_wait();
 
   const int my_tiles = (n_tiles - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
@@ -108,44 +97,7 @@ conv1_umma_kernel(const __grid_constant__ CUtensorMap tmX, const uint4* __restri
     if (my_tiles > 1) load_patch(1);
   }
 
-  // epilogue of tile t_i: TMEM lane = pixel; folded BN, clip, 16-bit pack into the (free) A tile of that buffer, then
-  // cooperative stores: 8 lanes write one 128-byte pixel row, so a warp store covers four full lines
-  auto epilogue = [&](int i) {
-    const int b = i & 1;
-    const int t = tile_of(i), n = t / tiles_h, h0 = (t - n * tiles_h) * ROWS;
-    mbar_wait(&mma_done[b], (i >> 1) & 1);
-    tc_fence_after();
-    uint8_t* stage = sA + b * 128 * 128;
-#pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      uint32_t v[32];
-      tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + b * 64 + half * 32, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        float f[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const int c = half * 32 + g * 8 + e;
-          f[e] = fminf(fmaxf(fmaf(__uint_as_float(v[g * 8 + e]), s_scale[c], s_bias[c]), 0.0f), clip_hi);
-        }
-        *reinterpret_cast<uint4*>(stage + tid * 128 + (((half * 4 + g) ^ (tid & 7)) << 4)) =
-            make_uint4(pack2<BF16>(f[0], f[1]), pack2<BF16>(f[2], f[3]), pack2<BF16>(f[4], f[5]), pack2<BF16>(f[6], f[7]));
-      }
-    }
-    tc_fence_before();
-    __syncthreads();
-    const int chunk = tid & 7;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      const int row = k * 16 + (tid >> 3);
-      const uint4 val = *reinterpret_cast<const uint4*>(stage + row * 128 + ((chunk ^ (row & 7)) << 4));
-      const long pix = (static_cast<long>(n) * (hout + 1) + h0 + (row >> 5) + 1) * (WOUT + 1) + 1 + (row & 31);
-      reinterpret_cast<uint4*>(out + pix * 64)[chunk] = val;
-    }
-    __syncthreads();  // the staging tile is the next-but-one operand tile: every row has been copied out before it is rebuilt
-  };
-
+  const int fr = frag_row(), fc = frag_col();
   for (int i = 0; i < my_tiles; ++i) {
     const int b = i & 1;
     mbar_wait(&patch_full[b], (i >> 1) & 1);
@@ -179,33 +131,59 @@ conv1_umma_kernel(const __grid_constant__ CUtensorMap tmX, const uint4* __restri
       }
     }
     fence_proxy_async_smem();  // generic-proxy writes of A -> visible to the tensor core's async proxy
-    tc_fence_before();
     __syncthreads();           // A[b] complete; patch[b] consumed by every thread
     if (tid == 0 && i + 2 < my_tiles) load_patch(i + 2);
-    if (warp == 0) {
-      tc_fence_after();
-      if (elect_one_sync()) {
-        constexpr uint32_t idesc = umma_idesc_f16(128, 64, BF16);
-        const uint64_t da = umma_desc_sw128(smem_u32(sA + b * 128 * 128));
-        const uint64_t db1 = umma_desc_sw128(smem_u32(sB));
-        const uint64_t db2 = umma_desc_sw128(smem_u32(sB + 64 * 128));
-        const uint32_t d = tmem_base + b * 64;
+    // ---- MMA: rows 0-63 and 64-127 of the tile, fp32 accumulators in registers
+    float acc[2][32];
+    {
+      const uint64_t da = gmma_desc_sw128(smem_u32(sA + b * 128 * 128));
+      const uint64_t db1 = gmma_desc_sw128(smem_u32(sB));
+      const uint64_t db2 = gmma_desc_sw128(smem_u32(sB + 64 * 128));
 #pragma unroll
-        for (int k = 0; k < 4; ++k) umma_f16(d, da + 2 * k, db1 + 2 * k, idesc, k > 0 ? 1u : 0u);
+      for (int m = 0; m < 2; ++m)
 #pragma unroll
-        for (int k = 0; k < 2; ++k) umma_f16(d, da + 2 * k, db2 + 2 * k, idesc, 1u);
-        umma_commit(&mma_done[b]);
+        for (int e = 0; e < 32; ++e) acc[m][e] = 0.0f;
+      wgmma_fence();
+#pragma unroll
+      for (int m = 0; m < 2; ++m) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_f16<64, BF16>(acc[m], da + m * kDescRows64 + 2 * k, db1 + 2 * k, k > 0 ? 1u : 0u);
+#pragma unroll
+        for (int k = 0; k < 2; ++k) wgmma_f16<64, BF16>(acc[m], da + m * kDescRows64 + 2 * k, db2 + 2 * k, 1u);
       }
-      __syncwarp();
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc[0]);
+      wgmma_fence_acc(acc[1]);
     }
-    if (i > 0) epilogue(i - 1);  // under MMA(t_i)
-  }
-  if (my_tiles > 0) epilogue(my_tiles - 1);
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 128);
+    __syncthreads();  // every warp's MMAs have read A[b]: it becomes the staging tile
+    // ---- epilogue: folded BN, clip, 16-bit pack into A[b], then cooperative stores: 8 lanes write one 128-byte pixel
+    // row, so a warp store covers four full lines
+    {
+      const int t = tile_of(i), n = t / tiles_h, h0 = (t - n * tiles_h) * ROWS;
+      uint8_t* stage = sA + b * 128 * 128;
+#pragma unroll
+      for (int m = 0; m < 2; ++m)
+#pragma unroll
+        for (int g = 0; g < 8; ++g)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = 64 * m + fr + 8 * h, c = 8 * g + fc;
+            const float f0 = fminf(fmaxf(fmaf(acc[m][4 * g + 2 * h], s_scale[c], s_bias[c]), 0.0f), clip_hi);
+            const float f1 = fminf(fmaxf(fmaf(acc[m][4 * g + 2 * h + 1], s_scale[c + 1], s_bias[c + 1]), 0.0f), clip_hi);
+            *reinterpret_cast<uint32_t*>(stage + sw128_off16(row, c)) = pack2<BF16>(f0, f1);
+          }
+      __syncthreads();
+      const int chunk = tid & 7;
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const int row = k * 16 + (tid >> 3);
+        const uint4 val = *reinterpret_cast<const uint4*>(stage + row * 128 + ((chunk ^ (row & 7)) << 4));
+        const long pix = (static_cast<long>(n) * (hout + 1) + h0 + (row >> 5) + 1) * (WOUT + 1) + 1 + (row & 31);
+        reinterpret_cast<uint4*>(out + pix * 64)[chunk] = val;
+      }
+      __syncthreads();  // the staging tile is the next-but-one operand tile: every row has been copied out before it is rebuilt
+    }
   }
 }
 

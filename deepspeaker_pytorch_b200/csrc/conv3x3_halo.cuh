@@ -1,15 +1,15 @@
-// 3x3 stride-1 convolution on tcgen05 tensor cores with halo-tile reuse (sm_100a) — the eval-forward kernel for
-// the eight BasicBlock convs (/root/reference/model.py:47-50,58,61 used at :69,73), with the folded BatchNorm
+// 3x3 stride-1 convolution on the Hopper tensor cores (wgmma) with halo-tile reuse (sm_90a) — the eval-forward kernel for
+// the eight BasicBlock convs (reference model.py:47-50,58,61 used at :69,73), with the folded BatchNorm
 // affine (:59,62), the residual add (:79) and the clipped ReLU (:36-39) in the epilogue.
 //
-// Why a second conv kernel: on B200 TMA delivery is bound by request rate (~100-170 ns per box per SM whatever its
-// size, tools/micro/tma_bw.cu), and the generic kernel issues one 16 KB A box per tap.  Here:
+// Why a second conv kernel: the generic kernel issues one 16 KB A box per tap, so every input pixel crosses L2 -> shared
+// memory nine times.  Here:
 //   * activations live in a ZERO-PADDED NHWC layout: rows R = n*(H+1)+h+1 (row 0 and the row after every image are
 //     zero), W+1 pixels per row (column 0 is zero), so position Q = R*(W+1) + w+1 and the 3x3 neighbourhood of Q is
 //     Q + (r-1)*(W+1) + (s-1) for every pixel, including image borders (the pads are real zeros in memory);
-//   * an output tile is 128 CONSECUTIVE padded positions; its A operand for one 64-channel chunk is ONE contiguous
-//     TMA box of 128 + 2W + 4 rows (the halo), and every filter tap reads it through a UMMA descriptor whose start
-//     address is shifted by (r*(W+1)+s) rows (row-shifted SWIZZLE_128B descriptors: tools/micro/umma_shift.cu);
+//   * an output tile is 128 (64 in the two-CTA shape) CONSECUTIVE padded positions; its A operand for one 64-channel
+//     chunk is ONE contiguous TMA box of tile + 2W + 4 rows (the halo), and every filter tap reads it through a wgmma descriptor whose start
+//     address is shifted by (r*(W+1)+s) rows (row-shifted SWIZZLE_128B descriptors: the swizzle follows the address);
 //   * weights arrive as one box per filter row (3 taps x N_TILE x 64 ch); with 64 channels all 9 taps stay resident;
 //   * junk outputs (pad positions, 1/(W+1) + 1/(H+1) of the rows) are written as zeros, which keeps the pads zero.
 #pragma once
@@ -28,7 +28,7 @@ constexpr int kHaloMaxStages = 4;
 struct HaloParams {
   int W, H, N;            // OUTPUT image geometry (real pixels); tiles run over its padded position space
   int q_begin;            // first position of tile 0 (= W+1: first real row)
-  int tiles_m, tiles_c;   // 128-position tiles, N_TILE channel tiles
+  int tiles_m, tiles_c;   // HaloSmem::kTileRows-position tiles, N_TILE channel tiles
   int chunks;             // Cin / 64
   int cout;
   // shared-memory carve (runtime): ring depths and buffer counts chosen by the host per layer
@@ -68,8 +68,7 @@ struct HaloParams {
   // sk_flags[cta]; the owner adds those partials in fixed order before its usual epilogue (deterministic).
   int stream_k;
   int sk_q, sk_r;      // CTA i owns units [i*sk_q + min(i, sk_r), (i+1)*sk_q + min(i+1, sk_r)) of the num_tiles * units of the layer
-  float* sk_partial;   // [gridDim.x][N_TILE / 4][128 rows] float4: slab-major, the 128 rows of one 4-column group contiguous
-                       // (a warp's 32 rows read / write 512 contiguous bytes per instruction)
+  float* sk_partial;   // [gridDim.x][accumulator register][consumer thread] fp32: each thread writes / reads its own column
   int* sk_flags;       // [gridDim.x], zero outside a launch
   const uint16_t* res_ptr;  // residual tensor (padded layout, cout channels per position): read straight from global / L2
                             // by the 4-epilogue-warp variant, which has no shared memory to spare for residual tiles
@@ -104,25 +103,19 @@ struct HaloPlan {
   }
 };
 
-// Two CTA shapes of the same kernel (template parameter EW = epilogue warps):
-//   EW = 8: 384 threads, the whole SM (up to 227 KB of shared memory, 512 TMEM columns, 3-tap weight boxes);
-//   EW = 4: 256 threads, <= 128 registers, <= 112.5 KB of shared memory and 256 TMEM columns, so that TWO CTAs share
-//           an SM.  A layer of this network gives an SM only one or two tiles, and a CTA spends ~1.8 us before its
-//           first MMA (launch, barrier / TMEM set-up, first operand fetch) and ~2.8 us after its last one (epilogue of
-//           the last tile) with the tensor pipe idle (clock64 traces, profiles/r02_trace_halo.txt).  With two CTAs per
-//           SM - two tiles of one layer, the early-launched CTA of the next kernel of the chain, or a CTA of another
-//           forward in flight - one CTA's set-up and epilogue run under the other's MMAs.  Weight boxes shrink to one
-//           tap (16 KB at 128 channels).  MEASURED SLOWER (single-tap boxes are TMA-request-rate bound: conv chain
-//           0.216 -> 0.275 ms, profiles/r02_stream_k.md): opt-in through DSK_SMALL_CTA=1, kept for the record.
+// Two CTA shapes of the same kernel (template parameter EW = consumer warps); every consumer warpgroup computes one
+// 64-row slice of a tile and holds its 64 x N_TILE fp32 accumulators in registers:
+//   EW = 8: 384 threads, the whole SM (up to 227 KB of shared memory, 3-tap weight boxes); 128-position tiles;
+//   EW = 4: 256 threads, <= 128 registers per thread and <= 112.5 KB of shared memory, so that TWO CTAs share an SM;
+//           64-position tiles and one-tap weight boxes (16 KB at 128 channels).  Opt-in through DSK_SMALL_CTA=1.
 template <int N_TILE, int EW = 8>
 struct HaloSmem {
+  static_assert(EW == 8 || EW == 4, "two consumer warpgroups (one CTA per SM) or one (two CTAs per SM)");
   static constexpr bool kSmall = EW == 4;
+  static constexpr int kTileRows = 16 * EW;  // positions per tile: 64 per consumer warpgroup
   static constexpr int kTapsPerBox = (N_TILE == 256 || kSmall) ? 1 : 3;  // weight box: 3 taps (48 KB at 128 channels) or 1
   static constexpr int kBStageBytes = kTapsPerBox * N_TILE * 128;
-  static constexpr int kTmemCols = kSmall ? 256 : (N_TILE == 256 ? 512 : 4 * N_TILE);
-  static constexpr int kAccStages = kTmemCols / N_TILE;      // TMEM accumulators
-  static constexpr int kRowDstBytes = 2 * 2 * 128 * 8;              // planar output: per-row destination, two tiles x two epilogue groups
-  static constexpr int kFixedBytes = kRowDstBytes + 512 + 1024;  // + barriers + alignment slack
+  static constexpr int kFixedBytes = 512 + 1024;  // barriers + alignment slack
   static int total(int a_stage_bytes, int a_stages, int b_stages, int stg_bufs, int res_bufs) {
     return a_stages * a_stage_bytes + b_stages * kBStageBytes + (stg_bufs + res_bufs) * kATileBytes + kFixedBytes;
   }
@@ -142,30 +135,28 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* s
                : "memory");
 }
 
-// tmIn : 2-D (C, positions) view of the padded input, box {64, 128 + 2W + 4}
+// tmIn : 2-D (C, positions) view of the padded input, box {64, kTileRows + 2W + 4}
 // tmW  : 3-D (cin, cout, 9 taps) packed weights, box {64, N_TILE, 3}
-// tmOut : 2-D (C, positions) view of the padded output, box {64, 128}   (tmRes: unused since the residual is read from
+// tmOut : 2-D (C, positions) view of the padded output, box {64, kTileRows}   (tmRes: unused since the residual is read from
 //         global memory through HaloParams::res_ptr; kept in the signature)
-constexpr int kHaloThreads = 384;  // EW = 8: 4 control warps + 8 epilogue warps (two per scheduler)
+constexpr int kHaloThreads = 384;  // EW = 8: one control warpgroup + two consumer warpgroups
 constexpr int halo_threads(int ew) { return 128 + 32 * ew; }
 
-// KIND: the compile-time tap plan the MMA issuer runs - 1 = 3x3 (HaloPlan<1>), 2 = parity-planar 5x5 s2 (HaloPlan<2>).
-// One plan per instantiation (and the resident-weights burst only where it can occur, 64-channel 3x3): the kernel is
-// sensitive to its code size - adding the stream-K paths to the SAME instantiation (+45 % instructions, none of them
-// executed) slowed every layer by 12-17 % (profiles/r02_stream_k.md), so each instantiation carries only what it runs.
+// KIND: the compile-time tap plan the consumers run - 1 = 3x3 (HaloPlan<1>), 2 = parity-planar 5x5 s2 (HaloPlan<2>).
+// One plan per instantiation (and the resident-weights burst only where it can occur, 64-channel 3x3): each
+// instantiation carries only what it runs.
 template <int N_TILE, bool BF16, int EW = 8, bool SK = false, int KIND = 1>
 __global__ void __launch_bounds__(128 + 32 * EW, EW == 4 ? 2 : 1)
 conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant__ CUtensorMap tmW,
                     const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmRes,
                     const HaloParams p) {
   using S = HaloSmem<N_TILE, EW>;
-  static_assert(EW == 8 || EW == 4, "8 epilogue warps (one CTA per SM) or 4 (two CTAs per SM)");
-  static_assert(!(EW == 4 && N_TILE == 256), "the two-CTA-per-SM shape has 256 TMEM columns");
-  constexpr bool kSmall = S::kSmall;
   constexpr int kEpiThreads = 32 * EW;
+  constexpr int kCG = EW / 4;   // consumer warpgroups
+  static_assert(!(EW == 4 && N_TILE == 256), "the two-CTA-per-SM shape runs 64- and 128-channel tiles");
+  constexpr int kMW = 1;        // 64-row slices of the tile per consumer warpgroup
+  constexpr int kTM = S::kTileRows;
   const int kAStages = p.a_stages, kBStages = p.b_stages;
-  constexpr int kAcc = S::kAccStages;
-  constexpr int kTmemCols = S::kTmemCols;
   constexpr int kChunksOut = N_TILE / 64;
 
   extern __shared__ uint8_t smem_raw[];
@@ -173,25 +164,18 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem_a + kAStages * p.a_stage_bytes;
   uint8_t* smem_stg = smem_b + kBStages * S::kBStageBytes;
-  uint8_t* smem_res = smem_stg + p.stg_bufs * kATileBytes;
-  uint16_t** row_dst = reinterpret_cast<uint16_t**>(smem_res + p.res_bufs * kATileBytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(row_dst) + S::kRowDstBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_stg + (p.stg_bufs + p.res_bufs) * kATileBytes);
   uint64_t* a_full = bars;
   uint64_t* a_empty = a_full + kHaloMaxStages;
   uint64_t* b_full = a_empty + kHaloMaxStages;
   uint64_t* b_empty = b_full + kHaloMaxStages;
-  uint64_t* tmem_full = b_empty + kHaloMaxStages;
-  uint64_t* tmem_empty = tmem_full + kAcc;
-  uint64_t* res_full = tmem_empty + kAcc;
-  uint64_t* res_empty = res_full + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(res_empty + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   if (threadIdx.x == 0) DSK_TRACE(0, 480);
   if (!p.late_trigger) pdl_launch_dependents();
   const int pitch = p.W + 1;
-  const int halo_rows = kTileM + 2 * p.W + 4;
+  const int halo_rows = kTM + 2 * p.W + 4;
   const int num_tiles = p.tiles_m * p.tiles_c;
 
   // channel tile slowest: a CTA's consecutive tiles (stride gridDim.x) mostly share the weight tile
@@ -199,7 +183,7 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
     const int ct = tile / p.tiles_m;
     const int mt = tile - ct * p.tiles_m;
     c0 = ct * N_TILE;
-    q0 = p.q_begin + mt * kTileM;
+    q0 = p.q_begin + mt * kTM;
   };
 
   // Work iteration shared by all roles.  Without stream-K a segment is a whole tile (tile = blockIdx.x + k * gridDim.x,
@@ -229,20 +213,16 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
     return true;
   };
 
-  // The producer warp owns the operand barriers and starts the first loads before the CTA-wide setup barrier: weight
-  // boxes at once (parameters), the first halo tile right after the dependency wait.  The TMEM allocation and the
-  // scale/bias fetch (a global-memory round trip) then overlap the first operand fetch instead of preceding it.
-  // Prologue, split over two warps so that the two first-use descriptor fetches (~1000 cycles each: the clock64 trace put
-  // the first halo load at cycle 1800 when one thread issued everything in turn) overlap: warp 0 sets up the weight ring
+  // Prologue, split over two warps so that the two first-use descriptor fetches overlap: warp 0 sets up the weight ring
   // and issues the first weight boxes (parameters: no dependency wait), warp 3 sets up the halo ring and issues the first
-  // halo tile right after the dependency wait.  TMEM allocation (warp 2) and the accumulator barriers (warp 1) run beside.
+  // halo tile right after the dependency wait.
   int pre_b = 0;  // weight boxes of the first tile already issued (producer warp only)
   if (warp == 0) {
     if (lane == 0) {
       tma_prefetch_desc(&tmW);
       for (int i = 0; i < kBStages; ++i) {
         mbar_init(&b_full[i], 1);
-        mbar_init(&b_empty[i], 1);
+        mbar_init(&b_empty[i], kCG);  // one arrive per consumer warpgroup
       }
       fence_barrier_init();
       DSK_TRACE(0, 484);
@@ -274,7 +254,7 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
       tma_prefetch_desc(&tmIn);
       for (int i = 0; i < kAStages; ++i) {
         mbar_init(&a_full[i], 1);
-        mbar_init(&a_empty[i], 1);
+        mbar_init(&a_empty[i], kCG);
       }
       fence_barrier_init();
     }
@@ -297,26 +277,8 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
       }
     }
   }
-  if (warp == 1 && lane == 0) {
-    tma_prefetch_desc(&tmOut);
-    for (int i = 0; i < kAcc; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      // a tile with >= 2 output chunks is shared by both epilogue groups (all EW warps arrive); a 64-channel tile
-      // belongs to ONE group of four warps (the groups alternate tiles)
-      mbar_init(&tmem_empty[i], (N_TILE >= 128) ? EW : 4);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 2) {
-    if (lane == 0) DSK_TRACE(0, 487);
-    tmem_alloc(tmem_ptr_smem, kTmemCols);
-    tmem_relinquish();
-    if (lane == 0) DSK_TRACE(0, 488);
-  }
-  tc_fence_before();
+  if (warp == 1 && lane == 0) tma_prefetch_desc(&tmOut);
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   if (threadIdx.x == 0) DSK_TRACE(0, 481);
   pdl_wait();  // everything above (but the producer's first halo tile) touched only parameters
   if (threadIdx.x == 0) DSK_TRACE(0, 482);
@@ -328,329 +290,186 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
     bool first = true;
     int tcount = 1;
     bool a_pre = true;  // the first halo tile was issued in the prologue
-    if constexpr (SK) {
-      int cur = seg_begin();
-      int tile, ub, ue;
-      while (next_seg(cur, tile, ub, ue)) {
-        int c0, q0;
-        decode(tile, c0, q0);
-        for (int u = ub; u < ue; ++u) {
-          const int ch = u / p.nboxes, b = u - ch * p.nboxes;
-          if (p.box_first[b] || u == ub) {  // a plane's halo tile: at its first box, or where this segment enters the plane
-            if (a_pre) {
-              a_pre = false;
-            } else {
-              mbar_wait(&a_empty[as], aph ^ 1);
-              if (elect_one_sync()) {
-                mbar_arrive_expect_tx(&a_full[as], halo_rows * 128);
-                tma_load_2d(smem_a + as * p.a_stage_bytes, &tmIn, &a_full[as], ch * 64,
-                            p.box_plane[b] * p.plane_positions + q0 - (p.W + 2));
-                DSK_TRACE(0, tcount);
-                ++tcount;
-              }
-              __syncwarp();
+    int cur = seg_begin();
+    int tile, ub, ue;
+    while (next_seg(cur, tile, ub, ue)) {
+      int c0, q0;
+      decode(tile, c0, q0);
+      for (int u = ub; u < ue; ++u) {
+        const int ch = u / p.nboxes, b = u - ch * p.nboxes;
+        if (p.box_first[b] || u == ub) {  // a plane's halo tile: at its first box, or where this segment enters the plane
+          if (a_pre) {
+            a_pre = false;
+          } else {
+            mbar_wait(&a_empty[as], aph ^ 1);
+            if (elect_one_sync()) {
+              mbar_arrive_expect_tx(&a_full[as], halo_rows * 128);
+              tma_load_2d(smem_a + as * p.a_stage_bytes, &tmIn, &a_full[as], ch * 64,
+                          p.box_plane[b] * p.plane_positions + q0 - (p.W + 2));
+              DSK_TRACE(0, tcount);
+              ++tcount;
             }
-            if (++as == kAStages) {
-              as = 0;
-              aph ^= 1;
-            }
+            __syncwarp();
           }
-          if (!p.b_resident || first) {
-            if (pre_b > 0) {
-              --pre_b;
-            } else {
-              mbar_wait(&b_empty[bs], bph ^ 1);
-              if (elect_one_sync()) {
-                mbar_arrive_expect_tx(&b_full[bs], S::kBStageBytes);
-                tma_load_3d(smem_b + bs * S::kBStageBytes, &tmW, &b_full[bs], ch * 64, c0, p.box_wtap[b]);
-              }
-              __syncwarp();
-            }
-            if (++bs == kBStages) {
-              bs = 0;
-              bph ^= 1;
-            }
+          if (++as == kAStages) {
+            as = 0;
+            aph ^= 1;
           }
         }
-        first = false;
-      }
-    } else {
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int c0, q0;
-        decode(tile, c0, q0);
-        for (int ch = 0; ch < p.chunks; ++ch) {
-          for (int b = 0; b < p.nboxes; ++b) {
-            if (p.box_first[b]) {
-              if (a_pre) {
-                a_pre = false;
-              } else {
-                mbar_wait(&a_empty[as], aph ^ 1);
-                if (elect_one_sync()) {
-                  mbar_arrive_expect_tx(&a_full[as], halo_rows * 128);
-                  tma_load_2d(smem_a + as * p.a_stage_bytes, &tmIn, &a_full[as], ch * 64,
-                              p.box_plane[b] * p.plane_positions + q0 - (p.W + 2));
-                  DSK_TRACE(0, tcount);
-                  ++tcount;
-                }
-                __syncwarp();
-              }
-              if (++as == kAStages) {
-                as = 0;
-                aph ^= 1;
-              }
+        if (!p.b_resident || first) {
+          if (pre_b > 0) {
+            --pre_b;
+          } else {
+            mbar_wait(&b_empty[bs], bph ^ 1);
+            if (elect_one_sync()) {
+              mbar_arrive_expect_tx(&b_full[bs], S::kBStageBytes);
+              tma_load_3d(smem_b + bs * S::kBStageBytes, &tmW, &b_full[bs], ch * 64, c0, p.box_wtap[b]);
             }
-            if (!p.b_resident || first) {
-              if (pre_b > 0) {
-                --pre_b;
-              } else {
-                mbar_wait(&b_empty[bs], bph ^ 1);
-                if (elect_one_sync()) {
-                  mbar_arrive_expect_tx(&b_full[bs], S::kBStageBytes);
-                  tma_load_3d(smem_b + bs * S::kBStageBytes, &tmW, &b_full[bs], ch * 64, c0, p.box_wtap[b]);
-                }
-                __syncwarp();
-              }
-              if (++bs == kBStages) {
-                bs = 0;
-                bph ^= 1;
-              }
-            }
+            __syncwarp();
+          }
+          if (++bs == kBStages) {
+            bs = 0;
+            bph ^= 1;
           }
         }
-        first = false;
       }
+      first = false;
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (warp-converged loop, one elected lane issues) =====================
-    constexpr uint32_t idesc = umma_idesc_f16(kTileM, N_TILE, BF16);
+  } else if (warp >= 4) {
+    // ===================== consumers: MMA of a segment, then its epilogue ======================================
+    // Warpgroup cg computes the 64-row slices cg*kMW .. cg*kMW + kMW - 1 of every tile (thread rows: frag_row() + 8*h
+    // of each slice).  A cut tile's later parts (stream-K) dump their accumulators for the CTA holding the tile's head.
+    const int cg = (warp >> 2) - 1;
+    const int etid = threadIdx.x - 128;
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    const int fr = frag_row(), fc = frag_col();
+    const bool has_res = (p.flags & CONV_RESIDUAL) != 0;
+    const bool do_clip = (p.flags & CONV_CLIP) != 0;
+    const int rows_real_end = p.N * (p.H + 1) + 1;  // first row index past the last image
+    const uint32_t clip_hi2 = pack2<BF16>(p.clip_hi, p.clip_hi);
+    float acc[kMW][N_TILE / 2];
     int as = 0, bs = 0;
     uint32_t aph = 0, bph = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
     bool first = true;
-    int tcount = 0;
-    if constexpr (SK) {
-      int cur = seg_begin();
-      int tile, ub, ue;
-      while (next_seg(cur, tile, ub, ue)) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        if (lane == 0) DSK_TRACE(1, tcount * 4 + 0);
-        const uint32_t d_tmem = tmem_base + acc * N_TILE;
-        {
-          auto issue_chunks = [&](auto plan_tag) {
-            using Plan = decltype(plan_tag);
-            // units [ub, ue) of this tile (the whole K loop unless stream-K cut the tile): unit u = box b of chunk ch
-            for (int ch = ub / Plan::kBoxes; ch * Plan::kBoxes < ue; ++ch) {
-              uint64_t da0 = 0;
-  #pragma unroll
-              for (int b = 0; b < Plan::kBoxes; ++b) {
-                const int u = ch * Plan::kBoxes + b;
-                if (u < ub || u >= ue) continue;  // warp-uniform
-                if (Plan::first(b) || u == ub) {
-                  mbar_wait(&a_full[as], aph);
-                  tc_fence_after();
-                  if (lane == 0 && u == ub) DSK_TRACE(1, tcount * 4 + 1);
-                  da0 = umma_desc_sw128(smem_u32(smem_a + as * p.a_stage_bytes));
-                }
-                mbar_wait(&b_full[bs], bph);
-                tc_fence_after();
-                const bool rel_a = Plan::last(b) || u == ue - 1;
-                if (elect_one_sync()) {
-                  const uint64_t db0 = umma_desc_sw128(smem_u32(smem_b + bs * S::kBStageBytes));
-  #pragma unroll
-                  for (int t = 0; t < Plan::ntaps(b); ++t) {
-                    const uint64_t da = da0 + static_cast<uint64_t>(Plan::row_i(b, t) * pitch + Plan::col_j(b, t)) * 8;
-  #pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                      umma_f16(d_tmem, da + 2 * k, db0 + (t * (N_TILE * 8) + 2 * k), idesc,
-                               (t > 0 || k > 0) ? 1u : (u > ub ? 1u : 0u));
-                  }
-                  umma_commit(&b_empty[bs]);
-                  if (rel_a) umma_commit(&a_empty[as]);
-                  if (u == ue - 1) umma_commit(&tmem_full[acc]);
-                }
-                __syncwarp();
-                if (++bs == kBStages) {
-                  bs = 0;
-                  bph ^= 1;
-                }
-                if (rel_a) {
-                  if (++as == kAStages) {
-                    as = 0;
-                    aph ^= 1;
-                  }
-                }
-              }
-            }
-          };
-          issue_chunks(HaloPlan<KIND, S::kTapsPerBox>{});
-        }
-        if (lane == 0) DSK_TRACE(1, tcount * 4 + 2);
-        ++tcount;
-        if (++acc == kAcc) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-        first = false;
+    int buf = 0;
+    int ecount = 0;
+    int cur = seg_begin();
+    int tile, ub, ue;
+    // stages read by the last committed weight box: handed back to the producer once a later wait shows it complete
+    int pend_b = -1, pend_a = -1;
+    auto release_pending = [&]() {
+      if (wg_leader) {
+        if (pend_b >= 0) mbar_arrive(&b_empty[pend_b]);
+        if (pend_a >= 0) mbar_arrive(&a_empty[pend_a]);
       }
-    } else {
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        if (lane == 0) DSK_TRACE(1, tcount * 4 + 0);
-        const uint32_t d_tmem = tmem_base + acc * N_TILE;
-        constexpr bool kResident = N_TILE == 64 && KIND == 1 && !kSmall;  // the only shape whose 9 taps fit the ring
+      pend_b = pend_a = -1;
+    };
+    // all taps of one weight box on the halo tile at da0 (committed, not waited for): scale_d = 0 for the first K16 step
+    // when `zero`
+    auto mma_box = [&](uint64_t da0, uint64_t db0, int ntaps_, const int16_t* shifts, bool zero) {
+      wgmma_fence();
+#pragma unroll
+      for (int m = 0; m < kMW; ++m) {
+        const uint64_t dam = da0 + static_cast<uint64_t>(cg * kMW + m) * kDescRows64;
+        for (int t = 0; t < ntaps_; ++t) {
+          const uint64_t da = dam + static_cast<uint64_t>(shifts[t]) * kDescRow;
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            wgmma_f16<N_TILE, BF16>(acc[m], da + 2 * k, db0 + (t * (N_TILE * 8) + 2 * k), (t > 0 || k > 0 || !zero) ? 1u : 0u);
+        }
+      }
+      wgmma_commit();
+    };
+    while (next_seg(cur, tile, ub, ue)) {
+      int c0, q0;
+      decode(tile, c0, q0);
+      // ---------------- MMA over units [ub, ue) of this tile ----------------
+      {
+        constexpr bool kResident = N_TILE == 64 && KIND == 1 && !S::kSmall;  // the only shape whose 9 taps fit the ring
         bool resident = false;
         if constexpr (kResident) resident = p.b_resident != 0;
         if (resident) {
-          // 64-channel 3x3: all nine weight taps stay resident; one straight-line burst of 36 MMAs per tile.
-          // Straight-line issue matters: descriptors are base + compile-time offsets + i*pitch, nothing is read from the
-          // tables between MMAs (the tensor pipe's queue drains while a table-driven issuer computes its next operands).
+          // 64-channel 3x3: all nine weight taps stay resident (three 3-tap boxes); one burst of 36 K16 steps per tile
           mbar_wait(&a_full[as], aph);
-          tc_fence_after();
-          if (lane == 0) DSK_TRACE(1, tcount * 4 + 1);
-          if (first) {
+          if (first)
             for (int b = 0; b < 3; ++b) mbar_wait(&b_full[b], 0);
-            tc_fence_after();
-          }
-          if (elect_one_sync()) {
-            const uint64_t da0 = umma_desc_sw128(smem_u32(smem_a + as * p.a_stage_bytes));
-            const uint64_t db0 = umma_desc_sw128(smem_u32(smem_b));
-  #pragma unroll
-            for (int b = 0; b < 3; ++b) {
-              const uint64_t dab = da0 + static_cast<uint64_t>(b * pitch) * 8;
-  #pragma unroll
+          const uint64_t da0 = gmma_desc_sw128(smem_u32(smem_a + as * p.a_stage_bytes));
+          const uint64_t db0 = gmma_desc_sw128(smem_u32(smem_b));
+          wgmma_fence();
+#pragma unroll
+          for (int m = 0; m < kMW; ++m) {
+            const uint64_t dam = da0 + static_cast<uint64_t>(cg * kMW + m) * kDescRows64;
+#pragma unroll
+            for (int b = 0; b < 3; ++b)
+#pragma unroll
               for (int t = 0; t < 3; ++t)
-  #pragma unroll
+#pragma unroll
                 for (int k = 0; k < 4; ++k)
-                  umma_f16(d_tmem, dab + (t * 8 + 2 * k), db0 + ((b * 3 + t) * (N_TILE * 8) + 2 * k), idesc,
-                           (b > 0 || t > 0 || k > 0) ? 1u : 0u);
-            }
-            umma_commit(&a_empty[as]);
-            umma_commit(&tmem_full[acc]);
+                  wgmma_f16<N_TILE, BF16>(acc[m], dam + static_cast<uint64_t>(b * pitch + t) * kDescRow + 2 * k,
+                                          db0 + ((b * 3 + t) * (N_TILE * 8) + 2 * k), (b > 0 || t > 0 || k > 0) ? 1u : 0u);
           }
-          __syncwarp();
+          wgmma_commit();
+          wgmma_wait<0>();
+          if (wg_leader) mbar_arrive(&a_empty[as]);
           if (++as == kAStages) {
             as = 0;
             aph ^= 1;
           }
         } else {
-          auto issue_chunks = [&](auto plan_tag) {
-            using Plan = decltype(plan_tag);
-            for (int ch = 0; ch < p.chunks; ++ch) {
-              uint64_t da0 = 0;
-  #pragma unroll
-              for (int b = 0; b < Plan::kBoxes; ++b) {
-                if (Plan::first(b)) {
-                  mbar_wait(&a_full[as], aph);
-                  tc_fence_after();
-                  if (lane == 0 && ch == 0 && b == 0) DSK_TRACE(1, tcount * 4 + 1);
-                  da0 = umma_desc_sw128(smem_u32(smem_a + as * p.a_stage_bytes));
-                }
-                mbar_wait(&b_full[bs], bph);
-                tc_fence_after();
-                if (elect_one_sync()) {
-                  const uint64_t db0 = umma_desc_sw128(smem_u32(smem_b + bs * S::kBStageBytes));
-  #pragma unroll
-                  for (int t = 0; t < Plan::ntaps(b); ++t) {
-                    const uint64_t da = da0 + static_cast<uint64_t>(Plan::row_i(b, t) * pitch + Plan::col_j(b, t)) * 8;
-  #pragma unroll
-                    for (int k = 0; k < 4; ++k)
-                      umma_f16(d_tmem, da + 2 * k, db0 + (t * (N_TILE * 8) + 2 * k), idesc,
-                               (b > 0 || t > 0 || k > 0) ? 1u : (ch > 0 ? 1u : 0u));
-                  }
-                  umma_commit(&b_empty[bs]);
-                  if (Plan::last(b)) umma_commit(&a_empty[as]);
-                  if (b == Plan::kBoxes - 1 && ch == p.chunks - 1) umma_commit(&tmem_full[acc]);
-                }
-                __syncwarp();
-                if (++bs == kBStages) {
-                  bs = 0;
-                  bph ^= 1;
-                }
-                if (Plan::last(b)) {
-                  if (++as == kAStages) {
-                    as = 0;
-                    aph ^= 1;
-                  }
+          using Plan = HaloPlan<KIND, S::kTapsPerBox>;
+          // unit u = box b of chunk ch
+          for (int ch = ub / Plan::kBoxes; ch * Plan::kBoxes < ue; ++ch) {
+            uint64_t da0 = 0;
+#pragma unroll
+            for (int b = 0; b < Plan::kBoxes; ++b) {
+              const int u = ch * Plan::kBoxes + b;
+              if (u < ub || u >= ue) continue;
+              if (Plan::first(b) || u == ub) {
+                mbar_wait(&a_full[as], aph);
+                da0 = gmma_desc_sw128(smem_u32(smem_a + as * p.a_stage_bytes));
+              }
+              mbar_wait(&b_full[bs], bph);
+              const bool rel_a = Plan::last(b) || u == ue - 1;
+              int16_t shifts[3];
+#pragma unroll
+              for (int t = 0; t < Plan::ntaps(b); ++t) shifts[t] = static_cast<int16_t>(Plan::row_i(b, t) * pitch + Plan::col_j(b, t));
+              mma_box(da0, gmma_desc_sw128(smem_u32(smem_b + bs * S::kBStageBytes)), Plan::ntaps(b), shifts, u == ub);
+              wgmma_wait<1>();  // the previous box's MMAs are done: its stages go back to the producer
+              release_pending();
+              pend_b = bs;
+              pend_a = rel_a ? as : -1;
+              if (++bs == kBStages) {
+                bs = 0;
+                bph ^= 1;
+              }
+              if (rel_a) {
+                if (++as == kAStages) {
+                  as = 0;
+                  aph ^= 1;
                 }
               }
             }
-          };
-          issue_chunks(HaloPlan<KIND, S::kTapsPerBox>{});
-        }
-        if (lane == 0) DSK_TRACE(1, tcount * 4 + 2);
-        ++tcount;
-        if (++acc == kAcc) {
-          acc = 0;
-          acc_phase ^= 1;
+          }
+          wgmma_wait<0>();
+          release_pending();
         }
         first = false;
+#pragma unroll
+        for (int m = 0; m < kMW; ++m) wgmma_fence_acc(acc[m]);
       }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue: EW / 4 independent GROUPS of four warps ===========================================
-    // A group = 128 threads = the 128 TMEM lanes (thread = one padded output position).  It owns one staging tile, one
-    // named barrier and its own TMA-store queue, and takes 64-channel output chunks whole (two 32-column TMEM loads):
-    //   tiles of >= 128 channels: group g takes chunks g, g + 2, ... of EVERY tile (both groups work on a tile at once);
-    //   64-channel tiles: the groups alternate tiles (two tiles' epilogues in flight).
-    // Round 1 ran all eight warps in lockstep through one chunk at a time (two 256-thread barriers per chunk, one
-    // staging tile): ~2700 cycles per chunk, 5400 per 128-channel tile, of which ~900 per chunk were barrier / load /
-    // store latency every warp sat through (profiles/r02_trace_halo.txt).  The residual is read straight from global
-    // memory (it was written two kernels ago and sits in L2), 64 bytes per thread one step ahead of their use: no
-    // residual tiles through shared memory, whose port the MMA operand fetch saturates.
-    constexpr int kGroups = EW / 4;
-    const int g = (warp - 4) >> 2;
-    const int ew = (warp - 4) & 3;          // == warp % 4 -> TMEM lanes [32*ew, 32*ew+32)
-    const int row = ew * 32 + lane;
-    const int gtid = (threadIdx.x - 128) & 127;
-    const int etid = threadIdx.x - 128;     // group 0's thread 0 carries the trace stamps
-    const int bar_id = 1 + g;
-    constexpr bool kShareTile = kChunksOut >= 2 || kGroups == 1;  // every group works on every tile
-    const int j_first = (kChunksOut >= 2) ? g : 0;
-    const bool has_res = (p.flags & CONV_RESIDUAL) != 0;
-    const bool do_clip = (p.flags & CONV_CLIP) != 0;
-    const int rows_real_end = p.N * (p.H + 1) + 1;  // first row index past the last image
-    const uint32_t clip_hi2 = pack2<BF16>(p.clip_hi, p.clip_hi);
-    uint8_t* stg = smem_stg + g * kATileBytes;
-    uint16_t** my_row_dst = row_dst + g * 256;
-    int nseg = 0;     // segments of this CTA so far (all groups count alike): accumulator stage and phase follow from it
-    int ecount = 0;   // tiles this group has written out
-    int cur = seg_begin();
-    int tile, ub, ue;
-    while (next_seg(cur, tile, ub, ue)) {
-      const int acc = nseg % kAcc;
-      const uint32_t acc_phase = (nseg / kAcc) & 1;
-      const bool mine = kShareTile || (nseg & 1) == g;
-      ++nseg;
-      if (!mine) continue;
-      int c0, q0;
-      decode(tile, c0, q0);
+      // partial accumulators of stream-K: [cta][register][consumer thread] (what one thread writes, the same thread
+      // of the owner CTA reads back)
+      auto sk_slot = [&](int cta, int m, int i) -> float* {
+        return p.sk_partial + (static_cast<size_t>(cta) * (kMW * N_TILE / 2) + m * (N_TILE / 2) + i) * kEpiThreads + etid;
+      };
       if (SK && ub > 0) {
         // ---- stream-K: a later part of a tile.  Dump the raw fp32 accumulator for the tile's owner and raise this CTA's flag.
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after();
-        float4* dst = reinterpret_cast<float4*>(p.sk_partial) + static_cast<size_t>(blockIdx.x) * (N_TILE / 4) * kTileM + row;
-#pragma unroll 1
-        for (int j = j_first; j < kChunksOut; j += kGroups) {
 #pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            uint32_t v[32];
-            tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + acc * N_TILE + j * 64 + half * 32, v);
-            tmem_ld_wait();
-            float4* d4 = dst + static_cast<size_t>(j * 16 + half * 8) * kTileM;   // 4-column group q of the tile at dst[q * 128]
+        for (int m = 0; m < kMW; ++m)
 #pragma unroll
-            for (int qq = 0; qq < 8; ++qq)
-              d4[qq * kTileM] = make_float4(__uint_as_float(v[4 * qq]), __uint_as_float(v[4 * qq + 1]),
-                                            __uint_as_float(v[4 * qq + 2]), __uint_as_float(v[4 * qq + 3]));
-          }
-        }
+          for (int i = 0; i < N_TILE / 2; ++i) __stcg(sk_slot(blockIdx.x, m, i), acc[m][i]);
         __threadfence();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-        named_bar_sync(3, kEpiThreads);  // every thread's partial rows (both groups) are written and fenced
+        named_bar_sync(3, kEpiThreads);  // every consumer thread's partial is written and fenced
         if (etid == 0) st_release_gpu(p.sk_flags + blockIdx.x, 1);
         continue;
       }
@@ -663,42 +482,8 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
                sk_lo(static_cast<int>(blockIdx.x) + 1 + n_parts) < tile_end)
           ++n_parts;
       }
-      const int q = q0 + row;
-      const int R = static_cast<int>(__umulhi(static_cast<unsigned>(q), p.pitch_magic));
-      const int cc = q - R * pitch;
-      const int img = static_cast<int>(__umulhi(static_cast<unsigned>(R), p.img_magic));
-      const bool junk = (cc == 0) || (R - img * (p.H + 1) == 0) || (R >= rows_real_end);
-      // parity-planar destination of this position (only when the consumer is a stride-2 conv): pixel (n, h, w) ->
-      // plane (h&1, w&1), padded position of (n, h>>1, w>>1) on the half-resolution grid
-      if (p.out_planar) {
-        uint16_t* planar_row = nullptr;
-        if (!junk) {
-          const int n = (R - 1 >= 0) ? img : 0;  // R = n*(H+1) + h + 1 with h < H  =>  img == n for real rows
-          const int hh = R - 1 - n * (p.H + 1), ww = cc - 1;
-          const int H2 = p.H >> 1, W2 = p.W >> 1;
-          const long q2 = static_cast<long>(n * (H2 + 1) + (hh >> 1) + 1) * (W2 + 1) + (ww >> 1) + 1;
-          const long plane = (hh & 1) * 2 + (ww & 1);
-          planar_row = p.out_ptr + (plane * p.out_plane_positions + q2) * p.out_C + c0;
-        }
-        // published before this tile's first chunk barrier; two tables per group because a fast thread may enter the
-        // next tile while others still copy this one out
-        my_row_dst[(ecount & 1) * 128 + row] = planar_row;
-      }
-      // residual: the 64 bytes of the first (chunk, half) now, every later one a step ahead of its use
-      const uint16_t* res_g = nullptr;
-      uint4 rn[4] = {};
-      if (has_res) {
-        res_g = p.res_ptr + static_cast<size_t>(q) * p.cout + c0;
-        const uint4* g4 = reinterpret_cast<const uint4*>(res_g + j_first * 64);
-#pragma unroll
-        for (int qq = 0; qq < 4; ++qq) rn[qq] = __ldg(g4 + qq);
-      }
       if (etid == 0) DSK_TRACE(2, ecount * 8 + 0);
       if (p.late_trigger && (sk ? cur >= u_hi : cur >= num_tiles)) pdl_launch_dependents();
-      // stream-K owner: the other parts of this tile were the FIRST work of their CTAs, so they are normally complete long
-      // before this CTA's own MMAs are: wait for their flags now and fetch the first slab of the first part, under the
-      // tail of the MMAs instead of after it
-      float4 pre[8];
       if (SK && n_parts > 0) {
         if (etid == 0) {
           const long long t_wait = clock64();
@@ -709,128 +494,93 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
             }
         }
         named_bar_sync(3, kEpiThreads);
-        const float4* s4 = reinterpret_cast<const float4*>(p.sk_partial) +
-                           (static_cast<size_t>(blockIdx.x + 1) * (N_TILE / 4) + j_first * 16) * kTileM + row;
+        for (int c = 1; c <= n_parts; ++c)  // fixed order: own head part + part 1 + part 2 ...
 #pragma unroll
-        for (int qq = 0; qq < 8; ++qq) pre[qq] = __ldcg(s4 + qq * kTileM);
-      }
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      if (etid == 0) DSK_TRACE(2, ecount * 8 + 1);
-#pragma unroll 1
-      for (int j = j_first; j < kChunksOut; j += kGroups) {
-        if (gtid == 0) tma_store_wait_read<0>();  // the group's previous TMA store has finished reading the staging tile
-        named_bar_sync(bar_id, 128);
-        if (etid == 0 && j == 0) DSK_TRACE(2, ecount * 8 + 2);
-        const uint32_t my_row = smem_u32(stg) + row * 128;
+          for (int m = 0; m < kMW; ++m)
 #pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          uint32_t v[32];
-          tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + acc * N_TILE + j * 64 + half * 32, v);
-          uint4 rc[4] = {rn[0], rn[1], rn[2], rn[3]};
-          if (has_res) {  // next (chunk, half) of this group, if any
-            const int nj = half == 0 ? j : j + kGroups;
-            if (nj < kChunksOut) {
-              const uint4* g4 = reinterpret_cast<const uint4*>(res_g + nj * 64 + (half ^ 1) * 32);
-#pragma unroll
-              for (int qq = 0; qq < 4; ++qq) rn[qq] = __ldg(g4 + qq);
-            }
-          }
-          tmem_ld_wait();
-          if (SK && n_parts > 0) {  // fixed order: own head part + part 1 + part 2 ...
-            for (int c = 1; c <= n_parts; ++c) {
-              const float4* s4 = reinterpret_cast<const float4*>(p.sk_partial) +
-                                 (static_cast<size_t>(blockIdx.x + c) * (N_TILE / 4) + j * 16 + half * 8) * kTileM + row;
-#pragma unroll
-              for (int qq = 0; qq < 8; ++qq) {
-                const float4 t4 = (c == 1 && j == j_first && half == 0) ? pre[qq] : __ldcg(s4 + qq * kTileM);
-                v[4 * qq + 0] = __float_as_uint(__uint_as_float(v[4 * qq + 0]) + t4.x);
-                v[4 * qq + 1] = __float_as_uint(__uint_as_float(v[4 * qq + 1]) + t4.y);
-                v[4 * qq + 2] = __float_as_uint(__uint_as_float(v[4 * qq + 2]) + t4.z);
-                v[4 * qq + 3] = __float_as_uint(__uint_as_float(v[4 * qq + 3]) + t4.w);
-              }
-            }
-          }
-          if (etid == 0 && j == 0 && half == 0) DSK_TRACE(2, ecount * 8 + 3);
-          const int cbase = c0 + j * 64 + half * 32;
-#pragma unroll
-          for (int qq = 0; qq < 4; ++qq) {
-            float f[8];
-            // per-channel scale / bias from the parameter (constant) bank: the index is warp-uniform
-            float scv[8], biv[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              scv[e] = p.scale_c[cbase + qq * 8 + e];
-              biv[e] = p.bias_c[cbase + qq * 8 + e];
-            }
-#pragma unroll
-            for (int e = 0; e < 8; ++e) f[e] = fmaf(__uint_as_float(v[qq * 8 + e]), scv[e], biv[e]);
-            if (has_res) {
-              const uint4 r4 = rc[qq];
-              float2 t;
-              t = unpack2<BF16>(r4.x); f[0] += t.x; f[1] += t.y;
-              t = unpack2<BF16>(r4.y); f[2] += t.x; f[3] += t.y;
-              t = unpack2<BF16>(r4.z); f[4] += t.x; f[5] += t.y;
-              t = unpack2<BF16>(r4.w); f[6] += t.x; f[7] += t.y;
-            }
-            uint4 o;
-            o.x = pack2<BF16>(f[0], f[1]);
-            o.y = pack2<BF16>(f[2], f[3]);
-            o.z = pack2<BF16>(f[4], f[5]);
-            o.w = pack2<BF16>(f[6], f[7]);
-            if (do_clip) {  // on the packed pairs: half the instructions of an fp32 clamp, same result (0 and 20 are exact)
-              o.x = clip2<BF16>(o.x, 0u, clip_hi2);
-              o.y = clip2<BF16>(o.y, 0u, clip_hi2);
-              o.z = clip2<BF16>(o.z, 0u, clip_hi2);
-              o.w = clip2<BF16>(o.w, 0u, clip_hi2);
-            }
-            if (junk) o = make_uint4(0u, 0u, 0u, 0u);  // pad positions stay zero
-            const int chunk16 = ((half * 4 + qq) ^ (row & 7)) << 4;  // 16-byte slot inside the swizzled 128-byte row
-            sts128(my_row + chunk16, o);
-          }
-        }
-        if (etid == 0 && j == 0) DSK_TRACE(2, ecount * 8 + 5);
-        fence_proxy_async_smem();
-        named_bar_sync(bar_id, 128);
-        if (!p.out_planar) {
-          if (gtid == 0) {
-            tma_store_2d(&tmOut, stg, c0 + j * 64, q0);
-            tma_store_commit();
-          }
-        } else {
-          // parity-planar destination: rows scatter over four planes, so no TMA box; 8 lanes copy one 128-byte row
-          // (full lines per warp store), 8 rows per thread
-          const int chunk = gtid & 7;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = i * 16 + (gtid >> 3);
-            uint16_t* d = my_row_dst[(ecount & 1) * 128 + rr];
-            if (d != nullptr)
-              *reinterpret_cast<uint4*>(d + j * 64 + chunk * 8) = lds128(smem_u32(stg) + rr * 128 + ((chunk ^ (rr & 7)) << 4));
-          }
-        }
-        if (etid == 0 && j == 0) DSK_TRACE(2, ecount * 8 + 6);
-      }
-      if (SK && n_parts > 0) {  // both groups have read the partials: the flags can go back to zero
-        named_bar_sync(3, kEpiThreads);
+            for (int i = 0; i < N_TILE / 2; ++i) acc[m][i] += __ldcg(sk_slot(blockIdx.x + c, m, i));
+        named_bar_sync(3, kEpiThreads);  // every thread has read the partials: the flags can go back to zero
         if (etid == 0)
           for (int c = 1; c <= n_parts; ++c) p.sk_flags[blockIdx.x + c] = 0;
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
+      // ---------------- epilogue ----------------
+      // this thread's rows: slice m, half h -> tile row (cg*kMW + m)*64 + fr + 8h; padded position q0 + row
+      bool junk[kMW][2];
+      uint16_t* planar_row[kMW][2];
+#pragma unroll
+      for (int m = 0; m < kMW; ++m)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = (cg * kMW + m) * 64 + fr + 8 * h;
+          const int q = q0 + row;
+          const int R = static_cast<int>(__umulhi(static_cast<unsigned>(q), p.pitch_magic));
+          const int cc = q - R * pitch;
+          const int img = static_cast<int>(__umulhi(static_cast<unsigned>(R), p.img_magic));
+          junk[m][h] = (cc == 0) || (R - img * (p.H + 1) == 0) || (R >= rows_real_end);
+          planar_row[m][h] = nullptr;
+          // parity-planar destination of this position (only when the consumer is a stride-2 conv): pixel (n, h, w) ->
+          // plane (h&1, w&1), padded position of (n, h>>1, w>>1) on the half-resolution grid
+          if (p.out_planar && !junk[m][h]) {
+            const int n = img;  // R = n*(H+1) + h + 1 with h < H  =>  img == n for real rows
+            const int hh = R - 1 - n * (p.H + 1), ww = cc - 1;
+            const int H2 = p.H >> 1, W2 = p.W >> 1;
+            const long q2 = static_cast<long>(n * (H2 + 1) + (hh >> 1) + 1) * (W2 + 1) + (ww >> 1) + 1;
+            const long plane = (hh & 1) * 2 + (ww & 1);
+            planar_row[m][h] = p.out_ptr + (plane * p.out_plane_positions + q2) * p.out_C + c0;
+          }
+        }
+#pragma unroll
+      for (int j = 0; j < kChunksOut; ++j) {
+        uint8_t* stg = smem_stg + buf * kATileBytes;
+        if (!p.out_planar) {
+          // staging buffer `buf`: its previous TMA store (stg_bufs chunks ago) has finished reading it
+          if (etid == 0) {
+            if (p.stg_bufs == 2) tma_store_wait_read<1>();
+            else tma_store_wait_read<0>();
+          }
+          named_bar_sync(1, kEpiThreads);
+        }
+#pragma unroll
+        for (int m = 0; m < kMW; ++m)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = (cg * kMW + m) * 64 + fr + 8 * h;
+            const uint32_t* res = has_res ? reinterpret_cast<const uint32_t*>(p.res_ptr + static_cast<size_t>(q0 + row) * p.cout + c0 + j * 64) : nullptr;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const int col = 8 * i + fc;  // within the 64-channel chunk
+              const int cabs = c0 + j * 64 + col;
+              float f0 = fmaf(acc[m][(8 * j + i) * 4 + 2 * h], p.scale_c[cabs], p.bias_c[cabs]);
+              float f1 = fmaf(acc[m][(8 * j + i) * 4 + 2 * h + 1], p.scale_c[cabs + 1], p.bias_c[cabs + 1]);
+              if (has_res) {
+                const float2 t = unpack2<BF16>(__ldg(res + (col >> 1)));
+                f0 += t.x;
+                f1 += t.y;
+              }
+              uint32_t o = pack2<BF16>(f0, f1);
+              if (do_clip) o = clip2<BF16>(o, 0u, clip_hi2);  // on the packed pair: same result as an fp32 clamp (0 and 20 are exact)
+              if (junk[m][h]) o = 0u;                         // pad positions stay zero
+              if (p.out_planar) {
+                if (planar_row[m][h] != nullptr) *reinterpret_cast<uint32_t*>(planar_row[m][h] + j * 64 + col) = o;
+              } else {
+                *reinterpret_cast<uint32_t*>(stg + sw128_off16(row, col)) = o;
+              }
+            }
+          }
+        if (!p.out_planar) {
+          fence_proxy_async_smem();
+          named_bar_sync(1, kEpiThreads);
+          if (etid == 0) {
+            tma_store_2d(&tmOut, stg, c0 + j * 64, q0);
+            tma_store_commit();
+          }
+          if (p.stg_bufs == 2) buf ^= 1;
+        }
+      }
       if (etid == 0) DSK_TRACE(2, ecount * 8 + 7);
       ++ecount;
     }
-    if (gtid == 0) tma_store_wait_all<0>();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x == 0) DSK_TRACE(0, 483);
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
+    if (etid == 0) tma_store_wait_all<0>();
   }
 }
 

@@ -1,8 +1,8 @@
-// Implicit-GEMM convolution on tcgen05 tensor cores (sm_100a).
+// Implicit-GEMM convolution on the Hopper tensor cores (wgmma, sm_90a).
 //
 // Replaces the cuDNN calls the reference reaches through nn.Conv2d for the 3x3 s1 p1 convs inside
-// BasicBlock (/root/reference/model.py:47-50,58,61 used at :69,73) and the 5x5 s2 p2 stage-entry
-// convs conv2..conv4 (/root/reference/model.py:98,102,106 used at :192,197,202), with the
+// BasicBlock (reference model.py:47-50,58,61 used at :69,73) and the 5x5 s2 p2 stage-entry
+// convs conv2..conv4 (reference model.py:98,102,106 used at :192,197,202), with the
 // BatchNorm affine (:59,62,99,103,107), the residual add (:79) and the clipped ReLU (:36-39)
 // folded into the epilogue.
 //
@@ -11,9 +11,10 @@
 //   A tile  (128 pixels x 64 ch)   one TMA box {64, wt, 1, hb, nb} of the (tap-shifted) input; zero padding
 //                                  comes from TMA out-of-bounds fill
 //   B tile  (N_TILE cout x 64 ch)  one TMA box of the [tap][cout][cin] weight tensor
-// both land in 128B-swizzled shared memory and feed tcgen05.mma (M=128, N=N_TILE, K=16) x 4.
-// Accumulators live in TMEM (double-buffered), the epilogue reads them with tcgen05.ld, applies
-// scale/bias (+residual) (+clip), converts to 16 bit and TMA-stores NHWC.
+// both land in 128B-swizzled shared memory and feed wgmma (M=64, N=N_TILE, K=16) x 4 in each of two consumer
+// warpgroups (rows 0-63 and 64-127 of the tile).  The fp32 accumulators stay in the consumers' registers; the same
+// warpgroups then apply scale/bias (+residual) (+clip), convert to 16 bit and TMA-store NHWC through a swizzled
+// staging tile.
 #pragma once
 #include "dsk_ptx.cuh"
 
@@ -50,18 +51,31 @@ struct ConvParams {
   int8_t tap_dh[kMaxTaps];
 };
 
-constexpr int kConvThreads = 384;  // 4 control warps (TMA, MMA, TMEM alloc, residual prefetch) + 8 epilogue warps
+constexpr int kConvThreads = 384;  // warpgroup 0: TMA producer (warp 0) and residual prefetcher (warp 3); 1, 2: consumers
+
+// Position of accumulator element d[4*i + 2*h + e] of a wgmma fragment (dsk_ptx.cuh) inside its warpgroup's 64 x N
+// slice: row frag_row() + 8*h, column 8*i + frag_col() + e.
+__device__ __forceinline__ int frag_row() { return 16 * ((threadIdx.x >> 5) & 3) + ((threadIdx.x & 31) >> 2); }
+__device__ __forceinline__ int frag_col() { return 2 * (threadIdx.x & 3); }
+// byte offset of 16-bit element (row, col) (col < 64) in a 128-row x 128-byte SWIZZLE_128B tile
+__device__ __forceinline__ uint32_t sw128_off16(int row, int col) {
+  return static_cast<uint32_t>(row * 128 + ((((col >> 3) ^ row) & 7) << 4) + (col & 7) * 2);
+}
+// byte offset of fp32 element (row, col) (col < 32) in a 128-row x 128-byte SWIZZLE_128B tile
+__device__ __forceinline__ uint32_t sw128_off32(int row, int col) {
+  return static_cast<uint32_t>(row * 128 + ((((col >> 2) ^ row) & 7) << 4) + (col & 3) * 4);
+}
 
 template <int N_TILE>
 struct ConvSmem {
-  static constexpr int kStages = (N_TILE == 64) ? 6 : (N_TILE == 128 ? 4 : 3);
+  static_assert(N_TILE == 64 || N_TILE == 128, "a consumer thread holds N_TILE / 2 fp32 accumulators");
+  static constexpr int kStages = N_TILE == 64 ? 6 : 4;
   static constexpr int kBTileBytes = N_TILE * 128;
   static constexpr int kStageBytes = kATileBytes + kBTileBytes;
   static constexpr int kStagingBytes = 2 * kATileBytes;  // two 128-row x 128-byte output chunks
   static constexpr int kResBytes = 2 * kATileBytes;      // residual tiles, prefetched by their own warp
   static constexpr int kScaleBiasBytes = 2 * 512 * 4;
   static constexpr int kBarBytes = 256;
-  static constexpr int kAccStages = (N_TILE == 256) ? 2 : 4;  // TMEM accumulators (<= 512 columns)
   static constexpr int kTotal =
       kStages * kStageBytes + kStagingBytes + kResBytes + kScaleBiasBytes + kBarBytes + 1024;
 };
@@ -75,8 +89,6 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                  const ConvParams p) {
   using S = ConvSmem<N_TILE>;
   constexpr int kStages = S::kStages;
-  constexpr int kAcc = S::kAccStages;
-  constexpr int kTmemCols = kAcc * N_TILE;
   constexpr int kChunks = N_TILE / 64;
 
   extern __shared__ uint8_t smem_raw[];
@@ -90,11 +102,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(smem_scale) + S::kScaleBiasBytes);
   uint64_t* full_bar = bars;                  // [kStages]
   uint64_t* empty_bar = bars + kStages;       // [kStages]
-  uint64_t* tmem_full = bars + 2 * kStages;   // [kAcc]
-  uint64_t* tmem_empty = tmem_full + kAcc;    // [kAcc]
-  uint64_t* res_full = tmem_empty + kAcc;     // [2]
+  uint64_t* res_full = empty_bar + kStages;   // [2]
   uint64_t* res_empty = res_full + 2;         // [2]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(res_empty + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -114,30 +123,19 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < kAcc; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 8);  // one arrive per epilogue warp
+      mbar_init(&empty_bar[i], 2);  // one arrive per consumer warpgroup
     }
     for (int i = 0; i < 2; ++i) {
       mbar_init(&res_full[i], 1);
-      mbar_init(&res_empty[i], 8);
+      mbar_init(&res_empty[i], 8);  // one arrive per consumer warp
     }
     fence_barrier_init();
-  }
-  if (warp == 2) {
-    tmem_alloc(tmem_ptr_smem, kTmemCols);
-    tmem_relinquish();
   }
   for (int i = threadIdx.x; i < p.cout && i < 512; i += blockDim.x) {
     smem_scale[i] = p.scale ? p.scale[i] : 1.0f;
     smem_bias[i] = p.bias ? p.bias[i] : 0.0f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_wait();  // everything above touched only parameters; activations of the previous kernel are read/written below
 
   // tile -> coordinates. Tile order: cout tile fastest so CTAs running concurrently share the A tile in L2.
@@ -178,42 +176,6 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (warp-converged loop, one elected lane issues) =====================
-    constexpr uint32_t idesc = umma_idesc_f16(kTileM, N_TILE, BF16);
-    int stage = 0;
-    uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * N_TILE;
-      for (int ks = 0; ks < ksteps; ++ks) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (elect_one_sync()) {
-          const uint64_t da = umma_desc_sw128(smem_u32(smem_a + stage * kATileBytes));
-          const uint64_t db = umma_desc_sw128(smem_u32(smem_b + stage * S::kBTileBytes));
-#pragma unroll
-          for (int k = 0; k < kKStep / 16; ++k) {
-            // advancing 16 elements (32 B) along K inside the swizzle atom = +2 in the (addr>>4) field
-            umma_f16(d_tmem, da + 2 * k, db + 2 * k, idesc, (ks > 0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (ks == ksteps - 1) umma_commit(&tmem_full[acc]);
-        }
-        __syncwarp();
-        if (++stage == kStages) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      if (++acc == kAcc) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
   } else if (warp == 3) {
     // ===================== residual prefetcher: one 128 x 64 tile per output chunk, two buffers =====================
     if (!OUT_F32 && (p.flags & CONV_RESIDUAL)) {
@@ -237,44 +199,67 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
     }
   } else if (warp >= 4) {
-    // ===================== epilogue: 8 warps; thread = one output pixel x 32 of the 64 channels of a chunk =========
-    const int ew = (warp - 4) & 3;          // == warp % 4 -> TMEM lanes [32*ew, 32*ew+32)
-    const int half = (warp - 4) >> 2;       // which 32 accumulator columns of each 64-column group
-    const int row = ew * 32 + lane;         // row of the 128-row tile
+    // ===================== consumers: warpgroup cg = rows [64*cg, 64*cg+64) of every tile: MMA, then epilogue ==========
+    const int cg = (warp >> 2) - 1;
     const int etid = threadIdx.x - 128;
+    const bool wg_leader = (threadIdx.x & 127) == 0;
     const bool has_res = (p.flags & CONV_RESIDUAL) != 0;
     const bool do_clip = (p.flags & CONV_CLIP) != 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    const int fr = 64 * cg + frag_row();
+    const int fc = frag_col();
+    float acc[N_TILE / 2];
+#pragma unroll
+    for (int i = 0; i < N_TILE / 2; ++i) acc[i] = 0.0f;
+    int stage = 0;
+    uint32_t phase = 0;
     int rb = 0;
     uint32_t rph = 0;
     int buf = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int c0, w0, h0, n0;
       decode(tile, c0, w0, h0, n0);
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-#pragma unroll 1
+      int prev = -1;
+      for (int ks = 0; ks < ksteps; ++ks) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint64_t da = gmma_desc_sw128(smem_u32(smem_a + stage * kATileBytes)) + cg * kDescRows64;
+        const uint64_t db = gmma_desc_sw128(smem_u32(smem_b + stage * S::kBTileBytes));
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kKStep / 16; ++k)
+          // advancing 16 elements (32 B) along K inside the swizzle atom = +2 in the (addr>>4) field
+          wgmma_f16<N_TILE, BF16>(acc, da + 2 * k, db + 2 * k, (ks > 0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous K-step's MMAs are done: its stage goes back to the producer
+        if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == kStages) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
+
+      // ---- epilogue: both warpgroups fill one 128-row staging tile per 64-channel chunk, one thread TMA-stores it
+#pragma unroll
       for (int j = 0; j < kChunks; ++j) {
-        uint32_t v[32];
-        const float* sc = smem_scale + c0 + j * 64 + half * 32;
-        const float* bi = smem_bias + c0 + j * 64 + half * 32;
+        const float* sc = smem_scale + c0 + j * 64;
+        const float* bi = smem_bias + c0 + j * 64;
         if constexpr (OUT_F32) {
-          // fp32 output: the two column halves fill one 128-row x 32-float staging buffer each (both buffers per group)
+          // fp32 output: columns 0-31 / 32-63 of the chunk fill one 128-row x 32-float staging buffer each
           if (etid == 0) tma_store_wait_read<0>();
           named_bar_sync(1, 256);
-          tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + acc * N_TILE + j * 64 + half * 32, v);
-          tmem_ld_wait();
-          uint8_t* my_row = smem_stg + half * kATileBytes + row * 128;
 #pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            uint4 o;
-            o.x = __float_as_uint(fmaf(__uint_as_float(v[q * 4 + 0]), sc[q * 4 + 0], bi[q * 4 + 0]));
-            o.y = __float_as_uint(fmaf(__uint_as_float(v[q * 4 + 1]), sc[q * 4 + 1], bi[q * 4 + 1]));
-            o.z = __float_as_uint(fmaf(__uint_as_float(v[q * 4 + 2]), sc[q * 4 + 2], bi[q * 4 + 2]));
-            o.w = __float_as_uint(fmaf(__uint_as_float(v[q * 4 + 3]), sc[q * 4 + 3], bi[q * 4 + 3]));
-            *reinterpret_cast<uint4*>(my_row + ((q ^ (row & 7)) << 4)) = o;
-          }
+          for (int i = 0; i < 8; ++i)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = fr + 8 * h, col = 8 * i + fc;
+              const float v0 = fmaf(acc[(8 * j + i) * 4 + 2 * h], sc[col], bi[col]);
+              const float v1 = fmaf(acc[(8 * j + i) * 4 + 2 * h + 1], sc[col + 1], bi[col + 1]);
+              *reinterpret_cast<float2*>(smem_stg + (col >> 5) * kATileBytes + sw128_off32(row, col & 31)) =
+                  make_float2(v0, v1);
+            }
           fence_proxy_async_smem();
           named_bar_sync(1, 256);
           if (etid == 0) {
@@ -287,42 +272,27 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           // staging buffer `buf` was last used two chunks ago: its TMA store must have finished reading smem
           if (etid == 0) tma_store_wait_read<1>();
           named_bar_sync(1, 256);
-          tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + acc * N_TILE + j * 64 + half * 32, v);
-          tmem_ld_wait();
           if (has_res) mbar_wait(&res_full[rb], rph);
-          const uint8_t* res_row = smem_res + rb * kATileBytes + row * 128;
-          uint8_t* my_row = stg + row * 128;
+          const uint8_t* res = smem_res + rb * kATileBytes;
 #pragma unroll
-          for (int qq = 0; qq < 4; ++qq) {  // 4 x 16-byte chunks = this thread's 32 channels
-            float f[8];
-            const float4 s0 = *reinterpret_cast<const float4*>(sc + qq * 8);
-            const float4 s1 = *reinterpret_cast<const float4*>(sc + qq * 8 + 4);
-            const float4 b0 = *reinterpret_cast<const float4*>(bi + qq * 8);
-            const float4 b1 = *reinterpret_cast<const float4*>(bi + qq * 8 + 4);
-            const float scv[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-            const float biv[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+          for (int i = 0; i < 8; ++i)
 #pragma unroll
-            for (int e = 0; e < 8; ++e) f[e] = fmaf(__uint_as_float(v[qq * 8 + e]), scv[e], biv[e]);
-            const int chunk16 = ((half * 4 + qq) ^ (row & 7)) << 4;
-            if (has_res) {
-              const uint4 r = *reinterpret_cast<const uint4*>(res_row + chunk16);
-              float2 t;
-              t = unpack2<BF16>(r.x); f[0] += t.x; f[1] += t.y;
-              t = unpack2<BF16>(r.y); f[2] += t.x; f[3] += t.y;
-              t = unpack2<BF16>(r.z); f[4] += t.x; f[5] += t.y;
-              t = unpack2<BF16>(r.w); f[6] += t.x; f[7] += t.y;
+            for (int h = 0; h < 2; ++h) {
+              const int row = fr + 8 * h, col = 8 * i + fc;
+              const uint32_t off = sw128_off16(row, col);
+              float f0 = fmaf(acc[(8 * j + i) * 4 + 2 * h], sc[col], bi[col]);
+              float f1 = fmaf(acc[(8 * j + i) * 4 + 2 * h + 1], sc[col + 1], bi[col + 1]);
+              if (has_res) {
+                const float2 t = unpack2<BF16>(*reinterpret_cast<const uint32_t*>(res + off));
+                f0 += t.x;
+                f1 += t.y;
+              }
+              if (do_clip) {
+                f0 = fminf(fmaxf(f0, 0.0f), p.clip_hi);
+                f1 = fminf(fmaxf(f1, 0.0f), p.clip_hi);
+              }
+              *reinterpret_cast<uint32_t*>(stg + off) = pack2<BF16>(f0, f1);
             }
-            if (do_clip) {
-#pragma unroll
-              for (int e = 0; e < 8; ++e) f[e] = fminf(fmaxf(f[e], 0.0f), p.clip_hi);
-            }
-            uint4 o;
-            o.x = pack2<BF16>(f[0], f[1]);
-            o.y = pack2<BF16>(f[2], f[3]);
-            o.z = pack2<BF16>(f[4], f[5]);
-            o.w = pack2<BF16>(f[6], f[7]);
-            *reinterpret_cast<uint4*>(my_row + chunk16) = o;
-          }
           fence_proxy_async_smem();
           if (has_res) {  // residual buffer consumed: hand it back to the prefetcher
             __syncwarp();
@@ -340,24 +310,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           buf ^= 1;
         }
       }
-      // accumulator fully read: hand the TMEM buffer back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (++acc == kAcc) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
     }
     if (etid == 0) tma_store_wait_all<0>();
-  }
-
-  // ---- teardown ---------------------------------------------------------------------------------
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
   }
 }
 

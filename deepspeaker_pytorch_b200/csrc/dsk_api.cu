@@ -155,7 +155,7 @@ struct HaloLaunch {
   CUtensorMap tmIn, tmW, tmOut, tmRes;
   dsk::HaloParams p;
   int n_tile = 0;
-  int ew = 8;   // epilogue warps: 8 = one CTA per SM, 4 = the two-CTAs-per-SM shape (conv3x3_halo.cuh)
+  int ew = 8;   // consumer warps: 8 = one CTA per SM, 4 = the two-CTAs-per-SM shape (conv3x3_halo.cuh)
   int grid = 0;
   int smem = 0;
 };
@@ -177,7 +177,7 @@ LayerCfg layer_cfg(int i) {
 struct dsk_handle_s {
   int device = 0;
   bool bf16 = false;
-  int num_sms = 148;
+  int num_sms = 132;
   bool weights_loaded = false;
   bool eval_packed = false;           // false after dsk_load_weights_train: only the training path's operand images are current
   int emb = 512;
@@ -255,10 +255,10 @@ struct dsk_handle_s {
   bool use_graph = true;       // DSK_GRAPH=0: always launch the forward kernel by kernel
   bool conv1_pdl = true;       // debug knob DSK_CONV1_PDL=0: launch conv1 with plain stream serialisation
   bool late_trigger = false;   // debug knob DSK_LATE_TRIGGER=1: halo kernels release their dependents at the last tile
-  bool stream_k = false;       // DSK_STREAM_K=1: equal K ranges per CTA (conv3x3_halo.cuh); measured 10 % SLOWER than whole tiles (profiles/r02_stream_k.md)
+  bool stream_k = false;       // DSK_STREAM_K=1: equal K ranges per CTA (conv3x3_halo.cuh) instead of whole tiles
   float* sk_partial = nullptr; // stream-K partial accumulators [num_sms][128][256] fp32 and flags, one set per handle
   int* sk_flags = nullptr;
-  bool small_cta = false;      // DSK_SMALL_CTA=1: 128-channel-tile halo convs as two 256-thread CTAs per SM (measured slower: 1-tap weight boxes are TMA-request bound)
+  bool small_cta = false;      // DSK_SMALL_CTA=1: 128-channel-tile halo convs as two 256-thread CTAs per SM (64-position tiles)
   bool planar_s2 = true;       // eval forward: run the 5x5 s2 convs in the halo kernel's parity-planar form (DSK_PLANAR_S2=0: generic kernel)
   long long* trace = nullptr;  // debug: device buffer [3][512] for conv3x3_halo_kernel clock stamps
   // optional per-launch timing (dsk_set_profiling): events recorded around every kernel of a forward
@@ -337,13 +337,11 @@ int launch_conv(const dsk_handle_s* h, const ConvLaunch& L, cudaStream_t s) {
       switch (L.n_tile) {
         case 64: return launch_conv_t<64, true, true>(L, s);
         case 128: return launch_conv_t<128, true, true>(L, s);
-        case 256: return launch_conv_t<256, true, true>(L, s);
       }
     } else {
       switch (L.n_tile) {
         case 64: return launch_conv_t<64, false, true>(L, s);
         case 128: return launch_conv_t<128, false, true>(L, s);
-        case 256: return launch_conv_t<256, false, true>(L, s);
       }
     }
     return fail(DSK_ERR_INVALID, "unsupported N tile %d", L.n_tile);
@@ -352,13 +350,11 @@ int launch_conv(const dsk_handle_s* h, const ConvLaunch& L, cudaStream_t s) {
     switch (L.n_tile) {
       case 64: return launch_conv_t<64, true>(L, s);
       case 128: return launch_conv_t<128, true>(L, s);
-      case 256: return launch_conv_t<256, true>(L, s);
     }
   } else {
     switch (L.n_tile) {
       case 64: return launch_conv_t<64, false>(L, s);
       case 128: return launch_conv_t<128, false>(L, s);
-      case 256: return launch_conv_t<256, false>(L, s);
     }
   }
   return fail(DSK_ERR_INVALID, "unsupported N tile %d", L.n_tile);
@@ -417,11 +413,11 @@ int build_conv_core(const dsk_handle_s* h, ConvLaunch* L, const View5& a, const 
   p.tiles_h = (Hgrid + p.hb - 1) / p.hb;
   p.tiles_n = (B + p.nb - 1) / p.nb;
   const int tiles_m = p.tiles_w * p.tiles_h * p.tiles_n;
-  // N tile: the kernel is bound by TMA request rate (two boxes per K-step whatever N is), so a tile costs the same
-  // for every N: minimise the number of waves over the SMs; ties go to the smaller tile (more SMs busy).
+  // N tile: minimise the number of waves over the SMs; ties go to the smaller tile (more SMs busy).  No 256-channel
+  // tile: its 64 x 256 fp32 accumulator slice per consumer warpgroup does not fit the registers.
   int n_tile = 64;
   long best_waves = -1;
-  for (int cand : {64, 128, 256}) {
+  for (int cand : {64, 128}) {
     if (n_out % cand) continue;
     const long tiles = static_cast<long>(tiles_m) * (n_out / cand);
     const long waves = (tiles + h->num_sms - 1) / h->num_sms;
@@ -578,7 +574,7 @@ template <int N_TILE, bool BF16>
 int launch_wgrad_t(const WgradLaunch& L, cudaStream_t s) {
   auto kern = dsk::wgrad_umma_kernel<N_TILE, BF16>;
   if (int rc = ensure_smem_optin(reinterpret_cast<const void*>(kern), dsk::WgradSmem<N_TILE>::kTotal)) return rc;
-  kern<<<L.grid, 256, dsk::WgradSmem<N_TILE>::kTotal, s>>>(L.tmG, L.tmX, L.p);
+  kern<<<L.grid, dsk::kWgradThreads, dsk::WgradSmem<N_TILE>::kTotal, s>>>(L.tmG, L.tmX, L.p);
   KERNEL_CHECK();
   return DSK_OK;
 }
@@ -671,13 +667,14 @@ int build_halo(const dsk_handle_s* h, HaloLaunch* L, const void* in, const void*
   p.W = W; p.H = H; p.N = N;
   p.q_begin = W + 1;
   const long q_end = static_cast<long>(N) * (H + 1) * (W + 1);   // one past the last real pixel position
-  p.tiles_m = static_cast<int>((q_end - p.q_begin + 127) / 128);
   // 256-channel tiles halve the weight-operand shared-memory traffic per FLOP (the binding resource, DESIGN.md §6)
   // but halve the tile count: used when the layer still has enough tiles to spread over the SMs
   const int tiles_m_ = static_cast<int>((q_end - p.q_begin + 127) / 128);
   const int n_tile = cout == 64 ? 64 : (h->n256 && cout % 256 == 0 && tiles_m_ * (cout / 256) >= h->n256_min_tiles) ? 256 : 128;
-  // 128-channel tiles (stages 2-4: one or two tiles per SM and layer) run as two 256-thread CTAs per SM
+  // 128-channel tiles optionally run as two 256-thread CTAs per SM, each with one consumer warpgroup and 64-position tiles
   const bool small = h->small_cta && n_tile == 128;
+  const int tm = small ? 64 : 128;  // positions per tile (HaloSmem::kTileRows)
+  p.tiles_m = static_cast<int>((q_end - p.q_begin + tm - 1) / tm);
   const int tpb = (n_tile == 256 || small) ? 1 : 3;
   L->n_tile = n_tile;
   L->ew = small ? 4 : 8;
@@ -749,7 +746,7 @@ int build_halo(const dsk_handle_s* h, HaloLaunch* L, const void* in, const void*
   // shared-memory carve: weight boxes are the latency-critical stream (48 KB each at N_TILE = 128), so they get the
   // deepest ring that fits in 227 KB; output staging / residual prefetch shrink to one buffer each when needed
   {
-    const int halo_rows = 128 + 2 * W + 4;
+    const int halo_rows = tm + 2 * W + 4;
     p.a_stage_bytes = (halo_rows * 128 + 1023) / 1024 * 1024;
     const int b_bytes = tpb * n_tile * 128;
     const int fixed = dsk::HaloSmem<128>::kFixedBytes;  // the same for every tile width
@@ -765,9 +762,8 @@ int build_halo(const dsk_handle_s* h, HaloLaunch* L, const void* in, const void*
       p.b_stages = nb;
       L->smem = p.a_stages * p.a_stage_bytes + p.b_stages * b_bytes + p.stg_bufs * 16384 + fixed;
     } else {
-      // one CTA per SM: two epilogue groups with one staging tile each; the residual is read from global memory
-      // (HaloParams::res_ptr), so everything else goes to the operand rings - weight boxes first (48 KB each at
-      // N_TILE = 128: the latency-critical stream)
+      // one CTA per SM: two output staging tiles; the residual is read from global memory (HaloParams::res_ptr), so
+    // everything else goes to the operand rings - weight boxes first (48 KB each at N_TILE = 128)
       const int limit = 227 * 1024;
       p.a_stages = n_tile == 64 ? 3 : 2;
       p.stg_bufs = 2;
@@ -814,7 +810,7 @@ int build_halo(const dsk_handle_s* h, HaloLaunch* L, const void* in, const void*
   const uint64_t in_pos = static_cast<uint64_t>(npos) * (ksize == 5 ? 4 : 1);
   uint64_t idims[2] = {(uint64_t)cin, in_pos};
   uint64_t istr[1] = {2ull * cin};
-  uint32_t box_in[2] = {64, (uint32_t)(128 + 2 * W + 4)};
+  uint32_t box_in[2] = {64, (uint32_t)(tm + 2 * W + 4)};
   int rc = make_tmap(&L->tmIn, bf, in, 2, idims, istr, box_in);
   if (rc) return rc;
   uint64_t wd[3] = {(uint64_t)cin, (uint64_t)cout, (uint64_t)ntaps_total};
@@ -826,7 +822,7 @@ int build_halo(const dsk_handle_s* h, HaloLaunch* L, const void* in, const void*
   // must be valid: point it at the residual or the input)
   uint64_t odims[2] = {(uint64_t)cout, (uint64_t)npos};
   uint64_t ostr[1] = {2ull * cout};
-  uint32_t box_out[2] = {64, 128};
+  uint32_t box_out[2] = {64, (uint32_t)tm};
   const void* res_ptr = (flags & dsk::CONV_RESIDUAL) ? res : (out_planar ? in : out);
   rc = make_tmap(&L->tmRes, bf, res_ptr, 2, odims, ostr, box_out);
   if (rc) return rc;
@@ -993,8 +989,8 @@ int32_t dsk_create(dsk_handle* out, int32_t device, int32_t operand) {
   CUDA_TRY(cudaSetDevice(device));
   cudaDeviceProp prop;
   CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10)
-    return fail(DSK_ERR_ARCH, "dsk_create: device %d is sm_%d%d; this library contains sm_100a code only", device,
+  if (prop.major != 9 || prop.minor != 0)
+    return fail(DSK_ERR_ARCH, "dsk_create: device %d is sm_%d%d; this library contains sm_90a code only", device,
                 prop.major, prop.minor);
   dsk_handle h = new dsk_handle_s();
   h->device = device;
@@ -2247,7 +2243,7 @@ int32_t dsk_adagrad_step(float* param, const float* grad, float* state_sum, int6
   // clr as torch computes it (Python double arithmetic, then one rounding to float at the kernel boundary)
   const double minus_clr = -lr / (1.0 + static_cast<double>(step - 1) * lr_decay);
   const long n4 = n / 4 > 0 ? n / 4 : 1;
-  const int blocks = static_cast<int>((n4 + 255) / 256 < 148 * 16 ? (n4 + 255) / 256 : 148 * 16);
+  const int blocks = static_cast<int>((n4 + 255) / 256 < 132 * 16 ? (n4 + 255) / 256 : 132 * 16);
   dsk::adagrad_flat_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       param, grad, state_sum, n, grad_mult, grad_denom, static_cast<float>(minus_clr), static_cast<float>(eps),
       static_cast<float>(weight_decay));

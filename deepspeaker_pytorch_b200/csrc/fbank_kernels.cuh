@@ -1,4 +1,4 @@
-// Log mel-filterbank front-end of the reference (/root/reference/audio_processing.py:9-36 `mk_MFB`, constants.py:6-16):
+// Log mel-filterbank front-end of the reference (reference audio_processing.py:9-36 `mk_MFB`, constants.py:6-16):
 //   filter_banks, _ = python_speech_features.fbank(audio, samplerate=16000, nfilt=64, winlen=0.025)     (:14)
 //   filter_banks = 20 * log10(max(filter_banks, 1e-5))                                                  (:16-17)
 //   filter_banks = filter_banks - mean(filter_banks, axis=0)          (normalize_frames, Scale=False)   (:29, :88-92)

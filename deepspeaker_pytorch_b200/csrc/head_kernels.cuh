@@ -1,14 +1,14 @@
 // Classifier head + cross-entropy of the reference's hard-triplet branch and the fused optimizer step.
 //
-//   * Linear(512, C) of DeepSpeakerModel.forward_classifier (/root/reference/model.py:167,220-223) and its backward:
+//   * Linear(512, C) of DeepSpeakerModel.forward_classifier (reference model.py:167,220-223) and its backward:
 //     three small fp32 GEMMs (M = 3k selected utterances <= 1536, N = C classes (1211 for VoxCeleb1), K = 512;
 //     0.24 GFLOP each at k = 128).  They are latency-sized and feed a log-softmax whose loss must match the fp32
 //     reference to 1e-3, so they run in fp32 on the CUDA cores (one 64x64 tile per CTA, fixed summation order:
 //     deterministic) instead of rounding embeddings and logit gradients to 16 bit for the tensor cores.
 //   * nn.CrossEntropyLoss()(cat[cls_a, cls_p, cls_n], cat[label_p, label_p, label_n])
-//     (/root/reference/train_triplet.py:281-285): row-wise log-sum-exp + NLL, mean over rows; backward
+//     (reference train_triplet.py:281-285): row-wise log-sum-exp + NLL, mean over rows; backward
 //     (softmax - onehot) * g / M.
-//   * torch.optim.Adagrad(lr, lr_decay, weight_decay) step (/root/reference/train_triplet.py:369-383, called at
+//   * torch.optim.Adagrad(lr, lr_decay, weight_decay) step (reference train_triplet.py:369-383, called at
 //     :224,291) over ONE flat parameter / gradient / state bucket, fused with the post-allreduce scale:
 //       g = grad * mult (/ *denom);  g += wd * p;  G = fma(g, g, G);  p += (g * -clr) / (sqrt(G) + eps)
 //     — the operation order of torch's foreach implementation, so results are bit-identical to torch.optim.Adagrad.

@@ -22,7 +22,7 @@ __device__ __forceinline__ float row_sqdist(const float* __restrict__ a, const f
   return acc;
 }
 
-// PairwiseDistance(2).forward, /root/reference/model.py:13-18.  One warp per row.
+// PairwiseDistance(2).forward, reference model.py:13-18.  One warp per row.
 __global__ void pairwise_distance_kernel(const float* __restrict__ x1, const float* __restrict__ x2, int B, int D,
                                          float eps, float* __restrict__ out) {
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -44,7 +44,7 @@ __global__ void pairwise_distance_bwd_kernel(const float* __restrict__ x1, const
   if (g2) g2[i] = -g;
 }
 
-// TripletMarginLoss.forward, /root/reference/model.py:27-33: d_p, d_n per row (one warp per row).
+// TripletMarginLoss.forward, reference model.py:27-33: d_p, d_n per row (one warp per row).
 __global__ void triplet_dist_kernel(const float* __restrict__ a, const float* __restrict__ p,
                                     const float* __restrict__ n, int B, int D, float eps, float* __restrict__ d_p,
                                     float* __restrict__ d_n) {
@@ -225,7 +225,7 @@ __global__ void topk_rows_kernel(const float* __restrict__ S, const int64_t* __r
 }  // namespace dsk
 
 // =================================================================================================
-// Tensor-core all-pairs path: fp16 Gram on tcgen05 (conv_umma_kernel used as a plain GEMM, fp32 output), candidate
+// Tensor-core all-pairs path: fp16 Gram on wgmma (conv_umma_kernel used as a plain GEMM, fp32 output), candidate
 // selection from the approximate distances, EXACT fp32 refinement of the candidates in the canonical order of
 // allpairs_sqdist_kernel (sequential-in-d fmaf), so the result is bit-identical to the exact path / the oracle.
 // =================================================================================================

@@ -1,5 +1,5 @@
 // Verification-metric counting kernel: the threshold sweeps of the reference's eval_metrics.py
-// (/root/reference/eval_metrics.py:16-37 calculate_roc over arange(0,30,0.01), :53-73 calculate_val over
+// (reference eval_metrics.py:16-37 calculate_roc over arange(0,30,0.01), :53-73 calculate_val over
 // arange(0,30,0.001)) evaluate, for every threshold t, np.less(dist, t) against the same-speaker labels and count.
 // The reference does 3 000 + 30 000 numpy passes over the distance array on the host; here one launch counts, for all
 // thresholds at once, tp(t) = #{same & d < t} and fp(t) = #{different & d < t}; every other quantity of the sweep

@@ -54,7 +54,7 @@ __global__ void pack_conv_weight_dgrad_kernel(const float* __restrict__ w, uint1
   }
 }
 
-// Eval-mode BatchNorm folded to y = x*scale + bias  (/root/reference/model.py:59,62,94,99,103,107;
+// Eval-mode BatchNorm folded to y = x*scale + bias  (reference model.py:59,62,94,99,103,107;
 // torch defaults eps=1e-5).
 __global__ void bn_fold_kernel(const float* __restrict__ gamma, const float* __restrict__ beta,
                                const float* __restrict__ mean, const float* __restrict__ var, float eps,
@@ -68,7 +68,7 @@ __global__ void bn_fold_kernel(const float* __restrict__ gamma, const float* __r
 }
 
 // ---------------------------------------------------------------------------------------------
-// conv1: 5x5 s2 p2, Cin=1 -> 64 (/root/reference/model.py:93, used at :187), + affine (+clip).
+// conv1: 5x5 s2 p2, Cin=1 -> 64 (reference model.py:93, used at :187), + affine (+clip).
 // x fp32 (B, T, 64) [= NCHW with C=1]; out NHWC 16-bit (B, T/2, 32, 64).
 // Block = 4 output rows of one utterance; warp = 16 pixels; lane = 2 output channels, whose
 // 50 filter weights live in registers; the input patch is broadcast from shared memory.
@@ -165,7 +165,7 @@ conv1_kernel(const float* __restrict__ x, const float* __restrict__ w /*[64][25]
 }
 
 // ---------------------------------------------------------------------------------------------
-// Tail: temporal mean (/root/reference/model.py:111,207-208) -> fc (:164,209) -> l2_norm*alpha
+// Tail: temporal mean (reference model.py:111,207-208) -> fc (:164,209) -> l2_norm*alpha
 // (:172-183,210-213).
 // pooled[b][w*C + c] = mean_h act[b][h][w][c]   (act NHWC 16-bit, W=4, C=512)
 // The fc weight is repacked once to the same (w, c) column order: wq[e][w*C + c] = W[e][c*4 + w].
@@ -290,7 +290,7 @@ fc_kernel(const float* __restrict__ pooled, const float* __restrict__ wq, float*
 }
 
 // y[b][:] = bias + sum_z part[z][b][:] (fixed order; written out for the backward pass), then
-// out[b][:] = alpha * y[b][:] / sqrt(sum(y^2) + 1e-10)   (/root/reference/model.py:172-183,210-213)
+// out[b][:] = alpha * y[b][:] / sqrt(sum(y^2) + 1e-10)   (reference model.py:172-183,210-213)
 // also writes inv_norm[b] = 1/sqrt(sum+1e-10) when inv_norm != nullptr (saved for backward).
 __global__ void l2norm_kernel(const float* __restrict__ part, int nsplit, const float* __restrict__ bias,
                               float* __restrict__ y, float* __restrict__ out, float* __restrict__ inv_norm, int B, int E,

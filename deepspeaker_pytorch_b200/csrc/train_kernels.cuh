@@ -47,7 +47,7 @@ __global__ void nhwc_f32_to_nchw_kernel(const float* __restrict__ in, float* __r
 }  // namespace dsk
 
 // =================================================================================================
-// Training mode.  BatchNorm2d with batch statistics (/root/reference/model.py:59,62,94,99,103,107 in
+// Training mode.  BatchNorm2d with batch statistics (reference model.py:59,62,94,99,103,107 in
 // train mode, called once per a/p/n forward: train_triplet.py:215) and the backward of every non-conv op.
 //
 // Elementwise kernels work on tiles of 64 pixels x 64 channels of an NHWC 16-bit tensor viewed as
@@ -572,8 +572,7 @@ __global__ void loss_scale_kernel(const float* __restrict__ g, long n, float fix
 
 // ---- weight repack of a training step: ONE launch for all eleven tensor-core convs -----------------------------------
 // A training step changes every parameter, so the 16-bit operand images are rebuilt once per step, on the caller's
-// stream, before the three forwards fork: 44 small launches with strided 4-byte gathers (0.3 ms of a 6.4 ms step,
-// profiles/r02_train_launches_ncu.md).  Here a block owns a 16 (cout) x 32 (cin) x taps tile of one layer: it reads the
+// stream, before the three forwards fork, in one launch rather than 44 small ones with strided 4-byte gathers.  Here a block owns a 16 (cout) x 32 (cin) x taps tile of one layer: it reads the
 // OIHW fp32 rows contiguously, keeps the rounded 16-bit values in shared memory and writes both images the training path
 // reads - [tap][cout][cin] for the forward / weight-gradient convs and [tap'][cin][cout] (filter turned by 180 degrees
 // for stride 1) for the data gradient - in 64- and 32-byte runs.  The last block copies conv1's 64x25 fp32 filter.

@@ -1,21 +1,22 @@
-// Weight-gradient GEMM on tcgen05 tensor cores (sm_100a).
+// Weight-gradient GEMM on the Hopper tensor cores (wgmma, sm_90a).
 //
 // Replaces cuDNN's convolution-backward-filter reached by autograd for every nn.Conv2d of the
-// ResCNN (/root/reference/model.py:58,61,98,102,106; backward triggered at train_triplet.py:223).
+// ResCNN (reference model.py:58,61,98,102,106; backward triggered at train_triplet.py:223).
 //
 //   dW[tap][co][ci] = sum over pixels  G[pix][co] * X[pix shifted by tap][ci]
 //
 // The reduction index is the pixel, and both tensors are NHWC (channels contiguous), so both operands are
 // "MN-major" for the tensor core: a TMA box of 128 pixels x 64 channels lands in shared memory as 128 rows of
 // 128 bytes (SWIZZLE_128B) and is consumed as one 64-wide operand atom (descriptor: leading byte offset = atom
-// stride, stride byte offset = 1024 B between 8-pixel groups, major bits = MN).  The tap shift and the zero padding
+// stride, stride byte offset = 1024 B between 8-pixel groups; wgmma's transpose flags mark both operands MN-major).
+// Two consumer warpgroups each own one 64-row atom of the 128-row A tile and keep their accumulators in registers.  The tap shift and the zero padding
 // are TMA coordinates on the outer (w, h) dims exactly as in the forward conv, so no transposed copies exist.
 //
 // Work item = (tap, 128 output channels, N_TILE input channels, K split).  Every K split writes its partial tile with
 // plain stores into its OWN slice dw[ks][tap][cout][cin]; unpack_wgrad_kernel then adds the slices in fixed order, so
 // the weight gradient is bit-reproducible from run to run (no atomics, no pre-zeroing).  Layers with 64 output
 // channels use the swapped form (M = two taps x 64 input channels, N = 64 output channels) so that the MMA still
-// has M = 128.
+// has M = 128 (one tap per consumer warpgroup).
 #pragma once
 #include "conv_umma.cuh"
 
@@ -44,35 +45,31 @@ struct WgradSmem {
   static constexpr int kStages = (N_TILE == 64) ? 4 : 3;
   static constexpr int kTotal = kStages * kStageBytes + 256 + 1024;
 };
+constexpr int kWgradThreads = 384;  // warp 0: TMA producer; warpgroups 1, 2: consumers (MMA + epilogue)
 
 // MN-major SWIZZLE_128B operand descriptor (see header comment)
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr) {
+__device__ __forceinline__ uint64_t gmma_desc_mn_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(kAtomBytes >> 4) << 16;  // leading byte offset: next 64-channel atom
   d |= static_cast<uint64_t>(1024 >> 4) << 32;        // stride byte offset: next group of 8 pixel rows
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
 template <int N_TILE, bool BF16>
-__global__ void __launch_bounds__(256, 1)
+__global__ void __launch_bounds__(kWgradThreads, 1)
 wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CUtensorMap tmX,
                   const WgradParams p) {
   using S = WgradSmem<N_TILE>;
   constexpr int kStages = S::kStages;
   constexpr int kBAtoms = S::kBAtoms;
-  constexpr int kTmemCols = 2 * N_TILE;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * S::kStageBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kStages;
-  uint64_t* tmem_full = bars + 2 * kStages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -87,22 +84,11 @@ wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 4);
+      mbar_init(&empty_bar[i], 2);  // one arrive per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_ptr_smem, kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   // item -> (tap unit, co tile, ci tile, K range); K split fastest
   auto decode = [&](int item, int& tu, int& co0, int& ci0, int& k_begin, int& k_end) -> int {
@@ -160,104 +146,71 @@ wgrad_umma_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    // MMA issuer: fp32 accumulate, both operands MN-major (bits 15 and 16)
-    constexpr uint32_t idesc = umma_idesc_f16(kTileM, N_TILE, BF16) | (1u << 15) | (1u << 16);
+  } else if (warp >= 4) {
+    // consumers: warpgroup cg multiplies A atom cg (64 rows of the 128) by the whole B tile, then stores its rows
+    const int cg = (warp >> 2) - 1;
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    const int fr = frag_row();  // row within this warpgroup's 64 (+ 8 for the odd register pairs)
+    const int fc = frag_col();
+    float acc[N_TILE / 2];
+#pragma unroll
+    for (int i = 0; i < N_TILE / 2; ++i) acc[i] = 0.0f;
     int stage = 0;
     uint32_t phase = 0;
-    int acc = 0;
-    uint32_t acc_phase = 0;
     for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
       int tu, co0, ci0, kb, ke;
-      decode(item, tu, co0, ci0, kb, ke);
-      mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * N_TILE;
+      const int ks = decode(item, tu, co0, ci0, kb, ke);
+      int prev = -1;
       for (int k = kb; k < ke; ++k) {
         mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (elect_one_sync()) {
-          const uint64_t da = umma_desc_mn_sw128(smem_u32(smem + stage * S::kStageBytes));
-          const uint64_t db = umma_desc_mn_sw128(smem_u32(smem + stage * S::kStageBytes + 2 * kAtomBytes));
+        const uint64_t da = gmma_desc_mn_sw128(smem_u32(smem + stage * S::kStageBytes + cg * kAtomBytes));
+        const uint64_t db = gmma_desc_mn_sw128(smem_u32(smem + stage * S::kStageBytes + 2 * kAtomBytes));
+        wgmma_fence();
 #pragma unroll
-          for (int kk = 0; kk < 8; ++kk)  // 128 pixels = 8 x K16; one K16 step = 16 rows x 128 B = +128 in the addr field
-            umma_f16(d_tmem, da + 128 * kk, db + 128 * kk, idesc, (k > kb || kk > 0) ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);
-          if (k == ke - 1) umma_commit(&tmem_full[acc]);
-        }
-        __syncwarp();
+        for (int kk = 0; kk < 8; ++kk)  // 128 pixels = 8 x K16; one K16 step = 16 rows x 128 B = +128 in the addr field
+          wgmma_f16<N_TILE, BF16, 1, 1>(acc, da + 128 * kk, db + 128 * kk, (k > kb || kk > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
         if (++stage == kStages) {
           stage = 0;
           phase ^= 1;
         }
       }
-      if (ke <= kb) {  // empty K range (split rounding): still hand an (ignored) accumulator to the epilogue
-        if (elect_one_sync()) umma_commit(&tmem_full[acc]);
-        __syncwarp();
-      }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
-    }
-  } else if (warp >= 4) {
-    const int ew = warp - 4;
-    const int row = ew * 32 + lane;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-      int tu, co0, ci0, kb, ke;
-      const int ks = decode(item, tu, co0, ci0, kb, ke);
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      if (prev >= 0 && wg_leader) mbar_arrive(&empty_bar[prev]);
       // destination of D[row][col] inside this K split's slice; an empty K range (split rounding) stores zeros
       float* dst = p.dw + static_cast<long>(ks) * p.slice_elems;
       const bool empty = ke <= kb;
-      bool live = true;
       if (!p.swapped) {
-        const int co = co0 + row;
-        live = co < p.cout;
-        dst += (static_cast<long>(tu) * p.cout + co) * p.cin + ci0;
-      } else {
-        const int tap = 2 * tu + (row >> 6);
-        live = tap < p.taps;
-        dst += static_cast<long>(tap) * p.cout * p.cin + (row & 63);  // [tap][co = col][ci = row % 64]
-      }
-#pragma unroll 1
-      for (int j = 0; j < N_TILE / 32; ++j) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(ew * 32) << 16) + acc * N_TILE + j * 32, v);
-        tmem_ld_wait();
-        if (empty) {
 #pragma unroll
-          for (int e = 0; e < 32; ++e) v[e] = 0u;
+        for (int h = 0; h < 2; ++h) {
+          const int co = co0 + 64 * cg + fr + 8 * h;
+          if (co < p.cout) {
+            float* drow = dst + (static_cast<long>(tu) * p.cout + co) * p.cin + ci0 + fc;
+#pragma unroll
+            for (int i = 0; i < N_TILE / 8; ++i)
+              *reinterpret_cast<float2*>(drow + 8 * i) =
+                  empty ? make_float2(0.f, 0.f) : make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+          }
         }
-        if (live) {
-          if (!p.swapped) {
+      } else {
+        const int tap = 2 * tu + cg;  // [tap][co = col][ci = row % 64]
+        if (tap < p.taps) {
 #pragma unroll
-            for (int e = 0; e < 8; ++e)
-              *reinterpret_cast<uint4*>(dst + j * 32 + e * 4) = make_uint4(v[e * 4], v[e * 4 + 1], v[e * 4 + 2], v[e * 4 + 3]);
-          } else {
+          for (int h = 0; h < 2; ++h) {
+            float* dcol = dst + static_cast<long>(tap) * p.cout * p.cin + fr + 8 * h;
 #pragma unroll
-            for (int e = 0; e < 32; ++e) dst[static_cast<long>(j * 32 + e) * p.cin] = __uint_as_float(v[e]);
+            for (int i = 0; i < N_TILE / 8; ++i) {
+              dcol[static_cast<long>(8 * i + fc) * p.cin] = empty ? 0.f : acc[4 * i + 2 * h];
+              dcol[static_cast<long>(8 * i + fc + 1) * p.cin] = empty ? 0.f : acc[4 * i + 2 * h + 1];
+            }
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
   }
 }
 

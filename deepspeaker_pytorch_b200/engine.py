@@ -35,7 +35,7 @@ class Engine:
         """``share_from``: another Engine of the same module whose packed weights this one borrows (inference lanes of
         ``EmbeddingPipeline``: one weight image in L2 for all forwards in flight)."""
         if device.type != "cuda":
-            raise RuntimeError("the B200 engine runs on CUDA devices only")
+            raise RuntimeError("the H100 engine runs on CUDA devices only")
         self.lib = L.load()
         self.device = device
         self.index = device.index if device.index is not None else torch.cuda.current_device()
@@ -169,7 +169,7 @@ def _check2d(*ts):
 
 
 class PairwiseDistanceFn(torch.autograd.Function):
-    """PairwiseDistance(2).forward — /root/reference/model.py:13-18."""
+    """PairwiseDistance(2).forward — reference model.py:13-18."""
 
     @staticmethod
     def forward(ctx, x1, x2):
@@ -197,7 +197,7 @@ class PairwiseDistanceFn(torch.autograd.Function):
 
 
 class TripletLossFn(torch.autograd.Function):
-    """TripletMarginLoss(margin).forward — /root/reference/model.py:27-33 (loss is a device scalar)."""
+    """TripletMarginLoss(margin).forward — reference model.py:27-33 (loss is a device scalar)."""
 
     @staticmethod
     def forward(ctx, a, p, n, margin):

@@ -1,4 +1,4 @@
-"""GPU log-fbank front-end: the reference's ``mk_MFB`` (/root/reference/audio_processing.py:9-36 with constants.py) on the
+"""GPU log-fbank front-end: the reference's ``mk_MFB`` (reference audio_processing.py:9-36 with constants.py) on the
 device, written directly in the ``(T, 64)`` layout the network's ``(B, 1, T, 64)`` input is cropped from (SURVEY §8f-4).
 
 The reference computes the features once per wav file on the CPU (python_speech_features + librosa) and stores ``.npy``

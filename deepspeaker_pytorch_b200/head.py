@@ -1,9 +1,9 @@
 """Classifier head and cross-entropy of the reference's hard-triplet branch on repo kernels (no cuBLAS / ATen math).
 
 * ``LinearFn``          — ``model.classifier`` = ``nn.Linear(embedding_size, num_classes)`` applied by
-  ``DeepSpeakerModel.forward_classifier`` (/root/reference/model.py:167,220-223)
+  ``DeepSpeakerModel.forward_classifier`` (reference model.py:167,220-223)
 * ``CrossEntropyLoss``  — ``nn.CrossEntropyLoss()`` as the reference's train loop uses it
-  (/root/reference/train_triplet.py:281-285): mean over rows of ``logsumexp(logits) - logits[label]``
+  (reference train_triplet.py:281-285): mean over rows of ``logsumexp(logits) - logits[label]``
 
 Both are ``torch.autograd.Function``s over the C ABI (``dsk_linear_*``, ``dsk_cross_entropy*``): fp32, fixed
 summation order (deterministic), asynchronous on the current stream, loss returned as a device scalar.

@@ -1,4 +1,4 @@
-"""Drop-in mirror of /root/reference/model.py for the hot path, backed by libdsk.so (sm_100a CUDA).
+"""Drop-in mirror of reference model.py for the hot path, backed by libdsk.so (sm_90a CUDA).
 
 Same names, constructor arguments, submodule tree and ``state_dict`` keys as the reference:
 
@@ -80,7 +80,7 @@ class myResNet(nn.Module):
 
 
 class DeepSpeakerModel(nn.Module):
-    """ResCNN speaker-embedding network — model.py:153-223 — running on the B200 engine.
+    """ResCNN speaker-embedding network — model.py:153-223 — running on the H100 engine.
 
     Extra keyword ``operand_dtype`` ("fp16" default, or "bf16") selects the 16-bit tensor-core operand
     format; accumulation, BatchNorm, pooling, fc and the L2-norm are fp32 either way.
@@ -126,7 +126,7 @@ class DeepSpeakerModel(nn.Module):
     def forward(self, x):
         """model.py:185-218: x (B,1,T,64) float CUDA tensor -> (B, embedding_size), L2 norm 10."""
         if not x.is_cuda:
-            raise RuntimeError("DeepSpeakerModel (B200 engine) needs CUDA tensors; there is no CPU fallback")
+            raise RuntimeError("DeepSpeakerModel (H100 engine) needs CUDA tensors; there is no CPU fallback")
         if x.dim() != 4 or x.size(1) != 1 or x.size(3) != 64:
             raise RuntimeError(f"expected input (B,1,T,64), got {tuple(x.shape)}")
         eng = self._get_engine(x.device)
@@ -135,14 +135,14 @@ class DeepSpeakerModel(nn.Module):
 
     def forward_triplet(self, anchor, positive, negative):
         """The three forwards of a triplet step, ``model(data_a), model(data_p), model(data_n)``
-        (/root/reference/train_triplet.py:215), issued together: same three results (bit-identical embeddings, batch
+        (reference train_triplet.py:215), issued together: same three results (bit-identical embeddings, batch
         statistics per call, running statistics updated in the order a, p, n), but in train mode the calls run on three
         streams and overlap - as do their backwards.  In eval mode it is simply three forwards.  ``self.features`` is
         left at the negative's embeddings, as after the reference's third call."""
         xs = (anchor, positive, negative)
         for x in xs:
             if not x.is_cuda:
-                raise RuntimeError("DeepSpeakerModel (B200 engine) needs CUDA tensors; there is no CPU fallback")
+                raise RuntimeError("DeepSpeakerModel (H100 engine) needs CUDA tensors; there is no CPU fallback")
             if x.dim() != 4 or x.size(1) != 1 or x.size(3) != 64:
                 raise RuntimeError(f"expected input (B,1,T,64), got {tuple(x.shape)}")
         if not self.training:
@@ -200,5 +200,5 @@ def select_hard_triplets(d_p, d_n, margin):
 
 def allpairs_topk(E, labels, k, exact_cuda_cores=False):
     """BASELINE config 4: per-row k nearest different-label embeddings (idx int64 (N,k), dist fp32 (N,k)).
-    Default: tcgen05 Gram GEMM + exact fp32 refinement (bit-identical to the all-fp32 path, `exact_cuda_cores=True`)."""
+    Default: wgmma Gram GEMM + exact fp32 refinement (bit-identical to the all-fp32 path, `exact_cuda_cores=True`)."""
     return _engine.allpairs_topk(E, labels, k, exact_cuda_cores)

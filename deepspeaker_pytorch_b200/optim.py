@@ -1,7 +1,7 @@
 """Fused optimizer step on ONE flat bucket (SURVEY §8f rank 3).
 
 The reference builds ``torch.optim.Adagrad(model.parameters(), lr=0.1, lr_decay=1e-4, weight_decay=0)``
-(/root/reference/train_triplet.py:369-383, defaults :70-77) and calls ``optimizer.step()`` after ``loss.backward()``
+(reference train_triplet.py:369-383, defaults :70-77) and calls ``optimizer.step()`` after ``loss.backward()``
 (:224,291).  ``FusedAdagrad`` keeps that call surface (``zero_grad() / step() / state_dict() / load_state_dict()``,
 ``param_groups``) but lays parameters, gradients and the running sum of squares out as three flat fp32 buffers with the
 same offsets: ``p.data`` and ``p.grad`` of every parameter become views into them, the data-parallel gradient

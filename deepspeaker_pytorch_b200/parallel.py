@@ -1,6 +1,6 @@
 """Utterance-sharded data parallelism: one process per GPU, ONE allreduce per step.
 
-The reference is single-device (/root/reference/train_triplet.py:97); SURVEY §8e adds exactly one
+The reference is single-device (reference train_triplet.py:97); SURVEY §8e adds exactly one
 strategy: every rank runs the triplet step on its own shard of the batch, and the gradients of the 38
 differentiated parameters are averaged with a single ``all_reduce`` over one flat fp32 bucket
 (11 624 128 elements, 46.5 MB).  BatchNorm statistics stay per replica, as in the reference (no SyncBN).

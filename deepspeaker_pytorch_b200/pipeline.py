@@ -1,6 +1,6 @@
 """Host-to-host (or device-to-device) embedding extraction with copy/compute overlap and several forwards in flight.
 
-The reference's ``test()`` loop (/root/reference/train_triplet.py:337-350) moves every batch to the GPU, runs the
+The reference's ``test()`` loop (reference train_triplet.py:337-350) moves every batch to the GPU, runs the
 model and pulls the distances back, all serialised on one stream.  ``EmbeddingPipeline`` keeps the same per-batch
 call but
 

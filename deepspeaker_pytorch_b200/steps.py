@@ -1,4 +1,4 @@
-"""The per-batch body of the reference's ``train()`` loop (/root/reference/train_triplet.py:208-299) on the B200 engine.
+"""The per-batch body of the reference's ``train()`` loop (reference train_triplet.py:208-299) on the H100 engine.
 
 ``train_step`` restates both branches of the loop with the drop-in classes and the repo's kernels:
 

@@ -1,7 +1,7 @@
-"""Train-mode forward/backward of DeepSpeakerModel on the B200 engine.
+"""Train-mode forward/backward of DeepSpeakerModel on the H100 engine.
 
 Mirrors what autograd does for the reference when the module is in train mode
-(/root/reference/train_triplet.py:203,215-224): BatchNorm uses the batch statistics of each call, running
+(reference train_triplet.py:203,215-224): BatchNorm uses the batch statistics of each call, running
 statistics are updated in place, and ``loss.backward()`` produces gradients for the 12 conv weights, the 12
 BatchNorm affine pairs and fc (the classifier is outside this path and gets no gradient, SURVEY §0 fact 5).
 """
@@ -107,7 +107,7 @@ class TripletForwardFn(torch.autograd.Function):
     backward chains on the same K streams, each into its own flat gradient buffer, then ONE ordered sum of the flat
     buffers on the caller's stream.  K separate nodes gave the same numbers, but autograd then summed the three
     gradients of each of the 38 parameters itself: 114 small ``add`` launches at the end of every step, serial, after the
-    last backward kernel (profiles/r02_train_launches_ncu.md).  The sum here runs in the order autograd used (last
+    last backward kernel.  The sum here runs in the order autograd used (last
     call first: (g_n + g_p) + g_a), so the gradients are the same bits as those of K sequential calls."""
 
     @staticmethod

@@ -1,6 +1,6 @@
-"""Verification loop of the reference's ``test()`` (/root/reference/train_triplet.py:330-366) on the B200 engine, plus
+"""Verification loop of the reference's ``test()`` (reference train_triplet.py:330-366) on the H100 engine, plus
 the derived equal error rate (SURVEY §8f rank 1: the reference sweeps thresholds for best accuracy,
-/root/reference/eval_metrics.py:5-50, and has no EER function).
+reference eval_metrics.py:5-50, and has no EER function).
 
 Distances come from the CUDA kernels (eval forward + PairwiseDistance).  ``evaluate`` is the drop-in for
 ``eval_metrics.evaluate`` (called at train_triplet.py:361): its two threshold sweeps (3 000 + 30 000 thresholds, one
@@ -75,7 +75,7 @@ def threshold_counts(distances: torch.Tensor, labels: torch.Tensor, thresholds):
 
 
 def evaluate(distances: torch.Tensor, labels: torch.Tensor, far_target: float = 1e-3):
-    """Drop-in for ``eval_metrics.evaluate(distances, labels)`` (/root/reference/eval_metrics.py:5-13) on CUDA tensors:
+    """Drop-in for ``eval_metrics.evaluate(distances, labels)`` (reference eval_metrics.py:5-13) on CUDA tensors:
     returns (tpr, fpr, accuracy, val, far) — tpr / fpr / accuracy at the best-accuracy threshold of arange(0, 30, 0.01)
     (first argmax, :16-37), and VAL / FAR at the threshold where the FAR curve over arange(0, 30, 0.001) crosses
     ``far_target`` (:53-88).

@@ -1,9 +1,9 @@
 /*
- * dsk.h — C ABI of the B200-native Deep Speaker hot path (libdsk.so).
+ * dsk.h — C ABI of the H100-native Deep Speaker hot path (libdsk.so).
  *
  * The reference (qqueing/DeepSpeaker-pytorch) is 100 % Python and reaches the GPU only through
  * torch.nn library calls; it has no FFI of its own.  Each entry point below therefore cites the
- * reference *Python* call site whose arithmetic it replaces (file:line in /root/reference).
+ * reference *Python* call site whose arithmetic it replaces (file:line in the reference project).
  * A maintainer binds these with ctypes (see INTEGRATION.md); the host-side mirror of the
  * reference's classes lives in deepspeaker_pytorch_b200/model.py.
  *
@@ -30,7 +30,7 @@ typedef enum {
   DSK_ERR_INVALID = -1, /* bad argument / unsupported shape */
   DSK_ERR_CUDA = -2,    /* a CUDA runtime / driver call failed */
   DSK_ERR_STATE = -3,   /* call sequence error (e.g. forward before load_weights) */
-  DSK_ERR_ARCH = -4     /* device is not sm_100 */
+  DSK_ERR_ARCH = -4     /* device is not sm_90 */
 } dsk_status;
 
 /* 16-bit tensor-core operand format (fp32 accumulation either way) */
@@ -41,7 +41,7 @@ typedef enum { DSK_EVAL = 0, DSK_TRAIN = 1 } dsk_mode_t;
 
 #define DSK_NUM_CONV 12 /* conv1, layer1.0.conv1, layer1.0.conv2, conv2, layer2.0.conv1, ... layer4.0.conv2 */
 
-/* Parameters of DeepSpeakerModel.model (fp32, PyTorch layouts), /root/reference/model.py:91-112,162-164.
+/* Parameters of DeepSpeakerModel.model (fp32, PyTorch layouts), reference model.py:91-112,162-164.
  * conv_w[i]: OIHW.  i = 3*stage + {0: convK (5x5 s2), 1: layerK.0.conv1, 2: layerK.0.conv2 (3x3)}.
  * bn_*[i]  : the BatchNorm2d that follows conv i (bnK, layerK.0.bn1, layerK.0.bn2).
  * fc_w     : (embedding_size, 2048) with column index c*4 + w (model.py:164,208-209). */
@@ -92,7 +92,7 @@ int32_t dsk_load_weights_train(dsk_handle h, const dsk_weights* w, void* stream)
  * forward; it is inference-only, must not be given weights of its own, and `src` must outlive it. */
 int32_t dsk_share_weights(dsk_handle h, dsk_handle src);
 
-/* DeepSpeakerModel.forward (/root/reference/model.py:185-218), BN in eval mode
+/* DeepSpeakerModel.forward (reference model.py:185-218), BN in eval mode
  * (train_triplet.py:332,347): x (B,1,T,64) fp32 contiguous -> emb (B,E) fp32 with ||emb||=10.
  * T must be a multiple of 16.
  * Asynchronous on `stream`, with one exception that synchronises the DEVICE: the first forward after
@@ -193,13 +193,13 @@ int32_t dsk_nchw_f32_to_nhwc16(dsk_handle h, const float* in, void* out, int32_t
 int32_t dsk_nhwc16_to_nchw_f32(dsk_handle h, const void* in, float* out, int32_t B, int32_t C, int32_t H, int32_t W,
                                void* stream);
 
-/* PairwiseDistance(p=2).forward (/root/reference/model.py:8-18): out[i] = sqrt(sum_j (x1-x2)^2 + 1e-4/D). */
+/* PairwiseDistance(p=2).forward (reference model.py:8-18): out[i] = sqrt(sum_j (x1-x2)^2 + 1e-4/D). */
 int32_t dsk_pairwise_distance(const float* x1, const float* x2, int32_t B, int32_t D, float* out, void* stream);
 /* d(out)/d(x1) and d(out)/d(x2) given grad_out (B,), dist (B,) from the forward. Either grad pointer may be NULL. */
 int32_t dsk_pairwise_distance_bwd(const float* x1, const float* x2, const float* dist, const float* grad_out,
                                   int32_t B, int32_t D, float* grad_x1, float* grad_x2, void* stream);
 
-/* TripletMarginLoss(margin).forward (/root/reference/model.py:19-33):
+/* TripletMarginLoss(margin).forward (reference model.py:19-33):
  * loss = mean(clamp(margin + d_p - d_n, 0)). Writes loss (1,), d_p (B,), d_n (B,). */
 int32_t dsk_triplet_loss(const float* a, const float* p, const float* n, int32_t B, int32_t D, float margin,
                          float* loss, float* d_p, float* d_n, void* stream);
@@ -208,7 +208,7 @@ int32_t dsk_triplet_loss_bwd(const float* a, const float* p, const float* n, con
                              const float* grad_loss, int32_t B, int32_t D, float margin, float* ga, float* gp,
                              float* gn, void* stream);
 
-/* "Choose the hard negatives" (/root/reference/train_triplet.py:251-262):
+/* "Choose the hard negatives" (reference train_triplet.py:251-262):
  * idx = ascending indices i with d_n[i] - d_p[i] < margin  (== np.where(mask == 1)); count on device. */
 int32_t dsk_margin_select(const float* d_p, const float* d_n, int32_t B, float margin, int64_t* idx,
                           int32_t* count, void* stream);
@@ -220,7 +220,7 @@ int32_t dsk_gather_rows(const float* src, const int64_t* idx, const int32_t* cou
  * implementation exists — defined from PairwiseDistance, model.py:13-18):
  * D[i][j] = sqrt(sum_d (E[i]-E[j])^2 + 1e-4/Dim), candidates j with labels[j] != labels[i];
  * ties broken by lower j. Writes idx (N,k) int64 and val (N,k) fp32, ascending distance. */
-/* Same result (bit-identical indices and values), computed with a tcgen05 fp16 Gram GEMM + candidate selection + exact
+/* Same result (bit-identical indices and values), computed with a wgmma fp16 Gram GEMM + candidate selection + exact
  * fp32 refinement of the k+8 best candidates per row (exact row scan on the device when the safety margin is not met).
  * Falls back to dsk_allpairs_topk when D % 64 != 0 or k > 8. */
 int32_t dsk_allpairs_topk_tc(dsk_handle h, const float* E, const int64_t* labels, int32_t N, int32_t D, int32_t k,
@@ -228,14 +228,14 @@ int32_t dsk_allpairs_topk_tc(dsk_handle h, const float* E, const int64_t* labels
 int32_t dsk_allpairs_topk(const float* E, const int64_t* labels, int32_t N, int32_t D, int32_t k, int64_t* idx,
                           float* val, void* stream);
 
-/* nn.Linear of DeepSpeakerModel.forward_classifier (/root/reference/model.py:167,220-223): y (M,N) = x (M,K) w(N,K)^T + b.
+/* nn.Linear of DeepSpeakerModel.forward_classifier (reference model.py:167,220-223): y (M,N) = x (M,K) w(N,K)^T + b.
  * fp32 on the CUDA cores, fixed summation order (deterministic).  b may be NULL. */
 int32_t dsk_linear_forward(const float* x, const float* w, const float* b, int32_t M, int32_t N, int32_t K, float* y,
                            void* stream);
 /* its backward: gx (M,K) = gy w, gw (N,K) = gy^T x, gb (N) = column sums of gy; any output pointer may be NULL. */
 int32_t dsk_linear_backward(const float* x, const float* w, const float* gy, int32_t M, int32_t N, int32_t K, float* gx,
                             float* gw, float* gb, void* stream);
-/* nn.CrossEntropyLoss() over (M,C) logits and int64 labels (/root/reference/train_triplet.py:281-285):
+/* nn.CrossEntropyLoss() over (M,C) logits and int64 labels (reference train_triplet.py:281-285):
  * loss (1,) = mean_i (logsumexp_j logits[i] - logits[i][label_i]); also writes lse (M,) and row_loss (M,) (workspace
  * the backward reads).  A label outside [0,C) yields NaN. */
 int32_t dsk_cross_entropy(const float* logits, const int64_t* labels, int32_t M, int32_t C, float* loss, float* lse,
@@ -244,7 +244,7 @@ int32_t dsk_cross_entropy(const float* logits, const int64_t* labels, int32_t M,
 int32_t dsk_cross_entropy_bwd(const float* logits, const int64_t* labels, const float* lse, const float* grad_loss,
                               int32_t M, int32_t C, float* dlogits, void* stream);
 
-/* torch.optim.Adagrad step (/root/reference/train_triplet.py:369-383, called at :224,291) on ONE flat bucket of n fp32
+/* torch.optim.Adagrad step (reference train_triplet.py:369-383, called at :224,291) on ONE flat bucket of n fp32
  * elements (parameters, gradients and the running sum of squares laid out identically), fused with the gradient scale
  * that follows the data-parallel allreduce:  g = grad * grad_mult (/ *grad_denom if non-NULL, a device scalar);
  * g += weight_decay * p;  sum = fma(g, g, sum);  p += (g * -clr) / (sqrt(sum) + eps),  clr = lr / (1 + (step-1) lr_decay).
@@ -254,7 +254,7 @@ int32_t dsk_adagrad_step(float* param, const float* grad, float* state_sum, int6
                          double weight_decay, double eps, int64_t step, float grad_mult, const float* grad_denom,
                          void* stream);
 
-/* Serving pipeline for the reference's test() loop (/root/reference/train_triplet.py:337-350: batch to the GPU, model(x),
+/* Serving pipeline for the reference's test() loop (reference train_triplet.py:337-350: batch to the GPU, model(x),
  * result back - serialised on one stream there).  `primary` owns the weights (dsk_load_weights); the pipeline adds
  * `lanes` handles that borrow them (dsk_share_weights; `primary` stays free for its caller), one compute stream per lane and two copy streams, and keeps depth*lanes device
  * slots.  dsk_pipeline_submit queues, without blocking the host: H2D of the PINNED input batch (B,1,T,64) fp32 -> eval forward
@@ -274,7 +274,7 @@ int32_t dsk_pipeline_wait(dsk_pipeline p, int64_t ticket);
 int32_t dsk_pipeline_sync(dsk_pipeline p);
 int32_t dsk_pipeline_lane_stream(dsk_pipeline p, int32_t lane, void** stream_out);
 
-/* Log mel-filterbank front-end of the reference (/root/reference/audio_processing.py:9-36 mk_MFB with constants.py:
+/* Log mel-filterbank front-end of the reference (reference audio_processing.py:9-36 mk_MFB with constants.py:
  * python_speech_features.fbank(audio, samplerate, nfilt=64, winlen=0.025) -> 20*log10(max(., 1e-5)) (log_scale) -> minus the
  * per-bin mean over the utterance (subtract_mean, normalize_frames with Scale=False).  audio: n_samples fp32 mono on the
  * device; feat: (dsk_fbank_num_frames(n_samples, sample_rate), 64) fp32 row-major, the (T, 64) layout the network's input
@@ -285,7 +285,7 @@ int64_t dsk_fbank_num_frames(int64_t n_samples, int32_t sample_rate);
 int32_t dsk_fbank(const float* audio, int64_t n_samples, int32_t sample_rate, int32_t log_scale, int32_t subtract_mean,
                   float* feat, void* stream);
 
-/* Threshold sweep of the verification metric (/root/reference/eval_metrics.py:16-37 calculate_roc, :53-88 calculate_val /
+/* Threshold sweep of the verification metric (reference eval_metrics.py:16-37 calculate_roc, :53-88 calculate_val /
  * calculate_val_far; called from train_triplet.py:361): for every threshold t (double, as numpy's arange yields them)
  * tp[t] = #{i : same[i] && (double)dist[i] < t}, fp[t] = #{i : !same[i] && (double)dist[i] < t} — numpy's
  * np.less(dist, t) with its float32 -> float64 promotion, so the counts are exactly the reference's.  All other sweep

@@ -4,9 +4,9 @@
  * never by the product library.
  *
  * Follows the reference formulas
- *   PairwiseDistance.forward     /root/reference/model.py:13-18   d = sqrt(sum |x1-x2|^2 + 1e-4/D)
- *   TripletMarginLoss.forward    /root/reference/model.py:27-33   mean(clamp(margin + d_p - d_n, 0))
- *   hard-triplet mask            /root/reference/train_triplet.py:251-262   where(d_n - d_p < margin)
+ *   PairwiseDistance.forward     reference model.py:13-18   d = sqrt(sum |x1-x2|^2 + 1e-4/D)
+ *   TripletMarginLoss.forward    reference model.py:27-33   mean(clamp(margin + d_p - d_n, 0))
+ *   hard-triplet mask            reference train_triplet.py:251-262   where(d_n - d_p < margin)
  * and, for the all-pairs top-k of BASELINE config 4 (absent from the reference, parity unpinned),
  * the same PairwiseDistance formula over every pair.
  *

@@ -1,6 +1,6 @@
 """CPU restatement of the reference's log-fbank front-end - TEST INFRASTRUCTURE ONLY.
 
-/root/reference/audio_processing.py:9-36 (`mk_MFB`) calls ``python_speech_features.fbank`` (package not vendored in the
+reference audio_processing.py:9-36 (`mk_MFB`) calls ``python_speech_features.fbank`` (package not vendored in the
 reference, no pinned version, absent from this image: **parity against the package itself is unpinned**).  Its published
 algorithm (python_speech_features 0.6, base.py ``fbank`` / ``get_filterbanks`` and sigproc.py ``preemphasis`` /
 ``framesig`` / ``powspec``) is restated here in numpy with the same operation order and dtypes (float64 from the framing

@@ -9,7 +9,7 @@ arithmetic itself lives in PyTorch (un-vendored third-party dependency of the re
 version; this container has torch 2.11 CPU kernels), exactly as it does for the reference.
 
 Pinning: tests/golden/*.npz hold outputs of the *reference's own* model.py
-(/root/reference/model.py imported unmodified by tools/make_golden.py in the build container);
+(reference model.py imported unmodified by tools/make_golden.py in the build container);
 tests/test_oracle_golden.py checks this restatement against them.
 """
 from __future__ import annotations

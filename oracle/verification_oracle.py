@@ -1,7 +1,7 @@
 """CPU restatement of the reference's verification metric — TEST INFRASTRUCTURE ONLY.
 
-* 8-crop distance averaging of the test loop, /root/reference/train_triplet.py:339-350;
-* best-threshold accuracy sweep, /root/reference/eval_metrics.py:5-50 (thresholds 0..30 step 0.01);
+* 8-crop distance averaging of the test loop, reference train_triplet.py:339-350;
+* best-threshold accuracy sweep, reference eval_metrics.py:5-50 (thresholds 0..30 step 0.01);
 * equal error rate: the reference has NO EER function (SURVEY §2, §8f); it is derived here from the same
   threshold sweep as the point where false-accept rate == false-reject rate (linear interpolation).
 """

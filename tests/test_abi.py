@@ -32,8 +32,8 @@ def test_every_declared_symbol_is_exported_and_bound():
         assert s in syms, f"{s} bound in _lib.py but not declared in include/dsk.h"
 
 
-def test_sass_is_blackwell_native():
-    """UTCHMMA (tcgen05.mma), UTMALDG/UTMASTG (TMA) and LDTM (tcgen05.ld) must be in the shipped SASS."""
+def test_sass_is_hopper_native():
+    """HGMMA (wgmma) and UTMALDG/UTMASTG (TMA) must be in the shipped SASS."""
     import shutil
     import subprocess
 
@@ -41,9 +41,9 @@ def test_sass_is_blackwell_native():
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", L.LIB_PATH], capture_output=True, text=True).stdout
-    for mnem in ("UTCHMMA", "UTMALDG", "UTMASTG", "LDTM"):
+    for mnem in ("HGMMA", "UTMALDG", "UTMASTG"):
         assert mnem in sass, f"{mnem} missing from libdsk.so SASS"
-    assert "sm_100a" in subprocess.run([cuobjdump, "-lelf", L.LIB_PATH], capture_output=True, text=True).stdout
+    assert "sm_90a" in subprocess.run([cuobjdump, "-lelf", L.LIB_PATH], capture_output=True, text=True).stdout
 
 
 def test_error_convention_without_gpu():

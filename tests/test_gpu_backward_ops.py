@@ -1,5 +1,5 @@
 """Backward building blocks through the C ABI vs torch autograd on the same (16-bit rounded) inputs:
-tcgen05 data-gradient convs (3x3 s1, 5x5 s2 in four parity classes), the MN-major weight-gradient GEMM, and the
+wgmma data-gradient convs (3x3 s1, 5x5 s2 in four parity classes), the MN-major weight-gradient GEMM, and the
 batch-statistics BatchNorm(+residual+clip) forward/backward kernels."""
 import ctypes
 

@@ -1,4 +1,4 @@
-"""tcgen05 implicit-GEMM conv (dsk_conv2d_nhwc) vs an fp64 CPU conv of the same 16-bit-rounded operands."""
+"""wgmma implicit-GEMM conv (dsk_conv2d_nhwc) vs an fp64 CPU conv of the same 16-bit-rounded operands."""
 import ctypes
 
 import pytest

@@ -1,4 +1,4 @@
-"""DeepSpeakerModel.forward on the B200 engine vs the oracle and the reference's golden embeddings."""
+"""DeepSpeakerModel.forward on the H100 engine vs the oracle and the reference's golden embeddings."""
 import os
 
 import numpy as np

@@ -1,4 +1,4 @@
-"""conv3x3_halo_kernel (zero-padded NHWC layout, row-shifted UMMA descriptors, resident / 3-tap weight boxes) vs an
+"""conv3x3_halo_kernel (zero-padded NHWC layout, row-shifted wgmma descriptors, resident / 3-tap weight boxes) vs an
 fp64 CPU conv of the same fp16-rounded operands; also checks that every pad position of the output stays zero."""
 import ctypes
 

@@ -85,7 +85,7 @@ def test_allpairs_topk_bit_exact_vs_oracle(cuda_dev, N, k, groups):
     E_ = torch.randn(N, 512, generator=g)
     E_ = 10.0 * E_ / E_.norm(dim=1, keepdim=True)
     labels = (torch.arange(N) % groups).long()
-    idx, val = dsk.allpairs_topk(E_.cuda(), labels.cuda(), k)                             # tcgen05 Gram + exact refinement
+    idx, val = dsk.allpairs_topk(E_.cuda(), labels.cuda(), k)                             # wgmma Gram + exact refinement
     oidx, oval = C.allpairs_topk(E_.numpy(), labels.numpy(), k)
     assert np.array_equal(idx.cpu().numpy(), oidx)
     assert np.array_equal(val.cpu().numpy(), oval)

@@ -1,4 +1,4 @@
-"""Train-mode forward (batch-statistics BN) and backward of the B200 engine vs the oracle and the
+"""Train-mode forward (batch-statistics BN) and backward of the H100 engine vs the oracle and the
 reference's golden branch-A step (train_triplet.py:215-224)."""
 import os
 

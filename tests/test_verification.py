@@ -1,5 +1,5 @@
 """Verification metric: restated sweep vs the reference's own eval_metrics (golden), and held-out EER parity of the
-B200 engine vs the oracle on synthetic speakers (north star: EER within 0.1 % absolute)."""
+H100 engine vs the oracle on synthetic speakers (north star: EER within 0.1 % absolute)."""
 import os
 
 import numpy as np

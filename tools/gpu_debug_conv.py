@@ -1,4 +1,4 @@
-"""GPU bring-up check of the tcgen05 conv kernel through the C ABI against a CPU fp64 conv of the
+"""GPU bring-up check of the wgmma conv kernel through the C ABI against a CPU fp64 conv of the
 same 16-bit-rounded operands.  Usage: python tools/gpu_debug_conv.py <case> [bf16]
 cases: s1..s4 (3x3 convs of stage 1..4), e2..e4 (5x5 s2 entry convs), all."""
 import ctypes

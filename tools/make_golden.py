@@ -1,7 +1,7 @@
-"""Generate tests/golden/*.npz from the REFERENCE ITSELF (/root/reference/model.py, imported unmodified).
+"""Generate tests/golden/*.npz from the REFERENCE ITSELF (qqueing/DeepSpeaker-pytorch's model.py, imported unmodified).
 
-Run in the build container only (the GPU box has no /root/reference):
-    python tools/make_golden.py
+Needs a checkout of the reference project (no GPU):
+    DEEPSPEAKER_REFERENCE=/path/to/DeepSpeaker-pytorch python tools/make_golden.py
 The fixtures pin oracle/rescnn_oracle.py (tests/test_oracle_golden.py) and, through it, the CUDA path.
 Inputs and parameters are regenerated from seeds by oracle.make_state_dict / make_input, so only
 outputs are stored.
@@ -14,7 +14,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ["DEEPSPEAKER_REFERENCE"])
 import model as R  # noqa: E402  (the reference's model.py)
 
 from oracle import rescnn_oracle as O  # noqa: E402
