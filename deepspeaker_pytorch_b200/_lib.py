@@ -126,6 +126,7 @@ SIGNATURES = {
     "dsk_rescnn_forward_train": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, POINTER(c_void_p), c_void_p]),
     "dsk_rescnn_backward": (c_int32, [c_void_p, c_void_p, c_void_p, POINTER(DskGrads), c_void_p]),
     "dsk_train_ctx_read": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p]),
+    "dsk_debug_read_eval_activation": (c_int32, [c_void_p, c_int32, c_void_p, c_int64, POINTER(c_int32), c_void_p]),
     "dsk_train_ctx_release": (c_int32, [c_void_p, c_void_p]),
     "dsk_set_loss_scale": (c_int32, [c_void_p, c_float]),
     "dsk_set_profiling": (c_int32, [c_void_p, c_int32]),

@@ -1497,7 +1497,7 @@ static int ctx_create(dsk_handle h, int cap, int T, cudaStream_t s, dsk_train_ct
   const size_t o_pooled = take(static_cast<size_t>(B) * 2048 * 4), o_fc = take(static_cast<size_t>(B) * h->emb * 4);
   const size_t o_fc_part = take(static_cast<size_t>(dsk::kFcSplit) * B * h->emb * 4);
   const size_t o_inv = take(B * 4), o_sc = take(512 * 4), o_sh = take(512 * 4), o_ls = take(2 * 4);
-  const size_t o_part = take(static_cast<size_t>(kStatBlocksMax) * 2 * 512 * 4), o_coef = take(3 * 512 * 4);
+  const size_t o_part = take(static_cast<size_t>(kStatBlocksMax) * 4 * 512 * 4), o_coef = take(3 * 512 * 4);
   const size_t o_gfc = take(static_cast<size_t>(B) * h->emb * 4), o_dP = take(static_cast<size_t>(B) * 2048 * 4);
   size_t dw_bytes = 0;  // [ksplit][tap][cout][cin] fp32 slices of the largest layer
   for (int i = 1; i < DSK_NUM_CONV; ++i) {
@@ -1642,7 +1642,7 @@ int32_t dsk_rescnn_forward_train(dsk_handle h, const float* x, int32_t B, int32_
     dim3 gs(gx, C / 64);
     dsk::bn_stats_partial_kernel<<<gs, 256, 0, s>>>(c->raw[i], M, C, c->partial);
     KERNEL_CHECK();
-    dsk::bn_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(c->partial, gx, C, M, h->w.bn_gamma[i], h->w.bn_beta[i],
+    dsk::bn_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(c->partial, c->raw[i], gx, C, M, h->w.bn_gamma[i], h->w.bn_beta[i],
                                                            h->w.bn_running_mean[i], h->w.bn_running_var[i], 0.1f, 1e-5f,
                                                            c->mean[i], c->rstd[i], c->scale_t, c->shift_t, c->unb[i],
                                                            h->defer_stats ? 0 : 1);
@@ -1804,6 +1804,28 @@ int32_t dsk_train_ctx_read(dsk_handle h, dsk_train_ctx c, int32_t which, int32_t
   return DSK_OK;
 }
 
+int32_t dsk_debug_read_eval_activation(dsk_handle h, int32_t layer, void* dst, int64_t dst_bytes, int32_t* planar_out,
+                                       void* stream) {
+  int rc = check_handle(h);
+  if (rc) return rc;
+  if (layer < 0 || layer >= DSK_NUM_CONV || !dst || !planar_out)
+    return fail(DSK_ERR_INVALID, "dsk_debug_read_eval_activation: bad arguments");
+  // get_plan keeps at most one shape, and dsk_load_weights drops it
+  if (h->plans.empty()) return fail(DSK_ERR_STATE, "dsk_debug_read_eval_activation: no eval forward plan is cached");
+  const dsk_handle_s::Plan& pl = h->plans.begin()->second;
+  int H, W, C;
+  act_shape(layer, pl.T, H, W, C);
+  // the layout get_plan chose for this buffer
+  const bool planar = h->planar_s2 && (layer % 3 == 2) && layer < DSK_NUM_CONV - 1;
+  const size_t bytes = planar ? 4 * padded_bytes(pl.B, H / 2, W / 2, C) : padded_bytes(pl.B, H, W, C);
+  if (dst_bytes < 0 || static_cast<size_t>(dst_bytes) != bytes)
+    return fail(DSK_ERR_INVALID, "dsk_debug_read_eval_activation: layer %d holds %zu bytes, dst_bytes is %lld", layer, bytes,
+                static_cast<long long>(dst_bytes));
+  CUDA_TRY(cudaMemcpyAsync(dst, pl.act[layer], bytes, cudaMemcpyDefault, static_cast<cudaStream_t>(stream)));
+  *planar_out = planar ? 1 : 0;
+  return DSK_OK;
+}
+
 int32_t dsk_train_ctx_release(dsk_handle h, dsk_train_ctx c) {
   if (!h || !c) return fail(DSK_ERR_INVALID, "dsk_train_ctx_release: null argument");
   c->in_use = false;
@@ -1886,11 +1908,11 @@ int32_t dsk_bn_act_train_forward(dsk_handle h, const float* raw, const float* ga
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   float* tmp = nullptr;
   const int gx = stat_blocks(M, C);
-  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&tmp), (static_cast<size_t>(gx) * 2 * C + 2 * C) * 4, s));
-  float *partial = tmp, *sc = tmp + static_cast<size_t>(gx) * 2 * C, *sh = sc + C;
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&tmp), (static_cast<size_t>(gx) * 4 * C + 2 * C) * 4, s));
+  float *partial = tmp, *sc = tmp + static_cast<size_t>(gx) * 4 * C, *sh = sc + C;
   dsk::bn_stats_partial_kernel<<<dim3(gx, C / 64), 256, 0, s>>>(raw, M, C, partial);
   KERNEL_CHECK();
-  dsk::bn_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(partial, gx, C, M, gamma, beta, running_mean, running_var, 0.1f,
+  dsk::bn_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(partial, raw, gx, C, M, gamma, beta, running_mean, running_var, 0.1f,
                                                          1e-5f, mean, rstd, sc, sh, nullptr, 1);
   KERNEL_CHECK();
   dim3 ga(static_cast<unsigned>((M + 63) / 64), C / 64);

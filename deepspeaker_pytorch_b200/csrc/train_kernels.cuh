@@ -84,15 +84,19 @@ __device__ __forceinline__ void load8f(const float* p, float (&f)[8]) {
 }
 
 // ---- forward: per-channel sum / sum of squares of the raw conv output --------------------------------------
-// grid (gx, C/64); partial[(bx*2 + stat)*C + c]
+// Two pairs of sums per channel: of x itself (stats 0, 1) and of x - k_c around the pivot k_c = the channel's first
+// element, row 0 of raw (stats 2, 3).  E[x^2] - mean^2 from the plain fp32 sums loses (mean/std)^2 ulps of the variance
+// (1e-3 relative at mean/std 300); bn_finalize_kernel takes the shifted sums where that matters.
+// grid (gx, C/64); partial[(bx*4 + stat)*C + c]
 __global__ void __launch_bounds__(256)
 bn_stats_partial_kernel(const float* __restrict__ raw, long M, int C, float* __restrict__ partial) {
-  __shared__ float red[2][32][65];
+  __shared__ float red[4][32][65];
   const int q = threadIdx.x & 7, p = threadIdx.x >> 3;
   const int c0 = blockIdx.y * 64 + q * 8;
-  float s[8], ss[8];
+  float s[8], ss[8], sd[8], ssd[8], k[8];
+  load8f(raw + c0, k);
 #pragma unroll
-  for (int e = 0; e < 8; ++e) s[e] = ss[e] = 0.f;
+  for (int e = 0; e < 8; ++e) s[e] = ss[e] = sd[e] = ssd[e] = 0.f;
   for (long m = blockIdx.x * 32L + p; m < M; m += 32L * gridDim.x) {
     float f[8];
     load8f(raw + m * C + c0, f);
@@ -100,30 +104,37 @@ bn_stats_partial_kernel(const float* __restrict__ raw, long M, int C, float* __r
     for (int e = 0; e < 8; ++e) {
       s[e] += f[e];
       ss[e] = fmaf(f[e], f[e], ss[e]);
+      const float d = f[e] - k[e];
+      sd[e] += d;
+      ssd[e] = fmaf(d, d, ssd[e]);
     }
   }
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
     red[0][p][q * 8 + e] = s[e];
     red[1][p][q * 8 + e] = ss[e];
+    red[2][p][q * 8 + e] = sd[e];
+    red[3][p][q * 8 + e] = ssd[e];
   }
   __syncthreads();
-  if (threadIdx.x < 128) {
+  {
     const int stat = threadIdx.x >> 6, c = threadIdx.x & 63;
     float t = 0.f;
     for (int i = 0; i < 32; ++i) t += red[stat][i][c];
-    partial[(static_cast<long>(blockIdx.x) * 2 + stat) * C + blockIdx.y * 64 + c] = t;
+    partial[(static_cast<long>(blockIdx.x) * 4 + stat) * C + blockIdx.y * 64 + c] = t;
   }
 }
 
 // Sum of the per-block partials of 32 channels by one 1024-thread block: thread (slice, channel) adds every 32nd
 // partial row in double, the slices are combined in fixed order (deterministic).  A single thread per channel walking
 // all ~1000 rows took ~50 us per launch, a quarter of the training step.
+// Rows of block b are b*rows + row0 (s) and b*rows + row0 + 1 (ss).  Every thread of the block must call it.
 // Returns the totals to the threads of slice 0 (threadIdx.x < 32); the others get ok == false.
 __device__ __forceinline__ bool bn_partial_totals(const float* __restrict__ partial, int nblk, int C, int c, double& s,
-                                                  double& ss) {
+                                                  double& ss, int rows = 2, int row0 = 0) {
   __shared__ double red[2][32][33];
   const int lane = threadIdx.x & 31, sl = threadIdx.x >> 5;
+  __syncthreads();  // a previous call's readers are done with red
   double a = 0.0, b2 = 0.0;
   if (c < C) {
     int b = sl;
@@ -131,8 +142,8 @@ __device__ __forceinline__ bool bn_partial_totals(const float* __restrict__ part
       float t0[4], t1[4];
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        t0[j] = partial[(static_cast<long>(b + 32 * j) * 2) * C + c];
-        t1[j] = partial[(static_cast<long>(b + 32 * j) * 2 + 1) * C + c];
+        t0[j] = partial[(static_cast<long>(b + 32 * j) * rows + row0) * C + c];
+        t1[j] = partial[(static_cast<long>(b + 32 * j) * rows + row0 + 1) * C + c];
       }
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
@@ -141,8 +152,8 @@ __device__ __forceinline__ bool bn_partial_totals(const float* __restrict__ part
       }
     }
     for (; b < nblk; b += 32) {
-      a += partial[(static_cast<long>(b) * 2) * C + c];
-      b2 += partial[(static_cast<long>(b) * 2 + 1) * C + c];
+      a += partial[(static_cast<long>(b) * rows + row0) * C + c];
+      b2 += partial[(static_cast<long>(b) * rows + row0 + 1) * C + c];
     }
   }
   red[0][sl][lane] = a;
@@ -164,19 +175,30 @@ __device__ __forceinline__ float bn_momentum_update(float running, float batch, 
   return __fmaf_rn(momentum, batch, __fmul_rn(1.f - momentum, running));
 }
 
-// mean / biased var -> rstd, scale = gamma*rstd, shift = beta - mean*scale; running stats (momentum, unbiased var)
+// mean / biased var -> rstd, scale = gamma*rstd, shift = beta - mean*scale; running stats (momentum, unbiased var).
+// `raw` is the tensor bn_stats_partial_kernel reduced: its row 0 holds the pivots of the shifted sums.  Channels with
+// mean^2 <= 1024 var keep the plain sums: their cancellation costs at most 10 bits (variance error <= 4e-5 relative in an
+// emulation of this summation order), and they reproduce the earlier kernels' bits, which a training run depends on (its
+// last bits compound over the steps).  The others, where E[x^2] - mean^2 would cancel more, use mean = k + sd/M,
+// var = ssd/M - (sd/M)^2.
 // grid ceil(C/32), block 1024
-__global__ void bn_finalize_kernel(const float* __restrict__ partial, int nblk, int C, long M,
+__global__ void bn_finalize_kernel(const float* __restrict__ partial, const float* __restrict__ raw, int nblk, int C, long M,
                                    const float* __restrict__ gamma, const float* __restrict__ beta,
                                    float* __restrict__ running_mean, float* __restrict__ running_var, float momentum,
                                    float eps, float* __restrict__ mean_out, float* __restrict__ rstd_out,
                                    float* __restrict__ scale_out, float* __restrict__ shift_out,
                                    float* __restrict__ unbiased_out, int update_running) {
   const int c = blockIdx.x * 32 + (threadIdx.x & 31);
-  double s, ss;
-  if (!bn_partial_totals(partial, nblk, C, c, s, ss)) return;
-  const double mean = s / static_cast<double>(M);
+  double s, ss, sd, ssd;
+  const bool ok = bn_partial_totals(partial, nblk, C, c, s, ss, 4, 0);
+  if (!bn_partial_totals(partial, nblk, C, c, sd, ssd, 4, 2) || !ok) return;
+  double mean = s / static_cast<double>(M);
   double var = ss / static_cast<double>(M) - mean * mean;
+  if (mean * mean > 1024.0 * var) {
+    const double dmean = sd / static_cast<double>(M);  // mean - k_c
+    mean = static_cast<double>(raw[c]) + dmean;
+    var = ssd / static_cast<double>(M) - dmean * dmean;
+  }
   if (var < 0.0) var = 0.0;
   const float rstd = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
   const float sc = gamma[c] * rstd;

@@ -127,6 +127,12 @@ int32_t dsk_rescnn_backward(dsk_handle h, dsk_train_ctx ctx, const float* grad_e
 /* Debug / test read-back of what a train-mode forward saved: which = 0 the pre-BatchNorm conv output (fp32),
  * 1 the post-activation tensor (16-bit), of conv layer `layer` (0..11), converted to fp32 NCHW. */
 int32_t dsk_train_ctx_read(dsk_handle h, dsk_train_ctx ctx, int32_t which, int32_t layer, float* out_nchw, void* stream);
+/* Debug / test read-back: activation `layer` (0..11: output of conv `layer` after BN, residual and clip) of this handle's
+ * most recent dsk_rescnn_forward, byte for byte as stored: 16-bit zero-padded NHWC (dsk_padded_positions(B,H,W) * C),
+ * or parity-planar (4 planes of dsk_padded_positions(B,H/2,W/2) * C) for the block outputs that feed a stride-2 conv.
+ * *planar_out says which; dst_bytes must equal that size.  Ordered on `stream`.  DSK_ERR_STATE if no plan is cached. */
+int32_t dsk_debug_read_eval_activation(dsk_handle h, int32_t layer, void* dst, int64_t dst_bytes, int32_t* planar_out,
+                                       void* stream);
 /* Return an unused context to the pool (forward without backward, e.g. under no_grad). */
 int32_t dsk_train_ctx_release(dsk_handle h, dsk_train_ctx ctx);
 /* fp16 operands: inside the backward the 16-bit gradient tensors are multiplied by a power of two S and every parameter

@@ -100,12 +100,12 @@ def test_rejects_bad_input(models):
         m(torch.zeros(2, 1, 100, 64, device="cuda"))
 
 
-def _fresh_model(sd, env):
+def _fresh_model(sd, env, dt="fp16"):
     """A model whose engine handle is created under the given environment knobs (read once by dsk_create)."""
     old = {k: os.environ.get(k) for k in env}
     os.environ.update(env)
     try:
-        m = dsk.DeepSpeakerModel(512, 16).cuda().eval()
+        m = dsk.DeepSpeakerModel(512, 16, operand_dtype=dt).cuda().eval()
         m.load_state_dict(sd)
         with torch.no_grad():
             m(O.make_input(1, 16, seed=1, scale=1.0).cuda())   # creates the handle now

@@ -30,15 +30,16 @@ def make_model(sd, dt, dev):
     return m.train()
 
 
-def read_saved_activations(m, emb, T):
-    """Post-activation tensors y[0..11] (fp32 NCHW) a train-mode forward saved, through the C ABI debug read."""
+def read_saved_activations(m, emb, T, which=1):
+    """What a train-mode forward saved, as fp32 NCHW through the C ABI debug read: the post-activation tensors y[0..11]
+    (which=1) or the pre-BatchNorm conv outputs raw[0..11] (which=0)."""
     eng, tctx = m._engine, emb.grad_fn.guard.tctx
     B = emb.shape[0]
     out = {}
     for i in range(12):
         st = i // 3
         t = torch.empty(B, 64 << st, T >> (st + 1), 64 >> (st + 1), device=emb.device, dtype=torch.float32)
-        L.check(eng.lib.dsk_train_ctx_read(eng.handle, tctx, 1, i, t.data_ptr(), L.cur_stream()), "dsk_train_ctx_read")
+        L.check(eng.lib.dsk_train_ctx_read(eng.handle, tctx, which, i, t.data_ptr(), L.cur_stream()), "dsk_train_ctx_read")
         out[i] = t
     return out
 
