@@ -1,12 +1,13 @@
 """H100-native Deep Speaker hot path: drop-in for reference model.py's DeepSpeakerModel,
 TripletMarginLoss and PairwiseDistance, backed by hand-written sm_90a CUDA behind a C ABI
 (include/dsk.h, lib/libdsk.so)."""
-from .model import (DeepSpeakerModel, PairwiseDistance, TripletMarginLoss, allpairs_topk,  # noqa: F401
-                    select_hard_triplets)
+from .model import (BatchHardTripletLoss, DeepSpeakerModel, PairwiseDistance, TripletMarginLoss,  # noqa: F401
+                    allpairs_topk, select_hard_triplets)
 
 from .pipeline import EmbeddingPipeline  # noqa: F401,E402
 from .head import CrossEntropyLoss  # noqa: F401,E402
 from .optim import FusedAdagrad  # noqa: F401,E402
-from .steps import train_step  # noqa: F401,E402
+from .steps import batch_hard_step, train_step  # noqa: F401,E402
 
-__all__ = ["train_step", "CrossEntropyLoss", "FusedAdagrad", "EmbeddingPipeline", "DeepSpeakerModel", "PairwiseDistance", "TripletMarginLoss", "select_hard_triplets", "allpairs_topk"]
+__all__ = ["train_step", "batch_hard_step", "CrossEntropyLoss", "FusedAdagrad", "EmbeddingPipeline", "DeepSpeakerModel",
+           "PairwiseDistance", "TripletMarginLoss", "BatchHardTripletLoss", "select_hard_triplets", "allpairs_topk"]

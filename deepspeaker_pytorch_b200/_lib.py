@@ -157,6 +157,9 @@ SIGNATURES = {
     "dsk_gather_rows": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int64, c_void_p, c_void_p]),
     "dsk_allpairs_topk_tc": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
     "dsk_allpairs_topk": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
+    "dsk_batch_hard_triplet": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float] + [c_void_p] * 7),
+    "dsk_batch_hard_triplet_bwd": (c_int32, [c_void_p] * 5 + [c_int32, c_int32, c_float, c_void_p, c_void_p, c_void_p,
+                                                              c_void_p]),
     "dsk_linear_forward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     "dsk_linear_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p,
                                       c_void_p, c_void_p]),

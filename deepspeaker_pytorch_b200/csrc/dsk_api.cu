@@ -2134,14 +2134,11 @@ int32_t dsk_gather_rows(const float* src, const int64_t* idx, const int32_t* cou
   return DSK_OK;
 }
 
-int32_t dsk_allpairs_topk_tc(dsk_handle h, const float* E, const int64_t* labels, int32_t N, int32_t D, int32_t k,
-                             int64_t* idx, float* val, void* stream) {
-  int rc = check_handle(h);
-  if (rc) return rc;
-  if (!E || !labels || !idx || !val || N <= 0 || D <= 0 || k <= 0 || k > N)
-    return fail(DSK_ERR_INVALID, "dsk_allpairs_topk_tc: bad arguments");
-  if (D % 64 || k > 8) return dsk_allpairs_topk(E, labels, N, D, k, idx, val, stream);  // exact CUDA-core path
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
+// The tensor-core Gram of the all-pairs ops: (re)builds the plan cached in the handle for (N, D) - buffers and the Gram
+// GEMM descriptors - then rounds E to 16 bit, takes the squared norms of the rounded rows and runs G = E16 E16^T on `s`.
+static int allpairs_gram(dsk_handle h, const float* E, int N, int D, cudaStream_t s, const float** G_out,
+                         const float** norms_out, int* Npad_out) {
+  int rc = 0;
   const int Npad = (N + 127) / 128 * 128;
   const size_t e16_bytes = static_cast<size_t>(Npad) * D * 2, g_bytes = static_cast<size_t>(Npad) * Npad * 4;
   if (h->ap_N != N || h->ap_D != D) {
@@ -2176,13 +2173,87 @@ int32_t dsk_allpairs_topk_tc(dsk_handle h, const float* E, const int64_t* labels
   else dsk::allpairs_prep_kernel<false><<<Npad, 128, 0, s>>>(E, N, D, E16, norms);
   KERNEL_CHECK();
   for (size_t i = 0; i < h->ap_gemm.size() && !rc; ++i) rc = launch_conv(h, h->ap_gemm[i], s);
+  *G_out = G;
+  *norms_out = norms;
+  *Npad_out = Npad;
+  return rc;
+}
+
+// unit roundoff of the 16-bit operand format of the Gram
+static inline float allpairs_unit_roundoff(dsk_handle h) { return h->bf16 ? 1.0f / 256.0f : 1.0f / 2048.0f; }
+
+int32_t dsk_allpairs_topk_tc(dsk_handle h, const float* E, const int64_t* labels, int32_t N, int32_t D, int32_t k,
+                             int64_t* idx, float* val, void* stream) {
+  int rc = check_handle(h);
+  if (rc) return rc;
+  if (!E || !labels || !idx || !val || N <= 0 || D <= 0 || k <= 0 || k > N)
+    return fail(DSK_ERR_INVALID, "dsk_allpairs_topk_tc: bad arguments");
+  if (D % 64 || k > 8) return dsk_allpairs_topk(E, labels, N, D, k, idx, val, stream);  // exact CUDA-core path
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const float *G = nullptr, *norms = nullptr;
+  int Npad = 0;
+  rc = allpairs_gram(h, E, N, D, s, &G, &norms, &Npad);
   if (!rc) {
-    const float u = h->bf16 ? 1.0f / 256.0f : 1.0f / 2048.0f;  // unit roundoff of the 16-bit operand format
+    const float u = allpairs_unit_roundoff(h);
     dsk::allpairs_select_refine_kernel<<<(N + 7) / 8, 256, 0, s>>>(E, G, norms, labels, N, Npad, D, pd_eps(D), k, u, idx, val);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) rc = fail(DSK_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
   }
   return rc;
+}
+
+int32_t dsk_batch_hard_triplet(dsk_handle h, const float* E, const int64_t* labels, int32_t N, int32_t D, float margin,
+                               float* loss, int64_t* pos_idx, int64_t* neg_idx, float* d_ap, float* d_an,
+                               uint8_t* valid, void* stream) {
+  if (!E || !labels || !loss || !pos_idx || !neg_idx || !d_ap || !d_an || !valid || D <= 0 || N < 2 ||
+      N > DSK_BATCH_HARD_MAX_N)
+    return fail(DSK_ERR_INVALID, "dsk_batch_hard_triplet: bad arguments (N must be 2..%d, got %d)", DSK_BATCH_HARD_MAX_N, N);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const float eps = pd_eps(D);
+  if (h && D % 64 == 0) {  // tensor-core Gram + exact refinement of the negative
+    int rc = check_handle(h);
+    if (rc) return rc;
+    const float *G = nullptr, *norms = nullptr;
+    int Npad = 0;
+    rc = allpairs_gram(h, E, N, D, s, &G, &norms, &Npad);
+    if (rc) return rc;
+    dsk::allpairs_select_refine_kernel<<<(N + 7) / 8, 256, 0, s>>>(E, G, norms, labels, N, Npad, D, eps, 1,
+                                                                    allpairs_unit_roundoff(h), neg_idx, d_an);
+    KERNEL_CHECK();
+    dsk::batch_hard_positive_kernel<false><<<(N + 7) / 8, 256, 0, s>>>(E, nullptr, labels, N, D, eps, pos_idx, d_ap, valid);
+    KERNEL_CHECK();
+  } else {  // exact CUDA-core all-pairs matrix (the same bits)
+    float* S = nullptr;
+    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&S), static_cast<size_t>(N) * N * sizeof(float), s));
+    dim3 g((N + 63) / 64, (N + 63) / 64);
+    dsk::allpairs_sqdist_kernel<<<g, 256, 0, s>>>(E, N, D, S);
+    KERNEL_CHECK();
+    dsk::topk_rows_kernel<<<(N + 7) / 8, 256, 0, s>>>(S, labels, N, eps, 1, neg_idx, d_an);
+    KERNEL_CHECK();
+    dsk::batch_hard_positive_kernel<true><<<(N + 7) / 8, 256, 0, s>>>(E, S, labels, N, D, eps, pos_idx, d_ap, valid);
+    KERNEL_CHECK();
+    CUDA_TRY(cudaFreeAsync(S, s));
+  }
+  dsk::batch_hard_mean_kernel<<<1, 1024, 0, s>>>(d_ap, d_an, valid, N, margin, loss);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_batch_hard_triplet_bwd(const float* E, const int64_t* pos_idx, const int64_t* neg_idx, const float* d_ap,
+                                   const float* d_an, int32_t N, int32_t D, float margin, const float* grad_loss,
+                                   const uint8_t* valid, float* gE, void* stream) {
+  if (!E || !pos_idx || !neg_idx || !d_ap || !d_an || !grad_loss || !valid || !gE || D <= 0 || N < 2 ||
+      N > DSK_BATCH_HARD_MAX_N)
+    return fail(DSK_ERR_INVALID, "dsk_batch_hard_triplet_bwd: bad arguments (N must be 2..%d, got %d)", DSK_BATCH_HARD_MAX_N, N);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  float* coef = nullptr;
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&coef), sizeof(float), s));
+  dsk::batch_hard_coef_kernel<<<1, 1024, 0, s>>>(valid, N, grad_loss, coef);
+  KERNEL_CHECK();
+  dsk::batch_hard_bwd_kernel<<<N, 128, 0, s>>>(E, pos_idx, neg_idx, d_ap, d_an, valid, N, D, margin, coef, gE);
+  KERNEL_CHECK();
+  CUDA_TRY(cudaFreeAsync(coef, s));
+  return DSK_OK;
 }
 
 int32_t dsk_allpairs_topk(const float* E, const int64_t* labels, int32_t N, int32_t D, int32_t k, int64_t* idx,

@@ -447,4 +447,163 @@ allpairs_select_refine_kernel(const float* __restrict__ E, const float* __restri
   }
 }
 
+// =================================================================================================
+// Batch-hard triplet loss over one batch of N embeddings: every anchor i takes its hardest positive (farthest same-label
+// row) and its hardest negative (nearest different-label row) inside the batch.  Distances are those of the all-pairs
+// ops above, bit for bit.  The negative is the k = 1 result of allpairs_select_refine_kernel / topk_rows_kernel.
+// =================================================================================================
+
+// Hardest positive, one warp per anchor: argmax over j != i with labels[j] == labels[i] of the exact distance, ties ->
+// lower j (FROM_S: sqrt(S[i][j] + eps) from allpairs_sqdist_kernel, else exact_dist_seq; the two are the same bits).
+// pos_idx = -1 and d_ap = 0 when the anchor has no positive.  valid[i] = 1 iff it has a positive and a negative.
+template <bool FROM_S>
+__global__ void __launch_bounds__(256)
+batch_hard_positive_kernel(const float* __restrict__ E, const float* __restrict__ S, const int64_t* __restrict__ labels,
+                           int N, int D, float eps, int64_t* __restrict__ pos_idx, float* __restrict__ d_ap,
+                           uint8_t* __restrict__ valid) {
+  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= N) return;
+  const int lane = threadIdx.x & 31;
+  const int64_t my_label = labels[row];
+  float bv = -1.f;  // below every distance (>= sqrt(eps) > 0)
+  int bj = 0x7fffffff;
+  bool has_neg = false;
+  for (int j = lane; j < N; j += 32) {
+    if (labels[j] != my_label) {
+      has_neg = true;
+      continue;
+    }
+    if (j == row) continue;
+    const float v = FROM_S ? sqrtf(S[static_cast<long>(row) * N + j] + eps)
+                           : exact_dist_seq(E + static_cast<long>(row) * D, E + static_cast<long>(j) * D, D, eps);
+    if (v > bv) {  // each lane scans ascending j: strict > keeps the lower index of a tie
+      bv = v;
+      bj = j;
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+    const int oj = __shfl_xor_sync(0xffffffffu, bj, o);
+    if (ov > bv || (ov == bv && oj < bj)) {
+      bv = ov;
+      bj = oj;
+    }
+  }
+  has_neg = __any_sync(0xffffffffu, has_neg);
+  if (lane == 0) {
+    const bool has_pos = bj != 0x7fffffff;
+    pos_idx[row] = has_pos ? bj : -1;
+    d_ap[row] = has_pos ? bv : 0.f;
+    valid[row] = (has_pos && has_neg) ? 1 : 0;
+  }
+}
+
+// loss = (1/V) sum over valid anchors of clamp(margin + d_ap - d_an, 0), V = number of valid anchors (loss 0 when
+// V = 0).  Single block of 1024 threads, the order of hinge_mean_kernel: strided partial sums, then a halving tree.
+__global__ void __launch_bounds__(1024)
+batch_hard_mean_kernel(const float* __restrict__ d_ap, const float* __restrict__ d_an,
+                       const uint8_t* __restrict__ valid, int N, float margin, float* __restrict__ loss) {
+  __shared__ float red[1024];
+  __shared__ int cnt[1024];
+  float s = 0.f;
+  int c = 0;
+  for (int i = threadIdx.x; i < N; i += blockDim.x)
+    if (valid[i]) {
+      s += fmaxf((margin + d_ap[i]) - d_an[i], 0.f);
+      ++c;
+    }
+  red[threadIdx.x] = s;
+  cnt[threadIdx.x] = c;
+  __syncthreads();
+  for (int o = blockDim.x >> 1; o > 0; o >>= 1) {
+    if (threadIdx.x < o) {
+      red[threadIdx.x] += red[threadIdx.x + o];
+      cnt[threadIdx.x] += cnt[threadIdx.x + o];
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) loss[0] = cnt[0] > 0 ? red[0] / static_cast<float>(cnt[0]) : 0.f;
+}
+
+// coef[0] = grad_loss / V (0 when V = 0): the weight of every anchor whose hinge passes the gradient.  Single block.
+__global__ void __launch_bounds__(1024)
+batch_hard_coef_kernel(const uint8_t* __restrict__ valid, int N, const float* __restrict__ grad_loss,
+                       float* __restrict__ coef) {
+  __shared__ int cnt[1024];
+  int c = 0;
+  for (int i = threadIdx.x; i < N; i += blockDim.x) c += valid[i] ? 1 : 0;
+  cnt[threadIdx.x] = c;
+  __syncthreads();
+  for (int o = blockDim.x >> 1; o > 0; o >>= 1) {
+    if (threadIdx.x < o) cnt[threadIdx.x] += cnt[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) coef[0] = cnt[0] > 0 ? grad_loss[0] / static_cast<float>(cnt[0]) : 0.f;
+}
+
+// The hinge passes the gradient where margin + d_ap - d_an >= 0 (torch.clamp(min=0), as triplet_loss_bwd_kernel).
+__device__ __forceinline__ bool batch_hard_active(const uint8_t* valid, const float* d_ap, const float* d_an, int i,
+                                                  float margin) {
+  return valid[i] && ((margin + d_ap[i]) - d_an[i] >= 0.f);
+}
+
+// gE[j] (written, not accumulated), one block of 128 threads per row j, thread t owning elements t, t+128, ...
+// Fixed order per row, no float atomics: row j's own anchor term first, then the terms of the anchors that chose j as
+// their positive or negative in ascending anchor order.  That inverse list is built on the device chunk by chunk: each
+// chunk of 128 anchors is compacted (warp ballots + a block prefix, stable) into shared memory, then applied.  A row that
+// many anchors chose (a hub) only makes its own block longer.  Terms, with g = coef[0] and one division per term:
+//   anchor a:  (g / d_ap) (a - p) - (g / d_an) (a - n);   its positive p: -(g / d_ap) (a - p);   its negative n: +(g / d_an) (a - n).
+__global__ void __launch_bounds__(128)
+batch_hard_bwd_kernel(const float* __restrict__ E, const int64_t* __restrict__ pos_idx,
+                      const int64_t* __restrict__ neg_idx, const float* __restrict__ d_ap,
+                      const float* __restrict__ d_an, const uint8_t* __restrict__ valid, int N, int D, float margin,
+                      const float* __restrict__ coef, float* __restrict__ gE) {
+  __shared__ int list[128];  // 2 * anchor + (1 if row j is that anchor's negative, 0 if its positive)
+  __shared__ int wcnt[4];
+  const int j = blockIdx.x;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const float g = coef[0];
+  const float* ej = E + static_cast<long>(j) * D;
+  float* gj = gE + static_cast<long>(j) * D;
+  if (batch_hard_active(valid, d_ap, d_an, j, margin)) {
+    const float* ep = E + pos_idx[j] * D;
+    const float* en = E + neg_idx[j] * D;
+    const float sp = g / d_ap[j], sn = g / d_an[j];
+    for (int d = threadIdx.x; d < D; d += 128) gj[d] = sp * (ej[d] - ep[d]) - sn * (ej[d] - en[d]);
+  } else {
+    for (int d = threadIdx.x; d < D; d += 128) gj[d] = 0.f;
+  }
+  for (int base = 0; base < N; base += 128) {
+    const int i = base + threadIdx.x;
+    int code = -1;
+    if (i < N && batch_hard_active(valid, d_ap, d_an, i, margin)) {
+      if (pos_idx[i] == j) code = 2 * i;
+      else if (neg_idx[i] == j) code = 2 * i + 1;
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, code >= 0);
+    if (lane == 0) wcnt[warp] = __popc(m);
+    __syncthreads();
+    int off = 0, total = 0;
+    for (int w = 0; w < 4; ++w) {
+      off += w < warp ? wcnt[w] : 0;
+      total += wcnt[w];
+    }
+    if (code >= 0) list[off + __popc(m & ((1u << lane) - 1u))] = code;
+    __syncthreads();
+    for (int e = 0; e < total; ++e) {
+      const int c = list[e];
+      const int a = c >> 1;
+      const float* ea = E + static_cast<long>(a) * D;
+      if (c & 1) {
+        const float sn = g / d_an[a];
+        for (int d = threadIdx.x; d < D; d += 128) gj[d] += sn * (ea[d] - ej[d]);
+      } else {
+        const float sp = g / d_ap[a];
+        for (int d = threadIdx.x; d < D; d += 128) gj[d] -= sp * (ea[d] - ej[d]);
+      }
+    }
+    __syncthreads();  // list and wcnt are rewritten by the next chunk
+  }
+}
+
 }  // namespace dsk

@@ -281,3 +281,54 @@ def allpairs_topk(E, labels, k, exact_cuda_cores: bool = False):
             L.check(L.load().dsk_allpairs_topk_tc(_allpairs_handle(E.device), E.data_ptr(), labels.data_ptr(), N, D, k,
                                                   idx.data_ptr(), val.data_ptr(), L.cur_stream()), "dsk_allpairs_topk_tc")
     return idx, val
+
+
+def batch_hard_mine(E, labels, margin, exact_cuda_cores: bool = False):
+    """dsk_batch_hard_triplet: (loss (1,), pos_idx, neg_idx, d_ap, d_an, valid (bool)) on E's device.  The default
+    tensor-core Gram path and ``exact_cuda_cores=True`` return the same bits."""
+    _check2d(E)
+    E = E.detach().float().contiguous()
+    labels = labels.to(device=E.device, dtype=torch.int64).contiguous()
+    N, D = E.shape
+    if labels.shape != (N,):
+        raise RuntimeError(f"expected labels of shape ({N},), got {tuple(labels.shape)}")
+    dev = E.device
+    loss = torch.empty(1, device=dev, dtype=torch.float32)
+    pos, neg = (torch.empty(N, device=dev, dtype=torch.int64) for _ in range(2))
+    d_ap, d_an = (torch.empty(N, device=dev, dtype=torch.float32) for _ in range(2))
+    valid = torch.empty(N, device=dev, dtype=torch.bool)
+    with torch.cuda.device(dev):
+        h = None if exact_cuda_cores else _allpairs_handle(dev)
+        L.check(L.load().dsk_batch_hard_triplet(h, E.data_ptr(), labels.data_ptr(), N, D, float(margin), loss.data_ptr(),
+                                                pos.data_ptr(), neg.data_ptr(), d_ap.data_ptr(), d_an.data_ptr(),
+                                                valid.data_ptr(), L.cur_stream()), "dsk_batch_hard_triplet")
+    return E, loss, pos, neg, d_ap, d_an, valid
+
+
+def batch_hard_backward(E, pos, neg, d_ap, d_an, valid, margin, grad_loss):
+    """dsk_batch_hard_triplet_bwd: d loss / d E scaled by the device scalar ``grad_loss``."""
+    N, D = E.shape
+    gl = grad_loss.float().reshape(1).contiguous()
+    gE = torch.empty_like(E)
+    with torch.cuda.device(E.device):
+        L.check(L.load().dsk_batch_hard_triplet_bwd(E.data_ptr(), pos.data_ptr(), neg.data_ptr(), d_ap.data_ptr(),
+                                                    d_an.data_ptr(), N, D, float(margin), gl.data_ptr(), valid.data_ptr(),
+                                                    gE.data_ptr(), L.cur_stream()), "dsk_batch_hard_triplet_bwd")
+    return gE
+
+
+class BatchHardTripletFn(torch.autograd.Function):
+    """Batch-hard triplet loss (in-batch hardest positive and negative per anchor, mean hinge over valid anchors);
+    the loss is a device scalar."""
+
+    @staticmethod
+    def forward(ctx, E, labels, margin, exact_cuda_cores):
+        Ec, loss, pos, neg, d_ap, d_an, valid = batch_hard_mine(E, labels, margin, exact_cuda_cores)
+        ctx.save_for_backward(Ec, pos, neg, d_ap, d_an, valid)
+        ctx.margin = margin
+        return loss.reshape(())
+
+    @staticmethod
+    def backward(ctx, gl):
+        E, pos, neg, d_ap, d_an, valid = ctx.saved_tensors
+        return batch_hard_backward(E, pos, neg, d_ap, d_an, valid, ctx.margin, gl), None, None, None

@@ -192,6 +192,43 @@ class TripletMarginLoss:
     __call__ = forward
 
 
+class BatchHardTripletLoss:
+    """In-batch hard-triplet mining (no reference implementation; built from PairwiseDistance and the hinge of
+    TripletMarginLoss): over a batch of P speakers x K utterances, each anchor takes its farthest same-label embedding
+    and its nearest different-label embedding; ``loss = mean over valid anchors of clamp(margin + d_ap - d_an, 0)``.
+    An anchor is valid when the batch holds another utterance of its speaker and one of another speaker.
+    ``exact_cuda_cores=True`` forces the all-fp32 distance matrix; the default tensor-core path returns the same bits."""
+
+    def __init__(self, margin, exact_cuda_cores=False):
+        self.margin = margin
+        self.exact_cuda_cores = exact_cuda_cores
+
+    def forward(self, embeddings, labels):
+        """embeddings (N, D) CUDA, labels (N,) int -> 0-dim device scalar; back-propagates into every embedding."""
+        return _engine.BatchHardTripletFn.apply(embeddings, labels, float(self.margin), self.exact_cuda_cores)
+
+    __call__ = forward
+
+    @torch.no_grad()
+    def mine(self, embeddings, labels):
+        """(pos_idx int64, neg_idx int64, d_ap fp32, d_an fp32, valid bool), each (N,) on the device.  Anchors without
+        a positive have pos_idx -1, d_ap 0; without a negative, neg_idx -1, d_an +inf."""
+        _, _, pos, neg, d_ap, d_an, valid = _engine.batch_hard_mine(embeddings, labels, float(self.margin),
+                                                                     self.exact_cuda_cores)
+        return pos, neg, d_ap, d_an, valid
+
+
+def batch_hard_valid_count(labels):
+    """V, the number of valid anchors of a batch-hard loss, from the labels alone (host-side: no device sync when the
+    labels are a CPU tensor, as a data loader yields them): anchors whose speaker has >= 2 utterances, provided the
+    batch holds >= 2 speakers."""
+    lab = torch.as_tensor(labels).detach().cpu().reshape(-1)
+    _, counts = torch.unique(lab, return_counts=True)
+    if counts.numel() < 2:
+        return 0
+    return int(counts[counts >= 2].sum())
+
+
 def select_hard_triplets(d_p, d_n, margin):
     """Device-side restatement of train_triplet.py:251-262: returns (idx int64 (B,), count int32 (1,)) on the
     GPU; idx[:count] equals np.where((d_n - d_p < margin) == 1)[0].  No host synchronisation."""

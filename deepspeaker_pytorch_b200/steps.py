@@ -26,7 +26,8 @@ import torch
 
 from . import engine as _engine
 from .head import CrossEntropyLoss
-from .model import PairwiseDistance, TripletMarginLoss, select_hard_triplets
+from .model import (BatchHardTripletLoss, PairwiseDistance, TripletMarginLoss, batch_hard_valid_count,
+                    select_hard_triplets)
 from .optim import FusedAdagrad
 
 _l2 = PairwiseDistance(2)   # train_triplet.py:119
@@ -95,3 +96,28 @@ def train_step(model, optimizer, data_a, data_p, data_n, label_p, label_n, *, ma
     _reduce_and_step(optimizer, bucket, cnt.to(torch.float32).reshape(()))              # :291 (k_r-weighted under DP)
     return {"loss": loss.detach(), "triplet": triplet.detach(), "ce": ce.detach(), "selected": k, "d_p": d_p, "d_n": d_n,
             "hard": hard}
+
+
+def batch_hard_step(model, optimizer, data, labels, *, margin, bucket=None):
+    """One batch-hard training step on a P speakers x K utterances batch: ONE train-mode forward of all N utterances
+    (BatchNorm statistics over the whole batch), ``BatchHardTripletLoss`` (hardest positive and negative of every anchor
+    inside the batch), backward through all N embeddings, optimizer step.  Under data parallelism each rank's gradient
+    is weighted by its number of valid anchors V_r (the mechanism of branch B), so the update is that of the mean over
+    the union of valid anchors.  V comes from the labels on the host: with CPU labels the step reads nothing back from
+    the device.  Returns ``{"loss": device scalar, "valid": V}``; raises ValueError for a batch with V = 0 (no speaker
+    with two utterances, or a single speaker)."""
+    if not model.training:
+        raise RuntimeError("batch_hard_step needs model.train()")
+    V = batch_hard_valid_count(labels)
+    if V == 0:
+        raise ValueError("batch_hard_step: no valid anchor in the batch (it needs >= 2 speakers, one of them with "
+                         ">= 2 utterances)")
+    labels = torch.as_tensor(labels, dtype=torch.int64)
+    if not labels.is_cuda:   # a pageable copy would wait for the stream; a pinned one is queued like a kernel
+        labels = labels.pin_memory().to(data.device, non_blocking=True)
+    emb = model(data)
+    loss = BatchHardTripletLoss(margin).forward(emb, labels)
+    optimizer.zero_grad()
+    loss.backward()
+    _reduce_and_step(optimizer, bucket, torch.tensor(float(V)))
+    return {"loss": loss.detach(), "valid": V}

@@ -234,6 +234,26 @@ int32_t dsk_allpairs_topk_tc(dsk_handle h, const float* E, const int64_t* labels
 int32_t dsk_allpairs_topk(const float* E, const int64_t* labels, int32_t N, int32_t D, int32_t k, int64_t* idx,
                           float* val, void* stream);
 
+/* Batch-hard triplet loss over one batch (P speakers x K utterances; no reference implementation exists - built from
+ * PairwiseDistance, model.py:13-18, and the hinge of TripletMarginLoss, model.py:27-33).  d(i,j) is the value
+ * dsk_allpairs_topk returns.  Per anchor i: pos_idx = argmax d(i,j) over j != i with labels[j] == labels[i], neg_idx =
+ * argmin d(i,j) over labels[j] != labels[i], ties to the lower j; d_ap, d_an those distances (-1 / 0 when there is no
+ * positive, -1 / +inf when there is no negative); valid[i] = 1 iff both exist (depends on the labels only).
+ * loss (1,) = (1/V) sum over valid i of clamp(margin + d_ap - d_an, 0) in a fixed order, V = #valid; 0 when V = 0.
+ * h != NULL and D % 64 == 0: the Gram plan of dsk_allpairs_topk_tc (cached in h, fp16 or bf16 per h) with exact fp32
+ * refinement; otherwise (h may be NULL) the exact CUDA-core all-pairs matrix.  Both give the same bits.
+ * 2 <= N <= DSK_BATCH_HARD_MAX_N (the N x N fp32 distance matrix, 1 GiB at the limit). */
+#define DSK_BATCH_HARD_MAX_N 16384
+int32_t dsk_batch_hard_triplet(dsk_handle h, const float* E, const int64_t* labels, int32_t N, int32_t D, float margin,
+                               float* loss, int64_t* pos_idx, int64_t* neg_idx, float* d_ap, float* d_an,
+                               uint8_t* valid, void* stream);
+/* Its backward: gE (N,D) = d loss / d E scaled by grad_loss (device scalar), WRITTEN not accumulated.  The hinge passes
+ * the gradient where margin + d_ap - d_an >= 0 (torch.clamp); row terms (E_i - E_j) / d(i,j).  Deterministic, no float
+ * atomics: row j adds its own anchor term, then the terms of the anchors that chose j, in ascending anchor order. */
+int32_t dsk_batch_hard_triplet_bwd(const float* E, const int64_t* pos_idx, const int64_t* neg_idx, const float* d_ap,
+                                   const float* d_an, int32_t N, int32_t D, float margin, const float* grad_loss,
+                                   const uint8_t* valid, float* gE, void* stream);
+
 /* nn.Linear of DeepSpeakerModel.forward_classifier (reference model.py:167,220-223): y (M,N) = x (M,K) w(N,K)^T + b.
  * fp32 on the CUDA cores, fixed summation order (deterministic).  b may be NULL. */
 int32_t dsk_linear_forward(const float* x, const float* w, const float* b, int32_t M, int32_t N, int32_t K, float* y,

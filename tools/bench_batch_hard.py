@@ -1,0 +1,94 @@
+"""Batch-hard triplet loss: one JSON line with
+  * microseconds per loss forward + backward at N = 1024, D = 512 (64 speakers x 16 utterances), on the tensor-core Gram
+    path and on the exact CUDA-core path (CUDA events around --iters back-to-back calls);
+  * utterances per second of batch_hard_step at N = 384 (96 x 4), T = 160, with FusedAdagrad (events around --steps
+    steps after --warmup);
+  * the card's name and power limit (read-only nvidia-smi query in the same run).
+Writes nothing but stdout.  Run: python tools/bench_batch_hard.py
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def gpu_info():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
+        name, power, clk = (s.strip() for s in out.split(","))
+        return {"gpu": name, "power_limit": power, "max_sm_clock": clk}
+    except Exception as e:  # the figures are still device timings; say that the card could not be named
+        return {"gpu": None, "gpu_query_error": str(e)}
+
+
+def time_events(fn, iters):
+    import torch
+
+    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    start.record()
+    for _ in range(iters):
+        fn()
+    end.record()
+    end.synchronize()
+    return start.elapsed_time(end) / iters   # ms
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--iters", type=int, default=500)
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=5)
+    args = ap.parse_args()
+    import torch
+
+    import deepspeaker_pytorch_b200 as dsk
+    from deepspeaker_pytorch_b200 import engine as EN
+
+    assert torch.cuda.is_available(), "bench_batch_hard needs a GPU"
+    dev = torch.device("cuda:0")
+    g = torch.Generator(device=dev).manual_seed(0)
+    rec = {"metric": "batch_hard_triplet", **gpu_info()}
+
+    N, D, K = 1024, 512, 16
+    E = torch.randn(N, D, device=dev, generator=g)
+    E = (10.0 * E / E.norm(dim=1, keepdim=True)).requires_grad_(True)
+    labels = (torch.arange(N, device=dev) // K)
+    for key, exact in (("loss_fwd_bwd_us_tensor_core", False), ("loss_fwd_bwd_us_exact", True)):
+        crit = dsk.BatchHardTripletLoss(0.3, exact_cuda_cores=exact)
+
+        def one():
+            E.grad = None
+            crit.forward(E, labels).backward()
+
+        for _ in range(20):
+            one()
+        torch.cuda.synchronize()
+        rec[key] = round(1e3 * time_events(one, args.iters), 2)
+    rec["loss_shape"] = {"N": N, "D": D, "speakers": N // K, "utterances_per_speaker": K}
+
+    from oracle import rescnn_oracle as O  # deterministic parameters only
+
+    P, Ku, T = 96, 4, 160
+    model = dsk.DeepSpeakerModel(512, 16).to(dev).train()
+    model.load_state_dict(O.make_state_dict(0, num_classes=16))
+    opt = dsk.FusedAdagrad(model.parameters(), lr=1e-3, lr_decay=1e-4)
+    x = torch.randn(P * Ku, 1, T, 64, device=dev, generator=g) * 3.0
+    lab = torch.arange(P * Ku) // Ku           # CPU labels, as a data loader yields them
+    step = lambda: dsk.batch_hard_step(model, opt, x, lab, margin=0.5)
+    for _ in range(args.warmup):
+        step()
+    torch.cuda.synchronize()
+    ms = time_events(step, args.steps)
+    rec["step_ms"] = round(ms, 3)
+    rec["step_utt_per_s"] = round(P * Ku / (ms / 1e3), 1)
+    rec["step_shape"] = {"N": P * Ku, "speakers": P, "utterances_per_speaker": Ku, "T": T, "optimizer": "FusedAdagrad"}
+    print(json.dumps(rec), flush=True)
+
+
+if __name__ == "__main__":
+    main()
