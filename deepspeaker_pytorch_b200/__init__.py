@@ -8,6 +8,8 @@ from .pipeline import EmbeddingPipeline  # noqa: F401,E402
 from .head import CrossEntropyLoss  # noqa: F401,E402
 from .optim import FusedAdagrad  # noqa: F401,E402
 from .steps import batch_hard_step, train_step  # noqa: F401,E402
+from .parallel import GlobalBatchHardTripletLoss  # noqa: F401,E402
 
 __all__ = ["train_step", "batch_hard_step", "CrossEntropyLoss", "FusedAdagrad", "EmbeddingPipeline", "DeepSpeakerModel",
-           "PairwiseDistance", "TripletMarginLoss", "BatchHardTripletLoss", "select_hard_triplets", "allpairs_topk"]
+           "PairwiseDistance", "TripletMarginLoss", "BatchHardTripletLoss", "GlobalBatchHardTripletLoss",
+           "select_hard_triplets", "allpairs_topk"]

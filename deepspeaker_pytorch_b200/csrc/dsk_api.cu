@@ -246,8 +246,8 @@ struct dsk_handle_s {
   float loss_scale = 0.f;  // 0 = automatic
   bool defer_stats = false;  // dsk_set_defer_running_stats: train forwards record batch statistics, the caller commits them in order
   std::vector<dsk_train_ctx_s*> ctx_pool;
-  // cached all-pairs plan (buffers + Gram GEMM descriptors) for the last (N, D)
-  int ap_N = 0, ap_D = 0;
+  // cached all-pairs plan (buffers + Gram GEMM descriptors) for the last (N, D) and anchor row range [row0, row0 + rows)
+  int ap_N = 0, ap_D = 0, ap_row0 = 0, ap_rows = 0;
   uint8_t* ap_buf = nullptr;
   std::vector<ConvLaunch> ap_gemm;
   bool n256 = false;           // DSK_N256=1: 256-channel tiles for layers with >= n256_min_tiles such tiles
@@ -2134,22 +2134,26 @@ int32_t dsk_gather_rows(const float* src, const int64_t* idx, const int32_t* cou
   return DSK_OK;
 }
 
-// The tensor-core Gram of the all-pairs ops: (re)builds the plan cached in the handle for (N, D) - buffers and the Gram
-// GEMM descriptors - then rounds E to 16 bit, takes the squared norms of the rounded rows and runs G = E16 E16^T on `s`.
-static int allpairs_gram(dsk_handle h, const float* E, int N, int D, cudaStream_t s, const float** G_out,
-                         const float** norms_out, int* Npad_out) {
+// The tensor-core Gram of the all-pairs ops for the anchor rows [row0, row0 + rows): (re)builds the plan cached in the
+// handle for (N, D, row0, rows) - buffers and the Gram GEMM descriptors - then rounds E to 16 bit, takes the squared
+// norms of the rounded rows and runs G = E16[row0 : row0 + rows_pad] E16^T (rows_pad x Npad) on `s`.  A rebuild
+// synchronises `s`: a caller that alternates row ranges pays it on every change.
+static int allpairs_gram(dsk_handle h, const float* E, int N, int D, int row0, int rows, cudaStream_t s,
+                         const float** G_out, const float** norms_out, int* Npad_out) {
   int rc = 0;
-  const int Npad = (N + 127) / 128 * 128;
-  const size_t e16_bytes = static_cast<size_t>(Npad) * D * 2, g_bytes = static_cast<size_t>(Npad) * Npad * 4;
-  if (h->ap_N != N || h->ap_D != D) {
-    // (re)build the plan: buffers and the Gram GEMM descriptors.  Gram = E16 E16^T on the tensor cores: rows of E16
-    // are the "pixels" (W = 128, H = Npad/128) and also the "output channels" (<= 512 per launch); one tap, K = D
+  const int Npad = (N + 127) / 128 * 128, rows_pad = (rows + 127) / 128 * 128;
+  // E16 rows: the "pixel" view reads rows_pad rows from row0, which may run past Npad; rows >= N are zero
+  const int Epad = row0 + rows_pad > Npad ? row0 + rows_pad : Npad;
+  const size_t e16_bytes = static_cast<size_t>(Epad) * D * 2, g_bytes = static_cast<size_t>(rows_pad) * Npad * 4;
+  if (h->ap_N != N || h->ap_D != D || h->ap_row0 != row0 || h->ap_rows != rows) {
+    // (re)build the plan: buffers and the Gram GEMM descriptors.  Gram on the tensor cores: the anchor rows of E16 are
+    // the "pixels" (W = 128, H = rows_pad/128), all rows of E16 the "output channels" (<= 512 per launch); one tap, K = D
     CUDA_TRY(cudaStreamSynchronize(s));
     if (h->ap_buf) CUDA_TRY(cudaFree(h->ap_buf));
     h->ap_buf = nullptr;
-    h->ap_N = h->ap_D = 0;
+    h->ap_N = h->ap_D = h->ap_row0 = h->ap_rows = 0;
     h->ap_gemm.clear();
-    CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&h->ap_buf), e16_bytes + g_bytes + Npad * 4));
+    CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&h->ap_buf), e16_bytes + g_bytes + static_cast<size_t>(Epad) * 4));
     uint16_t* E16p = reinterpret_cast<uint16_t*>(h->ap_buf);
     float* Gp = reinterpret_cast<float*>(h->ap_buf + e16_bytes);
     TapTable tt;
@@ -2157,20 +2161,22 @@ static int allpairs_gram(dsk_handle h, const float* E, int N, int D, cudaStream_
     for (int c0 = 0; c0 < Npad; c0 += 512) {
       const int n_out = Npad - c0 < 512 ? Npad - c0 : 512;
       ConvLaunch L;
-      rc = build_conv_core(h, &L, nhwc_view(E16p, 1, Npad / 128, 128, D), E16p + static_cast<size_t>(c0) * D, D, n_out, 1,
-                           nhwc_view(Gp, 1, Npad / 128, 128, Npad), nullptr, 1, Npad / 128, 128, tt, 0, 0.f, nullptr, nullptr,
-                           c0, 0, true);
+      rc = build_conv_core(h, &L, nhwc_view(E16p + static_cast<size_t>(row0) * D, 1, rows_pad / 128, 128, D),
+                           E16p + static_cast<size_t>(c0) * D, D, n_out, 1, nhwc_view(Gp, 1, rows_pad / 128, 128, Npad),
+                           nullptr, 1, rows_pad / 128, 128, tt, 0, 0.f, nullptr, nullptr, c0, 0, true);
       if (rc) return rc;
       h->ap_gemm.push_back(L);
     }
     h->ap_N = N;
     h->ap_D = D;
+    h->ap_row0 = row0;
+    h->ap_rows = rows;
   }
   uint16_t* E16 = reinterpret_cast<uint16_t*>(h->ap_buf);
   float* G = reinterpret_cast<float*>(h->ap_buf + e16_bytes);
   float* norms = reinterpret_cast<float*>(h->ap_buf + e16_bytes + g_bytes);
-  if (h->bf16) dsk::allpairs_prep_kernel<true><<<Npad, 128, 0, s>>>(E, N, D, E16, norms);
-  else dsk::allpairs_prep_kernel<false><<<Npad, 128, 0, s>>>(E, N, D, E16, norms);
+  if (h->bf16) dsk::allpairs_prep_kernel<true><<<Epad, 128, 0, s>>>(E, N, D, E16, norms);
+  else dsk::allpairs_prep_kernel<false><<<Epad, 128, 0, s>>>(E, N, D, E16, norms);
   KERNEL_CHECK();
   for (size_t i = 0; i < h->ap_gemm.size() && !rc; ++i) rc = launch_conv(h, h->ap_gemm[i], s);
   *G_out = G;
@@ -2192,14 +2198,69 @@ int32_t dsk_allpairs_topk_tc(dsk_handle h, const float* E, const int64_t* labels
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const float *G = nullptr, *norms = nullptr;
   int Npad = 0;
-  rc = allpairs_gram(h, E, N, D, s, &G, &norms, &Npad);
+  rc = allpairs_gram(h, E, N, D, 0, N, s, &G, &norms, &Npad);
   if (!rc) {
     const float u = allpairs_unit_roundoff(h);
-    dsk::allpairs_select_refine_kernel<<<(N + 7) / 8, 256, 0, s>>>(E, G, norms, labels, N, Npad, D, pd_eps(D), k, u, idx, val);
+    dsk::allpairs_select_refine_kernel<false><<<(N + 7) / 8, 256, 0, s>>>(E, G, norms, labels, N, Npad, 0, N, D, pd_eps(D),
+                                                                           k, u, idx, val);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) rc = fail(DSK_ERR_CUDA, "kernel launch failed: %s", cudaGetErrorString(e));
   }
   return rc;
+}
+
+static inline bool batch_hard_bad_range(int N, int row0, int rows) {
+  return N < 2 || N > DSK_BATCH_HARD_MAX_N || row0 < 0 || rows < 1 || row0 > N - rows;
+}
+
+int32_t dsk_batch_hard_select_rows(dsk_handle h, const float* E, const int64_t* labels, int32_t N, int32_t D,
+                                   int32_t row0, int32_t rows, int64_t* pos_idx, int64_t* neg_idx, float* d_ap,
+                                   float* d_an, uint8_t* valid, void* stream) {
+  if (!E || !labels || !pos_idx || !neg_idx || !d_ap || !d_an || !valid || D <= 0 || batch_hard_bad_range(N, row0, rows))
+    return fail(DSK_ERR_INVALID, "dsk_batch_hard_select_rows: bad arguments (N must be 2..%d, 0 <= row0, 1 <= rows, "
+                "row0 + rows <= N; got N %d, row0 %d, rows %d)", DSK_BATCH_HARD_MAX_N, N, row0, rows);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const float eps = pd_eps(D);
+  const int blocks = (rows + 7) / 8;
+  if (h && D % 64 == 0) {  // tensor-core Gram + exact refinement of the negative
+    int rc = check_handle(h);
+    if (rc) return rc;
+    const float *G = nullptr, *norms = nullptr;
+    int Npad = 0;
+    rc = allpairs_gram(h, E, N, D, row0, rows, s, &G, &norms, &Npad);
+    if (rc) return rc;
+    if (row0 == 0 && rows == N)
+      dsk::allpairs_select_refine_kernel<false><<<blocks, 256, 0, s>>>(E, G, norms, labels, N, Npad, 0, N, D, eps, 1,
+                                                                        allpairs_unit_roundoff(h), neg_idx, d_an);
+    else
+      dsk::allpairs_select_refine_kernel<true><<<blocks, 256, 0, s>>>(E, G, norms, labels, N, Npad, row0, rows, D, eps, 1,
+                                                                       allpairs_unit_roundoff(h), neg_idx, d_an);
+    KERNEL_CHECK();
+    dsk::batch_hard_positive_kernel<false><<<blocks, 256, 0, s>>>(E, nullptr, labels, N, row0, rows, D, eps, pos_idx,
+                                                                   d_ap, valid);
+    KERNEL_CHECK();
+  } else {  // exact CUDA-core rows x N distance matrix (the same bits)
+    float* S = nullptr;
+    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&S), static_cast<size_t>(rows) * N * sizeof(float), s));
+    dim3 g((N + 63) / 64, (rows + 63) / 64);
+    dsk::allpairs_sqdist_kernel<<<g, 256, 0, s>>>(E, N, D, row0, rows, S);
+    KERNEL_CHECK();
+    dsk::topk_rows_kernel<<<blocks, 256, 0, s>>>(S, labels, N, row0, rows, eps, 1, neg_idx, d_an);
+    KERNEL_CHECK();
+    dsk::batch_hard_positive_kernel<true><<<blocks, 256, 0, s>>>(E, S, labels, N, row0, rows, D, eps, pos_idx, d_ap, valid);
+    KERNEL_CHECK();
+    CUDA_TRY(cudaFreeAsync(S, s));
+  }
+  return DSK_OK;
+}
+
+int32_t dsk_batch_hard_mean(const float* d_ap, const float* d_an, const uint8_t* valid, int32_t N, float margin,
+                            float* loss, void* stream) {
+  if (!d_ap || !d_an || !valid || !loss || N < 2 || N > DSK_BATCH_HARD_MAX_N)
+    return fail(DSK_ERR_INVALID, "dsk_batch_hard_mean: bad arguments (N must be 2..%d, got %d)", DSK_BATCH_HARD_MAX_N, N);
+  dsk::batch_hard_mean_kernel<<<1, 1024, 0, static_cast<cudaStream_t>(stream)>>>(d_ap, d_an, valid, N, margin, loss);
+  KERNEL_CHECK();
+  return DSK_OK;
 }
 
 int32_t dsk_batch_hard_triplet(dsk_handle h, const float* E, const int64_t* labels, int32_t N, int32_t D, float margin,
@@ -2208,34 +2269,27 @@ int32_t dsk_batch_hard_triplet(dsk_handle h, const float* E, const int64_t* labe
   if (!E || !labels || !loss || !pos_idx || !neg_idx || !d_ap || !d_an || !valid || D <= 0 || N < 2 ||
       N > DSK_BATCH_HARD_MAX_N)
     return fail(DSK_ERR_INVALID, "dsk_batch_hard_triplet: bad arguments (N must be 2..%d, got %d)", DSK_BATCH_HARD_MAX_N, N);
+  const int rc = dsk_batch_hard_select_rows(h, E, labels, N, D, 0, N, pos_idx, neg_idx, d_ap, d_an, valid, stream);
+  return rc ? rc : dsk_batch_hard_mean(d_ap, d_an, valid, N, margin, loss, stream);
+}
+
+int32_t dsk_batch_hard_triplet_bwd_rows(const float* E, const int64_t* pos_idx, const int64_t* neg_idx,
+                                        const float* d_ap, const float* d_an, const uint8_t* valid, int32_t N,
+                                        int32_t D, int32_t row0, int32_t rows, float margin, const float* grad_loss,
+                                        float* gE_rows, void* stream) {
+  if (!E || !pos_idx || !neg_idx || !d_ap || !d_an || !grad_loss || !valid || !gE_rows || D <= 0 ||
+      batch_hard_bad_range(N, row0, rows))
+    return fail(DSK_ERR_INVALID, "dsk_batch_hard_triplet_bwd_rows: bad arguments (N must be 2..%d, 0 <= row0, "
+                "1 <= rows, row0 + rows <= N; got N %d, row0 %d, rows %d)", DSK_BATCH_HARD_MAX_N, N, row0, rows);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const float eps = pd_eps(D);
-  if (h && D % 64 == 0) {  // tensor-core Gram + exact refinement of the negative
-    int rc = check_handle(h);
-    if (rc) return rc;
-    const float *G = nullptr, *norms = nullptr;
-    int Npad = 0;
-    rc = allpairs_gram(h, E, N, D, s, &G, &norms, &Npad);
-    if (rc) return rc;
-    dsk::allpairs_select_refine_kernel<<<(N + 7) / 8, 256, 0, s>>>(E, G, norms, labels, N, Npad, D, eps, 1,
-                                                                    allpairs_unit_roundoff(h), neg_idx, d_an);
-    KERNEL_CHECK();
-    dsk::batch_hard_positive_kernel<false><<<(N + 7) / 8, 256, 0, s>>>(E, nullptr, labels, N, D, eps, pos_idx, d_ap, valid);
-    KERNEL_CHECK();
-  } else {  // exact CUDA-core all-pairs matrix (the same bits)
-    float* S = nullptr;
-    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&S), static_cast<size_t>(N) * N * sizeof(float), s));
-    dim3 g((N + 63) / 64, (N + 63) / 64);
-    dsk::allpairs_sqdist_kernel<<<g, 256, 0, s>>>(E, N, D, S);
-    KERNEL_CHECK();
-    dsk::topk_rows_kernel<<<(N + 7) / 8, 256, 0, s>>>(S, labels, N, eps, 1, neg_idx, d_an);
-    KERNEL_CHECK();
-    dsk::batch_hard_positive_kernel<true><<<(N + 7) / 8, 256, 0, s>>>(E, S, labels, N, D, eps, pos_idx, d_ap, valid);
-    KERNEL_CHECK();
-    CUDA_TRY(cudaFreeAsync(S, s));
-  }
-  dsk::batch_hard_mean_kernel<<<1, 1024, 0, s>>>(d_ap, d_an, valid, N, margin, loss);
+  float* coef = nullptr;
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&coef), sizeof(float), s));
+  dsk::batch_hard_coef_kernel<<<1, 1024, 0, s>>>(valid, N, grad_loss, coef);
   KERNEL_CHECK();
+  dsk::batch_hard_bwd_kernel<<<rows, 128, 0, s>>>(E, pos_idx, neg_idx, d_ap, d_an, valid, N, D, row0, margin, coef,
+                                                  gE_rows);
+  KERNEL_CHECK();
+  CUDA_TRY(cudaFreeAsync(coef, s));
   return DSK_OK;
 }
 
@@ -2245,15 +2299,8 @@ int32_t dsk_batch_hard_triplet_bwd(const float* E, const int64_t* pos_idx, const
   if (!E || !pos_idx || !neg_idx || !d_ap || !d_an || !grad_loss || !valid || !gE || D <= 0 || N < 2 ||
       N > DSK_BATCH_HARD_MAX_N)
     return fail(DSK_ERR_INVALID, "dsk_batch_hard_triplet_bwd: bad arguments (N must be 2..%d, got %d)", DSK_BATCH_HARD_MAX_N, N);
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  float* coef = nullptr;
-  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&coef), sizeof(float), s));
-  dsk::batch_hard_coef_kernel<<<1, 1024, 0, s>>>(valid, N, grad_loss, coef);
-  KERNEL_CHECK();
-  dsk::batch_hard_bwd_kernel<<<N, 128, 0, s>>>(E, pos_idx, neg_idx, d_ap, d_an, valid, N, D, margin, coef, gE);
-  KERNEL_CHECK();
-  CUDA_TRY(cudaFreeAsync(coef, s));
-  return DSK_OK;
+  return dsk_batch_hard_triplet_bwd_rows(E, pos_idx, neg_idx, d_ap, d_an, valid, N, D, 0, N, margin, grad_loss, gE,
+                                         stream);
 }
 
 int32_t dsk_allpairs_topk(const float* E, const int64_t* labels, int32_t N, int32_t D, int32_t k, int64_t* idx,
@@ -2264,9 +2311,9 @@ int32_t dsk_allpairs_topk(const float* E, const int64_t* labels, int32_t N, int3
   float* S = nullptr;
   CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&S), static_cast<size_t>(N) * N * sizeof(float), s));
   dim3 g((N + 63) / 64, (N + 63) / 64);
-  dsk::allpairs_sqdist_kernel<<<g, 256, 0, s>>>(E, N, D, S);
+  dsk::allpairs_sqdist_kernel<<<g, 256, 0, s>>>(E, N, D, 0, N, S);
   KERNEL_CHECK();
-  dsk::topk_rows_kernel<<<(N + 7) / 8, 256, 0, s>>>(S, labels, N, pd_eps(D), k, idx, val);
+  dsk::topk_rows_kernel<<<(N + 7) / 8, 256, 0, s>>>(S, labels, N, 0, N, pd_eps(D), k, idx, val);
   KERNEL_CHECK();
   CUDA_TRY(cudaFreeAsync(S, s));
   return DSK_OK;

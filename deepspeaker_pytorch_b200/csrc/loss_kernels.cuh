@@ -133,15 +133,16 @@ __global__ void gather_rows_kernel(const float* __restrict__ src, const int64_t*
 }
 
 // ---------------------------------------------------------------------------------------------
-// All-pairs distances (fp32, direct differences, sequential-in-d fmaf order) into a dense N x N
-// matrix, 64x64 tile per block of 256 threads (4x4 outputs per thread).
+// All-pairs distances (fp32, direct differences, sequential-in-d fmaf order) of the anchor rows [row0, row0 + rows)
+// against all N rows into a dense rows x N matrix, 64x64 tile per block of 256 threads (4x4 outputs per thread).
+// Every element depends only on its two rows, so any row range gives the bits of the full N x N matrix.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
-allpairs_sqdist_kernel(const float* __restrict__ E, int N, int D, float* __restrict__ S) {
+allpairs_sqdist_kernel(const float* __restrict__ E, int N, int D, int row0, int rows, float* __restrict__ S) {
   constexpr int TM = 64, TK = 16;
   __shared__ float As[TK][TM + 4];
   __shared__ float Bs[TK][TM + 4];
-  const int i0 = blockIdx.y * TM, j0 = blockIdx.x * TM;
+  const int i0 = row0 + blockIdx.y * TM, j0 = blockIdx.x * TM, row_end = row0 + rows;
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   float acc[4][4];
 #pragma unroll
@@ -151,7 +152,7 @@ allpairs_sqdist_kernel(const float* __restrict__ E, int N, int D, float* __restr
   for (int k0 = 0; k0 < D; k0 += TK) {
     for (int t = threadIdx.x; t < TM * TK; t += 256) {
       const int r = t / TK, k = t % TK;
-      As[k][r] = (i0 + r < N && k0 + k < D) ? E[static_cast<long>(i0 + r) * D + k0 + k] : 0.f;
+      As[k][r] = (i0 + r < row_end && k0 + k < D) ? E[static_cast<long>(i0 + r) * D + k0 + k] : 0.f;
       Bs[k][r] = (j0 + r < N && k0 + k < D) ? E[static_cast<long>(j0 + r) * D + k0 + k] : 0.f;
     }
     __syncthreads();
@@ -177,18 +178,20 @@ allpairs_sqdist_kernel(const float* __restrict__ E, int N, int D, float* __restr
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
       const int i = i0 + ty * 4 + r, j = j0 + tx * 4 + c;
-      if (i < N && j < N) S[static_cast<long>(i) * N + j] = acc[r][c];
+      if (i < row_end && j < N) S[static_cast<long>(i - row0) * N + j] = acc[r][c];
     }
 }
 
-// Per row: the k smallest sqrt(S+eps) among columns with a different label, ties -> lower column.
+// Per anchor row0 + i (i < rows): the k smallest sqrt(S+eps) among columns with a different label, ties -> lower
+// column.  S is the rows x N matrix of allpairs_sqdist_kernel; idx / val are written at local row i.
 // One warp per row; each pass extracts the lexicographic (value, index) minimum.
-__global__ void topk_rows_kernel(const float* __restrict__ S, const int64_t* __restrict__ labels, int N, float eps,
-                                 int k, int64_t* __restrict__ idx, float* __restrict__ val) {
-  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (row >= N) return;
+__global__ void topk_rows_kernel(const float* __restrict__ S, const int64_t* __restrict__ labels, int N, int row0,
+                                 int rows, float eps, int k, int64_t* __restrict__ idx, float* __restrict__ val) {
+  const int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (i >= rows) return;
+  const int row = row0 + i;
   const int lane = threadIdx.x & 31;
-  const float* s = S + static_cast<long>(row) * N;
+  const float* s = S + static_cast<long>(i) * N;
   const int64_t my_label = labels[row];
   float last_v = -1.f;
   int last_j = -1;
@@ -214,8 +217,8 @@ __global__ void topk_rows_kernel(const float* __restrict__ S, const int64_t* __r
       }
     }
     if (lane == 0) {
-      idx[static_cast<long>(row) * k + t] = (bj == 0x7fffffff) ? -1 : bj;
-      val[static_cast<long>(row) * k + t] = bv;
+      idx[static_cast<long>(i) * k + t] = (bj == 0x7fffffff) ? -1 : bj;
+      val[static_cast<long>(i) * k + t] = bv;
     }
     last_v = bv;
     last_j = bj;
@@ -269,22 +272,30 @@ __device__ __forceinline__ float exact_dist_seq(const float* __restrict__ a, con
   return sqrtf(acc + eps);
 }
 
-// One warp per row.  G: fp32 Gram of the rounded rows [Npad][Npad]; approximate squared distance
+// One warp per anchor row0 + i (i < rows).  G: fp32 Gram of the rounded anchor rows against all rounded rows
+// [rows_pad][Npad] (local row i); approximate squared distance
 // a_ij = n_i + n_j - 2 G_ij (exact squared distance of the ROUNDED rows up to fp32 accumulation).
 // Exactness argument: rounding row e to 16 bit moves it by at most u*||e|| (u = unit roundoff), so for every pair
 //   | a_ij - ||e_i - e_j||^2 | <= 2 d r + r^2 + slack,   r = u (||e_i|| + max_j ||e_j||),  d = ||e_i - e_j||.
 // If the worst kept candidate's a exceeds (k-th exact distance)^2 by more than that bound, no discarded column can
 // beat the k-th result and the refined top-k is the exact answer; otherwise the warp scans the whole row exactly.
+// Either way the result is the exact one, whatever the Gram's bits: idx / val (written at local row i) do not depend on
+// the row range the Gram was computed for.  ROWS = false is the whole batch (row0 = 0, rows = N, the arguments are
+// ignored): dsk_allpairs_topk_tc and the whole-batch loss run the instruction stream they ran before the row range
+// existed, without the offset arithmetic in this latency-bound kernel.
+template <bool ROWS>
 __global__ void __launch_bounds__(256)
 allpairs_select_refine_kernel(const float* __restrict__ E, const float* __restrict__ G, const float* __restrict__ norms,
-                              const int64_t* __restrict__ labels, int N, int Npad, int D, float eps, int k, float u,
-                              int64_t* __restrict__ idx, float* __restrict__ val) {
+                              const int64_t* __restrict__ labels, int N, int Npad, int row0_arg, int rows_arg, int D,
+                              float eps, int k, float u, int64_t* __restrict__ idx, float* __restrict__ val) {
   __shared__ int cand_j[8][kApCand];
   __shared__ float cand_a[8][kApCand];
+  const int row0 = ROWS ? row0_arg : 0, rows = ROWS ? rows_arg : N;
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int row = blockIdx.x * 8 + w;
-  if (row >= N) return;
-  const float* g = G + static_cast<long>(row) * Npad;
+  const int i = blockIdx.x * 8 + w;
+  if (i >= rows) return;
+  const int row = row0 + i;
+  const float* g = G + static_cast<long>(i) * Npad;
   const float ni = norms[row];
   const int64_t my_label = labels[row];
   const float INF = __int_as_float(0x7f800000);
@@ -411,8 +422,8 @@ allpairs_select_refine_kernel(const float* __restrict__ E, const float* __restri
         }
       }
       if (lane == 0) {
-        idx[static_cast<long>(row) * k + t] = (bj == 0x7fffffff) ? -1 : bj;
-        val[static_cast<long>(row) * k + t] = bv;
+        idx[static_cast<long>(i) * k + t] = (bj == 0x7fffffff) ? -1 : bj;
+        val[static_cast<long>(i) * k + t] = bv;
       }
       lv = bv;
       lj = bj;
@@ -439,8 +450,8 @@ allpairs_select_refine_kernel(const float* __restrict__ E, const float* __restri
       }
     }
     if (lane == 0) {
-      idx[static_cast<long>(row) * k + t] = (bj == 0x7fffffff) ? -1 : bj;
-      val[static_cast<long>(row) * k + t] = bv;
+      idx[static_cast<long>(i) * k + t] = (bj == 0x7fffffff) ? -1 : bj;
+      val[static_cast<long>(i) * k + t] = bv;
     }
     lv = bv;
     lj = bj;
@@ -456,13 +467,15 @@ allpairs_select_refine_kernel(const float* __restrict__ E, const float* __restri
 // Hardest positive, one warp per anchor: argmax over j != i with labels[j] == labels[i] of the exact distance, ties ->
 // lower j (FROM_S: sqrt(S[i][j] + eps) from allpairs_sqdist_kernel, else exact_dist_seq; the two are the same bits).
 // pos_idx = -1 and d_ap = 0 when the anchor has no positive.  valid[i] = 1 iff it has a positive and a negative.
+// Anchors row0 + i for i < rows; S (rows x N) and the outputs are indexed by the local row i, column indices are global.
 template <bool FROM_S>
 __global__ void __launch_bounds__(256)
 batch_hard_positive_kernel(const float* __restrict__ E, const float* __restrict__ S, const int64_t* __restrict__ labels,
-                           int N, int D, float eps, int64_t* __restrict__ pos_idx, float* __restrict__ d_ap,
-                           uint8_t* __restrict__ valid) {
-  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (row >= N) return;
+                           int N, int row0, int rows, int D, float eps, int64_t* __restrict__ pos_idx,
+                           float* __restrict__ d_ap, uint8_t* __restrict__ valid) {
+  const int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (i >= rows) return;
+  const int row = row0 + i;
   const int lane = threadIdx.x & 31;
   const int64_t my_label = labels[row];
   float bv = -1.f;  // below every distance (>= sqrt(eps) > 0)
@@ -474,7 +487,7 @@ batch_hard_positive_kernel(const float* __restrict__ E, const float* __restrict_
       continue;
     }
     if (j == row) continue;
-    const float v = FROM_S ? sqrtf(S[static_cast<long>(row) * N + j] + eps)
+    const float v = FROM_S ? sqrtf(S[static_cast<long>(i) * N + j] + eps)
                            : exact_dist_seq(E + static_cast<long>(row) * D, E + static_cast<long>(j) * D, D, eps);
     if (v > bv) {  // each lane scans ascending j: strict > keeps the lower index of a tie
       bv = v;
@@ -492,9 +505,9 @@ batch_hard_positive_kernel(const float* __restrict__ E, const float* __restrict_
   has_neg = __any_sync(0xffffffffu, has_neg);
   if (lane == 0) {
     const bool has_pos = bj != 0x7fffffff;
-    pos_idx[row] = has_pos ? bj : -1;
-    d_ap[row] = has_pos ? bv : 0.f;
-    valid[row] = (has_pos && has_neg) ? 1 : 0;
+    pos_idx[i] = has_pos ? bj : -1;
+    d_ap[i] = has_pos ? bv : 0.f;
+    valid[i] = (has_pos && has_neg) ? 1 : 0;
   }
 }
 
@@ -553,18 +566,22 @@ __device__ __forceinline__ bool batch_hard_active(const uint8_t* valid, const fl
 // chunk of 128 anchors is compacted (warp ballots + a block prefix, stable) into shared memory, then applied.  A row that
 // many anchors chose (a hub) only makes its own block longer.  Terms, with g = coef[0] and one division per term:
 //   anchor a:  (g / d_ap) (a - p) - (g / d_an) (a - n);   its positive p: -(g / d_ap) (a - p);   its negative n: +(g / d_an) (a - n).
+// The chooser's thread divides while the list is built, so the apply loop holds no division call (no spill).
+// Block b computes row j = row0 + b into gE[b]; the selection arrays cover all N anchors, so any row range gives the
+// bits of the full gradient.
 __global__ void __launch_bounds__(128)
 batch_hard_bwd_kernel(const float* __restrict__ E, const int64_t* __restrict__ pos_idx,
                       const int64_t* __restrict__ neg_idx, const float* __restrict__ d_ap,
-                      const float* __restrict__ d_an, const uint8_t* __restrict__ valid, int N, int D, float margin,
-                      const float* __restrict__ coef, float* __restrict__ gE) {
-  __shared__ int list[128];  // 2 * anchor + (1 if row j is that anchor's negative, 0 if its positive)
+                      const float* __restrict__ d_an, const uint8_t* __restrict__ valid, int N, int D, int row0,
+                      float margin, const float* __restrict__ coef, float* __restrict__ gE) {
+  __shared__ int list[128];     // anchors that chose row j, ascending
+  __shared__ float scale[128];  // their signed coefficients: -(g / d_ap) if j is the positive, +(g / d_an) if the negative
   __shared__ int wcnt[4];
-  const int j = blockIdx.x;
+  const int j = row0 + blockIdx.x;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const float g = coef[0];
   const float* ej = E + static_cast<long>(j) * D;
-  float* gj = gE + static_cast<long>(j) * D;
+  float* gj = gE + static_cast<long>(blockIdx.x) * D;
   if (batch_hard_active(valid, d_ap, d_an, j, margin)) {
     const float* ep = E + pos_idx[j] * D;
     const float* en = E + neg_idx[j] * D;
@@ -575,12 +592,18 @@ batch_hard_bwd_kernel(const float* __restrict__ E, const int64_t* __restrict__ p
   }
   for (int base = 0; base < N; base += 128) {
     const int i = base + threadIdx.x;
-    int code = -1;
+    bool chose = false;
+    float sc = 0.f;
     if (i < N && batch_hard_active(valid, d_ap, d_an, i, margin)) {
-      if (pos_idx[i] == j) code = 2 * i;
-      else if (neg_idx[i] == j) code = 2 * i + 1;
+      if (pos_idx[i] == j) {
+        chose = true;
+        sc = -(g / d_ap[i]);
+      } else if (neg_idx[i] == j) {
+        chose = true;
+        sc = g / d_an[i];
+      }
     }
-    const unsigned m = __ballot_sync(0xffffffffu, code >= 0);
+    const unsigned m = __ballot_sync(0xffffffffu, chose);
     if (lane == 0) wcnt[warp] = __popc(m);
     __syncthreads();
     int off = 0, total = 0;
@@ -588,21 +611,18 @@ batch_hard_bwd_kernel(const float* __restrict__ E, const int64_t* __restrict__ p
       off += w < warp ? wcnt[w] : 0;
       total += wcnt[w];
     }
-    if (code >= 0) list[off + __popc(m & ((1u << lane) - 1u))] = code;
+    if (chose) {
+      const int at = off + __popc(m & ((1u << lane) - 1u));
+      list[at] = i;
+      scale[at] = sc;
+    }
     __syncthreads();
     for (int e = 0; e < total; ++e) {
-      const int c = list[e];
-      const int a = c >> 1;
-      const float* ea = E + static_cast<long>(a) * D;
-      if (c & 1) {
-        const float sn = g / d_an[a];
-        for (int d = threadIdx.x; d < D; d += 128) gj[d] += sn * (ea[d] - ej[d]);
-      } else {
-        const float sp = g / d_ap[a];
-        for (int d = threadIdx.x; d < D; d += 128) gj[d] -= sp * (ea[d] - ej[d]);
-      }
+      const float* ea = E + static_cast<long>(list[e]) * D;
+      const float sc = scale[e];
+      for (int d = threadIdx.x; d < D; d += 128) gj[d] += sc * (ea[d] - ej[d]);
     }
-    __syncthreads();  // list and wcnt are rewritten by the next chunk
+    __syncthreads();  // list, scale and wcnt are rewritten by the next chunk
   }
 }
 

@@ -317,6 +317,52 @@ def batch_hard_backward(E, pos, neg, d_ap, d_an, valid, margin, grad_loss):
     return gE
 
 
+def batch_hard_select_rows(E, labels, row0, rows, exact_cuda_cores: bool = False):
+    """dsk_batch_hard_select_rows: the selection of the anchors [row0, row0 + rows) of the batch E (N, D) ->
+    (E fp32 contiguous, pos_idx, neg_idx, d_ap, d_an, valid (bool)), each (rows,) on E's device, bit-identical to those
+    rows of ``batch_hard_mine``.  Indices are global.  The tensor-core Gram plan is cached per (N, D, row0, rows)."""
+    _check2d(E)
+    E = E.detach().float().contiguous()
+    labels = labels.to(device=E.device, dtype=torch.int64).contiguous()
+    N, D = E.shape
+    if labels.shape != (N,):
+        raise RuntimeError(f"expected labels of shape ({N},), got {tuple(labels.shape)}")
+    dev, n = E.device, max(int(rows), 0)
+    pos, neg = (torch.empty(n, device=dev, dtype=torch.int64) for _ in range(2))
+    d_ap, d_an = (torch.empty(n, device=dev, dtype=torch.float32) for _ in range(2))
+    valid = torch.empty(n, device=dev, dtype=torch.bool)
+    with torch.cuda.device(dev):
+        h = None if exact_cuda_cores else _allpairs_handle(dev)
+        L.check(L.load().dsk_batch_hard_select_rows(h, E.data_ptr(), labels.data_ptr(), N, D, int(row0), int(rows),
+                                                    pos.data_ptr(), neg.data_ptr(), d_ap.data_ptr(), d_an.data_ptr(),
+                                                    valid.data_ptr(), L.cur_stream()), "dsk_batch_hard_select_rows")
+    return E, pos, neg, d_ap, d_an, valid
+
+
+def batch_hard_mean(d_ap, d_an, valid, margin):
+    """dsk_batch_hard_mean: loss (1,) from the selection of all N anchors, the bits of ``batch_hard_mine``'s loss."""
+    N = d_ap.shape[0]
+    loss = torch.empty(1, device=d_ap.device, dtype=torch.float32)
+    with torch.cuda.device(d_ap.device):
+        L.check(L.load().dsk_batch_hard_mean(d_ap.data_ptr(), d_an.data_ptr(), valid.data_ptr(), N, float(margin),
+                                             loss.data_ptr(), L.cur_stream()), "dsk_batch_hard_mean")
+    return loss
+
+
+def batch_hard_backward_rows(E, pos, neg, d_ap, d_an, valid, row0, rows, margin, grad_loss):
+    """dsk_batch_hard_triplet_bwd_rows: rows [row0, row0 + rows) of ``batch_hard_backward`` -> (rows, D), the same
+    bits.  The selection tensors cover all N anchors of E."""
+    N, D = E.shape
+    gl = grad_loss.float().reshape(1).contiguous()
+    gE = torch.empty(max(int(rows), 0), D, device=E.device, dtype=torch.float32)
+    with torch.cuda.device(E.device):
+        L.check(L.load().dsk_batch_hard_triplet_bwd_rows(E.data_ptr(), pos.data_ptr(), neg.data_ptr(), d_ap.data_ptr(),
+                                                         d_an.data_ptr(), valid.data_ptr(), N, D, int(row0), int(rows),
+                                                         float(margin), gl.data_ptr(), gE.data_ptr(), L.cur_stream()),
+                "dsk_batch_hard_triplet_bwd_rows")
+    return gE
+
+
 class BatchHardTripletFn(torch.autograd.Function):
     """Batch-hard triplet loss (in-batch hardest positive and negative per anchor, mean hinge over valid anchors);
     the loss is a device scalar."""

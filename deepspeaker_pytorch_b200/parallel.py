@@ -6,11 +6,17 @@ differentiated parameters are averaged with a single ``all_reduce`` over one fla
 (11 624 128 elements, 46.5 MB).  BatchNorm statistics stay per replica, as in the reference (no SyncBN).
 
 ``torch.distributed`` (NCCL over NVLink on the GPU box, gloo in the CPU tests) is plumbing here.
+
+Batch-hard mining over the global batch (``GlobalBatchHardTripletLoss``, ``batch_hard_step(..., across_ranks=True)``)
+adds three small all_gathers per step: the labels, the fp32 embeddings and the selection records.  The gradient
+reduction stays the one all-reduce.
 """
 from __future__ import annotations
 
 import torch
 import torch.distributed as dist
+
+from . import engine as _engine
 
 
 class GradBucket:
@@ -87,3 +93,107 @@ def shard(batch: torch.Tensor, rank: int, world: int) -> torch.Tensor:
         raise ValueError(f"global batch {n} is not divisible by world size {world}")
     per = n // world
     return batch[rank * per:(rank + 1) * per]
+
+
+# ---- batch-hard mining over the global batch --------------------------------------------------------------------------
+# Rank r holds the contiguous shard [r n, (r + 1) n) of a global batch of N = R n utterances (what ``shard`` produces).
+# EVERY RANK MUST HOLD THE SAME n: the gathers below are all_gather_into_tensor, which assumes equal sizes (with unequal
+# sizes NCCL waits forever rather than raising).
+
+def _distributed(process_group=None) -> bool:
+    return dist.is_available() and dist.is_initialized() and dist.get_world_size(process_group) > 1
+
+
+def gather_labels(local_labels, process_group=None) -> torch.Tensor:
+    """The global batch's labels (N,) int64 in rank order, from every rank's (n,) shard: one all_gather_into_tensor.
+    Under NCCL CPU labels are moved to the current CUDA device first.  Without a process group (or at world size 1)
+    the labels are returned as given."""
+    lab = torch.as_tensor(local_labels, dtype=torch.int64).reshape(-1)
+    if not _distributed(process_group):
+        return lab
+    if not lab.is_cuda and dist.get_backend(process_group) == "nccl":
+        lab = lab.to(torch.cuda.current_device())
+    lab = lab.contiguous()
+    out = lab.new_empty(dist.get_world_size(process_group) * lab.numel())
+    dist.all_gather_into_tensor(out, lab, group=process_group)
+    return out
+
+
+# The selection of one anchor travels as a 25-byte record: pos_idx, neg_idx (int64), d_ap, d_an (fp32), valid (1 byte).
+# A rank's n records are laid out field by field - (8 + 8 + 4 + 4 + 1) n bytes, every field aligned to its size - so
+# packing is one cat of byte views and unpacking one strided copy per field.
+_SELECTION_FIELDS = ((8, torch.int64), (8, torch.int64), (4, torch.float32), (4, torch.float32), (1, torch.bool))
+SELECTION_RECORD_BYTES = sum(b for b, _ in _SELECTION_FIELDS)
+
+
+def _pack_selection(pos, neg, d_ap, d_an, valid) -> torch.Tensor:
+    """(n,) each -> uint8 (25 n,)."""
+    return torch.cat([t.contiguous().view(torch.uint8) for t in (pos, neg, d_ap, d_an, valid)])
+
+
+def _unpack_selection(records, n):
+    """uint8 (R, 25 n), one row per rank -> (pos_idx, neg_idx, d_ap, d_an, valid), each (R n,) in rank order."""
+    out, lo = [], 0
+    for size, dtype in _SELECTION_FIELDS:
+        out.append(records[:, lo * n:(lo + size) * n].contiguous().view(dtype).reshape(-1))
+        lo += size
+    return tuple(out)
+
+
+class _GlobalBatchHardFn(torch.autograd.Function):
+    """Forward: all_gather of the fp32 embeddings, selection of this rank's anchor rows, all_gather of the selection
+    records, the mean over all N anchors.  Backward: this rank's rows of the gradient; no collective."""
+
+    @staticmethod
+    def forward(ctx, local_emb, global_labels, margin, exact_cuda_cores, group):
+        world, rank = dist.get_world_size(group), dist.get_rank(group)
+        x = local_emb.detach().float().contiguous()
+        n = x.shape[0]
+        E = x.new_empty(world * n, x.shape[1])
+        dist.all_gather_into_tensor(E, x, group=group)
+        row0 = rank * n
+        E, *sel = _engine.batch_hard_select_rows(E, global_labels, row0, n, exact_cuda_cores)
+        rec = _pack_selection(*sel)
+        records = rec.new_empty(world * rec.numel())
+        dist.all_gather_into_tensor(records, rec, group=group)
+        pos, neg, d_ap, d_an, valid = _unpack_selection(records.view(world, -1), n)
+        loss = _engine.batch_hard_mean(d_ap, d_an, valid, margin)
+        ctx.save_for_backward(E, pos, neg, d_ap, d_an, valid)
+        ctx.margin, ctx.row0, ctx.n = margin, row0, n
+        return loss.reshape(())
+
+    @staticmethod
+    def backward(ctx, gl):
+        E, pos, neg, d_ap, d_an, valid = ctx.saved_tensors
+        g = _engine.batch_hard_backward_rows(E, pos, neg, d_ap, d_an, valid, ctx.row0, ctx.n, ctx.margin, gl)
+        return g, None, None, None, None
+
+
+class GlobalBatchHardTripletLoss:
+    """``BatchHardTripletLoss`` over the GLOBAL batch under data parallelism: every anchor takes its hardest positive
+    and negative among all N = R n utterances, not only its own rank's n.  The loss is the same device scalar on every
+    rank and bit-identical to ``BatchHardTripletLoss`` on the gathered embeddings; its gradient w.r.t. ``local_emb`` is
+    this rank's rows of that loss's gradient.  Summed over ranks (the mean all-reduce of the gradients scaled by R, as
+    ``batch_hard_step(..., across_ranks=True)`` does) that is the gradient of the global loss.
+
+    Collectives per forward: two all_gathers (embeddings N·D·4 bytes, selection 25 bytes per anchor); none in the
+    backward.  The labels are an input: gather them once per batch with ``gather_labels``.  Precondition: every rank
+    holds the same n.  Without a process group, or at world size 1, this is exactly ``BatchHardTripletLoss`` and issues
+    no collective."""
+
+    def __init__(self, margin, process_group=None, exact_cuda_cores=False):
+        self.margin = margin
+        self.group = process_group
+        self.exact_cuda_cores = exact_cuda_cores
+
+    def forward(self, local_emb, global_labels):
+        """local_emb (n, D) this rank's shard, global_labels (N,) int64 of the whole batch -> 0-dim loss."""
+        if not _distributed(self.group):
+            return _engine.BatchHardTripletFn.apply(local_emb, global_labels, float(self.margin), self.exact_cuda_cores)
+        world = dist.get_world_size(self.group)
+        if global_labels.shape != (world * local_emb.shape[0],):
+            raise ValueError(f"expected global labels of shape ({world * local_emb.shape[0]},) for {world} ranks of "
+                             f"{local_emb.shape[0]} embeddings, got {tuple(global_labels.shape)}")
+        return _GlobalBatchHardFn.apply(local_emb, global_labels, float(self.margin), self.exact_cuda_cores, self.group)
+
+    __call__ = forward

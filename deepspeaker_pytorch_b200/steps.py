@@ -23,12 +23,14 @@ same single allreduce.
 from __future__ import annotations
 
 import torch
+import torch.distributed as dist
 
 from . import engine as _engine
 from .head import CrossEntropyLoss
 from .model import (BatchHardTripletLoss, PairwiseDistance, TripletMarginLoss, batch_hard_valid_count,
                     select_hard_triplets)
 from .optim import FusedAdagrad
+from .parallel import GlobalBatchHardTripletLoss, _distributed, gather_labels
 
 _l2 = PairwiseDistance(2)   # train_triplet.py:119
 
@@ -98,26 +100,63 @@ def train_step(model, optimizer, data_a, data_p, data_n, label_p, label_n, *, ma
             "hard": hard}
 
 
-def batch_hard_step(model, optimizer, data, labels, *, margin, bucket=None):
+def _labels_to(labels, device):
+    labels = torch.as_tensor(labels, dtype=torch.int64)
+    if not labels.is_cuda:   # a pageable copy would wait for the stream; a pinned one is queued like a kernel
+        labels = labels.pin_memory().to(device, non_blocking=True)
+    return labels
+
+
+def _no_valid_anchor():
+    return ValueError("batch_hard_step: no valid anchor in the batch (it needs >= 2 speakers, one of them with "
+                      ">= 2 utterances)")
+
+
+def batch_hard_step(model, optimizer, data, labels, *, margin, bucket=None, across_ranks=False):
     """One batch-hard training step on a P speakers x K utterances batch: ONE train-mode forward of all N utterances
     (BatchNorm statistics over the whole batch), ``BatchHardTripletLoss`` (hardest positive and negative of every anchor
     inside the batch), backward through all N embeddings, optimizer step.  Under data parallelism each rank's gradient
     is weighted by its number of valid anchors V_r (the mechanism of branch B), so the update is that of the mean over
     the union of valid anchors.  V comes from the labels on the host: with CPU labels the step reads nothing back from
     the device.  Returns ``{"loss": device scalar, "valid": V}``; raises ValueError for a batch with V = 0 (no speaker
-    with two utterances, or a single speaker)."""
+    with two utterances, or a single speaker).
+
+    ``across_ranks=True`` (data parallelism, ``data`` / ``labels`` this rank's shard, the same size on every rank):
+    anchors are mined over the GLOBAL batch with ``parallel.GlobalBatchHardTripletLoss``, so the loss and the selected
+    triplets do not depend on the number of ranks.  The labels are gathered first and read back to the host for the
+    global V - the step's one host synchronisation; every rank then sees the same V, so on V = 0 all ranks raise before
+    any other collective.  The backward is seeded with R: the unchanged mean all-reduce of the gradients (/R) then sums
+    the ranks' gradients, which is the gradient of the global loss (exactly so for power-of-two R).  The ranks are
+    those of the optimizer's (``FusedAdagrad``) or the bucket's process group.  BatchNorm statistics stay per replica.
+    ``valid`` is the global V.  Without a process group this is the step with ``across_ranks=False``."""
     if not model.training:
         raise RuntimeError("batch_hard_step needs model.train()")
+    if across_ranks:
+        return _global_batch_hard_step(model, optimizer, data, labels, margin, bucket)
     V = batch_hard_valid_count(labels)
     if V == 0:
-        raise ValueError("batch_hard_step: no valid anchor in the batch (it needs >= 2 speakers, one of them with "
-                         ">= 2 utterances)")
-    labels = torch.as_tensor(labels, dtype=torch.int64)
-    if not labels.is_cuda:   # a pageable copy would wait for the stream; a pinned one is queued like a kernel
-        labels = labels.pin_memory().to(data.device, non_blocking=True)
+        raise _no_valid_anchor()
+    labels = _labels_to(labels, data.device)
     emb = model(data)
     loss = BatchHardTripletLoss(margin).forward(emb, labels)
     optimizer.zero_grad()
     loss.backward()
     _reduce_and_step(optimizer, bucket, torch.tensor(float(V)))
+    return {"loss": loss.detach(), "valid": V}
+
+
+def _global_batch_hard_step(model, optimizer, data, labels, margin, bucket):
+    group = optimizer.group if isinstance(optimizer, FusedAdagrad) else (bucket.group if bucket is not None else None)
+    if not _distributed(group):
+        return batch_hard_step(model, optimizer, data, labels, margin=margin, bucket=bucket)
+    world = dist.get_world_size(group)
+    global_labels = gather_labels(_labels_to(labels, data.device), group)   # behind the last step's all-reduce
+    V = batch_hard_valid_count(global_labels.cpu())                          # the step's one host synchronisation
+    if V == 0:
+        raise _no_valid_anchor()
+    emb = model(data)
+    loss = GlobalBatchHardTripletLoss(margin, group).forward(emb, global_labels)
+    optimizer.zero_grad()
+    loss.backward(torch.full_like(loss, float(world)))       # R x this rank's share; the mean all-reduce divides by R
+    _reduce_and_step(optimizer, bucket, None)
     return {"loss": loss.detach(), "valid": V}

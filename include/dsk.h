@@ -253,6 +253,25 @@ int32_t dsk_batch_hard_triplet(dsk_handle h, const float* E, const int64_t* labe
 int32_t dsk_batch_hard_triplet_bwd(const float* E, const int64_t* pos_idx, const int64_t* neg_idx, const float* d_ap,
                                    const float* d_an, int32_t N, int32_t D, float margin, const float* grad_loss,
                                    const uint8_t* valid, float* gE, void* stream);
+/* Row-range form of the batch-hard op, for sharding the anchors of one N-row batch E (e.g. across data-parallel ranks)
+ * with results bit-identical to the single-device op on the whole batch.  Rows [row0, row0 + rows) of E are the
+ * anchors: 2 <= N <= DSK_BATCH_HARD_MAX_N, 0 <= row0, 1 <= rows, row0 + rows <= N (else DSK_ERR_INVALID).
+ * dsk_batch_hard_select_rows: outputs (rows,) hold anchor row0 + i's selection as in dsk_batch_hard_triplet (indices
+ * global in [0, N), self-exclusion j != row0 + i, the same tie rules and bits).  h != NULL and D % 64 == 0: the Gram
+ * plan is rows_pad x Npad and is cached in h for (N, D, row0, rows); a change of any of them rebuilds it, which
+ * synchronises the stream.  dsk_batch_hard_triplet = select_rows(0, N) + dsk_batch_hard_mean.
+ * dsk_batch_hard_mean: the loss of dsk_batch_hard_triplet from the selection of all N anchors.
+ * dsk_batch_hard_triplet_bwd_rows: rows [row0, row0 + rows) of dsk_batch_hard_triplet_bwd's gE into gE_rows (rows, D);
+ * the selection arrays cover all N anchors.  dsk_batch_hard_triplet_bwd = bwd_rows(0, N). */
+int32_t dsk_batch_hard_select_rows(dsk_handle h, const float* E, const int64_t* labels, int32_t N, int32_t D,
+                                   int32_t row0, int32_t rows, int64_t* pos_idx, int64_t* neg_idx, float* d_ap,
+                                   float* d_an, uint8_t* valid, void* stream);
+int32_t dsk_batch_hard_mean(const float* d_ap, const float* d_an, const uint8_t* valid, int32_t N, float margin,
+                            float* loss, void* stream);
+int32_t dsk_batch_hard_triplet_bwd_rows(const float* E, const int64_t* pos_idx, const int64_t* neg_idx,
+                                        const float* d_ap, const float* d_an, const uint8_t* valid, int32_t N,
+                                        int32_t D, int32_t row0, int32_t rows, float margin, const float* grad_loss,
+                                        float* gE_rows, void* stream);
 
 /* nn.Linear of DeepSpeakerModel.forward_classifier (reference model.py:167,220-223): y (M,N) = x (M,K) w(N,K)^T + b.
  * fp32 on the CUDA cores, fixed summation order (deterministic).  b may be NULL. */
