@@ -129,6 +129,11 @@ SIGNATURES = {
     "dsk_debug_read_eval_activation": (c_int32, [c_void_p, c_int32, c_void_p, c_int64, POINTER(c_int32), c_void_p]),
     "dsk_train_ctx_release": (c_int32, [c_void_p, c_void_p]),
     "dsk_set_loss_scale": (c_int32, [c_void_p, c_float]),
+    "dsk_sync_forward_begin": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, POINTER(c_void_p), c_void_p]),
+    "dsk_sync_backward_begin": (c_int32, [c_void_p, c_void_p, c_void_p, POINTER(DskGrads), c_void_p]),
+    "dsk_sync_records": (c_int32, [c_void_p, c_void_p, POINTER(c_void_p), POINTER(c_int64)]),
+    "dsk_sync_stage": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, POINTER(c_int32), c_void_p]),
+    "dsk_bn_act_sync_train_forward": (c_int32, [c_void_p] * 10 + [c_int32, c_int32, c_int32, c_void_p]),
     "dsk_set_profiling": (c_int32, [c_void_p, c_int32]),
     "dsk_get_launch_times": (c_int32, [c_void_p, c_void_p, c_int32, POINTER(c_int32)]),
     "dsk_conv2d_nhwc": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32,

@@ -291,6 +291,15 @@ struct dsk_train_ctx_s {
   ConvLaunch dgrad[DSK_NUM_CONV][4];
   int n_dgrad[DSK_NUM_CONV] = {};
   WgradLaunch wgrad[DSK_NUM_CONV];
+  // synchronised BatchNorm (dsk_sync_*): the staged forward or backward in progress
+  int sync_dir = 0;                    // 0 none, 1 forward, 2 backward
+  int sync_stage = 0;                  // forward: the layer whose records are out; backward: 12 (loss scale), then 11..0
+  bool sync_fwd = false;               // this context's forward ran with synchronised statistics
+  bool sync_update = false;            // the stages update the running statistics themselves (not deferred)
+  float* rec = nullptr;                // this stage's records of the B local utterances
+  long long* mtot = nullptr;           // [12] global pixel count of each layer's statistics
+  float* emb_out = nullptr;            // borrowed: where the forward's tail writes the embeddings
+  dsk_grads grads = {};                // the backward's output pointers
 };
 
 namespace {
@@ -1508,6 +1517,7 @@ static int ctx_create(dsk_handle h, int cap, int T, cudaStream_t s, dsk_train_ct
   }
   const size_t o_dw = take(dw_bytes), o_c1 = take(static_cast<size_t>(B) * ((T / 2 + 7) / 8) * 1600 * 4);
   const size_t o_gA = take(max_act), o_gB = take(max_act), o_G = take(max_act), o_gres = take(max_act);
+  const size_t o_rec = take(static_cast<size_t>(B) * (3 * 512 + 1) * 4), o_mtot = take(DSK_NUM_CONV * 8);
   if (cudaMalloc(reinterpret_cast<void**>(&c->base), bytes) != cudaSuccess) {
     cudaGetLastError();
     delete c;
@@ -1540,6 +1550,8 @@ static int ctx_create(dsk_handle h, int cap, int T, cudaStream_t s, dsk_train_ct
   c->gB = b + o_gB;
   c->G = b + o_G;
   c->gres = b + o_gres;
+  c->rec = reinterpret_cast<float*>(b + o_rec);
+  c->mtot = reinterpret_cast<long long*>(b + o_mtot);
   *out = c;
   return DSK_OK;
 }
@@ -1600,6 +1612,8 @@ static int ctx_acquire(dsk_handle h, int B, int T, cudaStream_t s, dsk_train_ctx
   }
   int rc = ctx_bind(h, best, B);
   if (rc) return rc;
+  best->sync_dir = 0;
+  best->sync_fwd = false;
   *out = best;
   return DSK_OK;
 }
@@ -1709,6 +1723,7 @@ int32_t dsk_rescnn_backward(dsk_handle h, dsk_train_ctx c, const float* grad_emb
   int rc = check_handle(h);
   if (rc) return rc;
   if (!c || !c->in_use || !c->forward_done) return fail(DSK_ERR_STATE, "dsk_rescnn_backward: context has no pending forward");
+  if (c->sync_fwd) return fail(DSK_ERR_STATE, "dsk_rescnn_backward: a synchronised forward needs dsk_sync_backward_begin");
   if (!grad_emb || !g) return fail(DSK_ERR_INVALID, "dsk_rescnn_backward: null argument");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const bool bf = h->bf16;
@@ -1833,6 +1848,237 @@ int32_t dsk_train_ctx_release(dsk_handle h, dsk_train_ctx c) {
   return DSK_OK;
 }
 
+// ---- synchronised BatchNorm: the train forward and backward as resumable stages -----------------------------------
+// Each stage ends where this rank's per-utterance records (train_kernels.cuh) are ready; the caller gathers every rank's
+// records in rank order and resumes with them.  Convs, the apply kernels, the weight gradients and the tail are the
+// kernels of dsk_rescnn_forward_train / dsk_rescnn_backward.
+
+// fp32 words of one utterance's record at the current stage
+static long sync_rec_words(const dsk_train_ctx_s* c) {
+  if (c->sync_dir == 2 && c->sync_stage == DSK_NUM_CONV) return 1;  // max |dL/d(fc out)|
+  int H, W, C;
+  act_shape(c->sync_stage, c->T, H, W, C);
+  return c->sync_dir == 1 ? 3L * C + 1 : 2L * C;
+}
+
+static void sync_fwd_records(dsk_train_ctx_s* c, int i, cudaStream_t s) {
+  int H, W, C;
+  act_shape(i, c->T, H, W, C);
+  dsk::bn_utt_record_kernel<<<dim3(c->B, C / 64), 256, 0, s>>>(c->raw[i], H * W, C, c->rec);
+}
+
+static void sync_bwd_records(dsk_handle h, dsk_train_ctx_s* c, int i, cudaStream_t s) {
+  int H, W, C;
+  act_shape(i, c->T, H, W, C);
+  const uint16_t* gy = (const uint16_t*)(((DSK_NUM_CONV - 1 - i) % 2 == 0) ? c->gA : c->gB);
+  dim3 g(c->B, C / 64);
+  if (h->bf16)
+    dsk::bn_bwd_utt_record_kernel<true><<<g, 256, 0, s>>>(gy, (const uint16_t*)c->y[i], c->raw[i], c->mean[i], c->rstd[i],
+                                                          H * W, C, 20.0f, c->rec);
+  else
+    dsk::bn_bwd_utt_record_kernel<false><<<g, 256, 0, s>>>(gy, (const uint16_t*)c->y[i], c->raw[i], c->mean[i], c->rstd[i],
+                                                           H * W, C, 20.0f, c->rec);
+}
+
+// forward of layer i up to its records
+static int sync_fwd_conv(dsk_handle h, dsk_train_ctx_s* c, int i, cudaStream_t s) {
+  if (i == 0) {
+    dsk::conv1_kernel<false, true><<<c->B * ((c->T / 2 + 7) / 8), 256, 0, s>>>(c->x, h->conv1_w, h->ones, h->zeros, c->raw[0],
+                                                                              c->T, 0, 0.f, 0);
+    KERNEL_CHECK();
+  } else {
+    int rc = launch_conv(h, c->conv[i], s);
+    if (rc) return rc;
+  }
+  sync_fwd_records(c, i, s);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// layer i's global statistics from the gathered records, its BatchNorm + residual + clip, then the next layer's conv
+// and records or the tail
+static int sync_fwd_stage(dsk_handle h, dsk_train_ctx_s* c, const float* gathered, int N, cudaStream_t s, int* more) {
+  const int i = c->sync_stage, B = c->B, T = c->T;
+  int H, W, C;
+  act_shape(i, T, H, W, C);
+  const long M = static_cast<long>(B) * H * W;
+  dsk::bn_record_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(
+      gathered, N, C, h->w.bn_gamma[i], h->w.bn_beta[i], h->w.bn_running_mean[i], h->w.bn_running_var[i], 0.1f, 1e-5f,
+      c->mean[i], c->rstd[i], c->scale_t, c->shift_t, c->unb[i], c->mtot + i, c->sync_update ? 1 : 0);
+  KERNEL_CHECK();
+  const uint16_t* res = (i % 3 == 2) ? (const uint16_t*)c->y[i - 2] : nullptr;
+  dim3 ga(static_cast<unsigned>((M + 63) / 64), C / 64);
+  if (h->bf16)
+    dsk::bn_apply_kernel<true><<<ga, 256, 0, s>>>(c->raw[i], c->scale_t, c->shift_t, res, (uint16_t*)c->y[i], M, C, 20.0f);
+  else
+    dsk::bn_apply_kernel<false><<<ga, 256, 0, s>>>(c->raw[i], c->scale_t, c->shift_t, res, (uint16_t*)c->y[i], M, C, 20.0f);
+  KERNEL_CHECK();
+  if (i + 1 < DSK_NUM_CONV) {
+    c->sync_stage = i + 1;
+    *more = 1;
+    return sync_fwd_conv(h, c, i + 1, s);
+  }
+  const int H4 = T / 16, WC = 4 * 512;
+  if (h->bf16) dsk::pool_time_kernel<true><<<dim3(B, WC / 512), 256, 0, s>>>((const uint16_t*)c->y[11], c->pooled, H4, WC, 512, 0);
+  else dsk::pool_time_kernel<false><<<dim3(B, WC / 512), 256, 0, s>>>((const uint16_t*)c->y[11], c->pooled, H4, WC, 512, 0);
+  KERNEL_CHECK();
+  const int fc_smem = (dsk::kFcUtt + dsk::kFcFeat) * dsk::kFcPitch * 4;
+  int rc = ensure_smem_optin(reinterpret_cast<const void*>(dsk::fc_kernel), fc_smem);
+  if (rc) return rc;
+  dim3 g((B + dsk::kFcUtt - 1) / dsk::kFcUtt, h->emb / dsk::kFcFeat, dsk::kFcSplit);
+  dsk::fc_kernel<<<g, 256, fc_smem, s>>>(c->pooled, h->fc_wq, c->fc_part, B, 2048, h->emb);
+  KERNEL_CHECK();
+  dsk::l2norm_kernel<<<B, 512, 0, s>>>(c->fc_part, dsk::kFcSplit, h->fc_b, c->fc_out, c->emb_out, c->inv_norm, B, h->emb, 10.0f);
+  KERNEL_CHECK();
+  c->sync_dir = 0;
+  c->forward_done = true;
+  c->stats_pending = !c->sync_update;
+  *more = 0;
+  return DSK_OK;
+}
+
+// stage 12: the loss scale from the gathered maxima, the fc / pooling backward and layer 11's records.  Stage i: layer i's
+// coefficients from the gathered records, the BatchNorm backward, its weight gradient, then the data gradient and layer
+// i-1's records (i > 0).
+static int sync_bwd_stage(dsk_handle h, dsk_train_ctx_s* c, const float* gathered, int N, cudaStream_t s, int* more) {
+  const bool bf = h->bf16;
+  const int B = c->B, T = c->T, E = h->emb;
+  const dsk_grads* g = &c->grads;
+  int rc;
+  if (c->sync_stage == DSK_NUM_CONV) {
+    dsk::loss_scale_kernel<<<1, 1024, 0, s>>>(gathered, N, h->loss_scale > 0.f ? h->loss_scale : (bf ? 1.0f : 0.0f), c->ls);
+    KERNEL_CHECK();
+    dsk::fc_bwd_weight_kernel<<<dim3(E / 8, 2048 / 256), 256, 0, s>>>(c->g_fc, c->pooled, g->fc_w, g->fc_b, B, 2048, E, 512, 4);
+    KERNEL_CHECK();
+    dsk::fc_bwd_input_kernel<<<dim3(B, 2048 / 256), 256, E * 4, s>>>(c->g_fc, h->fc_wq, c->dP, 2048, E);
+    KERNEL_CHECK();
+    const int H4 = T / 16;
+    if (bf) dsk::pool_bwd_kernel<true><<<B, 256, 0, s>>>(c->dP, (uint16_t*)c->gA, H4, 2048, 1.0f / H4, c->ls);
+    else dsk::pool_bwd_kernel<false><<<B, 256, 0, s>>>(c->dP, (uint16_t*)c->gA, H4, 2048, 1.0f / H4, c->ls);
+    KERNEL_CHECK();
+    c->sync_stage = DSK_NUM_CONV - 1;
+    sync_bwd_records(h, c, c->sync_stage, s);
+    KERNEL_CHECK();
+    *more = 1;
+    return DSK_OK;
+  }
+  const int i = c->sync_stage;
+  int H, W, C;
+  act_shape(i, T, H, W, C);
+  const long M = static_cast<long>(B) * H * W;
+  const uint16_t* gy = (const uint16_t*)(((DSK_NUM_CONV - 1 - i) % 2 == 0) ? c->gA : c->gB);
+  dsk::bn_bwd_record_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(gathered, N, c->rec, B, C, c->mtot + i, h->w.bn_gamma[i],
+                                                                    c->rstd[i], c->ls, g->bn_gamma[i], g->bn_beta[i], c->coef);
+  KERNEL_CHECK();
+  uint16_t* gres = (i % 3 == 2) ? (uint16_t*)c->gres : nullptr;
+  dim3 ga(static_cast<unsigned>((M + 63) / 64), C / 64);
+  if (bf)
+    dsk::bn_bwd_apply_kernel<true><<<ga, 256, 0, s>>>(gy, (const uint16_t*)c->y[i], c->raw[i], c->mean[i], c->rstd[i], c->coef,
+                                                      (uint16_t*)c->G, gres, M, C, 20.0f);
+  else
+    dsk::bn_bwd_apply_kernel<false><<<ga, 256, 0, s>>>(gy, (const uint16_t*)c->y[i], c->raw[i], c->mean[i], c->rstd[i], c->coef,
+                                                       (uint16_t*)c->G, gres, M, C, 20.0f);
+  KERNEL_CHECK();
+  if (i == 0) {
+    const int nblk = B * ((T / 2 + 7) / 8);
+    if (bf) dsk::conv1_wgrad_partial_kernel<true><<<nblk, 256, 0, s>>>((const uint16_t*)c->G, c->x, B, T, c->c1part);
+    else dsk::conv1_wgrad_partial_kernel<false><<<nblk, 256, 0, s>>>((const uint16_t*)c->G, c->x, B, T, c->c1part);
+    KERNEL_CHECK();
+    dsk::sum_partials_kernel<<<(1600 + 31) / 32, 1024, 0, s>>>(c->c1part, nblk, 1600, 1.0f, g->conv_w[0], c->ls);
+    KERNEL_CHECK();
+    c->sync_dir = 0;
+    c->forward_done = false;
+    c->in_use = false;
+    *more = 0;
+    return DSK_OK;
+  }
+  const LayerCfg lc = layer_cfg(i);
+  const int taps = lc.ksize * lc.ksize;
+  const size_t n = static_cast<size_t>(taps) * lc.cout * lc.cin;
+  rc = launch_wgrad(h, c->wgrad[i], s);
+  if (rc) return rc;
+  dsk::unpack_wgrad_kernel<<<static_cast<int>((n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096), 256, 0, s>>>(
+      c->dwacc, g->conv_w[i], lc.cout, lc.cin, taps, 1.0f, c->wgrad[i].p.ksplit, c->wgrad[i].p.slice_elems, c->ls);
+  KERNEL_CHECK();
+  for (int k = 0; k < c->n_dgrad[i]; ++k) {
+    rc = launch_conv(h, c->dgrad[i][k], s);
+    if (rc) return rc;
+  }
+  c->sync_stage = i - 1;
+  sync_bwd_records(h, c, i - 1, s);
+  KERNEL_CHECK();
+  *more = 1;
+  return DSK_OK;
+}
+
+int32_t dsk_sync_forward_begin(dsk_handle h, const float* x, int32_t B, int32_t T, float* emb, dsk_train_ctx* ctx_out,
+                               void* stream) {
+  int rc = check_handle(h);
+  if (rc) return rc;
+  if (!h->weights_loaded) return fail(DSK_ERR_STATE, "dsk_sync_forward_begin: call dsk_load_weights first");
+  if (!x || !emb || !ctx_out || B <= 0) return fail(DSK_ERR_INVALID, "dsk_sync_forward_begin: bad arguments");
+  if (T < 16 || T % 16) return fail(DSK_ERR_INVALID, "dsk_sync_forward_begin: T must be a positive multiple of 16 (got %d)", T);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  dsk_train_ctx_s* c = nullptr;
+  rc = ctx_acquire(h, B, T, s, &c);
+  if (rc) return rc;
+  c->in_use = true;
+  c->forward_done = false;
+  c->stats_pending = false;
+  c->x = x;
+  c->emb_out = emb;
+  c->sync_dir = 1;
+  c->sync_stage = 0;
+  c->sync_fwd = true;
+  c->sync_update = !h->defer_stats;
+  rc = sync_fwd_conv(h, c, 0, s);
+  if (rc) {
+    c->in_use = false;
+    c->sync_dir = 0;
+    return rc;
+  }
+  *ctx_out = c;
+  return DSK_OK;
+}
+
+int32_t dsk_sync_backward_begin(dsk_handle h, dsk_train_ctx c, const float* grad_emb, const dsk_grads* g, void* stream) {
+  int rc = check_handle(h);
+  if (rc) return rc;
+  if (!c || !c->in_use || !c->forward_done || !c->sync_fwd || c->sync_dir)
+    return fail(DSK_ERR_STATE, "dsk_sync_backward_begin: context has no finished synchronised forward");
+  if (!grad_emb || !g) return fail(DSK_ERR_INVALID, "dsk_sync_backward_begin: null argument");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  dsk::l2norm_bwd_kernel<<<c->B, 128, 0, s>>>(c->fc_out, c->inv_norm, grad_emb, c->g_fc, h->emb, 10.0f);
+  KERNEL_CHECK();
+  dsk::row_absmax_kernel<<<c->B, 128, 0, s>>>(c->g_fc, h->emb, c->rec);
+  KERNEL_CHECK();
+  c->grads = *g;
+  c->sync_dir = 2;
+  c->sync_stage = DSK_NUM_CONV;
+  return DSK_OK;
+}
+
+int32_t dsk_sync_records(dsk_handle h, dsk_train_ctx c, void** ptr, int64_t* bytes) {
+  int rc = check_handle(h);
+  if (rc) return rc;
+  if (!ptr || !bytes) return fail(DSK_ERR_INVALID, "dsk_sync_records: null argument");
+  if (!c || !c->in_use || !c->sync_dir) return fail(DSK_ERR_STATE, "dsk_sync_records: no synchronised stage in progress");
+  *ptr = c->rec;
+  *bytes = static_cast<int64_t>(c->B) * sync_rec_words(c) * 4;
+  return DSK_OK;
+}
+
+int32_t dsk_sync_stage(dsk_handle h, dsk_train_ctx c, const void* gathered, int32_t n_total, int32_t* more, void* stream) {
+  int rc = check_handle(h);
+  if (rc) return rc;
+  if (!c || !c->in_use || !c->sync_dir) return fail(DSK_ERR_STATE, "dsk_sync_stage: no synchronised stage in progress");
+  if (!gathered || !more || n_total < c->B)
+    return fail(DSK_ERR_INVALID, "dsk_sync_stage: need the gathered records of n_total >= %d utterances", c->B);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const float* gr = static_cast<const float*>(gathered);
+  return c->sync_dir == 1 ? sync_fwd_stage(h, c, gr, n_total, s, more) : sync_bwd_stage(h, c, gr, n_total, s, more);
+}
+
 
 // ---- per-op entry points for unit tests of the backward building blocks -------------------------------------------
 int32_t dsk_conv2d_dgrad_nhwc(dsk_handle h, const void* G, const float* w_oihw, const void* res, void* gin, int32_t B,
@@ -1949,6 +2195,35 @@ int32_t dsk_bn_act_train_backward(dsk_handle h, const void* gy, const void* y, c
     dsk::bn_bwd_apply_kernel<false><<<ga, 256, 0, s>>>((const uint16_t*)gy, (const uint16_t*)y, raw, mean, rstd, coef, (uint16_t*)G,
                                                        (uint16_t*)gres, M, C, 20.0f);
   }
+  KERNEL_CHECK();
+  CUDA_TRY(cudaFreeAsync(tmp, s));
+  return DSK_OK;
+}
+
+// dsk_bn_act_train_forward with the statistics of the synchronised path: B utterances of HW pixels each (M = B HW rows),
+// one record per utterance, combined by the record finalize as if gathered from any split of the B utterances.
+int32_t dsk_bn_act_sync_train_forward(dsk_handle h, const float* raw, const float* gamma, const float* beta,
+                                      float* running_mean, float* running_var, const void* res, void* y, float* mean,
+                                      float* rstd, int32_t B, int32_t HW, int32_t C, void* stream) {
+  int rc = check_handle(h);
+  if (rc) return rc;
+  if (!raw || !gamma || !beta || !running_mean || !running_var || !y || !mean || !rstd || C % 64 || C > 512 || B <= 0 ||
+      HW <= 0)
+    return fail(DSK_ERR_INVALID, "dsk_bn_act_sync_train_forward: bad arguments");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  float* tmp = nullptr;
+  const size_t rec_words = static_cast<size_t>(B) * (3 * C + 1);
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&tmp), (rec_words + 2 * C) * 4, s));
+  float *rec = tmp, *sc = tmp + rec_words, *sh = sc + C;
+  dsk::bn_utt_record_kernel<<<dim3(B, C / 64), 256, 0, s>>>(raw, HW, C, rec);
+  KERNEL_CHECK();
+  dsk::bn_record_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(rec, B, C, gamma, beta, running_mean, running_var, 0.1f, 1e-5f,
+                                                                mean, rstd, sc, sh, nullptr, nullptr, 1);
+  KERNEL_CHECK();
+  const long M = static_cast<long>(B) * HW;
+  dim3 ga(static_cast<unsigned>((M + 63) / 64), C / 64);
+  if (h->bf16) dsk::bn_apply_kernel<true><<<ga, 256, 0, s>>>(raw, sc, sh, (const uint16_t*)res, (uint16_t*)y, M, C, 20.0f);
+  else dsk::bn_apply_kernel<false><<<ga, 256, 0, s>>>(raw, sc, sh, (const uint16_t*)res, (uint16_t*)y, M, C, 20.0f);
   KERNEL_CHECK();
   CUDA_TRY(cudaFreeAsync(tmp, s));
   return DSK_OK;

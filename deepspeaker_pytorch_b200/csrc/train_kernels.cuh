@@ -592,6 +592,202 @@ __global__ void loss_scale_kernel(const float* __restrict__ g, long n, float fix
   }
 }
 
+// ---- synchronised BatchNorm: per-utterance records ----------------------------------------------------------------
+// Under data parallelism with synchronised BatchNorm every rank normalises with the statistics of the GLOBAL batch.  The
+// ranks exchange one record per utterance instead of per-rank totals: a record is summed in an order fixed by the
+// utterance's own pixel count, and the finalize kernels combine all N records in global utterance order, so the
+// statistics - and everything a rank computes for its own utterances - do not depend on how the batch is split.
+//
+// Forward record of utterance u (fp32 words, 3C + 1): [0, C) the pivots k_c = the utterance's first pixel,
+// [C, 2C) sum (x - k_c), [2C, 3C) sum (x - k_c)^2, [3C] the pixel count HW (int32 bits).  The pixels of u are the rows
+// [u HW, (u + 1) HW) of the NHWC raw conv output.
+// Backward record (2C words): [0, C) sum g_z, [C, 2C) sum g_z xhat, xhat from the global mean / rstd.
+//
+// Record sums: lane p (0..31) of the block walks pixels p, p + 32, ... of the utterance, then the 32 lanes are added by
+// a fixed tree.  grid (B, C/64), block 256; thread = lane p = t/8, 8 channels (t%8)*8 of the 64-channel group.
+__device__ __forceinline__ void utt_tree_sum(float (*red)[32][65], int nstat, int p, int q, float (*v)[8]) {
+#pragma unroll
+  for (int e = 0; e < 8; ++e)
+    for (int st = 0; st < nstat; ++st) red[st][p][q * 8 + e] = v[st][e];
+  __syncthreads();
+  for (int half = 16; half > 0; half >>= 1) {
+    if (p < half) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e)
+        for (int st = 0; st < nstat; ++st) red[st][p][q * 8 + e] += red[st][p + half][q * 8 + e];
+    }
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(256)
+bn_utt_record_kernel(const float* __restrict__ raw, int HW, int C, float* __restrict__ rec) {
+  __shared__ float red[2][32][65];
+  const int q = threadIdx.x & 7, p = threadIdx.x >> 3;
+  const int u = blockIdx.x;
+  const int c0 = blockIdx.y * 64 + q * 8;
+  const float* base = raw + static_cast<long>(u) * HW * C;
+  float k[8], v[2][8];
+  load8f(base + c0, k);
+#pragma unroll
+  for (int e = 0; e < 8; ++e) v[0][e] = v[1][e] = 0.f;
+  for (int m = p; m < HW; m += 32) {
+    float f[8];
+    load8f(base + static_cast<long>(m) * C + c0, f);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const float d = f[e] - k[e];
+      v[0][e] += d;
+      v[1][e] = fmaf(d, d, v[1][e]);
+    }
+  }
+  utt_tree_sum(red, 2, p, q, v);
+  float* r = rec + static_cast<long>(u) * (3 * C + 1);
+  if (p == 0) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      r[c0 + e] = k[e];
+      r[C + c0 + e] = red[0][0][q * 8 + e];
+      r[2 * C + c0 + e] = red[1][0][q * 8 + e];
+    }
+  }
+  if (blockIdx.y == 0 && threadIdx.x == 0) r[3 * C] = __int_as_float(HW);
+}
+
+// The global statistics from the gathered forward records of all N utterances, combined in double in utterance order
+// around K = record 0's pivot (slice sl of 32 adds utterances sl, sl + 32, ..., the slices are added in fixed order):
+// S1 = sum_u sd_u + n_u (k_u - K),  S2 = sum_u ssd_u + 2 (k_u - K) sd_u + n_u (k_u - K)^2,  mean = K + S1/M,
+// var = S2/M - (S1/M)^2.  Then rstd, scale / shift and the running statistics as bn_finalize_kernel; *count_out = M.
+// grid ceil(C/32), block 1024
+__global__ void __launch_bounds__(1024)
+bn_record_finalize_kernel(const float* __restrict__ rec, int N, int C, const float* __restrict__ gamma,
+                          const float* __restrict__ beta, float* __restrict__ running_mean,
+                          float* __restrict__ running_var, float momentum, float eps, float* __restrict__ mean_out,
+                          float* __restrict__ rstd_out, float* __restrict__ scale_out, float* __restrict__ shift_out,
+                          float* __restrict__ unbiased_out, long long* __restrict__ count_out, int update_running) {
+  __shared__ double red[3][32][33];
+  const int lane = threadIdx.x & 31, sl = threadIdx.x >> 5;
+  const int c = blockIdx.x * 32 + lane;
+  const long S = 3L * C + 1;
+  double a1 = 0.0, a2 = 0.0, an = 0.0, K = 0.0;
+  if (c < C) {
+    K = rec[c];
+    for (int u = sl; u < N; u += 32) {
+      const float* r = rec + u * S;
+      const double dk = static_cast<double>(r[c]) - K;
+      const double sd = r[C + c], ssd = r[2 * C + c];
+      const double n = static_cast<double>(__float_as_int(r[3 * C]));
+      a1 += sd + n * dk;
+      a2 += ssd + 2.0 * dk * sd + n * dk * dk;
+      an += n;
+    }
+  }
+  red[0][sl][lane] = a1;
+  red[1][sl][lane] = a2;
+  red[2][sl][lane] = an;
+  __syncthreads();
+  if (sl != 0 || c >= C) return;
+  double s1 = 0.0, s2 = 0.0, M = 0.0;
+  for (int i = 0; i < 32; ++i) {
+    s1 += red[0][i][lane];
+    s2 += red[1][i][lane];
+    M += red[2][i][lane];
+  }
+  const double dmean = s1 / M;
+  const double mean = K + dmean;
+  double var = s2 / M - dmean * dmean;
+  if (var < 0.0) var = 0.0;
+  const float rstd = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
+  const float sc = gamma[c] * rstd;
+  mean_out[c] = static_cast<float>(mean);
+  rstd_out[c] = rstd;
+  scale_out[c] = sc;
+  shift_out[c] = beta[c] - static_cast<float>(mean) * sc;
+  const double unbiased = M > 1.0 ? var * M / (M - 1.0) : var;
+  if (unbiased_out) unbiased_out[c] = static_cast<float>(unbiased);
+  if (update_running) {
+    running_mean[c] = bn_momentum_update(running_mean[c], static_cast<float>(mean), momentum);
+    running_var[c] = bn_momentum_update(running_var[c], static_cast<float>(unbiased), momentum);
+  }
+  if (c == 0 && count_out) *count_out = static_cast<long long>(M);
+}
+
+// Backward record of every utterance: sum g_z, sum g_z xhat (the terms of bn_bwd_reduce_kernel).  grid (B, C/64)
+template <bool BF16>
+__global__ void __launch_bounds__(256)
+bn_bwd_utt_record_kernel(const uint16_t* __restrict__ gy, const uint16_t* __restrict__ y, const float* __restrict__ raw,
+                         const float* __restrict__ mean, const float* __restrict__ rstd, int HW, int C, float clip_hi,
+                         float* __restrict__ rec) {
+  __shared__ float red[2][32][65];
+  const int q = threadIdx.x & 7, p = threadIdx.x >> 3;
+  const int u = blockIdx.x;
+  const int c0 = blockIdx.y * 64 + q * 8;
+  const long off = static_cast<long>(u) * HW * C + c0;
+  float mu[8], rs[8], v[2][8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) {
+    mu[e] = mean[c0 + e];
+    rs[e] = rstd[c0 + e];
+    v[0][e] = v[1][e] = 0.f;
+  }
+  for (int m = p; m < HW; m += 32) {
+    const long i = off + static_cast<long>(m) * C;
+    float g[8], yy[8], r[8];
+    unpack8<BF16>(*reinterpret_cast<const uint4*>(gy + i), g);
+    unpack8<BF16>(*reinterpret_cast<const uint4*>(y + i), yy);
+    load8f(raw + i, r);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const float gz = (yy[e] > 0.f && yy[e] < clip_hi) ? g[e] : 0.f;
+      v[0][e] += gz;
+      v[1][e] = fmaf(gz, (r[e] - mu[e]) * rs[e], v[1][e]);
+    }
+  }
+  utt_tree_sum(red, 2, p, q, v);
+  if (p == 0) {
+    float* r = rec + static_cast<long>(u) * 2 * C;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      r[c0 + e] = red[0][0][q * 8 + e];
+      r[C + c0 + e] = red[1][0][q * 8 + e];
+    }
+  }
+}
+
+// Backward finalize from the records: the coefficients of bn_bwd_apply_kernel from the GLOBAL sums over the N gathered
+// records (b = sum g_z / M, d = sum g_z xhat / M with M the forward's global pixel count), dgamma / dbeta from this rank's
+// own n records (the data-parallel gradient reduction adds the ranks' shares), divided by the loss scale dyn[1].
+// grid ceil(C/32), block 1024
+__global__ void __launch_bounds__(1024)
+bn_bwd_record_finalize_kernel(const float* __restrict__ gathered, int N, const float* __restrict__ local, int n, int C,
+                              const long long* __restrict__ count, const float* __restrict__ gamma,
+                              const float* __restrict__ rstd, const float* __restrict__ dyn, float* __restrict__ dgamma,
+                              float* __restrict__ dbeta, float* __restrict__ coef /*[3][C]*/) {
+  const int c = blockIdx.x * 32 + (threadIdx.x & 31);
+  double gs, gss, ls, lss;
+  const bool ok = bn_partial_totals(gathered, N, C, c, gs, gss);
+  if (!bn_partial_totals(local, n, C, c, ls, lss) || !ok) return;
+  const double M = static_cast<double>(*count);
+  dbeta[c] = static_cast<float>(ls) * dyn[1];
+  dgamma[c] = static_cast<float>(lss) * dyn[1];
+  coef[c] = gamma[c] * rstd[c];
+  coef[C + c] = static_cast<float>(gs / M);
+  coef[2 * C + c] = static_cast<float>(gss / M);
+}
+
+// max |g| of every row of a (B, E) matrix: the loss-scale record of one utterance (loss_scale_kernel over the gathered
+// maxima picks the S of the single-device backward over the union).  grid B, block 128
+__global__ void __launch_bounds__(128) row_absmax_kernel(const float* __restrict__ g, int E, float* __restrict__ out) {
+  __shared__ float red[4];
+  const float* r = g + static_cast<long>(blockIdx.x) * E;
+  float m = 0.f;
+  for (int i = threadIdx.x; i < E; i += blockDim.x) m = fmaxf(m, fabsf(r[i]));
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) out[blockIdx.x] = fmaxf(fmaxf(red[0], red[1]), fmaxf(red[2], red[3]));
+}
+
 // ---- weight repack of a training step: ONE launch for all eleven tensor-core convs -----------------------------------
 // A training step changes every parameter, so the 16-bit operand images are rebuilt once per step, on the caller's
 // stream, before the three forwards fork, in one launch rather than 44 small ones with strided 4-byte gathers.  Here a block owns a 16 (cout) x 32 (cin) x taps tile of one layer: it reads the

@@ -99,6 +99,30 @@ class DeepSpeakerModel(nn.Module):
         self.model.fc = nn.Linear(512 * 4, self.embedding_size)          # model.py:163-164
         self.model.classifier = nn.Linear(self.embedding_size, num_classes)  # :167
         self._engine = None
+        self._sync_bn = None          # (process group,) while BatchNorm statistics are synchronised
+
+    def sync_batchnorm(self, process_group=None):
+        """Synchronise the train-mode BatchNorm statistics over the ranks of ``process_group`` (the default group
+        when None and torch.distributed is initialised), as ``nn.SyncBatchNorm.convert_sync_batchnorm`` does for torch
+        modules; ``sync_batchnorm(False)`` returns to per-replica statistics (the default).  Returns the model.
+
+        Once on, every train-mode ``model(x)`` / ``forward_triplet`` normalises each layer with the statistics of the
+        global batch, combined from per-utterance records in global utterance order: the embeddings, the batch
+        statistics and the running statistics a rank computes for its own utterances are bit-identical for every split
+        of the batch over ranks, one rank (or no process group) included - that path is the same staged one.  The
+        forward exchanges records at each of the 12 BatchNorm layers and the backward at 13 points, so ``backward()``
+        issues collectives and every rank must run the same forwards and backwards in the same order, each with the
+        same batch size.  Eval mode is unchanged (it uses the running statistics)."""
+        if process_group is False:
+            self._sync_bn = None
+        else:
+            if process_group is None:
+                import torch.distributed as dist
+
+                if dist.is_available() and dist.is_initialized():
+                    process_group = dist.group.WORLD
+            self._sync_bn = (process_group,)
+        return self
 
     # -- engine plumbing -------------------------------------------------------------------------
     def _get_engine(self, device):
@@ -151,8 +175,12 @@ class DeepSpeakerModel(nn.Module):
             from . import train as _train
 
             eng = self._get_engine(anchor.device)
+            on, group = _train.sync_bn_setting(self)
             with torch.cuda.device(anchor.device):
-                outs = _train.forward_train_many(eng, list(xs))
+                if on:    # the three forwards in lockstep: one collective per stage carries all three record sets
+                    outs = _train.forward_train_sync(eng, list(xs), group)
+                else:
+                    outs = _train.forward_train_many(eng, list(xs))
         self.features = outs[-1]
         return tuple(outs)
 

@@ -3,13 +3,17 @@
 The reference is single-device (reference train_triplet.py:97); SURVEY §8e adds exactly one
 strategy: every rank runs the triplet step on its own shard of the batch, and the gradients of the 38
 differentiated parameters are averaged with a single ``all_reduce`` over one flat fp32 bucket
-(11 624 128 elements, 46.5 MB).  BatchNorm statistics stay per replica, as in the reference (no SyncBN).
+(11 624 128 elements, 46.5 MB).  By default BatchNorm statistics stay per replica, as in the reference;
+``DeepSpeakerModel.sync_batchnorm(process_group)`` synchronises them over the ranks instead (``gather_records``).
 
 ``torch.distributed`` (NCCL over NVLink on the GPU box, gloo in the CPU tests) is plumbing here.
 
 Batch-hard mining over the global batch (``GlobalBatchHardTripletLoss``, ``batch_hard_step(..., across_ranks=True)``)
 adds three small all_gathers per step: the labels, the fp32 embeddings and the selection records.  The gradient
 reduction stays the one all-reduce.
+
+Synchronised BatchNorm adds one all_gather of per-utterance records at each of the 12 BatchNorm layers of a forward
+and at 13 points of its backward (the loss scale, then the 12 layers); see ``gather_records`` for the record sizes.
 """
 from __future__ import annotations
 
@@ -197,3 +201,25 @@ class GlobalBatchHardTripletLoss:
         return _GlobalBatchHardFn.apply(local_emb, global_labels, float(self.margin), self.exact_cuda_cores, self.group)
 
     __call__ = forward
+
+
+# ---- synchronised BatchNorm --------------------------------------------------------------------------------------------
+# Per utterance and stage: a forward record is 4 (3C + 1) bytes (pivot, sum and sum of squares per channel, the pixel
+# count), 34.6 kB over the 12 layers (2880 channels); a backward record is 8C bytes (23 kB over the layers) and the
+# loss-scale record 4 bytes.  Every rank must hold the same number of utterances.
+
+def gather_records(local, process_group=None):
+    """The exchange of one synchronised-BatchNorm stage: ``local`` is a list of this rank's record tensors (uint8, one
+    per forward in lockstep); returns, for each, the records of all ranks concatenated in rank order.  All sets travel in
+    ONE all_gather_into_tensor.  Without a process group (or at world size 1) the local records are the global ones."""
+    if not _distributed(process_group):
+        return list(local)
+    world = dist.get_world_size(process_group)
+    flat = torch.cat([t.reshape(-1) for t in local])      # a copy: the library's buffer is reused by the next stage
+    out = flat.new_empty(world * flat.numel())
+    dist.all_gather_into_tensor(out, flat, group=process_group)
+    rows, parts, off = out.view(world, -1), [], 0
+    for t in local:
+        parts.append(rows[:, off:off + t.numel()].reshape(-1))
+        off += t.numel()
+    return parts

@@ -18,7 +18,8 @@ a different function of the parameters than anything the first forward computed.
 
 Data parallelism (SURVEY §8e): pass ``bucket`` (``parallel.GradBucket``) or a ``FusedAdagrad`` optimizer; branch A
 averages gradients over ranks, branch B weights each rank's mean gradient by its own k (``k_r / sum k``) through the
-same single allreduce.
+same single allreduce.  With synchronised BatchNorm (``DeepSpeakerModel.sync_batchnorm``) branch A runs unchanged and
+branch B raises ``ValueError`` before any collective.
 """
 from __future__ import annotations
 
@@ -26,6 +27,7 @@ import torch
 import torch.distributed as dist
 
 from . import engine as _engine
+from . import train as _train
 from .head import CrossEntropyLoss
 from .model import (BatchHardTripletLoss, PairwiseDistance, TripletMarginLoss, batch_hard_valid_count,
                     select_hard_triplets)
@@ -60,6 +62,11 @@ def train_step(model, optimizer, data_a, data_p, data_n, label_p, label_n, *, ma
     (:238-245, :251-252); ``None`` when branch B selects nothing (the reference's ``continue``)."""
     if not model.training:
         raise RuntimeError("train_step needs model.train() (train_triplet.py:203)")
+    if epoch <= min_softmax_epoch and _train.sync_bn_setting(model)[0]:
+        # branch B re-forwards the k_r selected utterances, and k_r differs per rank: the synchronised stages would
+        # gather unequal record sets.  Every rank decides this from the same epoch, before any collective.
+        raise ValueError("train_step: the hard-triplet branch (epoch <= min_softmax_epoch) is not supported with "
+                         "synchronised BatchNorm; call model.sync_batchnorm(False) for it")
     out_a, out_p, out_n = model.forward_triplet(data_a, data_p, data_n)                 # :215
     crit = TripletMarginLoss(margin)
     if epoch > min_softmax_epoch:
@@ -127,8 +134,10 @@ def batch_hard_step(model, optimizer, data, labels, *, margin, bucket=None, acro
     global V - the step's one host synchronisation; every rank then sees the same V, so on V = 0 all ranks raise before
     any other collective.  The backward is seeded with R: the unchanged mean all-reduce of the gradients (/R) then sums
     the ranks' gradients, which is the gradient of the global loss (exactly so for power-of-two R).  The ranks are
-    those of the optimizer's (``FusedAdagrad``) or the bucket's process group.  BatchNorm statistics stay per replica.
-    ``valid`` is the global V.  Without a process group this is the step with ``across_ranks=False``."""
+    those of the optimizer's (``FusedAdagrad``) or the bucket's process group.  BatchNorm statistics stay per replica
+    by default; on a model with ``sync_batchnorm(group)`` they are those of the global batch too, and the step's forward
+    and loss are then those of the single-device step on the gathered batch.  ``valid`` is the global V.  Without a
+    process group this is the step with ``across_ranks=False``."""
     if not model.training:
         raise RuntimeError("batch_hard_step needs model.train()")
     if across_ranks:

@@ -90,6 +90,9 @@ def _forward_one(engine, x, params, need_grad):
 
 def forward_train(engine, x):
     module = engine.module_ref
+    on, group = sync_bn_setting(module)
+    if on:
+        return forward_train_sync(engine, [x], group)[0]
     engine.sync_weights(eval_mode=False)
     engine.train_calls += 1  # running statistics are about to change: invalidates the eval-mode BN fold
     params = _train_params(module)
@@ -215,6 +218,187 @@ def forward_train_many(engine, xs):
     else:
         outs, ctxs = _launch_many(engine, xs)
     for tctx in ctxs:                                # momentum updates in call order, on the caller's stream
+        L.check(engine.lib.dsk_train_ctx_commit_stats(engine.handle, tctx, L.cur_stream()), "dsk_train_ctx_commit_stats")
+        if not need_grad:
+            L.check(engine.lib.dsk_train_ctx_release(engine.handle, tctx), "dsk_train_ctx_release")
+    torch._foreach_add_([bn.num_batches_tracked for _, bn in conv_bn_modules(module)], len(xs))
+    return outs
+
+
+# ---- synchronised BatchNorm ------------------------------------------------------------------------------------------
+# DeepSpeakerModel.sync_batchnorm(group): every train-mode BatchNorm layer normalises with the statistics of the GLOBAL
+# batch of all ranks.  The library runs the forward and the backward as resumable stages (include/dsk.h, dsk_sync_*);
+# at each of the 12 forward and 13 backward exchange points a stage generator below yields this rank's per-utterance
+# records (a uint8 device tensor) and receives the records of every rank's utterances, concatenated in rank order.
+# ``run_lockstep`` drives several generators through one exchange per stage; ``parallel.gather_records`` is the exchange
+# of a process group (one all_gather_into_tensor).
+
+def sync_bn_setting(module):
+    """(on, process group) of ``DeepSpeakerModel.sync_batchnorm``."""
+    s = getattr(module, "_sync_bn", None)
+    return (False, None) if s is None else (True, s[0])
+
+
+class _DeviceBytes:
+    """A library-owned device buffer as a zero-copy uint8 tensor (``torch.as_tensor`` reads this interface)."""
+
+    def __init__(self, ptr, nbytes):
+        self.__cuda_array_interface__ = {"shape": (nbytes,), "typestr": "|u1", "data": (ptr, False), "strides": None,
+                                         "version": 2}
+
+
+def _stage_loop(engine, tctx, B):
+    more = ctypes.c_int32(1)
+    while more.value:
+        p, nb = ctypes.c_void_p(), ctypes.c_int64()
+        L.check(engine.lib.dsk_sync_records(engine.handle, tctx, ctypes.byref(p), ctypes.byref(nb)), "dsk_sync_records")
+        local = torch.as_tensor(_DeviceBytes(p.value, nb.value), device=engine.device)
+        gathered = yield local
+        if gathered.dtype != torch.uint8 or gathered.numel() % (nb.value // B):
+            raise ValueError("gathered records must be the uint8 records of whole utterances")
+        n_total = gathered.numel() // (nb.value // B)
+        L.check(engine.lib.dsk_sync_stage(engine.handle, tctx, gathered.data_ptr(), n_total, ctypes.byref(more),
+                                          L.cur_stream()), "dsk_sync_stage")
+
+
+def sync_forward_stages(engine, x, emb):
+    """Generator of one synchronised train-mode forward of ``x`` (B, 1, T, 64) into ``emb`` (B, E) on the current
+    stream: yields this rank's records 12 times, each time receiving the gathered records (uint8, rank order); returns
+    the library context (StopIteration.value), which the backward stages consume."""
+    B, _, T, _ = x.shape
+    tctx = ctypes.c_void_p()
+    L.check(engine.lib.dsk_sync_forward_begin(engine.handle, x.data_ptr(), B, T, emb.data_ptr(), ctypes.byref(tctx),
+                                              L.cur_stream()), "dsk_sync_forward_begin")
+    done = False
+    try:
+        yield from _stage_loop(engine, tctx, B)
+        done = True
+    finally:
+        if not done:
+            engine.lib.dsk_train_ctx_release(engine.handle, tctx)
+    return tctx
+
+
+def _grads_struct(views):
+    g = L.DskGrads()
+    for i in range(L.NUM_CONV):
+        g.conv_w[i] = views[3 * i].data_ptr()
+        g.bn_gamma[i] = views[3 * i + 1].data_ptr()
+        g.bn_beta[i] = views[3 * i + 2].data_ptr()
+    g.fc_w = views[-2].data_ptr()
+    g.fc_b = views[-1].data_ptr()
+    return g
+
+
+def sync_backward_stages(engine, tctx, B, grad_emb, views):
+    """Generator of the backward of a synchronised forward: 13 exchanges (the loss scale, then BatchNorm layers 11..0).
+    The 38 parameter gradients are written into ``views``: dgamma / dbeta and the weight gradients are this rank's
+    share, which the data-parallel gradient reduction adds up."""
+    g = _grads_struct(views)
+    L.check(engine.lib.dsk_sync_backward_begin(engine.handle, tctx, grad_emb.data_ptr(), ctypes.byref(g), L.cur_stream()),
+            "dsk_sync_backward_begin")
+    yield from _stage_loop(engine, tctx, B)
+
+
+def run_lockstep(gens, exchange):
+    """Drives stage generators that exchange at the same points: ``exchange(list of local records)`` returns one
+    gathered record tensor per generator.  One exchange per stage for all of them.  Returns the generators' results."""
+    local = [next(g) for g in gens]
+    while True:
+        gathered = exchange(local)
+        nxt, results = [], []
+        for g, rec in zip(gens, gathered):
+            try:
+                nxt.append(g.send(rec))
+            except StopIteration as stop:
+                results.append(stop.value)
+        if len(results) == len(gens):
+            return results
+        if results:
+            raise RuntimeError("synchronised stage generators fell out of step")
+        local = nxt
+
+
+def _sync_forward(engine, xs, group):
+    """The synchronised forwards of ``xs`` in lockstep on the current stream: one exchange per stage for all of them.
+    With several forwards the running-statistics updates are deferred (committed afterwards in call order)."""
+    from .parallel import gather_records
+
+    embs = [torch.empty(x.shape[0], engine.module_ref.embedding_size, device=x.device, dtype=torch.float32) for x in xs]
+    gens = [sync_forward_stages(engine, x, e) for x, e in zip(xs, embs)]
+    defer = len(xs) > 1
+    if defer:
+        L.check(engine.lib.dsk_set_defer_running_stats(engine.handle, 1), "dsk_set_defer_running_stats")
+    try:
+        ctxs = run_lockstep(gens, lambda local: gather_records(local, group))
+    finally:
+        if defer:
+            L.check(engine.lib.dsk_set_defer_running_stats(engine.handle, 0), "dsk_set_defer_running_stats")
+    return embs, ctxs
+
+
+class SyncTrainForwardFn(torch.autograd.Function):
+    """K synchronised train-mode forwards of one step (K = 1 for ``model(x)``, 3 for ``forward_triplet``) as ONE
+    autograd node.  Forward and backward drive the K stage generators in lockstep, so a stage's K record sets travel in
+    one collective; the backward's collectives therefore run inside ``loss.backward()``, and every rank must run the
+    same backward.  The K gradients are summed as ``TripletForwardFn`` sums them (last call first), into an optimizer /
+    data-parallel bucket directly when the parameters' gradients are views of one."""
+
+    @staticmethod
+    def forward(ctx, engine, group, k, *args):
+        xs, params = args[:k], args[k:]
+        outs, tctxs = _sync_forward(engine, xs, group)
+        ctx.engine, ctx.group, ctx.k, ctx.params = engine, group, k, params
+        ctx.guards = [_CtxGuard(engine, t) for t in tctxs]
+        ctx.out_shapes = [o.shape for o in outs]
+        ctx.save_for_backward(*xs, *params)  # the inputs must outlive the backward (conv1's weight gradient reads them)
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, *grad_embs):
+        from .parallel import gather_records
+
+        engine, k, params = ctx.engine, ctx.k, ctx.params
+        _ = ctx.saved_tensors
+        dev = engine.device
+        with torch.cuda.device(dev):
+            flats, views, ges, gens = [], None, [], []
+            for ge, shape, guard in zip(grad_embs, ctx.out_shapes, ctx.guards):
+                ge = torch.zeros(shape, device=dev, dtype=torch.float32) if ge is None else ge.float().contiguous()
+                flat, views = engine.grad_scratch(params, with_flat=True)
+                gens.append(sync_backward_stages(engine, guard.tctx, shape[0], ge, views))
+                ges.append(ge)
+                flats.append(flat)
+            run_lockstep(gens, lambda local: gather_records(local, ctx.group))
+            for guard in ctx.guards:
+                guard.consume()
+            acc = flats[-1]                        # `views` are the views of this buffer
+            for f in reversed(flats[:-1]):
+                acc.add_(f)
+            if (all(p.grad is not None and p.grad is getattr(p, "_dsk_bucket_grad", None) for p in params)
+                    and _engine_accumulates_into(ctx, params)):
+                torch._foreach_add_([p.grad for p in params], list(views))
+                engine.bucket_accumulations += 1
+                return (None, None, None) + (None,) * k + (None,) * len(params)
+        return (None, None, None) + (None,) * k + tuple(views)
+
+
+def forward_train_sync(engine, xs, group):
+    """Train-mode forwards of ``xs`` with BatchNorm statistics synchronised over ``group`` (None: this process alone -
+    the same staged path, so results never depend on the number of ranks).  Running statistics are updated in call
+    order; every rank must call this with the same number of forwards of the same batch size."""
+    module = engine.module_ref
+    engine.sync_weights(eval_mode=False)
+    engine.train_calls += 1
+    params = _train_params(module)
+    need_grad = torch.is_grad_enabled() and any(p.requires_grad for p in params)
+    xs = [x.contiguous().float() for x in xs]
+    if need_grad:
+        outs = list(SyncTrainForwardFn.apply(engine, group, len(xs), *xs, *params))
+        ctxs = [g.tctx for g in outs[0].grad_fn.guards]
+    else:
+        outs, ctxs = _sync_forward(engine, xs, group)
+    for tctx in ctxs:                                # deferred momentum updates in call order
         L.check(engine.lib.dsk_train_ctx_commit_stats(engine.handle, tctx, L.cur_stream()), "dsk_train_ctx_commit_stats")
         if not need_grad:
             L.check(engine.lib.dsk_train_ctx_release(engine.handle, tctx), "dsk_train_ctx_release")

@@ -141,6 +141,37 @@ int32_t dsk_train_ctx_release(dsk_handle h, dsk_train_ctx ctx);
  * training; scale > 0: that fixed value.  bf16 operands: 1 unless set. */
 int32_t dsk_set_loss_scale(dsk_handle h, float scale);
 
+/* Synchronised BatchNorm under data parallelism: the train forward and backward as resumable stages, so that the caller
+ * can exchange per-utterance records between ranks at every BatchNorm layer (the library issues no collective).  Every
+ * layer normalises with the statistics of the GLOBAL batch, combined in global utterance order: what a rank computes for
+ * its own utterances is bit-identical for every way of splitting the batch over ranks, one rank included.
+ *
+ *   dsk_sync_forward_begin   conv1 and layer 0's records; *ctx is a pooled train context
+ *   dsk_sync_backward_begin  (after the forward's last stage) the l2-norm backward and the loss-scale records
+ *   dsk_sync_records         device pointer and byte size of this stage's records of the B local utterances
+ *   dsk_sync_stage           consumes the records of all n_total utterances, gathered in rank order, and runs up to the
+ *                            next exchange; *more = 0 after the forward's tail (emb written) / layer 0's weight gradient
+ *
+ * The forward has 12 exchanges (one per BatchNorm layer), the backward 13 (the loss scale, then layers 11..0).  Records,
+ * fp32 words per utterance (u in rank order, C the layer's channels):
+ *   forward, layer i:  3C + 1: [0,C) pivot k_c = the utterance's first pixel of channel c, [C,2C) sum (x - k_c),
+ *                      [2C,3C) sum (x - k_c)^2 over its H*W pixels (fp32, in an order fixed by H*W), [3C] H*W (int32)
+ *   backward, first:   1: max |dL/d(fc output)| of the utterance; every rank then uses the loss scale of the union
+ *   backward, layer i: 2C: [0,C) sum g_z, [C,2C) sum g_z * xhat (xhat from the global mean / rstd)
+ * The statistics combine the records in double around record 0's pivot; dgamma / dbeta are this rank's own sums (the
+ * data-parallel gradient reduction adds the ranks'), the BatchNorm input gradient uses the global sums.  Every rank
+ * must run the same stages in the same order.  The context works with dsk_train_ctx_read, dsk_train_ctx_commit_stats
+ * (dsk_set_defer_running_stats applies at dsk_sync_forward_begin) and dsk_train_ctx_release; dsk_rescnn_backward
+ * refuses it.  Calls out of sequence return DSK_ERR_STATE, n_total < B DSK_ERR_INVALID.  x, emb and the gathered
+ * buffer must stay alive until the stage's work on `stream` has run. */
+int32_t dsk_sync_forward_begin(dsk_handle h, const float* x, int32_t B, int32_t T, float* emb, dsk_train_ctx* ctx,
+                               void* stream);
+int32_t dsk_sync_backward_begin(dsk_handle h, dsk_train_ctx ctx, const float* grad_emb, const dsk_grads* grads,
+                                void* stream);
+int32_t dsk_sync_records(dsk_handle h, dsk_train_ctx ctx, void** ptr, int64_t* bytes);
+int32_t dsk_sync_stage(dsk_handle h, dsk_train_ctx ctx, const void* gathered, int32_t n_total, int32_t* more,
+                       void* stream);
+
 /* Device timing of the next dsk_rescnn_forward calls (which then launch kernel by kernel, not as a graph).
  * enable = 1: CUDA events are recorded on `stream` around every kernel of the forward (order: conv1, the 11
  * tensor-core convs in network order, pool, fc, l2norm); enable = 2: only at the section boundaries
@@ -170,6 +201,11 @@ int32_t dsk_conv2d_wgrad_nhwc(dsk_handle h, const void* G, const void* X, float*
 int32_t dsk_bn_act_train_forward(dsk_handle h, const float* raw, const float* gamma, const float* beta,
                                  float* running_mean, float* running_var, const void* res, void* y, float* mean,
                                  float* rstd, int64_t M, int32_t C, void* stream);
+/* The same with the statistics of the synchronised path: raw holds B utterances of HW pixels each (rows
+ * [u*HW, (u+1)*HW) are utterance u); one record per utterance, combined as dsk_sync_stage combines gathered records. */
+int32_t dsk_bn_act_sync_train_forward(dsk_handle h, const float* raw, const float* gamma, const float* beta,
+                                      float* running_mean, float* running_var, const void* res, void* y, float* mean,
+                                      float* rstd, int32_t B, int32_t HW, int32_t C, void* stream);
 /* its backward: gy -> G (w.r.t. raw), gres (w.r.t. res, may be NULL), dgamma, dbeta (x inv_scale). */
 int32_t dsk_bn_act_train_backward(dsk_handle h, const void* gy, const void* y, const float* raw, const float* gamma,
                                   const float* mean, const float* rstd, void* G, void* gres, float* dgamma,
