@@ -168,6 +168,8 @@ SIGNATURES = {
     "dsk_batch_hard_select_rows": (c_int32, [c_void_p] * 3 + [c_int32] * 4 + [c_void_p] * 6),
     "dsk_batch_hard_mean": (c_int32, [c_void_p] * 3 + [c_int32, c_float, c_void_p, c_void_p]),
     "dsk_batch_hard_triplet_bwd_rows": (c_int32, [c_void_p] * 6 + [c_int32] * 4 + [c_float] + [c_void_p] * 3),
+    "dsk_aam_softmax": (c_int32, [c_void_p] * 4 + [c_int32] * 3 + [c_float, c_float] + [c_void_p] * 4),
+    "dsk_aam_softmax_bwd": (c_int32, [c_void_p] * 6 + [c_int32] * 3 + [c_float, c_float] + [c_void_p] * 4),
     "dsk_linear_forward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     "dsk_linear_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p,
                                       c_void_p, c_void_p]),

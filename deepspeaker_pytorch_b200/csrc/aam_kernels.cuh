@@ -1,0 +1,302 @@
+// Additive angular margin softmax (ArcFace / AAM-softmax) over a cosine classifier: the element-wise and row kernels
+// around the tensor-core cosine GEMMs (dsk_aam_softmax / dsk_aam_softmax_bwd in dsk_api.cu).
+//
+// The three GEMMs (cos = E^ W^T, gE^ = dcos W^, gW^ = dcos^T E^) run on conv_umma_kernel as plain GEMMs with fp16
+// operands split into hi/lo halves (x = hi + lo, 22 significant bits) and concatenated along K, so that one fp32
+// accumulator sums lo*hi + hi*lo + hi*hi.  The "A" side of a GEMM is laid out [lo | hi | hi], the "B" side
+// [hi | lo | hi]: the two small lo-products come first in K (they are summed while the accumulator is still small).
+// The tensor cores add each 16-wide K step to the fp32 accumulator with truncation, so the error grows with the number
+// of steps times the accumulator's size.  The backward GEMMs (K = 3 Cp and 3 Np) therefore run in K slices of
+// kAamSlice classes / utterances, each slice a GEMM of its own into its own fp32 output, summed in slice order by the
+// Jacobian kernel (deterministic split K); and the target column's cosine, where an embedding sits close to its class
+// centre, is recomputed in fp64 from the fp32 inputs.
+#pragma once
+#include <cuda_fp16.h>
+#include <stdint.h>
+
+#include "head_kernels.cuh"
+
+namespace dsk {
+
+constexpr int kAamSlice = 512;  // classes (gE^) or utterances (gW^) per K slice of a backward GEMM
+
+// Element (row, seg, k) of a K-sliced backward operand image over Kp columns: slice s = k / kAamSlice holds columns
+// [s kAamSlice, s kAamSlice + w) as a [rows][3w] image (segments seg = 0, 1, 2 of width w), slices one after another
+// kAamSlice * 3 * rows elements apart.
+__device__ __forceinline__ size_t aam_kslice_off(int row, int rows, int seg, int k, int Kp) {
+  const int sl = k / kAamSlice, kk = k - sl * kAamSlice;
+  const int w = Kp - sl * kAamSlice < kAamSlice ? Kp - sl * kAamSlice : kAamSlice;
+  return static_cast<size_t>(sl) * kAamSlice * 3 * rows + static_cast<size_t>(row) * 3 * w + seg * w + kk;
+}
+
+struct AamMargin {
+  float cos_m, sin_m;  // cos m, sin m
+  float th, mm;        // cos(pi - m), sin(pi - m) * m: below th the target logit is cos - mm (non-"easy" margin)
+  float s;             // scale
+};
+
+// phi(cos) of the target column
+__device__ __forceinline__ float aam_phi(float c, const AamMargin& a) {
+  const float sn = sqrtf(fminf(fmaxf(1.f - c * c, 0.f), 1.f));
+  return c > a.th ? c * a.cos_m - sn * a.sin_m : c - a.mm;
+}
+// d phi / d cos; at sin = 0 (a row on its class centre) the finite limit cos m
+__device__ __forceinline__ float aam_dphi(float c, const AamMargin& a) {
+  if (!(c > a.th)) return 1.f;
+  const float sn = sqrtf(fminf(fmaxf(1.f - c * c, 0.f), 1.f));
+  return sn > 0.f ? a.cos_m + a.sin_m * c / sn : a.cos_m;
+}
+
+__device__ __forceinline__ void aam_split16(float x, uint16_t& hi, uint16_t& lo) {
+  const __half h = __float2half_rn(x);
+  hi = __half_as_ushort(h);
+  lo = __half_as_ushort(__float2half_rn(x - __half2float(h)));  // x - hi is exact in fp32
+}
+
+// Exponent e of the power of two 2^e that puts max|v| of a row (column) of dcos at [256, 512): the hi/lo halves of the
+// scaled values stay in fp16's normal range.  0 for an all-zero or non-finite row.
+__device__ __forceinline__ int aam_scale_exp(float m) {
+  if (!(m > 0.f) || !isfinite(m)) return 0;
+  const int e = static_cast<int>(floorf(log2f(512.f / m)));
+  return e < -24 ? -24 : (e > 100 ? 100 : e);
+}
+// 2^e for |e| <= 100, exactly
+__device__ __forceinline__ float aam_pow2(int e) { return __int_as_float((127 + e) << 23); }
+
+// nrm[r] = max(||X[r]||, 1e-12) (F.normalize's denominator); one warp per row, fixed order.  grid ceil(rows / 8), block 256.
+__global__ void __launch_bounds__(256) aam_norm_kernel(const float* __restrict__ X, int rows, int D, float* __restrict__ nrm) {
+  const int r = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (r >= rows) return;
+  const float* x = X + static_cast<size_t>(r) * D;
+  float s = 0.f;
+  for (int d = lane; d < D; d += 32) s = fmaf(x[d], x[d], s);
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) nrm[r] = fmaxf(sqrtf(s), 1e-12f);
+}
+
+// x^ = X[r] / nrm[r] split into fp16 hi/lo operand images; rows in [rows, rows_pad) are zero.
+//   img  (may be NULL): [rows_pad][3D], [lo | hi | hi] (lo_first, the A side) or [hi | lo | hi] (B side)
+//   imgT (may be NULL): [D][3 rows_pad] K-sliced (aam_kslice_off), [hi | lo | hi]: the transposed B-side image of the
+//                       backward GEMMs
+// grid (D / 64, rows_pad / 32), block 256.
+__global__ void __launch_bounds__(256)
+aam_split_kernel(const float* __restrict__ X, const float* __restrict__ nrm, int rows, int rows_pad, int D, int lo_first,
+                 uint16_t* __restrict__ img, uint16_t* __restrict__ imgT) {
+  __shared__ float t[32][65];
+  const int r0 = blockIdx.y * 32, d0 = blockIdx.x * 64;
+  const int tx = threadIdx.x & 63;
+  for (int rr = threadIdx.x >> 6; rr < 32; rr += 4) {
+    const int r = r0 + rr;
+    const float v = r < rows ? X[static_cast<size_t>(r) * D + d0 + tx] / nrm[r] : 0.f;
+    t[rr][tx] = v;
+    if (img) {
+      uint16_t hi, lo;
+      aam_split16(v, hi, lo);
+      uint16_t* o = img + static_cast<size_t>(r) * 3 * D + d0 + tx;
+      o[0] = lo_first ? lo : hi;
+      o[D] = lo_first ? hi : lo;
+      o[2 * D] = hi;
+    }
+  }
+  if (!imgT) return;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  for (int k = threadIdx.x >> 5; k < 64; k += 8) {
+    uint16_t hi, lo;
+    aam_split16(t[lane][k], hi, lo);
+    imgT[aam_kslice_off(d0 + k, D, 0, r0 + lane, rows_pad)] = hi;
+    imgT[aam_kslice_off(d0 + k, D, 1, r0 + lane, rows_pad)] = lo;
+    imgT[aam_kslice_off(d0 + k, D, 2, r0 + lane, rows_pad)] = hi;
+  }
+}
+
+// Forward rows: cos_out[i] = G[i][0, C) (the GEMM's padded output) except the target column, which is recomputed in
+// fp64 from E[i] and W[y] (a row near its class centre has cos ~ 1 there, where the GEMM's accumulation error is
+// largest); logits s*cos with s*phi on the target column, lse[i] = logsumexp over all C in a fixed order,
+// row_loss[i] = lse[i] - s*phi (NaN for a label outside [0, C)).  grid N, block 256.
+__global__ void __launch_bounds__(256)
+aam_rows_kernel(const float* __restrict__ G, int ldg, const float* __restrict__ E, const float* __restrict__ W, int D,
+                const int64_t* __restrict__ labels, int C, AamMargin a, float* __restrict__ cos_out,
+                float* __restrict__ lse, float* __restrict__ row_loss) {
+  __shared__ float red[8];
+  __shared__ double red3[3][8];
+  __shared__ float tcos;
+  const int i = blockIdx.x;
+  const float* g = G + static_cast<size_t>(i) * ldg;
+  float* co = cos_out + static_cast<size_t>(i) * C;
+  const int64_t y = labels[i];
+  const bool ok = y >= 0 && y < C;
+  if (ok) {
+    const float* e = E + static_cast<size_t>(i) * D;
+    const float* w = W + static_cast<size_t>(y) * D;
+    double ew = 0.0, ee = 0.0, ww = 0.0;
+    for (int d = threadIdx.x; d < D; d += blockDim.x) {
+      const double ed = e[d], wd = w[d];
+      ew = fma(ed, wd, ew);
+      ee = fma(ed, ed, ee);
+      ww = fma(wd, wd, ww);
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      ew += __shfl_xor_sync(0xffffffffu, ew, o);
+      ee += __shfl_xor_sync(0xffffffffu, ee, o);
+      ww += __shfl_xor_sync(0xffffffffu, ww, o);
+    }
+    if ((threadIdx.x & 31) == 0) {
+      red3[0][threadIdx.x >> 5] = ew;
+      red3[1][threadIdx.x >> 5] = ee;
+      red3[2][threadIdx.x >> 5] = ww;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int k = 1; k < static_cast<int>(blockDim.x >> 5); ++k) {
+        ew += red3[0][k];
+        ee += red3[1][k];
+        ww += red3[2][k];
+      }
+      tcos = static_cast<float>(ew / (fmax(sqrt(ee), 1e-12) * fmax(sqrt(ww), 1e-12)));
+    }
+    __syncthreads();
+  }
+  float m = -INFINITY;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const bool tgt = ok && c == y;
+    const float cv = tgt ? tcos : g[c];
+    co[c] = cv;
+    m = fmaxf(m, a.s * (tgt ? aam_phi(cv, a) : cv));
+  }
+  m = block_reduce_max(m, red);
+  float sum = 0.f;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const bool tgt = ok && c == y;
+    sum += expf(a.s * (tgt ? aam_phi(tcos, a) : g[c]) - m);
+  }
+  sum = block_reduce_sum(sum, red);
+  if (threadIdx.x == 0) {
+    const float l = m + logf(sum);
+    lse[i] = l;
+    row_loss[i] = ok ? l - a.s * aam_phi(tcos, a) : __int_as_float(0x7fc00000);
+  }
+}
+
+// Backward rows: dcos[i][c] = s (softmax - onehot) grad_loss / N, times dphi/dcos on the target column, into the fp32
+// workspace dcos [Np][Cp] and, multiplied by the row's power of two 2^e (rinv[i] = 2^-e), into the K-sliced A-side
+// image dimg [Np][3 Cp] = [lo | hi | hi] of gE^ = dcos W^.  The probabilities are e_c / sum_c e_c with e_c = exp(logit - lse):
+// the division removes the rounding of the saved lse, and the target's softmax - 1 is minus the sum over the other
+// columns, which keeps its relative accuracy in rows that are already well classified.  Rows i >= N and columns
+// c >= C are zero.  grid Np, block 256.
+__global__ void __launch_bounds__(256)
+aam_dcos_kernel(const float* __restrict__ cos, const float* __restrict__ lse, const int64_t* __restrict__ labels, int N,
+                int C, int Cp, AamMargin a, const float* __restrict__ grad_loss, float* __restrict__ dcos,
+                uint16_t* __restrict__ dimg, float* __restrict__ rinv) {
+  __shared__ float red[8];
+  const int i = blockIdx.x;
+  float* d = dcos + static_cast<size_t>(i) * Cp;
+  const int Np = gridDim.x;
+  if (i >= N) {
+    for (int c = threadIdx.x; c < Cp; c += blockDim.x) {
+      d[c] = 0.f;
+      dimg[aam_kslice_off(i, Np, 0, c, Cp)] = dimg[aam_kslice_off(i, Np, 1, c, Cp)] =
+          dimg[aam_kslice_off(i, Np, 2, c, Cp)] = 0;
+    }
+    if (threadIdx.x == 0) rinv[i] = 1.f;
+    return;
+  }
+  const float* co = cos + static_cast<size_t>(i) * C;
+  const int64_t y = labels[i];
+  const bool ok = y >= 0 && y < C;
+  const float l = lse[i];
+  float sig = 0.f, other = 0.f;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const bool tgt = ok && c == y;
+    const float e = expf(a.s * (tgt ? aam_phi(co[c], a) : co[c]) - l);
+    sig += e;
+    if (!tgt) other += e;
+  }
+  sig = block_reduce_sum(sig, red);
+  other = block_reduce_sum(other, red);
+  const float coef = grad_loss[0] / static_cast<float>(N) * a.s / sig;
+  float mx = 0.f;
+  for (int c = threadIdx.x; c < Cp; c += blockDim.x) {
+    float v = 0.f;
+    if (c < C) {
+      if (ok && c == y) v = -other * coef * aam_dphi(co[c], a);
+      else v = expf(a.s * co[c] - l) * coef;
+    }
+    d[c] = v;
+    mx = fmaxf(mx, fabsf(v));
+  }
+  const int e = aam_scale_exp(block_reduce_max(mx, red));
+  if (threadIdx.x == 0) rinv[i] = aam_pow2(-e);
+  const float S = aam_pow2(e);
+  for (int c = threadIdx.x; c < Cp; c += blockDim.x) {
+    uint16_t hi, lo;
+    aam_split16(d[c] * S, hi, lo);
+    dimg[aam_kslice_off(i, Np, 0, c, Cp)] = lo;
+    dimg[aam_kslice_off(i, Np, 1, c, Cp)] = hi;
+    dimg[aam_kslice_off(i, Np, 2, c, Cp)] = hi;
+  }
+}
+
+// The A-side image of gW^ = dcos^T E^: K-sliced dimgT [Cp][3 Np] = [lo | hi | hi] of column c of dcos times its own power of two
+// 2^e_c (cinv[c] = 2^-e_c; a per-column scale keeps classes whose every probability is small out of fp16's subnormals).
+// grid Cp / 32, block 256.
+__global__ void __launch_bounds__(256)
+aam_dcos_t_kernel(const float* __restrict__ dcos, int Np, int Cp, uint16_t* __restrict__ dimgT, float* __restrict__ cinv) {
+  __shared__ float tile[32][33];
+  __shared__ float red[8][32];
+  __shared__ float scl[32];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int c0 = blockIdx.x * 32;
+  float mx = 0.f;
+  for (int i = ty; i < Np; i += 8) mx = fmaxf(mx, fabsf(dcos[static_cast<size_t>(i) * Cp + c0 + tx]));
+  red[ty][tx] = mx;
+  __syncthreads();
+  if (ty == 0) {
+    for (int k = 1; k < 8; ++k) mx = fmaxf(mx, red[k][tx]);
+    const int e = aam_scale_exp(mx);
+    scl[tx] = aam_pow2(e);
+    cinv[c0 + tx] = aam_pow2(-e);
+  }
+  __syncthreads();
+  const float* src = dcos + static_cast<size_t>(ty) * Cp + c0 + tx;
+  for (int i0 = 0; i0 < Np; i0 += 32) {
+#pragma unroll
+    for (int r = 0; r < 32; r += 8) tile[ty + r][tx] = src[static_cast<size_t>(i0 + r) * Cp];
+    __syncthreads();
+#pragma unroll
+    for (int r = 0; r < 32; r += 8) {
+      uint16_t hi, lo;
+      aam_split16(tile[tx][ty + r] * scl[ty + r], hi, lo);
+      dimgT[aam_kslice_off(c0 + ty + r, Cp, 0, i0 + tx, Np)] = lo;
+      dimgT[aam_kslice_off(c0 + ty + r, Cp, 1, i0 + tx, Np)] = hi;
+      dimgT[aam_kslice_off(c0 + ty + r, Cp, 2, i0 + tx, Np)] = hi;
+    }
+    __syncthreads();
+  }
+}
+
+// The F.normalize Jacobian: out[r] = (g - x^ (x^ . g)) / nrm[r] with x^ = X[r] / nrm[r] and g = the sum of the K
+// slices' GEMM rows G[s][r] (slices `slice_elems` apart, added in slice order) times ginv[r] (un-scaling by its exact
+// power of two).  One warp per row, fixed order.  grid ceil(rows / 8), block 256.
+__global__ void __launch_bounds__(256)
+aam_normalize_bwd_kernel(const float* __restrict__ X, const float* __restrict__ nrm, const float* __restrict__ G,
+                         int slices, long slice_elems, const float* __restrict__ ginv, int rows, int D,
+                         float* __restrict__ out) {
+  const int r = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (r >= rows) return;
+  const float* x = X + static_cast<size_t>(r) * D;
+  const float* g = G + static_cast<size_t>(r) * D;
+  const float n = nrm[r], gi = ginv[r];
+  auto grad = [&](int d) {
+    float v = g[d];
+    for (int s = 1; s < slices; ++s) v += g[s * slice_elems + d];
+    return v * gi;
+  };
+  float dot = 0.f;
+  for (int d = lane; d < D; d += 32) dot = fmaf(x[d] / n, grad(d), dot);
+  for (int o = 16; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
+  float* y = out + static_cast<size_t>(r) * D;
+  for (int d = lane; d < D; d += 32) y[d] = (grad(d) - (x[d] / n) * dot) / n;
+}
+
+}  // namespace dsk

@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "../../include/dsk.h"
+#include "aam_kernels.cuh"
 #include "conv_umma.cuh"
 #include "conv3x3_halo.cuh"
 #include "conv1_umma.cuh"
@@ -164,6 +165,23 @@ struct LayerCfg {
   int cin, cout, ksize, stride;
 };
 
+// Cached plan of the AAM-softmax op for one (N, C, D): fp16 hi/lo operand images, fp32 GEMM outputs and workspaces, and
+// the descriptors of its three GEMMs.  Np / Cp: N and C rounded up to 128 (the GEMM's pixel tile).
+struct AamPlan {
+  int N = 0, C = 0, D = 0, Np = 0, Cp = 0;
+  uint8_t* buf = nullptr;
+  uint16_t *ea = nullptr, *wb = nullptr;     // forward operands: E^ [Np][3D] (A side), W^ [Cp][3D] (B side)
+  uint16_t *et = nullptr, *wt = nullptr;     // backward B operands, transposed: E^T [D][3Np], W^T [D][3Cp]
+  uint16_t *da = nullptr, *dt = nullptr;     // backward A operands: dcos [Np][3Cp], dcos^T [Cp][3Np] (K-sliced)
+  float *nrm_e = nullptr, *nrm_w = nullptr;  // [Np], [Cp]
+  float *gcos = nullptr, *dcos = nullptr;    // [Np][Cp]
+  float *rinv = nullptr, *cinv = nullptr;    // [Np], [Cp]: inverse power-of-two scales of dcos's rows / columns
+  int sc = 0, sn = 0;                        // K slices of the two backward GEMMs: ceil(Cp / kAamSlice), ceil(Np / ...)
+  float *ge = nullptr, *gw = nullptr;        // [sc][Np][D], [sn][Cp][D]: the slices' scaled gradients w.r.t. E^ and W^
+  float* row_loss = nullptr;                 // [Np]
+  std::vector<ConvLaunch> fwd, ge_gemm, gw_gemm;
+};
+
 // conv index i = 3*stage + {0: 5x5 s2 entry conv, 1,2: 3x3 block convs}
 LayerCfg layer_cfg(int i) {
   static const int ch[4] = {64, 128, 256, 512};
@@ -250,6 +268,7 @@ struct dsk_handle_s {
   int ap_N = 0, ap_D = 0, ap_row0 = 0, ap_rows = 0;
   uint8_t* ap_buf = nullptr;
   std::vector<ConvLaunch> ap_gemm;
+  AamPlan aam;                 // cached AAM-softmax plan (its own slot: a step may use both ops)
   bool n256 = false;           // DSK_N256=1: 256-channel tiles for layers with >= n256_min_tiles such tiles
   int n256_min_tiles = 80;
   bool use_graph = true;       // DSK_GRAPH=0: always launch the forward kernel by kernel
@@ -408,13 +427,13 @@ struct TapTable {
 int build_conv_core(const dsk_handle_s* h, ConvLaunch* L, const View5& a, const void* wpk, int k_ch, int n_out,
                     int w_slices, const View5& o, const void* res, int B, int Hgrid, int Wgrid, const TapTable& taps,
                     int flags, float clip_hi, const float* scale, const float* bias, int out_c_base, int out_ph,
-                    bool out_f32 = false) {
+                    bool out_f32 = false, bool f16 = false) {
   if (out_f32 && (flags != 0)) return fail(DSK_ERR_INVALID, "conv: fp32 output supports neither residual nor clip");
   L->out_f32 = out_f32;
   if (k_ch % 64 || n_out % 64 || k_ch < 64 || n_out < 64 || n_out > 512)
     return fail(DSK_ERR_INVALID, "conv: channel counts must be multiples of 64 and <= 512 outputs (got %d, %d)", k_ch, n_out);
   if (Wgrid > 128 || 128 % Wgrid) return fail(DSK_ERR_INVALID, "conv: output width %d must divide 128", Wgrid);
-  const bool bf = h->bf16;
+  const bool bf = h->bf16 && !f16;  // f16: fp16 operands whatever the handle's type (launch with launch_gemm_f16)
   dsk::ConvParams& p = L->p;
   memset(&p, 0, sizeof(p));
   choose_tile(B, Hgrid, Wgrid, 128, p.wt, p.hb, p.nb);
@@ -1057,6 +1076,7 @@ int32_t dsk_destroy(dsk_handle h) {
   cudaFree(h->sk_partial);
   cudaFree(h->sk_flags);
   cudaFree(h->ap_buf);
+  cudaFree(h->aam.buf);
   cudaFree(h->ones);
   cudaFree(h->zeros);
   for (dsk_train_ctx_s* c : h->ctx_pool) {
@@ -2591,6 +2611,166 @@ int32_t dsk_allpairs_topk(const float* E, const int64_t* labels, int32_t N, int3
   dsk::topk_rows_kernel<<<(N + 7) / 8, 256, 0, s>>>(S, labels, N, 0, N, pd_eps(D), k, idx, val);
   KERNEL_CHECK();
   CUDA_TRY(cudaFreeAsync(S, s));
+  return DSK_OK;
+}
+
+// ---- additive angular margin softmax ------------------------------------------------------------------------------
+// A GEMM of the AAM-softmax op: fp16 operands whatever the handle's type (a bf16 hi/lo split keeps 16 bits, not 22).
+static int launch_gemm_f16(const ConvLaunch& L, cudaStream_t s) {
+  switch (L.n_tile) {
+    case 64: return launch_conv_t<64, false, true>(L, s);
+    case 128: return launch_conv_t<128, false, true>(L, s);
+  }
+  return fail(DSK_ERR_INVALID, "unsupported N tile %d", L.n_tile);
+}
+
+// out (rows_pad x n_total fp32) = A (rows_pad x K) B^T (n_total x K), both 16-bit row-major images: rows of A are the
+// "pixels" (W = 128, H = rows_pad / 128), rows of B the "output channels", <= 512 per launch; one tap.
+static int aam_build_gemm(dsk_handle h, std::vector<ConvLaunch>* out, const uint16_t* A, int rows_pad, const uint16_t* B,
+                          int n_total, int K, float* O) {
+  TapTable tt;
+  tt.add(0, 0, 0, 0, 0);
+  for (int c0 = 0; c0 < n_total; c0 += 512) {
+    ConvLaunch L;
+    const int rc = build_conv_core(h, &L, nhwc_view(A, 1, rows_pad / 128, 128, K), B + static_cast<size_t>(c0) * K, K,
+                                   n_total - c0 < 512 ? n_total - c0 : 512, 1, nhwc_view(O, 1, rows_pad / 128, 128, n_total),
+                                   nullptr, 1, rows_pad / 128, 128, tt, 0, 0.f, nullptr, nullptr, c0, 0, true, true);
+    if (rc) return rc;
+    out->push_back(L);
+  }
+  return DSK_OK;
+}
+
+// (Re)build the handle's AAM plan for (N, C, D).  A rebuild synchronises `s` (buffers in use are freed).
+static int aam_plan(dsk_handle h, int N, int C, int D, cudaStream_t s, AamPlan** out) {
+  AamPlan& P = h->aam;
+  *out = &P;
+  if (P.buf && P.N == N && P.C == C && P.D == D) return DSK_OK;
+  CUDA_TRY(cudaStreamSynchronize(s));
+  if (P.buf) CUDA_TRY(cudaFree(P.buf));
+  P = AamPlan();
+  const int Np = (N + 127) / 128 * 128, Cp = (C + 127) / 128 * 128;
+  const int sc = (Cp + dsk::kAamSlice - 1) / dsk::kAamSlice, sn = (Np + dsk::kAamSlice - 1) / dsk::kAamSlice;
+  const size_t d3 = 3ull * D;
+  size_t off = 0;
+  std::vector<std::pair<void**, size_t>> parts = {
+      {reinterpret_cast<void**>(&P.ea), Np * d3 * 2},   {reinterpret_cast<void**>(&P.wb), Cp * d3 * 2},
+      {reinterpret_cast<void**>(&P.et), Np * d3 * 2},   {reinterpret_cast<void**>(&P.wt), Cp * d3 * 2},
+      {reinterpret_cast<void**>(&P.da), 3ull * Np * Cp * 2}, {reinterpret_cast<void**>(&P.dt), 3ull * Np * Cp * 2},
+      {reinterpret_cast<void**>(&P.nrm_e), Np * 4ull},  {reinterpret_cast<void**>(&P.nrm_w), Cp * 4ull},
+      {reinterpret_cast<void**>(&P.gcos), 1ull * Np * Cp * 4}, {reinterpret_cast<void**>(&P.dcos), 1ull * Np * Cp * 4},
+      {reinterpret_cast<void**>(&P.rinv), Np * 4ull},   {reinterpret_cast<void**>(&P.cinv), Cp * 4ull},
+      {reinterpret_cast<void**>(&P.ge), 1ull * sc * Np * D * 4}, {reinterpret_cast<void**>(&P.gw), 1ull * sn * Cp * D * 4},
+      {reinterpret_cast<void**>(&P.row_loss), Np * 4ull}};
+  for (auto& p : parts) off += (p.second + 255) / 256 * 256;
+  CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&P.buf), off));
+  off = 0;
+  for (auto& p : parts) {
+    *p.first = P.buf + off;
+    off += (p.second + 255) / 256 * 256;
+  }
+  int rc = aam_build_gemm(h, &P.fwd, P.ea, Np, P.wb, Cp, 3 * D, P.gcos);  // cos = E^ W^T, K = 3D
+  // gE^ = dcos W^ (K = 3Cp) and gW^ = dcos^T E^ (K = 3Np), one GEMM per K slice into the slice's own output
+  const size_t ks = dsk::kAamSlice;
+  for (int k = 0; k < sc && !rc; ++k) {
+    const int w = Cp - k * dsk::kAamSlice < dsk::kAamSlice ? Cp - k * dsk::kAamSlice : dsk::kAamSlice;
+    rc = aam_build_gemm(h, &P.ge_gemm, P.da + k * ks * 3 * Np, Np, P.wt + k * ks * 3 * D, D, 3 * w,
+                        P.ge + static_cast<size_t>(k) * Np * D);
+  }
+  for (int k = 0; k < sn && !rc; ++k) {
+    const int w = Np - k * dsk::kAamSlice < dsk::kAamSlice ? Np - k * dsk::kAamSlice : dsk::kAamSlice;
+    rc = aam_build_gemm(h, &P.gw_gemm, P.dt + k * ks * 3 * Cp, Cp, P.et + k * ks * 3 * D, D, 3 * w,
+                        P.gw + static_cast<size_t>(k) * Cp * D);
+  }
+  if (rc) {
+    cudaFree(P.buf);
+    P = AamPlan();
+    return rc;
+  }
+  P.N = N;
+  P.C = C;
+  P.D = D;
+  P.Np = Np;
+  P.Cp = Cp;
+  P.sc = sc;
+  P.sn = sn;
+  return DSK_OK;
+}
+
+static int aam_check(dsk_handle h, bool ptrs_ok, int N, int C, int D, float margin, float scale, const char* what) {
+  if (!ptrs_ok || N < 1 || C < 2 || C > DSK_AAM_MAX_C || D < 64 || D % 64 || !std::isfinite(margin) || margin < 0.f ||
+      !std::isfinite(scale) || !(scale > 0.f))
+    return fail(DSK_ERR_INVALID, "%s: bad arguments (need non-null pointers, N >= 1, 2 <= C <= %d, D a positive multiple "
+                "of 64, finite margin >= 0 and scale > 0; got N %d, C %d, D %d, margin %g, scale %g)", what,
+                DSK_AAM_MAX_C, N, C, D, margin, scale);
+  return check_handle(h);
+}
+
+static dsk::AamMargin aam_margin(float margin, float scale) {
+  const double m = margin, pi = 3.14159265358979323846;
+  return {static_cast<float>(std::cos(m)), static_cast<float>(std::sin(m)), static_cast<float>(std::cos(pi - m)),
+          static_cast<float>(std::sin(pi - m) * m), scale};
+}
+
+// norms of E and W, and their hi/lo operand images (forward: row-major; backward: transposed)
+static int aam_prep(const AamPlan& P, const float* E, const float* W, bool backward, cudaStream_t s) {
+  const int D = P.D;
+  dsk::aam_norm_kernel<<<(P.N + 7) / 8, 256, 0, s>>>(E, P.N, D, P.nrm_e);
+  KERNEL_CHECK();
+  dsk::aam_norm_kernel<<<(P.C + 7) / 8, 256, 0, s>>>(W, P.C, D, P.nrm_w);
+  KERNEL_CHECK();
+  dsk::aam_split_kernel<<<dim3(D / 64, P.Np / 32), 256, 0, s>>>(E, P.nrm_e, P.N, P.Np, D, 1, backward ? nullptr : P.ea,
+                                                                 backward ? P.et : nullptr);
+  KERNEL_CHECK();
+  dsk::aam_split_kernel<<<dim3(D / 64, P.Cp / 32), 256, 0, s>>>(W, P.nrm_w, P.C, P.Cp, D, 0, backward ? nullptr : P.wb,
+                                                                 backward ? P.wt : nullptr);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_aam_softmax(dsk_handle h, const float* E, const float* W, const int64_t* labels, int32_t N, int32_t C,
+                        int32_t D, float margin, float scale, float* loss, float* cos, float* lse, void* stream) {
+  int rc = aam_check(h, E && W && labels && loss && cos && lse, N, C, D, margin, scale, "dsk_aam_softmax");
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  AamPlan* P = nullptr;
+  if ((rc = aam_plan(h, N, C, D, s, &P))) return rc;
+  if ((rc = aam_prep(*P, E, W, false, s))) return rc;
+  for (const ConvLaunch& L : P->fwd)
+    if ((rc = launch_gemm_f16(L, s))) return rc;
+  dsk::aam_rows_kernel<<<N, 256, 0, s>>>(P->gcos, P->Cp, E, W, D, labels, C, aam_margin(margin, scale), cos, lse,
+                                         P->row_loss);
+  KERNEL_CHECK();
+  dsk::mean_rows_kernel<<<1, 1024, 0, s>>>(P->row_loss, N, loss);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_aam_softmax_bwd(dsk_handle h, const float* E, const float* W, const int64_t* labels, const float* cos,
+                            const float* lse, int32_t N, int32_t C, int32_t D, float margin, float scale,
+                            const float* grad_loss, float* gE, float* gW, void* stream) {
+  int rc = aam_check(h, E && W && labels && cos && lse && grad_loss && gE && gW, N, C, D, margin, scale,
+                     "dsk_aam_softmax_bwd");
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  AamPlan* P = nullptr;
+  if ((rc = aam_plan(h, N, C, D, s, &P))) return rc;
+  if ((rc = aam_prep(*P, E, W, true, s))) return rc;
+  dsk::aam_dcos_kernel<<<P->Np, 256, 0, s>>>(cos, lse, labels, N, C, P->Cp, aam_margin(margin, scale), grad_loss,
+                                             P->dcos, P->da, P->rinv);
+  KERNEL_CHECK();
+  dsk::aam_dcos_t_kernel<<<P->Cp / 32, 256, 0, s>>>(P->dcos, P->Np, P->Cp, P->dt, P->cinv);
+  KERNEL_CHECK();
+  for (const ConvLaunch& L : P->ge_gemm)
+    if ((rc = launch_gemm_f16(L, s))) return rc;
+  for (const ConvLaunch& L : P->gw_gemm)
+    if ((rc = launch_gemm_f16(L, s))) return rc;
+  dsk::aam_normalize_bwd_kernel<<<(N + 7) / 8, 256, 0, s>>>(E, P->nrm_e, P->ge, P->sc, static_cast<long>(P->Np) * D,
+                                                            P->rinv, N, D, gE);
+  KERNEL_CHECK();
+  dsk::aam_normalize_bwd_kernel<<<(C + 7) / 8, 256, 0, s>>>(W, P->nrm_w, P->gw, P->sn, static_cast<long>(P->Cp) * D,
+                                                            P->cinv, C, D, gW);
+  KERNEL_CHECK();
   return DSK_OK;
 }
 

@@ -255,7 +255,7 @@ _AP_HANDLES = {}
 
 
 def _allpairs_handle(device):
-    """Module-level fp16 engine handle for the tensor-core all-pairs path (one per device)."""
+    """Module-level fp16 engine handle for the tensor-core all-pairs and AAM-softmax ops (one per device)."""
     key = device.index if device.index is not None else torch.cuda.current_device()
     if key not in _AP_HANDLES:
         h = ctypes.c_void_p()
@@ -378,3 +378,67 @@ class BatchHardTripletFn(torch.autograd.Function):
     def backward(ctx, gl):
         E, pos, neg, d_ap, d_an, valid = ctx.saved_tensors
         return batch_hard_backward(E, pos, neg, d_ap, d_an, valid, ctx.margin, gl), None, None, None
+
+
+# ---------------------------------------------------------------------------------------------------
+# additive angular margin softmax
+# ---------------------------------------------------------------------------------------------------
+def _aam_inputs(E, W, labels):
+    for t in (E, W):
+        if not t.is_cuda:
+            raise RuntimeError("the AAM-softmax loss needs CUDA tensors; there is no CPU fallback")
+    if E.dim() != 2 or W.dim() != 2 or E.shape[1] != W.shape[1]:
+        raise RuntimeError(f"expected embeddings (N, D) and weight (C, D), got {tuple(E.shape)} and {tuple(W.shape)}")
+    if W.device != E.device:
+        raise RuntimeError("embeddings and weight must be on one device")
+    E = E.detach().float().contiguous()
+    W = W.detach().float().contiguous()
+    labels = torch.as_tensor(labels).to(device=E.device, dtype=torch.int64).contiguous()
+    if labels.shape != (E.shape[0],):
+        raise RuntimeError(f"expected labels of shape ({E.shape[0]},), got {tuple(labels.shape)}")
+    return E, W, labels
+
+
+def aam_softmax(E, W, labels, margin, scale):
+    """dsk_aam_softmax: (E, W, labels as the op read them, loss (1,), cos (N, C), lse (N,)) on E's device."""
+    E, W, labels = _aam_inputs(E, W, labels)
+    (N, D), C = E.shape, W.shape[0]
+    dev = E.device
+    loss = torch.empty(1, device=dev, dtype=torch.float32)
+    cos = torch.empty(N, C, device=dev, dtype=torch.float32)
+    lse = torch.empty(N, device=dev, dtype=torch.float32)
+    with torch.cuda.device(dev):
+        L.check(L.load().dsk_aam_softmax(_allpairs_handle(dev), E.data_ptr(), W.data_ptr(), labels.data_ptr(), N, C, D,
+                                         float(margin), float(scale), loss.data_ptr(), cos.data_ptr(), lse.data_ptr(),
+                                         L.cur_stream()), "dsk_aam_softmax")
+    return E, W, labels, loss, cos, lse
+
+
+def aam_softmax_backward(E, W, labels, cos, lse, margin, scale, grad_loss):
+    """dsk_aam_softmax_bwd: (gE (N, D), gW (C, D)) = d loss / d (E, W) scaled by the device scalar ``grad_loss``."""
+    (N, D), C = E.shape, W.shape[0]
+    gl = grad_loss.float().reshape(1).contiguous()
+    gE, gW = torch.empty_like(E), torch.empty_like(W)
+    with torch.cuda.device(E.device):
+        L.check(L.load().dsk_aam_softmax_bwd(_allpairs_handle(E.device), E.data_ptr(), W.data_ptr(), labels.data_ptr(),
+                                             cos.data_ptr(), lse.data_ptr(), N, C, D, float(margin), float(scale),
+                                             gl.data_ptr(), gE.data_ptr(), gW.data_ptr(), L.cur_stream()),
+                "dsk_aam_softmax_bwd")
+    return gE, gW
+
+
+class AAMSoftmaxFn(torch.autograd.Function):
+    """Additive angular margin softmax over a cosine classifier; the loss is a device scalar."""
+
+    @staticmethod
+    def forward(ctx, E, W, labels, margin, scale):
+        Ec, Wc, lab, loss, cos, lse = aam_softmax(E, W, labels, margin, scale)
+        ctx.save_for_backward(Ec, Wc, lab, cos, lse)
+        ctx.margin, ctx.scale = margin, scale
+        return loss.reshape(())
+
+    @staticmethod
+    def backward(ctx, gl):
+        E, W, lab, cos, lse = ctx.saved_tensors
+        gE, gW = aam_softmax_backward(E, W, lab, cos, lse, ctx.margin, ctx.scale, gl)
+        return (gE if ctx.needs_input_grad[0] else None), (gW if ctx.needs_input_grad[1] else None), None, None, None

@@ -246,6 +246,28 @@ class BatchHardTripletLoss:
         return pos, neg, d_ap, d_an, valid
 
 
+class AAMSoftmaxLoss:
+    """Additive angular margin softmax (ArcFace / AAM-softmax; no reference implementation - the usual modern form of the
+    reference's softmax over ``model.classifier``, train_triplet.py:277-287).  Cosines between the L2-normalised
+    embeddings and the L2-normalised rows of ``weight`` (C, E), margin ``m`` added to the angle of the target class
+    (``cos - sin(pi - m) m`` past pi - m), logits times ``scale``, cross-entropy averaged over the batch.  Pass
+    ``model.model.classifier.weight``: parameters, ``state_dict`` keys and optimizer buckets stay as they are, and the
+    classifier's bias is not used.  ``margin = 0`` is the normalised softmax (NormFace); a margin warm-up passes a
+    different ``margin`` per step."""
+
+    def __init__(self, weight, margin, scale):
+        self.weight = weight
+        self.margin = margin
+        self.scale = scale
+
+    def forward(self, embeddings, labels):
+        """embeddings (N, E) CUDA, labels (N,) int in [0, C) -> 0-dim device scalar; back-propagates into the
+        embeddings and the weight."""
+        return _engine.AAMSoftmaxFn.apply(embeddings, self.weight, labels, float(self.margin), float(self.scale))
+
+    __call__ = forward
+
+
 def batch_hard_valid_count(labels):
     """V, the number of valid anchors of a batch-hard loss, from the labels alone (host-side: no device sync when the
     labels are a CPU tensor, as a data loader yields them): anchors whose speaker has >= 2 utterances, provided the

@@ -29,7 +29,7 @@ import torch.distributed as dist
 from . import engine as _engine
 from . import train as _train
 from .head import CrossEntropyLoss
-from .model import (BatchHardTripletLoss, PairwiseDistance, TripletMarginLoss, batch_hard_valid_count,
+from .model import (AAMSoftmaxLoss, BatchHardTripletLoss, PairwiseDistance, TripletMarginLoss, batch_hard_valid_count,
                     select_hard_triplets)
 from .optim import FusedAdagrad
 from .parallel import GlobalBatchHardTripletLoss, _distributed, gather_labels
@@ -169,3 +169,21 @@ def _global_batch_hard_step(model, optimizer, data, labels, margin, bucket):
     loss.backward(torch.full_like(loss, float(world)))       # R x this rank's share; the mean all-reduce divides by R
     _reduce_and_step(optimizer, bucket, None)
     return {"loss": loss.detach(), "valid": V}
+
+
+def aam_softmax_step(model, optimizer, data, labels, *, margin, scale, bucket=None):
+    """One classification step with the additive angular margin softmax (``AAMSoftmaxLoss`` on
+    ``model.model.classifier.weight``): ONE train-mode forward of all N utterances, the loss, backward, optimizer step.
+    Returns ``{"loss": device scalar}``.  Every row of the loss depends only on its own embedding and the class weights,
+    so under data parallelism (``bucket`` or a ``FusedAdagrad`` optimizer, the same n on every rank) the plain mean
+    all-reduce of the gradients is the gradient of the global mean loss; the loss itself needs no collective.  Runs
+    unchanged on a model with ``sync_batchnorm()``."""
+    if not model.training:
+        raise RuntimeError("aam_softmax_step needs model.train()")
+    labels = _labels_to(labels, data.device)
+    emb = model(data)
+    loss = AAMSoftmaxLoss(model.model.classifier.weight, margin, scale).forward(emb, labels)
+    optimizer.zero_grad()
+    loss.backward()
+    _reduce_and_step(optimizer, bucket, None)
+    return {"loss": loss.detach()}

@@ -309,6 +309,33 @@ int32_t dsk_batch_hard_triplet_bwd_rows(const float* E, const int64_t* pos_idx, 
                                         int32_t D, int32_t row0, int32_t rows, float margin, const float* grad_loss,
                                         float* gE_rows, void* stream);
 
+/* Additive angular margin softmax (ArcFace / AAM-softmax) over a cosine classifier (no reference implementation exists;
+ * the usual modern form of the reference's softmax over the speaker classifier, train_triplet.py:277-287).  For
+ * embeddings E (N,D), class weights W (C,D) (e.g. model.classifier.weight), int64 labels y, margin m >= 0, scale s > 0:
+ *   e^_i = e_i / max(||e_i||, 1e-12), w^_c likewise (F.normalize);  cos (N,C) = e^_i . w^_c;
+ *   target column: sin = sqrt(clamp(1 - cos^2, 0, 1)), phi = cos > cos(pi - m) ? cos cos m - sin sin m
+ *                                                                           : cos - sin(pi - m) m;
+ *   logit_ic = s * (c == y_i ? phi : cos);  lse (N,) = logsumexp_c logit_ic;
+ *   loss (1,) = (1/N) sum_i (lse_i - logit_{i,y_i}), summed in a fixed order.  A label outside [0, C) yields NaN.
+ * cos and lse are caller-owned outputs that dsk_aam_softmax_bwd reads.  The cosines run on the tensor cores in fp16
+ * (whatever the handle's operand type) with each operand split into hi + lo halves, which keeps them at fp32-level
+ * accuracy; the target column's cosine is recomputed in fp64.  Every row of cos, lse and gE depends only on that row's
+ * embedding and label (and W): sharding the batch
+ * over ranks gives bit-identical rows when grad_loss / N is the same.
+ * The GEMM plan and its operand buffers are cached in h for (N, C, D), in a slot of their own; a change rebuilds them,
+ * which synchronises the stream.  1 <= N, 2 <= C <= DSK_AAM_MAX_C, D % 64 == 0, else DSK_ERR_INVALID. */
+#define DSK_AAM_MAX_C 65536
+int32_t dsk_aam_softmax(dsk_handle h, const float* E, const float* W, const int64_t* labels, int32_t N, int32_t C,
+                        int32_t D, float margin, float scale, float* loss, float* cos, float* lse, void* stream);
+/* Its backward: gE (N,D) and gW (C,D) = d loss / d E, d loss / d W scaled by grad_loss (device scalar), WRITTEN not
+ * accumulated.  dcos = s (softmax - onehot) grad_loss / N, times d phi / d cos on the target column (cos m + sin m
+ * cos / sin; cos m at sin = 0; 1 below cos(pi - m)), then gE^ = dcos W^, gW^ = dcos^T E^ and the F.normalize Jacobians
+ * g_i = (g^_i - e^_i (e^_i . g^_i)) / max(||e_i||, 1e-12).  Deterministic: no float atomics; the two GEMMs split K
+ * into fixed slices of 512 classes / utterances whose outputs are added in slice order. */
+int32_t dsk_aam_softmax_bwd(dsk_handle h, const float* E, const float* W, const int64_t* labels, const float* cos,
+                            const float* lse, int32_t N, int32_t C, int32_t D, float margin, float scale,
+                            const float* grad_loss, float* gE, float* gW, void* stream);
+
 /* nn.Linear of DeepSpeakerModel.forward_classifier (reference model.py:167,220-223): y (M,N) = x (M,K) w(N,K)^T + b.
  * fp32 on the CUDA cores, fixed summation order (deterministic).  b may be NULL. */
 int32_t dsk_linear_forward(const float* x, const float* w, const float* b, int32_t M, int32_t N, int32_t K, float* y,
