@@ -170,6 +170,10 @@ SIGNATURES = {
     "dsk_batch_hard_triplet_bwd_rows": (c_int32, [c_void_p] * 6 + [c_int32] * 4 + [c_float] + [c_void_p] * 3),
     "dsk_aam_softmax": (c_int32, [c_void_p] * 4 + [c_int32] * 3 + [c_float, c_float] + [c_void_p] * 4),
     "dsk_aam_softmax_bwd": (c_int32, [c_void_p] * 6 + [c_int32] * 3 + [c_float, c_float] + [c_void_p] * 4),
+    "dsk_cosine_matrix": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_void_p]),
+    "dsk_topk_mean_std": (c_int32, [c_void_p, c_int32, c_int32, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
+    "dsk_cohort_stats": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_int32] + [c_void_p] * 3),
+    "dsk_score_trials": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_int64] + [c_void_p] * 5),
     "dsk_linear_forward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     "dsk_linear_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p,
                                       c_void_p, c_void_p]),

@@ -22,6 +22,7 @@
 #include "head_kernels.cuh"
 #include "loss_kernels.cuh"
 #include "metric_kernels.cuh"
+#include "score_kernels.cuh"
 #include "simt_kernels.cuh"
 #include "train_kernels.cuh"
 #include "wgrad_umma.cuh"
@@ -182,6 +183,17 @@ struct AamPlan {
   std::vector<ConvLaunch> fwd, ge_gemm, gw_gemm;
 };
 
+// Cached plan of the cosine-scoring ops for one (Nc, D, chunk): the fp16 hi/lo operand images of a row chunk of E and of
+// the cohort, their norms, the chunk's fp32 cosines and the descriptors of the one GEMM.  Np: Nc rounded up to 128.
+struct ScorePlan {
+  int Nc = 0, D = 0, chunk = 0, Np = 0;
+  uint8_t* buf = nullptr;
+  uint16_t *ea = nullptr, *cb = nullptr;     // E^ chunk [chunk][3D] (A side), cohort^ [Np][3D] (B side)
+  float *nrm_e = nullptr, *nrm_c = nullptr;  // [chunk], [Np]
+  float* cos = nullptr;                      // [chunk][Np]
+  std::vector<ConvLaunch> gemm;
+};
+
 // conv index i = 3*stage + {0: 5x5 s2 entry conv, 1,2: 3x3 block convs}
 LayerCfg layer_cfg(int i) {
   static const int ch[4] = {64, 128, 256, 512};
@@ -269,6 +281,7 @@ struct dsk_handle_s {
   uint8_t* ap_buf = nullptr;
   std::vector<ConvLaunch> ap_gemm;
   AamPlan aam;                 // cached AAM-softmax plan (its own slot: a step may use both ops)
+  ScorePlan score;             // cached cosine-scoring plan (its own slot: evaluation runs between training steps)
   bool n256 = false;           // DSK_N256=1: 256-channel tiles for layers with >= n256_min_tiles such tiles
   int n256_min_tiles = 80;
   bool use_graph = true;       // DSK_GRAPH=0: always launch the forward kernel by kernel
@@ -1077,6 +1090,7 @@ int32_t dsk_destroy(dsk_handle h) {
   cudaFree(h->sk_flags);
   cudaFree(h->ap_buf);
   cudaFree(h->aam.buf);
+  cudaFree(h->score.buf);
   cudaFree(h->ones);
   cudaFree(h->zeros);
   for (dsk_train_ctx_s* c : h->ctx_pool) {
@@ -2770,6 +2784,148 @@ int32_t dsk_aam_softmax_bwd(dsk_handle h, const float* E, const float* W, const 
   KERNEL_CHECK();
   dsk::aam_normalize_bwd_kernel<<<(C + 7) / 8, 256, 0, s>>>(W, P->nrm_w, P->gw, P->sn, static_cast<long>(P->Cp) * D,
                                                             P->cinv, C, D, gW);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// ---- cosine scoring, cohort statistics (AS-norm) ------------------------------------------------------------------
+// Rows of E per GEMM chunk: the largest multiple of 128 with chunk x Np x 4 B <= kScoreChunkBytes (at least 128), and no
+// more than M rounded up to 128.
+constexpr size_t kScoreChunkBytes = 256ull << 20;
+static int score_chunk_rows(int M, int Np) {
+  const long cap = static_cast<long>(kScoreChunkBytes / (static_cast<size_t>(Np) * 4)) / 128 * 128;
+  const long m = (static_cast<long>(M) + 127) / 128 * 128;
+  const long c = cap < 128 ? 128 : cap;
+  return static_cast<int>(m < c ? m : c);
+}
+
+// (Re)build the handle's scoring plan for (Nc, D, chunk).  A rebuild synchronises `s` (buffers in use are freed).
+static int score_plan(dsk_handle h, int M, int Nc, int D, cudaStream_t s, ScorePlan** out) {
+  ScorePlan& P = h->score;
+  *out = &P;
+  const int Np = (Nc + 127) / 128 * 128, chunk = score_chunk_rows(M, Np);
+  if (P.buf && P.Nc == Nc && P.D == D && P.chunk == chunk) return DSK_OK;
+  CUDA_TRY(cudaStreamSynchronize(s));
+  if (P.buf) CUDA_TRY(cudaFree(P.buf));
+  P = ScorePlan();
+  const size_t d3 = 3ull * D;
+  std::vector<std::pair<void**, size_t>> parts = {
+      {reinterpret_cast<void**>(&P.ea), chunk * d3 * 2}, {reinterpret_cast<void**>(&P.cb), Np * d3 * 2},
+      {reinterpret_cast<void**>(&P.nrm_e), chunk * 4ull}, {reinterpret_cast<void**>(&P.nrm_c), Np * 4ull},
+      {reinterpret_cast<void**>(&P.cos), 1ull * chunk * Np * 4}};
+  size_t off = 0;
+  for (auto& p : parts) off += (p.second + 255) / 256 * 256;
+  CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&P.buf), off));
+  off = 0;
+  for (auto& p : parts) {
+    *p.first = P.buf + off;
+    off += (p.second + 255) / 256 * 256;
+  }
+  const int rc = aam_build_gemm(h, &P.gemm, P.ea, chunk, P.cb, Np, 3 * D, P.cos);  // cos = E^ C^T, K = 3D
+  if (rc) {
+    cudaFree(P.buf);
+    P = ScorePlan();
+    return rc;
+  }
+  P.Nc = Nc;
+  P.D = D;
+  P.chunk = chunk;
+  P.Np = Np;
+  return DSK_OK;
+}
+
+static int score_check(dsk_handle h, bool ptrs_ok, int M, int Nc, int D, int k, const char* what) {
+  if (!ptrs_ok || M < 1 || Nc < 2 || Nc > DSK_SCORE_MAX_COHORT || D < 64 || D % 64 || k < 2 || k > Nc)
+    return fail(DSK_ERR_INVALID, "%s: bad arguments (need non-null pointers, M >= 1, 2 <= Nc <= %d, D a positive multiple "
+                "of 64, 2 <= k <= Nc; got M %d, Nc %d, D %d, k %d)", what, DSK_SCORE_MAX_COHORT, M, Nc, D, k);
+  return check_handle(h);
+}
+
+// The cohort's norms and B-side operand image, rebuilt on every call
+static int score_prep_cohort(const ScorePlan& P, const float* B, cudaStream_t s) {
+  dsk::aam_norm_kernel<<<(P.Nc + 7) / 8, 256, 0, s>>>(B, P.Nc, P.D, P.nrm_c);
+  KERNEL_CHECK();
+  dsk::aam_split_kernel<<<dim3(P.D / 64, P.Np / 32), 256, 0, s>>>(B, P.nrm_c, P.Nc, P.Np, P.D, 0, P.cb, nullptr);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// P.cos[0, rows) = cosines of rows [0, rows) of E (rows <= chunk) against the cohort; rows [rows, chunk) are zero
+static int score_gemm_chunk(const ScorePlan& P, const float* E, int rows, cudaStream_t s) {
+  dsk::aam_norm_kernel<<<(rows + 7) / 8, 256, 0, s>>>(E, rows, P.D, P.nrm_e);
+  KERNEL_CHECK();
+  dsk::aam_split_kernel<<<dim3(P.D / 64, P.chunk / 32), 256, 0, s>>>(E, P.nrm_e, rows, P.chunk, P.D, 1, P.ea, nullptr);
+  KERNEL_CHECK();
+  for (const ConvLaunch& L : P.gemm)
+    if (int rc = launch_gemm_f16(L, s)) return rc;
+  return DSK_OK;
+}
+
+static int launch_topk_stats(const float* S, int rows, int cols, long ld, int k, float* mean, float* std, cudaStream_t s) {
+  if (cols <= dsk::kTopkStageCols) {
+    const int smem = cols * 4;
+    auto kern = dsk::topk_select_stats_kernel<true>;
+    if (int rc = ensure_smem_optin(reinterpret_cast<const void*>(kern), smem)) return rc;
+    kern<<<rows, dsk::kTopkThreads, smem, s>>>(S, cols, ld, k, mean, std);
+  } else {
+    dsk::topk_select_stats_kernel<false><<<rows, dsk::kTopkThreads, 0, s>>>(S, cols, ld, k, mean, std);
+  }
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_cosine_matrix(dsk_handle h, const float* A, int32_t M, const float* B, int32_t Nc, int32_t D, float* cos,
+                          void* stream) {
+  int rc = score_check(h, A && B && cos, M, Nc, D, 2, "dsk_cosine_matrix");
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  ScorePlan* P = nullptr;
+  if ((rc = score_plan(h, M, Nc, D, s, &P))) return rc;
+  if ((rc = score_prep_cohort(*P, B, s))) return rc;
+  for (int r0 = 0; r0 < M; r0 += P->chunk) {
+    const int rows = M - r0 < P->chunk ? M - r0 : P->chunk;
+    if ((rc = score_gemm_chunk(*P, A + static_cast<size_t>(r0) * D, rows, s))) return rc;
+    CUDA_TRY(cudaMemcpy2DAsync(cos + static_cast<size_t>(r0) * Nc, Nc * 4ull, P->cos, P->Np * 4ull, Nc * 4ull, rows,
+                               cudaMemcpyDeviceToDevice, s));
+  }
+  return DSK_OK;
+}
+
+int32_t dsk_topk_mean_std(const float* S, int32_t rows, int32_t cols, int64_t ld, int32_t k, float* mean, float* std,
+                          void* stream) {
+  if (!S || !mean || !std || rows < 1 || cols < 2 || cols > DSK_SCORE_MAX_COHORT || ld < cols || k < 2 || k > cols)
+    return fail(DSK_ERR_INVALID, "dsk_topk_mean_std: bad arguments (need non-null pointers, rows >= 1, 2 <= cols <= %d, "
+                "ld >= cols, 2 <= k <= cols; got rows %d, cols %d, ld %lld, k %d)", DSK_SCORE_MAX_COHORT, rows, cols,
+                static_cast<long long>(ld), k);
+  return launch_topk_stats(S, rows, cols, static_cast<long>(ld), k, mean, std, static_cast<cudaStream_t>(stream));
+}
+
+int32_t dsk_cohort_stats(dsk_handle h, const float* E, int32_t M, const float* cohort, int32_t Nc, int32_t D, int32_t k,
+                         float* mean, float* std, void* stream) {
+  int rc = score_check(h, E && cohort && mean && std, M, Nc, D, k, "dsk_cohort_stats");
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  ScorePlan* P = nullptr;
+  if ((rc = score_plan(h, M, Nc, D, s, &P))) return rc;
+  if ((rc = score_prep_cohort(*P, cohort, s))) return rc;
+  for (int r0 = 0; r0 < M; r0 += P->chunk) {
+    const int rows = M - r0 < P->chunk ? M - r0 : P->chunk;
+    if ((rc = score_gemm_chunk(*P, E + static_cast<size_t>(r0) * D, rows, s))) return rc;
+    if ((rc = launch_topk_stats(P->cos, rows, Nc, P->Np, k, mean + r0, std + r0, s))) return rc;
+  }
+  return DSK_OK;
+}
+
+int32_t dsk_score_trials(const float* X, int32_t U, int32_t D, const int64_t* trials, int64_t T, const float* mean,
+                         const float* std, float* raw, float* normed, void* stream) {
+  const bool stats = mean || std;
+  if (!X || !trials || !raw || U < 1 || D < 1 || T < 1 || T > (1ll << 33) || (stats && (!mean || !std || !normed)))
+    return fail(DSK_ERR_INVALID, "dsk_score_trials: bad arguments (need non-null X, trials and raw, U >= 1, D >= 1, "
+                "1 <= T <= 2^33, and mean, std and normed all non-null or mean and std both NULL; got U %d, D %d, T %lld)",
+                U, D, static_cast<long long>(T));
+  const unsigned blocks = static_cast<unsigned>((T + dsk::kScoreWarps - 1) / dsk::kScoreWarps);
+  dsk::score_trials_kernel<<<blocks, 32 * dsk::kScoreWarps, 0, static_cast<cudaStream_t>(stream)>>>(
+      X, U, D, trials, static_cast<long long>(T), stats ? mean : nullptr, std, raw, normed);
   KERNEL_CHECK();
   return DSK_OK;
 }

@@ -255,7 +255,8 @@ _AP_HANDLES = {}
 
 
 def _allpairs_handle(device):
-    """Module-level fp16 engine handle for the tensor-core all-pairs and AAM-softmax ops (one per device)."""
+    """Module-level fp16 engine handle for the tensor-core all-pairs, AAM-softmax and cosine-scoring ops (one per
+    device)."""
     key = device.index if device.index is not None else torch.cuda.current_device()
     if key not in _AP_HANDLES:
         h = ctypes.c_void_p()
@@ -442,3 +443,85 @@ class AAMSoftmaxFn(torch.autograd.Function):
         E, W, lab, cos, lse = ctx.saved_tensors
         gE, gW = aam_softmax_backward(E, W, lab, cos, lse, ctx.margin, ctx.scale, gl)
         return (gE if ctx.needs_input_grad[0] else None), (gW if ctx.needs_input_grad[1] else None), None, None, None
+
+
+# ---------------------------------------------------------------------------------------------------
+# cosine scoring and cohort statistics (AS-norm)
+# ---------------------------------------------------------------------------------------------------
+def _score_rows(X, what):
+    if not X.is_cuda:
+        raise RuntimeError(f"{what} needs CUDA tensors; there is no CPU fallback")
+    if X.dim() != 2:
+        raise RuntimeError(f"{what}: expected a 2-D (rows, D) tensor, got shape {tuple(X.shape)}")
+    return X.detach().float().contiguous()
+
+
+def _score_pair(A, B, what):
+    A, B = _score_rows(A, what), _score_rows(B, what)
+    if A.shape[1] != B.shape[1]:
+        raise RuntimeError(f"{what}: embedding sizes differ ({A.shape[1]} and {B.shape[1]})")
+    if A.device != B.device:
+        raise RuntimeError(f"{what}: both tensors must be on one device")
+    return A, B
+
+
+def cosine_matrix(A, B):
+    """dsk_cosine_matrix: cos (M, Nc) fp32 = normalised rows of A (M, D) times those of B (Nc, D)."""
+    A, B = _score_pair(A, B, "cosine_matrix")
+    (M, D), Nc = A.shape, B.shape[0]
+    cos = torch.empty(M, Nc, device=A.device, dtype=torch.float32)
+    with torch.cuda.device(A.device):
+        L.check(L.load().dsk_cosine_matrix(_allpairs_handle(A.device), A.data_ptr(), M, B.data_ptr(), Nc, D,
+                                           cos.data_ptr(), L.cur_stream()), "dsk_cosine_matrix")
+    return cos
+
+
+def topk_mean_std(S, k):
+    """dsk_topk_mean_std: (mean, std) (rows,) of the k largest values of every row of S (rows, cols) (its row stride is
+    kept: a column slice of a row-major matrix needs no copy)."""
+    if not S.is_cuda:
+        raise RuntimeError("topk_mean_std needs CUDA tensors; there is no CPU fallback")
+    if S.dim() != 2 or S.dtype != torch.float32 or S.stride(1) != 1:
+        raise RuntimeError(f"topk_mean_std: expected a row-major fp32 (rows, cols) tensor, got {S.dtype} {tuple(S.shape)}")
+    rows, cols = S.shape
+    mean = torch.empty(rows, device=S.device, dtype=torch.float32)
+    std = torch.empty_like(mean)
+    with torch.cuda.device(S.device):
+        L.check(L.load().dsk_topk_mean_std(S.data_ptr(), rows, cols, S.stride(0), int(k), mean.data_ptr(),
+                                           std.data_ptr(), L.cur_stream()), "dsk_topk_mean_std")
+    return mean, std
+
+
+def cohort_stats(E, cohort, k):
+    """dsk_cohort_stats: (mean, std) (M,) of the k largest cosines of every row of E against the cohort."""
+    E, C = _score_pair(E, cohort, "cohort_stats")
+    (M, D), Nc = E.shape, C.shape[0]
+    mean = torch.empty(M, device=E.device, dtype=torch.float32)
+    std = torch.empty_like(mean)
+    with torch.cuda.device(E.device):
+        L.check(L.load().dsk_cohort_stats(_allpairs_handle(E.device), E.data_ptr(), M, C.data_ptr(), Nc, D, int(k),
+                                          mean.data_ptr(), std.data_ptr(), L.cur_stream()), "dsk_cohort_stats")
+    return mean, std
+
+
+def score_trials(X, trials, mean=None, std=None):
+    """dsk_score_trials: (raw (T,), normed (T,) or None) for trials (T, 2) of row indices into X (U, D); ``mean`` /
+    ``std`` (U,) are the rows' cohort statistics (AS-norm), or None for raw scores only."""
+    X = _score_rows(X, "score_trials")
+    trials = torch.as_tensor(trials)
+    if trials.dim() != 2 or trials.shape[1] != 2 or trials.shape[0] < 1:
+        raise RuntimeError(f"score_trials: expected trials of shape (T, 2) with T >= 1, got {tuple(trials.shape)}")
+    trials = trials.to(device=X.device, dtype=torch.int64).contiguous()
+    (U, D), T = X.shape, trials.shape[0]
+    if (mean is None) != (std is None):
+        raise RuntimeError("score_trials: give both mean and std, or neither")
+    if mean is not None:
+        mean, std = (t.detach().to(device=X.device, dtype=torch.float32).contiguous() for t in (mean, std))
+        if mean.shape != (U,) or std.shape != (U,):
+            raise RuntimeError(f"score_trials: expected mean and std of shape ({U},)")
+    raw = torch.empty(T, device=X.device, dtype=torch.float32)
+    normed = None if mean is None else torch.empty_like(raw)
+    with torch.cuda.device(X.device):
+        L.check(L.load().dsk_score_trials(X.data_ptr(), U, D, trials.data_ptr(), T, L.ptr(mean), L.ptr(std),
+                                          raw.data_ptr(), L.ptr(normed), L.cur_stream()), "dsk_score_trials")
+    return raw, normed

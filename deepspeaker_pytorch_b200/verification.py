@@ -7,6 +7,10 @@ Distances come from the CUDA kernels (eval forward + PairwiseDistance).  ``evalu
 numpy pass over the distance array each in the reference) are ONE counting kernel launch each (``dsk_threshold_counts``,
 exact numpy comparison semantics); the handful of scalar operations that follow (argmax, the interpolation of the FAR
 curve) stay on the host as in the reference.  ``sweep`` (accuracy + the derived EER) keeps its numpy form for host arrays.
+
+For embeddings scored by cosine similarity (higher = same speaker, e.g. trained with ``AAMSoftmaxLoss``):
+``cosine_matrix``, ``cohort_stats`` and ``score_trials`` (AS-norm against an impostor cohort) run on the GPU, and
+``eer_min_dcf`` computes the exact EER and minDCF over every distinct score on the host.
 """
 from __future__ import annotations
 
@@ -14,6 +18,7 @@ import numpy as np
 import torch
 
 from . import _lib as L
+from . import engine
 from .model import PairwiseDistance
 
 
@@ -118,3 +123,66 @@ def val_threshold(far_train, thresholds, far_target):
     if far_target <= x[0]:
         return float(y[0])
     return float(np.interp(far_target, x, y))
+
+
+# ---------------------------------------------------------------------------------------------------
+# Cosine scoring with adaptive score normalisation (AS-norm) and exact EER / minDCF: the usual evaluation of embeddings
+# trained with a cosine classifier (AAMSoftmaxLoss), where a higher score means the same speaker.
+# ---------------------------------------------------------------------------------------------------
+def cosine_matrix(A: torch.Tensor, B: torch.Tensor) -> torch.Tensor:
+    """(M, Nc) fp32 cosines between the rows of A (M, D) and B (Nc, D) (CUDA tensors; D a multiple of 64)."""
+    return engine.cosine_matrix(A, B)
+
+
+def cohort_stats(emb: torch.Tensor, cohort: torch.Tensor, topk: int = 300):
+    """(mean, std), (M,) fp32 on the device: mean and standard deviation (divisor topk - 1) of the ``topk`` largest
+    cosines of each row of ``emb`` (M, D) against the impostor cohort (Nc, D); 2 <= topk <= Nc (topk = Nc: S-norm)."""
+    return engine.cohort_stats(emb, cohort, topk)
+
+
+def score_trials(emb: torch.Tensor, trials, cohort: torch.Tensor = None, topk: int = 300):
+    """(raw, normed) (T,) fp32 scores of trials (T, 2) of row indices (enrolment, test) into the embedding table ``emb``
+    (U, D): raw = the cosine, normed = its AS-norm 0.5 ((s - mu_e) / sigma_e + (s - mu_t) / sigma_t) with every row's
+    statistics against ``cohort`` (``cohort_stats``); normed is None without a cohort.  An index outside [0, U) gives
+    NaN."""
+    mean = std = None
+    if cohort is not None:
+        mean, std = engine.cohort_stats(emb, cohort, topk)
+    return engine.score_trials(emb, trials, mean, std)
+
+
+def eer_min_dcf(scores, targets, p_target: float = 0.01, c_miss: float = 1.0, c_fa: float = 1.0):
+    """(EER, minDCF) of ``scores`` (higher = same speaker) with boolean ``targets``, exact over every distinct score.
+
+    The operating points are the sorted distinct scores plus +inf; P_miss(t) = #{target, s < t} / n_tar and
+    P_fa(t) = #{non-target, s >= t} / n_non.  EER interpolates P_miss - P_fa as ``sweep`` does: at the first point where
+    P_miss >= P_fa, linearly from the previous point, and averages the two interpolated rates.  minDCF is the minimum over
+    the same points of (c_miss P_miss p + c_fa P_fa (1 - p)) / min(c_miss p, c_fa (1 - p)).  Host numpy, one sort.
+    Raises ValueError without target or non-target trials, or for a score that is not finite."""
+    s = (scores.detach().cpu().double().numpy() if isinstance(scores, torch.Tensor)
+         else np.asarray(scores, dtype=np.float64)).reshape(-1)
+    y = (targets.detach().cpu().numpy() if isinstance(targets, torch.Tensor) else np.asarray(targets)).reshape(-1)
+    y = y.astype(bool)
+    if s.shape != y.shape:
+        raise ValueError(f"scores and targets differ in length ({s.size} and {y.size})")
+    if not np.isfinite(s).all():
+        raise ValueError("every score must be finite")
+    n_tar = int(y.sum())
+    n_non = y.size - n_tar
+    if n_tar == 0 or n_non == 0:
+        raise ValueError(f"need target and non-target trials (got {n_tar} and {n_non})")
+    if not (0.0 < p_target < 1.0) or not (c_miss > 0.0) or not (c_fa > 0.0):
+        raise ValueError("need 0 < p_target < 1, c_miss > 0 and c_fa > 0")
+    order = np.argsort(s, kind="stable")
+    s, y = s[order], y[order]
+    cum_tar = np.concatenate(([0], np.cumsum(y)))                # targets among the i lowest scores
+    first = np.flatnonzero(np.concatenate(([True], s[1:] != s[:-1])))
+    idx = np.concatenate((first, [s.size]))                      # scores below each operating point; +inf last
+    p_miss = cum_tar[idx] / n_tar
+    p_fa = (n_non - (idx - cum_tar[idx])) / n_non
+    diff = p_miss - p_fa                                         # -1 at the lowest score, +1 at +inf
+    i = int(np.argmax(diff >= 0))
+    w = -diff[i - 1] / (diff[i] - diff[i - 1]) if diff[i] != diff[i - 1] else 0.0
+    eer = float((p_miss[i - 1] + w * (p_miss[i] - p_miss[i - 1]) + p_fa[i - 1] + w * (p_fa[i] - p_fa[i - 1])) / 2)
+    dcf = (c_miss * p_miss * p_target + c_fa * p_fa * (1.0 - p_target)) / min(c_miss * p_target, c_fa * (1.0 - p_target))
+    return eer, float(dcf.min())

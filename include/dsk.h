@@ -336,6 +336,41 @@ int32_t dsk_aam_softmax_bwd(dsk_handle h, const float* E, const float* W, const 
                             const float* lse, int32_t N, int32_t C, int32_t D, float margin, float scale,
                             const float* grad_loss, float* gE, float* gW, void* stream);
 
+/* Cosine scoring of verification trials with adaptive symmetric score normalisation (AS-norm) against an impostor
+ * cohort (no reference implementation exists; the reference scores Euclidean distances, eval_metrics.py:5-50).  Rows are
+ * normalised as in F.normalize, x^ = x / max(||x||, 1e-12).
+ *   dsk_cosine_matrix: cos (M,Nc) = a^_i . b^_j for A (M,D) and B (Nc,D), fp32 out.
+ *   dsk_topk_mean_std: for every row r of S (rows x cols, row stride ld floats), tau = its k-th largest value and the
+ *     multiset of every value > tau plus as many copies of tau as make k values (independent of tie breaking);
+ *     mean[r] = its mean, std[r] = its standard deviation with divisor k - 1 (torch.std), both accumulated in fp64 in a
+ *     fixed order as two passes (mean, then sum (x - mean)^2) and rounded to fp32.  A row with a NaN gives NaN for both;
+ *     +-inf and +-0 are ordered as numbers.  One CTA per row: an exact radix select of tau on order-preserving uint32
+ *     keys (shared-memory histograms), the row staged in shared memory when cols <= 16384.  No float atomics.
+ *   dsk_cohort_stats: mean, std (M,) of the k largest cosines of each row of E (M,D) against the cohort (Nc,D) (k = Nc:
+ *     plain S-norm); bit-identical to dsk_topk_mean_std(dsk_cosine_matrix(E, cohort)).
+ * The cosines run on the tensor cores as the AAM-softmax op's do (fp16 whatever the handle's type, each operand split
+ * into hi + lo halves, K = 3D).  E is processed in row chunks: rows per chunk = the largest multiple of 128 with
+ * chunk x Npad x 4 B <= 256 MiB (Npad = Nc rounded up to 128), at least 128, and no more than M rounded up to 128.
+ * Every chunk reuses one operand buffer and one set of GEMM launches in stream order, and each row's outputs depend only
+ * on that row and the cohort: they are bit-identical whatever M, wherever the row sits and however E is split.  The
+ * plan is cached in h for (Nc, D, chunk), in a slot of its own (the all-pairs, batch-hard and AAM plans are untouched);
+ * a change rebuilds it, which synchronises the stream.  The cohort's operand image is rebuilt on every call.
+ * M >= 1, 2 <= Nc <= DSK_SCORE_MAX_COHORT, 2 <= k <= Nc, D % 64 == 0, else DSK_ERR_INVALID. */
+#define DSK_SCORE_MAX_COHORT 65536
+int32_t dsk_cosine_matrix(dsk_handle h, const float* A, int32_t M, const float* B, int32_t Nc, int32_t D, float* cos,
+                          void* stream);
+int32_t dsk_topk_mean_std(const float* S, int32_t rows, int32_t cols, int64_t ld, int32_t k, float* mean, float* std,
+                          void* stream);
+int32_t dsk_cohort_stats(dsk_handle h, const float* E, int32_t M, const float* cohort, int32_t Nc, int32_t D,
+                         int32_t k, float* mean, float* std, void* stream);
+/* Trial scores: trials (T,2) int64 (e, t) index rows of one embedding table X (U,D).  raw[i] = x^_e . x^_t in fp64 from
+ * the fp32 inputs, rounded to fp32; with mean / std (U,) given (dsk_cohort_stats of X), normed[i] = 0.5 ((s - mean_e) /
+ * std_e + (s - mean_t) / std_t) in fp64 from the unrounded s (AS-norm; std = 0 gives what IEEE division gives).  mean and
+ * std may both be NULL, and then normed is not written.  An index outside [0, U) gives NaN in both outputs and reads
+ * nothing.  One warp per trial, fixed order. */
+int32_t dsk_score_trials(const float* X, int32_t U, int32_t D, const int64_t* trials, int64_t T, const float* mean,
+                         const float* std, float* raw, float* normed, void* stream);
+
 /* nn.Linear of DeepSpeakerModel.forward_classifier (reference model.py:167,220-223): y (M,N) = x (M,K) w(N,K)^T + b.
  * fp32 on the CUDA cores, fixed summation order (deterministic).  b may be NULL. */
 int32_t dsk_linear_forward(const float* x, const float* w, const float* b, int32_t M, int32_t N, int32_t K, float* y,
