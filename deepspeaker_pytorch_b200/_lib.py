@@ -174,6 +174,9 @@ SIGNATURES = {
     "dsk_topk_mean_std": (c_int32, [c_void_p, c_int32, c_int32, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
     "dsk_cohort_stats": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_int32] + [c_void_p] * 3),
     "dsk_score_trials": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_int64] + [c_void_p] * 5),
+    "dsk_topk_indices": (c_int32, [c_void_p, c_int32, c_int32, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
+    "dsk_cosine_topk": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_int32] + [c_void_p] * 3),
+    "dsk_class_centroids": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),
     "dsk_linear_forward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     "dsk_linear_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p,
                                       c_void_p, c_void_p]),

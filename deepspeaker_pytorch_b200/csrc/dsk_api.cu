@@ -282,6 +282,7 @@ struct dsk_handle_s {
   std::vector<ConvLaunch> ap_gemm;
   AamPlan aam;                 // cached AAM-softmax plan (its own slot: a step may use both ops)
   ScorePlan score;             // cached cosine-scoring plan (its own slot: evaluation runs between training steps)
+  ScorePlan search;            // cached gallery-search plan (its own slot: searches alternate with cohort statistics)
   bool n256 = false;           // DSK_N256=1: 256-channel tiles for layers with >= n256_min_tiles such tiles
   int n256_min_tiles = 80;
   bool use_graph = true;       // DSK_GRAPH=0: always launch the forward kernel by kernel
@@ -1091,6 +1092,7 @@ int32_t dsk_destroy(dsk_handle h) {
   cudaFree(h->ap_buf);
   cudaFree(h->aam.buf);
   cudaFree(h->score.buf);
+  cudaFree(h->search.buf);
   cudaFree(h->ones);
   cudaFree(h->zeros);
   for (dsk_train_ctx_s* c : h->ctx_pool) {
@@ -2799,9 +2801,9 @@ static int score_chunk_rows(int M, int Np) {
   return static_cast<int>(m < c ? m : c);
 }
 
-// (Re)build the handle's scoring plan for (Nc, D, chunk).  A rebuild synchronises `s` (buffers in use are freed).
-static int score_plan(dsk_handle h, int M, int Nc, int D, cudaStream_t s, ScorePlan** out) {
-  ScorePlan& P = h->score;
+// (Re)build the scoring plan in slot P of h (h->score or h->search) for (Nc, D, chunk).  A rebuild synchronises `s`
+// (buffers in use are freed).
+static int score_plan(dsk_handle h, ScorePlan& P, int M, int Nc, int D, cudaStream_t s, ScorePlan** out) {
   *out = &P;
   const int Np = (Nc + 127) / 128 * 128, chunk = score_chunk_rows(M, Np);
   if (P.buf && P.Nc == Nc && P.D == D && P.chunk == chunk) return DSK_OK;
@@ -2841,11 +2843,12 @@ static int score_check(dsk_handle h, bool ptrs_ok, int M, int Nc, int D, int k, 
   return check_handle(h);
 }
 
-// The cohort's norms and B-side operand image, rebuilt on every call
-static int score_prep_cohort(const ScorePlan& P, const float* B, cudaStream_t s) {
-  dsk::aam_norm_kernel<<<(P.Nc + 7) / 8, 256, 0, s>>>(B, P.Nc, P.D, P.nrm_c);
+// The norms and B-side operand image of the cohort's rows B (cols <= P.Nc of them; rows [cols, Np) are zero), rebuilt
+// on every call
+static int score_prep_cohort(const ScorePlan& P, const float* B, int cols, cudaStream_t s) {
+  dsk::aam_norm_kernel<<<(cols + 7) / 8, 256, 0, s>>>(B, cols, P.D, P.nrm_c);
   KERNEL_CHECK();
-  dsk::aam_split_kernel<<<dim3(P.D / 64, P.Np / 32), 256, 0, s>>>(B, P.nrm_c, P.Nc, P.Np, P.D, 0, P.cb, nullptr);
+  dsk::aam_split_kernel<<<dim3(P.D / 64, P.Np / 32), 256, 0, s>>>(B, P.nrm_c, cols, P.Np, P.D, 0, P.cb, nullptr);
   KERNEL_CHECK();
   return DSK_OK;
 }
@@ -2880,8 +2883,8 @@ int32_t dsk_cosine_matrix(dsk_handle h, const float* A, int32_t M, const float* 
   if (rc) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   ScorePlan* P = nullptr;
-  if ((rc = score_plan(h, M, Nc, D, s, &P))) return rc;
-  if ((rc = score_prep_cohort(*P, B, s))) return rc;
+  if ((rc = score_plan(h, h->score, M, Nc, D, s, &P))) return rc;
+  if ((rc = score_prep_cohort(*P, B, Nc, s))) return rc;
   for (int r0 = 0; r0 < M; r0 += P->chunk) {
     const int rows = M - r0 < P->chunk ? M - r0 : P->chunk;
     if ((rc = score_gemm_chunk(*P, A + static_cast<size_t>(r0) * D, rows, s))) return rc;
@@ -2906,8 +2909,8 @@ int32_t dsk_cohort_stats(dsk_handle h, const float* E, int32_t M, const float* c
   if (rc) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   ScorePlan* P = nullptr;
-  if ((rc = score_plan(h, M, Nc, D, s, &P))) return rc;
-  if ((rc = score_prep_cohort(*P, cohort, s))) return rc;
+  if ((rc = score_plan(h, h->score, M, Nc, D, s, &P))) return rc;
+  if ((rc = score_prep_cohort(*P, cohort, Nc, s))) return rc;
   for (int r0 = 0; r0 < M; r0 += P->chunk) {
     const int rows = M - r0 < P->chunk ? M - r0 : P->chunk;
     if ((rc = score_gemm_chunk(*P, E + static_cast<size_t>(r0) * D, rows, s))) return rc;
@@ -2926,6 +2929,85 @@ int32_t dsk_score_trials(const float* X, int32_t U, int32_t D, const int64_t* tr
   const unsigned blocks = static_cast<unsigned>((T + dsk::kScoreWarps - 1) / dsk::kScoreWarps);
   dsk::score_trials_kernel<<<blocks, 32 * dsk::kScoreWarps, 0, static_cast<cudaStream_t>(stream)>>>(
       X, U, D, trials, static_cast<long long>(T), stats ? mean : nullptr, std, raw, normed);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// ---- identification: gallery search, class centroids -------------------------------------------------------------
+static int launch_topk_indices(const float* S, int rows, int cols, long ld, int k, long long col0, int64_t* idx,
+                               float* val, long ldo, cudaStream_t s) {
+  if (cols <= dsk::kTopkStageCols) {
+    const int smem = cols * 4;
+    auto kern = dsk::topk_indices_kernel<true>;
+    if (int rc = ensure_smem_optin(reinterpret_cast<const void*>(kern), smem)) return rc;
+    kern<<<rows, dsk::kTopkThreads, smem, s>>>(S, cols, ld, k, col0, idx, val, ldo);
+  } else {
+    dsk::topk_indices_kernel<false><<<rows, dsk::kTopkThreads, 0, s>>>(S, cols, ld, k, col0, idx, val, ldo);
+  }
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_topk_indices(const float* S, int32_t rows, int32_t cols, int64_t ld, int32_t k, int64_t* idx, float* val,
+                         void* stream) {
+  if (!S || !idx || !val || rows < 1 || cols < 1 || cols > DSK_SCORE_MAX_COHORT || ld < cols || k < 1 || k > cols ||
+      k > DSK_SEARCH_MAX_K)
+    return fail(DSK_ERR_INVALID, "dsk_topk_indices: bad arguments (need non-null pointers, rows >= 1, 1 <= cols <= %d, "
+                "ld >= cols, 1 <= k <= min(cols, %d); got rows %d, cols %d, ld %lld, k %d)", DSK_SCORE_MAX_COHORT,
+                DSK_SEARCH_MAX_K, rows, cols, static_cast<long long>(ld), k);
+  return launch_topk_indices(S, rows, cols, static_cast<long>(ld), k, 0, idx, val, k, static_cast<cudaStream_t>(stream));
+}
+
+// Gallery columns per search chunk: every selection runs on a row staged in shared memory
+static_assert(dsk::kSearchMaxK == DSK_SEARCH_MAX_K && dsk::kSearchMaxK <= dsk::kTopkStageCols,
+              "the first gallery chunk holds at least k columns");
+
+int32_t dsk_cosine_topk(dsk_handle h, const float* Q, int32_t M, const float* G, int32_t Ng, int32_t D, int32_t k,
+                        int64_t* idx, float* val, void* stream) {
+  if (!Q || !G || !idx || !val || M < 1 || k < 1 || k > DSK_SEARCH_MAX_K || Ng < k || D < 64 || D % 64)
+    return fail(DSK_ERR_INVALID, "dsk_cosine_topk: bad arguments (need non-null pointers, M >= 1, 1 <= k <= %d, Ng >= k, "
+                "D a positive multiple of 64; got M %d, Ng %d, D %d, k %d)", DSK_SEARCH_MAX_K, M, Ng, D, k);
+  int rc = check_handle(h);
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int width = Ng < dsk::kTopkStageCols ? Ng : dsk::kTopkStageCols;
+  ScorePlan* P = nullptr;
+  if ((rc = score_plan(h, h->search, M, width, D, s, &P))) return rc;
+  // later chunks select into (wi, wv) [chunk][k] and are merged into the caller's running lists
+  int64_t* wi = nullptr;
+  float* wv = nullptr;
+  if (Ng > width) {
+    CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&wi), static_cast<size_t>(P->chunk) * k * 12, s));
+    wv = reinterpret_cast<float*>(wi + static_cast<size_t>(P->chunk) * k);
+  }
+  for (long c0 = 0; c0 < Ng && !rc; c0 += width) {
+    const int cols = Ng - c0 < width ? static_cast<int>(Ng - c0) : width, kc = cols < k ? cols : k;
+    rc = score_prep_cohort(*P, G + static_cast<size_t>(c0) * D, cols, s);
+    for (int r0 = 0; r0 < M && !rc; r0 += P->chunk) {
+      const int rows = M - r0 < P->chunk ? M - r0 : P->chunk;
+      int64_t* oi = idx + static_cast<size_t>(r0) * k;
+      float* ov = val + static_cast<size_t>(r0) * k;
+      if ((rc = score_gemm_chunk(*P, Q + static_cast<size_t>(r0) * D, rows, s))) break;
+      if (c0 == 0) {
+        rc = launch_topk_indices(P->cos, rows, cols, P->Np, k, 0, oi, ov, k, s);
+      } else if (!(rc = launch_topk_indices(P->cos, rows, cols, P->Np, kc, c0, wi, wv, k, s))) {
+        dsk::topk_merge_kernel<<<rows, dsk::kTopkThreads, 0, s>>>(oi, ov, wi, wv, k, kc);
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) rc = fail(DSK_ERR_CUDA, "kernel launch failed: %s (topk_merge_kernel)", cudaGetErrorString(e));
+      }
+    }
+  }
+  if (wi) cudaFreeAsync(wi, s);
+  return rc;
+}
+
+int32_t dsk_class_centroids(const float* X, int32_t U, int32_t D, const int64_t* order, const int64_t* offsets,
+                            int32_t S, float* out, void* stream) {
+  if (!X || !order || !offsets || !out || U < 1 || D < 1 || S < 1)
+    return fail(DSK_ERR_INVALID, "dsk_class_centroids: bad arguments (need non-null pointers, U >= 1, D >= 1, S >= 1; got "
+                "U %d, D %d, S %d)", U, D, S);
+  dsk::class_centroids_kernel<<<dim3(S, (D + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(X, U, D, order,
+                                                                                                       offsets, out);
   KERNEL_CHECK();
   return DSK_OK;
 }

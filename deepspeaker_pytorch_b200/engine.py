@@ -525,3 +525,53 @@ def score_trials(X, trials, mean=None, std=None):
         L.check(L.load().dsk_score_trials(X.data_ptr(), U, D, trials.data_ptr(), T, L.ptr(mean), L.ptr(std),
                                           raw.data_ptr(), L.ptr(normed), L.cur_stream()), "dsk_score_trials")
     return raw, normed
+
+
+# ---------------------------------------------------------------------------------------------------
+# identification: exact top-k search, class centroids
+# ---------------------------------------------------------------------------------------------------
+def topk_indices(S, k):
+    """dsk_topk_indices: (idx int64 (rows, k), val fp32 (rows, k)) of the k first columns of every row of S (rows, cols)
+    in the search order (descending, ties to the lower column, -0 == +0, NaN last); the row stride is kept."""
+    if not S.is_cuda:
+        raise RuntimeError("topk_indices needs CUDA tensors; there is no CPU fallback")
+    if S.dim() != 2 or S.dtype != torch.float32 or S.stride(1) != 1:
+        raise RuntimeError(f"topk_indices: expected a row-major fp32 (rows, cols) tensor, got {S.dtype} {tuple(S.shape)}")
+    rows, cols = S.shape
+    k = int(k)
+    idx = torch.empty(rows, max(k, 0), device=S.device, dtype=torch.int64)
+    val = torch.empty(rows, max(k, 0), device=S.device, dtype=torch.float32)
+    with torch.cuda.device(S.device):
+        L.check(L.load().dsk_topk_indices(S.data_ptr(), rows, cols, S.stride(0), k, idx.data_ptr(), val.data_ptr(),
+                                          L.cur_stream()), "dsk_topk_indices")
+    return idx, val
+
+
+def cosine_topk(Q, G, k):
+    """dsk_cosine_topk: (idx int64 (M, k), val fp32 (M, k)) of the k largest cosines of every row of Q (M, D) against
+    the gallery G (Ng, D), any Ng >= k, in the search order; val is the cosine cosine_matrix gives for the pair."""
+    Q, G = _score_pair(Q, G, "cosine_topk")
+    (M, D), Ng, k = Q.shape, G.shape[0], int(k)
+    idx = torch.empty(M, max(k, 0), device=Q.device, dtype=torch.int64)
+    val = torch.empty(M, max(k, 0), device=Q.device, dtype=torch.float32)
+    with torch.cuda.device(Q.device):
+        L.check(L.load().dsk_cosine_topk(_allpairs_handle(Q.device), Q.data_ptr(), M, G.data_ptr(), Ng, D, k,
+                                         idx.data_ptr(), val.data_ptr(), L.cur_stream()), "dsk_cosine_topk")
+    return idx, val
+
+
+def class_centroids(X, order, offsets):
+    """dsk_class_centroids: (S, D) fp32 mean of the normalised rows X[order[offsets[s]:offsets[s+1]]] per class s, in
+    fp64 in that order; ``order`` / ``offsets`` (S + 1,) are int64 (a CSR of the classes' rows)."""
+    X = _score_rows(X, "class_centroids")
+    order = torch.as_tensor(order).to(device=X.device, dtype=torch.int64).contiguous()
+    offsets = torch.as_tensor(offsets).to(device=X.device, dtype=torch.int64).contiguous()
+    if order.dim() != 1 or offsets.dim() != 1 or offsets.numel() < 2:
+        raise RuntimeError(f"class_centroids: expected 1-D order and offsets with >= 2 entries, got "
+                           f"{tuple(order.shape)} and {tuple(offsets.shape)}")
+    (U, D), S = X.shape, offsets.numel() - 1
+    out = torch.empty(S, D, device=X.device, dtype=torch.float32)
+    with torch.cuda.device(X.device):
+        L.check(L.load().dsk_class_centroids(X.data_ptr(), U, D, order.data_ptr(), offsets.data_ptr(), S,
+                                             out.data_ptr(), L.cur_stream()), "dsk_class_centroids")
+    return out

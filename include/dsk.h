@@ -371,6 +371,38 @@ int32_t dsk_cohort_stats(dsk_handle h, const float* E, int32_t M, const float* c
 int32_t dsk_score_trials(const float* X, int32_t U, int32_t D, const int64_t* trials, int64_t T, const float* mean,
                          const float* std, float* raw, float* normed, void* stream);
 
+/* Speaker identification: exact top-k cosine search against an enrolled gallery of any size (no reference
+ * implementation exists).  The search order ranks a above b when a > b as numbers, ties going to the lower column;
+ * -0 == +0, and NaN ranks below every number (-inf included), so one corrupt gallery row never becomes every query's
+ * top-1.  idx / val are (rows, k) row-major: the k first columns of each row in that order and their values (the
+ * input's bits).
+ *   dsk_topk_indices: the search order over every row r of S (rows x cols, row stride ld floats).  One CTA per row: the
+ *     k-th key by the exact radix select of dsk_topk_mean_std, every column above it plus the lowest columns equal to
+ *     it (an ordered compaction), a bitonic sort of the k entries in shared memory.  The row is staged in shared memory
+ *     when cols <= 16384.  1 <= k <= min(cols, DSK_SEARCH_MAX_K), cols <= DSK_SCORE_MAX_COHORT, ld >= cols.
+ *   dsk_cosine_topk: the search order over the row of cosines of query i of Q (M,D) against the gallery G (Ng,D), for
+ *     any Ng >= k.  val is exactly the fp32 cosine dsk_cosine_matrix gives for that pair, so the result equals
+ *     dsk_topk_indices of dsk_cosine_matrix(Q, G) for Ng <= DSK_SCORE_MAX_COHORT, and of dsk_cosine_matrix of column
+ *     slices, concatenated, beyond.  The gallery is taken in column chunks of 16384 rows in ascending order, each with
+ *     its operand image built once; the queries in row chunks as in dsk_cohort_stats (Npad = 16384, or Ng rounded up to
+ *     128 for a smaller gallery).  Each chunk's k best are merged into idx / val, which hold the running lists; the
+ *     workspace is one row chunk x k entries (stream-ordered allocation).  A query's result depends only on that query
+ *     and G: bit-identical whatever M and wherever the row sits.  The plan is cached in h in a slot of its own (the
+ *     scoring, all-pairs, batch-hard and AAM plans are untouched); a change rebuilds it, which synchronises the stream.
+ *     M >= 1, 1 <= k <= DSK_SEARCH_MAX_K, Ng >= k, D % 64 == 0.
+ *   dsk_class_centroids: enrolment.  out[s] (S,D) = (1/n_s) * the sum of x^_u over u = order[offsets[s] ..
+ *     offsets[s+1]), with x^_u = X[u] / max(||X[u]||, 1e-12) in fp64 from the fp32 row, summed in fp64 in that order
+ *     and rounded to fp32; n_s = offsets[s+1] - offsets[s].  An empty segment gives a zero row, an index outside [0, U)
+ *     a NaN row.  One CTA per class and 256 columns, no float atomics.  order, offsets (S+1) are device int64.
+ * Arguments outside these limits return DSK_ERR_INVALID. */
+#define DSK_SEARCH_MAX_K 1024
+int32_t dsk_topk_indices(const float* S, int32_t rows, int32_t cols, int64_t ld, int32_t k, int64_t* idx, float* val,
+                         void* stream);
+int32_t dsk_cosine_topk(dsk_handle h, const float* Q, int32_t M, const float* G, int32_t Ng, int32_t D, int32_t k,
+                        int64_t* idx, float* val, void* stream);
+int32_t dsk_class_centroids(const float* X, int32_t U, int32_t D, const int64_t* order, const int64_t* offsets,
+                            int32_t S, float* out, void* stream);
+
 /* nn.Linear of DeepSpeakerModel.forward_classifier (reference model.py:167,220-223): y (M,N) = x (M,K) w(N,K)^T + b.
  * fp32 on the CUDA cores, fixed summation order (deterministic).  b may be NULL. */
 int32_t dsk_linear_forward(const float* x, const float* w, const float* b, int32_t M, int32_t N, int32_t K, float* y,
