@@ -113,6 +113,18 @@ class DskGrads(ctypes.Structure):
     ]
 
 
+class DskBackwardCapture(ctypes.Structure):
+    _fields_ = [
+        ("gy", c_void_p * NUM_CONV),
+        ("G", c_void_p * NUM_CONV),
+        ("gres", c_void_p * NUM_CONV),
+        ("g_fc", c_void_p),
+        ("fc_out", c_void_p),
+        ("dP", c_void_p),
+        ("loss_scale", c_void_p),
+    ]
+
+
 # name -> (restype, argtypes); must list every symbol declared in include/dsk.h
 SIGNATURES = {
     "dsk_last_error": (c_char_p, []),
@@ -126,6 +138,7 @@ SIGNATURES = {
     "dsk_rescnn_forward_train": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, POINTER(c_void_p), c_void_p]),
     "dsk_rescnn_backward": (c_int32, [c_void_p, c_void_p, c_void_p, POINTER(DskGrads), c_void_p]),
     "dsk_train_ctx_read": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p]),
+    "dsk_debug_backward_plan": (c_int32, [c_void_p, c_void_p, c_int32, POINTER(c_int32)]),
     "dsk_debug_read_eval_activation": (c_int32, [c_void_p, c_int32, c_void_p, c_int64, POINTER(c_int32), c_void_p]),
     "dsk_train_ctx_release": (c_int32, [c_void_p, c_void_p]),
     "dsk_set_loss_scale": (c_int32, [c_void_p, c_float]),
@@ -147,6 +160,7 @@ SIGNATURES = {
     "dsk_conv3x3_padded": (c_int32, [c_void_p] * 7 + [c_int32, c_int32, c_int32, c_int32, c_int32, c_float, c_int32, c_void_p]),
     "dsk_conv5x5s2_planar": (c_int32, [c_void_p] * 6 + [c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_float, c_void_p]),
     "dsk_debug_set_trace": (c_int32, [c_void_p, c_void_p]),
+    "dsk_debug_set_backward_capture": (c_int32, [c_void_p, POINTER(DskBackwardCapture)]),
     "dsk_padded_positions": (c_int64, [c_int32, c_int32, c_int32]),
     "dsk_pack_conv_weight": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]),
     "dsk_nchw_f32_to_nhwc16": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p]),

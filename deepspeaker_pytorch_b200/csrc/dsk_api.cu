@@ -294,6 +294,8 @@ struct dsk_handle_s {
   bool small_cta = false;      // DSK_SMALL_CTA=1: 128-channel-tile halo convs as two 256-thread CTAs per SM (64-position tiles)
   bool planar_s2 = true;       // eval forward: run the 5x5 s2 convs in the halo kernel's parity-planar form (DSK_PLANAR_S2=0: generic kernel)
   long long* trace = nullptr;  // debug: device buffer [3][512] for conv3x3_halo_kernel clock stamps
+  bool bwd_capture_on = false; // debug: dsk_debug_set_backward_capture
+  dsk_backward_capture bwd_capture = {};
   // optional per-launch timing (dsk_set_profiling): events recorded around every kernel of a forward
   int profiling = 0;  // 0 off, 1 per launch, 2 per section
   std::vector<cudaEvent_t> events;
@@ -1755,6 +1757,46 @@ int32_t dsk_train_ctx_commit_stats(dsk_handle h, dsk_train_ctx c, void* stream) 
   return DSK_OK;
 }
 
+// ---- dsk_debug_set_backward_capture: copies of the backward's intermediate tensors -----------------------------------
+static int capture_copy(void* dst, const void* src, size_t bytes, cudaStream_t s) {
+  if (dst) CUDA_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s));
+  return DSK_OK;
+}
+
+// the l2-norm backward's input and output
+static int capture_gfc(dsk_handle h, const dsk_train_ctx_s* c, cudaStream_t s) {
+  if (!h->bwd_capture_on) return DSK_OK;
+  const size_t n = static_cast<size_t>(c->B) * h->emb * 4;
+  int rc = capture_copy(h->bwd_capture.g_fc, c->g_fc, n, s);
+  return rc ? rc : capture_copy(h->bwd_capture.fc_out, c->fc_out, n, s);
+}
+
+// the loss scale and the fc input gradient
+static int capture_head(dsk_handle h, const dsk_train_ctx_s* c, cudaStream_t s) {
+  if (!h->bwd_capture_on) return DSK_OK;
+  int rc = capture_copy(h->bwd_capture.loss_scale, c->ls, 2 * 4, s);
+  return rc ? rc : capture_copy(h->bwd_capture.dP, c->dP, static_cast<size_t>(c->B) * 2048 * 4, s);
+}
+
+// layer i's BatchNorm backward: its input gradient gy (before) or its outputs G and gres (after)
+static int capture_layer(dsk_handle h, const dsk_train_ctx_s* c, int i, bool after, cudaStream_t s) {
+  if (!h->bwd_capture_on) return DSK_OK;
+  int H, W, C;
+  act_shape(i, c->T, H, W, C);
+  const size_t bytes = static_cast<size_t>(c->B) * H * W * C * 2;
+  if (!after)
+    return capture_copy(h->bwd_capture.gy[i], ((DSK_NUM_CONV - 1 - i) % 2 == 0) ? c->gA : c->gB, bytes, s);
+  int rc = capture_copy(h->bwd_capture.G[i], c->G, bytes, s);
+  return (rc || i % 3 != 2) ? rc : capture_copy(h->bwd_capture.gres[i], c->gres, bytes, s);
+}
+
+int32_t dsk_debug_set_backward_capture(dsk_handle h, const dsk_backward_capture* cap) {
+  if (!h) return fail(DSK_ERR_INVALID, "null handle");
+  h->bwd_capture_on = cap != nullptr;
+  h->bwd_capture = cap ? *cap : dsk_backward_capture{};
+  return DSK_OK;
+}
+
 int32_t dsk_rescnn_backward(dsk_handle h, dsk_train_ctx c, const float* grad_emb, const dsk_grads* g, void* stream) {
   int rc = check_handle(h);
   if (rc) return rc;
@@ -1767,6 +1809,7 @@ int32_t dsk_rescnn_backward(dsk_handle h, dsk_train_ctx c, const float* grad_emb
   // tail
   dsk::l2norm_bwd_kernel<<<B, 128, 0, s>>>(c->fc_out, c->inv_norm, grad_emb, c->g_fc, E, 10.0f);
   KERNEL_CHECK();
+  if ((rc = capture_gfc(h, c, s))) return rc;
   // the loss scale of this backward: explicit (dsk_set_loss_scale), 1 for bf16 operands, else chosen on the device
   dsk::loss_scale_kernel<<<1, 1024, 0, s>>>(c->g_fc, static_cast<long>(B) * E, h->loss_scale > 0.f ? h->loss_scale : (bf ? 1.0f : 0.0f),
                                             c->ls);
@@ -1775,6 +1818,7 @@ int32_t dsk_rescnn_backward(dsk_handle h, dsk_train_ctx c, const float* grad_emb
   KERNEL_CHECK();
   dsk::fc_bwd_input_kernel<<<dim3(B, 2048 / 256), 256, E * 4, s>>>(c->g_fc, h->fc_wq, c->dP, 2048, E);
   KERNEL_CHECK();
+  if ((rc = capture_head(h, c, s))) return rc;
   {
     const int H4 = T / 16;
     if (bf) dsk::pool_bwd_kernel<true><<<B, 256, 0, s>>>(c->dP, (uint16_t*)c->gA, H4, 2048, 1.0f / H4, c->ls);
@@ -1786,6 +1830,7 @@ int32_t dsk_rescnn_backward(dsk_handle h, dsk_train_ctx c, const float* grad_emb
     act_shape(i, T, H, W, C);
     const long M = static_cast<long>(B) * H * W;
     const uint16_t* gy = (const uint16_t*)(((DSK_NUM_CONV - 1 - i) % 2 == 0) ? c->gA : c->gB);
+    if ((rc = capture_layer(h, c, i, false, s))) return rc;
     const int gx = stat_blocks(M, C);
     dim3 gs(gx, C / 64);
     if (bf)
@@ -1807,6 +1852,7 @@ int32_t dsk_rescnn_backward(dsk_handle h, dsk_train_ctx c, const float* grad_emb
       dsk::bn_bwd_apply_kernel<false><<<ga, 256, 0, s>>>(gy, (const uint16_t*)c->y[i], c->raw[i], c->mean[i],
                                                          c->rstd[i], c->coef, (uint16_t*)c->G, gres, M, C, 20.0f);
     KERNEL_CHECK();
+    if ((rc = capture_layer(h, c, i, true, s))) return rc;
     const LayerCfg lc = layer_cfg(i);
     if (i == 0) {
       const int nblk = B * ((T / 2 + 7) / 8);
@@ -1852,6 +1898,24 @@ int32_t dsk_train_ctx_read(dsk_handle h, dsk_train_ctx c, int32_t which, int32_t
   else
     dsk::nhwc16_to_nchw_kernel<false><<<blocks, 256, 0, s>>>((const uint16_t*)c->y[layer], out_nchw, c->B, C, H * W);
   KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_debug_backward_plan(dsk_handle h, dsk_train_ctx c, int32_t layer, int32_t* out) {
+  int rc = check_handle(h);
+  if (rc) return rc;
+  if (!c || !c->B) return fail(DSK_ERR_STATE, "dsk_debug_backward_plan: context is not bound to a batch");
+  if (layer < 0 || layer >= DSK_NUM_CONV || !out) return fail(DSK_ERR_INVALID, "dsk_debug_backward_plan: bad arguments");
+  int H, W, C;
+  act_shape(layer, c->T, H, W, C);
+  out[0] = out[1] = 0;
+  if (layer > 0) {
+    const dsk::WgradParams& p = c->wgrad[layer].p;
+    const int chunks = p.chunks_w * p.chunks_h * p.chunks_n;
+    out[0] = p.ksplit;
+    out[1] = (chunks + p.ksplit - 1) / p.ksplit;
+  }
+  out[2] = stat_blocks(static_cast<long>(c->B) * H * W, C);
   return DSK_OK;
 }
 
@@ -1988,6 +2052,7 @@ static int sync_bwd_stage(dsk_handle h, dsk_train_ctx_s* c, const float* gathere
     KERNEL_CHECK();
     dsk::fc_bwd_input_kernel<<<dim3(B, 2048 / 256), 256, E * 4, s>>>(c->g_fc, h->fc_wq, c->dP, 2048, E);
     KERNEL_CHECK();
+    if ((rc = capture_head(h, c, s))) return rc;
     const int H4 = T / 16;
     if (bf) dsk::pool_bwd_kernel<true><<<B, 256, 0, s>>>(c->dP, (uint16_t*)c->gA, H4, 2048, 1.0f / H4, c->ls);
     else dsk::pool_bwd_kernel<false><<<B, 256, 0, s>>>(c->dP, (uint16_t*)c->gA, H4, 2048, 1.0f / H4, c->ls);
@@ -2003,6 +2068,7 @@ static int sync_bwd_stage(dsk_handle h, dsk_train_ctx_s* c, const float* gathere
   act_shape(i, T, H, W, C);
   const long M = static_cast<long>(B) * H * W;
   const uint16_t* gy = (const uint16_t*)(((DSK_NUM_CONV - 1 - i) % 2 == 0) ? c->gA : c->gB);
+  if ((rc = capture_layer(h, c, i, false, s))) return rc;
   dsk::bn_bwd_record_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(gathered, N, c->rec, B, C, c->mtot + i, h->w.bn_gamma[i],
                                                                     c->rstd[i], c->ls, g->bn_gamma[i], g->bn_beta[i], c->coef);
   KERNEL_CHECK();
@@ -2015,6 +2081,7 @@ static int sync_bwd_stage(dsk_handle h, dsk_train_ctx_s* c, const float* gathere
     dsk::bn_bwd_apply_kernel<false><<<ga, 256, 0, s>>>(gy, (const uint16_t*)c->y[i], c->raw[i], c->mean[i], c->rstd[i], c->coef,
                                                        (uint16_t*)c->G, gres, M, C, 20.0f);
   KERNEL_CHECK();
+  if ((rc = capture_layer(h, c, i, true, s))) return rc;
   if (i == 0) {
     const int nblk = B * ((T / 2 + 7) / 8);
     if (bf) dsk::conv1_wgrad_partial_kernel<true><<<nblk, 256, 0, s>>>((const uint16_t*)c->G, c->x, B, T, c->c1part);
@@ -2086,6 +2153,7 @@ int32_t dsk_sync_backward_begin(dsk_handle h, dsk_train_ctx c, const float* grad
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   dsk::l2norm_bwd_kernel<<<c->B, 128, 0, s>>>(c->fc_out, c->inv_norm, grad_emb, c->g_fc, h->emb, 10.0f);
   KERNEL_CHECK();
+  if ((rc = capture_gfc(h, c, s))) return rc;
   dsk::row_absmax_kernel<<<c->B, 128, 0, s>>>(c->g_fc, h->emb, c->rec);
   KERNEL_CHECK();
   c->grads = *g;

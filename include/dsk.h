@@ -127,6 +127,11 @@ int32_t dsk_rescnn_backward(dsk_handle h, dsk_train_ctx ctx, const float* grad_e
 /* Debug / test read-back of what a train-mode forward saved: which = 0 the pre-BatchNorm conv output (fp32),
  * 1 the post-activation tensor (16-bit), of conv layer `layer` (0..11), converted to fp32 NCHW. */
 int32_t dsk_train_ctx_read(dsk_handle h, dsk_train_ctx ctx, int32_t which, int32_t layer, float* out_nchw, void* stream);
+/* Debug / test: the plan the backward of `ctx` (as bound by its last forward) uses for conv layer `layer` (0..11):
+ * out[0] = K splits of the weight-gradient GEMM, out[1] = 128-pixel chunks per split (both 0 for conv1),
+ * out[2] = partial-sum blocks per 64-channel group of the BatchNorm reductions (forward statistics and backward sums of
+ * the unsynchronised path).  Host-only: no device work. */
+int32_t dsk_debug_backward_plan(dsk_handle h, dsk_train_ctx ctx, int32_t layer, int32_t* out);
 /* Debug / test read-back: activation `layer` (0..11: output of conv `layer` after BN, residual and clip) of this handle's
  * most recent dsk_rescnn_forward, byte for byte as stored: 16-bit zero-padded NHWC (dsk_padded_positions(B,H,W) * C),
  * or parity-planar (4 planes of dsk_padded_positions(B,H/2,W/2) * C) for the block outputs that feed a stride-2 conv.
@@ -227,6 +232,24 @@ int64_t dsk_padded_positions(int32_t N, int32_t H, int32_t W);
 /* Debug: device buffer of 3*512 int64 that dsk_conv3x3_padded fills with clock64 stamps of CTA 0
  * (producer / MMA / epilogue roles); NULL switches tracing off. */
 int32_t dsk_debug_set_trace(dsk_handle h, void* device_buffer);
+/* Debug / test: copies of the intermediate tensors of a train backward, which otherwise live in buffers that the next
+ * layer overwrites.  Every non-NULL entry receives, by cudaMemcpyAsync on the backward's stream at the point where the
+ * tensor is final, B*H*W*C contiguous values (B, T, C, H, W of the context; layer i as act_shape: C = 64 << i/3,
+ * H = T >> (i/3 + 1), W = 64 >> (i/3 + 1); E the embedding size).  S is the backward's loss scale. */
+typedef struct {
+  void* gy[DSK_NUM_CONV];    /* 16-bit NHWC: gradient w.r.t. layer i's output y_i, times S, as the BatchNorm backward reads it */
+  void* G[DSK_NUM_CONV];     /* 16-bit NHWC: gradient w.r.t. the raw conv output raw_i (after the BatchNorm backward), times S */
+  void* gres[DSK_NUM_CONV];  /* 16-bit NHWC, i % 3 == 2 only: the skip-branch gradient (gy_i where 0 < y_i < 20, else 0) */
+  float* g_fc;               /* (B, E) fp32: the l2-norm backward's output, dL/d(fc output) */
+  float* fc_out;             /* (B, E) fp32: the saved fc output the l2-norm backward read */
+  float* dP;                 /* (B, 2048) fp32: gradient w.r.t. the pooled fc input, column w*512 + c, before the pool backward */
+  float* loss_scale;         /* 2 floats: {S, 1/S} of this backward */
+} dsk_backward_capture;
+/* Sets (copies *cap) or, with cap == NULL, clears the capture.  It stays set for every following dsk_rescnn_backward and
+ * synchronised backward (dsk_sync_backward_begin / dsk_sync_stage) of this handle; the caller keeps the buffers alive.
+ * Capturing adds copies only: no kernel and no result changes, and with the capture off the launches are those of a
+ * build without it. */
+int32_t dsk_debug_set_backward_capture(dsk_handle h, const dsk_backward_capture* cap);
 int32_t dsk_pack_conv_weight(dsk_handle h, const float* w_oihw, void* w_packed, int32_t cout, int32_t cin,
                              int32_t ksize, void* stream);
 /* fp32 NCHW <-> 16-bit NHWC converters (test helpers; also used at the boundary for C>1 inputs) */

@@ -68,11 +68,12 @@ def locate(viol, ratio):
 
 def check(name, got, ref, bound, saturating=True):
     """Every element within its bound.  Prints the largest err/bound (and, for clipped outputs, the fraction of the
-    reference strictly inside (0, 20)); returns (violation description or None, max err/bound, inside fraction)."""
-    ratio = (got.double() - ref).abs() / bound
+    reference strictly inside (0, 20)); returns (violation description or None, max err/bound, inside fraction).
+    A NaN anywhere (got, ref or bound) is a violation with err/bound = inf."""
+    ratio = torch.nan_to_num((got.double() - ref).abs() / bound, nan=float("inf"), posinf=float("inf"))
     worst = ratio.max().item()
     inside = ((ref > 0) & (ref < 20)).double().mean().item() if saturating else None
-    viol = ratio > 1.0
+    viol = ~(ratio <= 1.0)
     print(f"  {name:<12} max err/bound {worst:.3f}" + (f"   inside (0,20) {inside:.2f}" if saturating else ""))
     msg = locate(viol.cpu(), ratio.cpu()) if bool(viol.any()) else None
     return msg, worst, inside
