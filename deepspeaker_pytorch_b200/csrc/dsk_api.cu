@@ -316,7 +316,8 @@ struct dsk_train_ctx_s {
   float* mean[DSK_NUM_CONV] = {};
   float* rstd[DSK_NUM_CONV] = {};
   float* unb[DSK_NUM_CONV] = {};       // unbiased batch variance (what the running_var update consumes)
-  bool stats_pending = false;          // forward ran with deferred running statistics: dsk_train_ctx_commit_stats owes the update
+  bool stats_pending = false;          // the forward defers the running-statistics update (set at its start, both modes):
+                                       // dsk_train_ctx_commit_stats owes it
   float *pooled = nullptr, *fc_out = nullptr, *fc_part = nullptr, *inv_norm = nullptr;
   float *scale_t = nullptr, *shift_t = nullptr, *partial = nullptr, *coef = nullptr;
   float *g_fc = nullptr, *dP = nullptr, *dwacc = nullptr, *c1part = nullptr;
@@ -330,7 +331,6 @@ struct dsk_train_ctx_s {
   int sync_dir = 0;                    // 0 none, 1 forward, 2 backward
   int sync_stage = 0;                  // forward: the layer whose records are out; backward: 12 (loss scale), then 11..0
   bool sync_fwd = false;               // this context's forward ran with synchronised statistics
-  bool sync_update = false;            // the stages update the running statistics themselves (not deferred)
   float* rec = nullptr;                // this stage's records of the B local utterances
   long long* mtot = nullptr;           // [12] global pixel count of each layer's statistics
   float* emb_out = nullptr;            // borrowed: where the forward's tail writes the embeddings
@@ -1511,6 +1511,10 @@ static int stat_blocks(long M, int C) {
   return gx < 1 ? 1 : static_cast<int>(gx);
 }
 
+// the backward's gradient w.r.t. y[i]: gA and gB alternate from layer 11's (gA) down, so the dgrad of layer i reads G
+// and writes grad_buf(c, i - 1) while grad_buf(c, i) is still live
+static void* grad_buf(const dsk_train_ctx_s* c, int i) { return (DSK_NUM_CONV - 1 - i) % 2 == 0 ? c->gA : c->gB; }
+
 // Buffers of a train context are sized for `cap` utterances; the launch descriptors (TMA maps, tile counts) are bound
 // to the batch size of the current forward (ctx_bind), so one context serves every B <= cap of the same T: the
 // reference's hard-triplet branch re-forwards a different number of selected triplets every step
@@ -1607,8 +1611,7 @@ static int ctx_bind(dsk_handle h, dsk_train_ctx_s* c, int B) {
     int rc = build_conv(h, &c->conv[i], c->y[i - 1], h->wpk[i], nullptr, nullptr, nullptr, c->raw[i], B, Hi, Wi, lc.cin,
                         lc.cout, lc.ksize, lc.stride, 0, 0.f, true);
     if (rc) return rc;
-    // gradient w.r.t. y[i-1] lands in the buffer that is not holding the gradient w.r.t. y[i]
-    void* g_out = ((DSK_NUM_CONV - 1 - i) % 2 == 0) ? c->gB : c->gA;
+    void* g_out = grad_buf(c, i - 1);
     if (lc.stride == 1) {
       const void* res = (i % 3 == 1) ? c->gres : nullptr;  // skip connection joins at the block input
       rc = build_dgrad_s1(h, &c->dgrad[i][0], c->G, h->wpk_dgrad[i], res, g_out, B, Ho, Wo, lc.cin, lc.cout);
@@ -1663,6 +1666,209 @@ int32_t dsk_set_loss_scale(dsk_handle h, float scale) {
   return DSK_OK;
 }
 
+// ---- dsk_debug_set_backward_capture: copies of the backward's intermediate tensors -----------------------------------
+static int capture_copy(void* dst, const void* src, size_t bytes, cudaStream_t s) {
+  if (dst) CUDA_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s));
+  return DSK_OK;
+}
+
+// the l2-norm backward's input and output
+static int capture_gfc(dsk_handle h, const dsk_train_ctx_s* c, cudaStream_t s) {
+  if (!h->bwd_capture_on) return DSK_OK;
+  const size_t n = static_cast<size_t>(c->B) * h->emb * 4;
+  int rc = capture_copy(h->bwd_capture.g_fc, c->g_fc, n, s);
+  return rc ? rc : capture_copy(h->bwd_capture.fc_out, c->fc_out, n, s);
+}
+
+// the loss scale and the fc input gradient
+static int capture_head(dsk_handle h, const dsk_train_ctx_s* c, cudaStream_t s) {
+  if (!h->bwd_capture_on) return DSK_OK;
+  int rc = capture_copy(h->bwd_capture.loss_scale, c->ls, 2 * 4, s);
+  return rc ? rc : capture_copy(h->bwd_capture.dP, c->dP, static_cast<size_t>(c->B) * 2048 * 4, s);
+}
+
+// layer i's BatchNorm backward: its input gradient gy (before) or its outputs G and gres (after)
+static int capture_layer(dsk_handle h, const dsk_train_ctx_s* c, int i, bool after, cudaStream_t s) {
+  if (!h->bwd_capture_on) return DSK_OK;
+  int H, W, C;
+  act_shape(i, c->T, H, W, C);
+  const size_t bytes = static_cast<size_t>(c->B) * H * W * C * 2;
+  if (!after) return capture_copy(h->bwd_capture.gy[i], grad_buf(c, i), bytes, s);
+  int rc = capture_copy(h->bwd_capture.G[i], c->G, bytes, s);
+  return (rc || i % 3 != 2) ? rc : capture_copy(h->bwd_capture.gres[i], c->gres, bytes, s);
+}
+
+int32_t dsk_debug_set_backward_capture(dsk_handle h, const dsk_backward_capture* cap) {
+  if (!h) return fail(DSK_ERR_INVALID, "null handle");
+  h->bwd_capture_on = cap != nullptr;
+  h->bwd_capture = cap ? *cap : dsk_backward_capture{};
+  return DSK_OK;
+}
+
+// ---- the train-mode layer sequence ------------------------------------------------------------------------------
+// Each step below is the only code on the training path that launches its kernels: the default forward and backward,
+// the synchronised stages and the per-op BatchNorm entry points are sequences of these calls.  Where a step takes
+// `gathered`, a non-null pointer selects the synchronised statistics (the gathered records of N utterances of all
+// ranks) and null the statistics of this batch alone.
+
+// layer i's conv into raw[i]: conv1 from the input features, else the bound conv of y[i-1]
+static int train_conv(dsk_handle h, const dsk_train_ctx_s* c, int i, cudaStream_t s) {
+  if (i > 0) return launch_conv(h, c->conv[i], s);
+  dsk::conv1_kernel<false, true><<<c->B * ((c->T / 2 + 7) / 8), 256, 0, s>>>(c->x, h->conv1_w, h->ones, h->zeros, c->raw[0],
+                                                                            c->T, 0, 0.f, 0);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// BatchNorm batch statistics of raw [M][C] from these M rows alone: mean, rstd, the apply's scale / shift, the unbiased
+// variance (unb may be null) and, if update, the running statistics.  partial holds stat_blocks(M, C) * 4 * C floats.
+static int bn_local_stats(const float* raw, long M, int C, const float* gamma, const float* beta, float* running_mean,
+                          float* running_var, float* mean, float* rstd, float* scale, float* shift, float* unb, int update,
+                          float* partial, cudaStream_t s) {
+  const int gx = stat_blocks(M, C);
+  dsk::bn_stats_partial_kernel<<<dim3(gx, C / 64), 256, 0, s>>>(raw, M, C, partial);
+  KERNEL_CHECK();
+  dsk::bn_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(partial, raw, gx, C, M, gamma, beta, running_mean, running_var, 0.1f,
+                                                         1e-5f, mean, rstd, scale, shift, unb, update);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// BatchNorm apply + residual (res may be null) + clip: raw fp32 -> y 16-bit
+static int bn_apply(bool bf16, const float* raw, const float* scale, const float* shift, const void* res, void* y, long M,
+                    int C, cudaStream_t s) {
+  auto kern = bf16 ? dsk::bn_apply_kernel<true> : dsk::bn_apply_kernel<false>;
+  kern<<<dim3(static_cast<unsigned>((M + 63) / 64), C / 64), 256, 0, s>>>(raw, scale, shift, (const uint16_t*)res,
+                                                                          (uint16_t*)y, M, C, 20.0f);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// layer i's batch statistics, then its BatchNorm + residual + clip into y[i]
+static int train_bn_forward(dsk_handle h, dsk_train_ctx_s* c, int i, const float* gathered, int N, cudaStream_t s) {
+  int H, W, C;
+  act_shape(i, c->T, H, W, C);
+  const long M = static_cast<long>(c->B) * H * W;
+  const dsk_weights& w = h->w;
+  const int update = c->stats_pending ? 0 : 1;
+  int rc = DSK_OK;
+  if (gathered) {
+    dsk::bn_record_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(
+        gathered, N, C, w.bn_gamma[i], w.bn_beta[i], w.bn_running_mean[i], w.bn_running_var[i], 0.1f, 1e-5f, c->mean[i],
+        c->rstd[i], c->scale_t, c->shift_t, c->unb[i], c->mtot + i, update);
+    KERNEL_CHECK();
+  } else {
+    rc = bn_local_stats(c->raw[i], M, C, w.bn_gamma[i], w.bn_beta[i], w.bn_running_mean[i], w.bn_running_var[i], c->mean[i],
+                        c->rstd[i], c->scale_t, c->shift_t, c->unb[i], update, c->partial, s);
+  }
+  const void* res = (i % 3 == 2) ? c->y[i - 2] : nullptr;
+  return rc ? rc : bn_apply(h->bf16, c->raw[i], c->scale_t, c->shift_t, res, c->y[i], M, C, s);
+}
+
+// the tail after layer 11: time pooling, fc as K-slice partial sums, then bias + l2 norm into emb_out
+static int train_tail(dsk_handle h, dsk_train_ctx_s* c, cudaStream_t s) {
+  const int B = c->B, H4 = c->T / 16, WC = 4 * 512;
+  auto pool = h->bf16 ? dsk::pool_time_kernel<true> : dsk::pool_time_kernel<false>;
+  pool<<<dim3(B, WC / 512), 256, 0, s>>>((const uint16_t*)c->y[11], c->pooled, H4, WC, 512, 0);
+  KERNEL_CHECK();
+  const int fc_smem = (dsk::kFcUtt + dsk::kFcFeat) * dsk::kFcPitch * 4;
+  int rc = ensure_smem_optin(reinterpret_cast<const void*>(dsk::fc_kernel), fc_smem);
+  if (rc) return rc;
+  dim3 g((B + dsk::kFcUtt - 1) / dsk::kFcUtt, h->emb / dsk::kFcFeat, dsk::kFcSplit);
+  dsk::fc_kernel<<<g, 256, fc_smem, s>>>(c->pooled, h->fc_wq, c->fc_part, B, 2048, h->emb);
+  KERNEL_CHECK();
+  dsk::l2norm_kernel<<<B, 512, 0, s>>>(c->fc_part, dsk::kFcSplit, h->fc_b, c->fc_out, c->emb_out, c->inv_norm, B, h->emb, 10.0f);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// The loss scale of this backward from the n values of absmax_src (the local g_fc, or the gathered per-utterance maxima):
+// explicit (dsk_set_loss_scale), 1 for bf16 operands, else chosen on the device.  Then the fc and pooling backward into
+// the gy of layer 11.
+static int head_backward(dsk_handle h, dsk_train_ctx_s* c, const float* absmax_src, long n, const dsk_grads* g,
+                         cudaStream_t s) {
+  const int B = c->B, E = h->emb, H4 = c->T / 16;
+  dsk::loss_scale_kernel<<<1, 1024, 0, s>>>(absmax_src, n, h->loss_scale > 0.f ? h->loss_scale : (h->bf16 ? 1.0f : 0.0f), c->ls);
+  KERNEL_CHECK();
+  dsk::fc_bwd_weight_kernel<<<dim3(E / 8, 2048 / 256), 256, 0, s>>>(c->g_fc, c->pooled, g->fc_w, g->fc_b, B, 2048, E, 512, 4);
+  KERNEL_CHECK();
+  dsk::fc_bwd_input_kernel<<<dim3(B, 2048 / 256), 256, E * 4, s>>>(c->g_fc, h->fc_wq, c->dP, 2048, E);
+  KERNEL_CHECK();
+  int rc = capture_head(h, c, s);
+  if (rc) return rc;
+  auto pool = h->bf16 ? dsk::pool_bwd_kernel<true> : dsk::pool_bwd_kernel<false>;
+  pool<<<B, 256, 0, s>>>(c->dP, (uint16_t*)grad_buf(c, DSK_NUM_CONV - 1), H4, 2048, 1.0f / H4, c->ls);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// BatchNorm backward coefficients from these M rows alone: dgamma, dbeta (times inv_scale, and times the 1/S of dyn when
+// set) and the apply's coef [3][C].  partial holds stat_blocks(M, C) * 2 * C floats.
+static int bn_bwd_local_coef(bool bf16, const void* gy, const void* y, const float* raw, const float* mean, const float* rstd,
+                             long M, int C, const float* gamma, float inv_scale, const float* dyn, float* dgamma,
+                             float* dbeta, float* coef, float* partial, cudaStream_t s) {
+  const int gx = stat_blocks(M, C);
+  auto reduce = bf16 ? dsk::bn_bwd_reduce_kernel<true> : dsk::bn_bwd_reduce_kernel<false>;
+  reduce<<<dim3(gx, C / 64), 256, 0, s>>>((const uint16_t*)gy, (const uint16_t*)y, raw, mean, rstd, M, C, 20.0f, partial);
+  KERNEL_CHECK();
+  dsk::bn_bwd_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(partial, gx, C, M, gamma, rstd, inv_scale, dgamma, dbeta, coef, dyn);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// BatchNorm backward apply: gy (w.r.t. y) -> G (w.r.t. raw) and gres (w.r.t. the residual; may be null)
+static int bn_bwd_apply(bool bf16, const void* gy, const void* y, const float* raw, const float* mean, const float* rstd,
+                        const float* coef, void* G, void* gres, long M, int C, cudaStream_t s) {
+  auto kern = bf16 ? dsk::bn_bwd_apply_kernel<true> : dsk::bn_bwd_apply_kernel<false>;
+  kern<<<dim3(static_cast<unsigned>((M + 63) / 64), C / 64), 256, 0, s>>>(
+      (const uint16_t*)gy, (const uint16_t*)y, raw, mean, rstd, coef, (uint16_t*)G, (uint16_t*)gres, M, C, 20.0f);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// layer i's BatchNorm backward, its weight gradient and, for i > 0, the data gradient into the gy of layer i-1
+static int train_bn_backward(dsk_handle h, dsk_train_ctx_s* c, int i, const float* gathered, int N, const dsk_grads* g,
+                             cudaStream_t s) {
+  const bool bf = h->bf16;
+  const int B = c->B, T = c->T;
+  int H, W, C;
+  act_shape(i, T, H, W, C);
+  const long M = static_cast<long>(B) * H * W;
+  const void* gy = grad_buf(c, i);
+  int rc = capture_layer(h, c, i, false, s);
+  if (rc) return rc;
+  if (gathered) {
+    dsk::bn_bwd_record_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(gathered, N, c->rec, B, C, c->mtot + i, h->w.bn_gamma[i],
+                                                                      c->rstd[i], c->ls, g->bn_gamma[i], g->bn_beta[i], c->coef);
+    KERNEL_CHECK();
+  } else {
+    rc = bn_bwd_local_coef(bf, gy, c->y[i], c->raw[i], c->mean[i], c->rstd[i], M, C, h->w.bn_gamma[i], 1.0f, c->ls,
+                           g->bn_gamma[i], g->bn_beta[i], c->coef, c->partial, s);
+    if (rc) return rc;
+  }
+  void* gres = (i % 3 == 2) ? c->gres : nullptr;
+  if ((rc = bn_bwd_apply(bf, gy, c->y[i], c->raw[i], c->mean[i], c->rstd[i], c->coef, c->G, gres, M, C, s))) return rc;
+  if ((rc = capture_layer(h, c, i, true, s))) return rc;
+  if (i == 0) {
+    const int nblk = B * ((T / 2 + 7) / 8);
+    auto part = bf ? dsk::conv1_wgrad_partial_kernel<true> : dsk::conv1_wgrad_partial_kernel<false>;
+    part<<<nblk, 256, 0, s>>>((const uint16_t*)c->G, c->x, B, T, c->c1part);
+    KERNEL_CHECK();
+    dsk::sum_partials_kernel<<<(1600 + 31) / 32, 1024, 0, s>>>(c->c1part, nblk, 1600, 1.0f, g->conv_w[0], c->ls);
+    KERNEL_CHECK();
+    return DSK_OK;
+  }
+  const LayerCfg lc = layer_cfg(i);
+  const int taps = lc.ksize * lc.ksize;
+  const size_t n = static_cast<size_t>(taps) * lc.cout * lc.cin;
+  if ((rc = launch_wgrad(h, c->wgrad[i], s))) return rc;
+  dsk::unpack_wgrad_kernel<<<static_cast<int>((n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096), 256, 0, s>>>(
+      c->dwacc, g->conv_w[i], lc.cout, lc.cin, taps, 1.0f, c->wgrad[i].p.ksplit, c->wgrad[i].p.slice_elems, c->ls);
+  KERNEL_CHECK();
+  for (int k = 0; k < c->n_dgrad[i] && !rc; ++k) rc = launch_conv(h, c->dgrad[i][k], s);
+  return rc;
+}
+
 int32_t dsk_rescnn_forward_train(dsk_handle h, const float* x, int32_t B, int32_t T, float* emb, dsk_train_ctx* ctx_out,
                                  void* stream) {
   int rc = check_handle(h);
@@ -1676,55 +1882,13 @@ int32_t dsk_rescnn_forward_train(dsk_handle h, const float* x, int32_t B, int32_
   if (rc) return rc;
   c->in_use = true;
   c->forward_done = false;
-  c->x = x;
-  const bool bf = h->bf16;
-  for (int i = 0; i < DSK_NUM_CONV; ++i) {
-    int H, W, C;
-    act_shape(i, T, H, W, C);
-    const long M = static_cast<long>(B) * H * W;
-    if (i == 0) {
-      const int blocks = B * ((T / 2 + 7) / 8);
-      dsk::conv1_kernel<false, true><<<blocks, 256, 0, s>>>(x, h->conv1_w, h->ones, h->zeros, c->raw[0], T, 0, 0.f, 0);
-      KERNEL_CHECK();
-    } else {
-      rc = launch_conv(h, c->conv[i], s);
-      if (rc) return rc;
-    }
-    const int gx = stat_blocks(M, C);
-    dim3 gs(gx, C / 64);
-    dsk::bn_stats_partial_kernel<<<gs, 256, 0, s>>>(c->raw[i], M, C, c->partial);
-    KERNEL_CHECK();
-    dsk::bn_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(c->partial, c->raw[i], gx, C, M, h->w.bn_gamma[i], h->w.bn_beta[i],
-                                                           h->w.bn_running_mean[i], h->w.bn_running_var[i], 0.1f, 1e-5f,
-                                                           c->mean[i], c->rstd[i], c->scale_t, c->shift_t, c->unb[i],
-                                                           h->defer_stats ? 0 : 1);
-    KERNEL_CHECK();
-    const uint16_t* res = (i % 3 == 2) ? (const uint16_t*)c->y[i - 2] : nullptr;
-    dim3 ga(static_cast<unsigned>((M + 63) / 64), C / 64);
-    if (bf)
-      dsk::bn_apply_kernel<true><<<ga, 256, 0, s>>>(c->raw[i], c->scale_t, c->shift_t, res, (uint16_t*)c->y[i],
-                                                    M, C, 20.0f);
-    else
-      dsk::bn_apply_kernel<false><<<ga, 256, 0, s>>>(c->raw[i], c->scale_t, c->shift_t, res, (uint16_t*)c->y[i],
-                                                     M, C, 20.0f);
-    KERNEL_CHECK();
-  }
-  {
-    const int H4 = T / 16, WC = 4 * 512;
-    if (bf) dsk::pool_time_kernel<true><<<dim3(B, WC / 512), 256, 0, s>>>((const uint16_t*)c->y[11], c->pooled, H4, WC, 512, 0);
-    else dsk::pool_time_kernel<false><<<dim3(B, WC / 512), 256, 0, s>>>((const uint16_t*)c->y[11], c->pooled, H4, WC, 512, 0);
-    KERNEL_CHECK();
-    const int fc_smem = (dsk::kFcUtt + dsk::kFcFeat) * dsk::kFcPitch * 4;
-    rc = ensure_smem_optin(reinterpret_cast<const void*>(dsk::fc_kernel), fc_smem);
-    if (rc) return rc;
-    dim3 g((B + dsk::kFcUtt - 1) / dsk::kFcUtt, h->emb / dsk::kFcFeat, dsk::kFcSplit);
-    dsk::fc_kernel<<<g, 256, fc_smem, s>>>(c->pooled, h->fc_wq, c->fc_part, B, 2048, h->emb);
-    KERNEL_CHECK();
-    dsk::l2norm_kernel<<<B, 512, 0, s>>>(c->fc_part, dsk::kFcSplit, h->fc_b, c->fc_out, emb, c->inv_norm, B, h->emb, 10.0f);
-    KERNEL_CHECK();
-  }
-  c->forward_done = true;
   c->stats_pending = h->defer_stats;
+  c->x = x;
+  c->emb_out = emb;
+  for (int i = 0; i < DSK_NUM_CONV; ++i)
+    if ((rc = train_conv(h, c, i, s)) || (rc = train_bn_forward(h, c, i, nullptr, 0, s))) return rc;
+  if ((rc = train_tail(h, c, s))) return rc;
+  c->forward_done = true;
   *ctx_out = c;
   return DSK_OK;
 }
@@ -1757,46 +1921,6 @@ int32_t dsk_train_ctx_commit_stats(dsk_handle h, dsk_train_ctx c, void* stream) 
   return DSK_OK;
 }
 
-// ---- dsk_debug_set_backward_capture: copies of the backward's intermediate tensors -----------------------------------
-static int capture_copy(void* dst, const void* src, size_t bytes, cudaStream_t s) {
-  if (dst) CUDA_TRY(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s));
-  return DSK_OK;
-}
-
-// the l2-norm backward's input and output
-static int capture_gfc(dsk_handle h, const dsk_train_ctx_s* c, cudaStream_t s) {
-  if (!h->bwd_capture_on) return DSK_OK;
-  const size_t n = static_cast<size_t>(c->B) * h->emb * 4;
-  int rc = capture_copy(h->bwd_capture.g_fc, c->g_fc, n, s);
-  return rc ? rc : capture_copy(h->bwd_capture.fc_out, c->fc_out, n, s);
-}
-
-// the loss scale and the fc input gradient
-static int capture_head(dsk_handle h, const dsk_train_ctx_s* c, cudaStream_t s) {
-  if (!h->bwd_capture_on) return DSK_OK;
-  int rc = capture_copy(h->bwd_capture.loss_scale, c->ls, 2 * 4, s);
-  return rc ? rc : capture_copy(h->bwd_capture.dP, c->dP, static_cast<size_t>(c->B) * 2048 * 4, s);
-}
-
-// layer i's BatchNorm backward: its input gradient gy (before) or its outputs G and gres (after)
-static int capture_layer(dsk_handle h, const dsk_train_ctx_s* c, int i, bool after, cudaStream_t s) {
-  if (!h->bwd_capture_on) return DSK_OK;
-  int H, W, C;
-  act_shape(i, c->T, H, W, C);
-  const size_t bytes = static_cast<size_t>(c->B) * H * W * C * 2;
-  if (!after)
-    return capture_copy(h->bwd_capture.gy[i], ((DSK_NUM_CONV - 1 - i) % 2 == 0) ? c->gA : c->gB, bytes, s);
-  int rc = capture_copy(h->bwd_capture.G[i], c->G, bytes, s);
-  return (rc || i % 3 != 2) ? rc : capture_copy(h->bwd_capture.gres[i], c->gres, bytes, s);
-}
-
-int32_t dsk_debug_set_backward_capture(dsk_handle h, const dsk_backward_capture* cap) {
-  if (!h) return fail(DSK_ERR_INVALID, "null handle");
-  h->bwd_capture_on = cap != nullptr;
-  h->bwd_capture = cap ? *cap : dsk_backward_capture{};
-  return DSK_OK;
-}
-
 int32_t dsk_rescnn_backward(dsk_handle h, dsk_train_ctx c, const float* grad_emb, const dsk_grads* g, void* stream) {
   int rc = check_handle(h);
   if (rc) return rc;
@@ -1804,77 +1928,11 @@ int32_t dsk_rescnn_backward(dsk_handle h, dsk_train_ctx c, const float* grad_emb
   if (c->sync_fwd) return fail(DSK_ERR_STATE, "dsk_rescnn_backward: a synchronised forward needs dsk_sync_backward_begin");
   if (!grad_emb || !g) return fail(DSK_ERR_INVALID, "dsk_rescnn_backward: null argument");
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const bool bf = h->bf16;
-  const int B = c->B, T = c->T, E = h->emb;
-  // tail
-  dsk::l2norm_bwd_kernel<<<B, 128, 0, s>>>(c->fc_out, c->inv_norm, grad_emb, c->g_fc, E, 10.0f);
+  dsk::l2norm_bwd_kernel<<<c->B, 128, 0, s>>>(c->fc_out, c->inv_norm, grad_emb, c->g_fc, h->emb, 10.0f);
   KERNEL_CHECK();
-  if ((rc = capture_gfc(h, c, s))) return rc;
-  // the loss scale of this backward: explicit (dsk_set_loss_scale), 1 for bf16 operands, else chosen on the device
-  dsk::loss_scale_kernel<<<1, 1024, 0, s>>>(c->g_fc, static_cast<long>(B) * E, h->loss_scale > 0.f ? h->loss_scale : (bf ? 1.0f : 0.0f),
-                                            c->ls);
-  KERNEL_CHECK();
-  dsk::fc_bwd_weight_kernel<<<dim3(E / 8, 2048 / 256), 256, 0, s>>>(c->g_fc, c->pooled, g->fc_w, g->fc_b, B, 2048, E, 512, 4);
-  KERNEL_CHECK();
-  dsk::fc_bwd_input_kernel<<<dim3(B, 2048 / 256), 256, E * 4, s>>>(c->g_fc, h->fc_wq, c->dP, 2048, E);
-  KERNEL_CHECK();
-  if ((rc = capture_head(h, c, s))) return rc;
-  {
-    const int H4 = T / 16;
-    if (bf) dsk::pool_bwd_kernel<true><<<B, 256, 0, s>>>(c->dP, (uint16_t*)c->gA, H4, 2048, 1.0f / H4, c->ls);
-    else dsk::pool_bwd_kernel<false><<<B, 256, 0, s>>>(c->dP, (uint16_t*)c->gA, H4, 2048, 1.0f / H4, c->ls);
-    KERNEL_CHECK();
-  }
-  for (int i = DSK_NUM_CONV - 1; i >= 0; --i) {
-    int H, W, C;
-    act_shape(i, T, H, W, C);
-    const long M = static_cast<long>(B) * H * W;
-    const uint16_t* gy = (const uint16_t*)(((DSK_NUM_CONV - 1 - i) % 2 == 0) ? c->gA : c->gB);
-    if ((rc = capture_layer(h, c, i, false, s))) return rc;
-    const int gx = stat_blocks(M, C);
-    dim3 gs(gx, C / 64);
-    if (bf)
-      dsk::bn_bwd_reduce_kernel<true><<<gs, 256, 0, s>>>(gy, (const uint16_t*)c->y[i], c->raw[i], c->mean[i],
-                                                         c->rstd[i], M, C, 20.0f, c->partial);
-    else
-      dsk::bn_bwd_reduce_kernel<false><<<gs, 256, 0, s>>>(gy, (const uint16_t*)c->y[i], c->raw[i], c->mean[i],
-                                                          c->rstd[i], M, C, 20.0f, c->partial);
-    KERNEL_CHECK();
-    dsk::bn_bwd_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(c->partial, gx, C, M, h->w.bn_gamma[i], c->rstd[i], 1.0f,
-                                                               g->bn_gamma[i], g->bn_beta[i], c->coef, c->ls);
-    KERNEL_CHECK();
-    uint16_t* gres = (i % 3 == 2) ? (uint16_t*)c->gres : nullptr;
-    dim3 ga(static_cast<unsigned>((M + 63) / 64), C / 64);
-    if (bf)
-      dsk::bn_bwd_apply_kernel<true><<<ga, 256, 0, s>>>(gy, (const uint16_t*)c->y[i], c->raw[i], c->mean[i],
-                                                        c->rstd[i], c->coef, (uint16_t*)c->G, gres, M, C, 20.0f);
-    else
-      dsk::bn_bwd_apply_kernel<false><<<ga, 256, 0, s>>>(gy, (const uint16_t*)c->y[i], c->raw[i], c->mean[i],
-                                                         c->rstd[i], c->coef, (uint16_t*)c->G, gres, M, C, 20.0f);
-    KERNEL_CHECK();
-    if ((rc = capture_layer(h, c, i, true, s))) return rc;
-    const LayerCfg lc = layer_cfg(i);
-    if (i == 0) {
-      const int nblk = B * ((T / 2 + 7) / 8);
-      if (bf) dsk::conv1_wgrad_partial_kernel<true><<<nblk, 256, 0, s>>>((const uint16_t*)c->G, c->x, B, T, c->c1part);
-      else dsk::conv1_wgrad_partial_kernel<false><<<nblk, 256, 0, s>>>((const uint16_t*)c->G, c->x, B, T, c->c1part);
-      KERNEL_CHECK();
-      dsk::sum_partials_kernel<<<(1600 + 31) / 32, 1024, 0, s>>>(c->c1part, nblk, 1600, 1.0f, g->conv_w[0], c->ls);
-      KERNEL_CHECK();
-    } else {
-      const int taps = lc.ksize * lc.ksize;
-      const size_t n = static_cast<size_t>(taps) * lc.cout * lc.cin;
-      rc = launch_wgrad(h, c->wgrad[i], s);
-      if (rc) return rc;
-      dsk::unpack_wgrad_kernel<<<static_cast<int>((n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096), 256, 0, s>>>(
-          c->dwacc, g->conv_w[i], lc.cout, lc.cin, taps, 1.0f, c->wgrad[i].p.ksplit, c->wgrad[i].p.slice_elems, c->ls);
-      KERNEL_CHECK();
-      for (int k = 0; k < c->n_dgrad[i]; ++k) {
-        rc = launch_conv(h, c->dgrad[i][k], s);
-        if (rc) return rc;
-      }
-    }
-  }
+  if ((rc = capture_gfc(h, c, s)) || (rc = head_backward(h, c, c->g_fc, static_cast<long>(c->B) * h->emb, g, s))) return rc;
+  for (int i = DSK_NUM_CONV - 1; i >= 0; --i)
+    if ((rc = train_bn_backward(h, c, i, nullptr, 0, g, s))) return rc;
   c->forward_done = false;
   c->in_use = false;
   return DSK_OK;
@@ -1950,8 +2008,8 @@ int32_t dsk_train_ctx_release(dsk_handle h, dsk_train_ctx c) {
 
 // ---- synchronised BatchNorm: the train forward and backward as resumable stages -----------------------------------
 // Each stage ends where this rank's per-utterance records (train_kernels.cuh) are ready; the caller gathers every rank's
-// records in rank order and resumes with them.  Convs, the apply kernels, the weight gradients and the tail are the
-// kernels of dsk_rescnn_forward_train / dsk_rescnn_backward.
+// records in rank order and resumes with them.  The stages run the steps of the train-mode layer sequence above, with
+// the batch statistics, the backward coefficients and the loss scale taken from the gathered records.
 
 // fp32 words of one utterance's record at the current stage
 static long sync_rec_words(const dsk_train_ctx_s* c) {
@@ -1970,7 +2028,7 @@ static void sync_fwd_records(dsk_train_ctx_s* c, int i, cudaStream_t s) {
 static void sync_bwd_records(dsk_handle h, dsk_train_ctx_s* c, int i, cudaStream_t s) {
   int H, W, C;
   act_shape(i, c->T, H, W, C);
-  const uint16_t* gy = (const uint16_t*)(((DSK_NUM_CONV - 1 - i) % 2 == 0) ? c->gA : c->gB);
+  const uint16_t* gy = (const uint16_t*)grad_buf(c, i);
   dim3 g(c->B, C / 64);
   if (h->bf16)
     dsk::bn_bwd_utt_record_kernel<true><<<g, 256, 0, s>>>(gy, (const uint16_t*)c->y[i], c->raw[i], c->mean[i], c->rstd[i],
@@ -1982,14 +2040,8 @@ static void sync_bwd_records(dsk_handle h, dsk_train_ctx_s* c, int i, cudaStream
 
 // forward of layer i up to its records
 static int sync_fwd_conv(dsk_handle h, dsk_train_ctx_s* c, int i, cudaStream_t s) {
-  if (i == 0) {
-    dsk::conv1_kernel<false, true><<<c->B * ((c->T / 2 + 7) / 8), 256, 0, s>>>(c->x, h->conv1_w, h->ones, h->zeros, c->raw[0],
-                                                                              c->T, 0, 0.f, 0);
-    KERNEL_CHECK();
-  } else {
-    int rc = launch_conv(h, c->conv[i], s);
-    if (rc) return rc;
-  }
+  int rc = train_conv(h, c, i, s);
+  if (rc) return rc;
   sync_fwd_records(c, i, s);
   KERNEL_CHECK();
   return DSK_OK;
@@ -1998,41 +2050,17 @@ static int sync_fwd_conv(dsk_handle h, dsk_train_ctx_s* c, int i, cudaStream_t s
 // layer i's global statistics from the gathered records, its BatchNorm + residual + clip, then the next layer's conv
 // and records or the tail
 static int sync_fwd_stage(dsk_handle h, dsk_train_ctx_s* c, const float* gathered, int N, cudaStream_t s, int* more) {
-  const int i = c->sync_stage, B = c->B, T = c->T;
-  int H, W, C;
-  act_shape(i, T, H, W, C);
-  const long M = static_cast<long>(B) * H * W;
-  dsk::bn_record_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(
-      gathered, N, C, h->w.bn_gamma[i], h->w.bn_beta[i], h->w.bn_running_mean[i], h->w.bn_running_var[i], 0.1f, 1e-5f,
-      c->mean[i], c->rstd[i], c->scale_t, c->shift_t, c->unb[i], c->mtot + i, c->sync_update ? 1 : 0);
-  KERNEL_CHECK();
-  const uint16_t* res = (i % 3 == 2) ? (const uint16_t*)c->y[i - 2] : nullptr;
-  dim3 ga(static_cast<unsigned>((M + 63) / 64), C / 64);
-  if (h->bf16)
-    dsk::bn_apply_kernel<true><<<ga, 256, 0, s>>>(c->raw[i], c->scale_t, c->shift_t, res, (uint16_t*)c->y[i], M, C, 20.0f);
-  else
-    dsk::bn_apply_kernel<false><<<ga, 256, 0, s>>>(c->raw[i], c->scale_t, c->shift_t, res, (uint16_t*)c->y[i], M, C, 20.0f);
-  KERNEL_CHECK();
+  const int i = c->sync_stage;
+  int rc = train_bn_forward(h, c, i, gathered, N, s);
+  if (rc) return rc;
   if (i + 1 < DSK_NUM_CONV) {
     c->sync_stage = i + 1;
     *more = 1;
     return sync_fwd_conv(h, c, i + 1, s);
   }
-  const int H4 = T / 16, WC = 4 * 512;
-  if (h->bf16) dsk::pool_time_kernel<true><<<dim3(B, WC / 512), 256, 0, s>>>((const uint16_t*)c->y[11], c->pooled, H4, WC, 512, 0);
-  else dsk::pool_time_kernel<false><<<dim3(B, WC / 512), 256, 0, s>>>((const uint16_t*)c->y[11], c->pooled, H4, WC, 512, 0);
-  KERNEL_CHECK();
-  const int fc_smem = (dsk::kFcUtt + dsk::kFcFeat) * dsk::kFcPitch * 4;
-  int rc = ensure_smem_optin(reinterpret_cast<const void*>(dsk::fc_kernel), fc_smem);
-  if (rc) return rc;
-  dim3 g((B + dsk::kFcUtt - 1) / dsk::kFcUtt, h->emb / dsk::kFcFeat, dsk::kFcSplit);
-  dsk::fc_kernel<<<g, 256, fc_smem, s>>>(c->pooled, h->fc_wq, c->fc_part, B, 2048, h->emb);
-  KERNEL_CHECK();
-  dsk::l2norm_kernel<<<B, 512, 0, s>>>(c->fc_part, dsk::kFcSplit, h->fc_b, c->fc_out, c->emb_out, c->inv_norm, B, h->emb, 10.0f);
-  KERNEL_CHECK();
+  if ((rc = train_tail(h, c, s))) return rc;
   c->sync_dir = 0;
   c->forward_done = true;
-  c->stats_pending = !c->sync_update;
   *more = 0;
   return DSK_OK;
 }
@@ -2041,71 +2069,16 @@ static int sync_fwd_stage(dsk_handle h, dsk_train_ctx_s* c, const float* gathere
 // coefficients from the gathered records, the BatchNorm backward, its weight gradient, then the data gradient and layer
 // i-1's records (i > 0).
 static int sync_bwd_stage(dsk_handle h, dsk_train_ctx_s* c, const float* gathered, int N, cudaStream_t s, int* more) {
-  const bool bf = h->bf16;
-  const int B = c->B, T = c->T, E = h->emb;
-  const dsk_grads* g = &c->grads;
-  int rc;
-  if (c->sync_stage == DSK_NUM_CONV) {
-    dsk::loss_scale_kernel<<<1, 1024, 0, s>>>(gathered, N, h->loss_scale > 0.f ? h->loss_scale : (bf ? 1.0f : 0.0f), c->ls);
-    KERNEL_CHECK();
-    dsk::fc_bwd_weight_kernel<<<dim3(E / 8, 2048 / 256), 256, 0, s>>>(c->g_fc, c->pooled, g->fc_w, g->fc_b, B, 2048, E, 512, 4);
-    KERNEL_CHECK();
-    dsk::fc_bwd_input_kernel<<<dim3(B, 2048 / 256), 256, E * 4, s>>>(c->g_fc, h->fc_wq, c->dP, 2048, E);
-    KERNEL_CHECK();
-    if ((rc = capture_head(h, c, s))) return rc;
-    const int H4 = T / 16;
-    if (bf) dsk::pool_bwd_kernel<true><<<B, 256, 0, s>>>(c->dP, (uint16_t*)c->gA, H4, 2048, 1.0f / H4, c->ls);
-    else dsk::pool_bwd_kernel<false><<<B, 256, 0, s>>>(c->dP, (uint16_t*)c->gA, H4, 2048, 1.0f / H4, c->ls);
-    KERNEL_CHECK();
-    c->sync_stage = DSK_NUM_CONV - 1;
-    sync_bwd_records(h, c, c->sync_stage, s);
-    KERNEL_CHECK();
-    *more = 1;
-    return DSK_OK;
-  }
   const int i = c->sync_stage;
-  int H, W, C;
-  act_shape(i, T, H, W, C);
-  const long M = static_cast<long>(B) * H * W;
-  const uint16_t* gy = (const uint16_t*)(((DSK_NUM_CONV - 1 - i) % 2 == 0) ? c->gA : c->gB);
-  if ((rc = capture_layer(h, c, i, false, s))) return rc;
-  dsk::bn_bwd_record_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(gathered, N, c->rec, B, C, c->mtot + i, h->w.bn_gamma[i],
-                                                                    c->rstd[i], c->ls, g->bn_gamma[i], g->bn_beta[i], c->coef);
-  KERNEL_CHECK();
-  uint16_t* gres = (i % 3 == 2) ? (uint16_t*)c->gres : nullptr;
-  dim3 ga(static_cast<unsigned>((M + 63) / 64), C / 64);
-  if (bf)
-    dsk::bn_bwd_apply_kernel<true><<<ga, 256, 0, s>>>(gy, (const uint16_t*)c->y[i], c->raw[i], c->mean[i], c->rstd[i], c->coef,
-                                                      (uint16_t*)c->G, gres, M, C, 20.0f);
-  else
-    dsk::bn_bwd_apply_kernel<false><<<ga, 256, 0, s>>>(gy, (const uint16_t*)c->y[i], c->raw[i], c->mean[i], c->rstd[i], c->coef,
-                                                       (uint16_t*)c->G, gres, M, C, 20.0f);
-  KERNEL_CHECK();
-  if ((rc = capture_layer(h, c, i, true, s))) return rc;
+  int rc = i == DSK_NUM_CONV ? head_backward(h, c, gathered, N, &c->grads, s)
+                             : train_bn_backward(h, c, i, gathered, N, &c->grads, s);
+  if (rc) return rc;
   if (i == 0) {
-    const int nblk = B * ((T / 2 + 7) / 8);
-    if (bf) dsk::conv1_wgrad_partial_kernel<true><<<nblk, 256, 0, s>>>((const uint16_t*)c->G, c->x, B, T, c->c1part);
-    else dsk::conv1_wgrad_partial_kernel<false><<<nblk, 256, 0, s>>>((const uint16_t*)c->G, c->x, B, T, c->c1part);
-    KERNEL_CHECK();
-    dsk::sum_partials_kernel<<<(1600 + 31) / 32, 1024, 0, s>>>(c->c1part, nblk, 1600, 1.0f, g->conv_w[0], c->ls);
-    KERNEL_CHECK();
     c->sync_dir = 0;
     c->forward_done = false;
     c->in_use = false;
     *more = 0;
     return DSK_OK;
-  }
-  const LayerCfg lc = layer_cfg(i);
-  const int taps = lc.ksize * lc.ksize;
-  const size_t n = static_cast<size_t>(taps) * lc.cout * lc.cin;
-  rc = launch_wgrad(h, c->wgrad[i], s);
-  if (rc) return rc;
-  dsk::unpack_wgrad_kernel<<<static_cast<int>((n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096), 256, 0, s>>>(
-      c->dwacc, g->conv_w[i], lc.cout, lc.cin, taps, 1.0f, c->wgrad[i].p.ksplit, c->wgrad[i].p.slice_elems, c->ls);
-  KERNEL_CHECK();
-  for (int k = 0; k < c->n_dgrad[i]; ++k) {
-    rc = launch_conv(h, c->dgrad[i][k], s);
-    if (rc) return rc;
   }
   c->sync_stage = i - 1;
   sync_bwd_records(h, c, i - 1, s);
@@ -2127,13 +2100,12 @@ int32_t dsk_sync_forward_begin(dsk_handle h, const float* x, int32_t B, int32_t 
   if (rc) return rc;
   c->in_use = true;
   c->forward_done = false;
-  c->stats_pending = false;
+  c->stats_pending = h->defer_stats;
   c->x = x;
   c->emb_out = emb;
   c->sync_dir = 1;
   c->sync_stage = 0;
   c->sync_fwd = true;
-  c->sync_update = !h->defer_stats;
   rc = sync_fwd_conv(h, c, 0, s);
   if (rc) {
     c->in_use = false;
@@ -2260,17 +2232,10 @@ int32_t dsk_bn_act_train_forward(dsk_handle h, const float* raw, const float* ga
   const int gx = stat_blocks(M, C);
   CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&tmp), (static_cast<size_t>(gx) * 4 * C + 2 * C) * 4, s));
   float *partial = tmp, *sc = tmp + static_cast<size_t>(gx) * 4 * C, *sh = sc + C;
-  dsk::bn_stats_partial_kernel<<<dim3(gx, C / 64), 256, 0, s>>>(raw, M, C, partial);
-  KERNEL_CHECK();
-  dsk::bn_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(partial, raw, gx, C, M, gamma, beta, running_mean, running_var, 0.1f,
-                                                         1e-5f, mean, rstd, sc, sh, nullptr, 1);
-  KERNEL_CHECK();
-  dim3 ga(static_cast<unsigned>((M + 63) / 64), C / 64);
-  if (h->bf16) dsk::bn_apply_kernel<true><<<ga, 256, 0, s>>>(raw, sc, sh, (const uint16_t*)res, (uint16_t*)y, M, C, 20.0f);
-  else dsk::bn_apply_kernel<false><<<ga, 256, 0, s>>>(raw, sc, sh, (const uint16_t*)res, (uint16_t*)y, M, C, 20.0f);
-  KERNEL_CHECK();
+  rc = bn_local_stats(raw, M, C, gamma, beta, running_mean, running_var, mean, rstd, sc, sh, nullptr, 1, partial, s);
+  if (!rc) rc = bn_apply(h->bf16, raw, sc, sh, res, y, M, C, s);
   CUDA_TRY(cudaFreeAsync(tmp, s));
-  return DSK_OK;
+  return rc;
 }
 
 // Backward of the above: gy (16-bit, w.r.t. y) -> G (16-bit, w.r.t. raw), gres (16-bit, w.r.t. res; may be NULL),
@@ -2287,21 +2252,10 @@ int32_t dsk_bn_act_train_backward(dsk_handle h, const void* gy, const void* y, c
   const int gx = stat_blocks(M, C);
   CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&tmp), (static_cast<size_t>(gx) * 2 * C + 3 * C) * 4, s));
   float *partial = tmp, *coef = tmp + static_cast<size_t>(gx) * 2 * C;
-  dim3 gs(gx, C / 64), ga(static_cast<unsigned>((M + 63) / 64), C / 64);
-  if (h->bf16) {
-    dsk::bn_bwd_reduce_kernel<true><<<gs, 256, 0, s>>>((const uint16_t*)gy, (const uint16_t*)y, raw, mean, rstd, M, C, 20.0f, partial);
-    dsk::bn_bwd_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(partial, gx, C, M, gamma, rstd, inv_scale, dgamma, dbeta, coef);
-    dsk::bn_bwd_apply_kernel<true><<<ga, 256, 0, s>>>((const uint16_t*)gy, (const uint16_t*)y, raw, mean, rstd, coef, (uint16_t*)G,
-                                                      (uint16_t*)gres, M, C, 20.0f);
-  } else {
-    dsk::bn_bwd_reduce_kernel<false><<<gs, 256, 0, s>>>((const uint16_t*)gy, (const uint16_t*)y, raw, mean, rstd, M, C, 20.0f, partial);
-    dsk::bn_bwd_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(partial, gx, C, M, gamma, rstd, inv_scale, dgamma, dbeta, coef);
-    dsk::bn_bwd_apply_kernel<false><<<ga, 256, 0, s>>>((const uint16_t*)gy, (const uint16_t*)y, raw, mean, rstd, coef, (uint16_t*)G,
-                                                       (uint16_t*)gres, M, C, 20.0f);
-  }
-  KERNEL_CHECK();
+  rc = bn_bwd_local_coef(h->bf16, gy, y, raw, mean, rstd, M, C, gamma, inv_scale, nullptr, dgamma, dbeta, coef, partial, s);
+  if (!rc) rc = bn_bwd_apply(h->bf16, gy, y, raw, mean, rstd, coef, G, gres, M, C, s);
   CUDA_TRY(cudaFreeAsync(tmp, s));
-  return DSK_OK;
+  return rc;
 }
 
 // dsk_bn_act_train_forward with the statistics of the synchronised path: B utterances of HW pixels each (M = B HW rows),
@@ -2324,13 +2278,9 @@ int32_t dsk_bn_act_sync_train_forward(dsk_handle h, const float* raw, const floa
   dsk::bn_record_finalize_kernel<<<(C + 31) / 32, 1024, 0, s>>>(rec, B, C, gamma, beta, running_mean, running_var, 0.1f, 1e-5f,
                                                                 mean, rstd, sc, sh, nullptr, nullptr, 1);
   KERNEL_CHECK();
-  const long M = static_cast<long>(B) * HW;
-  dim3 ga(static_cast<unsigned>((M + 63) / 64), C / 64);
-  if (h->bf16) dsk::bn_apply_kernel<true><<<ga, 256, 0, s>>>(raw, sc, sh, (const uint16_t*)res, (uint16_t*)y, M, C, 20.0f);
-  else dsk::bn_apply_kernel<false><<<ga, 256, 0, s>>>(raw, sc, sh, (const uint16_t*)res, (uint16_t*)y, M, C, 20.0f);
-  KERNEL_CHECK();
+  rc = bn_apply(h->bf16, raw, sc, sh, res, y, static_cast<long>(B) * HW, C, s);
   CUDA_TRY(cudaFreeAsync(tmp, s));
-  return DSK_OK;
+  return rc;
 }
 
 int32_t dsk_conv3x3_padded(dsk_handle h, const void* in, const void* w_packed, const float* scale, const float* bias,

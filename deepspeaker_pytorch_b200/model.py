@@ -175,12 +175,8 @@ class DeepSpeakerModel(nn.Module):
             from . import train as _train
 
             eng = self._get_engine(anchor.device)
-            on, group = _train.sync_bn_setting(self)
             with torch.cuda.device(anchor.device):
-                if on:    # the three forwards in lockstep: one collective per stage carries all three record sets
-                    outs = _train.forward_train_sync(eng, list(xs), group)
-                else:
-                    outs = _train.forward_train_many(eng, list(xs))
+                outs = _train.forward_train_many(eng, list(xs))
         self.features = outs[-1]
         return tuple(outs)
 

@@ -60,13 +60,7 @@ class TrainForwardFn(torch.autograd.Function):
         saved = ctx.saved_tensors
         params = saved[1:]
         grads = engine.grad_scratch(params)
-        g = L.DskGrads()
-        for i in range(L.NUM_CONV):
-            g.conv_w[i] = grads[3 * i].data_ptr()
-            g.bn_gamma[i] = grads[3 * i + 1].data_ptr()
-            g.bn_beta[i] = grads[3 * i + 2].data_ptr()
-        g.fc_w = grads[-2].data_ptr()
-        g.fc_b = grads[-1].data_ptr()
+        g = _grads_struct(grads)
         ge = grad_emb.float().contiguous()
         with torch.cuda.device(ge.device):
             L.check(engine.lib.dsk_rescnn_backward(engine.handle, ctx.guard.tctx, ge.data_ptr(), ctypes.byref(g),
@@ -88,11 +82,22 @@ def _forward_one(engine, x, params, need_grad):
     return emb, tctx
 
 
+def _grads_struct(views):
+    """The ``dsk_grads`` output pointers of a backward: the 38 gradient tensors in ``_train_params`` order."""
+    g = L.DskGrads()
+    for i in range(L.NUM_CONV):
+        g.conv_w[i] = views[3 * i].data_ptr()
+        g.bn_gamma[i] = views[3 * i + 1].data_ptr()
+        g.bn_beta[i] = views[3 * i + 2].data_ptr()
+    g.fc_w = views[-2].data_ptr()
+    g.fc_b = views[-1].data_ptr()
+    return g
+
+
 def forward_train(engine, x):
     module = engine.module_ref
-    on, group = sync_bn_setting(module)
-    if on:
-        return forward_train_sync(engine, [x], group)[0]
+    if sync_bn_setting(module)[0]:
+        return forward_train_many(engine, [x])[0]
     engine.sync_weights(eval_mode=False)
     engine.train_calls += 1  # running statistics are about to change: invalidates the eval-mode BN fold
     params = _train_params(module)
@@ -135,13 +140,7 @@ class TripletForwardFn(torch.autograd.Function):
                 ge = (torch.zeros(ctx.out_shape, device=dev, dtype=torch.float32) if ge is None
                       else ge.float().contiguous())
                 flat, views = engine.grad_scratch(params, with_flat=True)
-                g = L.DskGrads()
-                for i in range(L.NUM_CONV):
-                    g.conv_w[i] = views[3 * i].data_ptr()
-                    g.bn_gamma[i] = views[3 * i + 1].data_ptr()
-                    g.bn_beta[i] = views[3 * i + 2].data_ptr()
-                g.fc_w = views[-2].data_ptr()
-                g.fc_b = views[-1].data_ptr()
+                g = _grads_struct(views)
                 st.wait_stream(cur)                # grad_emb was produced on the caller's stream
                 with torch.cuda.stream(st):
                     L.check(engine.lib.dsk_rescnn_backward(engine.handle, guard.tctx, ge.data_ptr(), ctypes.byref(g),
@@ -150,17 +149,24 @@ class TripletForwardFn(torch.autograd.Function):
                 flats.append(flat)
             for st in engine.side_streams[:k]:
                 cur.wait_stream(st)                # also keeps every grad_emb alive long enough: it is freed on `cur`
-            acc = flats[-1]                        # `views` are the views of this buffer
-            for f in reversed(flats[:-1]):
-                acc.add_(f)
-            # parameters whose .grad is a view of an optimizer / data-parallel bucket (FusedAdagrad, GradBucket):
-            # accumulate into the bucket with one multi-tensor add instead of 38 AccumulateGrad nodes
-            if (all(p.grad is not None and p.grad is getattr(p, "_dsk_bucket_grad", None) for p in params)
-                    and _engine_accumulates_into(ctx, params)):
-                torch._foreach_add_([p.grad for p in params], list(views))
-                engine.bucket_accumulations += 1
-                return (None, None) + (None,) * k + (None,) * len(params)
-        return (None, None) + (None,) * k + tuple(views)
+            return _sum_grads(ctx, engine, params, flats, views, 2 + k)
+
+
+def _sum_grads(node, engine, params, flats, views, n_inputs):
+    """The end of a K-call backward: ONE ordered sum of the K flat gradient buffers into the last one, whose ``views``
+    these are, in autograd's order for K separate calls (last call first: (g_n + g_p) + g_a).  Returns ``node``'s
+    backward result for its ``n_inputs`` non-parameter inputs followed by the parameters."""
+    acc = flats[-1]
+    for f in reversed(flats[:-1]):
+        acc.add_(f)
+    # parameters whose .grad is a view of an optimizer / data-parallel bucket (FusedAdagrad, GradBucket):
+    # accumulate into the bucket with one multi-tensor add instead of 38 AccumulateGrad nodes
+    if (all(p.grad is not None and p.grad is getattr(p, "_dsk_bucket_grad", None) for p in params)
+            and _engine_accumulates_into(node, params)):
+        torch._foreach_add_([p.grad for p in params], list(views))
+        engine.bucket_accumulations += 1
+        return (None,) * (n_inputs + len(params))
+    return (None,) * n_inputs + tuple(views)
 
 
 def _engine_accumulates_into(node, params):
@@ -201,22 +207,27 @@ def _launch_many(engine, xs):
 
 def forward_train_many(engine, xs):
     """Several independent train-mode forwards of one step (the anchor / positive / negative calls of
-    train_triplet.py:215) IN FLIGHT TOGETHER: forward k runs on its own side stream, so the HBM-bound BatchNorm passes
-    of one call overlap the tensor-core convs of another, and so do the three backwards (``TripletForwardFn``).
-    Results are those of the sequential calls, bit for bit: batch statistics are per call anyway, the running-statistics
-    updates are recorded per call and committed afterwards in call order (``dsk_train_ctx_commit_stats``), and the
-    gradients are summed in autograd's order.  All side streams are joined before returning."""
+    train_triplet.py:215) as ONE autograd node.  By default the calls are IN FLIGHT TOGETHER: forward k runs on its own
+    side stream, so the HBM-bound BatchNorm passes of one call overlap the tensor-core convs of another, and so do the
+    three backwards (``TripletForwardFn``).  With synchronised BatchNorm they run in lockstep on the current stream
+    (``SyncTrainForwardFn``): one collective per stage carries every call's records, and every rank must call this with
+    the same number of forwards of the same batch size (a group of None is this process alone, on the same staged path,
+    so results never depend on the number of ranks).  Results are those of the sequential calls, bit for bit: batch
+    statistics are per call anyway, the running-statistics updates are committed in call order
+    (``dsk_train_ctx_commit_stats``), and the gradients are summed in autograd's order."""
     module = engine.module_ref
+    on, group = sync_bn_setting(module)
+    node, launch, args = (SyncTrainForwardFn, _sync_forward, (group,)) if on else (TripletForwardFn, _launch_many, ())
     engine.sync_weights(eval_mode=False)
     engine.train_calls += 1
     params = _train_params(module)
     need_grad = torch.is_grad_enabled() and any(p.requires_grad for p in params)
     xs = [x.contiguous().float() for x in xs]
     if need_grad:
-        outs = list(TripletForwardFn.apply(engine, len(xs), *xs, *params))
+        outs = list(node.apply(engine, *args, len(xs), *xs, *params))
         ctxs = [g.tctx for g in outs[0].grad_fn.guards]
     else:
-        outs, ctxs = _launch_many(engine, xs)
+        outs, ctxs = launch(engine, xs, *args)
     for tctx in ctxs:                                # momentum updates in call order, on the caller's stream
         L.check(engine.lib.dsk_train_ctx_commit_stats(engine.handle, tctx, L.cur_stream()), "dsk_train_ctx_commit_stats")
         if not need_grad:
@@ -277,17 +288,6 @@ def sync_forward_stages(engine, x, emb):
         if not done:
             engine.lib.dsk_train_ctx_release(engine.handle, tctx)
     return tctx
-
-
-def _grads_struct(views):
-    g = L.DskGrads()
-    for i in range(L.NUM_CONV):
-        g.conv_w[i] = views[3 * i].data_ptr()
-        g.bn_gamma[i] = views[3 * i + 1].data_ptr()
-        g.bn_beta[i] = views[3 * i + 2].data_ptr()
-    g.fc_w = views[-2].data_ptr()
-    g.fc_b = views[-1].data_ptr()
-    return g
 
 
 def sync_backward_stages(engine, tctx, B, grad_emb, views):
@@ -372,35 +372,4 @@ class SyncTrainForwardFn(torch.autograd.Function):
             run_lockstep(gens, lambda local: gather_records(local, ctx.group))
             for guard in ctx.guards:
                 guard.consume()
-            acc = flats[-1]                        # `views` are the views of this buffer
-            for f in reversed(flats[:-1]):
-                acc.add_(f)
-            if (all(p.grad is not None and p.grad is getattr(p, "_dsk_bucket_grad", None) for p in params)
-                    and _engine_accumulates_into(ctx, params)):
-                torch._foreach_add_([p.grad for p in params], list(views))
-                engine.bucket_accumulations += 1
-                return (None, None, None) + (None,) * k + (None,) * len(params)
-        return (None, None, None) + (None,) * k + tuple(views)
-
-
-def forward_train_sync(engine, xs, group):
-    """Train-mode forwards of ``xs`` with BatchNorm statistics synchronised over ``group`` (None: this process alone -
-    the same staged path, so results never depend on the number of ranks).  Running statistics are updated in call
-    order; every rank must call this with the same number of forwards of the same batch size."""
-    module = engine.module_ref
-    engine.sync_weights(eval_mode=False)
-    engine.train_calls += 1
-    params = _train_params(module)
-    need_grad = torch.is_grad_enabled() and any(p.requires_grad for p in params)
-    xs = [x.contiguous().float() for x in xs]
-    if need_grad:
-        outs = list(SyncTrainForwardFn.apply(engine, group, len(xs), *xs, *params))
-        ctxs = [g.tctx for g in outs[0].grad_fn.guards]
-    else:
-        outs, ctxs = _sync_forward(engine, xs, group)
-    for tctx in ctxs:                                # deferred momentum updates in call order
-        L.check(engine.lib.dsk_train_ctx_commit_stats(engine.handle, tctx, L.cur_stream()), "dsk_train_ctx_commit_stats")
-        if not need_grad:
-            L.check(engine.lib.dsk_train_ctx_release(engine.handle, tctx), "dsk_train_ctx_release")
-    torch._foreach_add_([bn.num_batches_tracked for _, bn in conv_bn_modules(module)], len(xs))
-    return outs
+            return _sum_grads(ctx, engine, params, flats, views, 3 + k)
