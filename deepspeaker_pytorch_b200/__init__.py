@@ -1,16 +1,16 @@
 """H100-native Deep Speaker hot path: drop-in for reference model.py's DeepSpeakerModel,
 TripletMarginLoss and PairwiseDistance, backed by hand-written sm_90a CUDA behind a C ABI
 (include/dsk.h, lib/libdsk.so)."""
-from .model import (AAMSoftmaxLoss, BatchHardTripletLoss, DeepSpeakerModel, PairwiseDistance,  # noqa: F401
+from .model import (AAMSoftmaxLoss, BatchHardTripletLoss, DeepSpeakerModel, GE2ELoss, PairwiseDistance,  # noqa: F401
                     TripletMarginLoss, allpairs_topk, select_hard_triplets)
 
 from .pipeline import EmbeddingPipeline  # noqa: F401,E402
 from .head import CrossEntropyLoss  # noqa: F401,E402
 from .optim import FusedAdagrad  # noqa: F401,E402
-from .steps import aam_softmax_step, batch_hard_step, train_step  # noqa: F401,E402
+from .steps import aam_softmax_step, batch_hard_step, ge2e_step, train_step  # noqa: F401,E402
 from .parallel import GlobalBatchHardTripletLoss  # noqa: F401,E402
 
-__all__ = ["train_step", "batch_hard_step", "aam_softmax_step", "CrossEntropyLoss", "FusedAdagrad", "EmbeddingPipeline",
-           "DeepSpeakerModel", "PairwiseDistance", "TripletMarginLoss", "AAMSoftmaxLoss", "BatchHardTripletLoss",
-           "GlobalBatchHardTripletLoss",
+__all__ = ["train_step", "batch_hard_step", "aam_softmax_step", "ge2e_step", "CrossEntropyLoss", "FusedAdagrad",
+           "EmbeddingPipeline", "DeepSpeakerModel", "PairwiseDistance", "TripletMarginLoss", "AAMSoftmaxLoss",
+           "BatchHardTripletLoss", "GE2ELoss", "GlobalBatchHardTripletLoss",
            "select_hard_triplets", "allpairs_topk"]

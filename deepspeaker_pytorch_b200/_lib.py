@@ -20,6 +20,7 @@ INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
 NUM_CONV = 12
 DSK_F16, DSK_BF16 = 0, 1
 DSK_EVAL, DSK_TRAIN = 0, 1
+DSK_GE2E_SOFTMAX, DSK_GE2E_CONTRAST = 0, 1
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -184,6 +185,10 @@ SIGNATURES = {
     "dsk_batch_hard_triplet_bwd_rows": (c_int32, [c_void_p] * 6 + [c_int32] * 4 + [c_float] + [c_void_p] * 3),
     "dsk_aam_softmax": (c_int32, [c_void_p] * 4 + [c_int32] * 3 + [c_float, c_float] + [c_void_p] * 4),
     "dsk_aam_softmax_bwd": (c_int32, [c_void_p] * 6 + [c_int32] * 3 + [c_float, c_float] + [c_void_p] * 4),
+    "dsk_ge2e": (c_int32, [c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 3 + [c_int32, c_int32] + [c_void_p] * 2
+                 + [c_int32] + [c_void_p] * 4),
+    "dsk_ge2e_bwd": (c_int32, [c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 3 + [c_int32, c_int32]
+                     + [c_void_p] * 2 + [c_int32] + [c_void_p] * 7),
     "dsk_cosine_matrix": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_void_p]),
     "dsk_topk_mean_std": (c_int32, [c_void_p, c_int32, c_int32, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
     "dsk_cohort_stats": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_int32] + [c_void_p] * 3),

@@ -15,6 +15,7 @@
 
 #include "../../include/dsk.h"
 #include "aam_kernels.cuh"
+#include "ge2e_kernels.cuh"
 #include "conv_umma.cuh"
 #include "conv3x3_halo.cuh"
 #include "conv1_umma.cuh"
@@ -183,6 +184,22 @@ struct AamPlan {
   std::vector<ConvLaunch> fwd, ge_gemm, gw_gemm;
 };
 
+// Cached plan of the GE2E op for one (N, P, D): the AAM plan's operand images, GEMMs and workspaces with the P speaker
+// centroids in place of the class weights, plus GE2E's own per-row and per-speaker buffers.
+struct Ge2ePlan {
+  AamPlan g;
+  int N = 0, P = 0, D = 0;
+  uint8_t* buf = nullptr;
+  float* cent = nullptr;      // [P][D] inclusive centroids (mean of the normalised rows)
+  double* nr64 = nullptr;     // [N] fp64 row norms
+  float* tdc = nullptr;       // [N] the target column's dcos
+  double* part = nullptr;     // [2][Np] per-row shares of dL/dw and dL/db
+  float* gcent = nullptr;     // [P][D] the gradient w.r.t. the inclusive centroids
+  float* own = nullptr;       // [N][D] gê: the target's direct term, then the whole row
+  float* xg = nullptr;        // [N][D] each row's exclusive-centroid term, shared by the other members
+  float* ones = nullptr;      // [N] = 1 (the un-scaling factor of gê)
+};
+
 // Cached plan of the cosine-scoring ops for one (Nc, D, chunk): the fp16 hi/lo operand images of a row chunk of E and of
 // the cohort, their norms, the chunk's fp32 cosines and the descriptors of the one GEMM.  Np: Nc rounded up to 128.
 struct ScorePlan {
@@ -281,6 +298,7 @@ struct dsk_handle_s {
   uint8_t* ap_buf = nullptr;
   std::vector<ConvLaunch> ap_gemm;
   AamPlan aam;                 // cached AAM-softmax plan (its own slot: a step may use both ops)
+  Ge2ePlan ge2e;               // cached GE2E plan (its own slot: a step may sum the GE2E and AAM losses)
   ScorePlan score;             // cached cosine-scoring plan (its own slot: evaluation runs between training steps)
   ScorePlan search;            // cached gallery-search plan (its own slot: searches alternate with cohort statistics)
   bool n256 = false;           // DSK_N256=1: 256-channel tiles for layers with >= n256_min_tiles such tiles
@@ -1093,6 +1111,8 @@ int32_t dsk_destroy(dsk_handle h) {
   cudaFree(h->sk_flags);
   cudaFree(h->ap_buf);
   cudaFree(h->aam.buf);
+  cudaFree(h->ge2e.g.buf);
+  cudaFree(h->ge2e.buf);
   cudaFree(h->score.buf);
   cudaFree(h->search.buf);
   cudaFree(h->ones);
@@ -2675,9 +2695,9 @@ static int aam_build_gemm(dsk_handle h, std::vector<ConvLaunch>* out, const uint
   return DSK_OK;
 }
 
-// (Re)build the handle's AAM plan for (N, C, D).  A rebuild synchronises `s` (buffers in use are freed).
-static int aam_plan(dsk_handle h, int N, int C, int D, cudaStream_t s, AamPlan** out) {
-  AamPlan& P = h->aam;
+// (Re)build the AAM plan in slot P of h (h->aam or h->ge2e.g) for (N, C, D).  A rebuild synchronises `s` (buffers in
+// use are freed).
+static int aam_plan(dsk_handle h, AamPlan& P, int N, int C, int D, cudaStream_t s, AamPlan** out) {
   *out = &P;
   if (P.buf && P.N == N && P.C == C && P.D == D) return DSK_OK;
   CUDA_TRY(cudaStreamSynchronize(s));
@@ -2768,14 +2788,14 @@ int32_t dsk_aam_softmax(dsk_handle h, const float* E, const float* W, const int6
   if (rc) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   AamPlan* P = nullptr;
-  if ((rc = aam_plan(h, N, C, D, s, &P))) return rc;
+  if ((rc = aam_plan(h, h->aam, N, C, D, s, &P))) return rc;
   if ((rc = aam_prep(*P, E, W, false, s))) return rc;
   for (const ConvLaunch& L : P->fwd)
     if ((rc = launch_gemm_f16(L, s))) return rc;
   dsk::aam_rows_kernel<<<N, 256, 0, s>>>(P->gcos, P->Cp, E, W, D, labels, C, aam_margin(margin, scale), cos, lse,
                                          P->row_loss);
   KERNEL_CHECK();
-  dsk::mean_rows_kernel<<<1, 1024, 0, s>>>(P->row_loss, N, loss);
+  dsk::mean_rows_kernel<<<1, 1024, 0, s>>>(P->row_loss, N, N, loss);
   KERNEL_CHECK();
   return DSK_OK;
 }
@@ -2788,7 +2808,7 @@ int32_t dsk_aam_softmax_bwd(dsk_handle h, const float* E, const float* W, const 
   if (rc) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   AamPlan* P = nullptr;
-  if ((rc = aam_plan(h, N, C, D, s, &P))) return rc;
+  if ((rc = aam_plan(h, h->aam, N, C, D, s, &P))) return rc;
   if ((rc = aam_prep(*P, E, W, true, s))) return rc;
   dsk::aam_dcos_kernel<<<P->Np, 256, 0, s>>>(cos, lse, labels, N, C, P->Cp, aam_margin(margin, scale), grad_loss,
                                              P->dcos, P->da, P->rinv);
@@ -2804,6 +2824,116 @@ int32_t dsk_aam_softmax_bwd(dsk_handle h, const float* E, const float* W, const 
   KERNEL_CHECK();
   dsk::aam_normalize_bwd_kernel<<<(C + 7) / 8, 256, 0, s>>>(W, P->nrm_w, P->gw, P->sn, static_cast<long>(P->Cp) * D,
                                                             P->cinv, C, D, gW);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// ---- generalised end-to-end (GE2E) loss ---------------------------------------------------------------------------
+// (Re)build the handle's GE2E plan for (N, P, D): the GEMM plan (an AAM plan with C = P) and GE2E's own buffers.  A
+// rebuild synchronises `s`.
+static int ge2e_plan(dsk_handle h, int N, int P, int D, cudaStream_t s, Ge2ePlan** out) {
+  Ge2ePlan& G = h->ge2e;
+  *out = &G;
+  AamPlan* A = nullptr;
+  int rc = aam_plan(h, G.g, N, P, D, s, &A);
+  if (rc) return rc;
+  if (G.buf && G.N == N && G.P == P && G.D == D) return DSK_OK;
+  CUDA_TRY(cudaStreamSynchronize(s));
+  if (G.buf) CUDA_TRY(cudaFree(G.buf));
+  G.buf = nullptr;
+  G.N = G.P = G.D = 0;
+  const size_t nd = static_cast<size_t>(N) * D * 4, pd = static_cast<size_t>(P) * D * 4;
+  std::vector<std::pair<void**, size_t>> parts = {
+      {reinterpret_cast<void**>(&G.cent), pd},        {reinterpret_cast<void**>(&G.nr64), N * 8ull},
+      {reinterpret_cast<void**>(&G.tdc), N * 4ull},   {reinterpret_cast<void**>(&G.part), 2ull * A->Np * 8},
+      {reinterpret_cast<void**>(&G.gcent), pd},       {reinterpret_cast<void**>(&G.own), nd},
+      {reinterpret_cast<void**>(&G.xg), nd},          {reinterpret_cast<void**>(&G.ones), N * 4ull}};
+  size_t off = 0;
+  for (auto& p : parts) off += (p.second + 255) / 256 * 256;
+  CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&G.buf), off));
+  off = 0;
+  for (auto& p : parts) {
+    *p.first = G.buf + off;
+    off += (p.second + 255) / 256 * 256;
+  }
+  const std::vector<float> ones(N, 1.f);
+  CUDA_TRY(cudaMemcpy(G.ones, ones.data(), N * 4ull, cudaMemcpyHostToDevice));
+  G.N = N;
+  G.P = P;
+  G.D = D;
+  return DSK_OK;
+}
+
+static int ge2e_check(dsk_handle h, bool ptrs_ok, int N, int D, int P, int V, int method, const char* what) {
+  if (!ptrs_ok || N < 2 || P < 2 || P > DSK_AAM_MAX_C || P > N || D < 64 || D % 64 || V < 1 || V > N ||
+      (method != DSK_GE2E_SOFTMAX && method != DSK_GE2E_CONTRAST))
+    return fail(DSK_ERR_INVALID, "%s: bad arguments (need non-null pointers, 2 <= P <= min(N, %d), D a positive multiple "
+                "of 64, 1 <= V <= N and method DSK_GE2E_SOFTMAX or DSK_GE2E_CONTRAST; got N %d, P %d, D %d, V %d, "
+                "method %d)", what, DSK_AAM_MAX_C, N, P, D, V, method);
+  return check_handle(h);
+}
+
+// inclusive centroids, fp64 row norms, and the AAM plan's norms / operand images of E and the centroids
+static int ge2e_prep(const Ge2ePlan& G, const float* E, const int64_t* order, const int64_t* offsets, bool backward,
+                     cudaStream_t s) {
+  dsk::class_centroids_kernel<<<dim3(G.P, (G.D + 255) / 256), 256, 0, s>>>(E, G.N, G.D, order, offsets, G.cent);
+  KERNEL_CHECK();
+  dsk::ge2e_norm64_kernel<<<(G.N + 7) / 8, 256, 0, s>>>(E, G.N, G.D, G.nr64);
+  KERNEL_CHECK();
+  return aam_prep(G.g, E, G.cent, backward, s);
+}
+
+int32_t dsk_ge2e(dsk_handle h, const float* E, int32_t N, int32_t D, const int64_t* order, const int64_t* offsets,
+                 const int64_t* col, int32_t P, int32_t V, const float* w, const float* b, int32_t method, float* loss,
+                 float* cos, float* rec, void* stream) {
+  int rc = ge2e_check(h, E && order && offsets && col && w && b && loss && cos && rec, N, D, P, V, method, "dsk_ge2e");
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  Ge2ePlan* G = nullptr;
+  if ((rc = ge2e_plan(h, N, P, D, s, &G))) return rc;
+  if ((rc = ge2e_prep(*G, E, order, offsets, false, s))) return rc;
+  for (const ConvLaunch& L : G->g.fwd)
+    if ((rc = launch_gemm_f16(L, s))) return rc;
+  dsk::ge2e_rows_kernel<<<N, 256, 0, s>>>(G->g.gcos, G->g.Cp, E, D, G->nr64, order, offsets, col, P, w, b, method, cos,
+                                          rec, G->g.row_loss);
+  KERNEL_CHECK();
+  dsk::mean_rows_kernel<<<1, 1024, 0, s>>>(G->g.row_loss, N, V, loss);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_ge2e_bwd(dsk_handle h, const float* E, int32_t N, int32_t D, const int64_t* order, const int64_t* offsets,
+                     const int64_t* col, int32_t P, int32_t V, const float* w, const float* b, int32_t method,
+                     const float* cos, const float* rec, const float* grad_loss, float* gE, float* gw, float* gb,
+                     void* stream) {
+  int rc = ge2e_check(h, E && order && offsets && col && w && b && cos && rec && grad_loss && gE && gw && gb, N, D, P, V,
+                      method, "dsk_ge2e_bwd");
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  Ge2ePlan* G = nullptr;
+  if ((rc = ge2e_plan(h, N, P, D, s, &G))) return rc;
+  const AamPlan& A = G->g;
+  if ((rc = ge2e_prep(*G, E, order, offsets, true, s))) return rc;
+  dsk::ge2e_dcos_kernel<<<A.Np, 256, 0, s>>>(cos, rec, offsets, col, N, P, A.Cp, V, w, b, method, grad_loss, A.dcos,
+                                             A.da, A.rinv, G->tdc, G->part);
+  KERNEL_CHECK();
+  dsk::aam_dcos_t_kernel<<<A.Cp / 32, 256, 0, s>>>(A.dcos, A.Np, A.Cp, A.dt, A.cinv);
+  KERNEL_CHECK();
+  for (const ConvLaunch& L : A.ge_gemm)  // dcos C^ (target column zeroed)
+    if ((rc = launch_gemm_f16(L, s))) return rc;
+  for (const ConvLaunch& L : A.gw_gemm)  // dcos^T E^: the gradient w.r.t. the normalised inclusive centroids
+    if ((rc = launch_gemm_f16(L, s))) return rc;
+  dsk::aam_normalize_bwd_kernel<<<(P + 7) / 8, 256, 0, s>>>(G->cent, A.nrm_w, A.gw, A.sn, static_cast<long>(A.Cp) * D,
+                                                            A.cinv, P, D, G->gcent);
+  KERNEL_CHECK();
+  dsk::ge2e_excl_bwd_kernel<<<N, 256, 0, s>>>(E, D, G->nr64, order, offsets, col, G->tdc, G->own, G->xg);
+  KERNEL_CHECK();
+  dsk::ge2e_gather_kernel<<<dim3(N, (D + 255) / 256), 256, 0, s>>>(A.ge, A.sc, static_cast<long>(A.Np) * D, A.rinv,
+                                                                   G->gcent, order, offsets, col, G->xg, D, G->own);
+  KERNEL_CHECK();
+  dsk::aam_normalize_bwd_kernel<<<(N + 7) / 8, 256, 0, s>>>(E, A.nrm_e, G->own, 1, 0, G->ones, N, D, gE);
+  KERNEL_CHECK();
+  dsk::ge2e_scalars_kernel<<<1, 256, 0, s>>>(G->part, N, A.Np, w, method, gw, gb);
   KERNEL_CHECK();
   return DSK_OK;
 }
@@ -3068,7 +3198,7 @@ int32_t dsk_cross_entropy(const float* logits, const int64_t* labels, int32_t M,
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   dsk::ce_rows_kernel<<<M, 256, 0, s>>>(logits, labels, C, lse, row_loss);
   KERNEL_CHECK();
-  dsk::mean_rows_kernel<<<1, 1024, 0, s>>>(row_loss, M, loss);
+  dsk::mean_rows_kernel<<<1, 1024, 0, s>>>(row_loss, M, M, loss);
   KERNEL_CHECK();
   return DSK_OK;
 }

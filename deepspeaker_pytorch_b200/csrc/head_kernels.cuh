@@ -127,13 +127,15 @@ ce_rows_kernel(const float* __restrict__ logits, const int64_t* __restrict__ lab
   }
 }
 
-// loss = mean(row_loss)   (single block, fixed order)
-__global__ void __launch_bounds__(1024) mean_rows_kernel(const float* __restrict__ v, int M, float* __restrict__ out) {
+// loss = sum(row_loss[0, M)) / count   (single block, fixed order; count = M is the mean, count < M the mean over the
+// rows that carry a term when the others hold 0)
+__global__ void __launch_bounds__(1024)
+mean_rows_kernel(const float* __restrict__ v, int M, int count, float* __restrict__ out) {
   __shared__ float red[32];
   float s = 0.f;
   for (int i = threadIdx.x; i < M; i += blockDim.x) s += v[i];
   s = block_reduce_sum(s, red);
-  if (threadIdx.x == 0) out[0] = s / static_cast<float>(M);
+  if (threadIdx.x == 0) out[0] = s / static_cast<float>(count);
 }
 
 // dlogits[i][j] = (exp(logits - lse) - [j == label]) * g / M

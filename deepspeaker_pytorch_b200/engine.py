@@ -446,6 +446,83 @@ class AAMSoftmaxFn(torch.autograd.Function):
 
 
 # ---------------------------------------------------------------------------------------------------
+# generalised end-to-end (GE2E) loss
+# ---------------------------------------------------------------------------------------------------
+GE2E_METHODS = {"softmax": L.DSK_GE2E_SOFTMAX, "contrast": L.DSK_GE2E_CONTRAST}
+
+
+def _ge2e_method(method):
+    if method not in GE2E_METHODS:
+        raise ValueError(f"GE2E method must be one of {sorted(GE2E_METHODS)}, got {method!r}")
+    return GE2E_METHODS[method]
+
+
+def ge2e(E, csr, V, w, b, method):
+    """dsk_ge2e: (E as the op read it, loss (1,), cos (N, P), rec (N,)) on E's device.  ``csr`` = (order, offsets, col)
+    int64 device tensors (``model.ge2e_batch``), ``V`` the number of valid rows, ``w`` / ``b`` fp32 device scalars."""
+    m = _ge2e_method(method)
+    if not E.is_cuda:
+        raise RuntimeError("the GE2E loss needs CUDA tensors; there is no CPU fallback")
+    if E.dim() != 2:
+        raise RuntimeError(f"expected embeddings (N, D), got {tuple(E.shape)}")
+    E = E.detach().float().contiguous()
+    order, offsets, col = csr
+    (N, D), P = E.shape, offsets.numel() - 1
+    if order.numel() != N or col.numel() != N:
+        raise RuntimeError(f"GE2E: {order.numel()} labels for {N} embeddings")
+    dev = E.device
+    for t in (order, offsets, col, w, b):
+        if t.device != dev:
+            raise RuntimeError("GE2E: embeddings, speaker lists and the scalars w, b must be on one device")
+    loss = torch.empty(1, device=dev, dtype=torch.float32)
+    cos = torch.empty(N, P, device=dev, dtype=torch.float32)
+    rec = torch.empty(N, device=dev, dtype=torch.float32)
+    with torch.cuda.device(dev):
+        L.check(L.load().dsk_ge2e(_allpairs_handle(dev), E.data_ptr(), N, D, order.data_ptr(), offsets.data_ptr(),
+                                  col.data_ptr(), P, int(V), w.data_ptr(), b.data_ptr(), m, loss.data_ptr(),
+                                  cos.data_ptr(), rec.data_ptr(), L.cur_stream()), "dsk_ge2e")
+    return E, loss, cos, rec
+
+
+def ge2e_backward(E, csr, V, w, b, method, cos, rec, grad_loss):
+    """dsk_ge2e_bwd: (gE (N, D), gw (), gb ()) = d loss / d (E, w, b) scaled by the device scalar ``grad_loss``; gb is
+    exactly 0 for ``softmax``."""
+    order, offsets, col = csr
+    (N, D), P = E.shape, offsets.numel() - 1
+    gl = grad_loss.float().reshape(1).contiguous()
+    gE = torch.empty_like(E)
+    gw = torch.empty((), device=E.device, dtype=torch.float32)
+    gb = torch.empty((), device=E.device, dtype=torch.float32)
+    with torch.cuda.device(E.device):
+        L.check(L.load().dsk_ge2e_bwd(_allpairs_handle(E.device), E.data_ptr(), N, D, order.data_ptr(),
+                                      offsets.data_ptr(), col.data_ptr(), P, int(V), w.data_ptr(), b.data_ptr(),
+                                      _ge2e_method(method), cos.data_ptr(), rec.data_ptr(), gl.data_ptr(), gE.data_ptr(),
+                                      gw.data_ptr(), gb.data_ptr(), L.cur_stream()), "dsk_ge2e_bwd")
+    return gE, gw, gb
+
+
+class GE2EFn(torch.autograd.Function):
+    """GE2E loss over (E, w, b) against the batch's speaker centroids; the loss is a device scalar.  ``csr`` and ``V``
+    as in ``ge2e``."""
+
+    @staticmethod
+    def forward(ctx, E, w, b, csr, V, method):
+        wc, bc = (t.detach().float().reshape(1).contiguous() for t in (w, b))
+        Ec, loss, cos, rec = ge2e(E, csr, V, wc, bc, method)
+        ctx.save_for_backward(Ec, wc, bc, cos, rec, *csr)
+        ctx.V, ctx.method, ctx.shapes = V, method, (w.shape, b.shape)
+        return loss.reshape(())
+
+    @staticmethod
+    def backward(ctx, gl):
+        E, w, b, cos, rec, order, offsets, col = ctx.saved_tensors
+        gE, gw, gb = ge2e_backward(E, (order, offsets, col), ctx.V, w, b, ctx.method, cos, rec, gl)
+        ni = ctx.needs_input_grad
+        return (gE if ni[0] else None, gw.reshape(ctx.shapes[0]) if ni[1] else None,
+                gb.reshape(ctx.shapes[1]) if ni[2] else None, None, None, None)
+
+
+# ---------------------------------------------------------------------------------------------------
 # cosine scoring and cohort statistics (AS-norm)
 # ---------------------------------------------------------------------------------------------------
 def _score_rows(X, what):

@@ -16,6 +16,7 @@ from __future__ import annotations
 import ctypes
 import math
 
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -262,6 +263,71 @@ class AAMSoftmaxLoss:
         return _engine.AAMSoftmaxFn.apply(embeddings, self.weight, labels, float(self.margin), float(self.scale))
 
     __call__ = forward
+
+
+def ge2e_batch(labels):
+    """The speaker lists of a GE2E batch, built on the host from int64 labels of any values: (order, offsets, col, V)
+    as int64 numpy arrays and an int.  Speakers are the distinct labels in ascending order (``identification.
+    speaker_csr``'s order): speaker k's rows are order[offsets[k]:offsets[k+1]] in ascending row order, col[i] is row
+    i's speaker, and V (``batch_hard_valid_count``'s rule) counts the rows whose speaker has >= 2 rows, provided the
+    batch holds >= 2 speakers.  A CUDA tensor is read back to the host (one device synchronisation)."""
+    from .identification import speaker_csr
+
+    lab = torch.as_tensor(labels).detach().cpu().reshape(-1)
+    if lab.dtype.is_floating_point or lab.dtype == torch.bool:
+        raise ValueError(f"GE2E labels must be integers, got {lab.dtype}")
+    order, offsets, _ = speaker_csr(lab.to(torch.int64))
+    counts = np.diff(offsets)
+    col = np.empty(order.size, np.int64)
+    col[order] = np.repeat(np.arange(counts.size, dtype=np.int64), counts)
+    V = int(counts[counts >= 2].sum()) if counts.size >= 2 else 0
+    return order, offsets, col, V
+
+
+class GE2ELoss(nn.Module):
+    """Generalised end-to-end loss (Wan et al., "Generalized End-to-End Loss for Speaker Verification", ICASSP 2018; no
+    reference implementation) over a batch of P speakers x M utterances.  Every utterance is scored against every
+    speaker's centroid in the batch (the mean of its normalised embeddings), its own speaker's with the utterance left
+    out; the cosines pass through ``max(w, 1e-6) cos + b`` and then a softmax over the speakers (``method="softmax"``)
+    or the paper's contrast loss (``"contrast"``: 1 - sigmoid(own) + the largest sigmoid of another speaker).  The
+    loss is the mean over the utterances whose speaker has >= 2 of them; a singleton speaker's utterance adds no term
+    but its centroid is a column for every other one.  The definition is stated in full in ``include/dsk.h``.
+
+    ``w`` and ``b`` are learnable parameters: pass ``loss.parameters()`` to the optimizer (or bucket) with the model's.
+    With ``softmax`` the gradient of ``b`` is exactly 0 (b cancels out of the loss), so ``b`` never moves."""
+
+    def __init__(self, init_w=10.0, init_b=-5.0, method="softmax"):
+        super().__init__()
+        _engine._ge2e_method(method)
+        self.method = method
+        self.w = nn.Parameter(torch.tensor(float(init_w)))
+        self.b = nn.Parameter(torch.tensor(float(init_b)))
+
+    def extra_repr(self):
+        return f"method={self.method!r}"
+
+    def forward(self, embeddings, labels):
+        """embeddings (N, D) CUDA (D a multiple of 64), labels (N,) int -> 0-dim device scalar; back-propagates into the
+        embeddings, ``w`` and ``b``.  With CPU labels, as a data loader yields them, the speaker lists are built on the
+        host and the step reads nothing back from the device; CUDA labels are read back once.  Raises ValueError when no
+        utterance can contribute (V = 0: fewer than 2 speakers, or no speaker with 2 utterances), before any launch."""
+        order, offsets, col, V = ge2e_batch(labels)
+        if V == 0:
+            raise ValueError("GE2ELoss: no utterance contributes to the loss (it needs >= 2 speakers, one of them with "
+                             ">= 2 utterances)")
+        if not embeddings.is_cuda:
+            raise RuntimeError("GE2ELoss needs CUDA embeddings; there is no CPU fallback")
+        if order.size != embeddings.shape[0]:
+            raise RuntimeError(f"GE2ELoss: {order.size} labels for {embeddings.shape[0]} embeddings")
+        dev = embeddings.device
+        if self.w.device != dev:
+            raise RuntimeError("GE2ELoss: move the loss to the embeddings' device (loss.to(device))")
+        # one pinned copy, queued on the stream like a kernel
+        host = torch.from_numpy(np.concatenate([order, offsets, col])).pin_memory()
+        flat = host.to(dev, non_blocking=True)
+        N, P = order.size, offsets.size - 1
+        csr = (flat[:N], flat[N:N + P + 1], flat[N + P + 1:])
+        return _engine.GE2EFn.apply(embeddings, self.w, self.b, csr, V, self.method)
 
 
 def batch_hard_valid_count(labels):

@@ -187,3 +187,30 @@ def aam_softmax_step(model, optimizer, data, labels, *, margin, scale, bucket=No
     loss.backward()
     _reduce_and_step(optimizer, bucket, None)
     return {"loss": loss.detach()}
+
+
+def ge2e_step(model, optimizer, data, labels, *, loss, bucket=None):
+    """One step with the generalised end-to-end loss ``loss`` (a ``GE2ELoss``) on a P speakers x M utterances batch:
+    ONE train-mode forward of all N utterances, the loss against the batch's speaker centroids, backward, optimizer step.
+    The optimizer (or ``bucket``) must hold ``loss.parameters()`` beside the model's: ``w`` and ``b`` are then averaged
+    in the same single all-reduce.  Returns ``{"loss": device scalar, "valid": V}``; raises ValueError for a batch with
+    V = 0 (fewer than 2 speakers, or no speaker with 2 utterances).  With CPU labels the step reads nothing back from the
+    device.
+
+    Under data parallelism (``bucket`` or a ``FusedAdagrad`` optimizer) each rank's gradient is weighted by its own
+    number of valid utterances V_r, as in ``batch_hard_step``.  The centroids are each rank's own: a rank scores its
+    utterances against the speakers of its shard only, so the objective depends on the number of ranks R (keep each
+    speaker's utterances on one rank).  Runs unchanged on a model with ``sync_batchnorm()``."""
+    if not model.training:
+        raise RuntimeError("ge2e_step needs model.train()")
+    labels = torch.as_tensor(labels).detach().cpu()     # CUDA labels: the one read-back
+    V = batch_hard_valid_count(labels)
+    if V == 0:
+        raise ValueError("ge2e_step: no utterance contributes to the loss (it needs >= 2 speakers, one of them with "
+                         ">= 2 utterances)")
+    emb = model(data)
+    out = loss(emb, labels)
+    optimizer.zero_grad()
+    out.backward()
+    _reduce_and_step(optimizer, bucket, torch.tensor(float(V)))
+    return {"loss": out.detach(), "valid": V}

@@ -359,6 +359,53 @@ int32_t dsk_aam_softmax_bwd(dsk_handle h, const float* E, const float* W, const 
                             const float* lse, int32_t N, int32_t C, int32_t D, float margin, float scale,
                             const float* grad_loss, float* gE, float* gW, void* stream);
 
+/* Generalised end-to-end (GE2E) loss against in-batch speaker centroids (Wan et al., ICASSP 2018; no reference
+ * implementation exists).  For embeddings E (N,D) and a batch of P speakers given as a CSR: speaker k's rows are
+ * S_k = order[offsets[k] .. offsets[k+1]) (n_k of them, ascending row index within a speaker), col[i] = the speaker of
+ * row i (device int64; the host builds them from the labels, speakers in ascending label order):
+ *   e^_i = e_i / max(||e_i||, 1e-12) (F.normalize);  inclusive centroid c_k = (1/n_k) sum_{u in S_k} e^_u (exactly
+ *   dsk_class_centroids);  exclusive centroid c_k^(-i) = (1/(n_k - 1)) sum_{u in S_k, u != i} e^_u (n_k >= 2);
+ *   c^ = c / max(||c||, 1e-12);  cos (N,P): cos_ik = e^_i . c^_k for k != y_i, cos_{i,y_i} = e^_i . c^_{y_i}^(-i)
+ *   (a row of a singleton speaker keeps the inclusive cosine there);  S_ik = max(w, 1e-6) cos_ik + b.
+ *   Row i is valid when n_{y_i} >= 2 (with P >= 2); V = the number of valid rows.  Row losses:
+ *     DSK_GE2E_SOFTMAX:  L_i = logsumexp_k S_ik - S_{i,y_i};                       rec[i] = logsumexp_k S_ik
+ *     DSK_GE2E_CONTRAST: L_i = 1 - sigmoid(S_{i,y_i}) + max_{k != y_i} sigmoid(S_ik);  rec[i] = that k, ties to the
+ *                        lowest column (an integer stored in fp32)
+ *   loss (1,) = (1/V) sum over valid i of L_i, summed in a fixed order.  A singleton speaker's row has no loss term,
+ *   but its centroid is a column of every other row.
+ * w and b are device scalars (nothing is read back); cos and rec are caller-owned outputs that dsk_ge2e_bwd reads.
+ * Accuracy: the non-target cosines run on the AAM-softmax op's hi/lo fp16 tensor-core GEMM against the centroids
+ * (computed in fp64, rounded to fp32), within ~1e-6 of fp64; the target cosine is computed in fp64 from the fp32 rows
+ * in CSR order and rounded once.
+ * The GEMM plan and its buffers are cached in h for (N, P, D), in a slot of their own (the AAM, scoring, search and
+ * all-pairs plans are untouched); a change rebuilds them, which synchronises the stream.  Cost beyond the GEMMs:
+ * O(sum_k n_k^2 D) for the exclusive centroids.
+ * 2 <= P <= DSK_AAM_MAX_C, D % 64 == 0, 1 <= V <= N, method one of the two below, else DSK_ERR_INVALID before any
+ * launch. */
+#define DSK_GE2E_SOFTMAX 0
+#define DSK_GE2E_CONTRAST 1
+int32_t dsk_ge2e(dsk_handle h, const float* E, int32_t N, int32_t D, const int64_t* order, const int64_t* offsets,
+                 const int64_t* col, int32_t P, int32_t V, const float* w, const float* b, int32_t method, float* loss,
+                 float* cos, float* rec, void* stream);
+/* Its backward: gE (N,D), gw (1,), gb (1,) = d loss / d (E, w, b) scaled by grad_loss (device scalar), WRITTEN not
+ * accumulated.  dS_ik = grad_loss / V * dL_i / dS_ik on valid rows and 0 elsewhere, dcos = max(w, 1e-6) dS;
+ * gw = sum dS cos over every entry where w >= 1e-6 (torch.clamp passes the gradient there), else 0; gb = sum dS for
+ * contrast, and EXACTLY 0 for softmax: b cancels out of the softmax loss, and the rounding residue torch autograd
+ * returns instead would be amplified by an adaptive optimizer into steps of size lr.  gw and gb are summed in fp64 in a
+ * fixed order.  In e^-space, g^_i is the sum of
+ *   the direct term       sum_{k != y_i} dcos_ik c^_k + dcos_{i,y_i} c^_{y_i}^(-i);
+ *   the inclusive terms   g^c_k = sum_{i: y_i != k} dcos_ik e^_i, gc_k = (g^c_k - c^_k (c^_k . g^c_k)) / max(||c_k||,
+ *                         1e-12), added as gc_k / n_k to every member of S_k;
+ *   the exclusive terms   for every valid row j of speaker k, the Jacobian at c_k^(-j) applied to dcos_{j,k} e^_j,
+ *                         divided by n_k - 1 and added to every member u != j of S_k, in ascending j;
+ * then gE_u = (g^_u - e^_u (e^_u . g^_u)) / max(||e_u||, 1e-12).  The two products run on the AAM plan's GEMMs in
+ * fixed K slices; the exclusive-centroid terms are computed in fp64 from the fp32 rows, as fixed-order sums over each
+ * speaker's members.  Deterministic: no float atomics, two calls give the same bits. */
+int32_t dsk_ge2e_bwd(dsk_handle h, const float* E, int32_t N, int32_t D, const int64_t* order, const int64_t* offsets,
+                     const int64_t* col, int32_t P, int32_t V, const float* w, const float* b, int32_t method,
+                     const float* cos, const float* rec, const float* grad_loss, float* gE, float* gw, float* gb,
+                     void* stream);
+
 /* Cosine scoring of verification trials with adaptive symmetric score normalisation (AS-norm) against an impostor
  * cohort (no reference implementation exists; the reference scores Euclidean distances, eval_metrics.py:5-50).  Rows are
  * normalised as in F.normalize, x^ = x / max(||x||, 1e-12).
