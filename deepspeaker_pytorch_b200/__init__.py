@@ -8,9 +8,9 @@ from .pipeline import EmbeddingPipeline  # noqa: F401,E402
 from .head import CrossEntropyLoss  # noqa: F401,E402
 from .optim import FusedAdagrad  # noqa: F401,E402
 from .steps import aam_softmax_step, batch_hard_step, ge2e_step, train_step  # noqa: F401,E402
-from .parallel import GlobalBatchHardTripletLoss  # noqa: F401,E402
+from .parallel import GlobalBatchHardTripletLoss, GlobalGE2ELoss  # noqa: F401,E402
 
 __all__ = ["train_step", "batch_hard_step", "aam_softmax_step", "ge2e_step", "CrossEntropyLoss", "FusedAdagrad",
            "EmbeddingPipeline", "DeepSpeakerModel", "PairwiseDistance", "TripletMarginLoss", "AAMSoftmaxLoss",
-           "BatchHardTripletLoss", "GE2ELoss", "GlobalBatchHardTripletLoss",
+           "BatchHardTripletLoss", "GE2ELoss", "GlobalBatchHardTripletLoss", "GlobalGE2ELoss",
            "select_hard_triplets", "allpairs_topk"]

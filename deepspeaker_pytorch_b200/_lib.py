@@ -189,6 +189,13 @@ SIGNATURES = {
                  + [c_int32] + [c_void_p] * 4),
     "dsk_ge2e_bwd": (c_int32, [c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 3 + [c_int32, c_int32]
                      + [c_void_p] * 2 + [c_int32] + [c_void_p] * 7),
+    "dsk_ge2e_rows": (c_int32, [c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 3 + [c_int32, c_int32]
+                      + [c_void_p] * 2 + [c_int32] * 3 + [c_void_p] * 4),
+    "dsk_ge2e_mean": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p]),
+    "dsk_ge2e_dcos_rows": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p,
+                                     c_void_p, c_int32, c_void_p, c_int32, c_int32] + [c_void_p] * 5),
+    "dsk_ge2e_bwd_rows": (c_int32, [c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 3 + [c_int32]
+                          + [c_void_p] * 2 + [c_int32] * 2 + [c_void_p] * 2),
     "dsk_cosine_matrix": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_void_p]),
     "dsk_topk_mean_std": (c_int32, [c_void_p, c_int32, c_int32, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
     "dsk_cohort_stats": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_int32] + [c_void_p] * 3),

@@ -184,20 +184,33 @@ struct AamPlan {
   std::vector<ConvLaunch> fwd, ge_gemm, gw_gemm;
 };
 
-// Cached plan of the GE2E op for one (N, P, D): the AAM plan's operand images, GEMMs and workspaces with the P speaker
-// centroids in place of the class weights, plus GE2E's own per-row and per-speaker buffers.
+// Cached plan of the GE2E ops for one (N, P, D, row0, rows): the AAM op's hi/lo operand images and GEMMs with the P
+// speaker centroids in place of the class weights - the cosines and gE^ = dcos C^ for the rows x P block of the row
+// range [row0, row0 + rows), the centroid gradient gC^ = dcos^T E^ over all N rows - plus GE2E's own buffers.  Np, Rp,
+// Cp: N, rows and P rounded up to 128 (the GEMM's pixel tile).
 struct Ge2ePlan {
-  AamPlan g;
-  int N = 0, P = 0, D = 0;
+  int N = 0, P = 0, D = 0, row0 = 0, rows = 0, Np = 0, Rp = 0, Cp = 0;
+  int sc = 0, sn = 0;                        // K slices of gE^ and gC^: ceil(Cp / kAamSlice), ceil(Np / kAamSlice)
   uint8_t* buf = nullptr;
-  float* cent = nullptr;      // [P][D] inclusive centroids (mean of the normalised rows)
-  double* nr64 = nullptr;     // [N] fp64 row norms
-  float* tdc = nullptr;       // [N] the target column's dcos
-  double* part = nullptr;     // [2][Np] per-row shares of dL/dw and dL/db
-  float* gcent = nullptr;     // [P][D] the gradient w.r.t. the inclusive centroids
-  float* own = nullptr;       // [N][D] gê: the target's direct term, then the whole row
-  float* xg = nullptr;        // [N][D] each row's exclusive-centroid term, shared by the other members
-  float* ones = nullptr;      // [N] = 1 (the un-scaling factor of gê)
+  float* cent = nullptr;                     // [P][D] inclusive centroids (mean of the normalised rows)
+  double* nr64 = nullptr;                    // [N] fp64 row norms
+  float *nrm_e = nullptr, *nrm_c = nullptr;  // [N], [P] fp32 norms of the rows and the centroids
+  uint16_t *ea = nullptr, *cb = nullptr;     // forward operands: E^ of the range [Rp][3D] (A side), C^ [Cp][3D] (B side)
+  uint16_t *et = nullptr, *ct = nullptr;     // backward B operands, transposed: E^T [D][3Np] (all rows), C^T [D][3Cp]
+  uint16_t *da = nullptr, *dt = nullptr;     // backward A operands: the range's dcos [Rp][3Cp], dcos^T [Cp][3Np]
+  float* gcos = nullptr;                     // [Rp][Cp] the range's GEMM cosines
+  float* dcos = nullptr;                     // [Np][Cp] the whole batch's dcos, zero-padded
+  float *rinv = nullptr, *cinv = nullptr;    // [Rp], [Cp]: inverse power-of-two scales of dcos's rows / columns
+  float *ge = nullptr, *gc = nullptr;        // [sc][Rp][D], [sn][Cp][D]: the slices' scaled gradients w.r.t. E^, C^
+  float* gcent = nullptr;                    // [P][D] the gradient w.r.t. the inclusive centroids
+  float* own = nullptr;                      // [Rp][D] gê of the range: the target's direct term, then the whole row
+  float* xg = nullptr;                       // [N][D] each row's exclusive-centroid term, shared by the other members
+  float* ones = nullptr;                     // [Rp] = 1 (the un-scaling factor of gê)
+  // the whole-batch ops' intermediates (only in a plan for the range (0, N)): row losses [N], the target column's dcos
+  // [N] and the per-row shares of dL/dw and dL/db [2][N]; their dcos goes straight to dcos / da / rinv above
+  float *row_loss = nullptr, *tdc = nullptr;
+  double* part = nullptr;
+  std::vector<ConvLaunch> fwd, ge_gemm, gc_gemm;
 };
 
 // Cached plan of the cosine-scoring ops for one (Nc, D, chunk): the fp16 hi/lo operand images of a row chunk of E and of
@@ -1111,7 +1124,6 @@ int32_t dsk_destroy(dsk_handle h) {
   cudaFree(h->sk_flags);
   cudaFree(h->ap_buf);
   cudaFree(h->aam.buf);
-  cudaFree(h->ge2e.g.buf);
   cudaFree(h->ge2e.buf);
   cudaFree(h->score.buf);
   cudaFree(h->search.buf);
@@ -2695,7 +2707,7 @@ static int aam_build_gemm(dsk_handle h, std::vector<ConvLaunch>* out, const uint
   return DSK_OK;
 }
 
-// (Re)build the AAM plan in slot P of h (h->aam or h->ge2e.g) for (N, C, D).  A rebuild synchronises `s` (buffers in
+// (Re)build the AAM plan in slot P of h (h->aam) for (N, C, D).  A rebuild synchronises `s` (buffers in
 // use are freed).
 static int aam_plan(dsk_handle h, AamPlan& P, int N, int C, int D, cudaStream_t s, AamPlan** out) {
   *out = &P;
@@ -2829,113 +2841,251 @@ int32_t dsk_aam_softmax_bwd(dsk_handle h, const float* E, const float* W, const 
 }
 
 // ---- generalised end-to-end (GE2E) loss ---------------------------------------------------------------------------
-// (Re)build the handle's GE2E plan for (N, P, D): the GEMM plan (an AAM plan with C = P) and GE2E's own buffers.  A
-// rebuild synchronises `s`.
-static int ge2e_plan(dsk_handle h, int N, int P, int D, cudaStream_t s, Ge2ePlan** out) {
+// (Re)build the handle's GE2E plan for (N, P, D, row0, rows): buffers and the GEMM descriptors.  A rebuild
+// synchronises `s` (buffers in use are freed).
+static int ge2e_plan(dsk_handle h, int N, int P, int D, int row0, int rows, cudaStream_t s, Ge2ePlan** out) {
   Ge2ePlan& G = h->ge2e;
   *out = &G;
-  AamPlan* A = nullptr;
-  int rc = aam_plan(h, G.g, N, P, D, s, &A);
-  if (rc) return rc;
-  if (G.buf && G.N == N && G.P == P && G.D == D) return DSK_OK;
+  if (G.buf && G.N == N && G.P == P && G.D == D && G.row0 == row0 && G.rows == rows) return DSK_OK;
   CUDA_TRY(cudaStreamSynchronize(s));
   if (G.buf) CUDA_TRY(cudaFree(G.buf));
-  G.buf = nullptr;
-  G.N = G.P = G.D = 0;
-  const size_t nd = static_cast<size_t>(N) * D * 4, pd = static_cast<size_t>(P) * D * 4;
+  G = Ge2ePlan();
+  const int Np = (N + 127) / 128 * 128, Rp = (rows + 127) / 128 * 128, Cp = (P + 127) / 128 * 128;
+  const int sc = (Cp + dsk::kAamSlice - 1) / dsk::kAamSlice, sn = (Np + dsk::kAamSlice - 1) / dsk::kAamSlice;
+  const size_t d3 = 3ull * D, pd = static_cast<size_t>(P) * D * 4;
+  const size_t whole = row0 == 0 && rows == N ? 1 : 0;
   std::vector<std::pair<void**, size_t>> parts = {
-      {reinterpret_cast<void**>(&G.cent), pd},        {reinterpret_cast<void**>(&G.nr64), N * 8ull},
-      {reinterpret_cast<void**>(&G.tdc), N * 4ull},   {reinterpret_cast<void**>(&G.part), 2ull * A->Np * 8},
-      {reinterpret_cast<void**>(&G.gcent), pd},       {reinterpret_cast<void**>(&G.own), nd},
-      {reinterpret_cast<void**>(&G.xg), nd},          {reinterpret_cast<void**>(&G.ones), N * 4ull}};
+      {reinterpret_cast<void**>(&G.row_loss), whole * N * 4}, {reinterpret_cast<void**>(&G.tdc), whole * N * 4},
+      {reinterpret_cast<void**>(&G.part), whole * 2 * N * 8},
+      {reinterpret_cast<void**>(&G.cent), pd},                {reinterpret_cast<void**>(&G.nr64), N * 8ull},
+      {reinterpret_cast<void**>(&G.nrm_e), N * 4ull},         {reinterpret_cast<void**>(&G.nrm_c), P * 4ull},
+      {reinterpret_cast<void**>(&G.ea), Rp * d3 * 2},         {reinterpret_cast<void**>(&G.cb), Cp * d3 * 2},
+      {reinterpret_cast<void**>(&G.et), Np * d3 * 2},         {reinterpret_cast<void**>(&G.ct), Cp * d3 * 2},
+      {reinterpret_cast<void**>(&G.da), 3ull * Rp * Cp * 2},  {reinterpret_cast<void**>(&G.dt), 3ull * Np * Cp * 2},
+      {reinterpret_cast<void**>(&G.gcos), 1ull * Rp * Cp * 4}, {reinterpret_cast<void**>(&G.dcos), 1ull * Np * Cp * 4},
+      {reinterpret_cast<void**>(&G.rinv), Rp * 4ull},         {reinterpret_cast<void**>(&G.cinv), Cp * 4ull},
+      {reinterpret_cast<void**>(&G.ge), 1ull * sc * Rp * D * 4}, {reinterpret_cast<void**>(&G.gc), 1ull * sn * Cp * D * 4},
+      {reinterpret_cast<void**>(&G.gcent), pd},               {reinterpret_cast<void**>(&G.own), 1ull * Rp * D * 4},
+      {reinterpret_cast<void**>(&G.xg), 1ull * N * D * 4},    {reinterpret_cast<void**>(&G.ones), Rp * 4ull}};
   size_t off = 0;
   for (auto& p : parts) off += (p.second + 255) / 256 * 256;
   CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&G.buf), off));
+  // zero once: the rows [rows, Rp) of the dcos image, and (written by dsk_ge2e_bwd's path) the workspace rows [N, Np),
+  // are never written again
+  CUDA_TRY(cudaMemsetAsync(G.buf, 0, off, s));
   off = 0;
   for (auto& p : parts) {
     *p.first = G.buf + off;
     off += (p.second + 255) / 256 * 256;
   }
-  const std::vector<float> ones(N, 1.f);
-  CUDA_TRY(cudaMemcpy(G.ones, ones.data(), N * 4ull, cudaMemcpyHostToDevice));
+  const std::vector<float> ones(Rp, 1.f);
+  CUDA_TRY(cudaMemcpyAsync(G.ones, ones.data(), Rp * 4ull, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaStreamSynchronize(s));
+  // cos = E^ C^T for the range (K = 3D); gE^ = dcos C^ for the range (K = 3Cp) and gC^ = dcos^T E^ over all N rows
+  // (K = 3Np), one GEMM per K slice into the slice's own output (the AAM op's deterministic split K)
+  int rc = aam_build_gemm(h, &G.fwd, G.ea, Rp, G.cb, Cp, 3 * D, G.gcos);
+  const size_t ks = dsk::kAamSlice;
+  for (int k = 0; k < sc && !rc; ++k) {
+    const int w = Cp - k * dsk::kAamSlice < dsk::kAamSlice ? Cp - k * dsk::kAamSlice : dsk::kAamSlice;
+    rc = aam_build_gemm(h, &G.ge_gemm, G.da + k * ks * 3 * Rp, Rp, G.ct + k * ks * 3 * D, D, 3 * w,
+                        G.ge + static_cast<size_t>(k) * Rp * D);
+  }
+  for (int k = 0; k < sn && !rc; ++k) {
+    const int w = Np - k * dsk::kAamSlice < dsk::kAamSlice ? Np - k * dsk::kAamSlice : dsk::kAamSlice;
+    rc = aam_build_gemm(h, &G.gc_gemm, G.dt + k * ks * 3 * Cp, Cp, G.et + k * ks * 3 * D, D, 3 * w,
+                        G.gc + static_cast<size_t>(k) * Cp * D);
+  }
+  if (rc) {
+    cudaFree(G.buf);
+    G = Ge2ePlan();
+    return rc;
+  }
   G.N = N;
   G.P = P;
   G.D = D;
+  G.row0 = row0;
+  G.rows = rows;
+  G.Np = Np;
+  G.Rp = Rp;
+  G.Cp = Cp;
+  G.sc = sc;
+  G.sn = sn;
   return DSK_OK;
 }
 
-static int ge2e_check(dsk_handle h, bool ptrs_ok, int N, int D, int P, int V, int method, const char* what) {
+// The argument checks of the GE2E entry points, before any launch.  An op without a D, V or method passes 64, 1 and
+// DSK_GE2E_SOFTMAX for them; the whole-batch ops pass the range (0, N).
+static int ge2e_check(bool ptrs_ok, int N, int D, int P, int V, int method, int row0, int rows, const char* what) {
   if (!ptrs_ok || N < 2 || P < 2 || P > DSK_AAM_MAX_C || P > N || D < 64 || D % 64 || V < 1 || V > N ||
-      (method != DSK_GE2E_SOFTMAX && method != DSK_GE2E_CONTRAST))
+      (method != DSK_GE2E_SOFTMAX && method != DSK_GE2E_CONTRAST) || row0 < 0 || rows < 1 || row0 > N - rows)
     return fail(DSK_ERR_INVALID, "%s: bad arguments (need non-null pointers, 2 <= P <= min(N, %d), D a positive multiple "
-                "of 64, 1 <= V <= N and method DSK_GE2E_SOFTMAX or DSK_GE2E_CONTRAST; got N %d, P %d, D %d, V %d, "
-                "method %d)", what, DSK_AAM_MAX_C, N, P, D, V, method);
-  return check_handle(h);
+                "of 64, 1 <= V <= N, method DSK_GE2E_SOFTMAX or DSK_GE2E_CONTRAST, 0 <= row0, 1 <= rows and "
+                "row0 + rows <= N; got N %d, P %d, D %d, V %d, method %d, row0 %d, rows %d)", what, DSK_AAM_MAX_C, N,
+                P, D, V, method, row0, rows);
+  return DSK_OK;
 }
 
-// inclusive centroids, fp64 row norms, and the AAM plan's norms / operand images of E and the centroids
-static int ge2e_prep(const Ge2ePlan& G, const float* E, const int64_t* order, const int64_t* offsets, bool backward,
-                     cudaStream_t s) {
+// inclusive centroids, fp64 row norms and the centroids' fp32 norms: always over the whole batch
+static int ge2e_centroids(const Ge2ePlan& G, const float* E, const int64_t* order, const int64_t* offsets,
+                          cudaStream_t s) {
   dsk::class_centroids_kernel<<<dim3(G.P, (G.D + 255) / 256), 256, 0, s>>>(E, G.N, G.D, order, offsets, G.cent);
   KERNEL_CHECK();
   dsk::ge2e_norm64_kernel<<<(G.N + 7) / 8, 256, 0, s>>>(E, G.N, G.D, G.nr64);
   KERNEL_CHECK();
-  return aam_prep(G.g, E, G.cent, backward, s);
+  dsk::aam_norm_kernel<<<(G.P + 7) / 8, 256, 0, s>>>(G.cent, G.P, G.D, G.nrm_c);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// dsk_ge2e_rows after its checks
+static int ge2e_rows_run(dsk_handle h, const float* E, int N, int D, const int64_t* order, const int64_t* offsets,
+                         const int64_t* col, int P, const float* w, const float* b, int method, int row0, int rows,
+                         float* cos, float* rec, float* row_loss, cudaStream_t s) {
+  Ge2ePlan* G = nullptr;
+  int rc = ge2e_plan(h, N, P, D, row0, rows, s, &G);
+  if (rc || (rc = ge2e_centroids(*G, E, order, offsets, s))) return rc;
+  const float* Er = E + static_cast<size_t>(row0) * D;
+  dsk::aam_norm_kernel<<<(rows + 7) / 8, 256, 0, s>>>(Er, rows, D, G->nrm_e + row0);
+  KERNEL_CHECK();
+  dsk::aam_split_kernel<<<dim3(D / 64, G->Rp / 32), 256, 0, s>>>(Er, G->nrm_e + row0, rows, G->Rp, D, 1, G->ea, nullptr);
+  KERNEL_CHECK();
+  dsk::aam_split_kernel<<<dim3(D / 64, G->Cp / 32), 256, 0, s>>>(G->cent, G->nrm_c, P, G->Cp, D, 0, G->cb, nullptr);
+  KERNEL_CHECK();
+  for (const ConvLaunch& L : G->fwd)
+    if ((rc = launch_gemm_f16(L, s))) return rc;
+  dsk::ge2e_rows_kernel<<<rows, 256, 0, s>>>(G->gcos, G->Cp, E, D, G->nr64, order, offsets, col, P, w, b, method, row0,
+                                             cos, rec, row_loss);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// dsk_ge2e_dcos_rows after its checks; part: a [2][rows] fp64 workspace.  With G (the plan of the range (0, N), for
+// dsk_ge2e_bwd) the rows go straight into G's zero-padded dcos workspace and gE^ image instead of `dcos`.
+static int ge2e_dcos_run(const float* cos, const float* rec, const int64_t* offsets, const int64_t* col, int P, int V,
+                         const float* w, const float* b, int method, const float* grad_loss, int row0, int rows,
+                         float* dcos, float* tdc, float* gw, float* gb, double* part, Ge2ePlan* G, cudaStream_t s) {
+  if (G)
+    dsk::ge2e_dcos_rows_kernel<<<rows, 256, 0, s>>>(cos, rec, offsets, col, row0, P, V, w, b, method, grad_loss,
+                                                    G->dcos, G->Cp, tdc, part, G->Cp, G->Rp, G->da, G->rinv);
+  else
+    dsk::ge2e_dcos_rows_kernel<<<rows, 256, 0, s>>>(cos, rec, offsets, col, row0, P, V, w, b, method, grad_loss, dcos,
+                                                    P, tdc, part, P, 0, nullptr, nullptr);
+  KERNEL_CHECK();
+  dsk::ge2e_scalars_kernel<<<1, 256, 0, s>>>(part, rows, w, method, gw, gb);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// dsk_ge2e_bwd_rows after its checks; dcos == NULL: the plan's dcos workspace and gE^ image are already built (by
+// ge2e_dcos_run with the plan, in dsk_ge2e_bwd)
+static int ge2e_bwd_rows_run(dsk_handle h, const float* E, int N, int D, const int64_t* order, const int64_t* offsets,
+                             const int64_t* col, int P, const float* dcos, const float* tdc, int row0, int rows,
+                             float* gE_rows, cudaStream_t s) {
+  Ge2ePlan* G = nullptr;
+  int rc = ge2e_plan(h, N, P, D, row0, rows, s, &G);
+  if (rc || (rc = ge2e_centroids(*G, E, order, offsets, s))) return rc;
+  const int Np = G->Np, Rp = G->Rp, Cp = G->Cp;
+  dsk::aam_norm_kernel<<<(N + 7) / 8, 256, 0, s>>>(E, N, D, G->nrm_e);
+  KERNEL_CHECK();
+  dsk::aam_split_kernel<<<dim3(D / 64, Np / 32), 256, 0, s>>>(E, G->nrm_e, N, Np, D, 1, nullptr, G->et);
+  KERNEL_CHECK();
+  dsk::aam_split_kernel<<<dim3(D / 64, Cp / 32), 256, 0, s>>>(G->cent, G->nrm_c, P, Cp, D, 0, nullptr, G->ct);
+  KERNEL_CHECK();
+  if (dcos) {
+    dsk::ge2e_dcos_img_kernel<<<Np, 256, 0, s>>>(dcos, N, P, Cp, row0, rows, Rp, G->dcos, G->da, G->rinv);
+    KERNEL_CHECK();
+  }
+  dsk::aam_dcos_t_kernel<<<Cp / 32, 256, 0, s>>>(G->dcos, Np, Cp, G->dt, G->cinv);
+  KERNEL_CHECK();
+  for (const ConvLaunch& L : G->ge_gemm)  // dcos C^ for the range (target column zeroed)
+    if ((rc = launch_gemm_f16(L, s))) return rc;
+  for (const ConvLaunch& L : G->gc_gemm)  // dcos^T E^ over all N rows: the gradient w.r.t. the normalised centroids
+    if ((rc = launch_gemm_f16(L, s))) return rc;
+  dsk::aam_normalize_bwd_kernel<<<(P + 7) / 8, 256, 0, s>>>(G->cent, G->nrm_c, G->gc, G->sn, static_cast<long>(Cp) * D,
+                                                            G->cinv, P, D, G->gcent);
+  KERNEL_CHECK();
+  dsk::ge2e_excl_bwd_kernel<<<N, 256, 0, s>>>(E, D, G->nr64, order, offsets, col, tdc, row0, rows, G->own, G->xg);
+  KERNEL_CHECK();
+  dsk::ge2e_gather_kernel<<<dim3(rows, (D + 255) / 256), 256, 0, s>>>(G->ge, G->sc, static_cast<long>(Rp) * D, G->rinv,
+                                                                      G->gcent, order, offsets, col, G->xg, D, row0,
+                                                                      G->own);
+  KERNEL_CHECK();
+  dsk::aam_normalize_bwd_kernel<<<(rows + 7) / 8, 256, 0, s>>>(E + static_cast<size_t>(row0) * D, G->nrm_e + row0,
+                                                               G->own, 1, 0, G->ones, rows, D, gE_rows);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_ge2e_rows(dsk_handle h, const float* E, int32_t N, int32_t D, const int64_t* order, const int64_t* offsets,
+                      const int64_t* col, int32_t P, int32_t V, const float* w, const float* b, int32_t method,
+                      int32_t row0, int32_t rows, float* cos, float* rec, float* row_loss, void* stream) {
+  int rc = ge2e_check(E && order && offsets && col && w && b && cos && rec && row_loss, N, D, P, V, method, row0, rows,
+                      "dsk_ge2e_rows");
+  if (rc || (rc = check_handle(h))) return rc;
+  return ge2e_rows_run(h, E, N, D, order, offsets, col, P, w, b, method, row0, rows, cos, rec, row_loss,
+                       static_cast<cudaStream_t>(stream));
+}
+
+int32_t dsk_ge2e_mean(const float* row_loss, int32_t N, int32_t V, float* loss, void* stream) {
+  if (!row_loss || !loss || N < 2 || V < 1 || V > N)
+    return fail(DSK_ERR_INVALID, "dsk_ge2e_mean: bad arguments (need non-null pointers, N >= 2 and 1 <= V <= N; got N "
+                "%d, V %d)", N, V);
+  dsk::mean_rows_kernel<<<1, 1024, 0, static_cast<cudaStream_t>(stream)>>>(row_loss, N, V, loss);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_ge2e_dcos_rows(const float* cos, const float* rec, int32_t N, const int64_t* offsets, const int64_t* col,
+                           int32_t P, int32_t V, const float* w, const float* b, int32_t method, const float* grad_loss,
+                           int32_t row0, int32_t rows, float* dcos, float* tdc, float* gw, float* gb, void* stream) {
+  int rc = ge2e_check(cos && rec && offsets && col && w && b && grad_loss && dcos && tdc && gw && gb, N, 64, P, V,
+                      method, row0, rows, "dsk_ge2e_dcos_rows");
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  double* part = nullptr;
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&part), 2ull * rows * sizeof(double), s));
+  rc = ge2e_dcos_run(cos, rec, offsets, col, P, V, w, b, method, grad_loss, row0, rows, dcos, tdc, gw, gb, part,
+                     nullptr, s);
+  CUDA_TRY(cudaFreeAsync(part, s));
+  return rc;
+}
+
+int32_t dsk_ge2e_bwd_rows(dsk_handle h, const float* E, int32_t N, int32_t D, const int64_t* order,
+                          const int64_t* offsets, const int64_t* col, int32_t P, const float* dcos, const float* tdc,
+                          int32_t row0, int32_t rows, float* gE_rows, void* stream) {
+  int rc = ge2e_check(E && order && offsets && col && dcos && tdc && gE_rows, N, D, P, 1, DSK_GE2E_SOFTMAX, row0, rows,
+                      "dsk_ge2e_bwd_rows");
+  if (rc || (rc = check_handle(h))) return rc;
+  return ge2e_bwd_rows_run(h, E, N, D, order, offsets, col, P, dcos, tdc, row0, rows, gE_rows,
+                           static_cast<cudaStream_t>(stream));
 }
 
 int32_t dsk_ge2e(dsk_handle h, const float* E, int32_t N, int32_t D, const int64_t* order, const int64_t* offsets,
                  const int64_t* col, int32_t P, int32_t V, const float* w, const float* b, int32_t method, float* loss,
                  float* cos, float* rec, void* stream) {
-  int rc = ge2e_check(h, E && order && offsets && col && w && b && loss && cos && rec, N, D, P, V, method, "dsk_ge2e");
-  if (rc) return rc;
+  int rc = ge2e_check(E && order && offsets && col && w && b && loss && cos && rec, N, D, P, V, method, 0, N, "dsk_ge2e");
+  if (rc || (rc = check_handle(h))) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   Ge2ePlan* G = nullptr;
-  if ((rc = ge2e_plan(h, N, P, D, s, &G))) return rc;
-  if ((rc = ge2e_prep(*G, E, order, offsets, false, s))) return rc;
-  for (const ConvLaunch& L : G->g.fwd)
-    if ((rc = launch_gemm_f16(L, s))) return rc;
-  dsk::ge2e_rows_kernel<<<N, 256, 0, s>>>(G->g.gcos, G->g.Cp, E, D, G->nr64, order, offsets, col, P, w, b, method, cos,
-                                          rec, G->g.row_loss);
-  KERNEL_CHECK();
-  dsk::mean_rows_kernel<<<1, 1024, 0, s>>>(G->g.row_loss, N, V, loss);
-  KERNEL_CHECK();
-  return DSK_OK;
+  if ((rc = ge2e_plan(h, N, P, D, 0, N, s, &G))) return rc;
+  rc = ge2e_rows_run(h, E, N, D, order, offsets, col, P, w, b, method, 0, N, cos, rec, G->row_loss, s);
+  return rc ? rc : dsk_ge2e_mean(G->row_loss, N, V, loss, stream);
 }
 
 int32_t dsk_ge2e_bwd(dsk_handle h, const float* E, int32_t N, int32_t D, const int64_t* order, const int64_t* offsets,
                      const int64_t* col, int32_t P, int32_t V, const float* w, const float* b, int32_t method,
                      const float* cos, const float* rec, const float* grad_loss, float* gE, float* gw, float* gb,
                      void* stream) {
-  int rc = ge2e_check(h, E && order && offsets && col && w && b && cos && rec && grad_loss && gE && gw && gb, N, D, P, V,
-                      method, "dsk_ge2e_bwd");
-  if (rc) return rc;
+  int rc = ge2e_check(E && order && offsets && col && w && b && cos && rec && grad_loss && gE && gw && gb, N, D, P, V,
+                      method, 0, N, "dsk_ge2e_bwd");
+  if (rc || (rc = check_handle(h))) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   Ge2ePlan* G = nullptr;
-  if ((rc = ge2e_plan(h, N, P, D, s, &G))) return rc;
-  const AamPlan& A = G->g;
-  if ((rc = ge2e_prep(*G, E, order, offsets, true, s))) return rc;
-  dsk::ge2e_dcos_kernel<<<A.Np, 256, 0, s>>>(cos, rec, offsets, col, N, P, A.Cp, V, w, b, method, grad_loss, A.dcos,
-                                             A.da, A.rinv, G->tdc, G->part);
-  KERNEL_CHECK();
-  dsk::aam_dcos_t_kernel<<<A.Cp / 32, 256, 0, s>>>(A.dcos, A.Np, A.Cp, A.dt, A.cinv);
-  KERNEL_CHECK();
-  for (const ConvLaunch& L : A.ge_gemm)  // dcos C^ (target column zeroed)
-    if ((rc = launch_gemm_f16(L, s))) return rc;
-  for (const ConvLaunch& L : A.gw_gemm)  // dcos^T E^: the gradient w.r.t. the normalised inclusive centroids
-    if ((rc = launch_gemm_f16(L, s))) return rc;
-  dsk::aam_normalize_bwd_kernel<<<(P + 7) / 8, 256, 0, s>>>(G->cent, A.nrm_w, A.gw, A.sn, static_cast<long>(A.Cp) * D,
-                                                            A.cinv, P, D, G->gcent);
-  KERNEL_CHECK();
-  dsk::ge2e_excl_bwd_kernel<<<N, 256, 0, s>>>(E, D, G->nr64, order, offsets, col, G->tdc, G->own, G->xg);
-  KERNEL_CHECK();
-  dsk::ge2e_gather_kernel<<<dim3(N, (D + 255) / 256), 256, 0, s>>>(A.ge, A.sc, static_cast<long>(A.Np) * D, A.rinv,
-                                                                   G->gcent, order, offsets, col, G->xg, D, G->own);
-  KERNEL_CHECK();
-  dsk::aam_normalize_bwd_kernel<<<(N + 7) / 8, 256, 0, s>>>(E, A.nrm_e, G->own, 1, 0, G->ones, N, D, gE);
-  KERNEL_CHECK();
-  dsk::ge2e_scalars_kernel<<<1, 256, 0, s>>>(G->part, N, A.Np, w, method, gw, gb);
-  KERNEL_CHECK();
-  return DSK_OK;
+  if ((rc = ge2e_plan(h, N, P, D, 0, N, s, &G))) return rc;
+  // the dcos rows of all N go straight into the padded workspace and the gE^ image: no (N, P) round trip
+  rc = ge2e_dcos_run(cos, rec, offsets, col, P, V, w, b, method, grad_loss, 0, N, nullptr, G->tdc, gw, gb, G->part, G,
+                     s);
+  return rc ? rc : ge2e_bwd_rows_run(h, E, N, D, order, offsets, col, P, nullptr, G->tdc, 0, N, gE, s);
 }
 
 // ---- cosine scoring, cohort statistics (AS-norm) ------------------------------------------------------------------

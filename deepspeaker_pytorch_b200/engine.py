@@ -501,6 +501,85 @@ def ge2e_backward(E, csr, V, w, b, method, cos, rec, grad_loss):
     return gE, gw, gb
 
 
+def ge2e_rows(E, csr, V, w, b, method, row0, rows):
+    """dsk_ge2e_rows: rows [row0, row0 + rows) of ``ge2e`` on the whole batch E (N, D) -> (E fp32 contiguous, cos
+    (rows, P), rec (rows,), row_loss (rows,)), the same bits as those rows of ``ge2e``.  ``csr`` is the whole batch's.
+    The plan is cached per (N, P, D, row0, rows)."""
+    m = _ge2e_method(method)
+    if not E.is_cuda or E.dim() != 2:
+        raise RuntimeError(f"GE2E: expected CUDA embeddings (N, D), got {tuple(E.shape)} on {E.device}")
+    E = E.detach().float().contiguous()
+    order, offsets, col = csr
+    (N, D), P, dev, n = E.shape, offsets.numel() - 1, E.device, max(int(rows), 0)
+    if order.numel() != N or col.numel() != N:
+        raise RuntimeError(f"GE2E: {order.numel()} labels for {N} embeddings")
+    for t in (order, offsets, col, w, b):
+        if t.device != dev:
+            raise RuntimeError("GE2E: embeddings, speaker lists and the scalars w, b must be on one device")
+    cos = torch.empty(n, P, device=dev, dtype=torch.float32)
+    rec, row_loss = (torch.empty(n, device=dev, dtype=torch.float32) for _ in range(2))
+    with torch.cuda.device(dev):
+        L.check(L.load().dsk_ge2e_rows(_allpairs_handle(dev), E.data_ptr(), N, D, order.data_ptr(), offsets.data_ptr(),
+                                       col.data_ptr(), P, int(V), w.data_ptr(), b.data_ptr(), m, int(row0), int(rows),
+                                       cos.data_ptr(), rec.data_ptr(), row_loss.data_ptr(), L.cur_stream()),
+                "dsk_ge2e_rows")
+    return E, cos, rec, row_loss
+
+
+def ge2e_mean(row_loss, V):
+    """dsk_ge2e_mean: loss (1,) from the row losses (N,) of the whole batch, the bits of ``ge2e``'s loss."""
+    loss = torch.empty(1, device=row_loss.device, dtype=torch.float32)
+    with torch.cuda.device(row_loss.device):
+        L.check(L.load().dsk_ge2e_mean(row_loss.data_ptr(), row_loss.numel(), int(V), loss.data_ptr(), L.cur_stream()),
+                "dsk_ge2e_mean")
+    return loss
+
+
+def ge2e_dcos_rows(cos, rec, csr, V, w, b, method, row0, rows, grad_loss):
+    """dsk_ge2e_dcos_rows: from the range's ``ge2e_rows`` outputs -> (dcos (rows, P) with the target column zeroed, tdc
+    (rows,) the target column's dcos, gw (), gb ()): the range's part of ``ge2e_backward`` and its shares of gw, gb."""
+    _, offsets, col = csr
+    n, P = max(int(rows), 0), offsets.numel() - 1
+    dev = cos.device
+    if tuple(cos.shape) != (n, P) or tuple(rec.shape) != (n,):
+        raise RuntimeError(f"GE2E: expected cos ({n}, {P}) and rec ({n},) of the row range, got {tuple(cos.shape)} "
+                           f"and {tuple(rec.shape)}")
+    for t in (cos, rec, offsets, col, w, b):
+        if not t.is_cuda or t.device != dev:
+            raise RuntimeError("GE2E: cos, rec, speaker lists and the scalars w, b must be on one CUDA device")
+    cos, rec = cos.float().contiguous(), rec.float().contiguous()
+    gl = grad_loss.float().reshape(1).contiguous()
+    dcos = torch.empty(n, P, device=dev, dtype=torch.float32)
+    tdc = torch.empty(n, device=dev, dtype=torch.float32)
+    gw, gb = (torch.empty((), device=dev, dtype=torch.float32) for _ in range(2))
+    with torch.cuda.device(dev):
+        L.check(L.load().dsk_ge2e_dcos_rows(cos.data_ptr(), rec.data_ptr(), col.numel(), offsets.data_ptr(),
+                                            col.data_ptr(), P, int(V), w.data_ptr(), b.data_ptr(), _ge2e_method(method),
+                                            gl.data_ptr(), int(row0), int(rows), dcos.data_ptr(), tdc.data_ptr(),
+                                            gw.data_ptr(), gb.data_ptr(), L.cur_stream()), "dsk_ge2e_dcos_rows")
+    return dcos, tdc, gw, gb
+
+
+def ge2e_backward_rows(E, csr, dcos, tdc, row0, rows):
+    """dsk_ge2e_bwd_rows: rows [row0, row0 + rows) of ``ge2e_backward``'s gE -> (rows, D), the same bits.  ``dcos``
+    (N, P) and ``tdc`` (N,) are every range's ``ge2e_dcos_rows`` outputs, concatenated in row order."""
+    order, offsets, col = csr
+    (N, D), P = E.shape, offsets.numel() - 1
+    if dcos.shape != (N, P) or tdc.shape != (N,):
+        raise RuntimeError(f"GE2E: expected dcos ({N}, {P}) and tdc ({N},), got {tuple(dcos.shape)} and "
+                           f"{tuple(tdc.shape)}")
+    if not E.is_cuda or any(t.device != E.device for t in (order, offsets, col, dcos, tdc)):
+        raise RuntimeError("GE2E: embeddings, speaker lists, dcos and tdc must be on one CUDA device")
+    E = E.detach().float().contiguous()
+    dcos, tdc = dcos.float().contiguous(), tdc.float().contiguous()
+    gE = torch.empty(max(int(rows), 0), D, device=E.device, dtype=torch.float32)
+    with torch.cuda.device(E.device):
+        L.check(L.load().dsk_ge2e_bwd_rows(_allpairs_handle(E.device), E.data_ptr(), N, D, order.data_ptr(),
+                                           offsets.data_ptr(), col.data_ptr(), P, dcos.data_ptr(), tdc.data_ptr(),
+                                           int(row0), int(rows), gE.data_ptr(), L.cur_stream()), "dsk_ge2e_bwd_rows")
+    return gE
+
+
 class GE2EFn(torch.autograd.Function):
     """GE2E loss over (E, w, b) against the batch's speaker centroids; the loss is a device scalar.  ``csr`` and ``V``
     as in ``ge2e``."""

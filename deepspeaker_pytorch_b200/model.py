@@ -284,6 +284,15 @@ def ge2e_batch(labels):
     return order, offsets, col, V
 
 
+def ge2e_csr_to(order, offsets, col, device):
+    """``ge2e_batch``'s speaker lists as int64 tensors (order, offsets, col) on ``device``: to a CUDA device one pinned
+    copy, queued on the stream like a kernel."""
+    host = torch.from_numpy(np.concatenate([order, offsets, col]))
+    flat = host.pin_memory().to(device, non_blocking=True) if torch.device(device).type == "cuda" else host
+    N, P = order.size, offsets.size - 1
+    return flat[:N], flat[N:N + P + 1], flat[N + P + 1:]
+
+
 class GE2ELoss(nn.Module):
     """Generalised end-to-end loss (Wan et al., "Generalized End-to-End Loss for Speaker Verification", ICASSP 2018; no
     reference implementation) over a batch of P speakers x M utterances.  Every utterance is scored against every
@@ -322,11 +331,7 @@ class GE2ELoss(nn.Module):
         dev = embeddings.device
         if self.w.device != dev:
             raise RuntimeError("GE2ELoss: move the loss to the embeddings' device (loss.to(device))")
-        # one pinned copy, queued on the stream like a kernel
-        host = torch.from_numpy(np.concatenate([order, offsets, col])).pin_memory()
-        flat = host.to(dev, non_blocking=True)
-        N, P = order.size, offsets.size - 1
-        csr = (flat[:N], flat[N:N + P + 1], flat[N + P + 1:])
+        csr = ge2e_csr_to(order, offsets, col, dev)
         return _engine.GE2EFn.apply(embeddings, self.w, self.b, csr, V, self.method)
 
 

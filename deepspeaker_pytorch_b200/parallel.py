@@ -12,6 +12,10 @@ Batch-hard mining over the global batch (``GlobalBatchHardTripletLoss``, ``batch
 adds three small all_gathers per step: the labels, the fp32 embeddings and the selection records.  The gradient
 reduction stays the one all-reduce.
 
+GE2E over the global batch (``GlobalGE2ELoss``, ``ge2e_step(..., across_ranks=True)``) adds the same labels gather, two
+all_gathers in the forward (the fp32 embeddings, the row losses) and one in the backward (each row's dcos and the target
+column's dcos).  The gradient reduction stays the one all-reduce.
+
 Synchronised BatchNorm adds one all_gather of per-utterance records at each of the 12 BatchNorm layers of a forward
 and at 13 points of its backward (the loss scale, then the 12 layers); see ``gather_records`` for the record sizes.
 """
@@ -199,6 +203,88 @@ class GlobalBatchHardTripletLoss:
             raise ValueError(f"expected global labels of shape ({world * local_emb.shape[0]},) for {world} ranks of "
                              f"{local_emb.shape[0]} embeddings, got {tuple(global_labels.shape)}")
         return _GlobalBatchHardFn.apply(local_emb, global_labels, float(self.margin), self.exact_cuda_cores, self.group)
+
+    __call__ = forward
+
+
+# ---- GE2E over the global batch -----------------------------------------------------------------------------------------
+# Same layout and precondition as batch-hard: rank r holds the rows [r n, (r + 1) n) of N = R n, every rank the same n.
+
+class _GlobalGE2EFn(torch.autograd.Function):
+    """Forward: all_gather of the fp32 embeddings, this rank's rows of the GE2E op against the centroids of all N rows,
+    all_gather of the row losses, the mean over the global V.  Backward: this rank's dcos rows, ONE all_gather of (dcos,
+    tdc) rows, this rank's rows of gE; gw and gb are this rank's shares."""
+
+    @staticmethod
+    def forward(ctx, local_emb, w, b, csr, V, method, group):
+        world, rank = dist.get_world_size(group), dist.get_rank(group)
+        x = local_emb.detach().float().contiguous()
+        n = x.shape[0]
+        E = x.new_empty(world * n, x.shape[1])
+        dist.all_gather_into_tensor(E, x, group=group)
+        row0 = rank * n
+        wc, bc = (t.detach().float().reshape(1).contiguous() for t in (w, b))
+        E, cos, rec, row_loss = _engine.ge2e_rows(E, csr, V, wc, bc, method, row0, n)
+        losses = row_loss.new_empty(world * n)
+        dist.all_gather_into_tensor(losses, row_loss.contiguous(), group=group)
+        loss = _engine.ge2e_mean(losses, V)
+        ctx.save_for_backward(E, wc, bc, cos, rec, *csr)
+        ctx.V, ctx.method, ctx.group, ctx.row0, ctx.n = V, method, group, row0, n
+        ctx.shapes = (w.shape, b.shape)
+        return loss.reshape(())
+
+    @staticmethod
+    def backward(ctx, gl):
+        E, w, b, cos, rec, *csr = ctx.saved_tensors
+        dcos, tdc, gw, gb = _engine.ge2e_dcos_rows(cos, rec, csr, ctx.V, w, b, ctx.method, ctx.row0, ctx.n, gl)
+        world, P = dist.get_world_size(ctx.group), dcos.shape[1]
+        rows = torch.cat([dcos, tdc.reshape(-1, 1)], dim=1)             # (n, P + 1): one record per row
+        out = rows.new_empty(world * ctx.n, P + 1)
+        dist.all_gather_into_tensor(out, rows, group=ctx.group)
+        gE = _engine.ge2e_backward_rows(E, csr, out[:, :P], out[:, P], ctx.row0, ctx.n)
+        ni = ctx.needs_input_grad
+        return (gE if ni[0] else None, gw.reshape(ctx.shapes[0]) if ni[1] else None,
+                gb.reshape(ctx.shapes[1]) if ni[2] else None, None, None, None, None)
+
+
+class GlobalGE2ELoss:
+    """``GE2ELoss`` over the GLOBAL batch under data parallelism: every utterance is scored against the centroids of all
+    N = R n utterances, and its own speaker's leave-one-out centroid takes that speaker's rows from every rank, so a
+    speaker may span any number of ranks.  The loss is the same device scalar on every rank and bit-identical to
+    ``loss`` on the gathered embeddings with the global labels; its gradient w.r.t. ``local_emb`` is this rank's rows of
+    that loss's gradient, bit for bit.  The gradients of ``loss.w`` and ``loss.b`` are this rank's shares: summed over
+    ranks (the mean all-reduce of the gradients scaled by R, as ``ge2e_step(..., across_ranks=True)`` does) they are
+    the global loss's, to ~1e-7 relative.
+
+    Collectives: two all_gathers in the forward (embeddings N·D·4 bytes, row losses N·4 bytes) and one in the backward
+    (dcos rows and the target column's dcos, N·(P + 1)·4 bytes).  The labels are an input: gather them once per batch
+    with ``gather_labels``; they are read on the host to build the speaker lists (CPU labels need no device
+    synchronisation).  Precondition: every rank holds the same n.  Without a process group, or at world size 1, this is
+    exactly ``loss(local_emb, global_labels)`` and issues no collective."""
+
+    def __init__(self, loss, process_group=None):
+        self.loss = loss
+        self.group = process_group
+
+    def forward(self, local_emb, global_labels):
+        """local_emb (n, D) this rank's shard, global_labels (N,) int of the whole batch -> 0-dim loss."""
+        from .model import ge2e_batch, ge2e_csr_to
+
+        if not _distributed(self.group):
+            return self.loss(local_emb, global_labels)
+        world = dist.get_world_size(self.group)
+        if tuple(global_labels.shape) != (world * local_emb.shape[0],):
+            raise ValueError(f"expected global labels of shape ({world * local_emb.shape[0]},) for {world} ranks of "
+                             f"{local_emb.shape[0]} embeddings, got {tuple(global_labels.shape)}")
+        order, offsets, col, V = ge2e_batch(global_labels)
+        if V == 0:
+            raise ValueError("GlobalGE2ELoss: no utterance of the global batch contributes to the loss (it needs >= 2 "
+                             "speakers, one of them with >= 2 utterances)")
+        dev = local_emb.device
+        if self.loss.w.device != dev:
+            raise RuntimeError("GlobalGE2ELoss: move the loss to the embeddings' device (loss.to(device))")
+        csr = ge2e_csr_to(order, offsets, col, dev)
+        return _GlobalGE2EFn.apply(local_emb, self.loss.w, self.loss.b, csr, V, self.loss.method, self.group)
 
     __call__ = forward
 

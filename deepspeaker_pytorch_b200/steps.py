@@ -32,7 +32,7 @@ from .head import CrossEntropyLoss
 from .model import (AAMSoftmaxLoss, BatchHardTripletLoss, PairwiseDistance, TripletMarginLoss, batch_hard_valid_count,
                     select_hard_triplets)
 from .optim import FusedAdagrad
-from .parallel import GlobalBatchHardTripletLoss, _distributed, gather_labels
+from .parallel import GlobalBatchHardTripletLoss, GlobalGE2ELoss, _distributed, gather_labels
 
 _l2 = PairwiseDistance(2)   # train_triplet.py:119
 
@@ -189,28 +189,67 @@ def aam_softmax_step(model, optimizer, data, labels, *, margin, scale, bucket=No
     return {"loss": loss.detach()}
 
 
-def ge2e_step(model, optimizer, data, labels, *, loss, bucket=None):
+def _no_valid_ge2e_row():
+    return ValueError("ge2e_step: no utterance contributes to the loss (it needs >= 2 speakers, one of them with "
+                      ">= 2 utterances)")
+
+
+def ge2e_step(model, optimizer, data, labels, *, loss, bucket=None, across_ranks=False):
     """One step with the generalised end-to-end loss ``loss`` (a ``GE2ELoss``) on a P speakers x M utterances batch:
     ONE train-mode forward of all N utterances, the loss against the batch's speaker centroids, backward, optimizer step.
-    The optimizer (or ``bucket``) must hold ``loss.parameters()`` beside the model's: ``w`` and ``b`` are then averaged
+    The optimizer (or ``bucket``) must hold ``loss.parameters()`` beside the model's: ``w`` and ``b`` are then reduced
     in the same single all-reduce.  Returns ``{"loss": device scalar, "valid": V}``; raises ValueError for a batch with
     V = 0 (fewer than 2 speakers, or no speaker with 2 utterances).  With CPU labels the step reads nothing back from the
-    device.
+    device.  Runs unchanged on a model with ``sync_batchnorm()``.
 
-    Under data parallelism (``bucket`` or a ``FusedAdagrad`` optimizer) each rank's gradient is weighted by its own
-    number of valid utterances V_r, as in ``batch_hard_step``.  The centroids are each rank's own: a rank scores its
-    utterances against the speakers of its shard only, so the objective depends on the number of ranks R (keep each
-    speaker's utterances on one rank).  Runs unchanged on a model with ``sync_batchnorm()``."""
+    Data parallelism (``bucket`` or a ``FusedAdagrad`` optimizer; ``data`` / ``labels`` this rank's shard, the same size
+    on every rank) has two forms:
+
+    * ``across_ranks=False`` (the default): each rank computes GE2E on its own shard, against the centroids of the
+      speakers in that shard only, and its gradient is weighted by its number of valid utterances V_r, as in
+      ``batch_hard_step``.  The objective then depends on the number of ranks R: a softmax over R times fewer speakers,
+      and a speaker split over two ranks gets two smaller centroids.
+    * ``across_ranks=True``: GE2E over the GLOBAL batch with ``parallel.GlobalGE2ELoss``.  Every utterance is scored
+      against the centroids of all N = R n utterances and a speaker may span any number of ranks, so the loss does not
+      depend on R: it is bit-identical to ``GE2ELoss`` on the gathered embeddings.  The labels are gathered first and
+      read back to the host for the speaker lists and the global V - the step's one host synchronisation; every rank
+      then sees the same V, so on V = 0 all ranks raise before any other collective.  The backward is seeded with R:
+      the unchanged mean all-reduce of the gradients (/R, ``loss.parameters()`` in the same bucket) then sums the
+      ranks' gradients, which is the gradient of the global loss (exactly so for the embeddings at power-of-two R; w
+      and b are summed from per-rank shares).  The ranks are those of the optimizer's (``FusedAdagrad``) or the
+      bucket's process group.  BatchNorm statistics stay per replica by default; on a model with
+      ``sync_batchnorm(group)`` they are those of the global batch too, and the step's forward and loss are then those
+      of the single-device step on the gathered batch.  ``valid`` is the global V.  Without a process group this is
+      the step with ``across_ranks=False``."""
     if not model.training:
         raise RuntimeError("ge2e_step needs model.train()")
+    if across_ranks:
+        return _global_ge2e_step(model, optimizer, data, labels, loss, bucket)
     labels = torch.as_tensor(labels).detach().cpu()     # CUDA labels: the one read-back
     V = batch_hard_valid_count(labels)
     if V == 0:
-        raise ValueError("ge2e_step: no utterance contributes to the loss (it needs >= 2 speakers, one of them with "
-                         ">= 2 utterances)")
+        raise _no_valid_ge2e_row()
     emb = model(data)
     out = loss(emb, labels)
     optimizer.zero_grad()
     out.backward()
     _reduce_and_step(optimizer, bucket, torch.tensor(float(V)))
+    return {"loss": out.detach(), "valid": V}
+
+
+def _global_ge2e_step(model, optimizer, data, labels, loss, bucket):
+    group = optimizer.group if isinstance(optimizer, FusedAdagrad) else (bucket.group if bucket is not None else None)
+    if not _distributed(group):
+        return ge2e_step(model, optimizer, data, labels, loss=loss, bucket=bucket)
+    world = dist.get_world_size(group)
+    global_labels = gather_labels(_labels_to(labels, data.device), group)   # behind the last step's all-reduce
+    global_labels = global_labels.cpu()                                      # the step's one host synchronisation
+    V = batch_hard_valid_count(global_labels)
+    if V == 0:
+        raise _no_valid_ge2e_row()
+    emb = model(data)
+    out = GlobalGE2ELoss(loss, group).forward(emb, global_labels)
+    optimizer.zero_grad()
+    out.backward(torch.full_like(out, float(world)))         # R x this rank's share; the mean all-reduce divides by R
+    _reduce_and_step(optimizer, bucket, None)
     return {"loss": out.detach(), "valid": V}

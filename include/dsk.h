@@ -405,6 +405,33 @@ int32_t dsk_ge2e_bwd(dsk_handle h, const float* E, int32_t N, int32_t D, const i
                      const int64_t* col, int32_t P, int32_t V, const float* w, const float* b, int32_t method,
                      const float* cos, const float* rec, const float* grad_loss, float* gE, float* gw, float* gb,
                      void* stream);
+/* Row-range form of the GE2E op, for sharding the rows of one N-row batch E (e.g. across data-parallel ranks, each
+ * holding the gathered E) with results bit-identical to the whole-batch op.  The centroids, the exclusive centroid of
+ * every row and the fp64 row norms always come from all N rows, so a speaker's rows may sit anywhere in the batch.
+ * 0 <= row0, 1 <= rows, row0 + rows <= N, plus the limits of dsk_ge2e, else DSK_ERR_INVALID before any launch.
+ * The plan is cached in h for (N, P, D, row0, rows), in the GE2E slot; a change rebuilds it, which synchronises the
+ * stream.  dsk_ge2e = rows(0, N) + dsk_ge2e_mean;  dsk_ge2e_bwd = dcos_rows(0, N) + bwd_rows(0, N).
+ * dsk_ge2e_rows: rows [row0, row0 + rows) of dsk_ge2e's cos and rec into cos (rows, P) and rec (rows,), and the rows'
+ *   loss terms L_i (0 on invalid rows) into row_loss (rows,).  The cosine GEMM runs only for the rows x P block.
+ * dsk_ge2e_mean: dsk_ge2e's loss from row_loss (N,) of all N rows: (1/V) sum_i row_loss[i] in a fixed order.
+ * dsk_ge2e_dcos_rows: for the range, from its cos and rec (rows, P) / (rows,) and the whole batch's CSR: dcos (rows, P)
+ *   = max(w, 1e-6) dS as in dsk_ge2e_bwd, with the target column zeroed and its value in tdc (rows,); gw and gb (1,)
+ *   are the range's shares of dsk_ge2e_bwd's gw and gb (fp64 sums over the range's rows in a fixed order, rounded
+ *   once; gb exactly 0 for softmax).  Summed over the ranges of a split they equal the whole op's to ~1e-7 relative.
+ * dsk_ge2e_bwd_rows: rows [row0, row0 + rows) of dsk_ge2e_bwd's gE into gE_rows (rows, D), from dcos (N, P) and tdc
+ *   (N,) of ALL N rows (the concatenation of every range's dsk_ge2e_dcos_rows).  gC^ = dcos^T E^ runs over all N rows
+ *   in the whole op's K slices, the exclusive-centroid terms for the members of every speaker with a row in the range,
+ *   and gE^ = dcos C^ only for the rows x P block. */
+int32_t dsk_ge2e_rows(dsk_handle h, const float* E, int32_t N, int32_t D, const int64_t* order, const int64_t* offsets,
+                      const int64_t* col, int32_t P, int32_t V, const float* w, const float* b, int32_t method,
+                      int32_t row0, int32_t rows, float* cos, float* rec, float* row_loss, void* stream);
+int32_t dsk_ge2e_mean(const float* row_loss, int32_t N, int32_t V, float* loss, void* stream);
+int32_t dsk_ge2e_dcos_rows(const float* cos, const float* rec, int32_t N, const int64_t* offsets, const int64_t* col,
+                           int32_t P, int32_t V, const float* w, const float* b, int32_t method, const float* grad_loss,
+                           int32_t row0, int32_t rows, float* dcos, float* tdc, float* gw, float* gb, void* stream);
+int32_t dsk_ge2e_bwd_rows(dsk_handle h, const float* E, int32_t N, int32_t D, const int64_t* order,
+                          const int64_t* offsets, const int64_t* col, int32_t P, const float* dcos, const float* tdc,
+                          int32_t row0, int32_t rows, float* gE_rows, void* stream);
 
 /* Cosine scoring of verification trials with adaptive symmetric score normalisation (AS-norm) against an impostor
  * cohort (no reference implementation exists; the reference scores Euclidean distances, eval_metrics.py:5-50).  Rows are

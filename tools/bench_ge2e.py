@@ -6,7 +6,12 @@
   * utterances per second of ge2e_step at N = 384 (64 speakers x 6), T = 160 with FusedAdagrad (softmax), beside
     aam_softmax_step (C = 1211) and batch_hard_step (96 x 4) at the same size (events around --steps steps after
     --warmup, alternated twice);
+  * microseconds for one rank's share of the global-batch op at R = 8 (ge2e_rows + ge2e_mean + ge2e_dcos_rows +
+    ge2e_backward_rows for 384 of N = 3072 rows, P = 512, D = 512; the collectives' payloads taken as gathered) beside
+    the whole op at N = 3072, both methods;
   * the card's name and power limit (read-only nvidia-smi query in the same run).
+Under ``torchrun --nproc-per-node R``: ms per ge2e_step at 384 utterances per rank (64 x 6), T = 160, with across_ranks
+False vs True (rank 0 prints the line).
 Writes nothing but stdout.  Run: python tools/bench_ge2e.py
 """
 import argparse
@@ -64,6 +69,44 @@ def main():
                 rec[f"fwd_bwd_us_{key}_{method}_P{P}_M{M}"] = round(1e3 * time_events(fn, args.iters), 2)
         rec[f"tensor_gflop_P{P}_M{M}"] = round(3 * 3 * 2 * N * P * D / 1e9, 3)   # three GEMMs, hi/lo x3
 
+    # one rank's share of the global-batch op at R = 8: the rows ops for 384 of N = 3072 rows (512 speakers x 6), P =
+    # 512, forward + backward, beside the whole op at N = 3072 (what every rank would run on the gathered batch instead)
+    from deepspeaker_pytorch_b200 import engine as EN
+    from deepspeaker_pytorch_b200.model import ge2e_batch, ge2e_csr_to
+
+    N, rows, M = 3072, 384, 6
+    E = torch.randn(N, D, device=dev, generator=g)
+    E = 10.0 * E / E.norm(dim=1, keepdim=True)
+    order, offsets, col, V = ge2e_batch(torch.arange(N) % (N // M))      # every speaker spans the ranks
+    csr = ge2e_csr_to(order, offsets, col, dev)
+    w, b, one = (torch.full((1,), v, device=dev) for v in (10.0, -5.0, 1.0))
+    row0 = N - rows
+    for method in ("softmax", "contrast"):
+        Ec, _, cos, rec_all = EN.ge2e(E, csr, V, w, b, method)
+        row_loss = EN.ge2e_rows(E, csr, V, w, b, method, 0, N)[3]
+        dc_all, tdc_all, _, _ = EN.ge2e_dcos_rows(cos, rec_all, csr, V, w, b, method, 0, N, one)
+        cos_r, rec_r = cos[row0:].contiguous(), rec_all[row0:].contiguous()
+
+        def whole():
+            Ec, _, c, r = EN.ge2e(E, csr, V, w, b, method)
+            EN.ge2e_backward(Ec, csr, V, w, b, method, c, r, one)
+
+        def share():     # the collectives' payloads are taken as already gathered
+            EN.ge2e_rows(E, csr, V, w, b, method, row0, rows)
+            EN.ge2e_mean(row_loss, V)
+            EN.ge2e_dcos_rows(cos_r, rec_r, csr, V, w, b, method, row0, rows, one)
+            EN.ge2e_backward_rows(E, csr, dc_all, tdc_all, row0, rows)
+
+        for key, fn in ((f"whole_fwd_bwd_us_{method}_N3072", whole), (f"rows384_fwd_bwd_us_{method}_N3072", share)):
+            for _ in range(20):   # the first call of each (re)builds the plan for its row range
+                fn()
+            torch.cuda.synchronize()
+            rec[key] = round(1e3 * time_events(fn, args.iters), 2)
+    rec["rows_shape"] = {"N": N, "P": N // M, "D": D, "rows": rows, "ranks": N // rows,
+                         "tensor_gflop_whole": round(3 * 3 * 2 * N * (N // M) * D / 1e9, 2),
+                         "tensor_gflop_rows": round(3 * 2 * (2 * rows + N) * (N // M) * D / 1e9, 2)}
+    rec["data_parallel_step"] = "not measured in this run: run under torchrun --nproc-per-node R on R GPUs"
+
     Nst, T, C = 384, 160, 1211
     sd = O.make_state_dict(0, num_classes=C)
     x = torch.randn(Nst, 1, T, 64, device=dev, generator=g) * 3.0
@@ -100,5 +143,57 @@ def main():
     print(json.dumps(rec), flush=True)
 
 
+def main_distributed(args):
+    """Under torchrun: ms per ge2e_step at n = 384 utterances per rank, T = 160, softmax, with the centroids of the rank's
+    shard (across_ranks=False) vs of the global batch (across_ranks=True, including the label gather's host sync and the
+    three GE2E all_gathers).  Rank r holds its own 64 speakers x 6 utterances (speakers 64 r .. 64 r + 63), so both arms
+    run a full problem at every R: the shard arm 64 speakers x 6 per rank, the global arm P = 64 R speakers over
+    N = 384 R rows (P = 512 at R = 8).  The costs depend on N, P, D and the speaker sizes, not on which rank holds a
+    speaker's rows."""
+    import torch
+    import torch.distributed as dist
+
+    import deepspeaker_pytorch_b200 as dsk
+    from deepspeaker_pytorch_b200.model import ge2e_batch
+    from oracle import rescnn_oracle as O  # deterministic parameters only
+
+    rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
+    dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", rank)))
+    torch.cuda.set_device(dev)
+    dist.init_process_group("nccl", device_id=dev)
+    try:
+        n, M, T = 384, 6, 160
+        model = dsk.DeepSpeakerModel(512, 16).to(dev).train()
+        model.load_state_dict(O.make_state_dict(0, num_classes=16))
+        crit = dsk.GE2ELoss().to(dev)
+        opt = dsk.FusedAdagrad(list(model.parameters()) + list(crit.parameters()), lr=1e-3, lr_decay=1e-4)
+        g = torch.Generator(device=dev).manual_seed(rank)
+        x = torch.randn(n, 1, T, 64, device=dev, generator=g) * 3.0
+        lab = torch.arange(world * n)[rank * n:(rank + 1) * n] // M
+        glab = torch.arange(world * n) // M
+        assert ge2e_batch(lab)[3] == n and ge2e_batch(glab)[3] == world * n, "every row must carry a loss term"
+        rec = {"metric": "ge2e_step_data_parallel", "ranks": world, **gpu_info(),
+               "shape": {"n_per_rank": n, "N": world * n, "speakers_per_rank": n // M, "P_global": world * n // M,
+                         "utterances_per_speaker": M, "T": T}}
+        for key, across in (("step_ms_shard_centroids", False), ("step_ms_across_ranks", True)):
+            step = lambda: dsk.ge2e_step(model, opt, x, lab, loss=crit, across_ranks=across)
+            for _ in range(args.warmup):
+                step()
+            torch.cuda.synchronize()
+            dist.barrier()
+            rec[key] = round(time_events(step, args.steps), 3)
+        rec["across_ranks_overhead_ms"] = round(rec["step_ms_across_ranks"] - rec["step_ms_shard_centroids"], 3)
+        if rank == 0:
+            print(json.dumps(rec), flush=True)
+    finally:
+        dist.destroy_process_group()
+
+
 if __name__ == "__main__":
-    main()
+    if int(os.environ.get("WORLD_SIZE", "1")) > 1:
+        ap = argparse.ArgumentParser()
+        ap.add_argument("--steps", type=int, default=20)
+        ap.add_argument("--warmup", type=int, default=5)
+        main_distributed(ap.parse_known_args()[0])
+    else:
+        main()
