@@ -222,6 +222,10 @@ SIGNATURES = {
     "dsk_pipeline_lane_stream": (c_int32, [c_void_p, c_int32, POINTER(c_void_p)]),
     "dsk_fbank_num_frames": (c_int64, [c_int64, c_int32]),
     "dsk_fbank": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
+    "dsk_fbank_frame_offsets": (c_int32, [c_void_p, c_int32, c_int32, c_void_p]),
+    "dsk_fbank_batch": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
+    "dsk_fbank_crops": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int32,
+                                  c_void_p, c_int32, c_void_p, c_void_p]),
     "dsk_threshold_counts": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
 }
 

@@ -3,6 +3,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -3611,15 +3612,40 @@ int64_t dsk_fbank_num_frames(int64_t n_samples, int32_t sample_rate) {
   return 1 + static_cast<int64_t>(std::ceil((static_cast<double>(n_samples) - flen) / step));
 }
 
-int32_t dsk_fbank(const float* audio, int64_t n_samples, int32_t sample_rate, int32_t log_scale, int32_t subtract_mean,
-                  float* feat, void* stream) {
-  if (!audio || !feat || n_samples <= 0 || n_samples >= (1ll << 31) || sample_rate <= 0)
-    return fail(DSK_ERR_INVALID, "dsk_fbank: bad arguments");
+int32_t dsk_fbank_frame_offsets(const int64_t* sample_off, int32_t U, int32_t sample_rate, int64_t* frame_off) {
+  if (!sample_off || !frame_off || U < 1 || sample_rate <= 0 || sample_off[0] < 0)
+    return fail(DSK_ERR_INVALID, "dsk_fbank_frame_offsets: bad arguments (need non-null offsets, U >= 1, sample_rate > 0, "
+                "sample_off[0] >= 0; got U %d, sample_rate %d)", U, sample_rate);
+  frame_off[0] = 0;
+  for (int32_t u = 0; u < U; ++u) {
+    const int64_t len = sample_off[u + 1] - sample_off[u];
+    if (len <= 0 || len >= (1ll << 31))
+      return fail(DSK_ERR_INVALID, "dsk_fbank_frame_offsets: utterance %d has %lld samples (need 1 <= n < 2^31)", u,
+                  static_cast<long long>(len));
+    frame_off[u + 1] = frame_off[u] + dsk_fbank_num_frames(len, sample_rate);
+  }
+  return DSK_OK;
+}
+
+int32_t dsk_fbank_batch(const float* audio, const int64_t* sample_off, int32_t U, int32_t sample_rate, int32_t log_scale,
+                        int32_t subtract_mean, float* feat, void* stream) {
+  if (!audio || !feat || !sample_off || U < 1)
+    return fail(DSK_ERR_INVALID, "dsk_fbank_batch: bad arguments (need non-null pointers and U >= 1; got U %d)", U);
   const long flen = fbank_round_half_up(0.025 * sample_rate), step = fbank_round_half_up(0.01 * sample_rate);
-  if (flen > dsk::kFbNfft) return fail(DSK_ERR_INVALID, "dsk_fbank: the 25 ms frame (%ld samples) exceeds NFFT = 512", flen);
-  const int frames = static_cast<int>(dsk_fbank_num_frames(n_samples, sample_rate));
+  std::vector<int64_t> off(3 * (static_cast<size_t>(U) + 1));   // soff | foff | boff
+  std::copy(sample_off, sample_off + U + 1, off.begin());
+  int64_t* foff = off.data() + (U + 1);
+  int64_t* boff = foff + (U + 1);
+  if (int32_t rc = dsk_fbank_frame_offsets(sample_off, U, sample_rate, foff)) return rc;
+  if (flen > dsk::kFbNfft) return fail(DSK_ERR_INVALID, "dsk_fbank_batch: the 25 ms frame (%ld samples) exceeds NFFT = 512", flen);
+  boff[0] = 0;
+  for (int32_t u = 0; u < U; ++u)
+    boff[u + 1] = boff[u] + (foff[u + 1] - foff[u] + dsk::kFbFramesPerBlock - 1) / dsk::kFbFramesPerBlock;
+  const int64_t nblk = boff[U];
+  if (nblk >= (1ll << 31)) return fail(DSK_ERR_INVALID, "dsk_fbank_batch: %lld frames exceed one launch", static_cast<long long>(foff[U]));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  // python_speech_features.get_filterbanks(nfilt=64, nfft=512, samplerate, lowfreq=0, highfreq=samplerate/2)
+  // python_speech_features.get_filterbanks(nfilt=64, nfft=512, samplerate, lowfreq=0, highfreq=samplerate/2), built once
+  // per call for all U utterances
   std::vector<float> fb(static_cast<size_t>(dsk::kFbFilters) * dsk::kFbBins, 0.f);
   {
     auto hz2mel = [](double hz) { return 2595.0 * std::log10(1.0 + hz / 700.0); };
@@ -3637,21 +3663,56 @@ int32_t dsk_fbank(const float* audio, int64_t n_samples, int32_t sample_rate, in
         fb[j * dsk::kFbBins + i] = static_cast<float>((bin[j + 2] - i) / (bin[j + 2] - bin[j + 1]));
     }
   }
-  const int nblk = (frames + dsk::kFbFramesPerBlock - 1) / dsk::kFbFramesPerBlock;
-  float* scratch = nullptr;  // [64][257] filterbank + [nblk][64] column-sum partials
-  const size_t fb_bytes = fb.size() * sizeof(float);
-  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&scratch), fb_bytes + static_cast<size_t>(nblk) * dsk::kFbFilters * sizeof(float), s));
-  CUDA_TRY(cudaMemcpyAsync(scratch, fb.data(), fb_bytes, cudaMemcpyHostToDevice, s));
-  CUDA_TRY(cudaStreamSynchronize(s));  // fb is a stack-lifetime host vector (pageable copy): front-end call, not the hot loop
-  float* partial = scratch + fb.size();
-  dsk::fbank_kernel<<<nblk, dsk::kFbThreads, 0, s>>>(audio, static_cast<int>(n_samples), static_cast<int>(flen), static_cast<int>(step),
-                                                      frames, 0.97f, scratch, log_scale, 1e-5f, feat, partial);
+  // scratch: the three offset tables (int64) | [64][257] filterbank | [nblk][64] column-sum partials | [U][64] means
+  const size_t off_bytes = off.size() * sizeof(int64_t), fb_bytes = fb.size() * sizeof(float);
+  const size_t bytes = off_bytes + fb_bytes + (static_cast<size_t>(nblk) + U) * dsk::kFbFilters * sizeof(float);
+  char* scratch = nullptr;
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&scratch), bytes, s));
+  CUDA_TRY(cudaMemcpyAsync(scratch, off.data(), off_bytes, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaMemcpyAsync(scratch + off_bytes, fb.data(), fb_bytes, cudaMemcpyHostToDevice, s));
+  CUDA_TRY(cudaStreamSynchronize(s));  // off / fb are call-lifetime host vectors (pageable copies): the call's one sync
+  const int64_t* d_soff = reinterpret_cast<const int64_t*>(scratch);
+  const int64_t* d_foff = d_soff + (U + 1);
+  const int64_t* d_boff = d_foff + (U + 1);
+  const float* d_fb = reinterpret_cast<const float*>(scratch + off_bytes);
+  float* partial = reinterpret_cast<float*>(scratch + off_bytes + fb_bytes);
+  float* mean = partial + nblk * dsk::kFbFilters;
+  dsk::fbank_kernel<<<static_cast<unsigned>(nblk), dsk::kFbThreads, 0, s>>>(audio, d_soff, d_foff, d_boff, U, static_cast<int>(flen),
+                                                                            static_cast<int>(step), 0.97f, d_fb, log_scale, 1e-5f,
+                                                                            feat, partial);
   KERNEL_CHECK();
   if (subtract_mean) {
-    dsk::fbank_mean_sub_kernel<<<(frames + 63) / 64, 256, 0, s>>>(feat, frames, partial, nblk);
+    dsk::fbank_mean_kernel<<<static_cast<unsigned>((static_cast<long>(U) * dsk::kFbFilters + 255) / 256), 256, 0, s>>>(partial, d_foff, d_boff, U, mean);
+    KERNEL_CHECK();
+    dsk::fbank_mean_sub_kernel<<<static_cast<unsigned>(nblk), dsk::kFbThreads, 0, s>>>(feat, d_foff, d_boff, U, mean);
     KERNEL_CHECK();
   }
   CUDA_TRY(cudaFreeAsync(scratch, s));
+  return DSK_OK;
+}
+
+int32_t dsk_fbank(const float* audio, int64_t n_samples, int32_t sample_rate, int32_t log_scale, int32_t subtract_mean,
+                  float* feat, void* stream) {
+  if (!audio || !feat || n_samples <= 0 || n_samples >= (1ll << 31) || sample_rate <= 0)
+    return fail(DSK_ERR_INVALID, "dsk_fbank: bad arguments");
+  const int64_t sample_off[2] = {0, n_samples};
+  return dsk_fbank_batch(audio, sample_off, 1, sample_rate, log_scale, subtract_mean, feat, stream);
+}
+
+int32_t dsk_fbank_crops(const float* feat, const int64_t* frame_off, int32_t U, const int64_t* utt, const int64_t* start,
+                        int32_t B, int32_t T, const int32_t* time_masks, int32_t n_time, const int32_t* freq_masks,
+                        int32_t n_freq, float* out, void* stream) {
+  if (!feat || !frame_off || !utt || !start || !out || U < 1 || B < 1 || T < 1 || n_time < 0 || n_freq < 0 ||
+      (n_time > 0 && !time_masks) || (n_freq > 0 && !freq_masks))
+    return fail(DSK_ERR_INVALID, "dsk_fbank_crops: bad arguments (need non-null pointers, U, B, T >= 1, n_time, n_freq >= 0 "
+                "with their masks; got U %d, B %d, T %d, n_time %d, n_freq %d)", U, B, T, n_time, n_freq);
+  if ((reinterpret_cast<uintptr_t>(feat) | reinterpret_cast<uintptr_t>(out)) & 15)
+    return fail(DSK_ERR_INVALID, "dsk_fbank_crops: feat and out must be 16-byte aligned");
+  const int64_t grid = static_cast<int64_t>(B) * ((T + dsk::kCropRows - 1) / dsk::kCropRows);
+  if (grid >= (1ll << 31)) return fail(DSK_ERR_INVALID, "dsk_fbank_crops: %d crops of %d frames exceed one launch", B, T);
+  dsk::fbank_crop_kernel<<<static_cast<unsigned>(grid), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      feat, frame_off, U, utt, start, T, time_masks, n_time, freq_masks, n_freq, out);
+  KERNEL_CHECK();
   return DSK_OK;
 }
 

@@ -1,31 +1,295 @@
 """GPU log-fbank front-end: the reference's ``mk_MFB`` (reference audio_processing.py:9-36 with constants.py) on the
-device, written directly in the ``(T, 64)`` layout the network's ``(B, 1, T, 64)`` input is cropped from (SURVEY §8f-4).
+device, written directly in the ``(T, 64)`` layout the network's ``(B, 1, T, 64)`` input is cropped from (SURVEY §8f-4),
+and the input stage that feeds training and scoring from it.
 
 The reference computes the features once per wav file on the CPU (python_speech_features + librosa) and stores ``.npy``
 files; here one launch does pre-emphasis, framing, a 512-point FFT per frame in shared memory, the 64 mel filters and
-``20*log10(max(., 1e-5))``, a second one the per-bin mean subtraction.  python_speech_features is not vendored in the
-reference: parity is against the numpy restatement of its published algorithm (oracle/fbank_oracle.py), unpinned
-against the package itself.
+``20*log10(max(., 1e-5))``, a second pair the per-bin mean subtraction.  ``mk_mfb_batch`` does it for many waveforms in
+one call (one host synchronisation per call, not per file); ``mk_mfb`` is its one-waveform call.  python_speech_features
+is not vendored in the reference: parity is against the numpy restatement of its published algorithm
+(oracle/fbank_oracle.py), unpinned against the package itself.
+
+``FeatureBank`` keeps the features of a whole dataset on the device as one CSR bank (the frames of all utterances
+concatenated, plus frame offsets).  ``bank.crops`` cuts a step's ``(B, 1, T, 64)`` input from it in one launch, with
+SpecAugment time and frequency masks; ``random_starts`` and ``spec_augment_masks`` draw the crop positions and masks on
+the host.  ``bank.windows`` and ``embed_utterances`` turn whole utterances into utterance-level embeddings through the
+fixed-shape eval forward: the mean of the unit embeddings of sliding windows.
 """
 from __future__ import annotations
 
+import ctypes
+
+import numpy as np
 import torch
 
 from . import _lib as L
 
+N_MELS = 64
+
+
+def _host_int64(x, what):
+    a = x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
+    if a.dtype.kind not in "iu":
+        raise ValueError(f"{what}: expected integers, got dtype {a.dtype}")
+    return np.ascontiguousarray(a.reshape(-1), dtype=np.int64)
+
+
+def _ptr64(a):
+    return a.ctypes.data_as(ctypes.c_void_p)
+
+
+def fbank_frame_offsets(lengths, sample_rate: int = 16000) -> np.ndarray:
+    """Host only: frame offsets (U + 1,) int64 of utterances of ``lengths`` samples; utterance u gets
+    ``dsk_fbank_num_frames(lengths[u], sample_rate)`` frames.  ValueError for an empty list or a length outside
+    [1, 2^31)."""
+    lens = _host_int64(lengths, "fbank_frame_offsets")
+    if lens.size == 0:
+        raise ValueError("fbank_frame_offsets: no utterances")
+    if lens.min() < 1 or lens.max() >= 2 ** 31:
+        raise ValueError(f"fbank_frame_offsets: every length must lie in [1, 2^31), got min {lens.min()}, max {lens.max()}")
+    soff = np.concatenate(([0], np.cumsum(lens))).astype(np.int64)
+    foff = np.empty(lens.size + 1, np.int64)
+    L.check(L.load().dsk_fbank_frame_offsets(_ptr64(soff), lens.size, int(sample_rate), _ptr64(foff)),
+            "dsk_fbank_frame_offsets")
+    return foff
+
+
+def mk_mfb_batch(audio: torch.Tensor, lengths, sample_rate: int = 16000, use_logscale: bool = True,
+                 subtract_mean: bool = True):
+    """``audio``: 1-D fp32 CUDA tensor, U waveforms concatenated; ``lengths`` (U,) samples per waveform, on the host
+    -> ``(feats (F, 64) fp32 CUDA, offsets (U + 1,) int64 CPU)``: rows ``offsets[u]:offsets[u+1]`` are utterance u's,
+    bit-identical to ``mk_mfb`` on that waveform alone.  One launch sequence and one host synchronisation per call.
+    RuntimeError for a CPU tensor; ValueError for a zero length or lengths that do not add up to ``audio``, before any
+    launch."""
+    if not isinstance(audio, torch.Tensor) or not audio.is_cuda:
+        raise RuntimeError("mk_mfb_batch needs a CUDA tensor; there is no CPU fallback")
+    if isinstance(lengths, torch.Tensor) and lengths.is_cuda:
+        raise RuntimeError("mk_mfb_batch: lengths must be on the host (they size the output)")
+    a = audio.detach().reshape(-1).float().contiguous()
+    lens = _host_int64(lengths, "mk_mfb_batch")
+    if lens.size and int(lens.sum()) != a.numel():
+        raise ValueError(f"mk_mfb_batch: lengths add up to {int(lens.sum())} samples, audio has {a.numel()}")
+    foff = fbank_frame_offsets(lens, sample_rate)
+    soff = np.concatenate(([0], np.cumsum(lens))).astype(np.int64)
+    feat = torch.empty(int(foff[-1]), N_MELS, device=a.device, dtype=torch.float32)
+    with torch.cuda.device(a.device):
+        L.check(L.load().dsk_fbank_batch(a.data_ptr(), _ptr64(soff), lens.size, int(sample_rate), int(use_logscale),
+                                         int(subtract_mean), feat.data_ptr(), L.cur_stream()), "dsk_fbank_batch")
+    return feat, torch.from_numpy(foff)
+
 
 def mk_mfb(audio: torch.Tensor, sample_rate: int = 16000, use_logscale: bool = True, subtract_mean: bool = True) -> torch.Tensor:
     """audio: 1-D float CUDA tensor (mono samples, as ``librosa.load(..., sr=sample_rate, mono=True)`` yields) ->
-    ``(frames, 64)`` fp32 features.  No CPU fallback."""
+    ``(frames, 64)`` fp32 features: the one-waveform call of ``mk_mfb_batch``.  No CPU fallback."""
     if not audio.is_cuda:
         raise RuntimeError("mk_mfb needs a CUDA tensor; there is no CPU fallback")
-    a = audio.detach().reshape(-1).float().contiguous()
-    lib = L.load()
-    frames = int(lib.dsk_fbank_num_frames(a.numel(), sample_rate))
-    if frames <= 0:
+    if audio.numel() == 0:
         raise RuntimeError("mk_mfb: empty signal")
-    feat = torch.empty(frames, 64, device=a.device, dtype=torch.float32)
-    with torch.cuda.device(a.device):
-        L.check(lib.dsk_fbank(a.data_ptr(), a.numel(), sample_rate, int(use_logscale), int(subtract_mean), feat.data_ptr(),
-                              L.cur_stream()), "dsk_fbank")
-    return feat
+    return mk_mfb_batch(audio, [audio.numel()], sample_rate, use_logscale, subtract_mean)[0]
+
+
+# ---- host-side sampling -----------------------------------------------------------------------------------------------
+def _rng(generator):
+    return np.random.default_rng() if generator is None else generator
+
+
+def random_starts(lengths, utt, T: int, generator=None) -> torch.Tensor:
+    """Host: one crop start per entry of ``utt``, uniform in [0, n_u - T] (every start whose crop ends inside the
+    utterance, the last one included), or 0 when n_u < T (the crop then wraps).  ``generator`` is a
+    ``numpy.random.Generator``; the same generator state gives the same starts.  The reference draws
+    ``randrange(9, n - 23)`` (audio_processing.py:66), which never picks the last start."""
+    lens = _host_int64(lengths, "random_starts")
+    u = _host_int64(utt, "random_starts")
+    if u.size and (u.min() < 0 or u.max() >= lens.size):
+        raise ValueError(f"random_starts: utterance index outside [0, {lens.size})")
+    hi = np.maximum(lens[u] - int(T), 0)
+    return torch.from_numpy(_rng(generator).integers(0, hi + 1, dtype=np.int64) if u.size else np.zeros(0, np.int64))
+
+
+def spec_augment_masks(B: int, T: int, n_time: int, max_time: int, n_freq: int, max_freq: int, generator=None):
+    """Host: SpecAugment time and frequency masks (Park et al. 2019, masking only) for ``bank.crops``:
+    ``(time_masks (B, n_time, 2), freq_masks (B, n_freq, 2))`` int32 (start, width) pairs.  Each width is uniform in
+    [0, max] and each start uniform in [0, T - width] (time) or [0, 64 - width] (frequency); ``generator`` is a
+    ``numpy.random.Generator``."""
+    if not (0 <= max_time <= T and 0 <= max_freq <= N_MELS and n_time >= 0 and n_freq >= 0 and B >= 0):
+        raise ValueError(f"spec_augment_masks: need 0 <= max_time <= T ({max_time}, {T}), 0 <= max_freq <= 64 "
+                         f"({max_freq}), n_time, n_freq, B >= 0")
+    g = _rng(generator)
+
+    def draw(n, max_w, extent):
+        w = g.integers(0, max_w + 1, size=(B, n), dtype=np.int64)
+        s = g.integers(0, extent - w + 1, dtype=np.int64)
+        return torch.from_numpy(np.stack([s, w], axis=-1).astype(np.int32))
+
+    return draw(n_time, max_time, T), draw(n_freq, max_freq, N_MELS)
+
+
+def sliding_windows(lengths, utt, T: int, hop: int):
+    """Host: the sliding windows of the utterances ``utt``: ``(win_utt, win_start, win_off)`` int64, windows
+    ``win_off[i]:win_off[i+1]`` belong to ``utt[i]``.  Starts are 0, hop, 2 hop, ... up to n - T, plus n - T when the
+    last of those does not end at frame n, so every frame is covered; an utterance with n < T gets one window at 0,
+    which wraps."""
+    if T < 1 or hop < 1:
+        raise ValueError(f"sliding_windows: need T >= 1 and hop >= 1, got {T}, {hop}")
+    lens = _host_int64(lengths, "sliding_windows")
+    u = _host_int64(utt, "sliding_windows")
+    if u.size and (u.min() < 0 or u.max() >= lens.size):
+        raise ValueError(f"sliding_windows: utterance index outside [0, {lens.size})")
+    n = lens[u]
+    last = np.maximum(n - T, 0)
+    cnt = last // hop + 1 + (last % hop != 0)
+    win_off = np.concatenate(([0], np.cumsum(cnt))).astype(np.int64)
+    win_utt = np.repeat(u, cnt)
+    k = np.arange(win_off[-1], dtype=np.int64) - np.repeat(win_off[:-1], cnt)
+    win_start = np.minimum(k * hop, np.repeat(last, cnt))
+    return torch.from_numpy(win_utt), torch.from_numpy(win_start), torch.from_numpy(win_off)
+
+
+# ---- the device-resident bank -----------------------------------------------------------------------------------------
+class FeatureBank:
+    """The features of many utterances on one device, as one CSR bank: ``feats`` (F, 64) fp32 CUDA, the frames of all
+    utterances one after another, and ``offsets`` (U + 1,) int64, utterance u = rows ``offsets[u]:offsets[u+1]``
+    (every utterance at least one frame).  The frame counts stay on the host (``lengths``) for sampling."""
+
+    def __init__(self, feats: torch.Tensor, offsets):
+        if not isinstance(feats, torch.Tensor) or not feats.is_cuda:
+            raise RuntimeError("FeatureBank needs CUDA features; there is no CPU fallback")
+        if feats.dim() != 2 or feats.shape[1] != N_MELS or feats.dtype != torch.float32:
+            raise ValueError(f"FeatureBank: expected (F, 64) fp32 features, got {tuple(feats.shape)} {feats.dtype}")
+        off = _host_int64(offsets, "FeatureBank")
+        if off.size < 2 or off[0] != 0 or off[-1] != feats.shape[0] or np.any(np.diff(off) < 1):
+            raise ValueError("FeatureBank: offsets must start at 0, end at F and give every utterance >= 1 frame")
+        self.feats = feats.contiguous()
+        self.lengths = np.diff(off)
+        self.offsets = torch.from_numpy(off).to(feats.device)
+
+    @property
+    def num_utterances(self) -> int:
+        return int(self.lengths.size)
+
+    @property
+    def device(self):
+        return self.feats.device
+
+    @classmethod
+    def from_waveforms(cls, waveforms, sample_rate: int = 16000, chunk_samples: int = 1 << 26, device=None,
+                       use_logscale: bool = True, subtract_mean: bool = True):
+        """The bank of a list of 1-D waveforms (numpy arrays or tensors), through ``mk_mfb_batch`` in chunks of at most
+        ``chunk_samples`` samples (or one waveform, if longer), so only one chunk of audio is on the device at a time."""
+        device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        lens = np.array([int(np.prod(w.shape)) for w in waveforms], np.int64)
+        foff = fbank_frame_offsets(lens, sample_rate)          # ValueError on an empty list or waveform
+        feats = torch.empty(int(foff[-1]), N_MELS, device=device, dtype=torch.float32)
+        i = 0
+        while i < len(waveforms):
+            j, total = i + 1, lens[i]
+            while j < len(waveforms) and total + lens[j] <= chunk_samples:
+                total += lens[j]
+                j += 1
+            host = torch.cat([torch.as_tensor(w).reshape(-1).float() for w in waveforms[i:j]])
+            f, _ = mk_mfb_batch(host.to(device), lens[i:j], sample_rate, use_logscale, subtract_mean)
+            feats[foff[i]:foff[j]].copy_(f)
+            i = j
+        return cls(feats, foff)
+
+    @classmethod
+    def from_arrays(cls, arrays, device=None):
+        """The bank of a list of (n_u, 64) feature arrays, such as the reference's ``mk_MFB`` / ``read_MFB`` ``.npy``
+        files (float64): cast to fp32 on the host and copied to the device in one transfer."""
+        device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        arrs = [np.asarray(a) for a in arrays]
+        if not arrs or any(a.ndim != 2 or a.shape[1] != N_MELS or a.shape[0] < 1 for a in arrs):
+            raise ValueError("FeatureBank.from_arrays: expected a non-empty list of (n >= 1, 64) arrays")
+        host = torch.from_numpy(np.concatenate(arrs).astype(np.float32, copy=False))
+        off = np.concatenate(([0], np.cumsum([a.shape[0] for a in arrs]))).astype(np.int64)
+        return cls(host.pin_memory().to(device), off)
+
+    def crops(self, utt, start, T: int, time_masks=None, freq_masks=None) -> torch.Tensor:
+        """(B, 1, T, 64) fp32: crop b is frames ``start[b]`` .. of utterance ``utt[b]``, wrapping round the utterance
+        when it is shorter than T, with the masked frames and bins of ``time_masks`` / ``freq_masks`` ((B, n, 2) int32
+        (start, width) pairs, as ``spec_augment_masks`` gives) set to 0, the utterance mean.  One launch.  CPU indices
+        are checked on the host (ValueError); CUDA indices are not (a check would synchronise): a crop with an index
+        outside the bank or a start outside [0, n_u) comes out NaN."""
+        u = torch.as_tensor(utt)
+        s = torch.as_tensor(start)
+        if u.dim() != 1 or s.shape != u.shape or u.numel() == 0:
+            raise ValueError(f"crops: expected 1-D utt and start of one length >= 1, got {tuple(u.shape)}, {tuple(s.shape)}")
+        if u.is_floating_point() or s.is_floating_point():
+            raise ValueError("crops: utt and start must be integers")
+        if T < 1:
+            raise ValueError(f"crops: T must be >= 1, got {T}")
+        B = u.numel()
+        if not u.is_cuda:
+            uh, sh = u.to(torch.int64).numpy(), s.cpu().to(torch.int64).numpy()
+            if uh.min() < 0 or uh.max() >= self.num_utterances:
+                raise ValueError(f"crops: utterance index outside [0, {self.num_utterances})")
+            if sh.min() < 0 or np.any(sh >= self.lengths[uh]):
+                raise ValueError("crops: a start lies outside [0, n_u)")
+        dev = self.device
+        u, s = _to_dev(u, torch.int64, dev), _to_dev(s, torch.int64, dev)
+        tm, nt = self._masks(time_masks, B, "time_masks")
+        fm, nf = self._masks(freq_masks, B, "freq_masks")
+        out = torch.empty(B, 1, int(T), N_MELS, device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            L.check(L.load().dsk_fbank_crops(self.feats.data_ptr(), self.offsets.data_ptr(), self.num_utterances,
+                                             u.data_ptr(), s.data_ptr(), B, int(T), L.ptr(tm), nt, L.ptr(fm), nf,
+                                             out.data_ptr(), L.cur_stream()), "dsk_fbank_crops")
+        return out
+
+    def _masks(self, m, B, what):
+        if m is None:
+            return None, 0
+        m = torch.as_tensor(m)
+        if m.dim() != 3 or m.shape[0] != B or m.shape[2] != 2 or m.is_floating_point():
+            raise ValueError(f"crops: {what} must be integer (B, n, 2) with B = {B}, got {tuple(m.shape)} {m.dtype}")
+        if m.shape[1] == 0:
+            return None, 0
+        return _to_dev(m, torch.int32, self.device), int(m.shape[1])
+
+    def random_starts(self, utt, T: int, generator=None) -> torch.Tensor:
+        """``random_starts`` over this bank's frame counts (host int64 starts)."""
+        return random_starts(self.lengths, utt, T, generator)
+
+    def windows(self, utt, T: int, hop: int):
+        """``sliding_windows`` over this bank's frame counts: ``(win_utt, win_start, win_off)`` host int64."""
+        return sliding_windows(self.lengths, utt, T, hop)
+
+
+def _to_dev(t, dtype, dev):
+    t = t.to(dtype)
+    if not t.is_cuda:   # a pageable copy would wait for the stream; a pinned one is queued like a kernel
+        return t.contiguous().pin_memory().to(dev, non_blocking=True)
+    return t.to(dev).contiguous()
+
+
+def embed_utterances(model, bank: FeatureBank, utt, T: int = 160, hop: int = 80, batch: int = 256) -> torch.Tensor:
+    """(len(utt), D) fp32: one embedding per utterance ``utt[i]`` of ``bank``, the mean of the unit embeddings of its
+    sliding windows (``bank.windows(utt, T, hop)``), summed in fp64 in window order by ``engine.class_centroids``.
+    The rows are what ``identification.enroll`` gives for those windows: for cosine scoring (``verification``,
+    ``identification``), not of norm 10.  The eval forward runs over the windows in batches of ``min(batch, windows)``
+    rows, the last one padded, so every batch has the same shape and one captured forward serves them all.  RuntimeError
+    on a model in train mode."""
+    from . import engine
+
+    if model.training:
+        raise RuntimeError("embed_utterances needs model.eval() (train-mode BatchNorm would use batch statistics)")
+    if batch < 1:
+        raise ValueError(f"embed_utterances: batch must be >= 1, got {batch}")
+    win_utt, win_start, win_off = bank.windows(utt, T, hop)
+    W = win_utt.numel()
+    if W == 0:
+        raise ValueError("embed_utterances: no utterances")
+    Bb = min(int(batch), W)
+    nb = (W + Bb - 1) // Bb
+    pad = nb * Bb - W                                   # padded rows repeat the last window and are dropped
+    wu = torch.cat([win_utt, win_utt[-1:].expand(pad)])
+    ws = torch.cat([win_start, win_start[-1:].expand(pad)])
+    emb = None
+    with torch.no_grad():
+        for i in range(nb):
+            e = model(bank.crops(wu[i * Bb:(i + 1) * Bb], ws[i * Bb:(i + 1) * Bb], T))
+            if emb is None:
+                emb = torch.empty(nb * Bb, e.shape[1], device=e.device, dtype=torch.float32)
+            emb[i * Bb:(i + 1) * Bb].copy_(e)
+    order = torch.arange(W, dtype=torch.int64)
+    return engine.class_centroids(emb[:W], order, win_off)

@@ -557,6 +557,31 @@ int64_t dsk_fbank_num_frames(int64_t n_samples, int32_t sample_rate);
 int32_t dsk_fbank(const float* audio, int64_t n_samples, int32_t sample_rate, int32_t log_scale, int32_t subtract_mean,
                   float* feat, void* stream);
 
+/* Batched log-fbank and the crops of a feature bank.
+ *   dsk_fbank_frame_offsets: host only.  frame_off (U+1) int64 from sample_off (U+1) int64: frame_off[0] = 0,
+ *     frame_off[u+1] = frame_off[u] + dsk_fbank_num_frames(sample_off[u+1] - sample_off[u], sample_rate).  Every length
+ *     must lie in [1, 2^31) and sample_off[0] >= 0; otherwise DSK_ERR_INVALID.
+ *   dsk_fbank_batch: U waveforms, utterance u = audio[sample_off[u] .. sample_off[u+1]) (sample_off on the HOST, int64:
+ *     the concatenation may exceed 2^31 samples, each utterance may not) -> feat (frame_off[U], 64) fp32, rows
+ *     frame_off[u] .. frame_off[u+1] those of utterance u.  The rows of utterance u are bit-identical to dsk_fbank on
+ *     that waveform alone, whatever the other utterances and their order: each utterance starts on a 4-frame block
+ *     boundary and its mean is its own block partials added in block order in double.  The filterbank is built and
+ *     uploaded once per call; one host synchronisation per call, whatever U.  dsk_fbank is the U = 1 call of it.
+ *   dsk_fbank_crops: out (B, 1, T, 64) fp32 from a bank feat (F, 64) fp32 with frame offsets frame_off (U+1) (device
+ *     int64): for crop b with u = utt[b], s = start[b], n = frame_off[u+1] - frame_off[u],
+ *       out[b, 0, t, m] = feat[frame_off[u] + (s + t) mod n, m]   (wrapping repeats an utterance shorter than T),
+ *     set to 0 where t lies in one of the crop's n_time time masks or m in one of its n_freq frequency masks
+ *     (time_masks (B, n_time, 2), freq_masks (B, n_freq, 2) device int32 (start, width) pairs: [start, start + width)
+ *     clipped to the crop, width 0 = no mask).  u outside [0, U) or s outside [0, n): the whole crop is NaN and nothing
+ *     outside feat is read; the other crops are unaffected.  utt, start: device int64 (B,).  One launch, 16-byte
+ *     accesses (feat and out 16-byte aligned), no atomics, no host synchronisation. */
+int32_t dsk_fbank_frame_offsets(const int64_t* sample_off, int32_t U, int32_t sample_rate, int64_t* frame_off);
+int32_t dsk_fbank_batch(const float* audio, const int64_t* sample_off, int32_t U, int32_t sample_rate, int32_t log_scale,
+                        int32_t subtract_mean, float* feat, void* stream);
+int32_t dsk_fbank_crops(const float* feat, const int64_t* frame_off, int32_t U, const int64_t* utt, const int64_t* start,
+                        int32_t B, int32_t T, const int32_t* time_masks, int32_t n_time, const int32_t* freq_masks,
+                        int32_t n_freq, float* out, void* stream);
+
 /* Threshold sweep of the verification metric (reference eval_metrics.py:16-37 calculate_roc, :53-88 calculate_val /
  * calculate_val_far; called from train_triplet.py:361): for every threshold t (double, as numpy's arange yields them)
  * tp[t] = #{i : same[i] && (double)dist[i] < t}, fp[t] = #{i : !same[i] && (double)dist[i] < t} — numpy's
