@@ -226,6 +226,11 @@ SIGNATURES = {
     "dsk_fbank_batch": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     "dsk_fbank_crops": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int32,
                                   c_void_p, c_int32, c_void_p, c_void_p]),
+    "dsk_fbank_filterbank": (c_int32, [c_int32, c_void_p]),
+    "dsk_wave_augment": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p,
+                                   c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 5),
+    "dsk_fbank_segments": (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_int32,
+                                     c_void_p, c_int32, c_void_p, c_void_p]),
     "dsk_threshold_counts": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
 }
 

@@ -21,6 +21,7 @@
 #include "conv3x3_halo.cuh"
 #include "conv1_umma.cuh"
 #include "fbank_kernels.cuh"
+#include "augment_kernels.cuh"
 #include "head_kernels.cuh"
 #include "loss_kernels.cuh"
 #include "metric_kernels.cuh"
@@ -3627,6 +3628,28 @@ int32_t dsk_fbank_frame_offsets(const int64_t* sample_off, int32_t U, int32_t sa
   return DSK_OK;
 }
 
+int32_t dsk_fbank_filterbank(int32_t sample_rate, float* fb) {
+  if (!fb || sample_rate <= 0)
+    return fail(DSK_ERR_INVALID, "dsk_fbank_filterbank: bad arguments (need non-null fb and sample_rate > 0; got %d)", sample_rate);
+  // python_speech_features.get_filterbanks(nfilt=64, nfft=512, samplerate, lowfreq=0, highfreq=samplerate/2)
+  std::fill(fb, fb + static_cast<size_t>(dsk::kFbFilters) * dsk::kFbBins, 0.f);
+  auto hz2mel = [](double hz) { return 2595.0 * std::log10(1.0 + hz / 700.0); };
+  auto mel2hz = [](double mel) { return 700.0 * (std::pow(10.0, mel / 2595.0) - 1.0); };
+  const double lowmel = hz2mel(0.0), highmel = hz2mel(sample_rate / 2.0);
+  double bin[dsk::kFbFilters + 2];
+  for (int i = 0; i < dsk::kFbFilters + 2; ++i) {
+    const double mel = lowmel + (highmel - lowmel) * i / (dsk::kFbFilters + 1);
+    bin[i] = std::floor((dsk::kFbNfft + 1) * mel2hz(mel) / sample_rate);
+  }
+  for (int j = 0; j < dsk::kFbFilters; ++j) {
+    for (int i = static_cast<int>(bin[j]); i < static_cast<int>(bin[j + 1]); ++i)
+      fb[j * dsk::kFbBins + i] = static_cast<float>((i - bin[j]) / (bin[j + 1] - bin[j]));
+    for (int i = static_cast<int>(bin[j + 1]); i < static_cast<int>(bin[j + 2]); ++i)
+      fb[j * dsk::kFbBins + i] = static_cast<float>((bin[j + 2] - i) / (bin[j + 2] - bin[j + 1]));
+  }
+  return DSK_OK;
+}
+
 int32_t dsk_fbank_batch(const float* audio, const int64_t* sample_off, int32_t U, int32_t sample_rate, int32_t log_scale,
                         int32_t subtract_mean, float* feat, void* stream) {
   if (!audio || !feat || !sample_off || U < 1)
@@ -3644,25 +3667,9 @@ int32_t dsk_fbank_batch(const float* audio, const int64_t* sample_off, int32_t U
   const int64_t nblk = boff[U];
   if (nblk >= (1ll << 31)) return fail(DSK_ERR_INVALID, "dsk_fbank_batch: %lld frames exceed one launch", static_cast<long long>(foff[U]));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  // python_speech_features.get_filterbanks(nfilt=64, nfft=512, samplerate, lowfreq=0, highfreq=samplerate/2), built once
-  // per call for all U utterances
-  std::vector<float> fb(static_cast<size_t>(dsk::kFbFilters) * dsk::kFbBins, 0.f);
-  {
-    auto hz2mel = [](double hz) { return 2595.0 * std::log10(1.0 + hz / 700.0); };
-    auto mel2hz = [](double mel) { return 700.0 * (std::pow(10.0, mel / 2595.0) - 1.0); };
-    const double lowmel = hz2mel(0.0), highmel = hz2mel(sample_rate / 2.0);
-    double bin[dsk::kFbFilters + 2];
-    for (int i = 0; i < dsk::kFbFilters + 2; ++i) {
-      const double mel = lowmel + (highmel - lowmel) * i / (dsk::kFbFilters + 1);
-      bin[i] = std::floor((dsk::kFbNfft + 1) * mel2hz(mel) / sample_rate);
-    }
-    for (int j = 0; j < dsk::kFbFilters; ++j) {
-      for (int i = static_cast<int>(bin[j]); i < static_cast<int>(bin[j + 1]); ++i)
-        fb[j * dsk::kFbBins + i] = static_cast<float>((i - bin[j]) / (bin[j + 1] - bin[j]));
-      for (int i = static_cast<int>(bin[j + 1]); i < static_cast<int>(bin[j + 2]); ++i)
-        fb[j * dsk::kFbBins + i] = static_cast<float>((bin[j + 2] - i) / (bin[j + 2] - bin[j + 1]));
-    }
-  }
+  // built once per call for all U utterances
+  std::vector<float> fb(static_cast<size_t>(dsk::kFbFilters) * dsk::kFbBins);
+  if (int32_t rc = dsk_fbank_filterbank(sample_rate, fb.data())) return rc;
   // scratch: the three offset tables (int64) | [64][257] filterbank | [nblk][64] column-sum partials | [U][64] means
   const size_t off_bytes = off.size() * sizeof(int64_t), fb_bytes = fb.size() * sizeof(float);
   const size_t bytes = off_bytes + fb_bytes + (static_cast<size_t>(nblk) + U) * dsk::kFbFilters * sizeof(float);
@@ -3713,6 +3720,144 @@ int32_t dsk_fbank_crops(const float* feat, const int64_t* frame_off, int32_t U, 
   dsk::fbank_crop_kernel<<<static_cast<unsigned>(grid), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       feat, frame_off, U, utt, start, T, time_masks, n_time, freq_masks, n_freq, out);
   KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_fbank_segments(const float* audio, int32_t B, int32_t L, int32_t sample_rate, int32_t log_scale,
+                           int32_t subtract_mean, const float* fb, const int32_t* time_masks, int32_t n_time,
+                           const int32_t* freq_masks, int32_t n_freq, float* out, void* stream) {
+  if (!audio || !fb || !out || B < 1 || L < 1 || sample_rate <= 0 || n_time < 0 || n_freq < 0 ||
+      (n_time > 0 && !time_masks) || (n_freq > 0 && !freq_masks))
+    return fail(DSK_ERR_INVALID, "dsk_fbank_segments: bad arguments (need non-null pointers, B, L >= 1, sample_rate > 0, "
+                "n_time, n_freq >= 0 with their masks; got B %d, L %d, sample_rate %d, n_time %d, n_freq %d)", B, L,
+                sample_rate, n_time, n_freq);
+  if (reinterpret_cast<uintptr_t>(out) & 15) return fail(DSK_ERR_INVALID, "dsk_fbank_segments: out must be 16-byte aligned");
+  const long flen = fbank_round_half_up(0.025 * sample_rate), step = fbank_round_half_up(0.01 * sample_rate);
+  if (flen > dsk::kFbNfft) return fail(DSK_ERR_INVALID, "dsk_fbank_segments: the 25 ms frame (%ld samples) exceeds NFFT = 512", flen);
+  const int64_t T = dsk_fbank_num_frames(L, sample_rate);
+  const int64_t blocks_per = (T + dsk::kFbFramesPerBlock - 1) / dsk::kFbFramesPerBlock, nblk = blocks_per * B;
+  const int64_t mask_grid = static_cast<int64_t>(B) * ((T + dsk::kCropRows - 1) / dsk::kCropRows);
+  if (nblk >= (1ll << 31) || mask_grid >= (1ll << 31))
+    return fail(DSK_ERR_INVALID, "dsk_fbank_segments: %d segments of %lld frames exceed one launch", B, static_cast<long long>(T));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // scratch: soff | foff | boff (B + 1 each, int64) | [nblk][64] column-sum partials | [B][64] means
+  const size_t off_bytes = 3 * (static_cast<size_t>(B) + 1) * sizeof(int64_t);
+  const size_t bytes = off_bytes + (static_cast<size_t>(nblk) + B) * dsk::kFbFilters * sizeof(float);
+  char* scratch = nullptr;
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&scratch), bytes, s));
+  int64_t* d_soff = reinterpret_cast<int64_t*>(scratch);
+  int64_t* d_foff = d_soff + (B + 1);
+  int64_t* d_boff = d_foff + (B + 1);
+  float* partial = reinterpret_cast<float*>(scratch + off_bytes);
+  float* mean = partial + nblk * dsk::kFbFilters;
+  dsk::fbank_regular_offsets_kernel<<<(B + 1 + 255) / 256, 256, 0, s>>>(B, L, static_cast<int>(T), d_soff, d_foff, d_boff);
+  KERNEL_CHECK();
+  // (B, 1, T, 64) is the (B T, 64) layout of the B segments' frames: the features are written straight into out
+  dsk::fbank_kernel<<<static_cast<unsigned>(nblk), dsk::kFbThreads, 0, s>>>(audio, d_soff, d_foff, d_boff, B, static_cast<int>(flen),
+                                                                            static_cast<int>(step), 0.97f, fb, log_scale, 1e-5f,
+                                                                            out, partial);
+  KERNEL_CHECK();
+  if (subtract_mean) {
+    dsk::fbank_mean_kernel<<<static_cast<unsigned>((static_cast<long>(B) * dsk::kFbFilters + 255) / 256), 256, 0, s>>>(partial, d_foff, d_boff, B, mean);
+    KERNEL_CHECK();
+    dsk::fbank_mean_sub_kernel<<<static_cast<unsigned>(nblk), dsk::kFbThreads, 0, s>>>(out, d_foff, d_boff, B, mean);
+    KERNEL_CHECK();
+  }
+  if (n_time > 0 || n_freq > 0) {
+    dsk::fbank_mask_kernel<<<static_cast<unsigned>(mask_grid), 256, 0, s>>>(out, static_cast<int>(T), time_masks, n_time,
+                                                                            freq_masks, n_freq);
+    KERNEL_CHECK();
+  }
+  CUDA_TRY(cudaFreeAsync(scratch, s));
+  return DSK_OK;
+}
+
+// A bank pointer as the kernels read it: device (or managed) memory as is, page-locked host memory through its mapped
+// device address.  Pageable host memory is rejected: the kernels could not read it, and a copy would synchronise.
+static int32_t aug_resolve(const void* p, const void** dev, const char* what) {
+  cudaPointerAttributes a{};
+  CUDA_TRY(cudaPointerGetAttributes(&a, p));
+  if (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) {
+    *dev = p;
+    return DSK_OK;
+  }
+  if (a.type == cudaMemoryTypeHost) {
+    void* d = nullptr;
+    CUDA_TRY(cudaHostGetDevicePointer(&d, const_cast<void*>(p), 0));
+    *dev = d;
+    return DSK_OK;
+  }
+  return fail(DSK_ERR_INVALID, "dsk_wave_augment: %s is pageable host memory (use device or page-locked memory)", what);
+}
+
+int32_t dsk_wave_augment(const int16_t* speech, const int64_t* speech_off, int32_t U, const int64_t* utt,
+                         const int64_t* start, int32_t B, int32_t L, const float* rir, const int64_t* rir_off, int32_t R,
+                         int32_t max_rir_len, const int64_t* rir_idx, const int16_t* noise, const int64_t* noise_off,
+                         int32_t N, int32_t M, const int64_t* noise_idx, const int64_t* noise_start, const double* snr_db,
+                         float* out, void* stream) {
+  if (!speech || !speech_off || !utt || !start || !out || U < 1 || B < 1 || L < 1 || L > (1 << 24) || M < 0 ||
+      M > dsk::kAugMaxSources || max_rir_len < 1 || max_rir_len > dsk::kAugMaxRir)
+    return fail(DSK_ERR_INVALID, "dsk_wave_augment: bad arguments (need non-null speech, offsets, utt, start, out; U, B >= 1; "
+                "1 <= L <= 2^24; 0 <= M <= %d; 1 <= max_rir_len <= %d; got U %d, B %d, L %d, M %d, max_rir_len %d)",
+                dsk::kAugMaxSources, dsk::kAugMaxRir, U, B, L, M, max_rir_len);
+  if (rir_idx && (!rir || !rir_off || R < 1))
+    return fail(DSK_ERR_INVALID, "dsk_wave_augment: rir_idx needs a RIR bank (non-null rir, rir_off and R >= 1; got R %d)", R);
+  if (M > 0 && (!noise || !noise_off || N < 1 || !noise_idx || !noise_start || !snr_db))
+    return fail(DSK_ERR_INVALID, "dsk_wave_augment: M = %d sources need a noise bank (N >= 1; got %d) and non-null "
+                "noise_idx, noise_start, snr_db", M, N);
+  const int64_t tiles = (L + dsk::kAugGatherPerBlock - 1) / dsk::kAugGatherPerBlock;
+  const int64_t nb = (L + dsk::kAugPart - 1) / dsk::kAugPart, kp = (max_rir_len + dsk::kAugPart - 1) / dsk::kAugPart;
+  if (B * tiles >= (1ll << 31) || B * nb >= (1ll << 31) || B * kp >= (1ll << 31))
+    return fail(DSK_ERR_INVALID, "dsk_wave_augment: %d segments of %d samples exceed one launch", B, L);
+  const void *sp = nullptr, *sop = nullptr, *rp = nullptr, *rop = nullptr, *np_ = nullptr, *nop = nullptr;
+  if (int32_t rc = aug_resolve(speech, &sp, "the speech bank")) return rc;
+  if (int32_t rc = aug_resolve(speech_off, &sop, "the speech offsets")) return rc;
+  if (rir_idx) {
+    if (int32_t rc = aug_resolve(rir, &rp, "the RIR bank")) return rc;
+    if (int32_t rc = aug_resolve(rir_off, &rop, "the RIR offsets")) return rc;
+  }
+  if (M > 0) {
+    if (int32_t rc = aug_resolve(noise, &np_, "the noise bank")) return rc;
+    if (int32_t rc = aug_resolve(noise_off, &nop, "the noise offsets")) return rc;
+  }
+  const int16_t* d_speech = static_cast<const int16_t*>(sp);
+  const int64_t* d_soff = static_cast<const int64_t*>(sop);
+  const float* d_rir = static_cast<const float*>(rp);
+  const int64_t* d_roff = static_cast<const int64_t*>(rop);
+  const int16_t* d_noise = static_cast<const int16_t*>(np_);
+  const int64_t* d_noff = static_cast<const int64_t*>(nop);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // scratch: ok (B int32, padded to 256 bytes) | X [B][nb][P + 1] | H [B][kp][P + 1] (complex fp32, reverb only)
+  const size_t ok_bytes = (static_cast<size_t>(B) * sizeof(int) + 255) / 256 * 256;
+  const size_t x_elems = rir_idx ? static_cast<size_t>(B) * nb * dsk::kAugBins : 0;
+  const size_t h_elems = rir_idx ? static_cast<size_t>(B) * kp * dsk::kAugBins : 0;
+  char* scratch = nullptr;
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&scratch), ok_bytes + (x_elems + h_elems) * sizeof(float2), s));
+  int* ok = reinterpret_cast<int*>(scratch);
+  float2* X = reinterpret_cast<float2*>(scratch + ok_bytes);
+  float2* H = X + x_elems;
+  dsk::aug_check_kernel<<<(B + 255) / 256, 256, 0, s>>>(d_soff, U, utt, start, B, d_roff, R, rir_idx, max_rir_len, d_noff, N, M,
+                                                        noise_idx, noise_start, snr_db, ok);
+  KERNEL_CHECK();
+  dsk::aug_gather_kernel<<<static_cast<unsigned>(B * tiles), dsk::kAugGatherThreads, 0, s>>>(d_speech, d_soff, utt, start, ok, L, out);
+  KERNEL_CHECK();
+  if (rir_idx) {
+    dsk::aug_fft_in_kernel<<<static_cast<unsigned>(B * nb), dsk::kAugFftThreads, 0, s>>>(out, L, static_cast<int>(nb), ok, rir_idx,
+                                                                                       d_roff, X);
+    KERNEL_CHECK();
+    dsk::aug_fft_rir_kernel<<<static_cast<unsigned>(B * kp), dsk::kAugFftThreads, 0, s>>>(d_rir, d_roff, ok, rir_idx,
+                                                                                        static_cast<int>(kp), H);
+    KERNEL_CHECK();
+    dsk::aug_conv_out_kernel<<<static_cast<unsigned>(B * nb), dsk::kAugFftThreads, 0, s>>>(X, H, static_cast<int>(nb),
+                                                                                         static_cast<int>(kp), ok, rir_idx,
+                                                                                         d_roff, L, out);
+    KERNEL_CHECK();
+  }
+  if (M > 0) {
+    dsk::aug_mix_kernel<<<B, dsk::kAugMixThreads, 0, s>>>(d_noise, d_noff, M, noise_idx, noise_start, snr_db, ok, L, out);
+    KERNEL_CHECK();
+  }
+  CUDA_TRY(cudaFreeAsync(scratch, s));
   return DSK_OK;
 }
 

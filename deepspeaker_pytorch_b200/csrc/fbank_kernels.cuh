@@ -122,12 +122,56 @@ fbank_mean_sub_kernel(float* __restrict__ feat_all, const int64_t* __restrict__ 
   if (f < foff[u + 1] - foff[u]) feat_all[(foff[u] + f) * kFbFilters + m] -= mean[static_cast<long>(u) * kFbFilters + m];
 }
 
+// Regular offsets of B equal segments of L samples and T frames each: soff[u] = u L, foff[u] = u T,
+// boff[u] = u ceil(T / 4) for u in [0, B].  grid = ceil((B + 1) / 256), block = 256.
+__global__ void fbank_regular_offsets_kernel(int B, int L, int T, int64_t* __restrict__ soff, int64_t* __restrict__ foff,
+                                             int64_t* __restrict__ boff) {
+  const int u = blockIdx.x * blockDim.x + threadIdx.x;
+  if (u > B) return;
+  soff[u] = static_cast<int64_t>(u) * L;
+  foff[u] = static_cast<int64_t>(u) * T;
+  boff[u] = static_cast<int64_t>(u) * ((T + kFbFramesPerBlock - 1) / kFbFramesPerBlock);
+}
+
+// SpecAugment masks of crop b on bins 4q .. 4q+3 of its row t: all four zeroed when t lies in one of the n_time time
+// masks, each one zeroed when it lies in one of the n_freq frequency masks ((start, width) int32 pairs).
+__device__ __forceinline__ float4 fbank_apply_masks(float4 v, int b, int t, int q, const int* __restrict__ tmask,
+                                                    int n_time, const int* __restrict__ fmask, int n_freq) {
+  bool tm = false;
+  for (int k = 0; k < n_time; ++k) {
+    const long ms = tmask[(static_cast<long>(b) * n_time + k) * 2], mw = tmask[(static_cast<long>(b) * n_time + k) * 2 + 1];
+    tm |= t >= ms && t < ms + mw;
+  }
+  if (tm) return make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int k = 0; k < n_freq; ++k) {
+    const long fs = fmask[(static_cast<long>(b) * n_freq + k) * 2], fe = fs + fmask[(static_cast<long>(b) * n_freq + k) * 2 + 1];
+    const int m = 4 * q;
+    if (m >= fs && m < fe) v.x = 0.f;
+    if (m + 1 >= fs && m + 1 < fe) v.y = 0.f;
+    if (m + 2 >= fs && m + 2 < fe) v.z = 0.f;
+    if (m + 3 >= fs && m + 3 < fe) v.w = 0.f;
+  }
+  return v;
+}
+
+// The masks applied in place to (B, T, 64) features; grid = B * ceil(T / 16), block = 256, as fbank_crop_kernel.
+constexpr int kCropRows = 16;
+__global__ void __launch_bounds__(256)
+fbank_mask_kernel(float* feat, int T, const int* __restrict__ tmask, int n_time, const int* __restrict__ fmask,
+                  int n_freq) {
+  const int tiles = (T + kCropRows - 1) / kCropRows;
+  const int b = blockIdx.x / tiles;
+  const int t = (blockIdx.x - b * tiles) * kCropRows + (threadIdx.x >> 4), q = threadIdx.x & 15;
+  if (t >= T) return;
+  float4* p = reinterpret_cast<float4*>(feat + (static_cast<long>(b) * T + t) * kFbFilters) + q;
+  *p = fbank_apply_masks(*p, b, t, q, tmask, n_time, fmask, n_freq);
+}
+
 // Crops of a CSR feature bank (frames of U utterances concatenated, utterance u = rows [foff[u], foff[u+1]) of feat):
 //   out[b][t][m] = feat[foff[u] + (s + t) mod n][m],  u = utt[b], s = start[b], n = foff[u+1] - foff[u],
 // zeroed where t lies in one of the crop's n_time (start, width) time masks or m in one of its n_freq frequency masks.
 // u outside [0, U) or s outside [0, n): the whole crop is NaN and feat is not read.  Each 256-thread block writes 16 rows
 // of one crop, one float4 per thread; grid = B * ceil(T / 16).
-constexpr int kCropRows = 16;
 __global__ void __launch_bounds__(256)
 fbank_crop_kernel(const float* __restrict__ feat, const int64_t* __restrict__ foff, int U, const int64_t* __restrict__ utt,
                   const int64_t* __restrict__ start, int T, const int* __restrict__ tmask, int n_time,
@@ -150,23 +194,7 @@ fbank_crop_kernel(const float* __restrict__ feat, const int64_t* __restrict__ fo
     v = make_float4(nan, nan, nan, nan);
   } else {
     v = __ldg(reinterpret_cast<const float4*>(feat + (base + (s + t) % n) * kFbFilters) + q);
-    bool tm = false;
-    for (int k = 0; k < n_time; ++k) {
-      const long ms = tmask[(static_cast<long>(b) * n_time + k) * 2], mw = tmask[(static_cast<long>(b) * n_time + k) * 2 + 1];
-      tm |= t >= ms && t < ms + mw;
-    }
-    if (tm) {
-      v = make_float4(0.f, 0.f, 0.f, 0.f);
-    } else {
-      for (int k = 0; k < n_freq; ++k) {
-        const long fs = fmask[(static_cast<long>(b) * n_freq + k) * 2], fe = fs + fmask[(static_cast<long>(b) * n_freq + k) * 2 + 1];
-        const int m = 4 * q;
-        if (m >= fs && m < fe) v.x = 0.f;
-        if (m + 1 >= fs && m + 1 < fe) v.y = 0.f;
-        if (m + 2 >= fs && m + 2 < fe) v.z = 0.f;
-        if (m + 3 >= fs && m + 3 < fe) v.w = 0.f;
-      }
-    }
+    v = fbank_apply_masks(v, b, t, q, tmask, n_time, fmask, n_freq);
   }
   reinterpret_cast<float4*>(out + (static_cast<long>(b) * T + t) * kFbFilters)[q] = v;
 }

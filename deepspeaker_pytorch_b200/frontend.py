@@ -14,6 +14,11 @@ concatenated, plus frame offsets).  ``bank.crops`` cuts a step's ``(B, 1, T, 64)
 SpecAugment time and frequency masks; ``random_starts`` and ``spec_augment_masks`` draw the crop positions and masks on
 the host.  ``bank.windows`` and ``embed_utterances`` turn whole utterances into utterance-level embeddings through the
 fixed-shape eval forward: the mean of the unit embeddings of sliding windows.
+
+``WaveBank`` keeps int16 waveforms (on the device or in pinned host memory) for training on augmented speech:
+``augmented_crops`` gathers each step's segments, reverberates them by a ``RirBank`` RIR, mixes noise sources at target
+SNRs (``augment_plan`` draws them on the host) and computes their features, all on the device with no host
+synchronisation.  Training features then subtract the segment's own mean; ``FeatureBank`` subtracts the utterance's.
 """
 from __future__ import annotations
 
@@ -22,6 +27,7 @@ import ctypes
 import numpy as np
 import torch
 
+from . import _lib       # for methods whose segment-length argument is named L
 from . import _lib as L
 
 N_MELS = 64
@@ -260,6 +266,318 @@ def _to_dev(t, dtype, dev):
     if not t.is_cuda:   # a pageable copy would wait for the stream; a pinned one is queued like a kernel
         return t.contiguous().pin_memory().to(dev, non_blocking=True)
     return t.to(dev).contiguous()
+
+
+_FB_CACHE = {}
+
+
+def _filterbank(dev, sample_rate: int) -> torch.Tensor:
+    """The (64, 257) fp32 mel filterbank on ``dev`` (``dsk_fbank_filterbank``), uploaded once per (device, rate)."""
+    key = (dev.index, int(sample_rate))
+    if key not in _FB_CACHE:
+        fb = np.empty((N_MELS, 257), np.float32)
+        L.check(L.load().dsk_fbank_filterbank(int(sample_rate), fb.ctypes.data_as(ctypes.c_void_p)), "dsk_fbank_filterbank")
+        _FB_CACHE[key] = torch.from_numpy(fb).to(dev)
+    return _FB_CACHE[key]
+
+
+def _fbank_step(sample_rate: int):
+    return int(np.floor(0.025 * sample_rate + 0.5)), int(np.floor(0.01 * sample_rate + 0.5))
+
+
+def segment_samples(T: int, sample_rate: int = 16000) -> int:
+    """Samples L = flen + (T - 1) step of a segment whose log-fbank has exactly T frames (25 840 at 16 kHz, T = 160)."""
+    flen, step = _fbank_step(sample_rate)
+    return flen + (int(T) - 1) * step
+
+
+# ---- waveform augmentation ---------------------------------------------------------------------------------------------
+AUG_MAX_SOURCES = 8
+AUG_MAX_RIR = 65536
+
+
+def _bank_samples(samples, dtype, what):
+    if not isinstance(samples, torch.Tensor) or samples.dim() != 1 or samples.dtype != dtype or samples.numel() == 0:
+        raise ValueError(f"{what}: expected a non-empty 1-D {dtype} tensor")
+    if not samples.is_cuda and not (torch.cuda.is_available() and samples.is_pinned()):
+        raise ValueError(f"{what}: samples must be a CUDA tensor or page-locked (pinned) CPU memory, not pageable memory")
+    return samples.contiguous()
+
+
+def _bank_offsets(offsets, n, what):
+    off = _host_int64(offsets, what)
+    if off.size < 2 or off[0] != 0 or off[-1] != n or np.any(np.diff(off) < 1):
+        raise ValueError(f"{what}: offsets must start at 0, end at {n} and give every entry >= 1 sample")
+    return off
+
+
+def _bank_device(samples, device):
+    if samples.is_cuda:
+        return samples.device
+    return torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+
+
+class WaveBank:
+    """Int16 PCM waveforms of many utterances as one CSR bank: ``samples`` (S,) int16, the utterances one after
+    another, on the device or in page-locked host memory (read over the bus by the kernels: VoxCeleb2 as 16-bit PCM is
+    ~265 GB, more than a card holds), and ``offsets`` (U + 1,) int64, utterance u = ``samples[offsets[u]:offsets[u+1]]``.
+    The sample counts stay on the host (``lengths``) for sampling; the offsets are copied to ``device``."""
+
+    def __init__(self, samples: torch.Tensor, offsets, device=None):
+        self.samples = _bank_samples(samples, torch.int16, "WaveBank")
+        off = _bank_offsets(offsets, self.samples.numel(), "WaveBank")
+        self.lengths = np.diff(off)
+        self.device = _bank_device(self.samples, device)
+        self.offsets = torch.from_numpy(off).to(self.device)
+
+    @property
+    def num_utterances(self) -> int:
+        return int(self.lengths.size)
+
+    @classmethod
+    def from_waveforms(cls, waves, pin: bool = False, device=None):
+        """The bank of a list of 1-D waveforms: int16 arrays, or float arrays whose values are exactly k / 32768 (what
+        ``librosa.load`` returns for a 16-bit file at its native rate).  ``pin``: keep the samples in page-locked host
+        memory rather than on the device.  ValueError for anything else."""
+        arrs = []
+        for w in waves:
+            a = w.detach().cpu().numpy() if isinstance(w, torch.Tensor) else np.asarray(w)
+            a = a.reshape(-1)
+            if a.size == 0:
+                raise ValueError("WaveBank.from_waveforms: empty waveform")
+            if a.dtype == np.int16:
+                arrs.append(a)
+                continue
+            if a.dtype.kind != "f":
+                raise ValueError(f"WaveBank.from_waveforms: expected int16 or float samples, got {a.dtype}")
+            k = a.astype(np.float64) * 32768.0
+            if not np.all(np.isfinite(k)) or np.any(k != np.round(k)) or k.min() < -32768 or k.max() > 32767:
+                raise ValueError("WaveBank.from_waveforms: float samples must be exactly k / 32768 with k an int16")
+            arrs.append(k.astype(np.int16))
+        if not arrs:
+            raise ValueError("WaveBank.from_waveforms: no waveforms")
+        host = torch.from_numpy(np.concatenate(arrs))
+        off = np.concatenate(([0], np.cumsum([a.size for a in arrs]))).astype(np.int64)
+        if pin:
+            return cls(host.pin_memory(), off, device)
+        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        return cls(host.pin_memory().to(dev), off)
+
+    def random_starts(self, utt, L: int, generator=None) -> torch.Tensor:
+        """``random_starts`` over this bank's sample counts: uniform in [0, n - L], 0 when n < L (host int64)."""
+        return random_starts(self.lengths, utt, L, generator)
+
+    def segments(self, utt, start, L: int, plan=None, rir_bank=None, noise_bank=None) -> torch.Tensor:
+        """(B, L) fp32 augmented audio (``dsk_wave_augment``): segment b is samples ``start[b]`` .. of utterance
+        ``utt[b]`` (wrapping) times 2^-15, reverberated by RIR ``plan["rir_idx"][b]`` of ``rir_bank`` and mixed with the
+        sources of ``plan`` from ``noise_bank`` (see ``augment_plan``).  No plan: the clean segments.  CPU indices are
+        checked on the host (ValueError); CUDA ones are not: an example with an index, start or SNR out of range comes
+        out NaN.  No host synchronisation."""
+        u, s = _index_pair(utt, start, "segments")
+        B, L = u.numel(), int(L)
+        if not 1 <= L <= 1 << 24:
+            raise ValueError(f"segments: L must lie in [1, 2^24], got {L}")
+        plan = {} if plan is None else plan
+        rir_idx, noise_idx, noise_start, snr = (plan.get(k) for k in ("rir_idx", "noise_idx", "noise_start", "snr_db"))
+        if rir_idx is not None and rir_bank is None:
+            r = torch.as_tensor(rir_idx)
+            if r.is_cuda or bool((r != -1).any()):
+                raise ValueError("segments: the plan reverberates but no rir_bank is given")
+            rir_idx = None
+        M = 0
+        if noise_idx is not None:
+            noise_idx, noise_start, snr = (torch.as_tensor(x) for x in (noise_idx, noise_start, snr))
+            if noise_idx.dim() != 2 or noise_idx.shape[0] != B or noise_start.shape != noise_idx.shape \
+                    or snr.shape != noise_idx.shape:
+                raise ValueError(f"segments: noise_idx, noise_start, snr_db must be (B, M) with B = {B}")
+            M = int(noise_idx.shape[1])
+            if M > AUG_MAX_SOURCES:
+                raise ValueError(f"segments: at most {AUG_MAX_SOURCES} noise sources, got {M}")
+            if M and noise_bank is None:
+                raise ValueError("segments: the plan adds noise but no noise_bank is given")
+        if not u.is_cuda:
+            _check_host_index(u, s, self.lengths, "segments")
+        if rir_idx is not None:
+            rir_idx = torch.as_tensor(rir_idx)
+            if rir_idx.shape != u.shape or rir_idx.is_floating_point():
+                raise ValueError(f"segments: rir_idx must be integer (B,) with B = {B}")
+            if not rir_idx.is_cuda:
+                r = rir_idx.to(torch.int64).numpy()
+                if r.min() < -1 or r.max() >= rir_bank.num_rirs:
+                    raise ValueError(f"segments: rir_idx outside [-1, {rir_bank.num_rirs})")
+        if M and not noise_idx.is_cuda:
+            q, st, sn = noise_idx.to(torch.int64).numpy(), noise_start.cpu().to(torch.int64).numpy(), snr.cpu().double().numpy()
+            used = q != -1
+            if q.min() < -1 or q.max() >= noise_bank.num_utterances:
+                raise ValueError(f"segments: noise_idx outside [-1, {noise_bank.num_utterances})")
+            if np.any(st[used] < 0) or np.any(st[used] >= noise_bank.lengths[q[used]]):
+                raise ValueError("segments: a noise start lies outside [0, n)")
+            if not np.all(np.isfinite(sn[used])):
+                raise ValueError("segments: a non-finite SNR")
+        dev = self.device
+        u, s = _to_dev(u, torch.int64, dev), _to_dev(s, torch.int64, dev)
+        out = torch.empty(B, L, device=dev, dtype=torch.float32)
+        ri = _to_dev(rir_idx, torch.int64, dev) if rir_idx is not None else None
+        if M:
+            ni, ns = _to_dev(noise_idx, torch.int64, dev), _to_dev(noise_start, torch.int64, dev)
+            sd = _to_dev(snr, torch.float64, dev)
+        else:
+            ni = ns = sd = None
+        rb = rir_bank if ri is not None else None
+        nb = noise_bank if M else None
+        ptr = _lib.ptr
+        with torch.cuda.device(dev):
+            _lib.check(_lib.load().dsk_wave_augment(
+                self.samples.data_ptr(), self.offsets.data_ptr(), self.num_utterances, u.data_ptr(), s.data_ptr(), B, L,
+                ptr(rb.samples if rb else None), ptr(rb.offsets if rb else None), rb.num_rirs if rb else 0,
+                rb.max_len if rb else 1, ptr(ri),
+                ptr(nb.samples if nb else None), ptr(nb.offsets if nb else None), nb.num_utterances if nb else 0, M,
+                ptr(ni), ptr(ns), ptr(sd), out.data_ptr(), _lib.cur_stream()), "dsk_wave_augment")
+        return out
+
+    def augmented_crops(self, utt, start, T: int, plan=None, rir_bank=None, noise_bank=None, time_masks=None,
+                        freq_masks=None, sample_rate: int = 16000, use_logscale: bool = True,
+                        subtract_mean: bool = True) -> torch.Tensor:
+        """(B, 1, T, 64) fp32 training input: ``mk_mfb`` of each augmented segment of ``segment_samples(T)`` samples
+        (``segments``), the mean subtracted over the segment's own T frames, then the SpecAugment masks exactly as
+        ``FeatureBank.crops`` applies them.  ``start`` counts samples.  No host synchronisation once the filterbank of
+        ``sample_rate`` is on the device."""
+        Ls = segment_samples(T, sample_rate)
+        if T < 1 or L.load().dsk_fbank_num_frames(Ls, int(sample_rate)) != T:
+            raise ValueError(f"augmented_crops: no segment length gives T = {T} frames at {sample_rate} Hz")
+        audio = self.segments(utt, start, Ls, plan, rir_bank, noise_bank)
+        B = audio.shape[0]
+        dev = self.device
+        tm, nt = _masks(time_masks, B, "time_masks", dev)
+        fm, nf = _masks(freq_masks, B, "freq_masks", dev)
+        fb = _filterbank(dev, sample_rate)
+        out = torch.empty(B, 1, int(T), N_MELS, device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            L.check(L.load().dsk_fbank_segments(audio.data_ptr(), B, Ls, int(sample_rate), int(use_logscale),
+                                                int(subtract_mean), fb.data_ptr(), L.ptr(tm), nt, L.ptr(fm), nf,
+                                                out.data_ptr(), L.cur_stream()), "dsk_fbank_segments")
+        return out
+
+
+class RirBank:
+    """Room impulse responses as one CSR bank: ``samples`` (S,) fp32 (device or page-locked host memory), ``offsets``
+    (R + 1,) int64.  ``max_len`` (host) is the longest RIR, at most 65 536 taps."""
+
+    def __init__(self, samples: torch.Tensor, offsets, device=None):
+        self.samples = _bank_samples(samples, torch.float32, "RirBank")
+        off = _bank_offsets(offsets, self.samples.numel(), "RirBank")
+        self.lengths = np.diff(off)
+        if self.lengths.max() > AUG_MAX_RIR:
+            raise ValueError(f"RirBank: a RIR has {self.lengths.max()} taps, more than {AUG_MAX_RIR}")
+        self.max_len = int(self.lengths.max())
+        self.device = _bank_device(self.samples, device)
+        self.offsets = torch.from_numpy(off).to(self.device)
+
+    @property
+    def num_rirs(self) -> int:
+        return int(self.lengths.size)
+
+    @classmethod
+    def from_arrays(cls, rirs, pin: bool = False, device=None):
+        """The bank of a list of 1-D RIRs, each normalised to unit energy (in fp64 on the host, rounded once to fp32).
+        ValueError for an empty, non-finite or all-zero RIR."""
+        arrs = []
+        for h in rirs:
+            a = np.asarray(h.detach().cpu().numpy() if isinstance(h, torch.Tensor) else h, np.float64).reshape(-1)
+            e = float(np.sqrt(np.sum(a * a))) if a.size else 0.0
+            if a.size == 0 or not np.isfinite(e) or e == 0.0:
+                raise ValueError("RirBank.from_arrays: every RIR must be non-empty, finite and not all zero")
+            if a.size > AUG_MAX_RIR:
+                raise ValueError(f"RirBank.from_arrays: a RIR has {a.size} taps, more than {AUG_MAX_RIR}")
+            arrs.append((a / e).astype(np.float32))
+        if not arrs:
+            raise ValueError("RirBank.from_arrays: no RIRs")
+        host = torch.from_numpy(np.concatenate(arrs))
+        off = np.concatenate(([0], np.cumsum([a.size for a in arrs]))).astype(np.int64)
+        if pin:
+            return cls(host.pin_memory(), off, device)
+        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        return cls(host.pin_memory().to(dev), off)
+
+
+def augment_plan(B: int, L: int, generator=None, rir_bank=None, p_reverb: float = 0.5, noise_bank=None,
+                 noise_groups=(), p_noise: float = 0.5):
+    """Host: a random augmentation plan for B segments of L samples, as a dict of CPU tensors ``rir_idx`` (B,) int64,
+    ``noise_idx``, ``noise_start`` (B, M) int64 and ``snr_db`` (B, M) fp64, M the largest source count of any group and
+    unused slots -1 (start 0, SNR 0).  Per example: with probability ``p_reverb`` a uniform RIR of ``rir_bank`` (else
+    -1); with probability ``p_noise`` one of ``noise_groups`` chosen by weight, then a uniform source count, uniform
+    utterances, uniform starts in [0, n - L] (0 when n < L: the source wraps) and a uniform SNR.  A group is
+    ``(utterance ids in noise_bank, (snr_lo_db, snr_hi_db), (count_lo, count_hi), weight)``.  ``generator`` is a
+    ``numpy.random.Generator``; the same state gives the same plan."""
+    g = _rng(generator)
+    B, L = int(B), int(L)
+    if B < 0 or L < 1 or not (0.0 <= p_reverb <= 1.0 and 0.0 <= p_noise <= 1.0):
+        raise ValueError(f"augment_plan: need B >= 0, L >= 1 and probabilities in [0, 1] (got {B}, {L}, {p_reverb}, {p_noise})")
+    groups = []
+    for grp in noise_groups:
+        ids, (slo, shi), (clo, chi), w = grp
+        ids = _host_int64(ids, "augment_plan")
+        if noise_bank is None:
+            raise ValueError("augment_plan: noise groups need a noise_bank")
+        if ids.size == 0 or ids.min() < 0 or ids.max() >= noise_bank.num_utterances:
+            raise ValueError(f"augment_plan: a group's utterances must be a non-empty subset of [0, {noise_bank.num_utterances})")
+        if not (1 <= clo <= chi <= AUG_MAX_SOURCES) or not (np.isfinite(slo) and np.isfinite(shi) and slo <= shi) or w < 0:
+            raise ValueError(f"augment_plan: need 1 <= count_lo <= count_hi <= {AUG_MAX_SOURCES}, finite snr_lo <= snr_hi "
+                             "and weight >= 0")
+        groups.append((ids, float(slo), float(shi), int(clo), int(chi), float(w)))
+    if p_reverb > 0 and rir_bank is None:
+        raise ValueError("augment_plan: p_reverb > 0 needs a rir_bank")
+    if p_noise > 0 and not groups:
+        raise ValueError("augment_plan: p_noise > 0 needs noise groups")
+    weights = np.array([grp[5] for grp in groups], np.float64)
+    if groups and weights.sum() <= 0:
+        raise ValueError("augment_plan: the group weights add up to 0")
+    M = max((grp[4] for grp in groups), default=0)
+    rir_idx = np.full(B, -1, np.int64)
+    noise_idx = np.full((B, M), -1, np.int64)
+    noise_start = np.zeros((B, M), np.int64)
+    snr_db = np.zeros((B, M), np.float64)
+    for b in range(B):
+        if rir_bank is not None and g.random() < p_reverb:
+            rir_idx[b] = g.integers(0, rir_bank.num_rirs)
+        if groups and g.random() < p_noise:
+            ids, slo, shi, clo, chi, _ = groups[g.choice(len(groups), p=weights / weights.sum())]
+            c = int(g.integers(clo, chi + 1))
+            q = ids[g.integers(0, ids.size, c)]
+            noise_idx[b, :c] = q
+            noise_start[b, :c] = g.integers(0, np.maximum(noise_bank.lengths[q] - L, 0) + 1)
+            snr_db[b, :c] = g.uniform(slo, shi, c)
+    return {"rir_idx": torch.from_numpy(rir_idx), "noise_idx": torch.from_numpy(noise_idx),
+            "noise_start": torch.from_numpy(noise_start), "snr_db": torch.from_numpy(snr_db)}
+
+
+def _index_pair(utt, start, what):
+    u = torch.as_tensor(utt)
+    s = torch.as_tensor(start)
+    if u.dim() != 1 or s.shape != u.shape or u.numel() == 0:
+        raise ValueError(f"{what}: expected 1-D utt and start of one length >= 1, got {tuple(u.shape)}, {tuple(s.shape)}")
+    if u.is_floating_point() or s.is_floating_point():
+        raise ValueError(f"{what}: utt and start must be integers")
+    return u, s
+
+
+def _check_host_index(u, s, lengths, what):
+    uh, sh = u.to(torch.int64).numpy(), s.cpu().to(torch.int64).numpy()
+    if uh.min() < 0 or uh.max() >= lengths.size:
+        raise ValueError(f"{what}: utterance index outside [0, {lengths.size})")
+    if sh.min() < 0 or np.any(sh >= lengths[uh]):
+        raise ValueError(f"{what}: a start lies outside [0, n_u)")
+
+
+def _masks(m, B, what, dev):
+    if m is None:
+        return None, 0
+    m = torch.as_tensor(m)
+    if m.dim() != 3 or m.shape[0] != B or m.shape[2] != 2 or m.is_floating_point():
+        raise ValueError(f"{what} must be integer (B, n, 2) with B = {B}, got {tuple(m.shape)} {m.dtype}")
+    if m.shape[1] == 0:
+        return None, 0
+    return _to_dev(m, torch.int32, dev), int(m.shape[1])
 
 
 def embed_utterances(model, bank: FeatureBank, utt, T: int = 160, hop: int = 80, batch: int = 256) -> torch.Tensor:

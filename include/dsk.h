@@ -582,6 +582,48 @@ int32_t dsk_fbank_crops(const float* feat, const int64_t* frame_off, int32_t U, 
                         int32_t B, int32_t T, const int32_t* time_masks, int32_t n_time, const int32_t* freq_masks,
                         int32_t n_freq, float* out, void* stream);
 
+/* Waveform augmentation of training segments (reverberation by room impulse responses and additive noise, the MUSAN +
+ * RIR recipe) and the features of equal-length segments.
+ *   dsk_fbank_filterbank: host only.  fb[64][257] fp32, the triangular mel filterbank dsk_fbank_batch applies
+ *     (python_speech_features get_filterbanks(nfilt=64, nfft=512, samplerate)).
+ *   dsk_wave_augment: out (B, L) fp32.  For example b, u = utt[b]:
+ *     segment      s[i] = speech[speech_off[u] + (start[b] + i) mod n_u] * 2^-15, i in [0, L)  (n_u = the utterance's
+ *                  sample count; int16 PCM, so exactly what librosa.load returns for a 16-bit file; the wrap is crops')
+ *     reverb       rir_idx[b] = -1 (or rir_idx NULL): r = s, bit for bit.  Otherwise h = RIR rir_idx[b] (rir[rir_off[i] ..
+ *                  rir_off[i+1]), L_h taps, used exactly as stored) and r[i] = sum_{k=0}^{min(i, L_h-1)} h[k] s[i-k]: the
+ *                  full convolution truncated to its first L samples, no alignment to the direct path.  Computed by
+ *                  uniformly partitioned overlap-save (1024-sample partitions, 2048-point fp32 FFTs, the partitions
+ *                  summed in a fixed order).
+ *     noise        M <= DSK_AUG_MAX_SOURCES sources per example, (B, M) noise_idx (-1 = none), noise_start, snr_db
+ *                  (fp64); n_j is read from the noise bank like s, wrapping.  P(x) = sum x^2 / L in fp64 in a fixed order;
+ *                  g_j = sqrt(P(r) / (P(n_j) 10^(snr_j / 10))), 0 when P(n_j) = 0; out[i] = r[i] + sum_j g_j n_j[i]
+ *                  evaluated in fp64 and rounded once to fp32.
+ *     An index or start outside its bank, a RIR longer than max_rir_len, a noise index < -1 or a non-finite SNR of a
+ *     used source makes example b NaN; nothing outside any bank is read and the other examples are unaffected.  Each
+ *     example's output depends only on its own arguments (bit-identical for any B, batch position or interleaved call).
+ *     Banks (speech / rir / noise samples and their int64 offsets) may be device memory or page-locked host memory (read
+ *     over the bus by the same kernels); pageable memory is rejected.  utt, start, rir_idx, noise_idx, noise_start,
+ *     snr_db: device arrays.  max_rir_len (host) sizes the partition count.  Limits, checked before any launch
+ *     (DSK_ERR_INVALID): B >= 1, 1 <= L <= 2^24, 0 <= M <= DSK_AUG_MAX_SOURCES, 1 <= max_rir_len <= DSK_AUG_MAX_RIR,
+ *     non-null pointers (the RIR bank only with rir_idx, the noise arrays only with M > 0).  No host synchronisation,
+ *     no pageable copy; scratch is stream-ordered (cudaMallocAsync / cudaFreeAsync).
+ *   dsk_fbank_segments: out (B, 1, T, 64) fp32, T = dsk_fbank_num_frames(L, sample_rate), the features of the B
+ *     segments audio (B, L) fp32: row b is dsk_fbank on audio[b] alone (pre-emphasis from the segment's first sample;
+ *     with subtract_mean, the mean over the segment's own T frames), then the SpecAugment masks exactly as
+ *     dsk_fbank_crops applies them.  fb: the device copy of dsk_fbank_filterbank(sample_rate).  No host
+ *     synchronisation.  For training, take L = flen + (T - 1) step samples (25 840 at 16 kHz for T = 160). */
+#define DSK_AUG_MAX_SOURCES 8
+#define DSK_AUG_MAX_RIR 65536
+int32_t dsk_fbank_filterbank(int32_t sample_rate, float* fb);
+int32_t dsk_wave_augment(const int16_t* speech, const int64_t* speech_off, int32_t U, const int64_t* utt,
+                         const int64_t* start, int32_t B, int32_t L, const float* rir, const int64_t* rir_off, int32_t R,
+                         int32_t max_rir_len, const int64_t* rir_idx, const int16_t* noise, const int64_t* noise_off,
+                         int32_t N, int32_t M, const int64_t* noise_idx, const int64_t* noise_start, const double* snr_db,
+                         float* out, void* stream);
+int32_t dsk_fbank_segments(const float* audio, int32_t B, int32_t L, int32_t sample_rate, int32_t log_scale,
+                           int32_t subtract_mean, const float* fb, const int32_t* time_masks, int32_t n_time,
+                           const int32_t* freq_masks, int32_t n_freq, float* out, void* stream);
+
 /* Threshold sweep of the verification metric (reference eval_metrics.py:16-37 calculate_roc, :53-88 calculate_val /
  * calculate_val_far; called from train_triplet.py:361): for every threshold t (double, as numpy's arange yields them)
  * tp[t] = #{i : same[i] && (double)dist[i] < t}, fp[t] = #{i : !same[i] && (double)dist[i] < t} — numpy's
