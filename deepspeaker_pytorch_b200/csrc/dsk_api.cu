@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <array>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -146,6 +147,7 @@ struct ConvLaunch {
   dsk::ConvParams p;
   int n_tile = 0;
   int grid = 0;
+  bool bf16 = false;  // operand type the tensor maps were encoded for (launch_conv instantiates the kernel for it)
   bool out_f32 = false;
 };
 
@@ -169,11 +171,35 @@ struct LayerCfg {
   int cin, cout, ksize, stride;
 };
 
+// What every cached plan of the tensor-core cosine and Gram ops holds besides its buffers' pointers and GEMM
+// descriptors: the key it was built for and its one device buffer (arena_alloc).  plan_acquire rebuilds a plan when the
+// key changes; release() frees the buffer and empties the plan (empty key, no buffer, no descriptors).
+template <typename Plan, int KeyLen>
+struct CachedPlan {
+  std::array<int, KeyLen> key{};
+  uint8_t* buf = nullptr;
+  cudaError_t release() {
+    const cudaError_t e = cudaFree(buf);
+    static_cast<Plan&>(*this) = Plan();
+    return e;
+  }
+};
+
+// Cached plan of the all-pairs ops for one (N, D) and anchor row range [row0, row0 + rows): E rounded to 16 bit in the
+// handle's operand type, the squared norms of the rounded rows and the Gram G = E16[row0 : row0 + rows_pad] E16^T.
+// Npad: N rounded up to 128; Epad: the rows of E16 the Gram's "pixel" view can read (rows >= N are zero).
+struct AllpairsPlan : CachedPlan<AllpairsPlan, 4> {  // key (N, D, row0, rows)
+  int Npad = 0, Epad = 0;
+  uint16_t* e16 = nullptr;   // [Epad][D]
+  float* gram = nullptr;     // [rows_pad][Npad]
+  float* norms = nullptr;    // [Epad]
+  std::vector<ConvLaunch> gemm;
+};
+
 // Cached plan of the AAM-softmax op for one (N, C, D): fp16 hi/lo operand images, fp32 GEMM outputs and workspaces, and
 // the descriptors of its three GEMMs.  Np / Cp: N and C rounded up to 128 (the GEMM's pixel tile).
-struct AamPlan {
+struct AamPlan : CachedPlan<AamPlan, 3> {  // key (N, C, D)
   int N = 0, C = 0, D = 0, Np = 0, Cp = 0;
-  uint8_t* buf = nullptr;
   uint16_t *ea = nullptr, *wb = nullptr;     // forward operands: E^ [Np][3D] (A side), W^ [Cp][3D] (B side)
   uint16_t *et = nullptr, *wt = nullptr;     // backward B operands, transposed: E^T [D][3Np], W^T [D][3Cp]
   uint16_t *da = nullptr, *dt = nullptr;     // backward A operands: dcos [Np][3Cp], dcos^T [Cp][3Np] (K-sliced)
@@ -190,10 +216,9 @@ struct AamPlan {
 // speaker centroids in place of the class weights - the cosines and gE^ = dcos C^ for the rows x P block of the row
 // range [row0, row0 + rows), the centroid gradient gC^ = dcos^T E^ over all N rows - plus GE2E's own buffers.  Np, Rp,
 // Cp: N, rows and P rounded up to 128 (the GEMM's pixel tile).
-struct Ge2ePlan {
-  int N = 0, P = 0, D = 0, row0 = 0, rows = 0, Np = 0, Rp = 0, Cp = 0;
+struct Ge2ePlan : CachedPlan<Ge2ePlan, 5> {  // key (N, P, D, row0, rows)
+  int N = 0, P = 0, D = 0, Np = 0, Rp = 0, Cp = 0;
   int sc = 0, sn = 0;                        // K slices of gE^ and gC^: ceil(Cp / kAamSlice), ceil(Np / kAamSlice)
-  uint8_t* buf = nullptr;
   float* cent = nullptr;                     // [P][D] inclusive centroids (mean of the normalised rows)
   double* nr64 = nullptr;                    // [N] fp64 row norms
   float *nrm_e = nullptr, *nrm_c = nullptr;  // [N], [P] fp32 norms of the rows and the centroids
@@ -217,14 +242,53 @@ struct Ge2ePlan {
 
 // Cached plan of the cosine-scoring ops for one (Nc, D, chunk): the fp16 hi/lo operand images of a row chunk of E and of
 // the cohort, their norms, the chunk's fp32 cosines and the descriptors of the one GEMM.  Np: Nc rounded up to 128.
-struct ScorePlan {
-  int Nc = 0, D = 0, chunk = 0, Np = 0;
-  uint8_t* buf = nullptr;
+struct ScorePlan : CachedPlan<ScorePlan, 3> {  // key (Nc, D, chunk)
+  int D = 0, chunk = 0, Np = 0;
   uint16_t *ea = nullptr, *cb = nullptr;     // E^ chunk [chunk][3D] (A side), cohort^ [Np][3D] (B side)
   float *nrm_e = nullptr, *nrm_c = nullptr;  // [chunk], [Np]
   float* cos = nullptr;                      // [chunk][Np]
   std::vector<ConvLaunch> gemm;
 };
+
+// One part of a plan's buffer: the pointer arena_alloc sets and the part's size in bytes (0 allowed)
+struct ArenaPart {
+  template <typename T>
+  ArenaPart(T** p, size_t n) : slot(reinterpret_cast<void**>(p)), bytes(n) {}
+  void** slot;
+  size_t bytes;
+};
+
+// One cudaMalloc for all parts of a plan, each at a 256-byte aligned offset, zeroed on `s` once here (padding that no
+// kernel writes stays zero).  *buf receives the allocation, which the plan's release() frees.
+int arena_alloc(uint8_t** buf, std::initializer_list<ArenaPart> parts, cudaStream_t s) {
+  const auto aligned = [](size_t n) { return (n + 255) / 256 * 256; };
+  size_t bytes = 0;
+  for (const ArenaPart& p : parts) bytes += aligned(p.bytes);
+  CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(buf), bytes));
+  CUDA_TRY(cudaMemsetAsync(*buf, 0, bytes, s));
+  bytes = 0;
+  for (const ArenaPart& p : parts) {
+    *p.slot = *buf + bytes;
+    bytes += aligned(p.bytes);
+  }
+  return DSK_OK;
+}
+
+// Make the cached plan P current for `key`.  A plan built for another key is rebuilt: `s` is synchronised (its kernels
+// may still use the old buffer), P released, then build() allocates P's buffer and builds its GEMM descriptors.  A failed
+// build leaves P released.  A call whose key matches never synchronises.
+template <typename Plan, typename Build>
+int plan_acquire(Plan& P, const decltype(Plan::key)& key, cudaStream_t s, Build build) {
+  if (P.buf && P.key == key) return DSK_OK;
+  CUDA_TRY(cudaStreamSynchronize(s));
+  CUDA_TRY(P.release());
+  if (const int rc = build()) {
+    P.release();
+    return rc;
+  }
+  P.key = key;
+  return DSK_OK;
+}
 
 // conv index i = 3*stage + {0: 5x5 s2 entry conv, 1,2: 3x3 block convs}
 LayerCfg layer_cfg(int i) {
@@ -308,10 +372,7 @@ struct dsk_handle_s {
   float loss_scale = 0.f;  // 0 = automatic
   bool defer_stats = false;  // dsk_set_defer_running_stats: train forwards record batch statistics, the caller commits them in order
   std::vector<dsk_train_ctx_s*> ctx_pool;
-  // cached all-pairs plan (buffers + Gram GEMM descriptors) for the last (N, D) and anchor row range [row0, row0 + rows)
-  int ap_N = 0, ap_D = 0, ap_row0 = 0, ap_rows = 0;
-  uint8_t* ap_buf = nullptr;
-  std::vector<ConvLaunch> ap_gemm;
+  AllpairsPlan allpairs;       // cached all-pairs Gram plan (the batch-hard and tensor-core top-k ops)
   AamPlan aam;                 // cached AAM-softmax plan (its own slot: a step may use both ops)
   Ge2ePlan ge2e;               // cached GE2E plan (its own slot: a step may sum the GE2E and AAM losses)
   ScorePlan score;             // cached cosine-scoring plan (its own slot: evaluation runs between training steps)
@@ -400,7 +461,7 @@ void choose_tile(int B, int Hout, int Wout, int total, int& wt, int& hb, int& nb
   }
 }
 
-template <int N_TILE, bool BF16, bool OUT_F32 = false>
+template <int N_TILE, bool BF16, bool OUT_F32>
 int launch_conv_t(const ConvLaunch& L, cudaStream_t s) {
   auto kern = dsk::conv_umma_kernel<N_TILE, BF16, OUT_F32>;
   if (int rc = ensure_smem_optin(reinterpret_cast<const void*>(kern), dsk::ConvSmem<N_TILE>::kTotal)) return rc;
@@ -408,33 +469,19 @@ int launch_conv_t(const ConvLaunch& L, cudaStream_t s) {
   return DSK_OK;
 }
 
-int launch_conv(const dsk_handle_s* h, const ConvLaunch& L, cudaStream_t s) {
-  if (L.out_f32) {
-    if (h->bf16) {
-      switch (L.n_tile) {
-        case 64: return launch_conv_t<64, true, true>(L, s);
-        case 128: return launch_conv_t<128, true, true>(L, s);
-      }
-    } else {
-      switch (L.n_tile) {
-        case 64: return launch_conv_t<64, false, true>(L, s);
-        case 128: return launch_conv_t<128, false, true>(L, s);
-      }
-    }
-    return fail(DSK_ERR_INVALID, "unsupported N tile %d", L.n_tile);
-  }
-  if (h->bf16) {
-    switch (L.n_tile) {
-      case 64: return launch_conv_t<64, true>(L, s);
-      case 128: return launch_conv_t<128, true>(L, s);
-    }
-  } else {
-    switch (L.n_tile) {
-      case 64: return launch_conv_t<64, false>(L, s);
-      case 128: return launch_conv_t<128, false>(L, s);
-    }
+template <bool BF16, bool OUT_F32>
+int launch_conv_n(const ConvLaunch& L, cudaStream_t s) {
+  switch (L.n_tile) {
+    case 64: return launch_conv_t<64, BF16, OUT_F32>(L, s);
+    case 128: return launch_conv_t<128, BF16, OUT_F32>(L, s);
   }
   return fail(DSK_ERR_INVALID, "unsupported N tile %d", L.n_tile);
+}
+
+// Launch a conv or GEMM descriptor built by build_conv_core, on the kernel instantiated for what it was built for
+int launch_conv(const ConvLaunch& L, cudaStream_t s) {
+  if (L.bf16) return L.out_f32 ? launch_conv_n<true, true>(L, s) : launch_conv_n<true, false>(L, s);
+  return L.out_f32 ? launch_conv_n<false, true>(L, s) : launch_conv_n<false, false>(L, s);
 }
 
 // A 5-D TMA view (dims innermost first; str[i] = byte stride of dim i+1) of a 16-bit tensor.
@@ -482,7 +529,8 @@ int build_conv_core(const dsk_handle_s* h, ConvLaunch* L, const View5& a, const 
   if (k_ch % 64 || n_out % 64 || k_ch < 64 || n_out < 64 || n_out > 512)
     return fail(DSK_ERR_INVALID, "conv: channel counts must be multiples of 64 and <= 512 outputs (got %d, %d)", k_ch, n_out);
   if (Wgrid > 128 || 128 % Wgrid) return fail(DSK_ERR_INVALID, "conv: output width %d must divide 128", Wgrid);
-  const bool bf = h->bf16 && !f16;  // f16: fp16 operands whatever the handle's type (launch with launch_gemm_f16)
+  const bool bf = h->bf16 && !f16;  // f16: fp16 operands whatever the handle's type
+  L->bf16 = bf;
   dsk::ConvParams& p = L->p;
   memset(&p, 0, sizeof(p));
   choose_tile(B, Hgrid, Wgrid, 128, p.wt, p.hb, p.nb);
@@ -705,6 +753,39 @@ int build_conv_s2_padded(const dsk_handle_s* h, ConvLaunch* L, const void* in, c
   return build_conv_core(h, L, padded_parity_view(in, B, Hin, Win, cin), wpk, cin, cout, 25,
                          padded_nhwc_view(out, B, Hin / 2, Win / 2, cout), nullptr, B, Hin / 2, Win / 2, tt, dsk::CONV_CLIP,
                          20.0f, scale, bias, 0, 0);
+}
+
+// The GEMMs of the cached plans: O (rows_pad x n_total fp32) = A (rows_pad x K) B^T (n_total x K), both 16-bit row-major
+// images (f16: fp16 operands whatever the handle's type).  Rows of A are the "pixels" (W = 128, H = rows_pad / 128), rows
+// of B the "output channels", <= 512 per launch; one tap.
+int build_gemm(const dsk_handle_s* h, std::vector<ConvLaunch>* out, const uint16_t* A, int rows_pad, const uint16_t* B,
+               int n_total, int K, float* O, bool f16) {
+  TapTable tt;
+  tt.add(0, 0, 0, 0, 0);
+  for (int c0 = 0; c0 < n_total; c0 += 512) {
+    ConvLaunch L;
+    const int rc = build_conv_core(h, &L, nhwc_view(A, 1, rows_pad / 128, 128, K), B + static_cast<size_t>(c0) * K, K,
+                                   n_total - c0 < 512 ? n_total - c0 : 512, 1, nhwc_view(O, 1, rows_pad / 128, 128, n_total),
+                                   nullptr, 1, rows_pad / 128, 128, tt, 0, 0.f, nullptr, nullptr, c0, 0, true, f16);
+    if (rc) return rc;
+    out->push_back(L);
+  }
+  return DSK_OK;
+}
+
+// A backward product of the cosine ops over a K dimension of Kp (a multiple of 128) with fp16 operands, split K
+// deterministically: one build_gemm per kAamSlice-wide K slice, slice k of the K-sliced A image ([rows_pad][3w] at
+// k kAamSlice 3 rows_pad) times slice k of the transposed image Bt ([D][3w]) into its own output O + k rows_pad D.
+int build_sliced_gemm(const dsk_handle_s* h, std::vector<ConvLaunch>* out, const uint16_t* A, int rows_pad,
+                      const uint16_t* Bt, int D, int Kp, float* O) {
+  const size_t ks = dsk::kAamSlice;
+  for (int k = 0; k * dsk::kAamSlice < Kp; ++k) {
+    const int w = Kp - k * dsk::kAamSlice < dsk::kAamSlice ? Kp - k * dsk::kAamSlice : dsk::kAamSlice;
+    if (int rc = build_gemm(h, out, A + k * ks * 3 * rows_pad, rows_pad, Bt + k * ks * 3 * D, D, 3 * w,
+                            O + static_cast<size_t>(k) * rows_pad * D, true))
+      return rc;
+  }
+  return DSK_OK;
 }
 
 // Packed tap order of the parity-planar 5x5 s2 conv: plane (ph, pw) major, then r, then s. slot -> original r*5+s.
@@ -1124,11 +1205,11 @@ int32_t dsk_destroy(dsk_handle h) {
   cudaFree(h->ws);
   cudaFree(h->sk_partial);
   cudaFree(h->sk_flags);
-  cudaFree(h->ap_buf);
-  cudaFree(h->aam.buf);
-  cudaFree(h->ge2e.buf);
-  cudaFree(h->score.buf);
-  cudaFree(h->search.buf);
+  h->allpairs.release();
+  h->aam.release();
+  h->ge2e.release();
+  h->score.release();
+  h->search.release();
   cudaFree(h->ones);
   cudaFree(h->zeros);
   for (dsk_train_ctx_s* c : h->ctx_pool) {
@@ -1353,7 +1434,7 @@ int enqueue_forward(dsk_handle h, dsk_handle_s::Plan* pl, const float* x, int B,
     mark(true);
   }
   for (int i = 1; i < DSK_NUM_CONV; ++i) {
-    rc = (i % 3 == 0 && !h->planar_s2) ? launch_conv(h, pl->conv[i], s) : launch_halo(h, pl->halo[i], s);
+    rc = (i % 3 == 0 && !h->planar_s2) ? launch_conv(pl->conv[i], s) : launch_halo(h, pl->halo[i], s);
     if (rc) return rc;
     mark(i == DSK_NUM_CONV - 1);
   }
@@ -1747,7 +1828,7 @@ int32_t dsk_debug_set_backward_capture(dsk_handle h, const dsk_backward_capture*
 
 // layer i's conv into raw[i]: conv1 from the input features, else the bound conv of y[i-1]
 static int train_conv(dsk_handle h, const dsk_train_ctx_s* c, int i, cudaStream_t s) {
-  if (i > 0) return launch_conv(h, c->conv[i], s);
+  if (i > 0) return launch_conv(c->conv[i], s);
   dsk::conv1_kernel<false, true><<<c->B * ((c->T / 2 + 7) / 8), 256, 0, s>>>(c->x, h->conv1_w, h->ones, h->zeros, c->raw[0],
                                                                             c->T, 0, 0.f, 0);
   KERNEL_CHECK();
@@ -1899,7 +1980,7 @@ static int train_bn_backward(dsk_handle h, dsk_train_ctx_s* c, int i, const floa
   dsk::unpack_wgrad_kernel<<<static_cast<int>((n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096), 256, 0, s>>>(
       c->dwacc, g->conv_w[i], lc.cout, lc.cin, taps, 1.0f, c->wgrad[i].p.ksplit, c->wgrad[i].p.slice_elems, c->ls);
   KERNEL_CHECK();
-  for (int k = 0; k < c->n_dgrad[i] && !rc; ++k) rc = launch_conv(h, c->dgrad[i][k], s);
+  for (int k = 0; k < c->n_dgrad[i] && !rc; ++k) rc = launch_conv(c->dgrad[i][k], s);
   return rc;
 }
 
@@ -2213,11 +2294,11 @@ int32_t dsk_conv2d_dgrad_nhwc(dsk_handle h, const void* G, const float* w_oihw, 
   ConvLaunch L;
   if (stride == 1) {
     rc = build_dgrad_s1(h, &L, G, wpk, res, gin, B, Hin, Win, cin, cout);
-    if (!rc) rc = launch_conv(h, L, s);
+    if (!rc) rc = launch_conv(L, s);
   } else {
     for (int cls = 0; cls < 4 && !rc; ++cls) {
       rc = build_dgrad_s2(h, &L, G, wpk, gin, B, Hout, Wout, cin, cout, cls >> 1, cls & 1);
-      if (!rc) rc = launch_conv(h, L, s);
+      if (!rc) rc = launch_conv(L, s);
     }
   }
   CUDA_TRY(cudaFreeAsync(wpk, s));
@@ -2385,7 +2466,7 @@ int32_t dsk_conv2d_nhwc(dsk_handle h, const void* in, const void* w_packed, cons
   ConvLaunch L;
   rc = build_conv(h, &L, in, w_packed, scale, bias, res, out, B, Hin, Win, cin, cout, ksize, stride, flags, clip_hi);
   if (rc) return rc;
-  return launch_conv(h, L, static_cast<cudaStream_t>(stream));
+  return launch_conv(L, static_cast<cudaStream_t>(stream));
 }
 
 int32_t dsk_pack_conv_weight(dsk_handle h, const float* w_oihw, void* w_packed, int32_t cout, int32_t cin,
@@ -2503,48 +2584,26 @@ int32_t dsk_gather_rows(const float* src, const int64_t* idx, const int32_t* cou
 // synchronises `s`: a caller that alternates row ranges pays it on every change.
 static int allpairs_gram(dsk_handle h, const float* E, int N, int D, int row0, int rows, cudaStream_t s,
                          const float** G_out, const float** norms_out, int* Npad_out) {
-  int rc = 0;
-  const int Npad = (N + 127) / 128 * 128, rows_pad = (rows + 127) / 128 * 128;
-  // E16 rows: the "pixel" view reads rows_pad rows from row0, which may run past Npad; rows >= N are zero
-  const int Epad = row0 + rows_pad > Npad ? row0 + rows_pad : Npad;
-  const size_t e16_bytes = static_cast<size_t>(Epad) * D * 2, g_bytes = static_cast<size_t>(rows_pad) * Npad * 4;
-  if (h->ap_N != N || h->ap_D != D || h->ap_row0 != row0 || h->ap_rows != rows) {
-    // (re)build the plan: buffers and the Gram GEMM descriptors.  Gram on the tensor cores: the anchor rows of E16 are
-    // the "pixels" (W = 128, H = rows_pad/128), all rows of E16 the "output channels" (<= 512 per launch); one tap, K = D
-    CUDA_TRY(cudaStreamSynchronize(s));
-    if (h->ap_buf) CUDA_TRY(cudaFree(h->ap_buf));
-    h->ap_buf = nullptr;
-    h->ap_N = h->ap_D = h->ap_row0 = h->ap_rows = 0;
-    h->ap_gemm.clear();
-    CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&h->ap_buf), e16_bytes + g_bytes + static_cast<size_t>(Epad) * 4));
-    uint16_t* E16p = reinterpret_cast<uint16_t*>(h->ap_buf);
-    float* Gp = reinterpret_cast<float*>(h->ap_buf + e16_bytes);
-    TapTable tt;
-    tt.add(0, 0, 0, 0, 0);
-    for (int c0 = 0; c0 < Npad; c0 += 512) {
-      const int n_out = Npad - c0 < 512 ? Npad - c0 : 512;
-      ConvLaunch L;
-      rc = build_conv_core(h, &L, nhwc_view(E16p + static_cast<size_t>(row0) * D, 1, rows_pad / 128, 128, D),
-                           E16p + static_cast<size_t>(c0) * D, D, n_out, 1, nhwc_view(Gp, 1, rows_pad / 128, 128, Npad),
-                           nullptr, 1, rows_pad / 128, 128, tt, 0, 0.f, nullptr, nullptr, c0, 0, true);
-      if (rc) return rc;
-      h->ap_gemm.push_back(L);
-    }
-    h->ap_N = N;
-    h->ap_D = D;
-    h->ap_row0 = row0;
-    h->ap_rows = rows;
-  }
-  uint16_t* E16 = reinterpret_cast<uint16_t*>(h->ap_buf);
-  float* G = reinterpret_cast<float*>(h->ap_buf + e16_bytes);
-  float* norms = reinterpret_cast<float*>(h->ap_buf + e16_bytes + g_bytes);
-  if (h->bf16) dsk::allpairs_prep_kernel<true><<<Epad, 128, 0, s>>>(E, N, D, E16, norms);
-  else dsk::allpairs_prep_kernel<false><<<Epad, 128, 0, s>>>(E, N, D, E16, norms);
+  AllpairsPlan& A = h->allpairs;
+  int rc = plan_acquire(A, {N, D, row0, rows}, s, [&]() -> int {
+    const int rows_pad = (rows + 127) / 128 * 128;
+    A.Npad = (N + 127) / 128 * 128;
+    // the "pixel" view reads rows_pad rows of E16 from row0, which may run past Npad
+    A.Epad = row0 + rows_pad > A.Npad ? row0 + rows_pad : A.Npad;
+    if (int rc = arena_alloc(&A.buf, {{&A.e16, A.Epad * D * 2ull}, {&A.gram, 1ull * rows_pad * A.Npad * 4},
+                                      {&A.norms, A.Epad * 4ull}}, s))
+      return rc;
+    // the anchor rows of E16 against all its rows, K = D, in the handle's operand type
+    return build_gemm(h, &A.gemm, A.e16 + static_cast<size_t>(row0) * D, rows_pad, A.e16, A.Npad, D, A.gram, false);
+  });
+  if (rc) return rc;
+  if (h->bf16) dsk::allpairs_prep_kernel<true><<<A.Epad, 128, 0, s>>>(E, N, D, A.e16, A.norms);
+  else dsk::allpairs_prep_kernel<false><<<A.Epad, 128, 0, s>>>(E, N, D, A.e16, A.norms);
   KERNEL_CHECK();
-  for (size_t i = 0; i < h->ap_gemm.size() && !rc; ++i) rc = launch_conv(h, h->ap_gemm[i], s);
-  *G_out = G;
-  *norms_out = norms;
-  *Npad_out = Npad;
+  for (size_t i = 0; i < A.gemm.size() && !rc; ++i) rc = launch_conv(A.gemm[i], s);
+  *G_out = A.gram;
+  *norms_out = A.norms;
+  *Npad_out = A.Npad;
   return rc;
 }
 
@@ -2683,86 +2742,36 @@ int32_t dsk_allpairs_topk(const float* E, const int64_t* labels, int32_t N, int3
 }
 
 // ---- additive angular margin softmax ------------------------------------------------------------------------------
-// A GEMM of the AAM-softmax op: fp16 operands whatever the handle's type (a bf16 hi/lo split keeps 16 bits, not 22).
-static int launch_gemm_f16(const ConvLaunch& L, cudaStream_t s) {
-  switch (L.n_tile) {
-    case 64: return launch_conv_t<64, false, true>(L, s);
-    case 128: return launch_conv_t<128, false, true>(L, s);
-  }
-  return fail(DSK_ERR_INVALID, "unsupported N tile %d", L.n_tile);
-}
+// The GEMMs of the cosine ops (AAM-softmax, GE2E, scoring) take fp16 operands whatever the handle's type: a bf16 hi/lo
+// split keeps 16 bits, not 22.
 
-// out (rows_pad x n_total fp32) = A (rows_pad x K) B^T (n_total x K), both 16-bit row-major images: rows of A are the
-// "pixels" (W = 128, H = rows_pad / 128), rows of B the "output channels", <= 512 per launch; one tap.
-static int aam_build_gemm(dsk_handle h, std::vector<ConvLaunch>* out, const uint16_t* A, int rows_pad, const uint16_t* B,
-                          int n_total, int K, float* O) {
-  TapTable tt;
-  tt.add(0, 0, 0, 0, 0);
-  for (int c0 = 0; c0 < n_total; c0 += 512) {
-    ConvLaunch L;
-    const int rc = build_conv_core(h, &L, nhwc_view(A, 1, rows_pad / 128, 128, K), B + static_cast<size_t>(c0) * K, K,
-                                   n_total - c0 < 512 ? n_total - c0 : 512, 1, nhwc_view(O, 1, rows_pad / 128, 128, n_total),
-                                   nullptr, 1, rows_pad / 128, 128, tt, 0, 0.f, nullptr, nullptr, c0, 0, true, true);
-    if (rc) return rc;
-    out->push_back(L);
-  }
-  return DSK_OK;
-}
-
-// (Re)build the AAM plan in slot P of h (h->aam) for (N, C, D).  A rebuild synchronises `s` (buffers in
-// use are freed).
+// The AAM plan in slot P of h (h->aam) for (N, C, D).  A rebuild synchronises `s` (buffers in use are freed).
 static int aam_plan(dsk_handle h, AamPlan& P, int N, int C, int D, cudaStream_t s, AamPlan** out) {
   *out = &P;
-  if (P.buf && P.N == N && P.C == C && P.D == D) return DSK_OK;
-  CUDA_TRY(cudaStreamSynchronize(s));
-  if (P.buf) CUDA_TRY(cudaFree(P.buf));
-  P = AamPlan();
-  const int Np = (N + 127) / 128 * 128, Cp = (C + 127) / 128 * 128;
-  const int sc = (Cp + dsk::kAamSlice - 1) / dsk::kAamSlice, sn = (Np + dsk::kAamSlice - 1) / dsk::kAamSlice;
-  const size_t d3 = 3ull * D;
-  size_t off = 0;
-  std::vector<std::pair<void**, size_t>> parts = {
-      {reinterpret_cast<void**>(&P.ea), Np * d3 * 2},   {reinterpret_cast<void**>(&P.wb), Cp * d3 * 2},
-      {reinterpret_cast<void**>(&P.et), Np * d3 * 2},   {reinterpret_cast<void**>(&P.wt), Cp * d3 * 2},
-      {reinterpret_cast<void**>(&P.da), 3ull * Np * Cp * 2}, {reinterpret_cast<void**>(&P.dt), 3ull * Np * Cp * 2},
-      {reinterpret_cast<void**>(&P.nrm_e), Np * 4ull},  {reinterpret_cast<void**>(&P.nrm_w), Cp * 4ull},
-      {reinterpret_cast<void**>(&P.gcos), 1ull * Np * Cp * 4}, {reinterpret_cast<void**>(&P.dcos), 1ull * Np * Cp * 4},
-      {reinterpret_cast<void**>(&P.rinv), Np * 4ull},   {reinterpret_cast<void**>(&P.cinv), Cp * 4ull},
-      {reinterpret_cast<void**>(&P.ge), 1ull * sc * Np * D * 4}, {reinterpret_cast<void**>(&P.gw), 1ull * sn * Cp * D * 4},
-      {reinterpret_cast<void**>(&P.row_loss), Np * 4ull}};
-  for (auto& p : parts) off += (p.second + 255) / 256 * 256;
-  CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&P.buf), off));
-  off = 0;
-  for (auto& p : parts) {
-    *p.first = P.buf + off;
-    off += (p.second + 255) / 256 * 256;
-  }
-  int rc = aam_build_gemm(h, &P.fwd, P.ea, Np, P.wb, Cp, 3 * D, P.gcos);  // cos = E^ W^T, K = 3D
-  // gE^ = dcos W^ (K = 3Cp) and gW^ = dcos^T E^ (K = 3Np), one GEMM per K slice into the slice's own output
-  const size_t ks = dsk::kAamSlice;
-  for (int k = 0; k < sc && !rc; ++k) {
-    const int w = Cp - k * dsk::kAamSlice < dsk::kAamSlice ? Cp - k * dsk::kAamSlice : dsk::kAamSlice;
-    rc = aam_build_gemm(h, &P.ge_gemm, P.da + k * ks * 3 * Np, Np, P.wt + k * ks * 3 * D, D, 3 * w,
-                        P.ge + static_cast<size_t>(k) * Np * D);
-  }
-  for (int k = 0; k < sn && !rc; ++k) {
-    const int w = Np - k * dsk::kAamSlice < dsk::kAamSlice ? Np - k * dsk::kAamSlice : dsk::kAamSlice;
-    rc = aam_build_gemm(h, &P.gw_gemm, P.dt + k * ks * 3 * Cp, Cp, P.et + k * ks * 3 * D, D, 3 * w,
-                        P.gw + static_cast<size_t>(k) * Cp * D);
-  }
-  if (rc) {
-    cudaFree(P.buf);
-    P = AamPlan();
+  return plan_acquire(P, {N, C, D}, s, [&]() -> int {
+    const int Np = (N + 127) / 128 * 128, Cp = (C + 127) / 128 * 128;
+    P.N = N;
+    P.C = C;
+    P.D = D;
+    P.Np = Np;
+    P.Cp = Cp;
+    P.sc = (Cp + dsk::kAamSlice - 1) / dsk::kAamSlice;
+    P.sn = (Np + dsk::kAamSlice - 1) / dsk::kAamSlice;
+    const size_t d3 = 3ull * D;
+    int rc = arena_alloc(&P.buf, {{&P.ea, Np * d3 * 2},                {&P.wb, Cp * d3 * 2},
+                                  {&P.et, Np * d3 * 2},                {&P.wt, Cp * d3 * 2},
+                                  {&P.da, 3ull * Np * Cp * 2},         {&P.dt, 3ull * Np * Cp * 2},
+                                  {&P.nrm_e, Np * 4ull},               {&P.nrm_w, Cp * 4ull},
+                                  {&P.gcos, 1ull * Np * Cp * 4},       {&P.dcos, 1ull * Np * Cp * 4},
+                                  {&P.rinv, Np * 4ull},                {&P.cinv, Cp * 4ull},
+                                  {&P.ge, 1ull * P.sc * Np * D * 4},   {&P.gw, 1ull * P.sn * Cp * D * 4},
+                                  {&P.row_loss, Np * 4ull}}, s);
+    if (!rc) rc = build_gemm(h, &P.fwd, P.ea, Np, P.wb, Cp, 3 * D, P.gcos, true);  // cos = E^ W^T, K = 3D
+    // gE^ = dcos W^ (K = 3Cp) and gW^ = dcos^T E^ (K = 3Np)
+    if (!rc) rc = build_sliced_gemm(h, &P.ge_gemm, P.da, Np, P.wt, D, Cp, P.ge);
+    if (!rc) rc = build_sliced_gemm(h, &P.gw_gemm, P.dt, Cp, P.et, D, Np, P.gw);
     return rc;
-  }
-  P.N = N;
-  P.C = C;
-  P.D = D;
-  P.Np = Np;
-  P.Cp = Cp;
-  P.sc = sc;
-  P.sn = sn;
-  return DSK_OK;
+  });
 }
 
 static int aam_check(dsk_handle h, bool ptrs_ok, int N, int C, int D, float margin, float scale, const char* what) {
@@ -2780,20 +2789,39 @@ static dsk::AamMargin aam_margin(float margin, float scale) {
           static_cast<float>(std::sin(pi - m) * m), scale};
 }
 
+// Rows X[0, n) (D wide) of one operand of a cosine GEMM: their norms nrm (taken by cos_prep when `norm`, else already
+// there), and the hi/lo images cos_prep writes of them, padded with zero rows to n_pad: `img` row-major [n_pad][3D],
+// `imgT` transposed and K-sliced (either may be NULL).
+struct CosRows {
+  const float* X;
+  int n, n_pad;
+  float* nrm;
+  bool norm;
+  uint16_t *img, *imgT;
+};
+
+// Operand prep of a cosine GEMM on `s`: the norms of the A-side rows a and the B-side rows b, then their images.  Either
+// side may be NULL.
+static int cos_prep(int D, const CosRows* a, const CosRows* b, cudaStream_t s) {
+  for (const CosRows* r : {a, b})
+    if (r && r->norm) {
+      dsk::aam_norm_kernel<<<(r->n + 7) / 8, 256, 0, s>>>(r->X, r->n, D, r->nrm);
+      KERNEL_CHECK();
+    }
+  for (const CosRows* r : {a, b})
+    if (r && (r->img || r->imgT)) {
+      dsk::aam_split_kernel<<<dim3(D / 64, r->n_pad / 32), 256, 0, s>>>(r->X, r->nrm, r->n, r->n_pad, D, r == a ? 1 : 0,
+                                                                        r->img, r->imgT);
+      KERNEL_CHECK();
+    }
+  return DSK_OK;
+}
+
 // norms of E and W, and their hi/lo operand images (forward: row-major; backward: transposed)
 static int aam_prep(const AamPlan& P, const float* E, const float* W, bool backward, cudaStream_t s) {
-  const int D = P.D;
-  dsk::aam_norm_kernel<<<(P.N + 7) / 8, 256, 0, s>>>(E, P.N, D, P.nrm_e);
-  KERNEL_CHECK();
-  dsk::aam_norm_kernel<<<(P.C + 7) / 8, 256, 0, s>>>(W, P.C, D, P.nrm_w);
-  KERNEL_CHECK();
-  dsk::aam_split_kernel<<<dim3(D / 64, P.Np / 32), 256, 0, s>>>(E, P.nrm_e, P.N, P.Np, D, 1, backward ? nullptr : P.ea,
-                                                                 backward ? P.et : nullptr);
-  KERNEL_CHECK();
-  dsk::aam_split_kernel<<<dim3(D / 64, P.Cp / 32), 256, 0, s>>>(W, P.nrm_w, P.C, P.Cp, D, 0, backward ? nullptr : P.wb,
-                                                                 backward ? P.wt : nullptr);
-  KERNEL_CHECK();
-  return DSK_OK;
+  const CosRows e{E, P.N, P.Np, P.nrm_e, true, backward ? nullptr : P.ea, backward ? P.et : nullptr};
+  const CosRows w{W, P.C, P.Cp, P.nrm_w, true, backward ? nullptr : P.wb, backward ? P.wt : nullptr};
+  return cos_prep(P.D, &e, &w, s);
 }
 
 int32_t dsk_aam_softmax(dsk_handle h, const float* E, const float* W, const int64_t* labels, int32_t N, int32_t C,
@@ -2805,7 +2833,7 @@ int32_t dsk_aam_softmax(dsk_handle h, const float* E, const float* W, const int6
   if ((rc = aam_plan(h, h->aam, N, C, D, s, &P))) return rc;
   if ((rc = aam_prep(*P, E, W, false, s))) return rc;
   for (const ConvLaunch& L : P->fwd)
-    if ((rc = launch_gemm_f16(L, s))) return rc;
+    if ((rc = launch_conv(L, s))) return rc;
   dsk::aam_rows_kernel<<<N, 256, 0, s>>>(P->gcos, P->Cp, E, W, D, labels, C, aam_margin(margin, scale), cos, lse,
                                          P->row_loss);
   KERNEL_CHECK();
@@ -2830,9 +2858,9 @@ int32_t dsk_aam_softmax_bwd(dsk_handle h, const float* E, const float* W, const 
   dsk::aam_dcos_t_kernel<<<P->Cp / 32, 256, 0, s>>>(P->dcos, P->Np, P->Cp, P->dt, P->cinv);
   KERNEL_CHECK();
   for (const ConvLaunch& L : P->ge_gemm)
-    if ((rc = launch_gemm_f16(L, s))) return rc;
+    if ((rc = launch_conv(L, s))) return rc;
   for (const ConvLaunch& L : P->gw_gemm)
-    if ((rc = launch_gemm_f16(L, s))) return rc;
+    if ((rc = launch_conv(L, s))) return rc;
   dsk::aam_normalize_bwd_kernel<<<(N + 7) / 8, 256, 0, s>>>(E, P->nrm_e, P->ge, P->sc, static_cast<long>(P->Np) * D,
                                                             P->rinv, N, D, gE);
   KERNEL_CHECK();
@@ -2843,76 +2871,47 @@ int32_t dsk_aam_softmax_bwd(dsk_handle h, const float* E, const float* W, const 
 }
 
 // ---- generalised end-to-end (GE2E) loss ---------------------------------------------------------------------------
-// (Re)build the handle's GE2E plan for (N, P, D, row0, rows): buffers and the GEMM descriptors.  A rebuild
-// synchronises `s` (buffers in use are freed).
+// The handle's GE2E plan for (N, P, D, row0, rows).  A rebuild synchronises `s` (buffers in use are freed).
 static int ge2e_plan(dsk_handle h, int N, int P, int D, int row0, int rows, cudaStream_t s, Ge2ePlan** out) {
   Ge2ePlan& G = h->ge2e;
   *out = &G;
-  if (G.buf && G.N == N && G.P == P && G.D == D && G.row0 == row0 && G.rows == rows) return DSK_OK;
-  CUDA_TRY(cudaStreamSynchronize(s));
-  if (G.buf) CUDA_TRY(cudaFree(G.buf));
-  G = Ge2ePlan();
-  const int Np = (N + 127) / 128 * 128, Rp = (rows + 127) / 128 * 128, Cp = (P + 127) / 128 * 128;
-  const int sc = (Cp + dsk::kAamSlice - 1) / dsk::kAamSlice, sn = (Np + dsk::kAamSlice - 1) / dsk::kAamSlice;
-  const size_t d3 = 3ull * D, pd = static_cast<size_t>(P) * D * 4;
-  const size_t whole = row0 == 0 && rows == N ? 1 : 0;
-  std::vector<std::pair<void**, size_t>> parts = {
-      {reinterpret_cast<void**>(&G.row_loss), whole * N * 4}, {reinterpret_cast<void**>(&G.tdc), whole * N * 4},
-      {reinterpret_cast<void**>(&G.part), whole * 2 * N * 8},
-      {reinterpret_cast<void**>(&G.cent), pd},                {reinterpret_cast<void**>(&G.nr64), N * 8ull},
-      {reinterpret_cast<void**>(&G.nrm_e), N * 4ull},         {reinterpret_cast<void**>(&G.nrm_c), P * 4ull},
-      {reinterpret_cast<void**>(&G.ea), Rp * d3 * 2},         {reinterpret_cast<void**>(&G.cb), Cp * d3 * 2},
-      {reinterpret_cast<void**>(&G.et), Np * d3 * 2},         {reinterpret_cast<void**>(&G.ct), Cp * d3 * 2},
-      {reinterpret_cast<void**>(&G.da), 3ull * Rp * Cp * 2},  {reinterpret_cast<void**>(&G.dt), 3ull * Np * Cp * 2},
-      {reinterpret_cast<void**>(&G.gcos), 1ull * Rp * Cp * 4}, {reinterpret_cast<void**>(&G.dcos), 1ull * Np * Cp * 4},
-      {reinterpret_cast<void**>(&G.rinv), Rp * 4ull},         {reinterpret_cast<void**>(&G.cinv), Cp * 4ull},
-      {reinterpret_cast<void**>(&G.ge), 1ull * sc * Rp * D * 4}, {reinterpret_cast<void**>(&G.gc), 1ull * sn * Cp * D * 4},
-      {reinterpret_cast<void**>(&G.gcent), pd},               {reinterpret_cast<void**>(&G.own), 1ull * Rp * D * 4},
-      {reinterpret_cast<void**>(&G.xg), 1ull * N * D * 4},    {reinterpret_cast<void**>(&G.ones), Rp * 4ull}};
-  size_t off = 0;
-  for (auto& p : parts) off += (p.second + 255) / 256 * 256;
-  CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&G.buf), off));
-  // zero once: the rows [rows, Rp) of the dcos image, and (written by dsk_ge2e_bwd's path) the workspace rows [N, Np),
-  // are never written again
-  CUDA_TRY(cudaMemsetAsync(G.buf, 0, off, s));
-  off = 0;
-  for (auto& p : parts) {
-    *p.first = G.buf + off;
-    off += (p.second + 255) / 256 * 256;
-  }
-  const std::vector<float> ones(Rp, 1.f);
-  CUDA_TRY(cudaMemcpyAsync(G.ones, ones.data(), Rp * 4ull, cudaMemcpyHostToDevice, s));
-  CUDA_TRY(cudaStreamSynchronize(s));
-  // cos = E^ C^T for the range (K = 3D); gE^ = dcos C^ for the range (K = 3Cp) and gC^ = dcos^T E^ over all N rows
-  // (K = 3Np), one GEMM per K slice into the slice's own output (the AAM op's deterministic split K)
-  int rc = aam_build_gemm(h, &G.fwd, G.ea, Rp, G.cb, Cp, 3 * D, G.gcos);
-  const size_t ks = dsk::kAamSlice;
-  for (int k = 0; k < sc && !rc; ++k) {
-    const int w = Cp - k * dsk::kAamSlice < dsk::kAamSlice ? Cp - k * dsk::kAamSlice : dsk::kAamSlice;
-    rc = aam_build_gemm(h, &G.ge_gemm, G.da + k * ks * 3 * Rp, Rp, G.ct + k * ks * 3 * D, D, 3 * w,
-                        G.ge + static_cast<size_t>(k) * Rp * D);
-  }
-  for (int k = 0; k < sn && !rc; ++k) {
-    const int w = Np - k * dsk::kAamSlice < dsk::kAamSlice ? Np - k * dsk::kAamSlice : dsk::kAamSlice;
-    rc = aam_build_gemm(h, &G.gc_gemm, G.dt + k * ks * 3 * Cp, Cp, G.et + k * ks * 3 * D, D, 3 * w,
-                        G.gc + static_cast<size_t>(k) * Cp * D);
-  }
-  if (rc) {
-    cudaFree(G.buf);
-    G = Ge2ePlan();
+  return plan_acquire(G, {N, P, D, row0, rows}, s, [&]() -> int {
+    const int Np = (N + 127) / 128 * 128, Rp = (rows + 127) / 128 * 128, Cp = (P + 127) / 128 * 128;
+    G.N = N;
+    G.P = P;
+    G.D = D;
+    G.Np = Np;
+    G.Rp = Rp;
+    G.Cp = Cp;
+    G.sc = (Cp + dsk::kAamSlice - 1) / dsk::kAamSlice;
+    G.sn = (Np + dsk::kAamSlice - 1) / dsk::kAamSlice;
+    const size_t d3 = 3ull * D, pd = static_cast<size_t>(P) * D * 4;
+    const size_t whole = row0 == 0 && rows == N ? 1 : 0;
+    // the arena's zeros: the rows [rows, Rp) of the dcos image, and (written by dsk_ge2e_bwd's path) the workspace rows
+    // [N, Np), are never written again
+    int rc = arena_alloc(&G.buf, {{&G.row_loss, whole * N * 4},       {&G.tdc, whole * N * 4},
+                                  {&G.part, whole * 2 * N * 8},
+                                  {&G.cent, pd},                      {&G.nr64, N * 8ull},
+                                  {&G.nrm_e, N * 4ull},               {&G.nrm_c, P * 4ull},
+                                  {&G.ea, Rp * d3 * 2},               {&G.cb, Cp * d3 * 2},
+                                  {&G.et, Np * d3 * 2},               {&G.ct, Cp * d3 * 2},
+                                  {&G.da, 3ull * Rp * Cp * 2},        {&G.dt, 3ull * Np * Cp * 2},
+                                  {&G.gcos, 1ull * Rp * Cp * 4},      {&G.dcos, 1ull * Np * Cp * 4},
+                                  {&G.rinv, Rp * 4ull},               {&G.cinv, Cp * 4ull},
+                                  {&G.ge, 1ull * G.sc * Rp * D * 4},  {&G.gc, 1ull * G.sn * Cp * D * 4},
+                                  {&G.gcent, pd},                     {&G.own, 1ull * Rp * D * 4},
+                                  {&G.xg, 1ull * N * D * 4},          {&G.ones, Rp * 4ull}}, s);
+    if (rc) return rc;
+    const std::vector<float> ones(Rp, 1.f);
+    CUDA_TRY(cudaMemcpyAsync(G.ones, ones.data(), Rp * 4ull, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    // cos = E^ C^T for the range (K = 3D); gE^ = dcos C^ for the range (K = 3Cp) and gC^ = dcos^T E^ over all N rows
+    // (K = 3Np)
+    rc = build_gemm(h, &G.fwd, G.ea, Rp, G.cb, Cp, 3 * D, G.gcos, true);
+    if (!rc) rc = build_sliced_gemm(h, &G.ge_gemm, G.da, Rp, G.ct, D, Cp, G.ge);
+    if (!rc) rc = build_sliced_gemm(h, &G.gc_gemm, G.dt, Cp, G.et, D, Np, G.gc);
     return rc;
-  }
-  G.N = N;
-  G.P = P;
-  G.D = D;
-  G.row0 = row0;
-  G.rows = rows;
-  G.Np = Np;
-  G.Rp = Rp;
-  G.Cp = Cp;
-  G.sc = sc;
-  G.sn = sn;
-  return DSK_OK;
+  });
 }
 
 // The argument checks of the GE2E entry points, before any launch.  An op without a D, V or method passes 64, 1 and
@@ -2934,9 +2933,8 @@ static int ge2e_centroids(const Ge2ePlan& G, const float* E, const int64_t* orde
   KERNEL_CHECK();
   dsk::ge2e_norm64_kernel<<<(G.N + 7) / 8, 256, 0, s>>>(E, G.N, G.D, G.nr64);
   KERNEL_CHECK();
-  dsk::aam_norm_kernel<<<(G.P + 7) / 8, 256, 0, s>>>(G.cent, G.P, G.D, G.nrm_c);
-  KERNEL_CHECK();
-  return DSK_OK;
+  const CosRows c{G.cent, G.P, G.Cp, G.nrm_c, true, nullptr, nullptr};
+  return cos_prep(G.D, nullptr, &c, s);
 }
 
 // dsk_ge2e_rows after its checks
@@ -2946,15 +2944,11 @@ static int ge2e_rows_run(dsk_handle h, const float* E, int N, int D, const int64
   Ge2ePlan* G = nullptr;
   int rc = ge2e_plan(h, N, P, D, row0, rows, s, &G);
   if (rc || (rc = ge2e_centroids(*G, E, order, offsets, s))) return rc;
-  const float* Er = E + static_cast<size_t>(row0) * D;
-  dsk::aam_norm_kernel<<<(rows + 7) / 8, 256, 0, s>>>(Er, rows, D, G->nrm_e + row0);
-  KERNEL_CHECK();
-  dsk::aam_split_kernel<<<dim3(D / 64, G->Rp / 32), 256, 0, s>>>(Er, G->nrm_e + row0, rows, G->Rp, D, 1, G->ea, nullptr);
-  KERNEL_CHECK();
-  dsk::aam_split_kernel<<<dim3(D / 64, G->Cp / 32), 256, 0, s>>>(G->cent, G->nrm_c, P, G->Cp, D, 0, G->cb, nullptr);
-  KERNEL_CHECK();
+  const CosRows e{E + static_cast<size_t>(row0) * D, rows, G->Rp, G->nrm_e + row0, true, G->ea, nullptr};
+  const CosRows c{G->cent, P, G->Cp, G->nrm_c, false, G->cb, nullptr};
+  if ((rc = cos_prep(D, &e, &c, s))) return rc;
   for (const ConvLaunch& L : G->fwd)
-    if ((rc = launch_gemm_f16(L, s))) return rc;
+    if ((rc = launch_conv(L, s))) return rc;
   dsk::ge2e_rows_kernel<<<rows, 256, 0, s>>>(G->gcos, G->Cp, E, D, G->nr64, order, offsets, col, P, w, b, method, row0,
                                              cos, rec, row_loss);
   KERNEL_CHECK();
@@ -2987,12 +2981,9 @@ static int ge2e_bwd_rows_run(dsk_handle h, const float* E, int N, int D, const i
   int rc = ge2e_plan(h, N, P, D, row0, rows, s, &G);
   if (rc || (rc = ge2e_centroids(*G, E, order, offsets, s))) return rc;
   const int Np = G->Np, Rp = G->Rp, Cp = G->Cp;
-  dsk::aam_norm_kernel<<<(N + 7) / 8, 256, 0, s>>>(E, N, D, G->nrm_e);
-  KERNEL_CHECK();
-  dsk::aam_split_kernel<<<dim3(D / 64, Np / 32), 256, 0, s>>>(E, G->nrm_e, N, Np, D, 1, nullptr, G->et);
-  KERNEL_CHECK();
-  dsk::aam_split_kernel<<<dim3(D / 64, Cp / 32), 256, 0, s>>>(G->cent, G->nrm_c, P, Cp, D, 0, nullptr, G->ct);
-  KERNEL_CHECK();
+  const CosRows e{E, N, Np, G->nrm_e, true, nullptr, G->et};
+  const CosRows c{G->cent, P, Cp, G->nrm_c, false, nullptr, G->ct};
+  if ((rc = cos_prep(D, &e, &c, s))) return rc;
   if (dcos) {
     dsk::ge2e_dcos_img_kernel<<<Np, 256, 0, s>>>(dcos, N, P, Cp, row0, rows, Rp, G->dcos, G->da, G->rinv);
     KERNEL_CHECK();
@@ -3000,9 +2991,9 @@ static int ge2e_bwd_rows_run(dsk_handle h, const float* E, int N, int D, const i
   dsk::aam_dcos_t_kernel<<<Cp / 32, 256, 0, s>>>(G->dcos, Np, Cp, G->dt, G->cinv);
   KERNEL_CHECK();
   for (const ConvLaunch& L : G->ge_gemm)  // dcos C^ for the range (target column zeroed)
-    if ((rc = launch_gemm_f16(L, s))) return rc;
+    if ((rc = launch_conv(L, s))) return rc;
   for (const ConvLaunch& L : G->gc_gemm)  // dcos^T E^ over all N rows: the gradient w.r.t. the normalised centroids
-    if ((rc = launch_gemm_f16(L, s))) return rc;
+    if ((rc = launch_conv(L, s))) return rc;
   dsk::aam_normalize_bwd_kernel<<<(P + 7) / 8, 256, 0, s>>>(G->cent, G->nrm_c, G->gc, G->sn, static_cast<long>(Cp) * D,
                                                             G->cinv, P, D, G->gcent);
   KERNEL_CHECK();
@@ -3101,39 +3092,20 @@ static int score_chunk_rows(int M, int Np) {
   return static_cast<int>(m < c ? m : c);
 }
 
-// (Re)build the scoring plan in slot P of h (h->score or h->search) for (Nc, D, chunk).  A rebuild synchronises `s`
-// (buffers in use are freed).
+// The scoring plan in slot P of h (h->score or h->search) for (Nc, D, chunk).  A rebuild synchronises `s` (buffers in
+// use are freed).
 static int score_plan(dsk_handle h, ScorePlan& P, int M, int Nc, int D, cudaStream_t s, ScorePlan** out) {
   *out = &P;
   const int Np = (Nc + 127) / 128 * 128, chunk = score_chunk_rows(M, Np);
-  if (P.buf && P.Nc == Nc && P.D == D && P.chunk == chunk) return DSK_OK;
-  CUDA_TRY(cudaStreamSynchronize(s));
-  if (P.buf) CUDA_TRY(cudaFree(P.buf));
-  P = ScorePlan();
-  const size_t d3 = 3ull * D;
-  std::vector<std::pair<void**, size_t>> parts = {
-      {reinterpret_cast<void**>(&P.ea), chunk * d3 * 2}, {reinterpret_cast<void**>(&P.cb), Np * d3 * 2},
-      {reinterpret_cast<void**>(&P.nrm_e), chunk * 4ull}, {reinterpret_cast<void**>(&P.nrm_c), Np * 4ull},
-      {reinterpret_cast<void**>(&P.cos), 1ull * chunk * Np * 4}};
-  size_t off = 0;
-  for (auto& p : parts) off += (p.second + 255) / 256 * 256;
-  CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&P.buf), off));
-  off = 0;
-  for (auto& p : parts) {
-    *p.first = P.buf + off;
-    off += (p.second + 255) / 256 * 256;
-  }
-  const int rc = aam_build_gemm(h, &P.gemm, P.ea, chunk, P.cb, Np, 3 * D, P.cos);  // cos = E^ C^T, K = 3D
-  if (rc) {
-    cudaFree(P.buf);
-    P = ScorePlan();
-    return rc;
-  }
-  P.Nc = Nc;
-  P.D = D;
-  P.chunk = chunk;
-  P.Np = Np;
-  return DSK_OK;
+  return plan_acquire(P, {Nc, D, chunk}, s, [&]() -> int {
+    P.D = D;
+    P.chunk = chunk;
+    P.Np = Np;
+    const size_t d3 = 3ull * D;
+    const int rc = arena_alloc(&P.buf, {{&P.ea, chunk * d3 * 2}, {&P.cb, Np * d3 * 2}, {&P.nrm_e, chunk * 4ull},
+                                        {&P.nrm_c, Np * 4ull}, {&P.cos, 1ull * chunk * Np * 4}}, s);
+    return rc ? rc : build_gemm(h, &P.gemm, P.ea, chunk, P.cb, Np, 3 * D, P.cos, true);  // cos = E^ C^T, K = 3D
+  });
 }
 
 static int score_check(dsk_handle h, bool ptrs_ok, int M, int Nc, int D, int k, const char* what) {
@@ -3143,24 +3115,19 @@ static int score_check(dsk_handle h, bool ptrs_ok, int M, int Nc, int D, int k, 
   return check_handle(h);
 }
 
-// The norms and B-side operand image of the cohort's rows B (cols <= P.Nc of them; rows [cols, Np) are zero), rebuilt
+// The norms and B-side operand image of the cohort's rows B (cols <= the plan's Nc of them; rows [cols, Np) are zero), rebuilt
 // on every call
 static int score_prep_cohort(const ScorePlan& P, const float* B, int cols, cudaStream_t s) {
-  dsk::aam_norm_kernel<<<(cols + 7) / 8, 256, 0, s>>>(B, cols, P.D, P.nrm_c);
-  KERNEL_CHECK();
-  dsk::aam_split_kernel<<<dim3(P.D / 64, P.Np / 32), 256, 0, s>>>(B, P.nrm_c, cols, P.Np, P.D, 0, P.cb, nullptr);
-  KERNEL_CHECK();
-  return DSK_OK;
+  const CosRows c{B, cols, P.Np, P.nrm_c, true, P.cb, nullptr};
+  return cos_prep(P.D, nullptr, &c, s);
 }
 
 // P.cos[0, rows) = cosines of rows [0, rows) of E (rows <= chunk) against the cohort; rows [rows, chunk) are zero
 static int score_gemm_chunk(const ScorePlan& P, const float* E, int rows, cudaStream_t s) {
-  dsk::aam_norm_kernel<<<(rows + 7) / 8, 256, 0, s>>>(E, rows, P.D, P.nrm_e);
-  KERNEL_CHECK();
-  dsk::aam_split_kernel<<<dim3(P.D / 64, P.chunk / 32), 256, 0, s>>>(E, P.nrm_e, rows, P.chunk, P.D, 1, P.ea, nullptr);
-  KERNEL_CHECK();
+  const CosRows e{E, rows, P.chunk, P.nrm_e, true, P.ea, nullptr};
+  if (int rc = cos_prep(P.D, &e, nullptr, s)) return rc;
   for (const ConvLaunch& L : P.gemm)
-    if (int rc = launch_gemm_f16(L, s)) return rc;
+    if (int rc = launch_conv(L, s)) return rc;
   return DSK_OK;
 }
 
