@@ -278,7 +278,9 @@ __device__ __forceinline__ float exact_dist_seq(const float* __restrict__ a, con
 // Exactness argument: rounding row e to 16 bit moves it by at most u*||e|| (u = unit roundoff), so for every pair
 //   | a_ij - ||e_i - e_j||^2 | <= 2 d r + r^2 + slack,   r = u (||e_i|| + max_j ||e_j||),  d = ||e_i - e_j||.
 // If the worst kept candidate's a exceeds (k-th exact distance)^2 by more than that bound, no discarded column can
-// beat the k-th result and the refined top-k is the exact answer; otherwise the warp scans the whole row exactly.
+// beat the k-th result and the refined top-k is the exact answer; otherwise the warp scans the whole row exactly.  A row
+// with fewer valid columns than kApCand refines them all.  The bound says nothing once a norm or an approximate distance
+// is not finite (an fp16 entry of magnitude >= 65520 rounds to inf while the fp32 distance is finite): such a row scans.
 // Either way the result is the exact one, whatever the Gram's bits: idx / val (written at local row i) do not depend on
 // the row range the Gram was computed for.  ROWS = false is the whole batch (row0 = 0, rows = N, the arguments are
 // ignored): dsk_allpairs_topk_tc and the whole-batch loss run the instruction stream they ran before the row range
@@ -299,6 +301,10 @@ allpairs_select_refine_kernel(const float* __restrict__ E, const float* __restri
   const float ni = norms[row];
   const int64_t my_label = labels[row];
   const float INF = __int_as_float(0x7f800000);
+  // Valid (other-label) columns of the row, and whether any has a non-finite approximate distance (a 16-bit overflow
+  // of an entry makes a norm inf; such a column is never a candidate, so the row must take the exact scan).
+  int n_valid = 0;
+  bool nonfinite = false;
   // ---- candidates: the kApCand smallest approximate distances, extracted in lexicographic (a, j) order.
   // Rows of up to 1024 columns keep their 32 values per lane in registers; longer rows re-read G (L1/L2 hits).
   constexpr int kRegCols = 32;
@@ -308,9 +314,21 @@ allpairs_select_refine_kernel(const float* __restrict__ E, const float* __restri
 #pragma unroll
     for (int q = 0; q < kRegCols; ++q) {
       const int j = lane + 32 * q;
-      areg[q] = (j < N && labels[j] != my_label) ? (ni + norms[j]) - 2.0f * g[j] : INF;
+      const bool valid = j < N && labels[j] != my_label;
+      const float a = valid ? (ni + norms[j]) - 2.0f * g[j] : INF;
+      n_valid += valid;
+      nonfinite |= valid && !(fabsf(a) < INF);
+      areg[q] = a;
+    }
+  } else {
+    for (int j = lane; j < N; j += 32) {
+      if (labels[j] == my_label) continue;
+      ++n_valid;
+      nonfinite |= !(fabsf((ni + norms[j]) - 2.0f * g[j]) < INF);
     }
   }
+  n_valid = __reduce_add_sync(0xffffffffu, n_valid);
+  nonfinite = __any_sync(0xffffffffu, nonfinite);
   float last_a = -INF;
   int last_j = -1;
   for (int t = 0; t < kApCand; ++t) {
@@ -395,8 +413,11 @@ allpairs_select_refine_kernel(const float* __restrict__ E, const float* __restri
   const float r = u * (sqrtf(ni) + sqrtf(nmax)) * 1.01f;
   const float dmax = sqrtf(fmaxf(worst_a, 0.f)) + r + 1e-3f;
   const float tol = 2.f * dmax * r + r * r + 1e-5f * (ni + nmax) + 1e-4f;
-  const bool all_candidates = cand_j[w][kApCand - 1] == 0x7fffffff;  // fewer valid columns than candidates
-  const bool safe = all_candidates || (worst_a >= (kth * kth - eps) + tol);
+  // the candidates are every valid column, or no discarded one can come closer than the k-th; non-finite norms or
+  // approximate distances void both arguments
+  const bool finite = !nonfinite && fabsf(ni) < INF && fabsf(nmax) < INF;
+  const bool all_candidates = n_valid < kApCand;
+  const bool safe = finite && (all_candidates || worst_a >= (kth * kth - eps) + tol);
   if (!safe) {
     // ---- exact fallback: scan the whole row (rare); same arithmetic as the exact path
     float lv = -1.f;

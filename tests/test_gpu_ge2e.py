@@ -86,13 +86,13 @@ def _target_mask(labels):
     return tgt & valid[:, None], valid
 
 
-def _check_cos(cos, ref, labels):
+def _check_cos(cos, ref, labels, tol=1e-6):
     got = cos.double().cpu()
     tgt, _ = _target_mask(labels)
     d_nt = float((got - ref).abs()[~tgt].max())
     ulp = torch.from_numpy(np.spacing(np.abs(ref[tgt].numpy()).astype(np.float32)).astype(np.float64))
     d_t = (got[tgt] - ref[tgt]).abs()
-    assert d_nt <= 1e-6, d_nt
+    assert d_nt <= tol, d_nt
     assert bool((d_t <= ulp + 1e-12).all()), float((d_t - ulp).max())
     return d_nt, float(d_t.max())
 

@@ -1,6 +1,7 @@
 """Batch-hard triplet loss: one JSON line with
   * microseconds per loss forward + backward at N = 1024, D = 512 (64 speakers x 16 utterances), on the tensor-core Gram
-    path and on the exact CUDA-core path (CUDA events around --iters back-to-back calls);
+    path and on the exact CUDA-core path (CUDA events around --iters back-to-back calls), and per all-pairs top-8 query
+    (dsk_allpairs_topk_tc) on the same batch;
   * utterances per second of batch_hard_step at N = 384 (96 x 4), T = 160, with FusedAdagrad (events around --steps
     steps after --warmup);
   * microseconds for one rank's share of the global-batch op (select_rows + bwd_rows, 384 anchor rows of N = 3072,
@@ -74,6 +75,12 @@ def main():
         torch.cuda.synchronize()
         rec[key] = round(1e3 * time_events(one, args.iters), 2)
     rec["loss_shape"] = {"N": N, "D": D, "speakers": N // K, "utterances_per_speaker": K}
+    Ed = E.detach()
+    top8 = lambda: EN.allpairs_topk(Ed, labels, 8)   # noqa: E731
+    for _ in range(20):
+        top8()
+    torch.cuda.synchronize()
+    rec["allpairs_top8_us_N1024"] = round(1e3 * time_events(top8, args.iters), 2)
 
     from oracle import rescnn_oracle as O  # deterministic parameters only
 
