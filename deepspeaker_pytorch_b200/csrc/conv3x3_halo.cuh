@@ -44,7 +44,8 @@ struct HaloParams {
   int8_t box_ntaps[kHaloMaxBoxes];
   int16_t box_wtap[kHaloMaxBoxes];         // first packed tap index of the box
   int16_t tap_shift[kHaloMaxBoxes][3];     // halo-tile row offset of each tap
-  // output: standard padded layout (TMA store) or parity-planar (direct stores; feeds a stride-2 conv)
+  // output: standard padded layout (TMA store) or parity-planar (3x3 only; staged, then copied out in 128-byte rows;
+  // feeds a stride-2 conv)
   int out_planar;
   uint16_t* out_ptr;                       // planar destination base
   int out_plane_positions;                 // positions per output plane
@@ -505,40 +506,54 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
       }
       // ---------------- epilogue ----------------
       // this thread's rows: slice m, half h -> tile row (cg*kMW + m)*64 + fr + 8h; padded position q0 + row
+      // padded position q0 + row: junk (a pad position) or, for a parity-planar output, its destination (nullptr = junk)
+      auto is_junk = [&](int row, int& R, int& cc, int& img) -> bool {
+        const int q = q0 + row;
+        R = static_cast<int>(__umulhi(static_cast<unsigned>(q), p.pitch_magic));
+        cc = q - R * pitch;
+        img = static_cast<int>(__umulhi(static_cast<unsigned>(R), p.img_magic));
+        return (cc == 0) || (R - img * (p.H + 1) == 0) || (R >= rows_real_end);
+      };
+      // parity-planar destination of a position (only when the consumer is a stride-2 conv): pixel (n, h, w) ->
+      // plane (h&1, w&1), padded position of (n, h>>1, w>>1) on the half-resolution grid
+      auto planar_dst = [&](int row) -> uint16_t* {
+        int R, cc, img;
+        if (is_junk(row, R, cc, img)) return nullptr;
+        const int n = img;  // R = n*(H+1) + h + 1 with h < H  =>  img == n for real rows
+        const int hh = R - 1 - n * (p.H + 1), ww = cc - 1;
+        const int H2 = p.H >> 1, W2 = p.W >> 1;
+        const long q2 = static_cast<long>(n * (H2 + 1) + (hh >> 1) + 1) * (W2 + 1) + (ww >> 1) + 1;
+        const long plane = (hh & 1) * 2 + (ww & 1);
+        return p.out_ptr + (plane * p.out_plane_positions + q2) * p.out_C + c0;
+      };
       bool junk[kMW][2];
-      uint16_t* planar_row[kMW][2];
 #pragma unroll
       for (int m = 0; m < kMW; ++m)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const int row = (cg * kMW + m) * 64 + fr + 8 * h;
-          const int q = q0 + row;
-          const int R = static_cast<int>(__umulhi(static_cast<unsigned>(q), p.pitch_magic));
-          const int cc = q - R * pitch;
-          const int img = static_cast<int>(__umulhi(static_cast<unsigned>(R), p.img_magic));
-          junk[m][h] = (cc == 0) || (R - img * (p.H + 1) == 0) || (R >= rows_real_end);
-          planar_row[m][h] = nullptr;
-          // parity-planar destination of this position (only when the consumer is a stride-2 conv): pixel (n, h, w) ->
-          // plane (h&1, w&1), padded position of (n, h>>1, w>>1) on the half-resolution grid
-          if (p.out_planar && !junk[m][h]) {
-            const int n = img;  // R = n*(H+1) + h + 1 with h < H  =>  img == n for real rows
-            const int hh = R - 1 - n * (p.H + 1), ww = cc - 1;
-            const int H2 = p.H >> 1, W2 = p.W >> 1;
-            const long q2 = static_cast<long>(n * (H2 + 1) + (hh >> 1) + 1) * (W2 + 1) + (ww >> 1) + 1;
-            const long plane = (hh & 1) * 2 + (ww & 1);
-            planar_row[m][h] = p.out_ptr + (plane * p.out_plane_positions + q2) * p.out_C + c0;
-          }
+          int R, cc, img;
+          junk[m][h] = is_junk((cg * kMW + m) * 64 + fr + 8 * h, R, cc, img);
         }
+      // A planar output is staged like the padded one and then copied out row by row: thread etid moves the 16-byte
+      // pieces etid + i * kEpiThreads (row = piece / 8), so each warp writes four whole 128-byte rows.  (Stored straight
+      // from the accumulator fragment, every warp store touched 8 positions with 16 bytes each.)
+      // Only the 3x3 form writes a planar output (a block's last conv feeding the next stage's 5x5 s2 conv; the host
+      // rejects it for the 5x5 form), so the 5x5 instantiations carry none of this code.
+      const bool out_planar = KIND == 1 && p.out_planar;
+      constexpr int kCopyIters = kTM * 8 / kEpiThreads;
+      static_assert(kCopyIters * kEpiThreads == kTM * 8, "the copy-out covers the staging tile");
 #pragma unroll
       for (int j = 0; j < kChunksOut; ++j) {
         uint8_t* stg = smem_stg + buf * kATileBytes;
-        if (!p.out_planar) {
+        if (!out_planar) {
           // staging buffer `buf`: its previous TMA store (stg_bufs chunks ago) has finished reading it
           if (etid == 0) {
             if (p.stg_bufs == 2) tma_store_wait_read<1>();
             else tma_store_wait_read<0>();
           }
           named_bar_sync(1, kEpiThreads);
+        } else if (p.stg_bufs == 1) {
+          named_bar_sync(1, kEpiThreads);  // the previous chunk's copy-out has read the one staging buffer
         }
 #pragma unroll
         for (int m = 0; m < kMW; ++m)
@@ -560,14 +575,26 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
               uint32_t o = pack2<BF16>(f0, f1);
               if (do_clip) o = clip2<BF16>(o, 0u, clip_hi2);  // on the packed pair: same result as an fp32 clamp (0 and 20 are exact)
               if (junk[m][h]) o = 0u;                         // pad positions stay zero
-              if (p.out_planar) {
-                if (planar_row[m][h] != nullptr) *reinterpret_cast<uint32_t*>(planar_row[m][h] + j * 64 + col) = o;
-              } else {
-                *reinterpret_cast<uint32_t*>(stg + sw128_off16(row, col)) = o;
-              }
+              *reinterpret_cast<uint32_t*>(stg + sw128_off16(row, col)) = o;
             }
           }
-        if (!p.out_planar) {
+        if (out_planar) {
+          // with two staging buffers, the barrier after this chunk's writes also orders the copy-out of the chunk before
+          // (same buffer as the next chunk) ahead of the next chunk's writes
+          named_bar_sync(1, kEpiThreads);
+          const uint32_t stg_s = smem_u32(stg);
+#pragma unroll
+          for (int i = 0; i < kCopyIters; ++i) {
+            const int piece = i * kEpiThreads + etid;
+            const int row = piece >> 3, k = piece & 7;
+            uint16_t* dst = planar_dst(row);  // recomputed per chunk: a few integer ops, no registers held across the MMAs
+            if (dst != nullptr) {
+              const uint4 v = lds128(stg_s + row * 128 + (((k ^ row) & 7) << 4));
+              *reinterpret_cast<uint4*>(dst + j * 64 + k * 8) = v;
+            }
+          }
+          if (p.stg_bufs == 2) buf ^= 1;
+        } else {
           fence_proxy_async_smem();
           named_bar_sync(1, kEpiThreads);
           if (etid == 0) {

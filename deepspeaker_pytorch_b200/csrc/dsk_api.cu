@@ -819,6 +819,7 @@ int build_halo(const dsk_handle_s* h, HaloLaunch* L, const void* in, const void*
   if (ksize == 3 && cin != cout) return fail(DSK_ERR_INVALID, "halo conv: the 3x3 form needs cin == cout");
   if (W > 34) return fail(DSK_ERR_INVALID, "halo conv: W must be <= 34 (got %d)", W);
   if (out_planar && ((H & 1) || (W & 1))) return fail(DSK_ERR_INVALID, "halo conv: planar output needs even H, W");
+  if (out_planar && ksize != 3) return fail(DSK_ERR_INVALID, "halo conv: planar output is written by the 3x3 form only");
   const bool bf = h->bf16;
   dsk::HaloParams& p = L->p;
   memset(&p, 0, sizeof(p));
