@@ -21,6 +21,8 @@ NUM_CONV = 12
 DSK_F16, DSK_BF16 = 0, 1
 DSK_EVAL, DSK_TRAIN = 0, 1
 DSK_GE2E_SOFTMAX, DSK_GE2E_CONTRAST = 0, 1
+DSK_LINKAGE_AVERAGE, DSK_LINKAGE_COMPLETE = 0, 1
+DSK_AHC_MAX_N = 32768
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -203,6 +205,8 @@ SIGNATURES = {
     "dsk_topk_indices": (c_int32, [c_void_p, c_int32, c_int32, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
     "dsk_cosine_topk": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_int32] + [c_void_p] * 3),
     "dsk_class_centroids": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),
+    "dsk_ahc": (c_int32, [c_void_p, c_int32, c_int64, c_int32, c_int32, c_double, c_void_p, POINTER(c_int32), c_void_p,
+                          POINTER(c_int32), c_void_p]),
     "dsk_linear_forward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     "dsk_linear_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p,
                                       c_void_p, c_void_p]),

@@ -23,6 +23,7 @@
 #include "conv1_umma.cuh"
 #include "fbank_kernels.cuh"
 #include "augment_kernels.cuh"
+#include "cluster_kernels.cuh"
 #include "head_kernels.cuh"
 #include "loss_kernels.cuh"
 #include "metric_kernels.cuh"
@@ -3360,6 +3361,151 @@ int32_t dsk_threshold_counts(const float* dist, const uint8_t* same, int32_t P, 
   dsk::threshold_counts_kernel<<<blocks, dsk::kSweepThreads, 0, static_cast<cudaStream_t>(stream)>>>(dist, same, P, thresholds,
                                                                                                       nT, tp, fp);
   KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// ---- agglomerative clustering ------------------------------------------------------------------------------------
+// Rounds between two reads of the device-side done flag: a finished run costs at most this many rounds of launches
+// that return at once.
+static constexpr int kAhcRoundsPerBatch = 64;
+
+// The merge records, in round order, into scipy's linkage matrix: rows sorted by (height, round, representative of the
+// lower cluster), of which the first `keep` are written, and the flat labels after those `keep` merges.  The height used
+// for sorting is raised to the sorting height of the merged clusters, so a parent never sorts before a child whose
+// rounded height came out 1 ulp above its own (with exact arithmetic a reducible linkage is monotone and this changes
+// nothing).  The cut at k clusters is taken here, from the sorted tree, and not by stopping the rounds at k clusters: a
+// round may merge a mutual pair far above heights that later rounds merge below it (two isolated points that are each
+// other's nearest), so the rounds reach k clusters with a different partition than the tree's cut.
+static void ahc_assemble(const std::vector<dsk::AhcRecord>& rec, int N, int keep, double* Z, int32_t* labels) {
+  const int m = static_cast<int>(rec.size());
+  std::vector<double> key(m), cl_key(N, -HUGE_VAL);
+  for (int k = 0; k < m; ++k) {
+    const double h = std::max(rec[k].height, std::max(cl_key[rec[k].rep_a], cl_key[rec[k].rep_b]));
+    key[k] = h;
+    cl_key[rec[k].rep_a] = h;  // the merged cluster keeps the lower representative
+  }
+  std::vector<int> order(m);
+  for (int k = 0; k < m; ++k) order[k] = k;
+  std::sort(order.begin(), order.end(), [&](int x, int y) {
+    if (key[x] != key[y]) return key[x] < key[y];
+    if (rec[x].round != rec[y].round) return rec[x].round < rec[y].round;
+    return rec[x].rep_a < rec[y].rep_a;
+  });
+  std::vector<int> cur(N), parent(N);
+  for (int i = 0; i < N; ++i) cur[i] = parent[i] = i;
+  for (int r = 0; r < keep; ++r) {
+    const dsk::AhcRecord& e = rec[order[r]];
+    const int ia = cur[e.rep_a], ib = cur[e.rep_b];
+    Z[4 * r + 0] = std::min(ia, ib);
+    Z[4 * r + 1] = std::max(ia, ib);
+    Z[4 * r + 2] = e.height;
+    Z[4 * r + 3] = e.size;
+    cur[e.rep_a] = N + r;
+    parent[e.rep_b] = e.rep_a;  // representatives only ever point to lower representatives
+  }
+  int next = 0;
+  std::vector<int> lab(N, -1);
+  for (int i = 0; i < N; ++i) {
+    int r = i;
+    while (parent[r] != r) r = parent[r];
+    for (int x = i; parent[x] != x;) {  // path compression
+      const int nx = parent[x];
+      parent[x] = r;
+      x = nx;
+    }
+    if (lab[r] < 0) lab[r] = next++;
+    labels[i] = lab[r];
+  }
+}
+
+int32_t dsk_ahc(const float* S, int32_t N, int64_t ld, int32_t linkage, int32_t stop_k, double stop_height, double* Z,
+                int32_t* n_merges, int32_t* labels, int32_t* n_rounds, void* stream) {
+  if (!S || !Z || !n_merges || !labels || N < 2 || N > DSK_AHC_MAX_N || ld < N || stop_k < 1 || stop_k > N ||
+      (linkage != DSK_LINKAGE_AVERAGE && linkage != DSK_LINKAGE_COMPLETE) || std::isnan(stop_height))
+    return fail(DSK_ERR_INVALID, "dsk_ahc: bad arguments (need non-null S, Z, n_merges and labels, 2 <= N <= %d, "
+                "ld >= N, 1 <= stop_k <= N, linkage %d or %d, stop_height not NaN; got N %d, ld %lld, linkage %d, "
+                "stop_k %d)", DSK_AHC_MAX_N, DSK_LINKAGE_AVERAGE, DSK_LINKAGE_COMPLETE, N, static_cast<long long>(ld),
+                linkage, stop_k);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int dev = 0, sms = 0;
+  CUDA_TRY(cudaGetDevice(&dev));
+  CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const size_t n2 = static_cast<size_t>(N) * N, h = (N + 1) / 2, q2 = h * h;
+  // workspace: the matrix, the quarter-size repack target (the first repack leaves fewer than N / 2 slots, and every
+  // later one fewer than half of the previous), then the state, the per-slot arrays and the records
+  const size_t small = sizeof(dsk::AhcState) + 8 * static_cast<size_t>(N) * sizeof(double) +
+                       static_cast<size_t>(N) * sizeof(dsk::AhcRecord);
+  uint8_t* ws = nullptr;
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&ws), (n2 + q2) * sizeof(double) + small, s));
+  double* mat0 = reinterpret_cast<double*>(ws);
+  double* mat1 = mat0 + n2;
+  uint8_t* p = reinterpret_cast<uint8_t*>(mat1 + q2);
+  dsk::AhcState* st = reinterpret_cast<dsk::AhcState*>(p);
+  p += (sizeof(dsk::AhcState) + 15) / 16 * 16;
+  dsk::AhcBufs b;
+  b.nnd = reinterpret_cast<double*>(p);
+  p += N * sizeof(double);
+  b.rec = reinterpret_cast<dsk::AhcRecord*>(p);
+  p += N * sizeof(dsk::AhcRecord);
+  int32_t* ip = reinterpret_cast<int32_t*>(p);
+  int32_t** arrays[] = {&b.rep, &b.size, &b.active, &b.nn, &b.pair_of, &b.pa, &b.pb, &b.pna, &b.pnb, &b.map, &b.tmp};
+  for (int32_t** a : arrays) {
+    *a = ip;
+    ip += N;
+  }
+  ip += N;  // tmp holds 2 N
+  int rc = DSK_OK;
+  dsk::AhcState hs{};
+  std::vector<dsk::AhcRecord> rec;
+  do {
+    dsk::ahc_init_state_kernel<<<(N + 255) / 256, 256, 0, s>>>(st, b, N, mat0, mat1, linkage, stop_height);
+    const int tiles = (N + dsk::kAhcTile - 1) / dsk::kAhcTile;
+    dsk::ahc_init_matrix_kernel<<<dim3(tiles, tiles), dim3(dsk::kAhcTile, 8), 0, s>>>(S, ld, N, mat0, st);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&hs, st, sizeof(hs), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) {
+      rc = fail(DSK_ERR_CUDA, "dsk_ahc: %s", cudaGetErrorString(e));
+      break;
+    }
+    if (hs.bad) {
+      rc = fail(DSK_ERR_INVALID, "dsk_ahc: bad arguments (a non-finite similarity in the upper triangle of S)");
+      break;
+    }
+    const int grid = 8 * sms;
+    while (!hs.done) {
+      for (int r = 0; r < kAhcRoundsPerBatch; ++r) {
+        dsk::ahc_nn_kernel<<<grid, dsk::kAhcThreads, 0, s>>>(st, b);
+        dsk::ahc_decide_kernel<<<1, dsk::kAhcDecideThreads, 0, s>>>(st, b);
+        dsk::ahc_update_kernel<<<grid, dsk::kAhcThreads, 0, s>>>(st, b);
+        dsk::ahc_compact_kernel<<<grid, dsk::kAhcThreads, 0, s>>>(st, b);
+        dsk::ahc_finalize_kernel<<<1, dsk::kAhcDecideThreads, 0, s>>>(st, b);
+      }
+      e = cudaGetLastError();
+      if (e == cudaSuccess) e = cudaMemcpyAsync(&hs, st, sizeof(hs), cudaMemcpyDeviceToHost, s);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+      if (e != cudaSuccess) {
+        rc = fail(DSK_ERR_CUDA, "dsk_ahc: %s", cudaGetErrorString(e));
+        break;
+      }
+      if (hs.round > N) {  // every round that is not the last merges at least one pair
+        rc = fail(DSK_ERR_STATE, "dsk_ahc: %d rounds for %d points", hs.round, N);
+        break;
+      }
+    }
+    if (rc) break;
+    rec.resize(hs.n_rec);
+    if (hs.n_rec) e = cudaMemcpyAsync(rec.data(), b.rec, hs.n_rec * sizeof(dsk::AhcRecord), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) rc = fail(DSK_ERR_CUDA, "dsk_ahc: %s", cudaGetErrorString(e));
+  } while (false);
+  const cudaError_t fe = cudaFreeAsync(ws, s);
+  if (rc) return rc;
+  if (fe != cudaSuccess) return fail(DSK_ERR_CUDA, "dsk_ahc: cudaFreeAsync failed: %s", cudaGetErrorString(fe));
+  const int keep = std::min(hs.n_rec, N - stop_k);
+  ahc_assemble(rec, N, keep, Z, labels);
+  *n_merges = keep;
+  if (n_rounds) *n_rounds = hs.round;
   return DSK_OK;
 }
 

@@ -1,0 +1,125 @@
+"""Speaker diarization: who spoke when in one recording.
+
+``diarize`` embeds the sliding windows of every recording with the eval forward (one batched pass over all of them,
+``frontend.window_embeddings``), builds each recording's window-by-window cosine matrix on the tensor cores
+(``engine.cosine_matrix``) and clusters it by agglomerative clustering on the device (``engine.ahc``, average linkage
+by default), cut at a known number of speakers or at a distance threshold.  Each 10 ms frame then takes the speaker of
+the covering window whose centre is nearest, and runs of equal frame labels become segments.  ``to_rttm`` writes them
+in the RTTM format scoring tools read.
+
+Overlapped speech, voice activity detection and re-segmentation are not part of this module: every frame gets exactly
+one speaker.
+"""
+from __future__ import annotations
+
+from typing import NamedTuple
+
+import numpy as np
+
+from . import _lib as L
+from . import engine
+from . import frontend
+
+FRAME_SHIFT_S = 0.01   # the fbank's 10 ms frame shift, at every sample rate
+MAX_WINDOWS = L.DSK_AHC_MAX_N
+
+
+class Recording(NamedTuple):
+    """The diarization of one recording: ``segments`` [(start_s, end_s, speaker)], ``frame_labels`` (n_frames,)
+    int32, ``window_labels`` (W,) int32 and ``Z`` the linkage matrix of the windows (scipy's format; the first rows of
+    the full tree)."""
+    segments: list
+    frame_labels: np.ndarray
+    window_labels: np.ndarray
+    Z: np.ndarray
+
+
+def frame_labels(win_start, win_labels, n_frames: int, T: int) -> np.ndarray:
+    """Host: (n_frames,) int32, frame f taking the label of the covering window whose centre is nearest to the frame's
+    centre, ties to the earlier window.  Windows start at ``win_start`` (ascending, as ``frontend.sliding_windows``
+    gives them, so every frame is covered) and span T frames; a recording shorter than T has one window.  With equal
+    window lengths the nearest centre overall covers the frame, so a search over the centres suffices."""
+    s = np.asarray(win_start, np.int64).reshape(-1)
+    lab = np.asarray(win_labels).reshape(-1)
+    if s.size == 0 or s.size != lab.size:
+        raise ValueError(f"frame_labels: {s.size} window starts for {lab.size} labels")
+    c2 = 2 * s + int(T)                                # doubled centres, in half frames
+    q = 2 * np.arange(int(n_frames), dtype=np.int64) + 1
+    hi = np.clip(np.searchsorted(c2, q, side="left"), 0, s.size - 1)
+    lo = np.clip(hi - 1, 0, s.size - 1)
+    w = np.where(np.abs(q - c2[lo]) <= np.abs(c2[hi] - q), lo, hi)
+    return lab[w].astype(np.int32)
+
+
+def segments(labels, frame_shift: float = FRAME_SHIFT_S) -> list:
+    """Host: runs of equal frame labels -> [(start_s, end_s, speaker)]; frame f covers [f, f + 1) * frame_shift."""
+    lab = np.asarray(labels).reshape(-1)
+    if lab.size == 0:
+        return []
+    cut = np.flatnonzero(lab[1:] != lab[:-1]) + 1
+    starts = np.concatenate(([0], cut))
+    ends = np.concatenate((cut, [lab.size]))
+    return [(float(a * frame_shift), float(b * frame_shift), int(lab[a])) for a, b in zip(starts, ends)]
+
+
+def to_rttm(segs, recording_id: str) -> str:
+    """RTTM ``SPEAKER`` lines (one per segment, newline-terminated): onset and duration in seconds to the millisecond,
+    speaker ``spk<label>``."""
+    rid = str(recording_id)
+    if not rid or any(ch.isspace() for ch in rid):
+        raise ValueError(f"to_rttm: the recording id must be non-empty without white space, got {rid!r}")
+    return "".join(f"SPEAKER {rid} 1 {a:.3f} {b - a:.3f} <NA> <NA> spk{k} <NA> <NA>\n" for a, b, k in segs)
+
+
+def _per_recording(x, n, what):
+    if isinstance(x, (list, tuple, np.ndarray)):
+        if len(x) != n:
+            raise ValueError(f"diarize: {len(x)} values of {what} for {n} recordings")
+        return list(x)
+    return [x] * n
+
+
+def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40, num_speakers=None, threshold=None,
+            linkage: str = "average", batch: int = 256) -> list:
+    """Diarize the recordings ``utt`` (indices into ``bank``) -> [Recording] in the order of ``utt``.  Give exactly
+    one of ``num_speakers`` (an int, or one per recording; a recording with fewer windows gets one speaker per window)
+    and ``threshold`` (a cosine distance 1 - cos: windows merge while the linkage distance is <= threshold), else
+    ValueError.  Windows of T frames every ``hop`` frames; a recording needing more than ``MAX_WINDOWS`` windows is a
+    ValueError naming the smallest hop that fits.  RuntimeError on a model in train mode."""
+    if (num_speakers is None) == (threshold is None):
+        raise ValueError("diarize: give exactly one of num_speakers and threshold")
+    if linkage not in engine.LINKAGES:
+        raise ValueError(f"diarize: linkage must be one of {sorted(engine.LINKAGES)}, got {linkage!r}")
+    if model.training:
+        raise RuntimeError("diarize needs model.eval() (train-mode BatchNorm would use batch statistics)")
+    u = np.asarray(utt, np.int64).reshape(-1)
+    if u.size == 0:
+        raise ValueError("diarize: no recordings")
+    ks = _per_recording(num_speakers, u.size, "num_speakers")
+    if num_speakers is not None and any(int(k) < 1 for k in ks):
+        raise ValueError(f"diarize: num_speakers must be >= 1, got {num_speakers}")
+    _, _, win_off = bank.windows(u, T, hop)
+    counts = np.diff(win_off.numpy())
+    if counts.max() > MAX_WINDOWS:
+        n = int(bank.lengths[u[int(counts.argmax())]])
+        need = -(-max(n - int(T), 1) // (MAX_WINDOWS - 2))
+        raise ValueError(f"diarize: a recording of {n} frames has {int(counts.max())} windows at hop {hop}, more than "
+                         f"{MAX_WINDOWS}; use hop >= {need}")
+    emb, _, win_start, win_off = frontend.window_embeddings(model, bank, u, T, hop, batch, "diarize")
+    out = []
+    for r in range(u.size):
+        a, b = int(win_off[r]), int(win_off[r + 1])
+        W = b - a
+        if W == 1:
+            wl, Z = np.zeros(1, np.int32), np.zeros((0, 4))
+        else:
+            E = emb[a:b]
+            S = engine.cosine_matrix(E, E)
+            if threshold is not None:
+                Z, lab = engine.ahc(S, linkage, threshold=threshold)
+            else:
+                Z, lab = engine.ahc(S, linkage, num_clusters=min(int(ks[r]), W))
+            wl = lab.cpu().numpy()
+        fl = frame_labels(win_start[a:b].numpy(), wl, int(bank.lengths[u[r]]), T)
+        out.append(Recording(segments(fl), fl, wl, Z))
+    return out

@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib as L
@@ -731,3 +732,38 @@ def class_centroids(X, order, offsets):
         L.check(L.load().dsk_class_centroids(X.data_ptr(), U, D, order.data_ptr(), offsets.data_ptr(), S,
                                              out.data_ptr(), L.cur_stream()), "dsk_class_centroids")
     return out
+
+
+# ---------------------------------------------------------------------------------------------------
+# diarization: agglomerative clustering
+# ---------------------------------------------------------------------------------------------------
+LINKAGES = {"average": L.DSK_LINKAGE_AVERAGE, "complete": L.DSK_LINKAGE_COMPLETE}
+
+
+def ahc(S, linkage="average", num_clusters=None, threshold=None, return_rounds=False):
+    """dsk_ahc: agglomerative clustering of N items from their similarities S (N, N) fp32 on the device (higher =
+    closer, e.g. ``cosine_matrix(E, E)``; only the strict upper triangle is read, the row stride is kept), on the
+    distance 1 - S in fp64.  -> (Z np.float64 (m, 4) in scipy's linkage format, labels torch.int32 (N,) on S's device,
+    the flat clusters numbered by their smallest member).  ``num_clusters``: stop at that many clusters (exact: the cut
+    of the full tree).  ``threshold``: merge only at heights <= threshold (a distance).  Neither: the full tree, m =
+    N - 1.  ``return_rounds`` adds the number of merge rounds.  RuntimeError on a non-finite similarity."""
+    if linkage not in LINKAGES:
+        raise ValueError(f"ahc: linkage must be one of {sorted(LINKAGES)}, got {linkage!r}")
+    if num_clusters is not None and threshold is not None:
+        raise ValueError("ahc: give num_clusters or threshold, not both")
+    if not S.is_cuda:
+        raise RuntimeError("ahc needs a CUDA tensor; there is no CPU fallback")
+    if S.dim() != 2 or S.shape[0] != S.shape[1] or S.dtype != torch.float32 or S.stride(1) != 1:
+        raise RuntimeError(f"ahc: expected a row-major fp32 (N, N) tensor, got {S.dtype} {tuple(S.shape)}")
+    N = S.shape[0]
+    stop_k = 1 if num_clusters is None else int(num_clusters)
+    stop_h = float("inf") if threshold is None else float(threshold)
+    Z = np.empty((max(N - 1, 1), 4), np.float64)
+    labels = np.empty(max(N, 1), np.int32)
+    m, rounds = ctypes.c_int32(0), ctypes.c_int32(0)
+    with torch.cuda.device(S.device):
+        L.check(L.load().dsk_ahc(S.data_ptr(), N, S.stride(0), LINKAGES[linkage], stop_k, stop_h,
+                                 Z.ctypes.data_as(ctypes.c_void_p), ctypes.byref(m),
+                                 labels.ctypes.data_as(ctypes.c_void_p), ctypes.byref(rounds), L.cur_stream()), "dsk_ahc")
+    out = (Z[:m.value].copy(), torch.from_numpy(labels).to(S.device))
+    return out + (rounds.value,) if return_rounds else out

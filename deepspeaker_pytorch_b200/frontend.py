@@ -580,23 +580,21 @@ def _masks(m, B, what, dev):
     return _to_dev(m, torch.int32, dev), int(m.shape[1])
 
 
-def embed_utterances(model, bank: FeatureBank, utt, T: int = 160, hop: int = 80, batch: int = 256) -> torch.Tensor:
-    """(len(utt), D) fp32: one embedding per utterance ``utt[i]`` of ``bank``, the mean of the unit embeddings of its
-    sliding windows (``bank.windows(utt, T, hop)``), summed in fp64 in window order by ``engine.class_centroids``.
-    The rows are what ``identification.enroll`` gives for those windows: for cosine scoring (``verification``,
-    ``identification``), not of norm 10.  The eval forward runs over the windows in batches of ``min(batch, windows)``
-    rows, the last one padded, so every batch has the same shape and one captured forward serves them all.  RuntimeError
-    on a model in train mode."""
-    from . import engine
-
+def window_embeddings(model, bank: FeatureBank, utt, T: int = 160, hop: int = 80, batch: int = 256,
+                      what: str = "window_embeddings"):
+    """(emb (W, D) fp32, win_utt, win_start, win_off): the eval-forward embedding of every sliding window
+    ``bank.windows(utt, T, hop)`` of the utterances ``utt`` (windows ``win_off[i]:win_off[i+1]`` are ``utt[i]``'s, host
+    int64).  The forward runs over the windows in batches of ``min(batch, W)`` rows, the last one padded, so every
+    batch has the same shape and one captured forward serves them all: the rows are those of
+    ``model(bank.crops(...))`` over the same windows in the same batches.  RuntimeError on a model in train mode."""
     if model.training:
-        raise RuntimeError("embed_utterances needs model.eval() (train-mode BatchNorm would use batch statistics)")
+        raise RuntimeError(f"{what} needs model.eval() (train-mode BatchNorm would use batch statistics)")
     if batch < 1:
-        raise ValueError(f"embed_utterances: batch must be >= 1, got {batch}")
+        raise ValueError(f"{what}: batch must be >= 1, got {batch}")
     win_utt, win_start, win_off = bank.windows(utt, T, hop)
     W = win_utt.numel()
     if W == 0:
-        raise ValueError("embed_utterances: no utterances")
+        raise ValueError(f"{what}: no utterances")
     Bb = min(int(batch), W)
     nb = (W + Bb - 1) // Bb
     pad = nb * Bb - W                                   # padded rows repeat the last window and are dropped
@@ -609,5 +607,16 @@ def embed_utterances(model, bank: FeatureBank, utt, T: int = 160, hop: int = 80,
             if emb is None:
                 emb = torch.empty(nb * Bb, e.shape[1], device=e.device, dtype=torch.float32)
             emb[i * Bb:(i + 1) * Bb].copy_(e)
-    order = torch.arange(W, dtype=torch.int64)
-    return engine.class_centroids(emb[:W], order, win_off)
+    return emb[:W], win_utt, win_start, win_off
+
+
+def embed_utterances(model, bank: FeatureBank, utt, T: int = 160, hop: int = 80, batch: int = 256) -> torch.Tensor:
+    """(len(utt), D) fp32: one embedding per utterance ``utt[i]`` of ``bank``, the mean of the unit embeddings of its
+    sliding windows (``window_embeddings``), summed in fp64 in window order by ``engine.class_centroids``.
+    The rows are what ``identification.enroll`` gives for those windows: for cosine scoring (``verification``,
+    ``identification``), not of norm 10.  RuntimeError on a model in train mode."""
+    from . import engine
+
+    emb, _, _, win_off = window_embeddings(model, bank, utt, T, hop, batch, "embed_utterances")
+    order = torch.arange(emb.shape[0], dtype=torch.int64)
+    return engine.class_centroids(emb, order, win_off)

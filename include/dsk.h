@@ -500,6 +500,38 @@ int32_t dsk_cosine_topk(dsk_handle h, const float* Q, int32_t M, const float* G,
 int32_t dsk_class_centroids(const float* X, int32_t U, int32_t D, const int64_t* order, const int64_t* offsets,
                             int32_t S, float* out, void* stream);
 
+/* Diarization: agglomerative hierarchical clustering of N items from their similarities (no reference implementation
+ * exists).  S (N x N fp32, device, row stride ld floats) holds similarities, higher meaning closer; only its strict upper
+ * triangle is read (the diagonal and the lower triangle may hold anything).  The distance is d_ij = 1 - (double)S[i][j]
+ * for i < j, rounded once in fp64 (numpy's 1.0 - S.astype(float64)).  A non-finite value in the upper triangle gives
+ * DSK_ERR_INVALID after one validation pass and one flag read.
+ *   Linkage: DSK_LINKAGE_AVERAGE (UPGMA) or DSK_LINKAGE_COMPLETE, on an fp64 working matrix on the device kept exactly
+ *     symmetric.  Merging A u B against C u D (D absent, n_D = 0, when C did not merge in the same round), average is
+ *     (nA nC dAC + nA nD dAD + nB nC dBC + nB nD dBD) / ((nA + nB)(nC + nD)) summed in that order, A and C the lower
+ *     representatives (a cluster's representative is its smallest original index); complete is the max of the same.
+ *   Rounds (RAC, Sumengen et al. 2021): every live cluster finds its nearest live cluster (ties to the smaller
+ *     representative); every mutual pair whose height is <= stop_height merges; the merged rows and columns are
+ *     updated; once the live count falls below half the stored dimension the matrix is repacked into a smaller buffer.
+ *     For these reducible linkages the dendrogram is the sequential algorithm's.  The rounds run until one cluster is
+ *     left or no mutual pair lies at or below stop_height; the cut at stop_k clusters is then taken from the sorted
+ *     tree (its first N - stop_k rows), which is exact.  Stopping the rounds at stop_k clusters would not be: a round
+ *     may merge a mutual pair far above merges that later rounds make.  The host reads a device-side done flag once per
+ *     64 rounds; after it is set the kernels of the batch return at once.
+ *   Outputs (host memory; the call synchronises the stream): Z (n_merges, 4) fp64 row-major in scipy's linkage format
+ *     [id_a, id_b, height, size], id_a < id_b, points 0..N-1 and the cluster made by row r numbered N + r, rows sorted
+ *     by (height, round, representative); with stop_k = 1 and stop_height = +inf the full tree (n_merges = N - 1),
+ *     otherwise the first n_merges = min(N - stop_k, merges at or below stop_height) rows of it.  Z must hold N - 1 rows.  labels (N,) int32: the flat clusters at the
+ *     stop point, numbered from 0 in the order of each cluster's smallest member.  n_rounds (may be NULL): the rounds
+ *     that merged.
+ *   Workspace: N^2 + ceil(N/2)^2 doubles and O(N) more, stream-ordered (cudaMallocAsync / cudaFreeAsync).  Index
+ *   arithmetic is 64-bit.  2 <= N <= DSK_AHC_MAX_N, ld >= N, 1 <= stop_k <= N, a known linkage, stop_height not NaN,
+ *   non-null S, Z, n_merges, labels; else DSK_ERR_INVALID. */
+#define DSK_AHC_MAX_N 32768
+#define DSK_LINKAGE_AVERAGE 0
+#define DSK_LINKAGE_COMPLETE 1
+int32_t dsk_ahc(const float* S, int32_t N, int64_t ld, int32_t linkage, int32_t stop_k, double stop_height, double* Z,
+                int32_t* n_merges, int32_t* labels, int32_t* n_rounds, void* stream);
+
 /* nn.Linear of DeepSpeakerModel.forward_classifier (reference model.py:167,220-223): y (M,N) = x (M,K) w(N,K)^T + b.
  * fp32 on the CUDA cores, fixed summation order (deterministic).  b may be NULL. */
 int32_t dsk_linear_forward(const float* x, const float* w, const float* b, int32_t M, int32_t N, int32_t K, float* y,
