@@ -230,6 +230,12 @@ SIGNATURES = {
     "dsk_fbank_batch": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     "dsk_fbank_crops": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int32,
                                   c_void_p, c_int32, c_void_p, c_void_p]),
+    "dsk_fbank_batch_vad": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_double, c_double,
+                                      c_int32, c_double, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "dsk_frame_runs": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int64, c_int64, c_void_p,
+                                 c_void_p, c_void_p, c_void_p]),
+    "dsk_gather_runs": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p,
+                                  c_void_p]),
     "dsk_fbank_filterbank": (c_int32, [c_int32, c_void_p]),
     "dsk_wave_augment": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p,
                                    c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 5),

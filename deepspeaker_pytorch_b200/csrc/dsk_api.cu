@@ -22,6 +22,7 @@
 #include "conv3x3_halo.cuh"
 #include "conv1_umma.cuh"
 #include "fbank_kernels.cuh"
+#include "vad_kernels.cuh"
 #include "augment_kernels.cuh"
 #include "cluster_kernels.cuh"
 #include "head_kernels.cuh"
@@ -3764,8 +3765,16 @@ int32_t dsk_fbank_filterbank(int32_t sample_rate, float* fb) {
   return DSK_OK;
 }
 
-int32_t dsk_fbank_batch(const float* audio, const int64_t* sample_off, int32_t U, int32_t sample_rate, int32_t log_scale,
-                        int32_t subtract_mean, float* feat, void* stream) {
+struct FbankVad {
+  double energy_threshold, mean_scale, proportion;
+  int32_t context;
+  float* energy;      // may be null
+  uint8_t* speech;
+};
+
+// dsk_fbank_batch, and with vad the energies and speech decisions of the same frames (the features do not depend on it)
+static int32_t fbank_batch(const float* audio, const int64_t* sample_off, int32_t U, int32_t sample_rate, int32_t log_scale,
+                           int32_t subtract_mean, float* feat, const FbankVad* vad, void* stream) {
   if (!audio || !feat || !sample_off || U < 1)
     return fail(DSK_ERR_INVALID, "dsk_fbank_batch: bad arguments (need non-null pointers and U >= 1; got U %d)", U);
   const long flen = fbank_round_half_up(0.025 * sample_rate), step = fbank_round_half_up(0.01 * sample_rate);
@@ -3784,9 +3793,14 @@ int32_t dsk_fbank_batch(const float* audio, const int64_t* sample_off, int32_t U
   // built once per call for all U utterances
   std::vector<float> fb(static_cast<size_t>(dsk::kFbFilters) * dsk::kFbBins);
   if (int32_t rc = dsk_fbank_filterbank(sample_rate, fb.data())) return rc;
-  // scratch: the three offset tables (int64) | [64][257] filterbank | [nblk][64] column-sum partials | [U][64] means
+  // scratch: the three offset tables (int64) | [64][257] filterbank | [nblk][64] column-sum partials | [U][64] means,
+  // then with vad: ln E [F] | block partials [nblk] | thresholds [U] (fp64) | energies [F] fp32 when vad->energy is null
   const size_t off_bytes = off.size() * sizeof(int64_t), fb_bytes = fb.size() * sizeof(float);
-  const size_t bytes = off_bytes + fb_bytes + (static_cast<size_t>(nblk) + U) * dsk::kFbFilters * sizeof(float);
+  const size_t fbank_bytes = off_bytes + fb_bytes + (static_cast<size_t>(nblk) + U) * dsk::kFbFilters * sizeof(float);
+  const int64_t F = foff[U];
+  const size_t vad_bytes = !vad ? 0 : (static_cast<size_t>(F) + nblk + U) * sizeof(double) +
+                                          (vad->energy ? 0 : static_cast<size_t>(F) * sizeof(float));
+  const size_t bytes = fbank_bytes + vad_bytes;
   char* scratch = nullptr;
   CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&scratch), bytes, s));
   CUDA_TRY(cudaMemcpyAsync(scratch, off.data(), off_bytes, cudaMemcpyHostToDevice, s));
@@ -3798,9 +3812,13 @@ int32_t dsk_fbank_batch(const float* audio, const int64_t* sample_off, int32_t U
   const float* d_fb = reinterpret_cast<const float*>(scratch + off_bytes);
   float* partial = reinterpret_cast<float*>(scratch + off_bytes + fb_bytes);
   float* mean = partial + nblk * dsk::kFbFilters;
+  double* loge = reinterpret_cast<double*>(scratch + fbank_bytes);
+  double* lpartial = loge + F;
+  double* thr = lpartial + nblk;
+  float* energy = vad ? (vad->energy ? vad->energy : reinterpret_cast<float*>(thr + U)) : nullptr;
   dsk::fbank_kernel<<<static_cast<unsigned>(nblk), dsk::kFbThreads, 0, s>>>(audio, d_soff, d_foff, d_boff, U, static_cast<int>(flen),
                                                                             static_cast<int>(step), 0.97f, d_fb, log_scale, 1e-5f,
-                                                                            feat, partial);
+                                                                            feat, partial, energy);
   KERNEL_CHECK();
   if (subtract_mean) {
     dsk::fbank_mean_kernel<<<static_cast<unsigned>((static_cast<long>(U) * dsk::kFbFilters + 255) / 256), 256, 0, s>>>(partial, d_foff, d_boff, U, mean);
@@ -3808,7 +3826,85 @@ int32_t dsk_fbank_batch(const float* audio, const int64_t* sample_off, int32_t U
     dsk::fbank_mean_sub_kernel<<<static_cast<unsigned>(nblk), dsk::kFbThreads, 0, s>>>(feat, d_foff, d_boff, U, mean);
     KERNEL_CHECK();
   }
+  if (vad) {
+    dsk::vad_log_energy_kernel<<<static_cast<unsigned>((nblk + 255) / 256), 256, 0, s>>>(energy, d_foff, d_boff, U, nblk, loge,
+                                                                                        lpartial);
+    KERNEL_CHECK();
+    dsk::vad_threshold_kernel<<<(U + 255) / 256, 256, 0, s>>>(lpartial, d_foff, d_boff, U, vad->energy_threshold,
+                                                              vad->mean_scale, thr);
+    KERNEL_CHECK();
+    dsk::vad_decide_kernel<<<static_cast<unsigned>((F + 255) / 256), 256, 0, s>>>(loge, d_foff, U, thr, F, vad->context,
+                                                                                 vad->proportion, vad->speech);
+    KERNEL_CHECK();
+  }
   CUDA_TRY(cudaFreeAsync(scratch, s));
+  return DSK_OK;
+}
+
+int32_t dsk_fbank_batch(const float* audio, const int64_t* sample_off, int32_t U, int32_t sample_rate, int32_t log_scale,
+                        int32_t subtract_mean, float* feat, void* stream) {
+  return fbank_batch(audio, sample_off, U, sample_rate, log_scale, subtract_mean, feat, nullptr, stream);
+}
+
+int32_t dsk_fbank_batch_vad(const float* audio, const int64_t* sample_off, int32_t U, int32_t sample_rate,
+                            int32_t log_scale, int32_t subtract_mean, double energy_threshold, double mean_scale,
+                            int32_t context, double proportion, float* feat, float* energy, uint8_t* speech,
+                            void* stream) {
+  if (!speech || !std::isfinite(energy_threshold) || !std::isfinite(mean_scale) || !std::isfinite(proportion) ||
+      context < 0 || proportion < 0)
+    return fail(DSK_ERR_INVALID, "dsk_fbank_batch_vad: bad VAD arguments (need non-null speech, finite energy_threshold, "
+                "mean_scale and proportion, context >= 0, proportion >= 0; got %g, %g, %d, %g)", energy_threshold,
+                mean_scale, context, proportion);
+  const FbankVad vad{energy_threshold, mean_scale, proportion, context, energy, speech};
+  return fbank_batch(audio, sample_off, U, sample_rate, log_scale, subtract_mean, feat, &vad, stream);
+}
+
+int32_t dsk_frame_runs(const uint8_t* mask, const int64_t* frame_off, int32_t U, const int64_t* utt,
+                       const int64_t* list_off, int32_t K, int64_t P, int64_t capacity, int64_t* runs, int64_t* run_off,
+                       int64_t* counts, void* stream) {
+  if (!mask || !frame_off || !utt || !list_off || !runs || !run_off || !counts || U < 1 || K < 1 || P < K ||
+      capacity < 0)
+    return fail(DSK_ERR_INVALID, "dsk_frame_runs: bad arguments (need non-null pointers, U, K >= 1, P >= K, capacity >= 0; "
+                "got U %d, K %d, P %lld, capacity %lld)", U, K, static_cast<long long>(P), static_cast<long long>(capacity));
+  const int64_t ntiles = (P + dsk::kRunTile - 1) / dsk::kRunTile;
+  if (ntiles >= (1ll << 31)) return fail(DSK_ERR_INVALID, "dsk_frame_runs: %lld frames exceed one launch", static_cast<long long>(P));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // scratch: tile run starts [ntiles] | tile kept frames [ntiles] | totals [2]
+  int64_t* scratch = nullptr;
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&scratch), (2 * ntiles + 2) * sizeof(int64_t), s));
+  int64_t* tile_starts = scratch;
+  int64_t* tile_kept = scratch + ntiles;
+  int64_t* totals = tile_kept + ntiles;
+  dsk::run_count_kernel<<<static_cast<unsigned>(ntiles), dsk::kRunThreads, 0, s>>>(mask, frame_off, utt, list_off, K, P,
+                                                                                  tile_starts, tile_kept);
+  KERNEL_CHECK();
+  dsk::run_scan_kernel<<<1, dsk::kRunThreads, 0, s>>>(tile_starts, tile_kept, ntiles, capacity, run_off, totals);
+  KERNEL_CHECK();
+  dsk::run_write_kernel<<<static_cast<unsigned>(ntiles), dsk::kRunThreads, 0, s>>>(mask, frame_off, utt, list_off, K, P,
+                                                                                  tile_starts, tile_kept, capacity, runs,
+                                                                                  run_off);
+  KERNEL_CHECK();
+  CUDA_TRY(cudaMemcpyAsync(counts, totals, 2 * sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(cudaFreeAsync(scratch, s));
+  CUDA_TRY(cudaStreamSynchronize(s));   // the call's one host read: the run count sizes the caller's next step
+  if (counts[0] > capacity)
+    return fail(DSK_ERR_INVALID, "dsk_frame_runs: %lld runs exceed the capacity %lld", static_cast<long long>(counts[0]),
+                static_cast<long long>(capacity));
+  return DSK_OK;
+}
+
+int32_t dsk_gather_runs(const float* feat, const int64_t* frame_off, int32_t U, const int64_t* utt, const int64_t* runs,
+                        const int64_t* run_off, int64_t n_runs, int64_t rows, float* out, void* stream) {
+  if (!feat || !frame_off || !utt || !runs || !run_off || !out || U < 1 || n_runs < 1 || rows < n_runs)
+    return fail(DSK_ERR_INVALID, "dsk_gather_runs: bad arguments (need non-null pointers, U, n_runs >= 1, rows >= n_runs; "
+                "got U %d, n_runs %lld, rows %lld)", U, static_cast<long long>(n_runs), static_cast<long long>(rows));
+  if ((reinterpret_cast<uintptr_t>(feat) | reinterpret_cast<uintptr_t>(out)) & 15)
+    return fail(DSK_ERR_INVALID, "dsk_gather_runs: feat and out must be 16-byte aligned");
+  const int64_t grid = (rows + dsk::kRunGatherRows - 1) / dsk::kRunGatherRows;
+  if (grid >= (1ll << 31)) return fail(DSK_ERR_INVALID, "dsk_gather_runs: %lld rows exceed one launch", static_cast<long long>(rows));
+  dsk::run_gather_kernel<<<static_cast<unsigned>(grid), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      feat, frame_off, utt, runs, run_off, n_runs, rows, out);
+  KERNEL_CHECK();
   return DSK_OK;
 }
 

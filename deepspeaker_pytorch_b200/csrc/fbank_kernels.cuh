@@ -36,12 +36,14 @@ __device__ __forceinline__ int fbank_block_utt(const int64_t* __restrict__ boff,
 // feat[f][m] = 20 log10(max(sum_k pspec[f][k] * fb[m][k], floor)) for frame f of the block's utterance; partial column
 // sums per block for the mean.  Utterance u: n samples; its frame f covers samples [f*step, f*step + flen) of the
 // PRE-EMPHASISED signal, zero beyond n.  fb: [64][257] fp32.  grid = boff[U], block = 256: thread group g = tid / 64
-// owns local frame 4*(blockIdx.x - boff[u]) + g.
+// owns local frame 4*(blockIdx.x - boff[u]) + g.  energy_all (may be null): the frame energy E_f = pspec[f][0] +
+// pspec[f][1] + ... + pspec[f][256] added in fp32 in bin order, 0 replaced by eps (python_speech_features' `energy`),
+// one float per frame at foff[u] + f.
 __global__ void __launch_bounds__(kFbThreads)
 fbank_kernel(const float* __restrict__ audio_all, const int64_t* __restrict__ soff, const int64_t* __restrict__ foff,
              const int64_t* __restrict__ boff, int U, int flen, int step, float preemph,
              const float* __restrict__ fb, int log_scale, float log_floor, float* __restrict__ feat_all,
-             float* __restrict__ colsum_partial /* [gridDim.x][64] */) {
+             float* __restrict__ colsum_partial /* [gridDim.x][64] */, float* __restrict__ energy_all = nullptr) {
   __shared__ float2 buf[kFbFramesPerBlock][kFbNfft];     // complex FFT workspace per frame
   __shared__ float pspec[kFbFramesPerBlock][kFbBins + 3];
   __shared__ float rowfeat[kFbFramesPerBlock][kFbFilters];
@@ -91,6 +93,11 @@ fbank_kernel(const float* __restrict__ audio_all, const int64_t* __restrict__ so
     if (log_scale) acc = 20.0f * log10f(fmaxf(acc, log_floor));
     rowfeat[g][t] = live ? acc : 0.f;
     if (live) feat[static_cast<long>(f) * kFbFilters + t] = acc;
+  }
+  if (energy_all && live && t == 0) {
+    float e = 0.f;
+    for (int k = 0; k < kFbBins; ++k) e += pspec[g][k];
+    energy_all[foff[u] + f] = e == 0.f ? 2.220446049250313e-16f : e;
   }
   __syncthreads();
   if (g == 0) {  // per-block column sums, fixed order

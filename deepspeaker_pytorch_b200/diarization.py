@@ -7,8 +7,14 @@ by default), cut at a known number of speakers or at a distance threshold.  Each
 the covering window whose centre is nearest, and runs of equal frame labels become segments.  ``to_rttm`` writes them
 in the RTTM format scoring tools read.
 
-Overlapped speech, voice activity detection and re-segmentation are not part of this module: every frame gets exactly
-one speaker.
+With ``speech`` (an (F,) mask over the bank's rows: ``bank.speech`` from the frame-energy VAD of
+``FeatureBank.from_waveforms(..., vad={})``, or oracle speech from reference annotations) only speech is diarized: every
+run of speech frames is cut into windows of its own (``FeatureBank.runs``; a run shorter than T gets one window that
+wraps inside the run), all windows of a recording are clustered together, each speech frame takes the label of the
+nearest window centre within its run and every other frame is -1, which no segment or RTTM line covers.  Without it,
+every frame gets a speaker, silence included.
+
+Overlapped speech and re-segmentation are not part of this module: a frame gets at most one speaker.
 """
 from __future__ import annotations
 
@@ -79,13 +85,86 @@ def _per_recording(x, n, what):
     return [x] * n
 
 
+def _window_counts(last, hop):
+    """Windows per run of ``sliding_windows`` at ``hop``, from each run's last start n - T (clipped at 0)."""
+    return np.where(last > 0, -(-last // hop) + 1, 1)
+
+
+def _smallest_hop(last, rec, R, hop):
+    """The smallest hop >= ``hop`` at which no recording (``rec``: each run's recording, of R) has more than
+    MAX_WINDOWS windows, or None.  The counts do not grow with the hop, so a binary search finds it."""
+    def fits(h):
+        return np.bincount(rec, _window_counts(last, h), minlength=R).max() <= MAX_WINDOWS
+
+    hi = int(max(last.max(), 1)) + 1                      # past the longest run every run has at most 2 windows
+    if not fits(hi):
+        return None
+    lo = int(hop)
+    while lo < hi:
+        mid = (lo + hi) // 2
+        if fits(mid):
+            hi = mid
+        else:
+            lo = mid + 1
+    return lo
+
+
+def _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batch):
+    R = u.size
+    table, runs, run_off, kept = bank._run_table(speech, u, "diarize")
+    rec, first, end = table[:, 0], table[:, 1], table[:, 2]
+    rlen = end - first
+    if rec.size:
+        wcount = np.bincount(rec, _window_counts(np.maximum(rlen - int(T), 0), int(hop)), minlength=R)
+        if wcount.max() > MAX_WINDOWS:
+            need = _smallest_hop(np.maximum(rlen - int(T), 0), rec, R, hop)
+            fix = f"use hop >= {need}" if need is not None else "no hop fits: the recording has too many speech runs"
+            raise ValueError(f"diarize: a recording's speech runs have {int(wcount.max())} windows at hop {hop}, more "
+                             f"than {MAX_WINDOWS}; {fix}")
+        run_bank = frontend.FeatureBank(bank._gather(runs, run_off, rec.size, kept, u),
+                                        np.concatenate(([0], np.cumsum(rlen))))
+        emb, _, win_start, win_off = frontend.window_embeddings(model, run_bank, np.arange(rec.size), T, hop, batch,
+                                                                "diarize")
+        win_off = win_off.numpy()
+    run_off_rec = np.searchsorted(rec, np.arange(R + 1))     # runs of recording r: run_off_rec[r] .. [r + 1]
+    out = []
+    for r in range(R):
+        n = int(bank.lengths[u[r]])
+        r0, r1 = int(run_off_rec[r]), int(run_off_rec[r + 1])
+        fl = np.full(n, -1, np.int32)
+        if r0 == r1:
+            out.append(Recording([], fl, np.zeros(0, np.int32), np.zeros((0, 4))))
+            continue
+        a, b = int(win_off[r0]), int(win_off[r1])
+        W = b - a
+        if W == 1:
+            wl, Z = np.zeros(1, np.int32), np.zeros((0, 4))
+        else:
+            E = emb[a:b]
+            S = engine.cosine_matrix(E, E)
+            if threshold is not None:
+                Z, lab = engine.ahc(S, linkage, threshold=threshold)
+            else:
+                Z, lab = engine.ahc(S, linkage, num_clusters=min(int(ks[r]), W))
+            wl = lab.cpu().numpy()
+        for i in range(r0, r1):
+            w0, w1 = int(win_off[i]), int(win_off[i + 1])
+            fl[first[i]:end[i]] = frame_labels(win_start[w0:w1].numpy(), wl[w0 - a:w1 - a], int(rlen[i]), T)
+        out.append(Recording([sg for sg in segments(fl) if sg[2] >= 0], fl, wl, Z))
+    return out
+
+
 def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40, num_speakers=None, threshold=None,
-            linkage: str = "average", batch: int = 256) -> list:
+            linkage: str = "average", batch: int = 256, speech=None) -> list:
     """Diarize the recordings ``utt`` (indices into ``bank``) -> [Recording] in the order of ``utt``.  Give exactly
     one of ``num_speakers`` (an int, or one per recording; a recording with fewer windows gets one speaker per window)
     and ``threshold`` (a cosine distance 1 - cos: windows merge while the linkage distance is <= threshold), else
     ValueError.  Windows of T frames every ``hop`` frames; a recording needing more than ``MAX_WINDOWS`` windows is a
-    ValueError naming the smallest hop that fits.  RuntimeError on a model in train mode."""
+    ValueError naming the smallest hop that fits.  RuntimeError on a model in train mode.
+
+    ``speech``: None (every frame gets a speaker), or an (F,) bool mask over the bank's rows (CPU or CUDA, such as
+    ``bank.speech``): the windows are cut per run of speech frames, non-speech frames are labelled -1 and lie in no
+    segment, and a recording without speech has no windows, no segments and only -1 frames."""
     if (num_speakers is None) == (threshold is None):
         raise ValueError("diarize: give exactly one of num_speakers and threshold")
     if linkage not in engine.LINKAGES:
@@ -98,6 +177,8 @@ def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40,
     ks = _per_recording(num_speakers, u.size, "num_speakers")
     if num_speakers is not None and any(int(k) < 1 for k in ks):
         raise ValueError(f"diarize: num_speakers must be >= 1, got {num_speakers}")
+    if speech is not None:
+        return _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batch)
     _, _, win_off = bank.windows(u, T, hop)
     counts = np.diff(win_off.numpy())
     if counts.max() > MAX_WINDOWS:

@@ -15,6 +15,11 @@ SpecAugment time and frequency masks; ``random_starts`` and ``spec_augment_masks
 the host.  ``bank.windows`` and ``embed_utterances`` turn whole utterances into utterance-level embeddings through the
 fixed-shape eval forward: the mean of the unit embeddings of sliding windows.
 
+``mk_mfb_batch_vad`` adds a frame-energy voice activity decision (Kaldi's ``compute-vad`` rule on the fbank's own
+frame energies); ``FeatureBank.from_waveforms(..., vad={})`` keeps it as ``bank.speech``.  ``bank.select(mask)`` keeps
+each utterance's speech frames (``embed_utterances(model, bank.select(bank.speech), utt)`` embeds speech only) and
+``bank.runs(mask, utt)`` cuts every run of kept frames into an utterance of its own (what ``diarize`` windows).
+
 ``WaveBank`` keeps int16 waveforms (on the device or in pinned host memory) for training on augmented speech:
 ``augmented_crops`` gathers each step's segments, reverberates them by a ``RirBank`` RIR, mixes noise sources at target
 SNRs (``augment_plan`` draws them on the host) and computes their features, all on the device with no host
@@ -60,6 +65,32 @@ def fbank_frame_offsets(lengths, sample_rate: int = 16000) -> np.ndarray:
     return foff
 
 
+def _fbank_batch(audio, lengths, sample_rate, use_logscale, subtract_mean, vad, what):
+    if not isinstance(audio, torch.Tensor) or not audio.is_cuda:
+        raise RuntimeError(f"{what} needs a CUDA tensor; there is no CPU fallback")
+    if isinstance(lengths, torch.Tensor) and lengths.is_cuda:
+        raise RuntimeError(f"{what}: lengths must be on the host (they size the output)")
+    a = audio.detach().reshape(-1).float().contiguous()
+    lens = _host_int64(lengths, what)
+    if lens.size and int(lens.sum()) != a.numel():
+        raise ValueError(f"{what}: lengths add up to {int(lens.sum())} samples, audio has {a.numel()}")
+    foff = fbank_frame_offsets(lens, sample_rate)
+    soff = np.concatenate(([0], np.cumsum(lens))).astype(np.int64)
+    feat = torch.empty(int(foff[-1]), N_MELS, device=a.device, dtype=torch.float32)
+    with torch.cuda.device(a.device):
+        if vad is None:
+            L.check(L.load().dsk_fbank_batch(a.data_ptr(), _ptr64(soff), lens.size, int(sample_rate), int(use_logscale),
+                                             int(subtract_mean), feat.data_ptr(), L.cur_stream()), "dsk_fbank_batch")
+            return feat, torch.from_numpy(foff)
+        energy = torch.empty(int(foff[-1]), device=a.device, dtype=torch.float32)
+        speech = torch.empty(int(foff[-1]), device=a.device, dtype=torch.bool)
+        L.check(L.load().dsk_fbank_batch_vad(a.data_ptr(), _ptr64(soff), lens.size, int(sample_rate), int(use_logscale),
+                                             int(subtract_mean), vad["energy_threshold"], vad["mean_scale"],
+                                             vad["context"], vad["proportion"], feat.data_ptr(), energy.data_ptr(),
+                                             speech.data_ptr(), L.cur_stream()), "dsk_fbank_batch_vad")
+    return feat, torch.from_numpy(foff), energy, speech
+
+
 def mk_mfb_batch(audio: torch.Tensor, lengths, sample_rate: int = 16000, use_logscale: bool = True,
                  subtract_mean: bool = True):
     """``audio``: 1-D fp32 CUDA tensor, U waveforms concatenated; ``lengths`` (U,) samples per waveform, on the host
@@ -67,21 +98,57 @@ def mk_mfb_batch(audio: torch.Tensor, lengths, sample_rate: int = 16000, use_log
     bit-identical to ``mk_mfb`` on that waveform alone.  One launch sequence and one host synchronisation per call.
     RuntimeError for a CPU tensor; ValueError for a zero length or lengths that do not add up to ``audio``, before any
     launch."""
-    if not isinstance(audio, torch.Tensor) or not audio.is_cuda:
-        raise RuntimeError("mk_mfb_batch needs a CUDA tensor; there is no CPU fallback")
-    if isinstance(lengths, torch.Tensor) and lengths.is_cuda:
-        raise RuntimeError("mk_mfb_batch: lengths must be on the host (they size the output)")
-    a = audio.detach().reshape(-1).float().contiguous()
-    lens = _host_int64(lengths, "mk_mfb_batch")
-    if lens.size and int(lens.sum()) != a.numel():
-        raise ValueError(f"mk_mfb_batch: lengths add up to {int(lens.sum())} samples, audio has {a.numel()}")
-    foff = fbank_frame_offsets(lens, sample_rate)
-    soff = np.concatenate(([0], np.cumsum(lens))).astype(np.int64)
-    feat = torch.empty(int(foff[-1]), N_MELS, device=a.device, dtype=torch.float32)
-    with torch.cuda.device(a.device):
-        L.check(L.load().dsk_fbank_batch(a.data_ptr(), _ptr64(soff), lens.size, int(sample_rate), int(use_logscale),
-                                         int(subtract_mean), feat.data_ptr(), L.cur_stream()), "dsk_fbank_batch")
-    return feat, torch.from_numpy(foff)
+    return _fbank_batch(audio, lengths, sample_rate, use_logscale, subtract_mean, None, "mk_mfb_batch")
+
+
+# Kaldi's compute-vad threshold 5.5 is set against ln of an int16-scale sum of squares over the frame.  Float samples
+# are 2^-15 of int16 ones (2^-30 in energy) and bins 0..256 of |rfft|^2 / 512 hold about half the frame's sum of
+# squares (Parseval), so every e_f here is about ln(2^31) lower.  Lowering every e_f by D lowers the mean term by
+# mean_scale * D = 0.5 D, so the same decisions need the constant lowered by the other 0.5 D: 5.5 - 0.5 ln(2^31).
+# Pre-emphasis is not corrected for.
+VAD_ENERGY_THRESHOLD = 5.5 - 0.5 * float(np.log(2.0 ** 31))
+VAD_DEFAULTS = {"energy_threshold": VAD_ENERGY_THRESHOLD, "mean_scale": 0.5, "context": 2, "proportion": 0.12}
+
+
+def vad_params(vad=None, **kw) -> dict:
+    """The VAD parameters of a dict (``{}`` or None: the defaults ``VAD_DEFAULTS``) plus keyword overrides, checked:
+    ValueError for an unknown key, a non-finite value, a context that is not an integer in [0, 2^31) or a negative
+    proportion."""
+    p = dict(VAD_DEFAULTS)
+    for src in (vad or {}, kw):
+        for k, v in src.items():
+            if k not in VAD_DEFAULTS:
+                raise ValueError(f"vad: unknown parameter {k!r} (known: {sorted(VAD_DEFAULTS)})")
+            p[k] = v
+    for k in ("energy_threshold", "mean_scale", "proportion"):
+        p[k] = float(p[k])
+        if not np.isfinite(p[k]):
+            raise ValueError(f"vad: {k} must be finite, got {p[k]}")
+    c = p["context"]
+    if isinstance(c, bool) or not float(c).is_integer() or not 0 <= float(c) < 2 ** 31:
+        raise ValueError(f"vad: context must be an integer in [0, 2^31), got {c!r}")
+    p["context"] = int(c)
+    if p["proportion"] < 0:
+        raise ValueError(f"vad: proportion must be >= 0, got {p['proportion']}")
+    return p
+
+
+def mk_mfb_batch_vad(audio: torch.Tensor, lengths, sample_rate: int = 16000, use_logscale: bool = True,
+                     subtract_mean: bool = True, energy_threshold: float = VAD_ENERGY_THRESHOLD,
+                     mean_scale: float = 0.5, context: int = 2, proportion: float = 0.12):
+    """``mk_mfb_batch`` plus a frame-energy voice activity decision on the same frames -> ``(feats, offsets, energy,
+    speech)``: ``feats`` and ``offsets`` bit-identical to ``mk_mfb_batch``'s, ``energy`` (F,) fp32 CUDA the frame
+    energy E_f (the sum over bins 0..256 of the frame's power spectrum, added in fp32 in bin order; 0 becomes
+    2.220446049250313e-16; python_speech_features' ``energy``), ``speech`` (F,) bool CUDA.
+
+    The rule is Kaldi's ``compute-vad``: with e_f = ln E_f in fp64 and thr_u = energy_threshold + mean_scale * mean_f
+    e_f over the utterance, frame f is speech iff at least ``proportion`` of the frames within ``context`` frames of it
+    (clipped to the utterance) have e_g > thr_u.  The defaults are Kaldi's VoxCeleb ``vad.conf`` (0.5, 2, 0.12) with its
+    threshold 5.5 moved to float samples and this energy: 5.5 - 0.5 ln(2^31) ~ -5.2438.  **That threshold is not
+    calibrated on labelled speech**; check it on your data.  Each utterance's energies and decisions are bit-identical
+    whatever the other utterances of the batch.  ValueError for bad parameters (``vad_params``)."""
+    vad = vad_params(energy_threshold=energy_threshold, mean_scale=mean_scale, context=context, proportion=proportion)
+    return _fbank_batch(audio, lengths, sample_rate, use_logscale, subtract_mean, vad, "mk_mfb_batch_vad")
 
 
 def mk_mfb(audio: torch.Tensor, sample_rate: int = 16000, use_logscale: bool = True, subtract_mean: bool = True) -> torch.Tensor:
@@ -168,6 +235,7 @@ class FeatureBank:
         self.feats = feats.contiguous()
         self.lengths = np.diff(off)
         self.offsets = torch.from_numpy(off).to(feats.device)
+        self.speech = None      # (F,) bool CUDA voice activity of the rows, when the bank was built with a VAD
 
     @property
     def num_utterances(self) -> int:
@@ -179,13 +247,17 @@ class FeatureBank:
 
     @classmethod
     def from_waveforms(cls, waveforms, sample_rate: int = 16000, chunk_samples: int = 1 << 26, device=None,
-                       use_logscale: bool = True, subtract_mean: bool = True):
+                       use_logscale: bool = True, subtract_mean: bool = True, vad=None):
         """The bank of a list of 1-D waveforms (numpy arrays or tensors), through ``mk_mfb_batch`` in chunks of at most
-        ``chunk_samples`` samples (or one waveform, if longer), so only one chunk of audio is on the device at a time."""
+        ``chunk_samples`` samples (or one waveform, if longer), so only one chunk of audio is on the device at a time.
+        ``vad``: a dict of ``mk_mfb_batch_vad``'s VAD parameters (``{}``: the defaults) to also set ``bank.speech``,
+        the (F,) bool CUDA speech decision of every row (the features are the same bits either way)."""
         device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        params = None if vad is None else vad_params(vad)
         lens = np.array([int(np.prod(w.shape)) for w in waveforms], np.int64)
         foff = fbank_frame_offsets(lens, sample_rate)          # ValueError on an empty list or waveform
         feats = torch.empty(int(foff[-1]), N_MELS, device=device, dtype=torch.float32)
+        speech = None if params is None else torch.empty(int(foff[-1]), device=device, dtype=torch.bool)
         i = 0
         while i < len(waveforms):
             j, total = i + 1, lens[i]
@@ -193,10 +265,15 @@ class FeatureBank:
                 total += lens[j]
                 j += 1
             host = torch.cat([torch.as_tensor(w).reshape(-1).float() for w in waveforms[i:j]])
-            f, _ = mk_mfb_batch(host.to(device), lens[i:j], sample_rate, use_logscale, subtract_mean)
-            feats[foff[i]:foff[j]].copy_(f)
+            out = _fbank_batch(host.to(device), lens[i:j], sample_rate, use_logscale, subtract_mean, params,
+                               "FeatureBank.from_waveforms")
+            feats[foff[i]:foff[j]].copy_(out[0])
+            if speech is not None:
+                speech[foff[i]:foff[j]].copy_(out[3])
             i = j
-        return cls(feats, foff)
+        bank = cls(feats, foff)
+        bank.speech = speech
+        return bank
 
     @classmethod
     def from_arrays(cls, arrays, device=None):
@@ -259,6 +336,71 @@ class FeatureBank:
     def windows(self, utt, T: int, hop: int):
         """``sliding_windows`` over this bank's frame counts: ``(win_utt, win_start, win_off)`` host int64."""
         return sliding_windows(self.lengths, utt, T, hop)
+
+    def select(self, mask) -> "FeatureBank":
+        """The bank of each utterance's kept frames (``mask``: (F,) bool over this bank's rows, CPU or CUDA, such as
+        ``bank.speech``), in order: utterance u of the result is the rows of utterance u with ``mask`` set.  The rows
+        are copied bit for bit (the features keep the mean of the whole utterance).  ValueError naming every utterance
+        left without frames.  One host read (the run count) and one copy of the run table."""
+        table, runs, run_off, kept = self._run_table(mask, np.arange(self.num_utterances), "select")
+        counts = np.zeros(self.num_utterances, np.int64)
+        np.add.at(counts, table[:, 0], table[:, 2] - table[:, 1])
+        empty = np.flatnonzero(counts == 0)
+        if empty.size:
+            raise ValueError(f"select: {empty.size} utterance(s) left without frames: {empty.tolist()}")
+        feats = self._gather(runs, run_off, table.shape[0], kept, np.arange(self.num_utterances))
+        return FeatureBank(feats, np.concatenate(([0], np.cumsum(counts))))
+
+    def runs(self, mask, utt):
+        """Every run of kept frames (``mask`` as for ``select``) of the utterances ``utt`` as an utterance of its own
+        -> ``(run_bank, run_utt, run_start)``: run i is frames ``run_start[i]`` .. ``run_start[i] + run_bank.lengths[i]``
+        of utterance ``run_utt[i]`` (host int64), in the order of ``utt`` and in frame order within an utterance.
+        ValueError when no frame of ``utt`` is kept."""
+        u = _host_int64(utt, "runs")
+        table, runs, run_off, kept = self._run_table(mask, u, "runs")
+        if table.shape[0] == 0:
+            raise ValueError("runs: no frame of these utterances is kept")
+        feats = self._gather(runs, run_off, table.shape[0], kept, u)
+        bank = FeatureBank(feats, np.concatenate(([0], np.cumsum(table[:, 2] - table[:, 1]))))
+        return bank, torch.from_numpy(u[table[:, 0]]), torch.from_numpy(table[:, 1].copy())
+
+    def _mask(self, mask, what):
+        m = torch.as_tensor(mask)
+        if m.shape != (self.feats.shape[0],) or m.is_floating_point() or m.is_complex():
+            raise ValueError(f"{what}: expected an (F,) = ({self.feats.shape[0]},) bool mask, got {tuple(m.shape)} {m.dtype}")
+        if m.dtype != torch.bool:
+            m = m != 0
+        return _to_dev(m, torch.bool, self.device)
+
+    def _run_table(self, mask, u, what):
+        """(table (n, 3) host int64 rows (j, first, end), runs and run_off on the device, kept frames) of ``dsk_frame_runs``
+        over the utterances u (host int64)."""
+        m = self._mask(mask, what)
+        if u.size == 0 or u.min() < 0 or u.max() >= self.num_utterances:
+            raise ValueError(f"{what}: expected utterance indices in [0, {self.num_utterances}), at least one")
+        lens = self.lengths[u]
+        loff = np.concatenate(([0], np.cumsum(lens))).astype(np.int64)
+        cap = int(np.sum((lens + 1) // 2))                   # an utterance of n frames has at most ceil(n / 2) runs
+        dev = self.device
+        runs = torch.empty(cap, 3, device=dev, dtype=torch.int64)
+        run_off = torch.empty(cap + 1, device=dev, dtype=torch.int64)
+        ud, ld = _to_dev(torch.from_numpy(u), torch.int64, dev), _to_dev(torch.from_numpy(loff), torch.int64, dev)
+        counts = np.zeros(2, np.int64)
+        with torch.cuda.device(dev):
+            L.check(L.load().dsk_frame_runs(m.data_ptr(), self.offsets.data_ptr(), self.num_utterances, ud.data_ptr(),
+                                            ld.data_ptr(), u.size, int(loff[-1]), cap, runs.data_ptr(),
+                                            run_off.data_ptr(), _ptr64(counts), L.cur_stream()), "dsk_frame_runs")
+        n = int(counts[0])
+        return runs[:n].cpu().numpy(), runs, run_off, int(counts[1])
+
+    def _gather(self, runs, run_off, n, kept, u):
+        out = torch.empty(kept, N_MELS, device=self.device, dtype=torch.float32)
+        ud = _to_dev(torch.from_numpy(np.ascontiguousarray(u, np.int64)), torch.int64, self.device)
+        with torch.cuda.device(self.device):
+            L.check(L.load().dsk_gather_runs(self.feats.data_ptr(), self.offsets.data_ptr(), self.num_utterances,
+                                             ud.data_ptr(), runs.data_ptr(), run_off.data_ptr(), n, kept,
+                                             out.data_ptr(), L.cur_stream()), "dsk_gather_runs")
+        return out
 
 
 def _to_dev(t, dtype, dev):

@@ -614,6 +614,47 @@ int32_t dsk_fbank_crops(const float* feat, const int64_t* frame_off, int32_t U, 
                         int32_t B, int32_t T, const int32_t* time_masks, int32_t n_time, const int32_t* freq_masks,
                         int32_t n_freq, float* out, void* stream);
 
+/* Frame-energy voice activity detection (a restatement of the rule of Kaldi's compute-vad, the energy VAD of the usual
+ * speaker-embedding recipes) and the runs of kept frames of a feature bank.
+ *   Frame energy: E_f = pspec[f][0] + pspec[f][1] + ... + pspec[f][256], added in fp32 in bin order, where pspec is the
+ *     power spectrum the fbank computes for frame f (|rfft|^2 / 512 of the pre-emphasised, zero-padded rectangular
+ *     frame); 0 is replaced by 2.220446049250313e-16.  This is python_speech_features' `energy` output (the reference's
+ *     fbank call returns it and mk_MFB drops it).  Energy row f is feature row f.
+ *   Decision, per utterance u of n_u frames: e_f = ln(E_f) in fp64; thr_u = energy_threshold + mean_scale * (S_u / n_u),
+ *     S_u the sum of e_f over 4-frame blocks in frame order, the block sums added in block order (independent of the
+ *     batch's other utterances); frame f is speech iff #{g in [max(0, f - c), min(n_u - 1, f + c)] : e_g > thr_u} >=
+ *     proportion * (the size of that window), c = context.  Recipe values: mean_scale 0.5, context 2, proportion 0.12,
+ *     energy_threshold 5.5 - 0.5 ln(2^31) (Kaldi's 5.5 moved from an int16-scale sum of squares of the frame to float
+ *     samples and the half-spectrum energy; pre-emphasis not corrected for).  That threshold is not calibrated on
+ *     labelled speech.  Cost per frame: min(2c + 1, n_u) comparisons.
+ *   dsk_fbank_batch_vad: dsk_fbank_batch (feat bit-identical to it: dsk_fbank_batch is the same host code without the
+ *     VAD) plus energy (F,) fp32 (may be NULL) and speech (F,) uint8 0/1, device, F = frame_off[U].  Every utterance's
+ *     energies and decisions are bit-identical whatever the batch's other utterances and their order.  One host
+ *     synchronisation per call.  Non-finite energy_threshold, mean_scale or proportion, context < 0 or proportion < 0:
+ *     DSK_ERR_INVALID.
+ *   dsk_frame_runs: the runs of kept frames (mask[row] != 0, mask (F,) uint8 device over the rows of a bank with device
+ *     frame offsets frame_off (U+1)) of the K listed utterances utt (device int64, each in [0, U)); list_off (device,
+ *     K + 1) holds the prefix sums of their frame counts and P = list_off[K] (host).  runs (capacity, 3) int64 device:
+ *     row r = (j, first, end), local frames [first, end) of utterance utt[j], in list order and frame order within an
+ *     utterance; a run never spans two utterances.  run_off (capacity + 1) int64 device: the kept frames before run r,
+ *     run_off[n_runs] = all kept frames (the offsets of the bank of the runs).  counts (host, 2) = (n_runs, kept frames):
+ *     the call's one host read.  Ordered stream compaction (per-tile counts, one fixed-order scan, then the writes), no
+ *     atomics.  n_runs > capacity: DSK_ERR_INVALID and no row past capacity is written (the runs of an utterance of n
+ *     frames are at most ceil(n / 2)).
+ *   dsk_gather_runs: out (rows, 64) fp32, rows = run_off[n_runs] (host): rows run_off[r] .. run_off[r + 1] are bank rows
+ *     frame_off[utt[j]] + first .. + end of run r.  16-byte loads and stores (feat, out 16-byte aligned), no host
+ *     synchronisation.
+ *   Index arithmetic is 64-bit throughout. */
+int32_t dsk_fbank_batch_vad(const float* audio, const int64_t* sample_off, int32_t U, int32_t sample_rate,
+                            int32_t log_scale, int32_t subtract_mean, double energy_threshold, double mean_scale,
+                            int32_t context, double proportion, float* feat, float* energy, uint8_t* speech,
+                            void* stream);
+int32_t dsk_frame_runs(const uint8_t* mask, const int64_t* frame_off, int32_t U, const int64_t* utt,
+                       const int64_t* list_off, int32_t K, int64_t P, int64_t capacity, int64_t* runs, int64_t* run_off,
+                       int64_t* counts, void* stream);
+int32_t dsk_gather_runs(const float* feat, const int64_t* frame_off, int32_t U, const int64_t* utt, const int64_t* runs,
+                        const int64_t* run_off, int64_t n_runs, int64_t rows, float* out, void* stream);
+
 /* Waveform augmentation of training segments (reverberation by room impulse responses and additive noise, the MUSAN +
  * RIR recipe) and the features of equal-length segments.
  *   dsk_fbank_filterbank: host only.  fb[64][257] fp32, the triangular mel filterbank dsk_fbank_batch applies
