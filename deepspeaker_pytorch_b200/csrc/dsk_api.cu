@@ -3337,10 +3337,10 @@ int32_t dsk_cross_entropy_bwd(const float* logits, const int64_t* labels, const 
 }
 
 int32_t dsk_adagrad_step(float* param, const float* grad, float* state_sum, int64_t n, double lr, double lr_decay,
-                         double weight_decay, double eps, int64_t step, float grad_mult, const float* grad_denom,
+                         double weight_decay, double eps, int64_t step, float grad_div, const float* grad_denom,
                          void* stream) {
-  if (!param || !grad || !state_sum || n <= 0 || step < 1)
-    return fail(DSK_ERR_INVALID, "dsk_adagrad_step: bad arguments (step counts from 1)");
+  if (!param || !grad || !state_sum || n <= 0 || step < 1 || !(grad_div > 0.f))
+    return fail(DSK_ERR_INVALID, "dsk_adagrad_step: bad arguments (step counts from 1, grad_div > 0)");
   if ((reinterpret_cast<uintptr_t>(param) | reinterpret_cast<uintptr_t>(grad) | reinterpret_cast<uintptr_t>(state_sum)) & 15)
     return fail(DSK_ERR_INVALID, "dsk_adagrad_step: buffers must be 16-byte aligned");
   // clr as torch computes it (Python double arithmetic, then one rounding to float at the kernel boundary)
@@ -3348,7 +3348,7 @@ int32_t dsk_adagrad_step(float* param, const float* grad, float* state_sum, int6
   const long n4 = n / 4 > 0 ? n / 4 : 1;
   const int blocks = static_cast<int>((n4 + 255) / 256 < 132 * 16 ? (n4 + 255) / 256 : 132 * 16);
   dsk::adagrad_flat_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      param, grad, state_sum, n, grad_mult, grad_denom, static_cast<float>(minus_clr), static_cast<float>(eps),
+      param, grad, state_sum, n, grad_div, grad_denom, static_cast<float>(minus_clr), static_cast<float>(eps),
       static_cast<float>(weight_decay));
   KERNEL_CHECK();
   return DSK_OK;

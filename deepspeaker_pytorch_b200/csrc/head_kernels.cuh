@@ -10,8 +10,9 @@
 //     (softmax - onehot) * g / M.
 //   * torch.optim.Adagrad(lr, lr_decay, weight_decay) step (reference train_triplet.py:369-383, called at
 //     :224,291) over ONE flat parameter / gradient / state bucket, fused with the post-allreduce scale:
-//       g = grad * mult (/ *denom);  g += wd * p;  G = fma(g, g, G);  p += (g * -clr) / (sqrt(G) + eps)
-//     — the operation order of torch's foreach implementation, so results are bit-identical to torch.optim.Adagrad.
+//       g = grad / div (/ max(*denom, 1e-30));  g += wd * p;  G = fma(g, g, G);  p += (g * -clr) / (sqrt(G) + eps)
+//     — after the scale, the operation order of torch's foreach implementation, so results are bit-identical to
+//     torch.optim.Adagrad stepping on the divided gradient.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -138,7 +139,7 @@ mean_rows_kernel(const float* __restrict__ v, int M, int count, float* __restric
   if (threadIdx.x == 0) out[0] = s / static_cast<float>(count);
 }
 
-// dlogits[i][j] = (exp(logits - lse) - [j == label]) * g / M
+// dlogits[i][j] = (exp(logits - lse) - [j == label]) * g / M; a row whose label is outside [0, C) is NaN, like its loss
 __global__ void ce_bwd_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels,
                               const float* __restrict__ lse, const float* __restrict__ grad_loss, int M, int C,
                               float* __restrict__ dlogits) {
@@ -147,25 +148,30 @@ __global__ void ce_bwd_kernel(const float* __restrict__ logits, const int64_t* _
   for (long e = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; e < total;
        e += static_cast<long>(gridDim.x) * blockDim.x) {
     const int i = static_cast<int>(e / C), j = static_cast<int>(e - static_cast<long>(i) * C);
+    const int64_t y = labels[i];
     const float p = expf(logits[e] - lse[i]);
-    dlogits[e] = (p - (labels[i] == j ? 1.f : 0.f)) * g;
+    dlogits[e] = (y >= 0 && y < C) ? (p - (y == j ? 1.f : 0.f)) * g : __int_as_float(0x7fc00000);
   }
 }
 
 // ---- fused Adagrad over a flat bucket -------------------------------------------------------------------------------
 // Explicit round-to-nearest intrinsics pin the operation order (no re-association / contraction beyond the one fma
 // torch's foreach addcmul kernel performs).
+// The post-allreduce scale divides, as GradBucket's div_ does: g / div, then g / max(*denom, 1e-30) (torch's
+// clamp_min, NaN passes).  A product with the rounded reciprocal differs from the quotient in the last bit for a fifth
+// to a half of the elements when the divisor is 3, 5, 6, 7 or 37; with *denom = 0 it would be 0 * inf = NaN.
 __global__ void __launch_bounds__(256)
-adagrad_flat_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ sum, long n, float mult,
+adagrad_flat_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ sum, long n, float div,
                     const float* __restrict__ denom, float minus_clr, float eps, float wd) {
-  float m = mult;
-  if (denom) m = __fdiv_rn(mult, denom[0]);
+  float dd = 1.0f;
+  if (denom) dd = denom[0] < 1e-30f ? 1e-30f : denom[0];
   const long n4 = n >> 2;
   float4* p4 = reinterpret_cast<float4*>(p);
   const float4* g4 = reinterpret_cast<const float4*>(g);
   float4* s4 = reinterpret_cast<float4*>(sum);
   auto upd = [&](float& pv, float gv, float& sv) {
-    if (m != 1.0f) gv = __fmul_rn(gv, m);
+    if (div != 1.0f) gv = __fdiv_rn(gv, div);
+    if (denom) gv = __fdiv_rn(gv, dd);
     if (wd != 0.f) gv = __fmaf_rn(pv, wd, gv);        // grad.add(param, alpha=wd)
     sv = __fmaf_rn(gv, gv, sv);                       // state_sum.addcmul_(grad, grad, value=1)
     const float std_ = __fadd_rn(__fsqrt_rn(sv), eps);  // sqrt().add_(eps)

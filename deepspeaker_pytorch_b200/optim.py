@@ -6,9 +6,12 @@ The reference builds ``torch.optim.Adagrad(model.parameters(), lr=0.1, lr_decay=
 ``param_groups``) but lays parameters, gradients and the running sum of squares out as three flat fp32 buffers with the
 same offsets: ``p.data`` and ``p.grad`` of every parameter become views into them, the data-parallel gradient
 allreduce is a single collective on the gradient buffer, and the update is ONE kernel over 11.6 M elements
-(``dsk_adagrad_step``) that also applies the post-allreduce ``1/world`` (or ``1/sum_k`` for the weighted hard-triplet
-branch) — instead of ~6 foreach kernels over 38 tensors.  Same operation order as torch's foreach Adagrad: results
-are bit-identical to ``torch.optim.Adagrad`` (tests/test_gpu_optim.py).
+(``dsk_adagrad_step``) that also applies the post-allreduce division by ``world`` (or by ``max(sum_k, 1e-30)`` for the
+weighted hard-triplet branch, ``GradBucket.allreduce_weighted_mean``'s arithmetic) — instead of ~6 foreach kernels
+over 38 tensors.  Same operation order as torch's foreach Adagrad: the parameters and sums are bit-identical to
+``torch.optim.Adagrad`` (CUDA, foreach) stepping on the summed gradient divided by that divisor as a CUDA tensor
+(tests/test_gpu_fp32_head_ops.py, tests/test_gpu_head.py).  ``GradBucket.allreduce_mean`` divides BEFORE its sum, as
+DDP's default hook does; at world sizes that are not powers of two it differs from this step in the last bit.
 """
 from __future__ import annotations
 
@@ -83,11 +86,11 @@ class FusedAdagrad:
         self.step_count += 1
         world = dist.get_world_size(self.group) if (dist.is_available() and dist.is_initialized()) else 1
         denom = self._grad_ext[self.numel:self.numel + 1] if self._weighted else None
-        mult = 1.0 if self._weighted else 1.0 / world
+        div = 1.0 if self._weighted else float(world)
         with torch.cuda.device(self.device):
             L.check(L.load().dsk_adagrad_step(self.flat_param.data_ptr(), self.flat_grad.data_ptr(), self.flat_sum.data_ptr(),
                                               self.numel, float(g["lr"]), float(g["lr_decay"]), float(g["weight_decay"]),
-                                              float(g["eps"]), self.step_count, mult, L.ptr(denom), L.cur_stream()),
+                                              float(g["eps"]), self.step_count, div, L.ptr(denom), L.cur_stream()),
                     "dsk_adagrad_step")
         # the kernel wrote through raw pointers: tell autograd / the engine's repack check that the parameters changed
         torch.autograd.graph.increment_version(self.params)

@@ -541,21 +541,27 @@ int32_t dsk_linear_backward(const float* x, const float* w, const float* gy, int
                             float* gw, float* gb, void* stream);
 /* nn.CrossEntropyLoss() over (M,C) logits and int64 labels (reference train_triplet.py:281-285):
  * loss (1,) = mean_i (logsumexp_j logits[i] - logits[i][label_i]); also writes lse (M,) and row_loss (M,) (workspace
- * the backward reads).  A label outside [0,C) yields NaN. */
+ * the backward reads).  A label outside [0,C) yields a NaN row loss, so a NaN loss; the other rows are unaffected. */
 int32_t dsk_cross_entropy(const float* logits, const int64_t* labels, int32_t M, int32_t C, float* loss, float* lse,
                           float* row_loss, void* stream);
-/* dlogits (M,C) = (softmax(logits) - onehot(labels)) * grad_loss / M; grad_loss is a device scalar. */
+/* dlogits (M,C) = (softmax(logits) - onehot(labels)) * grad_loss / M; grad_loss is a device scalar.  The row of a
+ * label outside [0,C) is all NaN, so an invalid example cannot train the parameters silently. */
 int32_t dsk_cross_entropy_bwd(const float* logits, const int64_t* labels, const float* lse, const float* grad_loss,
                               int32_t M, int32_t C, float* dlogits, void* stream);
 
 /* torch.optim.Adagrad step (reference train_triplet.py:369-383, called at :224,291) on ONE flat bucket of n fp32
  * elements (parameters, gradients and the running sum of squares laid out identically), fused with the gradient scale
- * that follows the data-parallel allreduce:  g = grad * grad_mult (/ *grad_denom if non-NULL, a device scalar);
- * g += weight_decay * p;  sum = fma(g, g, sum);  p += (g * -clr) / (sqrt(sum) + eps),  clr = lr / (1 + (step-1) lr_decay).
- * `step` counts from 1.  Operation order = torch's foreach Adagrad, so the result is bit-identical to it.
- * Buffers must be 16-byte aligned. */
+ * that follows the data-parallel allreduce.  Per element, each step rounded to fp32:
+ *   g = grad / grad_div                        (skipped when grad_div == 1; grad_div > 0, e.g. the world size)
+ *   g = g / max(*grad_denom, 1e-30)            (only if grad_denom is non-NULL, a device scalar; NaN propagates)
+ *   g = fma(p, weight_decay, g)                (skipped when weight_decay == 0)
+ *   sum = fma(g, g, sum);  p = p + (g * -clr) / (sqrt(sum) + eps)
+ * where -clr = -lr / (1 + (step-1) lr_decay) is computed in double and rounded once to fp32.
+ * `step` counts from 1.  After the divisions this is the operation order of torch's foreach Adagrad on CUDA: the
+ * result is bit-identical to torch.optim.Adagrad stepping on grad.div(d) with d a CUDA tensor (a true division; ATen
+ * turns division by a CPU scalar into a product with its reciprocal).  Buffers must be 16-byte aligned. */
 int32_t dsk_adagrad_step(float* param, const float* grad, float* state_sum, int64_t n, double lr, double lr_decay,
-                         double weight_decay, double eps, int64_t step, float grad_mult, const float* grad_denom,
+                         double weight_decay, double eps, int64_t step, float grad_div, const float* grad_denom,
                          void* stream);
 
 /* Serving pipeline for the reference's test() loop (reference train_triplet.py:337-350: batch to the GPU, model(x),
