@@ -60,7 +60,10 @@ struct HaloParams {
   int plain3x3;           // MMA issuer plan: 1 = 3x3 (HaloPlan<1>), 2 = planar 5x5 s2 (HaloPlan<2>), 0 = walk the tables
   int late_trigger;       // release the dependent kernel when this CTA starts its last tile instead of at entry
   int b_resident;         // all weight boxes of a CTA's channel tile fit the B ring: load once
-  unsigned pitch_magic, img_magic;  // floor(2^32/d)+1 for d = W+1 and H+1: q/d == __umulhi(q, magic) for q < 2^32/d
+  // floor(2^64/d)+1 for d = W+1 and H+1: q/d == __umul64hi(q, magic) for every q < 2^32 (the error of the rounded-up
+  // reciprocal, q (magic d - 2^64) / (d 2^64) < q / 2^64, stays below 1/d).  A 32-bit reciprocal is exact only for
+  // q < 2^32/d, which the image index R / (H+1) of a long batch of long utterances passes.
+  unsigned long long pitch_magic, img_magic;
   // stream-K (DESIGN.md): a layer of this network has 1.3-2.4 tiles per SM, so whole-tile scheduling leaves 20-36 % of
   // the SM-time of stages 2-4 idle in the last wave.  With stream_k the K loop of the layer (tiles x chunks x weight
   // boxes "units") is cut into gridDim.x EQUAL contiguous ranges: a CTA's range covers the tail of one tile, whole
@@ -509,9 +512,9 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
       // padded position q0 + row: junk (a pad position) or, for a parity-planar output, its destination (nullptr = junk)
       auto is_junk = [&](int row, int& R, int& cc, int& img) -> bool {
         const int q = q0 + row;
-        R = static_cast<int>(__umulhi(static_cast<unsigned>(q), p.pitch_magic));
+        R = static_cast<int>(__umul64hi(static_cast<unsigned>(q), p.pitch_magic));
         cc = q - R * pitch;
-        img = static_cast<int>(__umulhi(static_cast<unsigned>(R), p.img_magic));
+        img = static_cast<int>(__umul64hi(static_cast<unsigned>(R), p.img_magic));
         return (cc == 0) || (R - img * (p.H + 1) == 0) || (R >= rows_real_end);
       };
       // parity-planar destination of a position (only when the consumer is a stride-2 conv): pixel (n, h, w) ->

@@ -850,9 +850,12 @@ int build_halo(const dsk_handle_s* h, HaloLaunch* L, const void* in, const void*
   }
   p.trace = h->trace;
   p.late_trigger = h->late_trigger ? 1 : 0;
-  p.pitch_magic = static_cast<unsigned>((1ull << 32) / static_cast<unsigned>(W + 1)) + 1u;
-  p.img_magic = static_cast<unsigned>((1ull << 32) / static_cast<unsigned>(H + 1)) + 1u;
+  p.pitch_magic = static_cast<unsigned long long>((static_cast<unsigned __int128>(1) << 64) / static_cast<unsigned>(W + 1)) + 1ull;
+  p.img_magic = static_cast<unsigned long long>((static_cast<unsigned __int128>(1) << 64) / static_cast<unsigned>(H + 1)) + 1ull;
   const long npos = padded_positions(N, H, W);
+  // the kernel's positions, tile indices and TMA row coordinates are 32-bit signed (four planes for the 5x5 input)
+  if (npos * (ksize == 5 ? 4 : 1) >= (1l << 31))
+    return fail(DSK_ERR_INVALID, "halo conv: %ld padded positions exceed 32-bit indexing (N %d, H %d, W %d)", npos, N, H, W);
   int ntaps_total;
   if (ksize == 3) {
     ntaps_total = 9;

@@ -95,6 +95,11 @@ int32_t dsk_share_weights(dsk_handle h, dsk_handle src);
 /* DeepSpeakerModel.forward (reference model.py:185-218), BN in eval mode
  * (train_triplet.py:332,347): x (B,1,T,64) fp32 contiguous -> emb (B,E) fp32 with ||emb||=10.
  * T must be a multiple of 16.
+ * An utterance's embedding, and every activation of it, has the same bits whatever else is in the batch (its size,
+ * order and content) under the default whole-tile scheduling; DSK_STREAM_K=1 cuts each tile's K loop where the tile
+ * count puts it, which can move the last bits.  Nothing else bounds B and T: the workspace grows with B * T (130 MiB at
+ * 64 x 160), and the halo convs' 32-bit position arithmetic is exact for every shape whose workspace fits in 80 GiB (a
+ * layer past 2^31 padded positions fails with DSK_ERR_INVALID).
  * Asynchronous on `stream`, with one exception that synchronises the DEVICE: the first forward after
  * dsk_load_weights (the folded BN affine is copied to the host and baked into the conv kernels' parameter block).
  * The first call of a new (B, T) shape rebuilds the plan and re-zeroes the padded activation workspace with a

@@ -55,6 +55,14 @@ def test_eval_forward_matches_oracle(models, B, T):
     assert (e - ref).abs().max().item() < 3e-3 * 10 / 512 ** 0.5
 
 
+def _stream_k_env():
+    """Whether handles created now schedule the halo convs stream-K (dsk_create reads DSK_STREAM_K; off by default)."""
+    try:
+        return int(os.environ.get("DSK_STREAM_K", "0")) != 0
+    except ValueError:
+        return False
+
+
 def test_full_size_properties(models):
     """BASELINE configs[1] size: determinism, unit-10 norms, batch-composition invariance (eval BN)."""
     sd, ms = models
@@ -67,12 +75,14 @@ def test_full_size_properties(models):
         assert torch.allclose(e1.norm(dim=1), torch.full((64,), 10.0, device=x.device), atol=1e-3)
         perm = torch.randperm(64, device=x.device)
         ep = m(x[perm].contiguous())
-        # each utterance is independent of its batch (eval BN).  Under stream-K scheduling the place where a tile's K loop
-        # is cut depends on the batch size and the tile index, so fp32 partial sums associate differently: a last-bit
-        # difference that the 16-bit activation storage occasionally turns into one fp16 ulp (<= 5e-5 of the norm)
-        assert torch.allclose(ep, e1[perm], atol=5e-4)
+        # each utterance is independent of its batch (eval BN), bit for bit under whole-tile scheduling (the default).
+        # Under stream-K the place where a tile's K loop is cut depends on the batch size and the tile index, so fp32
+        # partial sums associate differently: a last-bit difference that the 16-bit activation storage occasionally
+        # turns into one fp16 ulp (<= 5e-5 of the norm)
+        same = (lambda a, b: torch.allclose(a, b, atol=5e-4)) if _stream_k_env() else torch.equal
+        assert same(ep, e1[perm])
         e_small = m(x[5:8].contiguous())
-        assert torch.allclose(e_small, e1[5:8], atol=5e-4)
+        assert same(e_small, e1[5:8])
         assert torch.isfinite(m(torch.full_like(x, 1e4))).all()       # clip at 20 keeps everything finite
 
 

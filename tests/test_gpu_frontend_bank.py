@@ -248,7 +248,7 @@ def test_embed_utterances_against_an_fp64_mean(cuda_dev, case):
         err = np.abs(got.cpu().double().numpy() - ref)
         assert (err <= ulp).all(), (batch, (err / ulp).max())
         out[batch] = got
-    print(f"\n{case}: batch 7 vs 256 bit-identical: {_bits_equal(out[7], out[256])}, "
-          f"max |diff| {(out[7] - out[256]).abs().max().item():.3e}")
+    assert _bits_equal(out[7], out[256]), (f"{case}: batch 7 vs 256 differ, "
+                                           f"max |diff| {(out[7] - out[256]).abs().max().item():.3e}")
     with pytest.raises(RuntimeError):
         F.embed_utterances(model.train(), bank, utt)
