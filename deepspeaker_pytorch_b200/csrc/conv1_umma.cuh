@@ -169,8 +169,8 @@ conv1_umma_kernel(const __grid_constant__ CUtensorMap tmX, const uint4* __restri
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const int row = 64 * m + fr + 8 * h, c = 8 * g + fc;
-            const float f0 = fminf(fmaxf(fmaf(acc[m][4 * g + 2 * h], s_scale[c], s_bias[c]), 0.0f), clip_hi);
-            const float f1 = fminf(fmaxf(fmaf(acc[m][4 * g + 2 * h + 1], s_scale[c + 1], s_bias[c + 1]), 0.0f), clip_hi);
+            const float f0 = relu_clip(fmaf(acc[m][4 * g + 2 * h], s_scale[c], s_bias[c]), clip_hi);
+            const float f1 = relu_clip(fmaf(acc[m][4 * g + 2 * h + 1], s_scale[c + 1], s_bias[c + 1]), clip_hi);
             *reinterpret_cast<uint32_t*>(stage + sw128_off16(row, c)) = pack2<BF16>(f0, f1);
           }
       __syncthreads();

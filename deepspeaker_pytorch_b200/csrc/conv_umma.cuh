@@ -288,8 +288,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 f1 += t.y;
               }
               if (do_clip) {
-                f0 = fminf(fmaxf(f0, 0.0f), p.clip_hi);
-                f1 = fminf(fmaxf(f1, 0.0f), p.clip_hi);
+                f0 = relu_clip(f0, p.clip_hi);
+                f1 = relu_clip(f1, p.clip_hi);
               }
               *reinterpret_cast<uint32_t*>(stg + off) = pack2<BF16>(f0, f1);
             }

@@ -2665,7 +2665,7 @@ int32_t dsk_batch_hard_select_rows(dsk_handle h, const float* E, const int64_t* 
                                                                        allpairs_unit_roundoff(h), neg_idx, d_an);
     KERNEL_CHECK();
     dsk::batch_hard_positive_kernel<false><<<blocks, 256, 0, s>>>(E, nullptr, labels, N, row0, rows, D, eps, pos_idx,
-                                                                   d_ap, valid);
+                                                                   d_ap, d_an, valid);
     KERNEL_CHECK();
   } else {  // exact CUDA-core rows x N distance matrix (the same bits)
     float* S = nullptr;
@@ -2675,7 +2675,8 @@ int32_t dsk_batch_hard_select_rows(dsk_handle h, const float* E, const int64_t* 
     KERNEL_CHECK();
     dsk::topk_rows_kernel<<<blocks, 256, 0, s>>>(S, labels, N, row0, rows, eps, 1, neg_idx, d_an);
     KERNEL_CHECK();
-    dsk::batch_hard_positive_kernel<true><<<blocks, 256, 0, s>>>(E, S, labels, N, row0, rows, D, eps, pos_idx, d_ap, valid);
+    dsk::batch_hard_positive_kernel<true><<<blocks, 256, 0, s>>>(E, S, labels, N, row0, rows, D, eps, pos_idx, d_ap, d_an,
+                                                                  valid);
     KERNEL_CHECK();
     CUDA_TRY(cudaFreeAsync(S, s));
   }

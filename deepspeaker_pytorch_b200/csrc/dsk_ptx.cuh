@@ -266,18 +266,32 @@ __device__ __forceinline__ uint32_t pack2(float a, float b) {
     return *reinterpret_cast<uint32_t*>(&v);
   }
 }
+// NaN-propagating fp32 max / min (max.NaN / min.NaN, FMNMX.NAN): NaN when either operand is NaN, as torch.clamp,
+// Hardtanh and numpy.maximum give, where fmaxf / fminf return the other operand.  Otherwise the bits of fmaxf / fminf.
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+__device__ __forceinline__ float fmin_nan(float a, float b) {
+  float r;
+  asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+// clamp(x, 0, hi), NaN in -> NaN out (the reference's Hardtanh(0, 20))
+__device__ __forceinline__ float relu_clip(float x, float hi) { return fmin_nan(fmax_nan(x, 0.0f), hi); }
 // clamp both 16-bit halves of a packed pair to [lo, hi] (lo / hi packed the same way).  Identical to clamping in fp32
-// before the pack when lo and hi are exactly representable: rounding is monotonic, and like fminf / fmaxf the packed
-// min / max return the non-NaN operand.
+// before the pack when lo and hi are exactly representable: rounding is monotonic, and like relu_clip the packed
+// NaN-propagating min / max keep a NaN half NaN.
 template <bool BF16>
 __device__ __forceinline__ uint32_t clip2(uint32_t v, uint32_t lo, uint32_t hi) {
   if constexpr (BF16) {
     __nv_bfloat162 x = *reinterpret_cast<__nv_bfloat162*>(&v);
-    x = __hmin2(__hmax2(x, *reinterpret_cast<__nv_bfloat162*>(&lo)), *reinterpret_cast<__nv_bfloat162*>(&hi));
+    x = __hmin2_nan(__hmax2_nan(x, *reinterpret_cast<__nv_bfloat162*>(&lo)), *reinterpret_cast<__nv_bfloat162*>(&hi));
     return *reinterpret_cast<uint32_t*>(&x);
   } else {
     __half2 x = *reinterpret_cast<__half2*>(&v);
-    x = __hmin2(__hmax2(x, *reinterpret_cast<__half2*>(&lo)), *reinterpret_cast<__half2*>(&hi));
+    x = __hmin2_nan(__hmax2_nan(x, *reinterpret_cast<__half2*>(&lo)), *reinterpret_cast<__half2*>(&hi));
     return *reinterpret_cast<uint32_t*>(&x);
   }
 }

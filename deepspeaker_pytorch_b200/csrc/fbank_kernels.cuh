@@ -11,6 +11,8 @@
 #pragma once
 #include <stdint.h>
 
+#include "dsk_ptx.cuh"
+
 namespace dsk {
 
 constexpr int kFbNfft = 512;
@@ -90,7 +92,7 @@ fbank_kernel(const float* __restrict__ audio_all, const int64_t* __restrict__ so
     float acc = 0.f;
     for (int k = 0; k < kFbBins; ++k) acc = fmaf(pspec[g][k], w[k], acc);
     if (acc == 0.f) acc = 2.220446049250313e-16f;           // numpy.finfo(float).eps, as fbank() substitutes
-    if (log_scale) acc = 20.0f * log10f(fmaxf(acc, log_floor));
+    if (log_scale) acc = 20.0f * log10f(fmax_nan(acc, log_floor));   // a NaN frame stays NaN, as numpy.maximum
     rowfeat[g][t] = live ? acc : 0.f;
     if (live) feat[static_cast<long>(f) * kFbFilters + t] = acc;
   }

@@ -65,7 +65,7 @@ __global__ void hinge_mean_kernel(const float* __restrict__ d_p, const float* __
                                   float* __restrict__ loss) {
   __shared__ float red[1024];
   float s = 0.f;
-  for (int i = threadIdx.x; i < B; i += blockDim.x) s += fmaxf((margin + d_p[i]) - d_n[i], 0.f);
+  for (int i = threadIdx.x; i < B; i += blockDim.x) s += fmax_nan((margin + d_p[i]) - d_n[i], 0.f);
   red[threadIdx.x] = s;
   __syncthreads();
   for (int o = blockDim.x >> 1; o > 0; o >>= 1) {
@@ -487,27 +487,36 @@ allpairs_select_refine_kernel(const float* __restrict__ E, const float* __restri
 
 // Hardest positive, one warp per anchor: argmax over j != i with labels[j] == labels[i] of the exact distance, ties ->
 // lower j (FROM_S: sqrt(S[i][j] + eps) from allpairs_sqdist_kernel, else exact_dist_seq; the two are the same bits).
-// pos_idx = -1 and d_ap = 0 when the anchor has no positive.  valid[i] = 1 iff it has a positive and a negative.
+// A NaN distance is never selected.  pos_idx = -1 and d_ap = 0 when the anchor has no positive.  valid[i] = 1 iff it
+// has a positive and a negative.
+// An anchor whose row holds a NaN or an infinity gets d_ap = d_an = NaN and valid[i] = 1 iff another row has its label
+// and one has another label, so the loss is NaN, as torch's would be; its indices stay those of the scans (the hinge
+// NaN >= 0 is false: the backward never reads them).  Runs after the negative's kernel on the stream, whose d_an it
+// overwrites for those anchors.
 // Anchors row0 + i for i < rows; S (rows x N) and the outputs are indexed by the local row i, column indices are global.
 template <bool FROM_S>
 __global__ void __launch_bounds__(256)
 batch_hard_positive_kernel(const float* __restrict__ E, const float* __restrict__ S, const int64_t* __restrict__ labels,
                            int N, int row0, int rows, int D, float eps, int64_t* __restrict__ pos_idx,
-                           float* __restrict__ d_ap, uint8_t* __restrict__ valid) {
+                           float* __restrict__ d_ap, float* __restrict__ d_an, uint8_t* __restrict__ valid) {
   const int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (i >= rows) return;
   const int row = row0 + i;
   const int lane = threadIdx.x & 31;
   const int64_t my_label = labels[row];
+  bool nonfinite = false;
+  for (int d = lane; d < D; d += 32) nonfinite |= !isfinite(E[static_cast<long>(row) * D + d]);
+  nonfinite = __any_sync(0xffffffffu, nonfinite);
   float bv = -1.f;  // below every distance (>= sqrt(eps) > 0)
   int bj = 0x7fffffff;
-  bool has_neg = false;
+  bool has_neg = false, has_same = false;
   for (int j = lane; j < N; j += 32) {
     if (labels[j] != my_label) {
       has_neg = true;
       continue;
     }
     if (j == row) continue;
+    has_same = true;
     const float v = FROM_S ? sqrtf(S[static_cast<long>(i) * N + j] + eps)
                            : exact_dist_seq(E + static_cast<long>(row) * D, E + static_cast<long>(j) * D, D, eps);
     if (v > bv) {  // each lane scans ascending j: strict > keeps the lower index of a tie
@@ -524,16 +533,18 @@ batch_hard_positive_kernel(const float* __restrict__ E, const float* __restrict_
     }
   }
   has_neg = __any_sync(0xffffffffu, has_neg);
+  has_same = __any_sync(0xffffffffu, has_same);
   if (lane == 0) {
     const bool has_pos = bj != 0x7fffffff;
     pos_idx[i] = has_pos ? bj : -1;
-    d_ap[i] = has_pos ? bv : 0.f;
-    valid[i] = (has_pos && has_neg) ? 1 : 0;
+    d_ap[i] = nonfinite ? __int_as_float(0x7fffffff) : has_pos ? bv : 0.f;
+    if (nonfinite) d_an[i] = __int_as_float(0x7fffffff);
+    valid[i] = ((nonfinite ? has_same : has_pos) && has_neg) ? 1 : 0;
   }
 }
 
 // loss = (1/V) sum over valid anchors of clamp(margin + d_ap - d_an, 0), V = number of valid anchors (loss 0 when
-// V = 0).  Single block of 1024 threads, the order of hinge_mean_kernel: strided partial sums, then a halving tree.
+// V = 0).  The clamp keeps NaN.  Single block of 1024 threads, the order of hinge_mean_kernel: strided partial sums, then a halving tree.
 __global__ void __launch_bounds__(1024)
 batch_hard_mean_kernel(const float* __restrict__ d_ap, const float* __restrict__ d_an,
                        const uint8_t* __restrict__ valid, int N, float margin, float* __restrict__ loss) {
@@ -543,7 +554,7 @@ batch_hard_mean_kernel(const float* __restrict__ d_ap, const float* __restrict__
   int c = 0;
   for (int i = threadIdx.x; i < N; i += blockDim.x)
     if (valid[i]) {
-      s += fmaxf((margin + d_ap[i]) - d_an[i], 0.f);
+      s += fmax_nan((margin + d_ap[i]) - d_an[i], 0.f);
       ++c;
     }
   red[threadIdx.x] = s;

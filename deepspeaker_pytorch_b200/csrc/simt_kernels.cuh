@@ -153,8 +153,8 @@ conv1_kernel(const float* __restrict__ x, const float* __restrict__ w /*[64][25]
       float a0 = fmaf(a[q][0], s0, b0);
       float a1 = fmaf(a[q][1], s1, b1);
       if (do_clip) {
-        a0 = fminf(fmaxf(a0, 0.f), clip_hi);
-        a1 = fminf(fmaxf(a1, 0.f), clip_hi);
+        a0 = relu_clip(a0, clip_hi);
+        a1 = relu_clip(a1, clip_hi);
       }
       if constexpr (OUT_F32)
         reinterpret_cast<float2*>(out)[(pix0 + ow + q) * 32 + lane] = make_float2(a0, a1);

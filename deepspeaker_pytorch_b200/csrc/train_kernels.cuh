@@ -267,7 +267,7 @@ bn_apply_kernel(const float* __restrict__ raw, const float* __restrict__ scale, 
       for (int e = 0; e < 8; ++e) f[e] += r[e];
     }
 #pragma unroll
-    for (int e = 0; e < 8; ++e) f[e] = fminf(fmaxf(f[e], 0.f), clip_hi);
+    for (int e = 0; e < 8; ++e) f[e] = relu_clip(f[e], clip_hi);
     *reinterpret_cast<uint4*>(y + m * C + c0) = pack8<BF16>(f);
   }
 }

@@ -100,6 +100,12 @@ int32_t dsk_share_weights(dsk_handle h, dsk_handle src);
  * count puts it, which can move the last bits.  Nothing else bounds B and T: the workspace grows with B * T (130 MiB at
  * 64 x 160), and the halo convs' 32-bit position arithmetic is exact for every shape whose workspace fits in 80 GiB (a
  * layer past 2^31 padded positions fails with DSK_ERR_INVALID).
+ * Non-finite input: a NaN or +-inf element of x makes that utterance's embedding all NaN (every activation is NaN
+ * exactly where a conv window reaches it, in every channel; the clamps keep NaN, as Hardtanh does) and leaves every
+ * other utterance's bits unchanged; pads stay +0.  conv1 splits x into 16-bit halves x_hi + x_lo, so the finite input
+ * range is per operand type: fp16 |x| < 65520 (past it x_hi is inf and the element acts as a NaN), bf16 every finite
+ * fp32.  An infinite element gives NaN too, where the reference's fp32 conv would carry +-inf into its clamp.  A NaN
+ * running statistic makes every embedding NaN, as nn.BatchNorm2d in eval does.
  * Asynchronous on `stream`, with one exception that synchronises the DEVICE: the first forward after
  * dsk_load_weights (the folded BN affine is copied to the host and baked into the conv kernels' parameter block).
  * The first call of a new (B, T) shape rebuilds the plan and re-zeroes the padded activation workspace with a
@@ -114,7 +120,9 @@ int32_t dsk_rescnn_forward(dsk_handle h, const float* x, int32_t B, int32_t T, f
 /* DeepSpeakerModel.forward with the module in train mode (train_triplet.py:203,215): BatchNorm uses the batch
  * statistics of THIS call (the reference forwards a, p and n separately, so statistics are per call) and updates
  * running_mean / running_var in place (momentum 0.1, unbiased variance).  Saves activations in *ctx for
- * dsk_rescnn_backward; x must stay alive until then.  Contexts are pooled inside the handle. */
+ * dsk_rescnn_backward; x must stay alive until then.  Contexts are pooled inside the handle.
+ * A non-finite element of any utterance makes the batch statistics NaN, so every embedding of the call and the running
+ * statistics become NaN, as in torch; nothing is clamped back to a number. */
 int32_t dsk_rescnn_forward_train(dsk_handle h, const float* x, int32_t B, int32_t T, float* emb, dsk_train_ctx* ctx,
                                  void* stream);
 /* Several train-mode forwards of one step in flight at once (DeepSpeakerModel.forward_triplet runs the anchor / positive /
@@ -270,7 +278,9 @@ int32_t dsk_pairwise_distance_bwd(const float* x1, const float* x2, const float*
                                   int32_t B, int32_t D, float* grad_x1, float* grad_x2, void* stream);
 
 /* TripletMarginLoss(margin).forward (reference model.py:19-33):
- * loss = mean(clamp(margin + d_p - d_n, 0)). Writes loss (1,), d_p (B,), d_n (B,). */
+ * loss = mean(clamp(margin + d_p - d_n, 0)). Writes loss (1,), d_p (B,), d_n (B,).  As torch.clamp, the clamp keeps
+ * NaN: a row with a NaN or an infinity gives the reference's non-finite loss (NaN, or +inf for an infinite d_p; an
+ * infinite d_n alone clamps to 0).  The backward passes the gradient where the hinge is >= 0, false for NaN. */
 int32_t dsk_triplet_loss(const float* a, const float* p, const float* n, int32_t B, int32_t D, float margin,
                          float* loss, float* d_p, float* d_n, void* stream);
 /* Gradients of the loss w.r.t. a, p, n scaled by grad_loss (device scalar). */
@@ -304,6 +314,9 @@ int32_t dsk_allpairs_topk(const float* E, const int64_t* labels, int32_t N, int3
  * argmin d(i,j) over labels[j] != labels[i], ties to the lower j; d_ap, d_an those distances (-1 / 0 when there is no
  * positive, -1 / +inf when there is no negative); valid[i] = 1 iff both exist (depends on the labels only).
  * loss (1,) = (1/V) sum over valid i of clamp(margin + d_ap - d_an, 0) in a fixed order, V = #valid; 0 when V = 0.
+ * Non-finite rows: a NaN distance is never selected (an infinite one is, with the same tie rule).  An anchor whose row
+ * holds a NaN or an infinity gets d_ap = d_an = NaN, keeps the indices of the scans, and is valid iff its label has
+ * another row and another label exists: the loss is NaN, and its hinge passes no gradient.
  * h != NULL and D % 64 == 0: the Gram plan of dsk_allpairs_topk_tc (cached in h, fp16 or bf16 per h) with exact fp32
  * refinement; otherwise (h may be NULL) the exact CUDA-core all-pairs matrix.  Both give the same bits.
  * 2 <= N <= DSK_BATCH_HARD_MAX_N (the N x N fp32 distance matrix, 1 GiB at the limit). */
@@ -595,7 +608,10 @@ int32_t dsk_pipeline_lane_stream(dsk_pipeline p, int32_t lane, void** stream_out
  * device; feat: (dsk_fbank_num_frames(n_samples, sample_rate), 64) fp32 row-major, the (T, 64) layout the network's input
  * is cropped from.  python_speech_features is not vendored in the reference (parity against it unpinned): its published
  * algorithm is restated (pre-emphasis 0.97, 25 ms / 10 ms rectangular frames, NFFT 512, |rfft|^2 / NFFT, triangular mel
- * filters, zeros -> eps). */
+ * filters, zeros -> eps).  A NaN or infinite sample makes every frame whose pre-emphasised window covers it (the
+ * sample and the next) NaN in all 64 filters, log floor included, as numpy.maximum does; with subtract_mean the
+ * utterance's mean, so all its features, are NaN.  This holds for dsk_fbank_batch (the other utterances keep their
+ * bits) and dsk_fbank_segments (so an example dsk_wave_augment made NaN is all NaN). */
 int64_t dsk_fbank_num_frames(int64_t n_samples, int32_t sample_rate);
 int32_t dsk_fbank(const float* audio, int64_t n_samples, int32_t sample_rate, int32_t log_scale, int32_t subtract_mean,
                   float* feat, void* stream);

@@ -1,7 +1,8 @@
 """Oracles of the batch-hard triplet loss — TEST INFRASTRUCTURE ONLY (the product never imports this module).
 
 * ``batch_hard_triplet``: ctypes wrapper of oracle/batch_hard_oracle.c, the step-by-step fp32 restatement of the
-  selection, its tie rules and the fixed-order mean (bit-exact target of dsk_batch_hard_triplet).
+  selection, its tie rules, the rule for non-finite rows (NaN distances for the anchor, a NaN loss) and the
+  fixed-order mean (bit-exact target of dsk_batch_hard_triplet).
 * ``batch_hard_loss``: fp64-capable torch-autograd restatement of the loss with the selection GIVEN, for gradient
   checks (the selection is piecewise constant in E, so the gradient is taken with the engine's choice pinned).
 
