@@ -23,6 +23,9 @@ DSK_EVAL, DSK_TRAIN = 0, 1
 DSK_GE2E_SOFTMAX, DSK_GE2E_CONTRAST = 0, 1
 DSK_LINKAGE_AVERAGE, DSK_LINKAGE_COMPLETE = 0, 1
 DSK_AHC_MAX_N = 32768
+DSK_NORM_NONE, DSK_NORM_LENGTH, DSK_NORM_PLDA = 0, 1, 2
+DSK_F64_MAX_DIM = 4096
+DSK_PLDA_MAX_ROWS = 4194240
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -207,6 +210,15 @@ SIGNATURES = {
     "dsk_class_centroids": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),
     "dsk_ahc": (c_int32, [c_void_p, c_int32, c_int64, c_int32, c_int32, c_double, c_void_p, POINTER(c_int32), c_void_p,
                           POINTER(c_int32), c_void_p]),
+    "dsk_class_sums_f64": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
+                                     c_void_p]),
+    "dsk_gram_f64": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
+    "dsk_affine_norm_f64": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_void_p,
+                                      c_void_p, c_void_p, c_void_p]),
+    "dsk_plda_score_trials": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
+                                        c_void_p]),
+    "dsk_plda_score_matrix": (c_int32, [c_void_p, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_int64,
+                                        c_void_p]),
     "dsk_linear_forward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     "dsk_linear_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p,
                                       c_void_p, c_void_p]),

@@ -28,6 +28,7 @@
 #include "head_kernels.cuh"
 #include "loss_kernels.cuh"
 #include "metric_kernels.cuh"
+#include "plda_kernels.cuh"
 #include "score_kernels.cuh"
 #include "simt_kernels.cuh"
 #include "train_kernels.cuh"
@@ -3283,6 +3284,111 @@ int32_t dsk_class_centroids(const float* X, int32_t U, int32_t D, const int64_t*
   dsk::class_centroids_kernel<<<dim3(S, (D + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(X, U, D, order,
                                                                                                        offsets, out);
   KERNEL_CHECK();
+  return DSK_OK;
+}
+
+// ---- PLDA backend: fit statistics, transforms, LLR scoring --------------------------------------------------------
+int32_t dsk_class_sums_f64(const float* X, int64_t N, int32_t D, const int64_t* order, const int64_t* offsets,
+                           int32_t C, const double* mu, double* out, void* stream) {
+  if (!X || !order || !offsets || !out || N < 1 || D < 1 || C < 1)
+    return fail(DSK_ERR_INVALID, "dsk_class_sums_f64: bad arguments (need non-null X, order, offsets and out, N >= 1, "
+                "D >= 1, C >= 1; got N %lld, D %d, C %d)", static_cast<long long>(N), D, C);
+  dsk::class_sums_f64_kernel<<<dim3(C, (D + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      X, static_cast<long long>(N), D, order, offsets, mu, out);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_gram_f64(const float* X, int64_t N, int32_t D, const double* mu, double* G, void* stream) {
+  if (!X || !G || N < 1 || D < 1 || D > DSK_F64_MAX_DIM)
+    return fail(DSK_ERR_INVALID, "dsk_gram_f64: bad arguments (need non-null X and G, N >= 1, 1 <= D <= %d; got N %lld, "
+                "D %d)", DSK_F64_MAX_DIM, static_cast<long long>(N), D);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // split-K over rows: a function of (N, D) only, so the partials and their fixed-order sum are too
+  const long long tiles = (D + dsk::kF64Tile - 1) / dsk::kF64Tile, nt = tiles * (tiles + 1) / 2;
+  const long long kblocks = (N + dsk::kF64K - 1) / dsk::kF64K;
+  long long splits = std::max(1ll, std::min((dsk::kF64GramCtas + nt - 1) / nt, kblocks));
+  const long long rows_per = (kblocks + splits - 1) / splits * dsk::kF64K;
+  splits = (N + rows_per - 1) / rows_per;
+  double* ws = nullptr;
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&ws),
+                           static_cast<size_t>(splits * nt) * dsk::kF64Tile * dsk::kF64Tile * sizeof(double), s));
+  dsk::gram_f64_kernel<<<dim3(static_cast<unsigned>(nt), static_cast<unsigned>(splits)), dsk::kF64Threads, 0, s>>>(
+      X, static_cast<long long>(N), D, mu, rows_per, ws);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) {
+    dsk::gram_reduce_kernel<<<static_cast<unsigned>(nt), 256, 0, s>>>(ws, D, static_cast<int>(splits), G);
+    e = cudaGetLastError();
+  }
+  const cudaError_t fe = cudaFreeAsync(ws, s);
+  if (e != cudaSuccess) return fail(DSK_ERR_CUDA, "dsk_gram_f64: kernel launch failed: %s", cudaGetErrorString(e));
+  if (fe != cudaSuccess) return fail(DSK_ERR_CUDA, "dsk_gram_f64: cudaFreeAsync failed: %s", cudaGetErrorString(fe));
+  return DSK_OK;
+}
+
+int32_t dsk_affine_norm_f64(const float* X, int64_t N, int32_t D, const double* A, int32_t d, const double* c,
+                            int32_t mode, const double* psi, const int32_t* counts, float* Y, void* stream) {
+  if (!X || !A || !Y || N < 1 || D < 1 || D > DSK_F64_MAX_DIM || d < 1 || d > DSK_F64_MAX_DIM ||
+      (mode != DSK_NORM_NONE && mode != DSK_NORM_LENGTH && mode != DSK_NORM_PLDA) || (mode == DSK_NORM_PLDA && !psi))
+    return fail(DSK_ERR_INVALID, "dsk_affine_norm_f64: bad arguments (need non-null X, A and Y, N >= 1, 1 <= D, d <= %d, "
+                "mode %d, %d or %d, psi non-null in mode %d; got N %lld, D %d, d %d, mode %d)", DSK_F64_MAX_DIM,
+                DSK_NORM_NONE, DSK_NORM_LENGTH, DSK_NORM_PLDA, DSK_NORM_PLDA, static_cast<long long>(N), D, d, mode);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // the fp64 rows go through a workspace of at most 128 MiB, taken in row chunks in order
+  const long long per = std::max<long long>(dsk::kF64Tile, (128ll << 20) / (8ll * d) / dsk::kF64Tile * dsk::kF64Tile);
+  const long long chunk = std::min<long long>(per, (N + dsk::kF64Tile - 1) / dsk::kF64Tile * dsk::kF64Tile);
+  double* Z = nullptr;
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&Z), static_cast<size_t>(chunk) * d * sizeof(double), s));
+  cudaError_t e = cudaSuccess;
+  for (long long r0 = 0; r0 < N && e == cudaSuccess; r0 += chunk) {
+    const long long rows = std::min(chunk, static_cast<long long>(N) - r0);
+    dsk::affine_f64_kernel<<<dim3((d + dsk::kF64Tile - 1) / dsk::kF64Tile,
+                                  static_cast<unsigned>((rows + dsk::kF64Tile - 1) / dsk::kF64Tile)),
+                             dsk::kF64Threads, 0, s>>>(X + r0 * D, rows, D, A, d, c, Z);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) break;
+    dsk::affine_scale_kernel<<<static_cast<unsigned>((rows + dsk::kPldaWarps - 1) / dsk::kPldaWarps), 256, 0, s>>>(
+        Z, rows, d, mode, psi, counts ? counts + r0 : nullptr, Y + r0 * d);
+    e = cudaGetLastError();
+  }
+  const cudaError_t fe = cudaFreeAsync(Z, s);
+  if (e != cudaSuccess) return fail(DSK_ERR_CUDA, "dsk_affine_norm_f64: kernel launch failed: %s", cudaGetErrorString(e));
+  if (fe != cudaSuccess) return fail(DSK_ERR_CUDA, "dsk_affine_norm_f64: cudaFreeAsync failed: %s", cudaGetErrorString(fe));
+  return DSK_OK;
+}
+
+int32_t dsk_plda_score_trials(const float* Y, int32_t U, int32_t d, const double* psi, const int32_t* counts,
+                              const int64_t* trials, int64_t T, float* llr, void* stream) {
+  if (!Y || !psi || !trials || !llr || U < 1 || d < 1 || T < 1 || T > (1ll << 33))
+    return fail(DSK_ERR_INVALID, "dsk_plda_score_trials: bad arguments (need non-null Y, psi, trials and llr, U >= 1, "
+                "d >= 1, 1 <= T <= 2^33; got U %d, d %d, T %lld)", U, d, static_cast<long long>(T));
+  const unsigned blocks = static_cast<unsigned>((T + dsk::kPldaWarps - 1) / dsk::kPldaWarps);
+  dsk::plda_trials_kernel<<<blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(Y, U, d, psi, counts, trials,
+                                                                                 static_cast<long long>(T), llr);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_plda_score_matrix(const float* Ya, int32_t M, const float* Yb, int32_t N, int32_t d, const double* psi,
+                              float* S, int64_t ld, void* stream) {
+  if (!Ya || !Yb || !psi || !S || M < 1 || M > DSK_PLDA_MAX_ROWS || N < 1 || d < 1 || ld < N)
+    return fail(DSK_ERR_INVALID, "dsk_plda_score_matrix: bad arguments (need non-null Ya, Yb, psi and S, 1 <= M <= %d, "
+                "N >= 1, d >= 1, ld >= N; got M %d, N %d, d %d, ld %lld)", DSK_PLDA_MAX_ROWS, M, N, d,
+                static_cast<long long>(ld));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const long long rows = static_cast<long long>(M) + N;
+  double* ws = nullptr;  // [w (d), beta (d), k], then q of Ya's rows and Yb's rows
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&ws), static_cast<size_t>(2 * d + 1 + rows) * sizeof(double), s));
+  double* q = ws + 2 * d + 1;
+  dsk::plda_coef_kernel<<<1, 32, 0, s>>>(psi, d, ws);
+  dsk::plda_q_kernel<<<static_cast<unsigned>((rows + dsk::kPldaWarps - 1) / dsk::kPldaWarps), 256, 0, s>>>(
+      Ya, M, Yb, N, d, ws, q);
+  dsk::plda_matrix_kernel<<<dim3((N + dsk::kF64Tile - 1) / dsk::kF64Tile, (M + dsk::kF64Tile - 1) / dsk::kF64Tile),
+                            dsk::kF64Threads, 0, s>>>(Ya, M, Yb, N, d, ws, q, S, static_cast<long long>(ld));
+  const cudaError_t e = cudaGetLastError();
+  const cudaError_t fe = cudaFreeAsync(ws, s);
+  if (e != cudaSuccess) return fail(DSK_ERR_CUDA, "dsk_plda_score_matrix: kernel launch failed: %s", cudaGetErrorString(e));
+  if (fe != cudaSuccess) return fail(DSK_ERR_CUDA, "dsk_plda_score_matrix: cudaFreeAsync failed: %s", cudaGetErrorString(fe));
   return DSK_OK;
 }
 

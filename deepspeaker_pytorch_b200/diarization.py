@@ -7,6 +7,9 @@ by default), cut at a known number of speakers or at a distance threshold.  Each
 the covering window whose centre is nearest, and runs of equal frame labels become segments.  ``to_rttm`` writes them
 in the RTTM format scoring tools read.
 
+With ``plda`` (a fitted ``plda.PLDA`` backend) the affinity is the PLDA log-likelihood ratio of the windows instead of
+their cosine, as in the Kaldi diarization recipe.
+
 With ``speech`` (an (F,) mask over the bank's rows: ``bank.speech`` from the frame-energy VAD of
 ``FeatureBank.from_waveforms(..., vad={})``, or oracle speech from reference annotations) only speech is diarized: every
 run of speech frames is cut into windows of its own (``FeatureBank.runs``; a run shorter than T gets one window that
@@ -109,7 +112,22 @@ def _smallest_hop(last, rec, R, hop):
     return lo
 
 
-def _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batch):
+def _cluster(E, plda, threshold, linkage, k):
+    """AHC of one recording's window embeddings E: on their cosines, or with a PLDA backend on the LLRs of their
+    transformed rows (a threshold on LLRs s is the threshold 1 - s on ahc's distance 1 - S)."""
+    if plda is None:
+        S = engine.cosine_matrix(E, E)
+    else:
+        Y = plda.transform(E)
+        S = plda.score_matrix(Y, Y)
+        if threshold is not None:
+            threshold = 1.0 - float(threshold)
+    if threshold is not None:
+        return engine.ahc(S, linkage, threshold=threshold)
+    return engine.ahc(S, linkage, num_clusters=k)
+
+
+def _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batch, plda):
     R = u.size
     table, runs, run_off, kept = bank._run_table(speech, u, "diarize")
     rec, first, end = table[:, 0], table[:, 1], table[:, 2]
@@ -140,12 +158,7 @@ def _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batc
         if W == 1:
             wl, Z = np.zeros(1, np.int32), np.zeros((0, 4))
         else:
-            E = emb[a:b]
-            S = engine.cosine_matrix(E, E)
-            if threshold is not None:
-                Z, lab = engine.ahc(S, linkage, threshold=threshold)
-            else:
-                Z, lab = engine.ahc(S, linkage, num_clusters=min(int(ks[r]), W))
+            Z, lab = _cluster(emb[a:b], plda, threshold, linkage, min(int(ks[r]), W) if threshold is None else None)
             wl = lab.cpu().numpy()
         for i in range(r0, r1):
             w0, w1 = int(win_off[i]), int(win_off[i + 1])
@@ -155,7 +168,7 @@ def _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batc
 
 
 def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40, num_speakers=None, threshold=None,
-            linkage: str = "average", batch: int = 256, speech=None) -> list:
+            linkage: str = "average", batch: int = 256, speech=None, plda=None) -> list:
     """Diarize the recordings ``utt`` (indices into ``bank``) -> [Recording] in the order of ``utt``.  Give exactly
     one of ``num_speakers`` (an int, or one per recording; a recording with fewer windows gets one speaker per window)
     and ``threshold`` (a cosine distance 1 - cos: windows merge while the linkage distance is <= threshold), else
@@ -164,7 +177,12 @@ def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40,
 
     ``speech``: None (every frame gets a speaker), or an (F,) bool mask over the bank's rows (CPU or CUDA, such as
     ``bank.speech``): the windows are cut per run of speech frames, non-speech frames are labelled -1 and lie in no
-    segment, and a recording without speech has no windows, no segments and only -1 frames."""
+    segment, and a recording without speech has no windows, no segments and only -1 frames.
+
+    ``plda``: None (the affinity is the windows' cosine), or a fitted ``plda.PLDA``: the affinity is then the PLDA
+    log-likelihood ratio of the transformed window embeddings (``plda.score_matrix(plda.transform(E), ...)``), and
+    ``threshold`` is an LLR: windows merge while the linkage of LLRs is >= threshold (``engine.ahc`` gets
+    1 - threshold, its distance being 1 - S, and ``Z``'s heights are 1 - LLR)."""
     if (num_speakers is None) == (threshold is None):
         raise ValueError("diarize: give exactly one of num_speakers and threshold")
     if linkage not in engine.LINKAGES:
@@ -178,7 +196,7 @@ def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40,
     if num_speakers is not None and any(int(k) < 1 for k in ks):
         raise ValueError(f"diarize: num_speakers must be >= 1, got {num_speakers}")
     if speech is not None:
-        return _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batch)
+        return _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batch, plda)
     _, _, win_off = bank.windows(u, T, hop)
     counts = np.diff(win_off.numpy())
     if counts.max() > MAX_WINDOWS:
@@ -194,12 +212,7 @@ def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40,
         if W == 1:
             wl, Z = np.zeros(1, np.int32), np.zeros((0, 4))
         else:
-            E = emb[a:b]
-            S = engine.cosine_matrix(E, E)
-            if threshold is not None:
-                Z, lab = engine.ahc(S, linkage, threshold=threshold)
-            else:
-                Z, lab = engine.ahc(S, linkage, num_clusters=min(int(ks[r]), W))
+            Z, lab = _cluster(emb[a:b], plda, threshold, linkage, min(int(ks[r]), W) if threshold is None else None)
             wl = lab.cpu().numpy()
         fl = frame_labels(win_start[a:b].numpy(), wl, int(bank.lengths[u[r]]), T)
         out.append(Recording(segments(fl), fl, wl, Z))

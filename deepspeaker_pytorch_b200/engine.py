@@ -767,3 +767,112 @@ def ahc(S, linkage="average", num_clusters=None, threshold=None, return_rounds=F
                                  labels.ctypes.data_as(ctypes.c_void_p), ctypes.byref(rounds), L.cur_stream()), "dsk_ahc")
     out = (Z[:m.value].copy(), torch.from_numpy(labels).to(S.device))
     return out + (rounds.value,) if return_rounds else out
+
+
+# ---------------------------------------------------------------------------------------------------
+# PLDA backend: fp64 fit statistics, transforms, LLR scoring
+# ---------------------------------------------------------------------------------------------------
+NORM_MODES = {"none": L.DSK_NORM_NONE, "length": L.DSK_NORM_LENGTH, "plda": L.DSK_NORM_PLDA}
+
+
+def _f64_vec(v, device, n, what):
+    if v is None:
+        return None
+    v = torch.as_tensor(v).detach().to(device=device, dtype=torch.float64).contiguous()
+    if v.shape != (n,):
+        raise RuntimeError(f"{what}: expected shape ({n},), got {tuple(v.shape)}")
+    return v
+
+
+def _counts(counts, device, n, what):
+    if counts is None:
+        return None
+    c = torch.as_tensor(counts).detach().to(device=device, dtype=torch.int32).contiguous()
+    if c.shape != (n,):
+        raise RuntimeError(f"{what}: expected counts of shape ({n},), got {tuple(c.shape)}")
+    return c
+
+
+def class_sums_f64(X, order, offsets, mu=None):
+    """dsk_class_sums_f64: (C, D) fp64 sums of X[u] - mu over u = order[offsets[c]:offsets[c+1]] per class c, in that
+    order; ``mu`` (D,) fp64 or None (0)."""
+    X = _score_rows(X, "class_sums_f64")
+    order = torch.as_tensor(order).to(device=X.device, dtype=torch.int64).contiguous()
+    offsets = torch.as_tensor(offsets).to(device=X.device, dtype=torch.int64).contiguous()
+    if order.dim() != 1 or offsets.dim() != 1 or offsets.numel() < 2:
+        raise RuntimeError(f"class_sums_f64: expected 1-D order and offsets with >= 2 entries, got "
+                           f"{tuple(order.shape)} and {tuple(offsets.shape)}")
+    (N, D), C = X.shape, offsets.numel() - 1
+    mu = _f64_vec(mu, X.device, D, "class_sums_f64")
+    out = torch.empty(C, D, device=X.device, dtype=torch.float64)
+    with torch.cuda.device(X.device):
+        L.check(L.load().dsk_class_sums_f64(X.data_ptr(), N, D, order.data_ptr(), offsets.data_ptr(), C, L.ptr(mu),
+                                            out.data_ptr(), L.cur_stream()), "dsk_class_sums_f64")
+    return out
+
+
+def gram_f64(X, mu=None):
+    """dsk_gram_f64: (D, D) fp64 sum over the rows of (X[u] - mu)(X[u] - mu)^T on the fp64 tensor cores, exactly
+    symmetric and the same bits on every call; ``mu`` (D,) fp64 or None (0)."""
+    X = _score_rows(X, "gram_f64")
+    N, D = X.shape
+    mu = _f64_vec(mu, X.device, D, "gram_f64")
+    G = torch.empty(D, D, device=X.device, dtype=torch.float64)
+    with torch.cuda.device(X.device):
+        L.check(L.load().dsk_gram_f64(X.data_ptr(), N, D, L.ptr(mu), G.data_ptr(), L.cur_stream()), "dsk_gram_f64")
+    return G
+
+
+def affine_norm_f64(X, A, c=None, mode="none", psi=None, counts=None):
+    """dsk_affine_norm_f64: (N, d) fp32 rows s_u A (X[u] - c), accumulated in fp64 and rounded once.  ``mode``: "none"
+    (s = 1), "length" (s = sqrt(d) / ||A (x - c)||) or "plda" (s = sqrt(d / sum_l z_l^2 / (psi_l + 1 / n_u)), with
+    ``counts`` (N,) the n_u, None for 1)."""
+    if mode not in NORM_MODES:
+        raise ValueError(f"affine_norm_f64: mode must be one of {sorted(NORM_MODES)}, got {mode!r}")
+    X = _score_rows(X, "affine_norm_f64")
+    N, D = X.shape
+    A = torch.as_tensor(A).detach().to(device=X.device, dtype=torch.float64).contiguous()
+    if A.dim() != 2 or A.shape[1] != D:
+        raise RuntimeError(f"affine_norm_f64: expected A of shape (d, {D}), got {tuple(A.shape)}")
+    d = A.shape[0]
+    c = _f64_vec(c, X.device, D, "affine_norm_f64")
+    psi = _f64_vec(psi, X.device, d, "affine_norm_f64")
+    if mode == "plda" and psi is None:
+        raise RuntimeError("affine_norm_f64: mode 'plda' needs psi")
+    counts = _counts(counts, X.device, N, "affine_norm_f64")
+    Y = torch.empty(N, d, device=X.device, dtype=torch.float32)
+    with torch.cuda.device(X.device):
+        L.check(L.load().dsk_affine_norm_f64(X.data_ptr(), N, D, A.data_ptr(), d, L.ptr(c), NORM_MODES[mode], L.ptr(psi),
+                                             L.ptr(counts), Y.data_ptr(), L.cur_stream()), "dsk_affine_norm_f64")
+    return Y
+
+
+def plda_score_trials(Y, psi, trials, counts=None):
+    """dsk_plda_score_trials: (T,) fp32 PLDA LLRs of trials (T, 2) (enrolment, test) of row indices into the
+    transformed rows Y (U, d); ``counts`` (U,) the utterances averaged into each row (None: 1), used on the enrolment
+    side.  An index outside [0, U) or a count < 1 gives NaN."""
+    Y = _score_rows(Y, "plda_score_trials")
+    U, d = Y.shape
+    trials = torch.as_tensor(trials)
+    if trials.dim() != 2 or trials.shape[1] != 2 or trials.shape[0] < 1:
+        raise RuntimeError(f"plda_score_trials: expected trials of shape (T, 2) with T >= 1, got {tuple(trials.shape)}")
+    trials = trials.to(device=Y.device, dtype=torch.int64).contiguous()
+    psi = _f64_vec(psi, Y.device, d, "plda_score_trials")
+    counts = _counts(counts, Y.device, U, "plda_score_trials")
+    llr = torch.empty(trials.shape[0], device=Y.device, dtype=torch.float32)
+    with torch.cuda.device(Y.device):
+        L.check(L.load().dsk_plda_score_trials(Y.data_ptr(), U, d, psi.data_ptr(), L.ptr(counts), trials.data_ptr(),
+                                               trials.shape[0], llr.data_ptr(), L.cur_stream()), "dsk_plda_score_trials")
+    return llr
+
+
+def plda_score_matrix(Ya, Yb, psi):
+    """dsk_plda_score_matrix: (M, N) fp32 n = 1 PLDA LLRs of every row of Ya (M, d) against every row of Yb (N, d)."""
+    Ya, Yb = _score_pair(Ya, Yb, "plda_score_matrix")
+    (M, d), N = Ya.shape, Yb.shape[0]
+    psi = _f64_vec(psi, Ya.device, d, "plda_score_matrix")
+    S = torch.empty(M, N, device=Ya.device, dtype=torch.float32)
+    with torch.cuda.device(Ya.device):
+        L.check(L.load().dsk_plda_score_matrix(Ya.data_ptr(), M, Yb.data_ptr(), N, d, psi.data_ptr(), S.data_ptr(), N,
+                                               L.cur_stream()), "dsk_plda_score_matrix")
+    return S

@@ -550,6 +550,49 @@ int32_t dsk_class_centroids(const float* X, int32_t U, int32_t D, const int64_t*
 int32_t dsk_ahc(const float* S, int32_t N, int64_t ld, int32_t linkage, int32_t stop_k, double stop_height, double* Z,
                 int32_t* n_merges, int32_t* labels, int32_t* n_rounds, void* stream);
 
+/* PLDA backend: the N-sized passes of an LDA + two-covariance PLDA fit (the Kaldi x-vector recipe) and PLDA
+ * log-likelihood-ratio scoring (no reference implementation exists; oracle/plda_oracle.py defines the model).  Inputs
+ * are fp32 rows, every statistic is fp64, no float atomics: each output is the same bits on every call.  All pointers
+ * are device memory; workspaces are stream-ordered (cudaMallocAsync / cudaFreeAsync).
+ *   dsk_class_sums_f64: out[c] (C,D) fp64 = the sum of x_u - mu over u = order[offsets[c] .. offsets[c+1]), in that
+ *     order; mu (D,) fp64 may be NULL (0).  An empty segment gives a zero row, an index outside [0, N) a NaN row.  One
+ *     CTA per class and 256 columns.  order, offsets (C+1) are int64.
+ *   dsk_gram_f64: G (D,D) fp64 = sum over all N rows of (x_u - mu)(x_u - mu)^T (mu may be NULL) on the fp64 tensor
+ *     cores (mma.sync m8n8k4 f64): the 64 x 64 tiles on and above the diagonal only, each over a split of the rows;
+ *     the split depends only on (N, D) (about 1024 CTAs), the splits' partials are summed in split order and written to
+ *     both halves, so G is exactly symmetric and the same bits on every call.  Workspace: splits x upper tiles x 32 KiB.
+ *   dsk_affine_norm_f64: Y (N,d) fp32 = s_u A (x_u - c), A (d,D) and c (D,) fp64 (c may be NULL), accumulated in fp64
+ *     on the tensor cores and rounded once.  The row scale s_u by mode: DSK_NORM_NONE 1; DSK_NORM_LENGTH sqrt(d) / ||z||
+ *     (z = A (x_u - c)); DSK_NORM_PLDA sqrt(d / sum_l z_l^2 / (psi_l + 1 / n_u)) with psi (d,) fp64 and n_u = counts[u]
+ *     (int32, may be NULL: n = 1); a count < 1 gives a NaN row.  The fp64 z pass through a workspace of at most 128 MiB
+ *     taken in row chunks; a row's output depends only on that row.
+ *   dsk_plda_score_trials: llr (T,) fp32 of trials (T,2) int64 (e, t) into rows of Y (U,d) (transformed rows, e.g.
+ *     dsk_affine_norm_f64 in mode DSK_NORM_PLDA): log N(y_t; a o y_e, diag(1 + psi / (n psi + 1))) - log N(y_t; 0,
+ *     diag(1 + psi)), a = n psi / (n psi + 1), n = counts[e] the utterances averaged into the enrolment row (counts may
+ *     be NULL: n = 1), the test side always n = 1.  fp64 inside, one warp per trial in a fixed order: a trial's bits do
+ *     not depend on the other trials.  An index outside [0, U) or a count < 1 gives NaN and reads no row.
+ *   dsk_plda_score_matrix: S (M,N) fp32 (row stride ld floats) of the n = 1 LLRs of every row of Ya (M,d) against every
+ *     row of Yb (N,d), in the expanded form k + q(a_i) + q(b_j) + sum_l beta_l a_il b_jl (q(y) = sum_l w_l y_l^2,
+ *     w = -psi^2 / (2 (1 + psi)(2 psi + 1)), beta = psi / (2 psi + 1), k = sum_l (log(1 + psi) - log((2 psi + 1) /
+ *     (1 + psi))) / 2), fp64 throughout with the cross term on the fp64 tensor cores; the output feeds dsk_ahc.
+ * A NaN in an input row reaches only that row's outputs: its class sum, its transformed row, its trials, its row and
+ * column of S (and every Gram entry, which is a sum over all rows).  1 <= D, d <= DSK_F64_MAX_DIM, N, U, T, C >= 1,
+ * T <= 2^33, M <= DSK_PLDA_MAX_ROWS, ld >= N, non-null pointers where not stated otherwise, else DSK_ERR_INVALID. */
+#define DSK_F64_MAX_DIM 4096
+#define DSK_PLDA_MAX_ROWS 4194240
+#define DSK_NORM_NONE 0
+#define DSK_NORM_LENGTH 1
+#define DSK_NORM_PLDA 2
+int32_t dsk_class_sums_f64(const float* X, int64_t N, int32_t D, const int64_t* order, const int64_t* offsets,
+                           int32_t C, const double* mu, double* out, void* stream);
+int32_t dsk_gram_f64(const float* X, int64_t N, int32_t D, const double* mu, double* G, void* stream);
+int32_t dsk_affine_norm_f64(const float* X, int64_t N, int32_t D, const double* A, int32_t d, const double* c,
+                            int32_t mode, const double* psi, const int32_t* counts, float* Y, void* stream);
+int32_t dsk_plda_score_trials(const float* Y, int32_t U, int32_t d, const double* psi, const int32_t* counts,
+                              const int64_t* trials, int64_t T, float* llr, void* stream);
+int32_t dsk_plda_score_matrix(const float* Ya, int32_t M, const float* Yb, int32_t N, int32_t d, const double* psi,
+                              float* S, int64_t ld, void* stream);
+
 /* nn.Linear of DeepSpeakerModel.forward_classifier (reference model.py:167,220-223): y (M,N) = x (M,K) w(N,K)^T + b.
  * fp32 on the CUDA cores, fixed summation order (deterministic).  b may be NULL. */
 int32_t dsk_linear_forward(const float* x, const float* w, const float* b, int32_t M, int32_t N, int32_t K, float* y,
