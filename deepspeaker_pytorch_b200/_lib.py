@@ -26,6 +26,7 @@ DSK_AHC_MAX_N = 32768
 DSK_NORM_NONE, DSK_NORM_LENGTH, DSK_NORM_PLDA = 0, 1, 2
 DSK_F64_MAX_DIM = 4096
 DSK_PLDA_MAX_ROWS = 4194240
+DSK_VBX_MAX_SPEAKERS = 128
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -219,6 +220,8 @@ SIGNATURES = {
                                         c_void_p]),
     "dsk_plda_score_matrix": (c_int32, [c_void_p, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_int64,
                                         c_void_p]),
+    "dsk_vbx": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_double, c_double,
+                          c_double, c_double, c_int32, c_double] + [c_void_p] * 6),
     "dsk_linear_forward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
     "dsk_linear_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p,
                                       c_void_p, c_void_p]),

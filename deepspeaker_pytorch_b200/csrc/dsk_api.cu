@@ -32,6 +32,7 @@
 #include "score_kernels.cuh"
 #include "simt_kernels.cuh"
 #include "train_kernels.cuh"
+#include "vbx_kernels.cuh"
 #include "wgrad_umma.cuh"
 
 namespace {
@@ -3389,6 +3390,121 @@ int32_t dsk_plda_score_matrix(const float* Ya, int32_t M, const float* Yb, int32
   const cudaError_t fe = cudaFreeAsync(ws, s);
   if (e != cudaSuccess) return fail(DSK_ERR_CUDA, "dsk_plda_score_matrix: kernel launch failed: %s", cudaGetErrorString(e));
   if (fe != cudaSuccess) return fail(DSK_ERR_CUDA, "dsk_plda_score_matrix: cudaFreeAsync failed: %s", cudaGetErrorString(fe));
+  return DSK_OK;
+}
+
+// ---- VBx: Bayesian HMM clustering of window embeddings ------------------------------------------------------------
+constexpr int kVbxItersPerCheck = 8;  // iterations between reads of the device-side count of finished recordings
+
+int32_t dsk_vbx(const float* X, int64_t W, int32_t d, const int64_t* offsets, int32_t R, const int32_t* init_labels,
+                int32_t S, const double* phi, double Fa, double Fb, double loop_p, double init_smoothing,
+                int32_t max_iters, double epsilon, double* gamma, double* pi, double* elbo, int32_t* iters,
+                int32_t* labels, void* stream) {
+  bool ok = X && offsets && init_labels && phi && gamma && pi && elbo && iters && labels && R >= 1 && d >= 1 &&
+            d <= DSK_F64_MAX_DIM && S >= 1 && S <= DSK_VBX_MAX_SPEAKERS && !std::isnan(Fa) && !std::isnan(Fb) &&
+            !std::isnan(loop_p) && !std::isnan(init_smoothing) && !std::isnan(epsilon) && Fa > 0 && Fb > 0 &&
+            loop_p >= 0 && loop_p <= 1 && init_smoothing >= 0 && max_iters >= 1;
+  if (ok) ok = offsets[0] == 0 && offsets[R] == W;
+  for (int32_t r = 0; ok && r < R; ++r)
+    ok = offsets[r + 1] > offsets[r] && offsets[r + 1] - offsets[r] <= DSK_AHC_MAX_N;
+  if (!ok)
+    return fail(DSK_ERR_INVALID, "dsk_vbx: bad arguments (need non-null pointers, R >= 1, 1 <= d <= %d, 1 <= S <= %d, "
+                "offsets strictly increasing from 0 to W with at most %d rows per recording, Fa > 0, Fb > 0, loop_p in "
+                "[0, 1], init_smoothing >= 0, max_iters >= 1, no NaN parameter; got W %lld, d %d, R %d, S %d, Fa %g, "
+                "Fb %g, loop_p %g, init_smoothing %g, max_iters %d, epsilon %g)", DSK_F64_MAX_DIM,
+                DSK_VBX_MAX_SPEAKERS, DSK_AHC_MAX_N, static_cast<long long>(W), d, R, S, Fa, Fb, loop_p,
+                init_smoothing, max_iters, epsilon);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  // work tables: (recording, split) for the statistics, (recording, row tile) for the log-likelihoods; every split
+  // depends only on the recording's own length
+  std::vector<int32_t> stat_tab, ll_tab, split_base(R + 1, 0);
+  for (int32_t r = 0; r < R; ++r) {
+    const int64_t n = offsets[r + 1] - offsets[r];
+    const int splits = static_cast<int>((n + dsk::kVbxSplitRows - 1) / dsk::kVbxSplitRows);
+    for (int k = 0; k < splits; ++k) stat_tab.insert(stat_tab.end(), {r, k});
+    for (int k = 0; k < (n + dsk::kF64Tile - 1) / dsk::kF64Tile; ++k) ll_tab.insert(ll_tab.end(), {r, k});
+    split_base[r + 1] = split_base[r] + splits;
+  }
+  const int n_stat = static_cast<int>(stat_tab.size() / 2), n_ll = static_cast<int>(ll_tab.size() / 2);
+  const int tiles_s = (S + dsk::kF64Tile - 1) / dsk::kF64Tile, tiles_c = (d + 1 + dsk::kF64Tile - 1) / dsk::kF64Tile;
+  // workspace: rho (W,d), G (W), lnp (W,S), ln C (W), the partials, alpha (R,S,d), cst and kl (R,S), then the tables,
+  // offsets and per-recording ints
+  const size_t Wd = static_cast<size_t>(W);
+  size_t sizes[] = {Wd * d * 8, Wd * 8, Wd * S * 8, Wd * 8,
+                    static_cast<size_t>(n_stat) * tiles_s * tiles_c * dsk::kF64Tile * dsk::kF64Tile * 8,
+                    static_cast<size_t>(R) * S * d * 8, static_cast<size_t>(R) * S * 8, static_cast<size_t>(R) * S * 8,
+                    static_cast<size_t>(R + 1) * 8, stat_tab.size() * 4, ll_tab.size() * 4,
+                    static_cast<size_t>(R + 1) * 4, (3 * static_cast<size_t>(R) + 1) * 4};
+  size_t total = 0;
+  for (size_t& z : sizes) total += z = (z + 255) / 256 * 256;
+  uint8_t* ws = nullptr;
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&ws), total, s));
+  uint8_t* p = ws;
+  auto take = [&](int i) {
+    uint8_t* q = p;
+    p += sizes[i];
+    return q;
+  };
+  double* rho = reinterpret_cast<double*>(take(0));
+  double* G = reinterpret_cast<double*>(take(1));
+  double* lnp = reinterpret_cast<double*>(take(2));
+  double* lnc = reinterpret_cast<double*>(take(3));
+  double* part = reinterpret_cast<double*>(take(4));
+  double* alpha = reinterpret_cast<double*>(take(5));
+  double* cst = reinterpret_cast<double*>(take(6));
+  double* kl = reinterpret_cast<double*>(take(7));
+  int64_t* off_d = reinterpret_cast<int64_t*>(take(8));
+  int32_t* stat_d = reinterpret_cast<int32_t*>(take(9));
+  int32_t* ll_d = reinterpret_cast<int32_t*>(take(10));
+  int32_t* base_d = reinterpret_cast<int32_t*>(take(11));
+  int32_t* rec_S = reinterpret_cast<int32_t*>(take(12));
+  int32_t* bad = rec_S + R;
+  int32_t* done = bad + R;
+  int32_t* n_done = done + R;
+  const double ratio = Fa / Fb;
+  int rc = DSK_OK;
+  cudaError_t e = cudaSuccess;
+  do {
+    // pageable sources: each copy has read its host buffer when it returns
+    e = cudaMemcpyAsync(off_d, offsets, (R + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(stat_d, stat_tab.data(), stat_tab.size() * 4, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ll_d, ll_tab.data(), ll_tab.size() * 4, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(base_d, split_base.data(), (R + 1) * 4, cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(rec_S, 0, (3 * static_cast<size_t>(R) + 1) * 4, s);
+    if (e != cudaSuccess) break;
+    dsk::vbx_prep_kernel<<<static_cast<unsigned>((W + dsk::kPldaWarps - 1) / dsk::kPldaWarps), 256, 0, s>>>(
+        X, W, d, off_d, R, init_labels, S, phi, rho, G, rec_S, bad);
+    dsk::vbx_rec_init_kernel<<<(R + 127) / 128, 128, 0, s>>>(R, S, max_iters, rec_S, bad, done, n_done, pi, elbo,
+                                                             iters);
+    dsk::vbx_gamma0_kernel<<<static_cast<unsigned>((W + 255) / 256), 256, 0, s>>>(W, off_d, R, init_labels, S,
+                                                                                   init_smoothing, rec_S, bad, gamma);
+    e = cudaGetLastError();
+    for (int it = 0; it < max_iters && e == cudaSuccess; ++it) {
+      dsk::vbx_stats_kernel<<<dim3(n_stat, tiles_s * tiles_c), dsk::kF64Threads, 0, s>>>(gamma, S, rho, d, off_d, stat_d,
+                                                                                         rec_S, done, part);
+      dsk::vbx_model_kernel<<<dim3(R, (S + dsk::kPldaWarps - 1) / dsk::kPldaWarps), 256, 0, s>>>(
+          part, off_d, base_d, S, d, phi, ratio, rec_S, done, alpha, cst, kl);
+      dsk::vbx_loglik_kernel<<<dim3(n_ll, tiles_s), dsk::kF64Threads, 0, s>>>(rho, d, alpha, cst, G, S, Fa, off_d, ll_d,
+                                                                              rec_S, done, lnp);
+      dsk::vbx_fb_kernel<<<R, 32, 0, s>>>(off_d, S, lnp, gamma, lnc, kl, loop_p, Fb, epsilon, it, max_iters, rec_S,
+                                          done, n_done, pi, elbo, iters);
+      e = cudaGetLastError();
+      if (e == cudaSuccess && (it + 1) % kVbxItersPerCheck == 0 && it + 1 < max_iters) {
+        int32_t nd = 0;
+        e = cudaMemcpyAsync(&nd, n_done, sizeof(nd), cudaMemcpyDeviceToHost, s);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (e == cudaSuccess && nd == R) break;
+      }
+    }
+    if (e != cudaSuccess) break;
+    dsk::vbx_labels_kernel<<<static_cast<unsigned>((W + 255) / 256), 256, 0, s>>>(W, off_d, R, S, rec_S, bad, gamma,
+                                                                                  labels);
+    e = cudaGetLastError();
+  } while (false);
+  if (e != cudaSuccess) rc = fail(DSK_ERR_CUDA, "dsk_vbx: %s", cudaGetErrorString(e));
+  const cudaError_t fe = cudaFreeAsync(ws, s);
+  if (rc) return rc;
+  if (fe != cudaSuccess) return fail(DSK_ERR_CUDA, "dsk_vbx: cudaFreeAsync failed: %s", cudaGetErrorString(fe));
   return DSK_OK;
 }
 

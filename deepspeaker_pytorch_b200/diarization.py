@@ -17,6 +17,11 @@ wraps inside the run), all windows of a recording are clustered together, each s
 nearest window centre within its run and every other frame is -1, which no segment or RTTM line covers.  Without it,
 every frame gets a speaker, silence included.
 
+With ``plda`` and ``vbx`` (a dict of ``vbx`` options, ``{}`` for the defaults) the AHC labels are only the start:
+``vbx`` refines every recording's window labels with VBx, a variational-Bayes HMM whose states are speakers and whose
+emission model is the PLDA itself (Landini et al., 2022), so neighbouring windows tend to share a speaker and surplus
+initial clusters lose their windows.  ``der`` scores per-frame labels against a reference.
+
 Overlapped speech and re-segmentation are not part of this module: a frame gets at most one speaker.
 """
 from __future__ import annotations
@@ -24,6 +29,7 @@ from __future__ import annotations
 from typing import NamedTuple
 
 import numpy as np
+import torch
 
 from . import _lib as L
 from . import engine
@@ -80,6 +86,134 @@ def to_rttm(segs, recording_id: str) -> str:
     return "".join(f"SPEAKER {rid} 1 {a:.3f} {b - a:.3f} <NA> <NA> spk{k} <NA> <NA>\n" for a, b, k in segs)
 
 
+class VBxResult(NamedTuple):
+    """The VBx refinement of R recordings' windows: ``labels`` (W,) int32 numpy, renumbered per recording in the order
+    of first window (-1 for a recording with a non-finite embedding); ``gamma`` (W, S) and ``pi`` (R, S) fp64, ``elbo``
+    (R, max_iters) fp64 (NaN past a recording's last iteration) and ``iters`` (R,) int32, device tensors whose speaker
+    columns are the initial labels' (not renumbered)."""
+    labels: np.ndarray
+    gamma: torch.Tensor
+    pi: torch.Tensor
+    elbo: torch.Tensor
+    iters: torch.Tensor
+
+
+VBX_OPTIONS = ("Fa", "Fb", "loop_p", "init_smoothing", "max_iters", "epsilon")
+
+
+def _plda_space(plda, E):
+    """The PLDA-space rows P (y - m_bar) of raw embeddings E, y their length-normalised LDA outputs (PLDA.transform
+    without the scoring normalisation)."""
+    m = plda._on(E.device)
+    y = engine.affine_norm_f64(E, m["lda"], m["mu"], mode="length")
+    return engine.affine_norm_f64(y, m["plda_transform"], m["plda_mean"], mode="none")
+
+
+def _renumber(labels, offsets):
+    """Labels renumbered per recording offsets[r] .. offsets[r + 1] in the order of first appearance; -1 stays."""
+    out = np.asarray(labels, np.int32).copy()
+    for a, b in zip(offsets[:-1], offsets[1:]):
+        seg = out[a:b]
+        keep = seg >= 0
+        _, first, inv = np.unique(seg[keep], return_index=True, return_inverse=True)
+        seg[keep] = np.argsort(np.argsort(first))[inv]
+    return out
+
+
+def vbx(plda, E, offsets, init_labels, Fa: float = 0.3, Fb: float = 17.0, loop_p: float = 0.99,
+        init_smoothing: float = 5.0, max_iters: int = 40, epsilon: float = 1e-4) -> VBxResult:
+    """Refine the initial speaker labels of the window embeddings E (W, D) (raw, a CUDA tensor) of R recordings
+    (``offsets`` (R + 1,): recording r is rows offsets[r] .. offsets[r + 1], in time order) with VBx on the PLDA
+    model ``plda``.  ``init_labels`` (W,): each recording's initial clusters numbered from 0 (``engine.ahc`` labels,
+    over-clustered), at most DSK_VBX_MAX_SPEAKERS per recording.
+
+    The rows are taken into the PLDA space without the scoring normalisation, where the within-speaker covariance is
+    I and the across-speaker one diag(psi); ``engine.vbx`` then runs the iteration of oracle/vbx_oracle.py on all
+    recordings in one call.  Fa scales the acoustic likelihoods, Fb the speaker-model prior, loop_p is the
+    probability of staying with the same speaker from one window to the next, init_smoothing the softmax temperature
+    of the initial labels; a recording stops when its ELBO gains less than epsilon.  The defaults are starting values
+    common in the VBx literature for x-vectors every 0.25 s; they are NOT tuned for this model or for other hops."""
+    if not isinstance(E, torch.Tensor) or not E.is_cuda:
+        raise RuntimeError("vbx needs a CUDA embedding tensor; there is no CPU fallback")
+    off = np.asarray(offsets, np.int64).reshape(-1)
+    X = _plda_space(plda, E)
+    gamma, pi, elbo, iters, lab = engine.vbx(X, off, init_labels, plda._on(E.device)["psi"], Fa, Fb, loop_p,
+                                             init_smoothing, max_iters, epsilon)
+    return VBxResult(_renumber(lab.cpu().numpy(), off), gamma, pi, elbo, iters)
+
+
+class DER(NamedTuple):
+    """``der``'s result: fractions of the reference's speech frames, and the speaker mapping."""
+    der: float
+    miss: float
+    false_alarm: float
+    confusion: float
+    mapping: dict
+
+
+def der(ref, hyp):
+    """Host: the frame-level diarization error of per-frame labels ``hyp`` against ``ref`` (equal lengths; -1 is
+    non-speech) -> (der, miss, false_alarm, confusion, mapping): the three errors are fractions of the reference's
+    speech frames and der is their sum; mapping {hyp speaker: ref speaker} is the one-to-one mapping that maximises the
+    frames both label alike (Hungarian algorithm), listing matched pairs that share frames.
+
+    Frames are scored one speaker each, with no forgiveness collar around reference boundaries: this is NOT the
+    md-eval / dscore DER (no collar, no overlap, 10 ms frames).  ValueError on a length mismatch or a reference without
+    speech."""
+    from scipy.optimize import linear_sum_assignment
+
+    r = np.asarray(ref).reshape(-1)
+    h = np.asarray(hyp).reshape(-1)
+    if r.size != h.size:
+        raise ValueError(f"der: {r.size} reference frames and {h.size} hypothesis frames")
+    speech = r >= 0
+    n = int(speech.sum())
+    if n == 0:
+        raise ValueError("der: the reference has no speech")
+    miss = int((speech & (h < 0)).sum())
+    fa = int((~speech & (h >= 0)).sum())
+    both = speech & (h >= 0)
+    r_ids, ri = np.unique(r[both], return_inverse=True)
+    h_ids, hi = np.unique(h[both], return_inverse=True)
+    C = np.zeros((h_ids.size, r_ids.size), np.int64)
+    np.add.at(C, (hi, ri), 1)
+    rows, cols = linear_sum_assignment(C, maximize=True)
+    conf = int(both.sum()) - int(C[rows, cols].sum())
+    mapping = {int(h_ids[i]): int(r_ids[j]) for i, j in zip(rows, cols) if C[i, j] > 0}
+    return DER((miss + fa + conf) / n, miss / n, fa / n, conf / n, mapping)
+
+
+def _vbx_options(vbx, plda):
+    if vbx is None:
+        return None
+    if plda is None:
+        raise ValueError("diarize: vbx needs a PLDA backend (plda=)")
+    if not isinstance(vbx, dict):
+        raise ValueError(f"diarize: vbx must be None or a dict of options, got {type(vbx).__name__}")
+    unknown = sorted(set(vbx) - set(VBX_OPTIONS))
+    if unknown:
+        raise ValueError(f"diarize: unknown vbx options {unknown}; known: {list(VBX_OPTIONS)}")
+    return dict(vbx)
+
+
+def _refine(plda, emb, spans, wls, opts):
+    """VBx on every recording of more than one window (rows spans[r] of emb, AHC labels wls[r]), in one call; the
+    window labels of those recordings are replaced in place."""
+    multi = [r for r, (a, b) in enumerate(spans) if b - a > 1]
+    if not multi:
+        return
+    most = max(int(wls[r].max()) + 1 for r in multi)
+    if most > L.DSK_VBX_MAX_SPEAKERS:
+        raise ValueError(f"diarize: AHC gave {most} initial clusters, more than VBx takes "
+                         f"({L.DSK_VBX_MAX_SPEAKERS}); use a higher threshold or fewer speakers")
+    lens = [spans[r][1] - spans[r][0] for r in multi]
+    off = np.concatenate(([0], np.cumsum(lens)))
+    E = torch.cat([emb[spans[r][0]:spans[r][1]] for r in multi])
+    res = vbx(plda, E, off, np.concatenate([wls[r] for r in multi]), **opts)
+    for i, r in enumerate(multi):
+        wls[r] = res.labels[off[i]:off[i + 1]]
+
+
 def _per_recording(x, n, what):
     if isinstance(x, (list, tuple, np.ndarray)):
         if len(x) != n:
@@ -127,7 +261,7 @@ def _cluster(E, plda, threshold, linkage, k):
     return engine.ahc(S, linkage, num_clusters=k)
 
 
-def _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batch, plda):
+def _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batch, plda, vbx):
     R = u.size
     table, runs, run_off, kept = bank._run_table(speech, u, "diarize")
     rec, first, end = table[:, 0], table[:, 1], table[:, 2]
@@ -145,30 +279,37 @@ def _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batc
                                                                 "diarize")
         win_off = win_off.numpy()
     run_off_rec = np.searchsorted(rec, np.arange(R + 1))     # runs of recording r: run_off_rec[r] .. [r + 1]
-    out = []
+    spans, wls, Zs = [], [], []
     for r in range(R):
-        n = int(bank.lengths[u[r]])
         r0, r1 = int(run_off_rec[r]), int(run_off_rec[r + 1])
-        fl = np.full(n, -1, np.int32)
-        if r0 == r1:
-            out.append(Recording([], fl, np.zeros(0, np.int32), np.zeros((0, 4))))
-            continue
-        a, b = int(win_off[r0]), int(win_off[r1])
+        a, b = (int(win_off[r0]), int(win_off[r1])) if r0 < r1 else (0, 0)
         W = b - a
-        if W == 1:
+        if W == 0:
+            wl, Z = np.zeros(0, np.int32), np.zeros((0, 4))
+        elif W == 1:
             wl, Z = np.zeros(1, np.int32), np.zeros((0, 4))
         else:
             Z, lab = _cluster(emb[a:b], plda, threshold, linkage, min(int(ks[r]), W) if threshold is None else None)
             wl = lab.cpu().numpy()
+        spans.append((a, b))
+        wls.append(wl)
+        Zs.append(Z)
+    if vbx is not None:
+        _refine(plda, emb, spans, wls, vbx)
+    out = []
+    for r in range(R):
+        fl = np.full(int(bank.lengths[u[r]]), -1, np.int32)
+        r0, r1 = int(run_off_rec[r]), int(run_off_rec[r + 1])
+        a, wl = spans[r][0], wls[r]
         for i in range(r0, r1):
             w0, w1 = int(win_off[i]), int(win_off[i + 1])
             fl[first[i]:end[i]] = frame_labels(win_start[w0:w1].numpy(), wl[w0 - a:w1 - a], int(rlen[i]), T)
-        out.append(Recording([sg for sg in segments(fl) if sg[2] >= 0], fl, wl, Z))
+        out.append(Recording([sg for sg in segments(fl) if sg[2] >= 0] if r0 < r1 else [], fl, wl, Zs[r]))
     return out
 
 
 def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40, num_speakers=None, threshold=None,
-            linkage: str = "average", batch: int = 256, speech=None, plda=None) -> list:
+            linkage: str = "average", batch: int = 256, speech=None, plda=None, vbx=None) -> list:
     """Diarize the recordings ``utt`` (indices into ``bank``) -> [Recording] in the order of ``utt``.  Give exactly
     one of ``num_speakers`` (an int, or one per recording; a recording with fewer windows gets one speaker per window)
     and ``threshold`` (a cosine distance 1 - cos: windows merge while the linkage distance is <= threshold), else
@@ -182,11 +323,19 @@ def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40,
     ``plda``: None (the affinity is the windows' cosine), or a fitted ``plda.PLDA``: the affinity is then the PLDA
     log-likelihood ratio of the transformed window embeddings (``plda.score_matrix(plda.transform(E), ...)``), and
     ``threshold`` is an LLR: windows merge while the linkage of LLRs is >= threshold (``engine.ahc`` gets
-    1 - threshold, its distance being 1 - S, and ``Z``'s heights are 1 - LLR)."""
+    1 - threshold, its distance being 1 - S, and ``Z``'s heights are 1 - LLR).
+
+    ``vbx``: None, or a dict of options of ``vbx`` (``{}`` for its defaults; needs ``plda``, else ValueError, as is an
+    unknown key).  The AHC cut (``threshold`` or ``num_speakers``) is then the initial over-clustering, and one ``vbx``
+    call refines the window labels of every recording of more than one window (with ``speech``, all speech windows of
+    a recording in time order form one sequence).  ``window_labels`` are VBx's, renumbered by first window; frame
+    labels and segments follow from them as above; ``Z`` stays the AHC tree.  More than DSK_VBX_MAX_SPEAKERS initial
+    clusters in a recording is a ValueError."""
     if (num_speakers is None) == (threshold is None):
         raise ValueError("diarize: give exactly one of num_speakers and threshold")
     if linkage not in engine.LINKAGES:
         raise ValueError(f"diarize: linkage must be one of {sorted(engine.LINKAGES)}, got {linkage!r}")
+    vbx = _vbx_options(vbx, plda)
     if model.training:
         raise RuntimeError("diarize needs model.eval() (train-mode BatchNorm would use batch statistics)")
     u = np.asarray(utt, np.int64).reshape(-1)
@@ -196,7 +345,7 @@ def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40,
     if num_speakers is not None and any(int(k) < 1 for k in ks):
         raise ValueError(f"diarize: num_speakers must be >= 1, got {num_speakers}")
     if speech is not None:
-        return _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batch, plda)
+        return _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batch, plda, vbx)
     _, _, win_off = bank.windows(u, T, hop)
     counts = np.diff(win_off.numpy())
     if counts.max() > MAX_WINDOWS:
@@ -205,7 +354,7 @@ def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40,
         raise ValueError(f"diarize: a recording of {n} frames has {int(counts.max())} windows at hop {hop}, more than "
                          f"{MAX_WINDOWS}; use hop >= {need}")
     emb, _, win_start, win_off = frontend.window_embeddings(model, bank, u, T, hop, batch, "diarize")
-    out = []
+    spans, wls, Zs = [], [], []
     for r in range(u.size):
         a, b = int(win_off[r]), int(win_off[r + 1])
         W = b - a
@@ -214,6 +363,14 @@ def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40,
         else:
             Z, lab = _cluster(emb[a:b], plda, threshold, linkage, min(int(ks[r]), W) if threshold is None else None)
             wl = lab.cpu().numpy()
-        fl = frame_labels(win_start[a:b].numpy(), wl, int(bank.lengths[u[r]]), T)
-        out.append(Recording(segments(fl), fl, wl, Z))
+        spans.append((a, b))
+        wls.append(wl)
+        Zs.append(Z)
+    if vbx is not None:
+        _refine(plda, emb, spans, wls, vbx)
+    out = []
+    for r in range(u.size):
+        a, b = spans[r]
+        fl = frame_labels(win_start[a:b].numpy(), wls[r], int(bank.lengths[u[r]]), T)
+        out.append(Recording(segments(fl), fl, wls[r], Zs[r]))
     return out

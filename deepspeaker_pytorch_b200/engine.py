@@ -876,3 +876,40 @@ def plda_score_matrix(Ya, Yb, psi):
         L.check(L.load().dsk_plda_score_matrix(Ya.data_ptr(), M, Yb.data_ptr(), N, d, psi.data_ptr(), S.data_ptr(), N,
                                                L.cur_stream()), "dsk_plda_score_matrix")
     return S
+
+
+# ---------------------------------------------------------------------------------------------------
+# VBx: Bayesian HMM clustering of window embeddings in the PLDA space
+# ---------------------------------------------------------------------------------------------------
+def vbx(X, offsets, init_labels, phi, Fa, Fb, loop_p, init_smoothing, max_iters, epsilon):
+    """dsk_vbx over the recordings offsets[r] .. offsets[r + 1] of the PLDA-space rows X (W, d) (CUDA; fp32 without
+    the scoring normalisation), ``offsets`` (R + 1,) on the CPU, ``init_labels`` (W,) CUDA or CPU, ``phi`` (d,) the
+    PLDA's psi.  S = min(1 + the largest label, DSK_VBX_MAX_SPEAKERS) columns; recording r has S_r = 1 + its largest
+    label speakers, and a label outside [0, S) makes its recording NaN with labels -1.
+    -> device tensors (gamma (W, S) fp64, pi (R, S) fp64, elbo (R, max_iters) fp64 (NaN past a recording's last
+    iteration), iters (R,) int32, labels (W,) int32 (the argmax of each gamma row, not renumbered))."""
+    X = _score_rows(X, "vbx")
+    W, d = X.shape
+    off = torch.as_tensor(offsets)
+    if off.is_cuda:
+        raise RuntimeError("vbx: offsets must be a CPU tensor or array")
+    off = off.to(torch.int64).contiguous()
+    if off.dim() != 1 or off.numel() < 2:
+        raise RuntimeError(f"vbx: expected 1-D offsets with >= 2 entries, got shape {tuple(off.shape)}")
+    lab = torch.as_tensor(init_labels).detach().to(device=X.device, dtype=torch.int32).contiguous()
+    if lab.shape != (W,):
+        raise RuntimeError(f"vbx: expected init_labels of shape ({W},), got {tuple(lab.shape)}")
+    phi = _f64_vec(phi, X.device, d, "vbx")
+    R = off.numel() - 1
+    S = max(1, min(int(lab.max().item()) + 1, L.DSK_VBX_MAX_SPEAKERS)) if W else 1
+    gamma = torch.empty(W, S, device=X.device, dtype=torch.float64)
+    pi = torch.empty(R, S, device=X.device, dtype=torch.float64)
+    elbo = torch.empty(R, max(int(max_iters), 1), device=X.device, dtype=torch.float64)
+    iters = torch.empty(R, device=X.device, dtype=torch.int32)
+    labels = torch.empty(W, device=X.device, dtype=torch.int32)
+    with torch.cuda.device(X.device):
+        L.check(L.load().dsk_vbx(X.data_ptr(), W, d, off.data_ptr(), R, lab.data_ptr(), S, phi.data_ptr(), float(Fa),
+                                 float(Fb), float(loop_p), float(init_smoothing), int(max_iters), float(epsilon),
+                                 gamma.data_ptr(), pi.data_ptr(), elbo.data_ptr(), iters.data_ptr(), labels.data_ptr(),
+                                 L.cur_stream()), "dsk_vbx")
+    return gamma, pi, elbo, iters, labels

@@ -593,6 +593,36 @@ int32_t dsk_plda_score_trials(const float* Y, int32_t U, int32_t d, const double
 int32_t dsk_plda_score_matrix(const float* Ya, int32_t M, const float* Yb, int32_t N, int32_t d, const double* psi,
                               float* S, int64_t ld, void* stream);
 
+/* VBx: variational-Bayes clustering of window embeddings with a Bayesian HMM whose states are speakers (Landini et al.,
+ * Computer Speech & Language 2022; no reference implementation exists, oracle/vbx_oracle.py defines the iteration).
+ * Batched over R recordings: recording r is rows offsets[r] .. offsets[r+1] of X (W,d) fp32, PLDA-space rows
+ * t = P (y - m_bar) without the scoring normalisation; phi (d,) fp64 the across-speaker variances psi of that space.
+ * Its S_r = 1 + its largest initial label speakers start from gamma = softmax(init_smoothing one_hot(label)) and
+ * pi = 1 / S_r.  Each iteration forms N_s and sum_t gamma_ts rho_t (rho = x o sqrt(phi)) on the fp64 tensor cores,
+ * invL = 1 / (1 + (Fa / Fb) N_s phi), alpha_s = (Fa / Fb) invL o sum_t gamma_ts rho_t, the log-likelihoods
+ * ln p_ts = Fa (rho_t . alpha_s - sum_l phi_l (invL_sl + alpha_sl^2) / 2 - (|x_t|^2 + d ln 2 pi) / 2), then one warp
+ * per recording runs the forward-backward of the transitions loop_p I + (1 - loop_p) 1 pi^T (rank one: O(S) per
+ * window) for gamma and ln p(X), updates pi and records ELBO_i = ln p(X) + (Fb / 2) sum_s sum_l (ln invL - invL -
+ * alpha^2 + 1).  A recording stops after iteration i when i >= 1 and ELBO_i - ELBO_{i-1} < epsilon, or at max_iters.
+ *   Outputs (device memory): gamma (W,S) fp64 and pi (R,S) fp64 as the last iteration left them, columns >= S_r 0;
+ *   elbo (R,max_iters) fp64, NaN after a recording's last iteration; iters (R) int32 the iterations run; labels (W)
+ *   int32 the argmax of each gamma row (ties to the lower speaker, not renumbered).
+ *   fp64 inside, fixed-order sums, no float atomics: a recording's outputs are the same bits alone or in any batch and
+ *   on every call.  A non-finite element in a recording's rows or an initial label outside [0, S) makes its gamma, pi
+ *   and ELBO NaN, its iters 0 and its labels -1; the other recordings are unaffected.
+ *   Workspace: about W (d + S + 2) + R S (d + 2) doubles plus 32 KiB per (split of 256 rows, 64 x 64 tile),
+ *   stream-ordered.  The host reads a device-side count of finished recordings once per 8 iterations and stops
+ *   launching when all are done; the call does not otherwise synchronise.
+ *   offsets (R+1) int64 in HOST memory.  Non-null pointers, R >= 1, 1 <= d <= DSK_F64_MAX_DIM,
+ *   1 <= S <= DSK_VBX_MAX_SPEAKERS, offsets strictly increasing from 0 to W with at most DSK_AHC_MAX_N rows per
+ *   recording, Fa > 0, Fb > 0, 0 <= loop_p <= 1, init_smoothing >= 0, max_iters >= 1 and no NaN parameter, else
+ *   DSK_ERR_INVALID before any device work. */
+#define DSK_VBX_MAX_SPEAKERS 128
+int32_t dsk_vbx(const float* X, int64_t W, int32_t d, const int64_t* offsets, int32_t R, const int32_t* init_labels,
+                int32_t S, const double* phi, double Fa, double Fb, double loop_p, double init_smoothing,
+                int32_t max_iters, double epsilon, double* gamma, double* pi, double* elbo, int32_t* iters,
+                int32_t* labels, void* stream);
+
 /* nn.Linear of DeepSpeakerModel.forward_classifier (reference model.py:167,220-223): y (M,N) = x (M,K) w(N,K)^T + b.
  * fp32 on the CUDA cores, fixed summation order (deterministic).  b may be NULL. */
 int32_t dsk_linear_forward(const float* x, const float* w, const float* b, int32_t M, int32_t N, int32_t K, float* y,
