@@ -27,6 +27,7 @@ DSK_NORM_NONE, DSK_NORM_LENGTH, DSK_NORM_PLDA = 0, 1, 2
 DSK_F64_MAX_DIM = 4096
 DSK_PLDA_MAX_ROWS = 4194240
 DSK_VBX_MAX_SPEAKERS = 128
+DSK_SPEED_MAX_DEN, DSK_SPEED_TAPS, DSK_SPEED_MAX_FACTORS = 32, 50, 8
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -254,6 +255,10 @@ SIGNATURES = {
     "dsk_fbank_filterbank": (c_int32, [c_int32, c_void_p]),
     "dsk_wave_augment": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p,
                                    c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 5),
+    "dsk_speed_filter": (c_int32, [c_int32, c_int32, c_void_p]),
+    "dsk_wave_augment_speed": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p,
+                                         c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_int32]
+                               + [c_void_p] * 5 + [c_int32] + [c_void_p] * 3),
     "dsk_fbank_segments": (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_int32,
                                      c_void_p, c_int32, c_void_p, c_void_p]),
     "dsk_threshold_counts": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),

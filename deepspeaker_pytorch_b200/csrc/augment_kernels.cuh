@@ -1,8 +1,10 @@
 // Waveform-domain augmentation of training segments (the MUSAN + RIR recipe of Kaldi x-vectors / voxceleb_trainer):
 // a segment of int16 speech, reverberated by a room impulse response and mixed with noise sources at target SNRs.
 // Definition in include/dsk.h (dsk_wave_augment).  The call runs, on one stream:
-//   aug_check_kernel   per-example validity (indices, starts, RIR length, SNRs), read from the banks' offsets only
-//   aug_gather_kernel  s = bank[u][(start + i) mod n] * 2^-15 into out (NaN rows for invalid examples)
+//   aug_check_kernel   per-example validity (indices, starts, RIR length, SNRs, speed factor), read from the banks'
+//                      offsets only
+//   aug_speed_kernel   s = the speed-perturbed segment into out (examples with a non-unit factor only)
+//   aug_gather_kernel  s = bank[u][(start + i) mod n] * 2^-15 into out (the other examples; NaN rows for invalid ones)
 //   aug_fft_in_kernel / aug_fft_rir_kernel / aug_conv_out_kernel
 //                      uniformly partitioned overlap-save convolution, in place in out (examples with a RIR only)
 //   aug_mix_kernel     fp64 energies and the mix, in place in out (when there are noise sources)
@@ -22,16 +24,33 @@ constexpr int kAugFftThreads = 512;
 constexpr int kAugGatherThreads = 256;
 constexpr int kAugGatherPerBlock = 4 * kAugGatherThreads;
 constexpr int kAugMixThreads = 256;
+constexpr int kSpeedMaxDen = 32;                 // DSK_SPEED_MAX_DEN
+constexpr int kSpeedTaps = 50;                   // DSK_SPEED_TAPS: d = -24 .. 25
+constexpr int kSpeedMaxFactors = 8;              // DSK_SPEED_MAX_FACTORS
+constexpr int kSpeedTapStride = 51;              // odd, so rows of different phases start in different bank pairs
+constexpr int kSpeedMaxSpan = 2 * (kAugGatherPerBlock - 1) + 1 + kSpeedTaps;   // inputs of one tile at alpha = 2
+
+// ok[b] codes written by aug_check_kernel
+constexpr int kAugBad = 0, kAugGather = 1, kAugSpeed = 2;
 
 __device__ __forceinline__ float aug_nan() { return __int_as_float(0x7fc00000); }
 
-// ok[b] = 1 when every index and start of example b lies inside its bank, its RIR has 1 .. max_rir_len taps and the SNR
-// of every used noise source is finite; only offsets are read.
+__device__ __forceinline__ bool aug_speed_ratio_ok(int p, int q) {
+  if (q < 1 || q > kSpeedMaxDen || p < 1 || 2 * p < q || p > 2 * q) return false;
+  int a = p, c = q;
+  while (c) { const int t = a % c; a = c; c = t; }
+  return a == 1;
+}
+
+// ok[b] = kAugBad unless every index and start of example b lies inside its bank, its RIR has 1 .. max_rir_len taps,
+// the SNR of every used noise source is finite and its speed factor is -1 or a table entry whose ratio is within the
+// limits; then kAugSpeed for a non-unit factor, else kAugGather.  Only offsets and ratios are read.
 __global__ void aug_check_kernel(const int64_t* __restrict__ soff, int U, const int64_t* __restrict__ utt,
                                  const int64_t* __restrict__ start, int B, const int64_t* __restrict__ roff, int R,
                                  const int64_t* __restrict__ rir_idx, int max_rir_len, const int64_t* __restrict__ noff,
                                  int N, int M, const int64_t* __restrict__ noise_idx, const int64_t* __restrict__ noise_start,
-                                 const double* __restrict__ snr_db, int* __restrict__ ok) {
+                                 const double* __restrict__ snr_db, const int32_t* __restrict__ speed_ratio, int K,
+                                 const int64_t* __restrict__ speed_idx, int* __restrict__ ok) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   bool good = false;
@@ -56,7 +75,18 @@ __global__ void aug_check_kernel(const int64_t* __restrict__ soff, int U, const 
     const long n = noff[q + 1] - noff[q], st = noise_start[static_cast<long>(b) * M + j];
     good = n >= 1 && st >= 0 && st < n && isfinite(snr_db[static_cast<long>(b) * M + j]);
   }
-  ok[b] = good;
+  bool speed = false;
+  if (good && K > 0) {
+    const long k = speed_idx[b];
+    if (k >= 0 && k < K) {
+      const int p = speed_ratio[2 * k], q = speed_ratio[2 * k + 1];
+      good = aug_speed_ratio_ok(p, q);
+      speed = p != q;
+    } else {
+      good = k == -1;
+    }
+  }
+  ok[b] = good ? (speed ? kAugSpeed : kAugGather) : kAugBad;
 }
 
 // out[b][i] = bank[soff[u] + (s + i) mod n] * 2^-15 (exact in fp32); NaN for an invalid example.
@@ -68,16 +98,68 @@ aug_gather_kernel(const int16_t* __restrict__ bank, const int64_t* __restrict__ 
   const int b = blockIdx.x / tiles;
   const long i0 = static_cast<long>(blockIdx.x - b * tiles) * kAugGatherPerBlock;
   float* __restrict__ o = out + static_cast<long>(b) * L;
-  if (!ok[b]) {
+  if (ok[b] == kAugBad) {
     for (long i = i0 + threadIdx.x; i < L && i < i0 + kAugGatherPerBlock; i += kAugGatherThreads) o[i] = aug_nan();
     return;
   }
+  if (ok[b] == kAugSpeed) return;      // written by aug_speed_kernel
   const long u = utt[b], base = soff[u], n = soff[u + 1] - base;
   long p = (start[b] + i0 + threadIdx.x) % n;
   for (long i = i0 + threadIdx.x; i < L && i < i0 + kAugGatherPerBlock; i += kAugGatherThreads) {
     o[i] = static_cast<float>(bank[base + p]) * (1.0f / 32768.0f);
     p += kAugGatherThreads;
     if (p >= n) p %= n;
+  }
+}
+
+// Speed perturbation of the examples with ok[b] == kAugSpeed (definition in include/dsk.h): out[b][i] =
+// fp32((sum_{d=-24}^{25} h_r[d] x[(start + m + d) mod n]) * 2^-15), i p = m q + r, the sum in fp64 in ascending d.
+// grid = B * ceil(L / 1024) as aug_gather_kernel, block = 256, four outputs i0 + t + 256 j per thread.  The tile's
+// m_last - m_first + 50 <= 2096 input samples are staged once into shared memory (coalesced, wrapped), so each bank
+// sample is read about once per tile, together with the factor's q rows of taps; both as fp64, which makes every
+// product h x exact and the fma chain the definition's sum.
+__global__ void __launch_bounds__(kAugGatherThreads)
+aug_speed_kernel(const int16_t* __restrict__ bank, const int64_t* __restrict__ soff, const int64_t* __restrict__ utt,
+                 const int64_t* __restrict__ start, const int* __restrict__ ok, const int32_t* __restrict__ speed_ratio,
+                 const float* __restrict__ speed_taps, const int64_t* __restrict__ speed_idx, int L,
+                 float* __restrict__ out) {
+  __shared__ double xs[kSpeedMaxSpan];
+  __shared__ double hs[kSpeedMaxDen * kSpeedTapStride];
+  const int tiles = (L + kAugGatherPerBlock - 1) / kAugGatherPerBlock;
+  const int b = blockIdx.x / tiles;
+  if (ok[b] != kAugSpeed) return;
+  const long i0 = static_cast<long>(blockIdx.x - b * tiles) * kAugGatherPerBlock;
+  const long i1 = min(static_cast<long>(L), i0 + kAugGatherPerBlock) - 1;
+  const long k = speed_idx[b];
+  const int p = speed_ratio[2 * k], q = speed_ratio[2 * k + 1];
+  const long m0 = i0 * p / q, span = i1 * p / q - m0 + kSpeedTaps;
+  const long u = utt[b], base = soff[u], n = soff[u + 1] - base;
+  long pos = (start[b] + m0 - (kSpeedTaps / 2 - 1)) % n;           // x[start + m0 - 24], wrapped
+  if (pos < 0) pos += n;
+  pos = (pos + threadIdx.x) % n;
+  for (long j = threadIdx.x; j < span; j += kAugGatherThreads) {
+    xs[j] = static_cast<double>(bank[base + pos]);
+    pos += kAugGatherThreads;
+    if (pos >= n) pos %= n;
+  }
+  const float* __restrict__ h = speed_taps + k * kSpeedMaxDen * kSpeedTaps;
+  for (int e = threadIdx.x; e < q * kSpeedTaps; e += kAugGatherThreads) {
+    const int r = e / kSpeedTaps;
+    hs[r * kSpeedTapStride + (e - r * kSpeedTaps)] = static_cast<double>(h[e]);
+  }
+  __syncthreads();
+  float* __restrict__ o = out + static_cast<long>(b) * L;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const long i = i0 + threadIdx.x + j * kAugGatherThreads;
+    if (i > i1) break;
+    const long ip = i * p, m = ip / q;
+    const double* __restrict__ hr = hs + (ip - m * q) * kSpeedTapStride;
+    const double* __restrict__ xr = xs + (m - m0);
+    double acc = 0.0;
+#pragma unroll
+    for (int d = 0; d < kSpeedTaps; ++d) acc = fma(hr[d], xr[d], acc);
+    o[i] = static_cast<float>(acc * (1.0 / 32768.0));
   }
 }
 

@@ -11,6 +11,7 @@
 #include <cmath>
 #include <cstring>
 #include <map>
+#include <numeric>
 #include <string>
 #include <tuple>
 #include <vector>
@@ -4226,11 +4227,44 @@ static int32_t aug_resolve(const void* p, const void** dev, const char* what) {
   return fail(DSK_ERR_INVALID, "dsk_wave_augment: %s is pageable host memory (use device or page-locked memory)", what);
 }
 
+int32_t dsk_speed_filter(int32_t p, int32_t q, float* taps) {
+  if (!taps || p < 1 || q < 1 || q > dsk::kSpeedMaxDen || 2 * p < q || p > 2 * q || std::gcd(p, q) != 1)
+    return fail(DSK_ERR_INVALID, "dsk_speed_filter: bad arguments (need non-null taps and p / q in lowest terms with "
+                "1/2 <= p / q <= 2, q <= %d; got %d / %d)", dsk::kSpeedMaxDen, p, q);
+  const double pi = 3.141592653589793;
+  const double fc = 0.5 * 0.99 * std::min(1.0, static_cast<double>(q) / static_cast<double>(p));
+  const double zs = 12.0 / (2.0 * fc);
+  for (int32_t r = 0; r < q; ++r) {
+    for (int32_t j = 0; j < dsk::kSpeedTaps; ++j) {
+      const double tau = static_cast<double>(r) / static_cast<double>(q) - static_cast<double>(j - (dsk::kSpeedTaps / 2 - 1));
+      double h = 0.0;
+      if (std::fabs(tau) <= zs) {
+        const double x = 2.0 * fc * tau;
+        const double sinc = x == 0.0 ? 1.0 : std::sin(pi * x) / (pi * x);
+        const double w = std::cos(pi * tau / (2.0 * zs));
+        h = 2.0 * fc * sinc * (w * w);
+      }
+      taps[r * dsk::kSpeedTaps + j] = static_cast<float>(h);
+    }
+  }
+  return DSK_OK;
+}
+
 int32_t dsk_wave_augment(const int16_t* speech, const int64_t* speech_off, int32_t U, const int64_t* utt,
                          const int64_t* start, int32_t B, int32_t L, const float* rir, const int64_t* rir_off, int32_t R,
                          int32_t max_rir_len, const int64_t* rir_idx, const int16_t* noise, const int64_t* noise_off,
                          int32_t N, int32_t M, const int64_t* noise_idx, const int64_t* noise_start, const double* snr_db,
                          float* out, void* stream) {
+  return dsk_wave_augment_speed(speech, speech_off, U, utt, start, B, L, rir, rir_off, R, max_rir_len, rir_idx, noise,
+                                noise_off, N, M, noise_idx, noise_start, snr_db, nullptr, nullptr, 0, nullptr, out, stream);
+}
+
+int32_t dsk_wave_augment_speed(const int16_t* speech, const int64_t* speech_off, int32_t U, const int64_t* utt,
+                               const int64_t* start, int32_t B, int32_t L, const float* rir, const int64_t* rir_off,
+                               int32_t R, int32_t max_rir_len, const int64_t* rir_idx, const int16_t* noise,
+                               const int64_t* noise_off, int32_t N, int32_t M, const int64_t* noise_idx,
+                               const int64_t* noise_start, const double* snr_db, const int32_t* speed_ratio,
+                               const float* speed_taps, int32_t K, const int64_t* speed_idx, float* out, void* stream) {
   if (!speech || !speech_off || !utt || !start || !out || U < 1 || B < 1 || L < 1 || L > (1 << 24) || M < 0 ||
       M > dsk::kAugMaxSources || max_rir_len < 1 || max_rir_len > dsk::kAugMaxRir)
     return fail(DSK_ERR_INVALID, "dsk_wave_augment: bad arguments (need non-null speech, offsets, utt, start, out; U, B >= 1; "
@@ -4241,6 +4275,9 @@ int32_t dsk_wave_augment(const int16_t* speech, const int64_t* speech_off, int32
   if (M > 0 && (!noise || !noise_off || N < 1 || !noise_idx || !noise_start || !snr_db))
     return fail(DSK_ERR_INVALID, "dsk_wave_augment: M = %d sources need a noise bank (N >= 1; got %d) and non-null "
                 "noise_idx, noise_start, snr_db", M, N);
+  if (K < 0 || K > dsk::kSpeedMaxFactors || (K > 0 && (!speed_ratio || !speed_taps || !speed_idx)))
+    return fail(DSK_ERR_INVALID, "dsk_wave_augment: need 0 <= K <= %d speed factors, with non-null speed_ratio, "
+                "speed_taps and speed_idx when K > 0; got K %d", dsk::kSpeedMaxFactors, K);
   const int64_t tiles = (L + dsk::kAugGatherPerBlock - 1) / dsk::kAugGatherPerBlock;
   const int64_t nb = (L + dsk::kAugPart - 1) / dsk::kAugPart, kp = (max_rir_len + dsk::kAugPart - 1) / dsk::kAugPart;
   if (B * tiles >= (1ll << 31) || B * nb >= (1ll << 31) || B * kp >= (1ll << 31))
@@ -4273,8 +4310,13 @@ int32_t dsk_wave_augment(const int16_t* speech, const int64_t* speech_off, int32
   float2* X = reinterpret_cast<float2*>(scratch + ok_bytes);
   float2* H = X + x_elems;
   dsk::aug_check_kernel<<<(B + 255) / 256, 256, 0, s>>>(d_soff, U, utt, start, B, d_roff, R, rir_idx, max_rir_len, d_noff, N, M,
-                                                        noise_idx, noise_start, snr_db, ok);
+                                                        noise_idx, noise_start, snr_db, speed_ratio, K, speed_idx, ok);
   KERNEL_CHECK();
+  if (K > 0) {
+    dsk::aug_speed_kernel<<<static_cast<unsigned>(B * tiles), dsk::kAugGatherThreads, 0, s>>>(
+        d_speech, d_soff, utt, start, ok, speed_ratio, speed_taps, speed_idx, L, out);
+    KERNEL_CHECK();
+  }
   dsk::aug_gather_kernel<<<static_cast<unsigned>(B * tiles), dsk::kAugGatherThreads, 0, s>>>(d_speech, d_soff, utt, start, ok, L, out);
   KERNEL_CHECK();
   if (rir_idx) {

@@ -24,10 +24,13 @@ each utterance's speech frames (``embed_utterances(model, bank.select(bank.speec
 ``augmented_crops`` gathers each step's segments, reverberates them by a ``RirBank`` RIR, mixes noise sources at target
 SNRs (``augment_plan`` draws them on the host) and computes their features, all on the device with no host
 synchronisation.  Training features then subtract the segment's own mean; ``FeatureBank`` subtracts the utterance's.
+``augment_plan(..., speeds=(0.9, 1.0, 1.1))`` adds speed perturbation in front of the reverb (a windowed-sinc resampler
+on the device), and ``speed_labels`` gives each perturbed copy of a speaker a class of its own.
 """
 from __future__ import annotations
 
 import ctypes
+from fractions import Fraction
 
 import numpy as np
 import torch
@@ -505,16 +508,34 @@ class WaveBank:
         dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         return cls(host.pin_memory().to(dev), off)
 
-    def random_starts(self, utt, L: int, generator=None) -> torch.Tensor:
-        """``random_starts`` over this bank's sample counts: uniform in [0, n - L], 0 when n < L (host int64)."""
-        return random_starts(self.lengths, utt, L, generator)
+    def random_starts(self, utt, L: int, generator=None, plan=None) -> torch.Tensor:
+        """``random_starts`` over this bank's sample counts: uniform in [0, n - L], 0 when n < L (host int64).  With a
+        ``plan`` that has speeds, example b reads about alpha_b L input samples, so its start is uniform in
+        [0, n - ceil(alpha_b L)] (0 when that is negative).  Draw the plan first, then the starts from it: a plan's
+        draws do not depend on the starts, and without a plan (or without speeds) the draws are those of
+        ``random_starts``.  A CUDA ``speed_idx`` is read back to the host."""
+        if plan is None or plan.get("speed_idx") is None:
+            return random_starts(self.lengths, utt, L, generator)
+        u = _host_int64(utt, "random_starts")
+        if u.size and (u.min() < 0 or u.max() >= self.num_utterances):
+            raise ValueError(f"random_starts: utterance index outside [0, {self.num_utterances})")
+        speeds = _speed_factors(plan.get("speeds"), "random_starts")
+        k = _host_int64(plan["speed_idx"], "random_starts")
+        if k.shape != u.shape or (k.size and (k.min() < -1 or k.max() >= len(speeds))):
+            raise ValueError(f"random_starts: speed_idx must be ({u.size},) in [-1, {len(speeds)})")
+        p = np.array([1] + [a.numerator for a in speeds], np.int64)[k + 1]
+        q = np.array([1] + [a.denominator for a in speeds], np.int64)[k + 1]
+        need = -(-p * int(L) // q)                           # ceil(alpha L)
+        hi = np.maximum(self.lengths[u] - need, 0)
+        return torch.from_numpy(_rng(generator).integers(0, hi + 1, dtype=np.int64) if u.size else np.zeros(0, np.int64))
 
     def segments(self, utt, start, L: int, plan=None, rir_bank=None, noise_bank=None) -> torch.Tensor:
-        """(B, L) fp32 augmented audio (``dsk_wave_augment``): segment b is samples ``start[b]`` .. of utterance
-        ``utt[b]`` (wrapping) times 2^-15, reverberated by RIR ``plan["rir_idx"][b]`` of ``rir_bank`` and mixed with the
-        sources of ``plan`` from ``noise_bank`` (see ``augment_plan``).  No plan: the clean segments.  CPU indices are
-        checked on the host (ValueError); CUDA ones are not: an example with an index, start or SNR out of range comes
-        out NaN.  No host synchronisation."""
+        """(B, L) fp32 augmented audio (``dsk_wave_augment_speed``): segment b is samples ``start[b]`` .. of utterance
+        ``utt[b]`` (wrapping) times 2^-15, resampled by the speed factor ``plan["speeds"][plan["speed_idx"][b]]`` (-1:
+        none), reverberated by RIR ``plan["rir_idx"][b]`` of ``rir_bank`` and mixed with the sources of ``plan`` from
+        ``noise_bank`` (see ``augment_plan``).  No plan: the clean segments.  CPU indices are checked on the host
+        (ValueError); CUDA ones are not: an example with an index, start, SNR or speed index out of range comes out NaN.
+        No host synchronisation once the plan's speed table is on the device."""
         u, s = _index_pair(utt, start, "segments")
         B, L = u.numel(), int(L)
         if not 1 <= L <= 1 << 24:
@@ -537,6 +558,17 @@ class WaveBank:
                 raise ValueError(f"segments: at most {AUG_MAX_SOURCES} noise sources, got {M}")
             if M and noise_bank is None:
                 raise ValueError("segments: the plan adds noise but no noise_bank is given")
+        speed_idx, K = plan.get("speed_idx"), 0
+        if speed_idx is not None:
+            speeds = _speed_factors(plan.get("speeds"), "segments")
+            K = len(speeds)
+            speed_idx = torch.as_tensor(speed_idx)
+            if speed_idx.shape != u.shape or speed_idx.is_floating_point():
+                raise ValueError(f"segments: speed_idx must be integer (B,) with B = {B}")
+            if not speed_idx.is_cuda:
+                k = speed_idx.to(torch.int64).numpy()
+                if k.min() < -1 or k.max() >= K:
+                    raise ValueError(f"segments: speed_idx outside [-1, {K})")
         if not u.is_cuda:
             _check_host_index(u, s, self.lengths, "segments")
         if rir_idx is not None:
@@ -567,14 +599,19 @@ class WaveBank:
             ni = ns = sd = None
         rb = rir_bank if ri is not None else None
         nb = noise_bank if M else None
+        si, ratio, taps = None, None, None
+        if K:
+            si = _to_dev(speed_idx, torch.int64, dev)
+            ratio, taps = _speed_table(dev, speeds)
         ptr = _lib.ptr
         with torch.cuda.device(dev):
-            _lib.check(_lib.load().dsk_wave_augment(
+            _lib.check(_lib.load().dsk_wave_augment_speed(
                 self.samples.data_ptr(), self.offsets.data_ptr(), self.num_utterances, u.data_ptr(), s.data_ptr(), B, L,
                 ptr(rb.samples if rb else None), ptr(rb.offsets if rb else None), rb.num_rirs if rb else 0,
                 rb.max_len if rb else 1, ptr(ri),
                 ptr(nb.samples if nb else None), ptr(nb.offsets if nb else None), nb.num_utterances if nb else 0, M,
-                ptr(ni), ptr(ns), ptr(sd), out.data_ptr(), _lib.cur_stream()), "dsk_wave_augment")
+                ptr(ni), ptr(ns), ptr(sd), ptr(ratio), ptr(taps), K, ptr(si), out.data_ptr(), _lib.cur_stream()),
+                "dsk_wave_augment_speed")
         return out
 
     def augmented_crops(self, utt, start, T: int, plan=None, rir_bank=None, noise_bank=None, time_masks=None,
@@ -643,15 +680,30 @@ class RirBank:
 
 
 def augment_plan(B: int, L: int, generator=None, rir_bank=None, p_reverb: float = 0.5, noise_bank=None,
-                 noise_groups=(), p_noise: float = 0.5):
+                 noise_groups=(), p_noise: float = 0.5, speeds=None, speed_weights=None):
     """Host: a random augmentation plan for B segments of L samples, as a dict of CPU tensors ``rir_idx`` (B,) int64,
     ``noise_idx``, ``noise_start`` (B, M) int64 and ``snr_db`` (B, M) fp64, M the largest source count of any group and
     unused slots -1 (start 0, SNR 0).  Per example: with probability ``p_reverb`` a uniform RIR of ``rir_bank`` (else
     -1); with probability ``p_noise`` one of ``noise_groups`` chosen by weight, then a uniform source count, uniform
     utterances, uniform starts in [0, n - L] (0 when n < L: the source wraps) and a uniform SNR.  A group is
     ``(utterance ids in noise_bank, (snr_lo_db, snr_hi_db), (count_lo, count_hi), weight)``.  ``generator`` is a
-    ``numpy.random.Generator``; the same state gives the same plan."""
+    ``numpy.random.Generator``; the same state gives the same plan.
+
+    ``speeds``: up to 8 distinct speed factors (floats or ``Fraction``s, each taken exactly, 0.9 as 9/10; each a ratio
+    p / q with 1/2 <= p / q <= 2 and q <= 32), drawn per example by ``speed_weights`` (default uniform) in one draw
+    after all the others, so the other keys are the same with or without speeds for one generator state.  The plan
+    then also holds ``speed_idx`` (B,) int64 and ``speeds`` (a tuple of ``Fraction``s, host metadata).  Draw the starts
+    after the plan with ``WaveBank.random_starts(utt, L, generator, plan)``, and the labels with ``speed_labels``."""
     g = _rng(generator)
+    if speeds is not None:
+        speeds = _speed_factors(speeds, "augment_plan")
+        if len(set(speeds)) != len(speeds):
+            raise ValueError(f"augment_plan: the speed factors must be distinct, got {[str(a) for a in speeds]}")
+        sw = np.ones(len(speeds)) if speed_weights is None else np.asarray(speed_weights, np.float64).reshape(-1)
+        if sw.shape != (len(speeds),) or not np.all(np.isfinite(sw)) or sw.min() < 0 or sw.sum() <= 0:
+            raise ValueError(f"augment_plan: speed_weights must be {len(speeds)} finite weights >= 0 with a positive sum")
+    elif speed_weights is not None:
+        raise ValueError("augment_plan: speed_weights without speeds")
     B, L = int(B), int(L)
     if B < 0 or L < 1 or not (0.0 <= p_reverb <= 1.0 and 0.0 <= p_noise <= 1.0):
         raise ValueError(f"augment_plan: need B >= 0, L >= 1 and probabilities in [0, 1] (got {B}, {L}, {p_reverb}, {p_noise})")
@@ -689,8 +741,95 @@ def augment_plan(B: int, L: int, generator=None, rir_bank=None, p_reverb: float 
             noise_idx[b, :c] = q
             noise_start[b, :c] = g.integers(0, np.maximum(noise_bank.lengths[q] - L, 0) + 1)
             snr_db[b, :c] = g.uniform(slo, shi, c)
-    return {"rir_idx": torch.from_numpy(rir_idx), "noise_idx": torch.from_numpy(noise_idx),
+    plan = {"rir_idx": torch.from_numpy(rir_idx), "noise_idx": torch.from_numpy(noise_idx),
             "noise_start": torch.from_numpy(noise_start), "snr_db": torch.from_numpy(snr_db)}
+    if speeds is not None:
+        plan["speed_idx"] = torch.from_numpy(g.choice(len(speeds), size=B, p=sw / sw.sum()).astype(np.int64))
+        plan["speeds"] = speeds
+    return plan
+
+
+# ---- speed perturbation ------------------------------------------------------------------------------------------------
+SPEED_MAX_DEN = 32
+SPEED_TAPS = 50
+SPEED_MAX_FACTORS = 8
+
+
+def speed_factor(a) -> Fraction:
+    """The exact ratio of a speed factor: a float through its shortest decimal form (0.9 -> 9/10), an int or a
+    ``Fraction`` as is.  ValueError unless 1/2 <= alpha <= 2 with a denominator of at most 32."""
+    if isinstance(a, bool) or not isinstance(a, (int, float, Fraction, np.integer, np.floating)):
+        raise ValueError(f"speed factor: expected a number, got {a!r}")
+    if isinstance(a, (float, np.floating)):
+        if not np.isfinite(a):
+            raise ValueError(f"speed factor: {a} is not finite")
+        f = Fraction(str(float(a)))
+    else:
+        f = Fraction(a)
+    if not (Fraction(1, 2) <= f <= 2) or f.denominator > SPEED_MAX_DEN:
+        raise ValueError(f"speed factor {a} = {f}: need 1/2 <= p / q <= 2 and q <= {SPEED_MAX_DEN}")
+    return f
+
+
+def _speed_factors(speeds, what):
+    if speeds is None:
+        raise ValueError(f"{what}: speed_idx needs the plan's speeds")
+    out = tuple(speed_factor(a) for a in speeds)
+    if not 1 <= len(out) <= SPEED_MAX_FACTORS:
+        raise ValueError(f"{what}: need 1 .. {SPEED_MAX_FACTORS} speed factors, got {len(out)}")
+    return out
+
+
+def speed_filter(alpha) -> np.ndarray:
+    """Host: the (q, 50) fp32 polyphase taps of the factor alpha = p / q (``dsk_speed_filter``)."""
+    f = speed_factor(alpha)
+    taps = np.empty((f.denominator, SPEED_TAPS), np.float32)
+    L.check(L.load().dsk_speed_filter(f.numerator, f.denominator, taps.ctypes.data_as(ctypes.c_void_p)),
+            "dsk_speed_filter")
+    return taps
+
+
+_SPEED_CACHE = {}
+
+
+def _speed_table(dev, speeds):
+    """(ratio (K, 2) int32, taps (K, 32, 50) fp32) of the factors ``speeds`` on ``dev``, uploaded once per (device,
+    factors)."""
+    key = (dev.index, tuple(speeds))
+    if key not in _SPEED_CACHE:
+        ratio = np.array([[a.numerator, a.denominator] for a in speeds], np.int32)
+        taps = np.zeros((len(speeds), SPEED_MAX_DEN, SPEED_TAPS), np.float32)
+        for k, a in enumerate(speeds):
+            taps[k, :a.denominator] = speed_filter(a)
+        _SPEED_CACHE[key] = (torch.from_numpy(ratio).to(dev), torch.from_numpy(taps).to(dev))
+    return _SPEED_CACHE[key]
+
+
+def speed_labels(labels, plan, num_speakers: int) -> torch.Tensor:
+    """Labels of speed-perturbed examples as new classes ("speed perturb + extend speakers"): labels[b] +
+    num_speakers * j_b, j_b = 0 for a unit factor or speed_idx -1, else the 1-based rank (by value) of the example's
+    factor among the plan's non-unit factors, so the classifier has num_speakers * (1 + #non-unit factors) classes.  A
+    plan without speeds leaves the labels as they are.  On the labels' device; a CPU speed_idx is checked (ValueError),
+    a CUDA one is not (an out-of-range example, NaN in ``segments``, keeps its label)."""
+    lab = torch.as_tensor(labels)
+    if lab.dim() != 1 or lab.is_floating_point() or int(num_speakers) < 1:
+        raise ValueError(f"speed_labels: need 1-D integer labels and num_speakers >= 1, got {tuple(lab.shape)} "
+                         f"{lab.dtype}, {num_speakers}")
+    lab = lab.to(torch.int64)
+    if plan is None or plan.get("speed_idx") is None:
+        return lab
+    speeds = _speed_factors(plan.get("speeds"), "speed_labels")
+    ranked = sorted(a for a in speeds if a != 1)
+    j = [0] + [0 if a == 1 else 1 + ranked.index(a) for a in speeds]
+    k = torch.as_tensor(plan["speed_idx"])
+    if k.shape != lab.shape or k.is_floating_point():
+        raise ValueError(f"speed_labels: speed_idx must be integer ({lab.numel()},)")
+    if not k.is_cuda and k.numel() and (int(k.min()) < -1 or int(k.max()) >= len(speeds)):
+        raise ValueError(f"speed_labels: speed_idx outside [-1, {len(speeds)})")
+    k = k.to(lab.device, torch.int64) + 1
+    lut = torch.tensor(j, dtype=torch.int64, device=lab.device)
+    valid = (k >= 0) & (k <= len(speeds))
+    return lab + int(num_speakers) * torch.where(valid, lut[k.clamp(0, len(speeds))], 0)
 
 
 def _index_pair(utt, start, what):

@@ -784,15 +784,44 @@ int32_t dsk_gather_runs(const float* feat, const int64_t* frame_off, int32_t U, 
  *     segments audio (B, L) fp32: row b is dsk_fbank on audio[b] alone (pre-emphasis from the segment's first sample;
  *     with subtract_mean, the mean over the segment's own T frames), then the SpecAugment masks exactly as
  *     dsk_fbank_crops applies them.  fb: the device copy of dsk_fbank_filterbank(sample_rate).  No host
- *     synchronisation.  For training, take L = flen + (T - 1) step samples (25 840 at 16 kHz for T = 160). */
+ *     synchronisation.  For training, take L = flen + (T - 1) step samples (25 840 at 16 kHz for T = 160).
+ *   Speed perturbation (the "speed perturb + extend speakers" recipe: tempo and pitch change together).  A factor is a
+ *     ratio alpha = p / q in lowest terms with 1/2 <= alpha <= 2 and q <= DSK_SPEED_MAX_DEN.  Output sample i reads
+ *     the input at time i alpha (a tone at f comes out at alpha f; alpha < 1 slows the speech down).  With
+ *     i p = m_i q + r_i, 0 <= r_i < q:
+ *       s[i] = ( sum_{d = -24}^{25} h_{r_i}[d] * x[(start + m_i + d) mod n_u] ) * 2^-15   (fp64, d ascending, one
+ *              rounding to fp32; x the int16 utterance, the wrap applied to negative indices too)
+ *       h_r[d] = fp32(h(r / q - d)),  h(tau) = 2 f_c sinc(2 f_c tau) cos^2(pi tau / (2 Z_s)) for |tau| <= Z_s, else 0,
+ *       f_c = 0.5 * 0.99 * min(1, 1 / alpha),  Z_s = 12 / (2 f_c)   (12 zero crossings; |tau| <= 24.24, so the
+ *       DSK_SPEED_TAPS = 50 taps d = -24 .. 25 cover every allowed alpha).
+ *     A Hann-windowed sinc (the family of common resamplers); parity with sox or torchaudio is unpinned.  A factor of
+ *     exactly 1 (or speed_idx -1) is the plain gather, bit for bit.  Speed comes first: reverb and noise act on the
+ *     perturbed segment s, and the SNR is measured against it; noise sources are not perturbed.
+ *   dsk_speed_filter: host only.  taps (q, DSK_SPEED_TAPS) fp32, row r = h_r[-24 .. 25], built in fp64 and rounded once.
+ *     DSK_ERR_INVALID for a null taps or a ratio outside the limits or not in lowest terms.
+ *   dsk_wave_augment_speed: dsk_wave_augment plus speed_ratio (K, 2) int32 (p, q), speed_taps (K, DSK_SPEED_MAX_DEN,
+ *     DSK_SPEED_TAPS) fp32 (factor k's dsk_speed_filter rows, the rest unread), 0 <= K <= DSK_SPEED_MAX_FACTORS and
+ *     speed_idx (B,) int64 (factor of example b, -1 = none), all device arrays (NULL when K = 0).  A speed_idx outside
+ *     [-1, K) or a table ratio outside the limits makes that example NaN, checked on the device like the other
+ *     per-example arguments.  dsk_wave_augment is the K = 0 call. */
 #define DSK_AUG_MAX_SOURCES 8
 #define DSK_AUG_MAX_RIR 65536
+#define DSK_SPEED_MAX_DEN 32
+#define DSK_SPEED_TAPS 50
+#define DSK_SPEED_MAX_FACTORS 8
 int32_t dsk_fbank_filterbank(int32_t sample_rate, float* fb);
 int32_t dsk_wave_augment(const int16_t* speech, const int64_t* speech_off, int32_t U, const int64_t* utt,
                          const int64_t* start, int32_t B, int32_t L, const float* rir, const int64_t* rir_off, int32_t R,
                          int32_t max_rir_len, const int64_t* rir_idx, const int16_t* noise, const int64_t* noise_off,
                          int32_t N, int32_t M, const int64_t* noise_idx, const int64_t* noise_start, const double* snr_db,
                          float* out, void* stream);
+int32_t dsk_speed_filter(int32_t p, int32_t q, float* taps);
+int32_t dsk_wave_augment_speed(const int16_t* speech, const int64_t* speech_off, int32_t U, const int64_t* utt,
+                               const int64_t* start, int32_t B, int32_t L, const float* rir, const int64_t* rir_off,
+                               int32_t R, int32_t max_rir_len, const int64_t* rir_idx, const int16_t* noise,
+                               const int64_t* noise_off, int32_t N, int32_t M, const int64_t* noise_idx,
+                               const int64_t* noise_start, const double* snr_db, const int32_t* speed_ratio,
+                               const float* speed_taps, int32_t K, const int64_t* speed_idx, float* out, void* stream);
 int32_t dsk_fbank_segments(const float* audio, int32_t B, int32_t L, int32_t sample_rate, int32_t log_scale,
                            int32_t subtract_mean, const float* fb, const int32_t* time_masks, int32_t n_time,
                            const int32_t* freq_masks, int32_t n_freq, float* out, void* stream);
