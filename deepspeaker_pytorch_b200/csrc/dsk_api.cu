@@ -3948,17 +3948,28 @@ int32_t dsk_pipeline_lane_stream(dsk_pipeline p, int32_t lane, void** stream_out
 // ---- log-fbank front-end (audio_processing.py:9-36) ------------------------------------------------------------------
 static long fbank_round_half_up(double v) { return static_cast<long>(std::floor(v + 0.5)); }
 
+// A rate the front-end can frame: a 10 ms step of at least one sample (a zero step has no frame count) and a 25 ms
+// frame within NFFT = 512, that is DSK_FBANK_MIN_RATE <= sample_rate <= DSK_FBANK_MAX_RATE.
+static bool fbank_rate_ok(int32_t sample_rate) {
+  return sample_rate > 0 && fbank_round_half_up(0.01 * sample_rate) >= 1 &&
+         fbank_round_half_up(0.025 * sample_rate) <= dsk::kFbNfft;
+}
+
+#define FBANK_RATE_MSG "sample_rate must lie in [50, 20499] Hz"
+
 int64_t dsk_fbank_num_frames(int64_t n_samples, int32_t sample_rate) {
-  if (n_samples <= 0 || sample_rate <= 0) return 0;
+  if (n_samples <= 0 || !fbank_rate_ok(sample_rate)) return 0;
   const long flen = fbank_round_half_up(0.025 * sample_rate), step = fbank_round_half_up(0.01 * sample_rate);
   if (n_samples <= flen) return 1;
   return 1 + static_cast<int64_t>(std::ceil((static_cast<double>(n_samples) - flen) / step));
 }
 
 int32_t dsk_fbank_frame_offsets(const int64_t* sample_off, int32_t U, int32_t sample_rate, int64_t* frame_off) {
-  if (!sample_off || !frame_off || U < 1 || sample_rate <= 0 || sample_off[0] < 0)
-    return fail(DSK_ERR_INVALID, "dsk_fbank_frame_offsets: bad arguments (need non-null offsets, U >= 1, sample_rate > 0, "
-                "sample_off[0] >= 0; got U %d, sample_rate %d)", U, sample_rate);
+  if (!sample_off || !frame_off || U < 1 || sample_off[0] < 0)
+    return fail(DSK_ERR_INVALID, "dsk_fbank_frame_offsets: bad arguments (need non-null offsets, U >= 1, "
+                "sample_off[0] >= 0; got U %d)", U);
+  if (!fbank_rate_ok(sample_rate))
+    return fail(DSK_ERR_INVALID, "dsk_fbank_frame_offsets: " FBANK_RATE_MSG ", got %d", sample_rate);
   frame_off[0] = 0;
   for (int32_t u = 0; u < U; ++u) {
     const int64_t len = sample_off[u + 1] - sample_off[u];
@@ -3971,8 +3982,9 @@ int32_t dsk_fbank_frame_offsets(const int64_t* sample_off, int32_t U, int32_t sa
 }
 
 int32_t dsk_fbank_filterbank(int32_t sample_rate, float* fb) {
-  if (!fb || sample_rate <= 0)
-    return fail(DSK_ERR_INVALID, "dsk_fbank_filterbank: bad arguments (need non-null fb and sample_rate > 0; got %d)", sample_rate);
+  if (!fb) return fail(DSK_ERR_INVALID, "dsk_fbank_filterbank: fb is null");
+  if (!fbank_rate_ok(sample_rate))
+    return fail(DSK_ERR_INVALID, "dsk_fbank_filterbank: " FBANK_RATE_MSG ", got %d", sample_rate);
   // python_speech_features.get_filterbanks(nfilt=64, nfft=512, samplerate, lowfreq=0, highfreq=samplerate/2)
   std::fill(fb, fb + static_cast<size_t>(dsk::kFbFilters) * dsk::kFbBins, 0.f);
   auto hz2mel = [](double hz) { return 2595.0 * std::log10(1.0 + hz / 700.0); };
@@ -4004,13 +4016,13 @@ static int32_t fbank_batch(const float* audio, const int64_t* sample_off, int32_
                            int32_t subtract_mean, float* feat, const FbankVad* vad, void* stream) {
   if (!audio || !feat || !sample_off || U < 1)
     return fail(DSK_ERR_INVALID, "dsk_fbank_batch: bad arguments (need non-null pointers and U >= 1; got U %d)", U);
+  if (!fbank_rate_ok(sample_rate)) return fail(DSK_ERR_INVALID, "dsk_fbank_batch: " FBANK_RATE_MSG ", got %d", sample_rate);
   const long flen = fbank_round_half_up(0.025 * sample_rate), step = fbank_round_half_up(0.01 * sample_rate);
   std::vector<int64_t> off(3 * (static_cast<size_t>(U) + 1));   // soff | foff | boff
   std::copy(sample_off, sample_off + U + 1, off.begin());
   int64_t* foff = off.data() + (U + 1);
   int64_t* boff = foff + (U + 1);
   if (int32_t rc = dsk_fbank_frame_offsets(sample_off, U, sample_rate, foff)) return rc;
-  if (flen > dsk::kFbNfft) return fail(DSK_ERR_INVALID, "dsk_fbank_batch: the 25 ms frame (%ld samples) exceeds NFFT = 512", flen);
   boff[0] = 0;
   for (int32_t u = 0; u < U; ++u)
     boff[u + 1] = boff[u] + (foff[u + 1] - foff[u] + dsk::kFbFramesPerBlock - 1) / dsk::kFbFramesPerBlock;
@@ -4137,8 +4149,9 @@ int32_t dsk_gather_runs(const float* feat, const int64_t* frame_off, int32_t U, 
 
 int32_t dsk_fbank(const float* audio, int64_t n_samples, int32_t sample_rate, int32_t log_scale, int32_t subtract_mean,
                   float* feat, void* stream) {
-  if (!audio || !feat || n_samples <= 0 || n_samples >= (1ll << 31) || sample_rate <= 0)
+  if (!audio || !feat || n_samples <= 0 || n_samples >= (1ll << 31))
     return fail(DSK_ERR_INVALID, "dsk_fbank: bad arguments");
+  if (!fbank_rate_ok(sample_rate)) return fail(DSK_ERR_INVALID, "dsk_fbank: " FBANK_RATE_MSG ", got %d", sample_rate);
   const int64_t sample_off[2] = {0, n_samples};
   return dsk_fbank_batch(audio, sample_off, 1, sample_rate, log_scale, subtract_mean, feat, stream);
 }
@@ -4163,14 +4176,13 @@ int32_t dsk_fbank_crops(const float* feat, const int64_t* frame_off, int32_t U, 
 int32_t dsk_fbank_segments(const float* audio, int32_t B, int32_t L, int32_t sample_rate, int32_t log_scale,
                            int32_t subtract_mean, const float* fb, const int32_t* time_masks, int32_t n_time,
                            const int32_t* freq_masks, int32_t n_freq, float* out, void* stream) {
-  if (!audio || !fb || !out || B < 1 || L < 1 || sample_rate <= 0 || n_time < 0 || n_freq < 0 ||
-      (n_time > 0 && !time_masks) || (n_freq > 0 && !freq_masks))
-    return fail(DSK_ERR_INVALID, "dsk_fbank_segments: bad arguments (need non-null pointers, B, L >= 1, sample_rate > 0, "
-                "n_time, n_freq >= 0 with their masks; got B %d, L %d, sample_rate %d, n_time %d, n_freq %d)", B, L,
-                sample_rate, n_time, n_freq);
+  if (!audio || !fb || !out || B < 1 || L < 1 || n_time < 0 || n_freq < 0 || (n_time > 0 && !time_masks) ||
+      (n_freq > 0 && !freq_masks))
+    return fail(DSK_ERR_INVALID, "dsk_fbank_segments: bad arguments (need non-null pointers, B, L >= 1, "
+                "n_time, n_freq >= 0 with their masks; got B %d, L %d, n_time %d, n_freq %d)", B, L, n_time, n_freq);
+  if (!fbank_rate_ok(sample_rate)) return fail(DSK_ERR_INVALID, "dsk_fbank_segments: " FBANK_RATE_MSG ", got %d", sample_rate);
   if (reinterpret_cast<uintptr_t>(out) & 15) return fail(DSK_ERR_INVALID, "dsk_fbank_segments: out must be 16-byte aligned");
   const long flen = fbank_round_half_up(0.025 * sample_rate), step = fbank_round_half_up(0.01 * sample_rate);
-  if (flen > dsk::kFbNfft) return fail(DSK_ERR_INVALID, "dsk_fbank_segments: the 25 ms frame (%ld samples) exceeds NFFT = 512", flen);
   const int64_t T = dsk_fbank_num_frames(L, sample_rate);
   const int64_t blocks_per = (T + dsk::kFbFramesPerBlock - 1) / dsk::kFbFramesPerBlock, nblk = blocks_per * B;
   const int64_t mask_grid = static_cast<int64_t>(B) * ((T + dsk::kCropRows - 1) / dsk::kCropRows);

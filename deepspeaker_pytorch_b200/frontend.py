@@ -52,10 +52,24 @@ def _ptr64(a):
     return a.ctypes.data_as(ctypes.c_void_p)
 
 
+# The rates the front-end frames: a 10 ms step of at least one sample and a 25 ms frame within NFFT = 512 (dsk.h)
+FBANK_MIN_RATE, FBANK_MAX_RATE = 50, 20499
+
+
+def _fbank_step(sample_rate, what="fbank"):
+    """(flen, step) of ``sample_rate``; ValueError unless it is an integer in [FBANK_MIN_RATE, FBANK_MAX_RATE]."""
+    sr = float(sample_rate)
+    if not sr.is_integer() or not FBANK_MIN_RATE <= sr <= FBANK_MAX_RATE:
+        raise ValueError(f"{what}: sample_rate must be an integer in [{FBANK_MIN_RATE}, {FBANK_MAX_RATE}] Hz (a 10 ms "
+                         f"step of at least one sample, a 25 ms frame of at most 512), got {sample_rate}")
+    return int(np.floor(0.025 * sr + 0.5)), int(np.floor(0.01 * sr + 0.5))
+
+
 def fbank_frame_offsets(lengths, sample_rate: int = 16000) -> np.ndarray:
     """Host only: frame offsets (U + 1,) int64 of utterances of ``lengths`` samples; utterance u gets
-    ``dsk_fbank_num_frames(lengths[u], sample_rate)`` frames.  ValueError for an empty list or a length outside
-    [1, 2^31)."""
+    ``dsk_fbank_num_frames(lengths[u], sample_rate)`` frames.  ValueError for an empty list, a length outside
+    [1, 2^31) or a sample rate outside [FBANK_MIN_RATE, FBANK_MAX_RATE]."""
+    _fbank_step(sample_rate, "fbank_frame_offsets")
     lens = _host_int64(lengths, "fbank_frame_offsets")
     if lens.size == 0:
         raise ValueError("fbank_frame_offsets: no utterances")
@@ -69,6 +83,7 @@ def fbank_frame_offsets(lengths, sample_rate: int = 16000) -> np.ndarray:
 
 
 def _fbank_batch(audio, lengths, sample_rate, use_logscale, subtract_mean, vad, what):
+    _fbank_step(sample_rate, what)
     if not isinstance(audio, torch.Tensor) or not audio.is_cuda:
         raise RuntimeError(f"{what} needs a CUDA tensor; there is no CPU fallback")
     if isinstance(lengths, torch.Tensor) and lengths.is_cuda:
@@ -99,8 +114,8 @@ def mk_mfb_batch(audio: torch.Tensor, lengths, sample_rate: int = 16000, use_log
     """``audio``: 1-D fp32 CUDA tensor, U waveforms concatenated; ``lengths`` (U,) samples per waveform, on the host
     -> ``(feats (F, 64) fp32 CUDA, offsets (U + 1,) int64 CPU)``: rows ``offsets[u]:offsets[u+1]`` are utterance u's,
     bit-identical to ``mk_mfb`` on that waveform alone.  One launch sequence and one host synchronisation per call.
-    RuntimeError for a CPU tensor; ValueError for a zero length or lengths that do not add up to ``audio``, before any
-    launch."""
+    RuntimeError for a CPU tensor; ValueError for a zero length, lengths that do not add up to ``audio`` or a sample
+    rate outside [FBANK_MIN_RATE, FBANK_MAX_RATE] = [50, 20499] Hz, before any launch."""
     return _fbank_batch(audio, lengths, sample_rate, use_logscale, subtract_mean, None, "mk_mfb_batch")
 
 
@@ -426,13 +441,10 @@ def _filterbank(dev, sample_rate: int) -> torch.Tensor:
     return _FB_CACHE[key]
 
 
-def _fbank_step(sample_rate: int):
-    return int(np.floor(0.025 * sample_rate + 0.5)), int(np.floor(0.01 * sample_rate + 0.5))
-
-
 def segment_samples(T: int, sample_rate: int = 16000) -> int:
-    """Samples L = flen + (T - 1) step of a segment whose log-fbank has exactly T frames (25 840 at 16 kHz, T = 160)."""
-    flen, step = _fbank_step(sample_rate)
+    """Samples L = flen + (T - 1) step of a segment whose log-fbank has exactly T frames (25 840 at 16 kHz, T = 160).
+    ValueError for a sample rate outside [FBANK_MIN_RATE, FBANK_MAX_RATE] = [50, 20499] Hz."""
+    flen, step = _fbank_step(sample_rate, "segment_samples")
     return flen + (int(T) - 1) * step
 
 
@@ -620,7 +632,8 @@ class WaveBank:
         """(B, 1, T, 64) fp32 training input: ``mk_mfb`` of each augmented segment of ``segment_samples(T)`` samples
         (``segments``), the mean subtracted over the segment's own T frames, then the SpecAugment masks exactly as
         ``FeatureBank.crops`` applies them.  ``start`` counts samples.  No host synchronisation once the filterbank of
-        ``sample_rate`` is on the device."""
+        ``sample_rate`` is on the device.  ValueError for a sample rate outside [FBANK_MIN_RATE, FBANK_MAX_RATE]."""
+        _fbank_step(sample_rate, "augmented_crops")
         Ls = segment_samples(T, sample_rate)
         if T < 1 or L.load().dsk_fbank_num_frames(Ls, int(sample_rate)) != T:
             raise ValueError(f"augmented_crops: no segment length gives T = {T} frames at {sample_rate} Hz")

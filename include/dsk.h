@@ -684,7 +684,16 @@ int32_t dsk_pipeline_lane_stream(dsk_pipeline p, int32_t lane, void** stream_out
  * filters, zeros -> eps).  A NaN or infinite sample makes every frame whose pre-emphasised window covers it (the
  * sample and the next) NaN in all 64 filters, log floor included, as numpy.maximum does; with subtract_mean the
  * utterance's mean, so all its features, are NaN.  This holds for dsk_fbank_batch (the other utterances keep their
- * bits) and dsk_fbank_segments (so an example dsk_wave_augment made NaN is all NaN). */
+ * bits) and dsk_fbank_segments (so an example dsk_wave_augment made NaN is all NaN).
+ * Sample rates: a frame is flen = round_half_up(0.025 sr) samples every step = round_half_up(0.01 sr), and the front-end
+ * needs step >= 1 and flen <= 512, that is DSK_FBANK_MIN_RATE <= sample_rate <= DSK_FBANK_MAX_RATE (50 Hz: flen 1,
+ * step 1; 20 499 Hz: flen 512).  Every fbank entry point fails with DSK_ERR_INVALID on any other rate, before any
+ * allocation or launch: dsk_fbank_frame_offsets, dsk_fbank_filterbank, dsk_fbank, dsk_fbank_batch,
+ * dsk_fbank_batch_vad and dsk_fbank_segments.
+ *   dsk_fbank_num_frames: host only.  1 for n_samples <= flen, else 1 + ceil((n_samples - flen) / step); 0 for
+ *     n_samples <= 0 or a rate outside that range. */
+#define DSK_FBANK_MIN_RATE 50
+#define DSK_FBANK_MAX_RATE 20499
 int64_t dsk_fbank_num_frames(int64_t n_samples, int32_t sample_rate);
 int32_t dsk_fbank(const float* audio, int64_t n_samples, int32_t sample_rate, int32_t log_scale, int32_t subtract_mean,
                   float* feat, void* stream);
