@@ -28,6 +28,7 @@ DSK_F64_MAX_DIM = 4096
 DSK_PLDA_MAX_ROWS = 4194240
 DSK_VBX_MAX_SPEAKERS = 128
 DSK_SPEED_MAX_DEN, DSK_SPEED_TAPS, DSK_SPEED_MAX_FACTORS = 32, 50, 8
+DSK_AAM_MAX_C, DSK_AAM_MAX_SUBCENTRES, DSK_AAM_MAX_TOPK = 65536, 16, 64
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -192,6 +193,11 @@ SIGNATURES = {
     "dsk_batch_hard_triplet_bwd_rows": (c_int32, [c_void_p] * 6 + [c_int32] * 4 + [c_float] + [c_void_p] * 3),
     "dsk_aam_softmax": (c_int32, [c_void_p] * 4 + [c_int32] * 3 + [c_float, c_float] + [c_void_p] * 4),
     "dsk_aam_softmax_bwd": (c_int32, [c_void_p] * 6 + [c_int32] * 3 + [c_float, c_float] + [c_void_p] * 4),
+    "dsk_aam_softmax_sc": (c_int32, [c_void_p] * 4 + [c_int32] * 4 + [c_float, c_float, c_int32, c_float]
+                           + [c_void_p] * 6),
+    "dsk_aam_softmax_sc_bwd": (c_int32, [c_void_p] * 8 + [c_int32] * 4 + [c_float, c_float, c_int32, c_float]
+                               + [c_void_p] * 4),
+    "dsk_aam_subcentre_cos": (c_int32, [c_void_p] * 3 + [c_int32] * 4 + [c_void_p] * 2),
     "dsk_ge2e": (c_int32, [c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 3 + [c_int32, c_int32] + [c_void_p] * 2
                  + [c_int32] + [c_void_p] * 4),
     "dsk_ge2e_bwd": (c_int32, [c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 3 + [c_int32, c_int32]

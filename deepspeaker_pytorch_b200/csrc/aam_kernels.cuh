@@ -1,5 +1,6 @@
 // Additive angular margin softmax (ArcFace / AAM-softmax) over a cosine classifier: the element-wise and row kernels
-// around the tensor-core cosine GEMMs (dsk_aam_softmax / dsk_aam_softmax_bwd in dsk_api.cu).
+// around the tensor-core cosine GEMMs (dsk_aam_softmax_sc / dsk_aam_softmax_sc_bwd in dsk_api.cu, of which
+// dsk_aam_softmax / _bwd are the K = 1, topk = 0 calls).
 //
 // The three GEMMs (cos = E^ W^T, gE^ = dcos W^, gW^ = dcos^T E^) run on conv_umma_kernel as plain GEMMs with fp16
 // operands split into hi/lo halves (x = hi + lo, 22 significant bits) and concatenated along K, so that one fp32
@@ -33,6 +34,7 @@ struct AamMargin {
   float cos_m, sin_m;  // cos m, sin m
   float th, mm;        // cos(pi - m), sin(pi - m) * m: below th the target logit is cos - mm (non-"easy" margin)
   float s;             // scale
+  float cos_t, sin_t;  // cos m', sin m' of the inter-top-k margin
 };
 
 // phi(cos) of the target column
@@ -45,6 +47,78 @@ __device__ __forceinline__ float aam_dphi(float c, const AamMargin& a) {
   if (!(c > a.th)) return 1.f;
   const float sn = sqrtf(fminf(fmaxf(1.f - c * c, 0.f), 1.f));
   return sn > 0.f ? a.cos_m + a.sin_m * c / sn : a.cos_m;
+}
+// psi(cos) = cos(theta - m') of a class in the row's top-k set
+__device__ __forceinline__ float aam_psi(float c, const AamMargin& a) {
+  const float sn = sqrtf(fminf(fmaxf(1.f - c * c, 0.f), 1.f));
+  return c * a.cos_t + sn * a.sin_t;
+}
+// d psi / d cos; at sin = 0 the finite value cos m', as aam_dphi
+__device__ __forceinline__ float aam_dpsi(float c, const AamMargin& a) {
+  const float sn = sqrtf(fminf(fmaxf(1.f - c * c, 0.f), 1.f));
+  return sn > 0.f ? a.cos_t - a.sin_t * c / sn : a.cos_t;
+}
+
+// Key of class c with class cosine v in the top-k order: a larger key ranks first.  Larger cosines first, ties to the
+// lower class, -0 == +0, and NaN after every number (-inf included), as dsk_topk_indices orders.  Keys are distinct and
+// nonzero.
+__device__ __forceinline__ unsigned long long aam_topk_key(float v, int c) {
+  uint32_t u = __float_as_uint(v == 0.f ? 0.f : v);
+  u = isnan(v) ? 0u : ((u & 0x80000000u) ? ~u : (u | 0x80000000u));
+  return (static_cast<unsigned long long>(u) << 32) | (0xffffffffu - static_cast<uint32_t>(c));
+}
+__device__ __forceinline__ unsigned long long block_reduce_max_u64(unsigned long long v, unsigned long long* red) {
+  for (int o = 16; o > 0; o >>= 1) {
+    const unsigned long long t = __shfl_xor_sync(0xffffffffu, v, o);
+    v = t > v ? t : v;
+  }
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  unsigned long long t = red[0];
+  for (int i = 1; i < static_cast<int>(blockDim.x >> 5); ++i) t = red[i] > t ? red[i] : t;
+  __syncthreads();
+  return t;
+}
+
+// fp64 cosine of the fp32 rows e and w (D wide) with F.normalize's 1e-12 floors, summed in a fixed order; the value is
+// that of thread 0 (0 elsewhere).  Block 256; red3 [3][8] is free again on return.
+__device__ double aam_cos64(const float* __restrict__ e, const float* __restrict__ w, int D, double (*red3)[8]) {
+  double ew = 0.0, ee = 0.0, ww = 0.0;
+  for (int d = threadIdx.x; d < D; d += blockDim.x) {
+    const double ed = e[d], wd = w[d];
+    ew = fma(ed, wd, ew);
+    ee = fma(ed, ed, ee);
+    ww = fma(wd, wd, ww);
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    ew += __shfl_xor_sync(0xffffffffu, ew, o);
+    ee += __shfl_xor_sync(0xffffffffu, ee, o);
+    ww += __shfl_xor_sync(0xffffffffu, ww, o);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    red3[0][threadIdx.x >> 5] = ew;
+    red3[1][threadIdx.x >> 5] = ee;
+    red3[2][threadIdx.x >> 5] = ww;
+  }
+  __syncthreads();
+  double r = 0.0;
+  if (threadIdx.x == 0) {
+    for (int k = 1; k < static_cast<int>(blockDim.x >> 5); ++k) {
+      ew += red3[0][k];
+      ee += red3[1][k];
+      ww += red3[2][k];
+    }
+    r = ew / (fmax(sqrt(ee), 1e-12) * fmax(sqrt(ww), 1e-12));
+  }
+  __syncthreads();
+  return r;
+}
+
+// Sub-centre max: v replaces the running best b when b is a number and v is NaN or larger (ties keep the lower k, the
+// first NaN wins and stays)
+template <typename T>
+__device__ __forceinline__ bool aam_sub_better(T v, T b) {
+  return !isnan(b) && (isnan(v) || v > b);
 }
 
 __device__ __forceinline__ void aam_split16(float x, uint16_t& hi, uint16_t& lo) {
@@ -110,17 +184,25 @@ aam_split_kernel(const float* __restrict__ X, const float* __restrict__ nrm, int
   }
 }
 
-// Forward rows: cos_out[i] = G[i][0, C) (the GEMM's padded output) except the target column, which is recomputed in
-// fp64 from E[i] and W[y] (a row near its class centre has cos ~ 1 there, where the GEMM's accumulation error is
-// largest); logits s*cos with s*phi on the target column, lse[i] = logsumexp over all C in a fixed order,
-// row_loss[i] = lse[i] - s*phi (NaN for a label outside [0, C)).  grid N, block 256.
+// Forward rows over C classes of K sub-centres each (columns c K + k of the GEMM's padded output G; K = 1 and topk = 0
+// is the plain AAM-softmax):
+//   cos_out[i][c] = max_k G[i][cK + k] and sub[i][c] (may be NULL) its argmax, by aam_sub_better; on the target column
+//     all K cosines are recomputed in fp64 from E[i] and W[yK + k] (a row near its class centre has cos ~ 1 there, where
+//     the GEMM's accumulation error is largest), the max taken in fp64 and rounded once;
+//   top[i] (topk of them) = the non-target classes first in aam_topk_key's order, by topk block arg-max passes (each the
+//     largest key below the previous one); a class is in the set when its key is at least the last one's;
+//   logits s cos, s phi on the target column, s psi in the top-k set; lse[i] = logsumexp over all C in a fixed order,
+//   row_loss[i] = lse[i] - s*phi (NaN for a label outside [0, C)).  grid N, block 256.
 __global__ void __launch_bounds__(256)
 aam_rows_kernel(const float* __restrict__ G, int ldg, const float* __restrict__ E, const float* __restrict__ W, int D,
-                const int64_t* __restrict__ labels, int C, AamMargin a, float* __restrict__ cos_out,
-                float* __restrict__ lse, float* __restrict__ row_loss) {
+                const int64_t* __restrict__ labels, int C, int K, int topk, AamMargin a, float* __restrict__ cos_out,
+                uint8_t* __restrict__ sub, int32_t* __restrict__ top, float* __restrict__ lse,
+                float* __restrict__ row_loss) {
   __shared__ float red[8];
   __shared__ double red3[3][8];
+  __shared__ unsigned long long redk[8];
   __shared__ float tcos;
+  __shared__ int tsub;
   const int i = blockIdx.x;
   const float* g = G + static_cast<size_t>(i) * ldg;
   float* co = cos_out + static_cast<size_t>(i) * C;
@@ -128,48 +210,66 @@ aam_rows_kernel(const float* __restrict__ G, int ldg, const float* __restrict__ 
   const bool ok = y >= 0 && y < C;
   if (ok) {
     const float* e = E + static_cast<size_t>(i) * D;
-    const float* w = W + static_cast<size_t>(y) * D;
-    double ew = 0.0, ee = 0.0, ww = 0.0;
-    for (int d = threadIdx.x; d < D; d += blockDim.x) {
-      const double ed = e[d], wd = w[d];
-      ew = fma(ed, wd, ew);
-      ee = fma(ed, ed, ee);
-      ww = fma(wd, wd, ww);
-    }
-    for (int o = 16; o > 0; o >>= 1) {
-      ew += __shfl_xor_sync(0xffffffffu, ew, o);
-      ee += __shfl_xor_sync(0xffffffffu, ee, o);
-      ww += __shfl_xor_sync(0xffffffffu, ww, o);
-    }
-    if ((threadIdx.x & 31) == 0) {
-      red3[0][threadIdx.x >> 5] = ew;
-      red3[1][threadIdx.x >> 5] = ee;
-      red3[2][threadIdx.x >> 5] = ww;
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      for (int k = 1; k < static_cast<int>(blockDim.x >> 5); ++k) {
-        ew += red3[0][k];
-        ee += red3[1][k];
-        ww += red3[2][k];
+    double best = 0.0;
+    int bk = 0;
+    for (int k = 0; k < K; ++k) {
+      const double v = aam_cos64(e, W + (static_cast<size_t>(y) * K + k) * D, D, red3);
+      if (k == 0 || aam_sub_better(v, best)) {
+        best = v;
+        bk = k;
       }
-      tcos = static_cast<float>(ew / (fmax(sqrt(ee), 1e-12) * fmax(sqrt(ww), 1e-12)));
+    }
+    if (threadIdx.x == 0) {
+      tcos = static_cast<float>(best);
+      tsub = bk;
     }
     __syncthreads();
   }
-  float m = -INFINITY;
+  float m = -INFINITY;  // the row's largest logit; without a top-k set taken in the same pass
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    float cv;
+    int ak = 0;
     const bool tgt = ok && c == y;
-    const float cv = tgt ? tcos : g[c];
+    if (tgt) {
+      cv = tcos;
+      ak = tsub;
+    } else {
+      const float* gc = g + static_cast<size_t>(c) * K;
+      cv = gc[0];
+      for (int k = 1; k < K; ++k)
+        if (aam_sub_better(gc[k], cv)) {
+          cv = gc[k];
+          ak = k;
+        }
+    }
     co[c] = cv;
-    m = fmaxf(m, a.s * (tgt ? aam_phi(cv, a) : cv));
+    if (sub) sub[static_cast<size_t>(i) * C + c] = static_cast<uint8_t>(ak);
+    if (topk == 0) m = fmaxf(m, a.s * (tgt ? aam_phi(cv, a) : cv));
   }
+  unsigned long long thr = ~0ull;
+  if (topk > 0) {
+    __syncthreads();  // the row's class cosines, written above by every thread
+    for (int j = 0; j < topk; ++j) {
+      unsigned long long b = 0;
+      for (int c = threadIdx.x; c < C; c += blockDim.x) {
+        if (ok && c == y) continue;
+        const unsigned long long kc = aam_topk_key(co[c], c);
+        if (kc < thr && kc > b) b = kc;
+      }
+      thr = block_reduce_max_u64(b, redk);
+      if (threadIdx.x == 0) top[static_cast<size_t>(i) * topk + j] = static_cast<int32_t>(0xffffffffu - static_cast<uint32_t>(thr));
+    }
+  }
+  auto logit = [&](int c) {
+    const float cv = co[c];
+    if (ok && c == y) return aam_phi(cv, a);
+    return topk > 0 && aam_topk_key(cv, c) >= thr ? aam_psi(cv, a) : cv;
+  };
+  if (topk > 0)
+    for (int c = threadIdx.x; c < C; c += blockDim.x) m = fmaxf(m, a.s * logit(c));
   m = block_reduce_max(m, red);
   float sum = 0.f;
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    const bool tgt = ok && c == y;
-    sum += expf(a.s * (tgt ? aam_phi(tcos, a) : g[c]) - m);
-  }
+  for (int c = threadIdx.x; c < C; c += blockDim.x) sum += expf(a.s * logit(c) - m);
   sum = block_reduce_sum(sum, red);
   if (threadIdx.x == 0) {
     const float l = m + logf(sum);
@@ -178,16 +278,19 @@ aam_rows_kernel(const float* __restrict__ G, int ldg, const float* __restrict__ 
   }
 }
 
-// Backward rows: dcos[i][c] = s (softmax - onehot) grad_loss / N, times dphi/dcos on the target column, into the fp32
-// workspace dcos [Np][Cp] and, multiplied by the row's power of two 2^e (rinv[i] = 2^-e), into the K-sliced A-side
-// image dimg [Np][3 Cp] = [lo | hi | hi] of gE^ = dcos W^.  The probabilities are e_c / sum_c e_c with e_c = exp(logit - lse):
-// the division removes the rounding of the saved lse, and the target's softmax - 1 is minus the sum over the other
-// columns, which keeps its relative accuracy in rows that are already well classified.  Rows i >= N and columns
-// c >= C are zero.  grid Np, block 256.
+// Backward rows: the class gradient dc[i][c] = s (softmax - onehot) grad_loss / N, times dphi/dcos on the target column
+// and dpsi/dcos in the top-k set (the classes whose key is at least that of top[i][topk - 1]), goes to column
+// c K + sub[i][c] of the fp32 workspace dcos [Np][Cp] (sub may be NULL when K = 1); the other K - 1 columns of the class
+// are 0.  dcos is also written, multiplied by the row's power of two 2^e (rinv[i] = 2^-e), into the K-sliced A-side
+// image dimg [Np][3 Cp] = [lo | hi | hi] of gE^ = dcos W^.  The probabilities are e_c / sum_c e_c with
+// e_c = exp(logit - lse): the division removes the rounding of the saved lse, and the target's softmax - 1 is minus the
+// sum over the other classes, which keeps its relative accuracy in rows that are already well classified.  Rows i >= N
+// and columns past C K are zero.  grid Np, block 256.
 __global__ void __launch_bounds__(256)
-aam_dcos_kernel(const float* __restrict__ cos, const float* __restrict__ lse, const int64_t* __restrict__ labels, int N,
-                int C, int Cp, AamMargin a, const float* __restrict__ grad_loss, float* __restrict__ dcos,
-                uint16_t* __restrict__ dimg, float* __restrict__ rinv) {
+aam_dcos_kernel(const float* __restrict__ cos, const uint8_t* __restrict__ sub, const int32_t* __restrict__ top,
+                const float* __restrict__ lse, const int64_t* __restrict__ labels, int N, int C, int K, int Cp, int topk,
+                AamMargin a, const float* __restrict__ grad_loss, float* __restrict__ dcos, uint16_t* __restrict__ dimg,
+                float* __restrict__ rinv) {
   __shared__ float red[8];
   const int i = blockIdx.x;
   float* d = dcos + static_cast<size_t>(i) * Cp;
@@ -205,24 +308,36 @@ aam_dcos_kernel(const float* __restrict__ cos, const float* __restrict__ lse, co
   const int64_t y = labels[i];
   const bool ok = y >= 0 && y < C;
   const float l = lse[i];
+  unsigned long long thr = ~0ull;
+  if (topk > 0) {
+    const int t = top[static_cast<size_t>(i) * topk + topk - 1];
+    if (t >= 0 && t < C) thr = aam_topk_key(co[t], t);
+  }
+  auto in_top = [&](int c, float cv) { return topk > 0 && aam_topk_key(cv, c) >= thr; };
   float sig = 0.f, other = 0.f;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     const bool tgt = ok && c == y;
-    const float e = expf(a.s * (tgt ? aam_phi(co[c], a) : co[c]) - l);
+    const float cv = co[c];
+    const float e = expf(a.s * (tgt ? aam_phi(cv, a) : (in_top(c, cv) ? aam_psi(cv, a) : cv)) - l);
     sig += e;
     if (!tgt) other += e;
   }
   sig = block_reduce_sum(sig, red);
   other = block_reduce_sum(other, red);
   const float coef = grad_loss[0] / static_cast<float>(N) * a.s / sig;
+  const uint8_t* sb = sub ? sub + static_cast<size_t>(i) * C : nullptr;
+  const int CK = C * K;
   float mx = 0.f;
-  for (int c = threadIdx.x; c < Cp; c += blockDim.x) {
+  for (int j = threadIdx.x; j < Cp; j += blockDim.x) {
     float v = 0.f;
-    if (c < C) {
-      if (ok && c == y) v = -other * coef * aam_dphi(co[c], a);
-      else v = expf(a.s * co[c] - l) * coef;
+    const int c = K == 1 ? j : j / K;
+    if (j < CK && (K == 1 || j - c * K == sb[c])) {
+      const float cv = co[c];
+      if (ok && c == y) v = -other * coef * aam_dphi(cv, a);
+      else if (in_top(c, cv)) v = expf(a.s * aam_psi(cv, a) - l) * coef * aam_dpsi(cv, a);
+      else v = expf(a.s * cv - l) * coef;
     }
-    d[c] = v;
+    d[j] = v;
     mx = fmaxf(mx, fabsf(v));
   }
   const int e = aam_scale_exp(block_reduce_max(mx, red));
@@ -234,6 +349,25 @@ aam_dcos_kernel(const float* __restrict__ cos, const float* __restrict__ lse, co
     dimg[aam_kslice_off(i, Np, 0, c, Cp)] = lo;
     dimg[aam_kslice_off(i, Np, 1, c, Cp)] = hi;
     dimg[aam_kslice_off(i, Np, 2, c, Cp)] = hi;
+  }
+}
+
+// Each row's fp64 cosines to the K sub-centres of its own class, rounded once: out[i][k] = cos(E[i], W[y_i K + k]),
+// the forward's target recompute (NaN for a label outside [0, C)).  grid N, block 256.
+__global__ void __launch_bounds__(256)
+aam_subcentre_cos_kernel(const float* __restrict__ E, const float* __restrict__ W, const int64_t* __restrict__ labels,
+                         int C, int K, int D, float* __restrict__ out) {
+  __shared__ double red3[3][8];
+  const int i = blockIdx.x;
+  const int64_t y = labels[i];
+  float* o = out + static_cast<size_t>(i) * K;
+  if (!(y >= 0 && y < C)) {
+    if (threadIdx.x < K) o[threadIdx.x] = __int_as_float(0x7fc00000);
+    return;
+  }
+  for (int k = 0; k < K; ++k) {
+    const double v = aam_cos64(E + static_cast<size_t>(i) * D, W + (static_cast<size_t>(y) * K + k) * D, D, red3);
+    if (threadIdx.x == 0) o[k] = static_cast<float>(v);
   }
 }
 

@@ -2784,19 +2784,24 @@ static int aam_plan(dsk_handle h, AamPlan& P, int N, int C, int D, cudaStream_t 
   });
 }
 
-static int aam_check(dsk_handle h, bool ptrs_ok, int N, int C, int D, float margin, float scale, const char* what) {
-  if (!ptrs_ok || N < 1 || C < 2 || C > DSK_AAM_MAX_C || D < 64 || D % 64 || !std::isfinite(margin) || margin < 0.f ||
-      !std::isfinite(scale) || !(scale > 0.f))
-    return fail(DSK_ERR_INVALID, "%s: bad arguments (need non-null pointers, N >= 1, 2 <= C <= %d, D a positive multiple "
-                "of 64, finite margin >= 0 and scale > 0; got N %d, C %d, D %d, margin %g, scale %g)", what,
-                DSK_AAM_MAX_C, N, C, D, margin, scale);
+static int aam_check(dsk_handle h, bool ptrs_ok, int N, int C, int K, int D, float margin, float scale, int topk,
+                     float topk_margin, const char* what) {
+  if (!ptrs_ok || N < 1 || C < 2 || K < 1 || K > DSK_AAM_MAX_SUBCENTRES ||
+      static_cast<int64_t>(C) * K > DSK_AAM_MAX_C || D < 64 || D % 64 || !std::isfinite(margin) || margin < 0.f ||
+      !std::isfinite(scale) || !(scale > 0.f) || topk < 0 || topk > C - 1 || topk > DSK_AAM_MAX_TOPK ||
+      !std::isfinite(topk_margin) || topk_margin < 0.f)
+    return fail(DSK_ERR_INVALID, "%s: bad arguments (need non-null pointers, N >= 1, C >= 2, 1 <= K <= %d, C K <= %d, D "
+                "a positive multiple of 64, finite margin >= 0 and scale > 0, 0 <= topk <= min(C - 1, %d), finite "
+                "topk_margin >= 0; got N %d, C %d, K %d, D %d, margin %g, scale %g, topk %d, topk_margin %g)", what,
+                DSK_AAM_MAX_SUBCENTRES, DSK_AAM_MAX_C, DSK_AAM_MAX_TOPK, N, C, K, D, margin, scale, topk, topk_margin);
   return check_handle(h);
 }
 
-static dsk::AamMargin aam_margin(float margin, float scale) {
+static dsk::AamMargin aam_margin(float margin, float scale, float topk_margin) {
   const double m = margin, pi = 3.14159265358979323846;
   return {static_cast<float>(std::cos(m)), static_cast<float>(std::sin(m)), static_cast<float>(std::cos(pi - m)),
-          static_cast<float>(std::sin(pi - m) * m), scale};
+          static_cast<float>(std::sin(pi - m) * m), scale, static_cast<float>(std::cos(double(topk_margin))),
+          static_cast<float>(std::sin(double(topk_margin)))};
 }
 
 // Rows X[0, n) (D wide) of one operand of a cosine GEMM: their norms nrm (taken by cos_prep when `norm`, else already
@@ -2834,36 +2839,39 @@ static int aam_prep(const AamPlan& P, const float* E, const float* W, bool backw
   return cos_prep(P.D, &e, &w, s);
 }
 
-int32_t dsk_aam_softmax(dsk_handle h, const float* E, const float* W, const int64_t* labels, int32_t N, int32_t C,
-                        int32_t D, float margin, float scale, float* loss, float* cos, float* lse, void* stream) {
-  int rc = aam_check(h, E && W && labels && loss && cos && lse, N, C, D, margin, scale, "dsk_aam_softmax");
+static int aam_forward(dsk_handle h, const float* E, const float* W, const int64_t* labels, int N, int C, int K, int D,
+                       float margin, float scale, int topk, float topk_margin, float* loss, float* cos, float* lse,
+                       uint8_t* sub, int32_t* top, void* stream, const char* what) {
+  int rc = aam_check(h, E && W && labels && loss && cos && lse && (K == 1 || sub) && (topk == 0 || top), N, C, K, D,
+                     margin, scale, topk, topk_margin, what);
   if (rc) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   AamPlan* P = nullptr;
-  if ((rc = aam_plan(h, h->aam, N, C, D, s, &P))) return rc;
+  if ((rc = aam_plan(h, h->aam, N, C * K, D, s, &P))) return rc;
   if ((rc = aam_prep(*P, E, W, false, s))) return rc;
   for (const ConvLaunch& L : P->fwd)
     if ((rc = launch_conv(L, s))) return rc;
-  dsk::aam_rows_kernel<<<N, 256, 0, s>>>(P->gcos, P->Cp, E, W, D, labels, C, aam_margin(margin, scale), cos, lse,
-                                         P->row_loss);
+  dsk::aam_rows_kernel<<<N, 256, 0, s>>>(P->gcos, P->Cp, E, W, D, labels, C, K, topk,
+                                         aam_margin(margin, scale, topk_margin), cos, sub, top, lse, P->row_loss);
   KERNEL_CHECK();
   dsk::mean_rows_kernel<<<1, 1024, 0, s>>>(P->row_loss, N, N, loss);
   KERNEL_CHECK();
   return DSK_OK;
 }
 
-int32_t dsk_aam_softmax_bwd(dsk_handle h, const float* E, const float* W, const int64_t* labels, const float* cos,
-                            const float* lse, int32_t N, int32_t C, int32_t D, float margin, float scale,
-                            const float* grad_loss, float* gE, float* gW, void* stream) {
-  int rc = aam_check(h, E && W && labels && cos && lse && grad_loss && gE && gW, N, C, D, margin, scale,
-                     "dsk_aam_softmax_bwd");
+static int aam_backward(dsk_handle h, const float* E, const float* W, const int64_t* labels, const float* cos,
+                        const float* lse, const uint8_t* sub, const int32_t* top, int N, int C, int K, int D,
+                        float margin, float scale, int topk, float topk_margin, const float* grad_loss, float* gE,
+                        float* gW, void* stream, const char* what) {
+  int rc = aam_check(h, E && W && labels && cos && lse && grad_loss && gE && gW && (K == 1 || sub) && (topk == 0 || top),
+                     N, C, K, D, margin, scale, topk, topk_margin, what);
   if (rc) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   AamPlan* P = nullptr;
-  if ((rc = aam_plan(h, h->aam, N, C, D, s, &P))) return rc;
+  if ((rc = aam_plan(h, h->aam, N, C * K, D, s, &P))) return rc;
   if ((rc = aam_prep(*P, E, W, true, s))) return rc;
-  dsk::aam_dcos_kernel<<<P->Np, 256, 0, s>>>(cos, lse, labels, N, C, P->Cp, aam_margin(margin, scale), grad_loss,
-                                             P->dcos, P->da, P->rinv);
+  dsk::aam_dcos_kernel<<<P->Np, 256, 0, s>>>(cos, sub, top, lse, labels, N, C, K, P->Cp, topk,
+                                             aam_margin(margin, scale, topk_margin), grad_loss, P->dcos, P->da, P->rinv);
   KERNEL_CHECK();
   dsk::aam_dcos_t_kernel<<<P->Cp / 32, 256, 0, s>>>(P->dcos, P->Np, P->Cp, P->dt, P->cinv);
   KERNEL_CHECK();
@@ -2874,8 +2882,48 @@ int32_t dsk_aam_softmax_bwd(dsk_handle h, const float* E, const float* W, const 
   dsk::aam_normalize_bwd_kernel<<<(N + 7) / 8, 256, 0, s>>>(E, P->nrm_e, P->ge, P->sc, static_cast<long>(P->Np) * D,
                                                             P->rinv, N, D, gE);
   KERNEL_CHECK();
-  dsk::aam_normalize_bwd_kernel<<<(C + 7) / 8, 256, 0, s>>>(W, P->nrm_w, P->gw, P->sn, static_cast<long>(P->Cp) * D,
-                                                            P->cinv, C, D, gW);
+  dsk::aam_normalize_bwd_kernel<<<(C * K + 7) / 8, 256, 0, s>>>(W, P->nrm_w, P->gw, P->sn,
+                                                                static_cast<long>(P->Cp) * D, P->cinv, C * K, D, gW);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_aam_softmax_sc(dsk_handle h, const float* E, const float* W, const int64_t* labels, int32_t N, int32_t C,
+                           int32_t K, int32_t D, float margin, float scale, int32_t topk, float topk_margin, float* loss,
+                           float* cos, float* lse, uint8_t* sub, int32_t* top, void* stream) {
+  return aam_forward(h, E, W, labels, N, C, K, D, margin, scale, topk, topk_margin, loss, cos, lse, sub, top, stream,
+                     "dsk_aam_softmax_sc");
+}
+
+int32_t dsk_aam_softmax_sc_bwd(dsk_handle h, const float* E, const float* W, const int64_t* labels, const float* cos,
+                               const float* lse, const uint8_t* sub, const int32_t* top, int32_t N, int32_t C, int32_t K,
+                               int32_t D, float margin, float scale, int32_t topk, float topk_margin,
+                               const float* grad_loss, float* gE, float* gW, void* stream) {
+  return aam_backward(h, E, W, labels, cos, lse, sub, top, N, C, K, D, margin, scale, topk, topk_margin, grad_loss, gE,
+                      gW, stream, "dsk_aam_softmax_sc_bwd");
+}
+
+int32_t dsk_aam_softmax(dsk_handle h, const float* E, const float* W, const int64_t* labels, int32_t N, int32_t C,
+                        int32_t D, float margin, float scale, float* loss, float* cos, float* lse, void* stream) {
+  return aam_forward(h, E, W, labels, N, C, 1, D, margin, scale, 0, 0.f, loss, cos, lse, nullptr, nullptr, stream,
+                     "dsk_aam_softmax");
+}
+
+int32_t dsk_aam_softmax_bwd(dsk_handle h, const float* E, const float* W, const int64_t* labels, const float* cos,
+                            const float* lse, int32_t N, int32_t C, int32_t D, float margin, float scale,
+                            const float* grad_loss, float* gE, float* gW, void* stream) {
+  return aam_backward(h, E, W, labels, cos, lse, nullptr, nullptr, N, C, 1, D, margin, scale, 0, 0.f, grad_loss, gE, gW,
+                      stream, "dsk_aam_softmax_bwd");
+}
+
+int32_t dsk_aam_subcentre_cos(const float* E, const float* W, const int64_t* labels, int32_t N, int32_t C, int32_t K,
+                              int32_t D, float* out, void* stream) {
+  if (!E || !W || !labels || !out || N < 1 || C < 1 || K < 1 || K > DSK_AAM_MAX_SUBCENTRES || D < 1 ||
+      static_cast<int64_t>(C) * K > INT32_MAX)
+    return fail(DSK_ERR_INVALID, "dsk_aam_subcentre_cos: bad arguments (need non-null pointers, N >= 1, C >= 1, "
+                "1 <= K <= %d, D >= 1; got N %d, C %d, K %d, D %d)", DSK_AAM_MAX_SUBCENTRES, N, C, K, D);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  dsk::aam_subcentre_cos_kernel<<<N, 256, 0, s>>>(E, W, labels, C, K, D, out);
   KERNEL_CHECK();
   return DSK_OK;
 }

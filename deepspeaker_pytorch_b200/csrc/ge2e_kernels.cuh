@@ -28,19 +28,6 @@ __device__ __forceinline__ double block_reduce_sum_f64(double v, double* red) {
   return t;
 }
 
-__device__ __forceinline__ unsigned long long block_reduce_max_u64(unsigned long long v, unsigned long long* red) {
-  for (int o = 16; o > 0; o >>= 1) {
-    const unsigned long long x = __shfl_xor_sync(0xffffffffu, v, o);
-    v = x > v ? x : v;
-  }
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  unsigned long long t = red[0];
-  for (int i = 1; i < static_cast<int>(blockDim.x >> 5); ++i) t = red[i] > t ? red[i] : t;
-  __syncthreads();
-  return t;
-}
-
 __device__ __forceinline__ float ge2e_sigmoid(float x) { return 1.f / (1.f + expf(-x)); }
 
 // nr[r] = max(||X[r]||, 1e-12) in fp64 from the fp32 row (class_centroids_kernel's norm: one warp, the same order).

@@ -6,6 +6,7 @@ PyTorch is plumbing here (device memory, streams, autograd graph); all arithmeti
 from __future__ import annotations
 
 import ctypes
+import math
 
 import numpy as np
 import torch
@@ -401,49 +402,115 @@ def _aam_inputs(E, W, labels):
     return E, W, labels
 
 
-def aam_softmax(E, W, labels, margin, scale):
-    """dsk_aam_softmax: (E, W, labels as the op read them, loss (1,), cos (N, C), lse (N,)) on E's device."""
+def aam_subcentre_args(rows, subcentres, topk, topk_margin):
+    """Checks the sub-centre arguments for a (C K, D) weight of ``rows`` rows and returns C: ValueError unless
+    1 <= K <= 16, K divides the rows, 0 <= topk <= min(C - 1, 64) and m' is finite and >= 0.  C >= 2 and
+    C K <= 65536 are the op's own checks."""
+    K = subcentres
+    if isinstance(K, bool) or not isinstance(K, int) or not 1 <= K <= L.DSK_AAM_MAX_SUBCENTRES:
+        raise ValueError(f"subcentres must be an int in [1, {L.DSK_AAM_MAX_SUBCENTRES}], got {K!r}")
+    if rows % K:
+        raise ValueError(f"the weight must have C * subcentres rows; {rows} rows are not a multiple of {K}")
+    C = rows // K
+    if isinstance(topk, bool) or not isinstance(topk, int) or topk < 0 or \
+            (topk > 0 and topk > min(C - 1, L.DSK_AAM_MAX_TOPK)):
+        raise ValueError(f"topk must be an int in [0, min(C - 1, {L.DSK_AAM_MAX_TOPK})] with C = {C}, got {topk!r}")
+    if not math.isfinite(float(topk_margin)) or float(topk_margin) < 0.0:
+        raise ValueError(f"topk_margin must be finite and >= 0, got {topk_margin!r}")
+    return C
+
+
+def aam_softmax_sc(E, W, labels, margin, scale, subcentres=1, topk=0, topk_margin=0.0):
+    """dsk_aam_softmax_sc: (E, W, labels as the op read them, loss (1,), cos (N, C), lse (N,), sub (N, C) uint8 or
+    None when subcentres = 1, top (N, topk) int32 or None when topk = 0) on E's device.  W is (C * subcentres, D)."""
     E, W, labels = _aam_inputs(E, W, labels)
-    (N, D), C = E.shape, W.shape[0]
+    C = aam_subcentre_args(W.shape[0], subcentres, topk, topk_margin)
+    N, D = E.shape
     dev = E.device
     loss = torch.empty(1, device=dev, dtype=torch.float32)
     cos = torch.empty(N, C, device=dev, dtype=torch.float32)
     lse = torch.empty(N, device=dev, dtype=torch.float32)
+    sub = torch.empty(N, C, device=dev, dtype=torch.uint8) if subcentres > 1 else None
+    top = torch.empty(N, topk, device=dev, dtype=torch.int32) if topk > 0 else None
     with torch.cuda.device(dev):
-        L.check(L.load().dsk_aam_softmax(_allpairs_handle(dev), E.data_ptr(), W.data_ptr(), labels.data_ptr(), N, C, D,
-                                         float(margin), float(scale), loss.data_ptr(), cos.data_ptr(), lse.data_ptr(),
-                                         L.cur_stream()), "dsk_aam_softmax")
-    return E, W, labels, loss, cos, lse
+        L.check(L.load().dsk_aam_softmax_sc(_allpairs_handle(dev), E.data_ptr(), W.data_ptr(), labels.data_ptr(), N, C,
+                                            subcentres, D, float(margin), float(scale), topk, float(topk_margin),
+                                            loss.data_ptr(), cos.data_ptr(), lse.data_ptr(), L.ptr(sub), L.ptr(top),
+                                            L.cur_stream()), "dsk_aam_softmax_sc")
+    return E, W, labels, loss, cos, lse, sub, top
+
+
+def aam_softmax_sc_backward(E, W, labels, cos, lse, sub, top, margin, scale, subcentres, topk, topk_margin, grad_loss):
+    """dsk_aam_softmax_sc_bwd: (gE (N, D), gW (C * subcentres, D)) = d loss / d (E, W) scaled by the device scalar
+    ``grad_loss``, from the forward's cos, lse, sub and top."""
+    N, D = E.shape
+    C = aam_subcentre_args(W.shape[0], subcentres, topk, topk_margin)
+    gl = grad_loss.float().reshape(1).contiguous()
+    gE, gW = torch.empty_like(E), torch.empty_like(W)
+    with torch.cuda.device(E.device):
+        L.check(L.load().dsk_aam_softmax_sc_bwd(_allpairs_handle(E.device), E.data_ptr(), W.data_ptr(),
+                                                labels.data_ptr(), cos.data_ptr(), lse.data_ptr(), L.ptr(sub),
+                                                L.ptr(top), N, C, subcentres, D, float(margin), float(scale), topk,
+                                                float(topk_margin), gl.data_ptr(), gE.data_ptr(), gW.data_ptr(),
+                                                L.cur_stream()), "dsk_aam_softmax_sc_bwd")
+    return gE, gW
+
+
+def aam_softmax(E, W, labels, margin, scale):
+    """dsk_aam_softmax: (E, W, labels as the op read them, loss (1,), cos (N, C), lse (N,)) on E's device."""
+    return aam_softmax_sc(E, W, labels, margin, scale)[:6]
 
 
 def aam_softmax_backward(E, W, labels, cos, lse, margin, scale, grad_loss):
     """dsk_aam_softmax_bwd: (gE (N, D), gW (C, D)) = d loss / d (E, W) scaled by the device scalar ``grad_loss``."""
-    (N, D), C = E.shape, W.shape[0]
-    gl = grad_loss.float().reshape(1).contiguous()
-    gE, gW = torch.empty_like(E), torch.empty_like(W)
+    return aam_softmax_sc_backward(E, W, labels, cos, lse, None, None, margin, scale, 1, 0, 0.0, grad_loss)
+
+
+def subcentre_cosines(E, W, labels, subcentres):
+    """dsk_aam_subcentre_cos: (N, K) fp32, each row's cosines to the K sub-centres of its own class (W is (C K, D),
+    row c K + k sub-centre k of class c), in fp64 from the fp32 inputs and rounded once; NaN rows for labels outside
+    [0, C).  These are the target cosines the sub-centre AAM-softmax forward takes its max over.
+
+    Label cleaning and pruning after sub-centre training are torch plumbing on top (E a bank of embeddings, y its
+    labels, W the trained (C K, D) weight)::
+
+        sc = subcentre_cosines(E, W, y, K)                          # (N, K)
+        best = sc.argmax(1)                                          # each utterance's nearest sub-centre
+        counts = torch.zeros(C, K, dtype=torch.long, device=E.device)
+        counts.index_put_((y, best), torch.ones_like(y), accumulate=True)
+        dom = counts.argmax(1)                                       # (C,) each class's dominant sub-centre
+        ang = torch.rad2deg(torch.acos(sc[torch.arange(len(y)), dom[y]].clamp(-1, 1)))
+        keep = ang <= 75.0                                           # drop utterances far from their dominant centre
+        W1 = W.view(C, K, -1)[torch.arange(C), dom]                  # (C, D) rows for a K = 1 fine-tune
+    """
+    K = subcentres
+    C = aam_subcentre_args(W.shape[0] if W.dim() == 2 else 0, K, 0, 0.0)
+    E, W, labels = _aam_inputs(E, W, labels)
+    N, D = E.shape
+    out = torch.empty(N, K, device=E.device, dtype=torch.float32)
     with torch.cuda.device(E.device):
-        L.check(L.load().dsk_aam_softmax_bwd(_allpairs_handle(E.device), E.data_ptr(), W.data_ptr(), labels.data_ptr(),
-                                             cos.data_ptr(), lse.data_ptr(), N, C, D, float(margin), float(scale),
-                                             gl.data_ptr(), gE.data_ptr(), gW.data_ptr(), L.cur_stream()),
-                "dsk_aam_softmax_bwd")
-    return gE, gW
+        L.check(L.load().dsk_aam_subcentre_cos(E.data_ptr(), W.data_ptr(), labels.data_ptr(), N, C, K, D,
+                                               out.data_ptr(), L.cur_stream()), "dsk_aam_subcentre_cos")
+    return out
 
 
 class AAMSoftmaxFn(torch.autograd.Function):
-    """Additive angular margin softmax over a cosine classifier; the loss is a device scalar."""
+    """Additive angular margin softmax over a cosine classifier with K sub-centres per class and the inter-top-k
+    penalty (K = 1, topk = 0: plain AAM-softmax); the loss is a device scalar."""
 
     @staticmethod
-    def forward(ctx, E, W, labels, margin, scale):
-        Ec, Wc, lab, loss, cos, lse = aam_softmax(E, W, labels, margin, scale)
-        ctx.save_for_backward(Ec, Wc, lab, cos, lse)
-        ctx.margin, ctx.scale = margin, scale
+    def forward(ctx, E, W, labels, margin, scale, subcentres, topk, topk_margin):
+        Ec, Wc, lab, loss, cos, lse, sub, top = aam_softmax_sc(E, W, labels, margin, scale, subcentres, topk,
+                                                               topk_margin)
+        ctx.save_for_backward(Ec, Wc, lab, cos, lse, sub, top)
+        ctx.args = margin, scale, subcentres, topk, topk_margin
         return loss.reshape(())
 
     @staticmethod
     def backward(ctx, gl):
-        E, W, lab, cos, lse = ctx.saved_tensors
-        gE, gW = aam_softmax_backward(E, W, lab, cos, lse, ctx.margin, ctx.scale, gl)
-        return (gE if ctx.needs_input_grad[0] else None), (gW if ctx.needs_input_grad[1] else None), None, None, None
+        E, W, lab, cos, lse, sub, top = ctx.saved_tensors
+        gE, gW = aam_softmax_sc_backward(E, W, lab, cos, lse, sub, top, *ctx.args, gl)
+        return ((gE if ctx.needs_input_grad[0] else None), (gW if ctx.needs_input_grad[1] else None)) + (None,) * 6
 
 
 # ---------------------------------------------------------------------------------------------------

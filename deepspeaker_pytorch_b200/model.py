@@ -250,17 +250,27 @@ class AAMSoftmaxLoss:
     (``cos - sin(pi - m) m`` past pi - m), logits times ``scale``, cross-entropy averaged over the batch.  Pass
     ``model.model.classifier.weight``: parameters, ``state_dict`` keys and optimizer buckets stay as they are, and the
     classifier's bias is not used.  ``margin = 0`` is the normalised softmax (NormFace); a margin warm-up passes a
-    different ``margin`` per step."""
+    different ``margin`` per step.
 
-    def __init__(self, weight, margin, scale):
+    Sub-centres and the inter-top-k penalty (Deng et al., "Sub-center ArcFace", ECCV 2020; Zhao et al., ICASSP 2022;
+    no reference implementation, parity unpinned): with ``subcentres`` K > 1 the weight is (C K, E), row c K + k being
+    sub-centre k of class c (as ``reshape(C, K, E)``), and a class's cosine is the largest of its K; with ``topk`` > 0
+    the ``topk`` hardest non-target classes of each row get the logit s cos(theta - ``topk_margin``).  The defaults
+    (K = 1, topk = 0) are the plain loss above, bit for bit.  The weight must have C K rows, 1 <= K <= 16,
+    0 <= topk <= min(C - 1, 64), and ``topk_margin`` must be finite and >= 0; anything else raises ValueError."""
+
+    def __init__(self, weight, margin, scale, *, subcentres=1, topk=0, topk_margin=0.0):
+        _engine.aam_subcentre_args(weight.shape[0] if weight.dim() == 2 else 0, subcentres, topk, topk_margin)
         self.weight = weight
         self.margin = margin
         self.scale = scale
+        self.subcentres, self.topk, self.topk_margin = subcentres, topk, topk_margin
 
     def forward(self, embeddings, labels):
         """embeddings (N, E) CUDA, labels (N,) int in [0, C) -> 0-dim device scalar; back-propagates into the
         embeddings and the weight."""
-        return _engine.AAMSoftmaxFn.apply(embeddings, self.weight, labels, float(self.margin), float(self.scale))
+        return _engine.AAMSoftmaxFn.apply(embeddings, self.weight, labels, float(self.margin), float(self.scale),
+                                          self.subcentres, self.topk, float(self.topk_margin))
 
     __call__ = forward
 

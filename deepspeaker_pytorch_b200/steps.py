@@ -171,18 +171,29 @@ def _global_batch_hard_step(model, optimizer, data, labels, margin, bucket):
     return {"loss": loss.detach(), "valid": V}
 
 
-def aam_softmax_step(model, optimizer, data, labels, *, margin, scale, bucket=None):
+def aam_softmax_step(model, optimizer, data, labels, *, margin, scale, bucket=None, weight=None, subcentres=1, topk=0,
+                     topk_margin=0.0):
     """One classification step with the additive angular margin softmax (``AAMSoftmaxLoss`` on
     ``model.model.classifier.weight``): ONE train-mode forward of all N utterances, the loss, backward, optimizer step.
     Returns ``{"loss": device scalar}``.  Every row of the loss depends only on its own embedding and the class weights,
     so under data parallelism (``bucket`` or a ``FusedAdagrad`` optimizer, the same n on every rank) the plain mean
     all-reduce of the gradients is the gradient of the global mean loss; the loss itself needs no collective.  Runs
-    unchanged on a model with ``sync_batchnorm()``."""
+    unchanged on a model with ``sync_batchnorm()``.
+
+    Sub-centres and the inter-top-k penalty (``AAMSoftmaxLoss``'s ``subcentres``, ``topk``, ``topk_margin``) need a
+    (C * subcentres, E) weight: pass it as ``weight``, a parameter the optimizer (or ``bucket``) holds beside the
+    model's.  The model's ``state_dict`` keys stay as they are, and with a separate ``weight`` the step leaves
+    ``classifier.weight`` and ``classifier.bias`` untouched.  A row of the sub-centre loss still depends only on its own
+    embedding, its label and the weight, so the same single mean all-reduce is right under data parallelism.
+    ``weight=None`` is ``model.model.classifier.weight``."""
     if not model.training:
         raise RuntimeError("aam_softmax_step needs model.train()")
+    if weight is None:
+        weight = model.model.classifier.weight
+    crit = AAMSoftmaxLoss(weight, margin, scale, subcentres=subcentres, topk=topk, topk_margin=topk_margin)
     labels = _labels_to(labels, data.device)
     emb = model(data)
-    loss = AAMSoftmaxLoss(model.model.classifier.weight, margin, scale).forward(emb, labels)
+    loss = crit.forward(emb, labels)
     optimizer.zero_grad()
     loss.backward()
     _reduce_and_step(optimizer, bucket, None)

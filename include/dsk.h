@@ -377,6 +377,43 @@ int32_t dsk_aam_softmax_bwd(dsk_handle h, const float* E, const float* W, const 
                             const float* lse, int32_t N, int32_t C, int32_t D, float margin, float scale,
                             const float* grad_loss, float* gE, float* gW, void* stream);
 
+/* Sub-centre AAM-softmax with the inter-top-k penalty (Deng et al., "Sub-center ArcFace", ECCV 2020; Zhao et al.,
+ * ICASSP 2022; no reference implementation exists and parity with any published one is unpinned).  dsk_aam_softmax /
+ * _bwd are its K = 1, topk = 0 calls and give the same bits.  For embeddings E (N,D), weight W (C K, D) whose row
+ * c K + k is sub-centre k of class c (class-major, as reshape(C, K, D)), labels y in [0, C), margin m, scale s, topk
+ * and topk_margin m':
+ *   e^, w^ as above;  g_{i,cK+k} = e^_i . w^_{cK+k};
+ *   class cosine cos (N,C): cos_ic = max_k g_{i,cK+k}, sub (N,C) uint8 its argmax: ties to the lowest k; a NaN
+ *     sub-centre cosine makes cos_ic NaN and sub that k (the lowest such).  On the target column all K cosines are
+ *     recomputed in fp64 from the fp32 inputs, the max and argmax taken in fp64 and the result rounded once;
+ *   top (N,topk) int32: T_i, the topk non-target classes with the largest cos_ic in rank order: ties to the lower class,
+ *     -0 == +0, NaN after every number (dsk_topk_indices's order);
+ *   logit_ic = s * (phi(cos_ic) on the target column, psi(cos_ic) for c in T_i, cos_ic elsewhere), with
+ *     psi(c) = c cos m' + sqrt(clamp(1 - c^2, 0, 1)) sin m' = cos(theta - m');
+ *   lse and loss as above (a label outside [0, C) yields NaN).
+ * Backward: dcos = s (softmax - onehot) grad_loss / N per class, times d phi / d cos on the target and
+ * d psi / d cos = cos m' - sin m' cos / sin on T_i (cos m' at sin = 0); class c's value goes to column c K + sub_ic
+ * only, the other K - 1 columns get exactly 0, and the GEMMs and Jacobians of dsk_aam_softmax_bwd run over the C K
+ * columns (gW (C K, D)).  The backward reads sub and top; it takes T_i as the classes ranked no later than
+ * top[i][topk - 1] in cos.  sub may be NULL when K = 1, top when topk = 0.  Rows depend only on their own embedding,
+ * label and W, as above.  The plan is that of dsk_aam_softmax for (N, C K, D).
+ * 1 <= N, 2 <= C, 1 <= K <= DSK_AAM_MAX_SUBCENTRES, C K <= DSK_AAM_MAX_C, 0 <= topk <= min(C - 1, DSK_AAM_MAX_TOPK),
+ * finite m' >= 0, D % 64 == 0, else DSK_ERR_INVALID. */
+#define DSK_AAM_MAX_SUBCENTRES 16
+#define DSK_AAM_MAX_TOPK 64
+int32_t dsk_aam_softmax_sc(dsk_handle h, const float* E, const float* W, const int64_t* labels, int32_t N, int32_t C,
+                           int32_t K, int32_t D, float margin, float scale, int32_t topk, float topk_margin, float* loss,
+                           float* cos, float* lse, uint8_t* sub, int32_t* top, void* stream);
+int32_t dsk_aam_softmax_sc_bwd(dsk_handle h, const float* E, const float* W, const int64_t* labels, const float* cos,
+                               const float* lse, const uint8_t* sub, const int32_t* top, int32_t N, int32_t C, int32_t K,
+                               int32_t D, float margin, float scale, int32_t topk, float topk_margin,
+                               const float* grad_loss, float* gE, float* gW, void* stream);
+/* out (N,K) fp32: each row's cosines to its own class's K sub-centres, cos(E[i], W[y_i K + k]) in fp64 from the fp32
+ * inputs, rounded once (the forward's target recompute; a NaN row for a label outside [0, C)).  One CTA per row.
+ * 1 <= N, 1 <= C, 1 <= K <= DSK_AAM_MAX_SUBCENTRES, 1 <= D, else DSK_ERR_INVALID. */
+int32_t dsk_aam_subcentre_cos(const float* E, const float* W, const int64_t* labels, int32_t N, int32_t C, int32_t K,
+                              int32_t D, float* out, void* stream);
+
 /* Generalised end-to-end (GE2E) loss against in-batch speaker centroids (Wan et al., ICASSP 2018; no reference
  * implementation exists).  For embeddings E (N,D) and a batch of P speakers given as a CSR: speaker k's rows are
  * S_k = order[offsets[k] .. offsets[k+1]) (n_k of them, ascending row index within a speaker), col[i] = the speaker of
