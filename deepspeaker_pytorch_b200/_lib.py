@@ -198,6 +198,13 @@ SIGNATURES = {
     "dsk_aam_softmax_sc_bwd": (c_int32, [c_void_p] * 8 + [c_int32] * 4 + [c_float, c_float, c_int32, c_float]
                                + [c_void_p] * 4),
     "dsk_aam_subcentre_cos": (c_int32, [c_void_p] * 3 + [c_int32] * 4 + [c_void_p] * 2),
+    "dsk_aam_shard_cos": (c_int32, [c_void_p] * 4 + [c_int32] * 7 + [c_void_p] * 4),
+    "dsk_aam_shard_merge": (c_int32, [c_void_p] * 3 + [c_int32] * 6 + [c_float] * 3 + [c_void_p] * 4),
+    "dsk_aam_shard_partials": (c_int32, [c_void_p] * 4 + [c_int32] * 7 + [c_float] * 3 + [c_void_p] * 3),
+    "dsk_aam_shard_finish": (c_int32, [c_void_p] * 3 + [c_int32] * 4 + [c_void_p] * 5),
+    "dsk_aam_shard_bwd": (c_int32, [c_void_p] * 9 + [c_int32] * 6 + [c_float, c_float, c_int32, c_float]
+                          + [c_void_p] * 4),
+    "dsk_aam_shard_bwd_rows": (c_int32, [c_void_p] * 2 + [c_int32] * 3 + [c_void_p] * 2),
     "dsk_ge2e": (c_int32, [c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 3 + [c_int32, c_int32] + [c_void_p] * 2
                  + [c_int32] + [c_void_p] * 4),
     "dsk_ge2e_bwd": (c_int32, [c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 3 + [c_int32, c_int32]

@@ -433,4 +433,324 @@ aam_normalize_bwd_kernel(const float* __restrict__ X, const float* __restrict__ 
   for (int d = lane; d < D; d += 32) y[d] = (grad(d) - (x[d] / n) * dot) / n;
 }
 
+// ---- the class-sharded op (dsk_aam_shard_*): rank r holds the classes [c0, c0 + Cr) of C, all N gathered rows --------
+// Local class c is global class c0 + c; c0 is a multiple of kAamShardBlock, so the 128-class blocks of a shard are
+// blocks of the global class axis and the block partials below do not depend on the split.
+constexpr int kAamShardBlock = 128;
+
+// The logit of local class c with class cosine cv: s phi on the row's target (local index yl, -1 when the target is
+// on another rank or the label is invalid), s psi when the global key is at least the top-k threshold thr, else s cos.
+__device__ __forceinline__ float aam_shard_logit(float cv, int c, int yl, int c0, int topk, unsigned long long thr,
+                                                 const AamMargin& a) {
+  if (c == yl) return a.s * aam_phi(cv, a);
+  return a.s * (topk > 0 && aam_topk_key(cv, c0 + c) >= thr ? aam_psi(cv, a) : cv);
+}
+
+__device__ __forceinline__ int aam_shard_target(int64_t y, int c0, int Cr) {
+  return y >= c0 && y < static_cast<int64_t>(c0) + Cr ? static_cast<int>(y - c0) : -1;
+}
+
+// Stage 1: class cosines and sub-centre argmax of the shard (aam_rows_kernel's first pass over the shard's columns of
+// the padded GEMM output G, the target recomputed in fp64 when it is local), then the row's local top-k candidate keys
+// keys[i] (topk of them, global class ids, target excluded, ranked by topk block arg-max passes; 0 once the shard has
+// no candidate left).  grid N, block 256.
+__global__ void __launch_bounds__(256)
+aam_shard_cos_kernel(const float* __restrict__ G, int ldg, const float* __restrict__ E, const float* __restrict__ W,
+                     int D, const int64_t* __restrict__ labels, int c0, int Cr, int K, int topk,
+                     float* __restrict__ cos_out, uint8_t* __restrict__ sub, unsigned long long* __restrict__ keys) {
+  __shared__ double red3[3][8];
+  __shared__ unsigned long long redk[8];
+  __shared__ float tcos;
+  __shared__ int tsub;
+  const int i = blockIdx.x;
+  const float* g = G + static_cast<size_t>(i) * ldg;
+  float* co = cos_out + static_cast<size_t>(i) * Cr;
+  const int yl = aam_shard_target(labels[i], c0, Cr);
+  if (yl >= 0) {
+    const float* e = E + static_cast<size_t>(i) * D;
+    double best = 0.0;
+    int bk = 0;
+    for (int k = 0; k < K; ++k) {
+      const double v = aam_cos64(e, W + (static_cast<size_t>(yl) * K + k) * D, D, red3);
+      if (k == 0 || aam_sub_better(v, best)) {
+        best = v;
+        bk = k;
+      }
+    }
+    if (threadIdx.x == 0) {
+      tcos = static_cast<float>(best);
+      tsub = bk;
+    }
+    __syncthreads();
+  }
+  for (int c = threadIdx.x; c < Cr; c += blockDim.x) {
+    float cv;
+    int ak = 0;
+    if (c == yl) {
+      cv = tcos;
+      ak = tsub;
+    } else {
+      const float* gc = g + static_cast<size_t>(c) * K;
+      cv = gc[0];
+      for (int k = 1; k < K; ++k)
+        if (aam_sub_better(gc[k], cv)) {
+          cv = gc[k];
+          ak = k;
+        }
+    }
+    co[c] = cv;
+    if (sub) sub[static_cast<size_t>(i) * Cr + c] = static_cast<uint8_t>(ak);
+  }
+  if (topk == 0) return;
+  __syncthreads();
+  unsigned long long thr = ~0ull;
+  for (int j = 0; j < topk; ++j) {
+    unsigned long long b = 0;
+    for (int c = threadIdx.x; c < Cr; c += blockDim.x) {
+      if (c == yl) continue;
+      const unsigned long long kc = aam_topk_key(co[c], c0 + c);
+      if (kc < thr && kc > b) b = kc;
+    }
+    thr = block_reduce_max_u64(b, redk);
+    if (threadIdx.x == 0) keys[static_cast<size_t>(i) * topk + j] = thr;
+  }
+}
+
+// Stage 2: the global top-k of row i from every rank's candidates keys_all [R][N][topk] (the topk largest keys, by topk
+// block arg-max passes: the keys are distinct but for the 0 sentinels, and topk <= C - 1 real ones exist), top[i] their
+// global class ids and thr[i] the last key; then mloc[i], the largest logit of the shard's classes.  grid N, block 256.
+__global__ void __launch_bounds__(256)
+aam_shard_merge_kernel(const float* __restrict__ cos, const int64_t* __restrict__ labels,
+                       const unsigned long long* __restrict__ keys_all, int R, int N, int c0, int Cr, int topk,
+                       AamMargin a, int32_t* __restrict__ top, unsigned long long* __restrict__ thr_out,
+                       float* __restrict__ mloc) {
+  __shared__ float red[8];
+  __shared__ unsigned long long redk[8];
+  const int i = blockIdx.x;
+  const int yl = aam_shard_target(labels[i], c0, Cr);
+  unsigned long long thr = ~0ull;
+  if (topk > 0) {
+    for (int j = 0; j < topk; ++j) {
+      unsigned long long b = 0;
+      for (int t = threadIdx.x; t < R * topk; t += blockDim.x) {
+        const int r = t / topk;
+        const unsigned long long kc = keys_all[(static_cast<size_t>(r) * N + i) * topk + (t - r * topk)];
+        if (kc < thr && kc > b) b = kc;
+      }
+      thr = block_reduce_max_u64(b, redk);
+      if (threadIdx.x == 0) top[static_cast<size_t>(i) * topk + j] = static_cast<int32_t>(0xffffffffu - static_cast<uint32_t>(thr));
+    }
+    if (threadIdx.x == 0) thr_out[i] = thr;
+  }
+  const float* co = cos + static_cast<size_t>(i) * Cr;
+  float m = -INFINITY;
+  for (int c = threadIdx.x; c < Cr; c += blockDim.x) m = fmaxf(m, aam_shard_logit(co[c], c, yl, c0, topk, thr, a));
+  m = block_reduce_max(m, red);
+  if (threadIdx.x == 0) mloc[i] = m;
+}
+
+// Stage 3: m[i] = the largest of the ranks' maxima maxima [R][N] (exact in any order), and the record of row i over
+// the shard: rec[i] = [S_b, S_other_b] for b < nb, then the target logit and the flags (as float bits), 2 nb + 2 floats.
+// S_b is the sum of exp(logit - m) over the classes of the shard's block b (one thread per class, a fixed tree: the sum
+// depends on the block's classes only), S_other_b the same without the target; blocks past the shard are +0.  A NaN
+// term sets flag 1 and is left out of the sums; flag 2: the target is on this shard and rec[2 nb] = s phi(cos_target);
+// bits 8 and up: the shard's block count ceil(Cr / 128), which places its blocks on the global block axis in stage 4.
+// grid N, block kAamShardBlock.
+__global__ void __launch_bounds__(kAamShardBlock)
+aam_shard_partials_kernel(const float* __restrict__ cos, const int64_t* __restrict__ labels,
+                          const unsigned long long* __restrict__ thr_in, const float* __restrict__ maxima, int R, int N,
+                          int c0, int Cr, int topk, int nb, AamMargin a, float* __restrict__ m_out,
+                          float* __restrict__ rec) {
+  __shared__ float red[2][kAamShardBlock / 32];
+  const int i = blockIdx.x, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int yl = aam_shard_target(labels[i], c0, Cr);
+  float m = maxima[i];
+  for (int r = 1; r < R; ++r) m = fmaxf(m, maxima[static_cast<size_t>(r) * N + i]);
+  const unsigned long long thr = topk > 0 ? thr_in[i] : ~0ull;
+  const float* co = cos + static_cast<size_t>(i) * Cr;
+  float* out = rec + static_cast<size_t>(i) * (2 * nb + 2);
+  int nan = 0;
+  for (int blk = 0; blk < nb; ++blk) {
+    const int c = blk * kAamShardBlock + threadIdx.x;
+    float s = 0.f, so = 0.f;
+    if (c < Cr) {
+      const float e = expf(aam_shard_logit(co[c], c, yl, c0, topk, thr, a) - m);
+      if (isnan(e)) {
+        nan = 1;
+      } else {
+        s = e;
+        so = c == yl ? 0.f : e;
+      }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      s += __shfl_xor_sync(0xffffffffu, s, o);
+      so += __shfl_xor_sync(0xffffffffu, so, o);
+    }
+    if (lane == 0) {
+      red[0][w] = s;
+      red[1][w] = so;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int k = 1; k < kAamShardBlock / 32; ++k) {
+        s += red[0][k];
+        so += red[1][k];
+      }
+      out[2 * blk] = s;
+      out[2 * blk + 1] = so;
+    }
+    __syncthreads();
+  }
+  nan = __syncthreads_or(nan);
+  if (threadIdx.x == 0) {
+    out[2 * nb] = yl >= 0 ? a.s * aam_phi(co[yl], a) : 0.f;
+    const int nbr = (Cr + kAamShardBlock - 1) / kAamShardBlock;
+    out[2 * nb + 1] = __int_as_float((nan ? 1 : 0) | (yl >= 0 ? 2 : 0) | (nbr << 8));
+    m_out[i] = m;
+  }
+}
+
+// Stage 4, on every rank alike: the records of all ranks rec_all [R][N][2 nb + 2] summed in fp64 in an order fixed by
+// the global block index g alone (rank r's blocks are g = its predecessors' block counts + b), so the sums do not depend
+// on R or the split: lane g mod 32 adds its blocks in ascending g, then a fixed butterfly over the 32 lanes.  lse[i] =
+// m + log S rounded once, row_loss[i] = lse - the target logit (NaN for a label outside [0, C)), den[i] = (S, S_other)
+// in fp32; a NaN flag makes all four NaN.  One warp per row, lane-contiguous loads; grid ceil(N / 8), block 256.
+__global__ void __launch_bounds__(256)
+aam_shard_finish_kernel(const float* __restrict__ rec_all, const float* __restrict__ m, const int64_t* __restrict__ labels,
+                        int R, int N, int C, int nb, float* __restrict__ lse, float* __restrict__ row_loss,
+                        float* __restrict__ den) {
+  const int i = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (i >= N) return;
+  const size_t w = 2 * static_cast<size_t>(nb) + 2;
+  auto rec = [&](int r) { return rec_all + (static_cast<size_t>(r) * N + i) * w; };
+  auto flags_of = [&](int r) { return __float_as_int(rec(r)[2 * nb + 1]); };
+  int fl = 0, total = 0;
+  float t = 0.f;
+  for (int r = lane; r < R; r += 32) {
+    const int f = flags_of(r);
+    fl |= f & 3;
+    total += f >> 8;
+    if (f & 2) t = rec(r)[2 * nb];
+  }
+  const unsigned own = __ballot_sync(0xffffffffu, fl & 2);
+  t = own ? __shfl_sync(0xffffffffu, t, __ffs(own) - 1) : 0.f;
+  const int flags = __reduce_or_sync(0xffffffffu, fl);
+  total = __reduce_add_sync(0xffffffffu, total);
+  double S = 0.0, So = 0.0;
+  int r = 0, off = 0, cnt = flags_of(0) >> 8;
+  for (int g = lane; g < total; g += 32) {
+    while (g >= off + cnt) {
+      off += cnt;
+      cnt = flags_of(++r) >> 8;
+    }
+    const float* p = rec(r) + 2 * (g - off);
+    S += p[0];
+    So += p[1];
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    S += __shfl_xor_sync(0xffffffffu, S, o);
+    So += __shfl_xor_sync(0xffffffffu, So, o);
+  }
+  if (lane) return;
+  const float qnan = __int_as_float(0x7fc00000);
+  const int64_t y = labels[i];
+  const bool nan = flags & 1;
+  const float l = nan ? qnan : static_cast<float>(static_cast<double>(m[i]) + log(S));
+  lse[i] = l;
+  row_loss[i] = y >= 0 && y < C && (flags & 2) ? l - t : qnan;
+  den[2 * i] = nan ? qnan : static_cast<float>(S);
+  den[2 * i + 1] = nan ? qnan : static_cast<float>(So);
+}
+
+// Backward dcos over the shard's columns for all N rows: aam_dcos_kernel's values with the probabilities
+// exp(logit - m) / S and the target's softmax - 1 = -S_other / S from the forward's den = (S, S_other); the row's
+// power-of-two scale is that of the shard's columns.  grid Np, block 256.
+__global__ void __launch_bounds__(256)
+aam_shard_dcos_kernel(const float* __restrict__ cos, const uint8_t* __restrict__ sub,
+                      const unsigned long long* __restrict__ thr_in, const float* __restrict__ m_in,
+                      const float* __restrict__ den, const int64_t* __restrict__ labels, int N, int c0, int Cr, int K,
+                      int Cp, int topk, AamMargin a, const float* __restrict__ grad_loss, float* __restrict__ dcos,
+                      uint16_t* __restrict__ dimg, float* __restrict__ rinv) {
+  __shared__ float red[8];
+  const int i = blockIdx.x;
+  float* d = dcos + static_cast<size_t>(i) * Cp;
+  const int Np = gridDim.x;
+  if (i >= N) {
+    for (int c = threadIdx.x; c < Cp; c += blockDim.x) {
+      d[c] = 0.f;
+      dimg[aam_kslice_off(i, Np, 0, c, Cp)] = dimg[aam_kslice_off(i, Np, 1, c, Cp)] =
+          dimg[aam_kslice_off(i, Np, 2, c, Cp)] = 0;
+    }
+    if (threadIdx.x == 0) rinv[i] = 1.f;
+    return;
+  }
+  const float* co = cos + static_cast<size_t>(i) * Cr;
+  const int yl = aam_shard_target(labels[i], c0, Cr);
+  const unsigned long long thr = topk > 0 ? thr_in[i] : ~0ull;
+  const float m = m_in[i], S = den[2 * i], So = den[2 * i + 1];
+  const float coef = grad_loss[0] / static_cast<float>(N) * a.s / S;
+  const uint8_t* sb = sub ? sub + static_cast<size_t>(i) * Cr : nullptr;
+  const int CK = Cr * K;
+  float mx = 0.f;
+  for (int j = threadIdx.x; j < Cp; j += blockDim.x) {
+    float v = 0.f;
+    const int c = K == 1 ? j : j / K;
+    if (j < CK && (K == 1 || j - c * K == sb[c])) {
+      const float cv = co[c];
+      if (c == yl) v = -So * coef * aam_dphi(cv, a);
+      else if (topk > 0 && aam_topk_key(cv, c0 + c) >= thr) v = expf(a.s * aam_psi(cv, a) - m) * coef * aam_dpsi(cv, a);
+      else v = expf(a.s * cv - m) * coef;
+    }
+    d[j] = v;
+    mx = fmaxf(mx, fabsf(v));
+  }
+  const int e = aam_scale_exp(block_reduce_max(mx, red));
+  if (threadIdx.x == 0) rinv[i] = aam_pow2(-e);
+  const float sc = aam_pow2(e);
+  for (int c = threadIdx.x; c < Cp; c += blockDim.x) {
+    uint16_t hi, lo;
+    aam_split16(d[c] * sc, hi, lo);
+    dimg[aam_kslice_off(i, Np, 0, c, Cp)] = lo;
+    dimg[aam_kslice_off(i, Np, 1, c, Cp)] = hi;
+    dimg[aam_kslice_off(i, Np, 2, c, Cp)] = hi;
+  }
+}
+
+// The shard's partial gradient w.r.t. the normalised rows: part[i][d] = (the K slices of G summed in slice order)
+// times rinv[i], un-scaled by its power of two.  grid ceil(N D / 256), block 256.
+__global__ void __launch_bounds__(256)
+aam_shard_gpart_kernel(const float* __restrict__ G, int slices, size_t slice_elems, const float* __restrict__ rinv,
+                       int N, int D, float* __restrict__ part) {
+  const size_t t = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= static_cast<size_t>(N) * D) return;
+  float v = G[t];
+  for (int s = 1; s < slices; ++s) v += G[s * slice_elems + t];
+  part[t] = v * rinv[t / D];
+}
+
+// gE of this rank's n rows X: g = the R ranks' partials parts [R][n][D] added in rank order, then the F.normalize
+// Jacobian (g - x^ (x^ . g)) / nrm with nrm taken as aam_norm_kernel takes it.  One warp per row; grid ceil(n / 8),
+// block 256.
+__global__ void __launch_bounds__(256)
+aam_shard_rows_bwd_kernel(const float* __restrict__ X, const float* __restrict__ parts, int R, int n, int D,
+                          float* __restrict__ out) {
+  const int r = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (r >= n) return;
+  const float* x = X + static_cast<size_t>(r) * D;
+  float ss = 0.f;
+  for (int d = lane; d < D; d += 32) ss = fmaf(x[d], x[d], ss);
+  for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+  const float nr = fmaxf(sqrtf(ss), 1e-12f);
+  auto grad = [&](int d) {
+    float v = parts[static_cast<size_t>(r) * D + d];
+    for (int q = 1; q < R; ++q) v += parts[(static_cast<size_t>(q) * n + r) * D + d];
+    return v;
+  };
+  float dot = 0.f;
+  for (int d = lane; d < D; d += 32) dot = fmaf(x[d] / nr, grad(d), dot);
+  for (int o = 16; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
+  float* y = out + static_cast<size_t>(r) * D;
+  for (int d = lane; d < D; d += 32) y[d] = (grad(d) - (x[d] / nr) * dot) / nr;
+}
+
 }  // namespace dsk

@@ -2928,6 +2928,138 @@ int32_t dsk_aam_subcentre_cos(const float* E, const float* W, const int64_t* lab
   return DSK_OK;
 }
 
+// ---- the class-sharded AAM-softmax --------------------------------------------------------------------------------
+// The shard [c0, c1) of C classes: 0 <= c0 < c1 <= C, c0 a multiple of 128 and c1 one too unless it is C, (c1 - c0) K
+// within the per-call cap; the other arguments as aam_check.  R ranks, nb record blocks (stages 3 and 4).
+static int aam_shard_check(bool ptrs_ok, int R, int N, int C, int c0, int c1, int K, int D, float margin, float scale,
+                           int topk, float topk_margin, const char* what) {
+  const int B = dsk::kAamShardBlock;
+  if (!ptrs_ok || R < 1 || N < 1 || C < 2 || K < 1 || K > DSK_AAM_MAX_SUBCENTRES || c0 < 0 || c0 % B || c1 <= c0 ||
+      c1 > C || (c1 % B && c1 != C) || static_cast<int64_t>(c1 - c0) * K > DSK_AAM_MAX_C || D < 64 || D % 64 ||
+      !std::isfinite(margin) || margin < 0.f || !std::isfinite(scale) || !(scale > 0.f) || topk < 0 || topk > C - 1 ||
+      topk > DSK_AAM_MAX_TOPK || !std::isfinite(topk_margin) || topk_margin < 0.f)
+    return fail(DSK_ERR_INVALID, "%s: bad arguments (need non-null pointers, R >= 1, N >= 1, C >= 2, 1 <= K <= %d, a "
+                "class range 0 <= c0 < c1 <= C with c0 and c1 (unless c1 = C) multiples of %d and (c1 - c0) K <= %d, D a "
+                "positive multiple of 64, finite margin >= 0 and scale > 0, 0 <= topk <= min(C - 1, %d), finite "
+                "topk_margin >= 0; got R %d, N %d, C %d, c0 %d, c1 %d, K %d, D %d, margin %g, scale %g, topk %d, "
+                "topk_margin %g)", what, DSK_AAM_MAX_SUBCENTRES, B, DSK_AAM_MAX_C, DSK_AAM_MAX_TOPK, R, N, C, c0, c1, K,
+                D, margin, scale, topk, topk_margin);
+  return DSK_OK;
+}
+
+int32_t dsk_aam_shard_cos(dsk_handle h, const float* E, const float* W, const int64_t* labels, int32_t N, int32_t C,
+                          int32_t c0, int32_t c1, int32_t K, int32_t D, int32_t topk, float* cos, uint8_t* sub,
+                          uint64_t* keys, void* stream) {
+  int rc = aam_shard_check(E && W && labels && cos && (K == 1 || sub) && (topk == 0 || keys), 1, N, C, c0, c1, K, D,
+                           0.f, 1.f, topk, 0.f, "dsk_aam_shard_cos");
+  if (rc || (rc = check_handle(h))) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int Cr = c1 - c0;
+  AamPlan* P = nullptr;
+  if ((rc = aam_plan(h, h->aam, N, Cr * K, D, s, &P))) return rc;
+  if ((rc = aam_prep(*P, E, W, false, s))) return rc;
+  for (const ConvLaunch& L : P->fwd)
+    if ((rc = launch_conv(L, s))) return rc;
+  dsk::aam_shard_cos_kernel<<<N, 256, 0, s>>>(P->gcos, P->Cp, E, W, D, labels, c0, Cr, K, topk, cos, sub,
+                                              reinterpret_cast<unsigned long long*>(keys));
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_aam_shard_merge(const float* cos, const int64_t* labels, const uint64_t* keys, int32_t R, int32_t N,
+                            int32_t C, int32_t c0, int32_t c1, int32_t topk, float margin, float scale,
+                            float topk_margin, int32_t* top, uint64_t* thr, float* mloc, void* stream) {
+  if (int rc = aam_shard_check(cos && labels && mloc && (topk == 0 || (keys && top && thr)), R, N, C, c0, c1, 1, 64,
+                               margin, scale, topk, topk_margin, "dsk_aam_shard_merge"))
+    return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  dsk::aam_shard_merge_kernel<<<N, 256, 0, s>>>(cos, labels, reinterpret_cast<const unsigned long long*>(keys), R, N, c0,
+                                                c1 - c0, topk, aam_margin(margin, scale, topk_margin), top,
+                                                reinterpret_cast<unsigned long long*>(thr), mloc);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+static bool aam_shard_nb_ok(int nb, int c0, int c1) {
+  return nb >= (c1 - c0 + dsk::kAamShardBlock - 1) / dsk::kAamShardBlock && nb <= 1 << 20;
+}
+
+int32_t dsk_aam_shard_partials(const float* cos, const int64_t* labels, const uint64_t* thr, const float* maxima,
+                               int32_t R, int32_t N, int32_t C, int32_t c0, int32_t c1, int32_t topk, int32_t nb,
+                               float margin, float scale, float topk_margin, float* m, float* rec, void* stream) {
+  if (int rc = aam_shard_check(cos && labels && maxima && m && rec && (topk == 0 || thr), R, N, C, c0, c1, 1, 64, margin,
+                               scale, topk, topk_margin, "dsk_aam_shard_partials"))
+    return rc;
+  if (!aam_shard_nb_ok(nb, c0, c1))
+    return fail(DSK_ERR_INVALID, "dsk_aam_shard_partials: nb %d is not in [ceil((c1 - c0) / %d), 2^20] for c0 %d, c1 %d",
+                nb, dsk::kAamShardBlock, c0, c1);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  dsk::aam_shard_partials_kernel<<<N, dsk::kAamShardBlock, 0, s>>>(
+      cos, labels, reinterpret_cast<const unsigned long long*>(thr), maxima, R, N, c0, c1 - c0, topk, nb,
+      aam_margin(margin, scale, topk_margin), m, rec);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_aam_shard_finish(const float* rec, const float* m, const int64_t* labels, int32_t R, int32_t N, int32_t C,
+                             int32_t nb, float* loss, float* lse, float* row_loss, float* den, void* stream) {
+  if (!rec || !m || !labels || !loss || !lse || !row_loss || !den || R < 1 || N < 1 || C < 2 || nb < 1 ||
+      nb > 1 << 20 || static_cast<int64_t>(R) * nb * dsk::kAamShardBlock < C)
+    return fail(DSK_ERR_INVALID, "dsk_aam_shard_finish: bad arguments (need non-null pointers, R >= 1, N >= 1, C >= 2, "
+                "1 <= nb <= 2^20 with R nb %d >= C; got R %d, N %d, C %d, nb %d)", dsk::kAamShardBlock, R, N, C, nb);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  dsk::aam_shard_finish_kernel<<<(N + 7) / 8, 256, 0, s>>>(rec, m, labels, R, N, C, nb, lse, row_loss, den);
+  KERNEL_CHECK();
+  dsk::mean_rows_kernel<<<1, 1024, 0, s>>>(row_loss, N, N, loss);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_aam_shard_bwd(dsk_handle h, const float* E, const float* W, const int64_t* labels, const float* cos,
+                          const uint8_t* sub, const uint64_t* thr, const float* m, const float* den, int32_t N,
+                          int32_t C, int32_t c0, int32_t c1, int32_t K, int32_t D, float margin, float scale,
+                          int32_t topk, float topk_margin, const float* grad_loss, float* gW, float* gE_part,
+                          void* stream) {
+  int rc = aam_shard_check(E && W && labels && cos && (K == 1 || sub) && (topk == 0 || thr) && m && den && grad_loss &&
+                               gW && gE_part, 1, N, C, c0, c1, K, D, margin, scale, topk, topk_margin,
+                           "dsk_aam_shard_bwd");
+  if (rc || (rc = check_handle(h))) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int CK = (c1 - c0) * K;
+  AamPlan* P = nullptr;
+  if ((rc = aam_plan(h, h->aam, N, CK, D, s, &P))) return rc;
+  if ((rc = aam_prep(*P, E, W, true, s))) return rc;
+  dsk::aam_shard_dcos_kernel<<<P->Np, 256, 0, s>>>(cos, sub, reinterpret_cast<const unsigned long long*>(thr), m, den,
+                                                   labels, N, c0, c1 - c0, K, P->Cp, topk,
+                                                   aam_margin(margin, scale, topk_margin), grad_loss, P->dcos, P->da,
+                                                   P->rinv);
+  KERNEL_CHECK();
+  dsk::aam_dcos_t_kernel<<<P->Cp / 32, 256, 0, s>>>(P->dcos, P->Np, P->Cp, P->dt, P->cinv);
+  KERNEL_CHECK();
+  for (const ConvLaunch& L : P->ge_gemm)
+    if ((rc = launch_conv(L, s))) return rc;
+  for (const ConvLaunch& L : P->gw_gemm)
+    if ((rc = launch_conv(L, s))) return rc;
+  const size_t nd = static_cast<size_t>(N) * D;
+  dsk::aam_shard_gpart_kernel<<<static_cast<unsigned>((nd + 255) / 256), 256, 0, s>>>(
+      P->ge, P->sc, static_cast<size_t>(P->Np) * D, P->rinv, N, D, gE_part);
+  KERNEL_CHECK();
+  dsk::aam_normalize_bwd_kernel<<<(CK + 7) / 8, 256, 0, s>>>(W, P->nrm_w, P->gw, P->sn, static_cast<long>(P->Cp) * D,
+                                                             P->cinv, CK, D, gW);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_aam_shard_bwd_rows(const float* E, const float* parts, int32_t R, int32_t n, int32_t D, float* gE,
+                               void* stream) {
+  if (!E || !parts || !gE || R < 1 || n < 1 || D < 1)
+    return fail(DSK_ERR_INVALID, "dsk_aam_shard_bwd_rows: bad arguments (need non-null pointers, R >= 1, n >= 1, "
+                "D >= 1; got R %d, n %d, D %d)", R, n, D);
+  dsk::aam_shard_rows_bwd_kernel<<<(n + 7) / 8, 256, 0, static_cast<cudaStream_t>(stream)>>>(E, parts, R, n, D, gE);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
 // ---- generalised end-to-end (GE2E) loss ---------------------------------------------------------------------------
 // The handle's GE2E plan for (N, P, D, row0, rows).  A rebuild synchronises `s` (buffers in use are freed).
 static int ge2e_plan(dsk_handle h, int N, int P, int D, int row0, int rows, cudaStream_t s, Ge2ePlan** out) {

@@ -513,6 +513,146 @@ class AAMSoftmaxFn(torch.autograd.Function):
         return ((gE if ctx.needs_input_grad[0] else None), (gW if ctx.needs_input_grad[1] else None)) + (None,) * 6
 
 
+# ---- the class-sharded op (include/dsk.h, dsk_aam_shard_*): the stages of parallel.ShardedAAMSoftmaxLoss --------------
+# Rank r holds the classes [c0, c1) of C, i.e. the rows [c0 K, c1 K) of the (C K, D) weight as W_r, and all N gathered
+# rows.  Every tensor a stage returns is caller-owned; the handle's plan holds nothing between stages.
+
+def _shard_tensor(t, name, shape, dtype, device):
+    """A caller's tensor for a dsk_aam_shard_* call: on ``device``, of ``dtype`` and ``shape`` (None entries free) and
+    contiguous, or RuntimeError (the C ABI sees pointers only)."""
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != device:
+        raise RuntimeError(f"{name} must be a CUDA tensor on {device}")
+    if t.dtype != dtype:
+        raise RuntimeError(f"{name} must be {dtype}, got {t.dtype}")
+    if t.dim() != len(shape) or any(s is not None and s != d for s, d in zip(shape, t.shape)):
+        raise RuntimeError(f"{name} must have shape {tuple('*' if s is None else s for s in shape)}, got {tuple(t.shape)}")
+    if not t.is_contiguous():
+        raise RuntimeError(f"{name} must be contiguous")
+    return t
+
+
+def _shard_rows(cos, labels, c0, c1):
+    """The (N, c1 - c0) class cosines of a shard and the (N,) global labels; a valid range is the C ABI's check."""
+    if not isinstance(cos, torch.Tensor) or cos.dim() != 2:
+        raise RuntimeError("cos must be the (N, c1 - c0) shard cosines")
+    dev, N = cos.device, cos.shape[0]
+    _shard_tensor(cos, "cos", (N, c1 - c0), torch.float32, dev)
+    _shard_tensor(labels, "labels", (N,), torch.int64, dev)
+    return N, dev
+
+
+def aam_shard_cos(E, W, labels, C, c0, c1, subcentres, topk):
+    """dsk_aam_shard_cos: (cos (N, c1 - c0), sub (N, c1 - c0) uint8 or None when subcentres = 1, keys (N, topk) int64
+    (the uint64 candidate keys' bits) or None when topk = 0)."""
+    if not isinstance(E, torch.Tensor) or E.dim() != 2:
+        raise RuntimeError("E must be the (N, D) gathered embeddings")
+    N, D = E.shape
+    dev, Cr = E.device, c1 - c0
+    _shard_tensor(E, "E", (N, D), torch.float32, dev)
+    _shard_tensor(W, "W", (Cr * subcentres, D), torch.float32, dev)
+    _shard_tensor(labels, "labels", (N,), torch.int64, dev)
+    cos = torch.empty(N, Cr, device=dev, dtype=torch.float32)
+    sub = torch.empty(N, Cr, device=dev, dtype=torch.uint8) if subcentres > 1 else None
+    keys = torch.empty(N, topk, device=dev, dtype=torch.int64) if topk > 0 else None
+    with torch.cuda.device(dev):
+        L.check(L.load().dsk_aam_shard_cos(_allpairs_handle(dev), E.data_ptr(), W.data_ptr(), labels.data_ptr(), N, C,
+                                           c0, c1, subcentres, D, topk, cos.data_ptr(), L.ptr(sub), L.ptr(keys),
+                                           L.cur_stream()), "dsk_aam_shard_cos")
+    return cos, sub, keys
+
+
+def aam_shard_merge(cos, labels, keys_all, R, C, c0, c1, topk, margin, scale, topk_margin):
+    """dsk_aam_shard_merge: (top (N, topk) int32 or None, thr (N,) int64 (uint64 bits) or None, mloc (N,)) from the
+    gathered candidate keys keys_all (R N topk,) in rank order."""
+    N, dev = _shard_rows(cos, labels, c0, c1)
+    if topk > 0:
+        _shard_tensor(keys_all, "keys_all", (R * N * topk,) if keys_all.dim() == 1 else (R * N, topk), torch.int64,
+                      dev)
+    top = torch.empty(N, topk, device=dev, dtype=torch.int32) if topk > 0 else None
+    thr = torch.empty(N, device=dev, dtype=torch.int64) if topk > 0 else None
+    mloc = torch.empty(N, device=dev, dtype=torch.float32)
+    with torch.cuda.device(dev):
+        L.check(L.load().dsk_aam_shard_merge(cos.data_ptr(), labels.data_ptr(), L.ptr(keys_all), R, N, C, c0, c1, topk,
+                                             float(margin), float(scale), float(topk_margin), L.ptr(top), L.ptr(thr),
+                                             mloc.data_ptr(), L.cur_stream()), "dsk_aam_shard_merge")
+    return top, thr, mloc
+
+
+def aam_shard_partials(cos, labels, thr, maxima, R, C, c0, c1, topk, nb, margin, scale, topk_margin):
+    """dsk_aam_shard_partials: (m (N,) the global row max, rec (N, 2 nb + 2) fp32 records) from the gathered maxima
+    (R N,) in rank order."""
+    N, dev = _shard_rows(cos, labels, c0, c1)
+    if topk > 0:
+        _shard_tensor(thr, "thr", (N,), torch.int64, dev)
+    _shard_tensor(maxima, "maxima", (R * N,), torch.float32, dev)
+    m = torch.empty(N, device=dev, dtype=torch.float32)
+    rec = torch.empty(N, 2 * nb + 2, device=dev, dtype=torch.float32)
+    with torch.cuda.device(dev):
+        L.check(L.load().dsk_aam_shard_partials(cos.data_ptr(), labels.data_ptr(), L.ptr(thr), maxima.data_ptr(), R, N,
+                                                C, c0, c1, topk, nb, float(margin), float(scale), float(topk_margin),
+                                                m.data_ptr(), rec.data_ptr(), L.cur_stream()), "dsk_aam_shard_partials")
+    return m, rec
+
+
+def aam_shard_finish(rec_all, m, labels, R, C, nb):
+    """dsk_aam_shard_finish: (loss (1,), lse (N,), row_loss (N,), den (N, 2)) from the gathered records
+    (R N (2 nb + 2),) in rank order; the same bits on every rank and for every split."""
+    if not isinstance(m, torch.Tensor) or m.dim() != 1:
+        raise RuntimeError("m must be the (N,) row maxima")
+    N, dev = m.shape[0], m.device
+    _shard_tensor(m, "m", (N,), torch.float32, dev)
+    _shard_tensor(labels, "labels", (N,), torch.int64, dev)
+    _shard_tensor(rec_all, "rec_all", (R * N * (2 * nb + 2),) if rec_all.dim() == 1 else (R * N, 2 * nb + 2),
+                  torch.float32, dev)
+    loss = torch.empty(1, device=dev, dtype=torch.float32)
+    lse, row_loss = (torch.empty(N, device=dev, dtype=torch.float32) for _ in range(2))
+    den = torch.empty(N, 2, device=dev, dtype=torch.float32)
+    with torch.cuda.device(dev):
+        L.check(L.load().dsk_aam_shard_finish(rec_all.data_ptr(), m.data_ptr(), labels.data_ptr(), R, N, C, nb,
+                                              loss.data_ptr(), lse.data_ptr(), row_loss.data_ptr(), den.data_ptr(),
+                                              L.cur_stream()), "dsk_aam_shard_finish")
+    return loss, lse, row_loss, den
+
+
+def aam_shard_backward(E, W, labels, cos, sub, thr, m, den, C, c0, c1, margin, scale, subcentres, topk, topk_margin,
+                       grad_loss):
+    """dsk_aam_shard_bwd: (gW (shard rows, D), gE_part (N, D)): the shard's weight gradient and its partial gradient
+    w.r.t. the normalised rows, scaled by the device scalar ``grad_loss``."""
+    N, dev = _shard_rows(cos, labels, c0, c1)
+    D = E.shape[1] if isinstance(E, torch.Tensor) and E.dim() == 2 else 0
+    _shard_tensor(E, "E", (N, D), torch.float32, dev)
+    _shard_tensor(W, "W", ((c1 - c0) * subcentres, D), torch.float32, dev)
+    if subcentres > 1:
+        _shard_tensor(sub, "sub", (N, c1 - c0), torch.uint8, dev)
+    if topk > 0:
+        _shard_tensor(thr, "thr", (N,), torch.int64, dev)
+    _shard_tensor(m, "m", (N,), torch.float32, dev)
+    _shard_tensor(den, "den", (N, 2), torch.float32, dev)
+    gl = grad_loss.float().reshape(1).contiguous()
+    gW, part = torch.empty_like(W), torch.empty_like(E)
+    with torch.cuda.device(E.device):
+        L.check(L.load().dsk_aam_shard_bwd(_allpairs_handle(E.device), E.data_ptr(), W.data_ptr(), labels.data_ptr(),
+                                           cos.data_ptr(), L.ptr(sub), L.ptr(thr), m.data_ptr(), den.data_ptr(), N, C,
+                                           c0, c1, subcentres, D, float(margin), float(scale), topk, float(topk_margin),
+                                           gl.data_ptr(), gW.data_ptr(), part.data_ptr(), L.cur_stream()),
+                "dsk_aam_shard_bwd")
+    return gW, part
+
+
+def aam_shard_backward_rows(E_local, parts, R):
+    """dsk_aam_shard_bwd_rows: gE (n, D) of this rank's rows from the R ranks' partials of them (R n D,), rank order."""
+    if not isinstance(E_local, torch.Tensor) or E_local.dim() != 2:
+        raise RuntimeError("E_local must be this rank's (n, D) embeddings")
+    n, D = E_local.shape
+    _shard_tensor(E_local, "E_local", (n, D), torch.float32, E_local.device)
+    _shard_tensor(parts, "parts", (R * n * D,) if parts.dim() == 1 else (R * n, D), torch.float32, E_local.device)
+    gE = torch.empty_like(E_local)
+    with torch.cuda.device(E_local.device):
+        L.check(L.load().dsk_aam_shard_bwd_rows(E_local.data_ptr(), parts.data_ptr(), R, n, D, gE.data_ptr(),
+                                                L.cur_stream()), "dsk_aam_shard_bwd_rows")
+    return gE
+
+
 # ---------------------------------------------------------------------------------------------------
 # generalised end-to-end (GE2E) loss
 # ---------------------------------------------------------------------------------------------------

@@ -18,8 +18,16 @@ column's dcos).  The gradient reduction stays the one all-reduce.
 
 Synchronised BatchNorm adds one all_gather of per-utterance records at each of the 12 BatchNorm layers of a forward
 and at 13 points of its backward (the loss scale, then the 12 layers); see ``gather_records`` for the record sizes.
+
+The sharded AAM-softmax head (``ShardedAAMSoftmaxLoss``, ``steps.sharded_aam_softmax_step``) is model parallel in its
+classes: rank r holds the contiguous class range ``class_shards(C, R)[r]`` of the (C K, D) weight, its gradient and
+its optimizer state, and the weight leaves the gradient all-reduce.  Per forward it adds four all_gathers (the fp32
+embeddings, the top-k candidate keys, the row maxima, the per-block partial sums) and per backward one all_to_all of
+the embedding rows' gradients; see ``ShardedAAMSoftmaxLoss`` for the sizes.
 """
 from __future__ import annotations
+
+import math
 
 import torch
 import torch.distributed as dist
@@ -309,3 +317,248 @@ def gather_records(local, process_group=None):
         parts.append(rows[:, off:off + t.numel()].reshape(-1))
         off += t.numel()
     return parts
+
+
+# ---- the class-sharded AAM-softmax head ------------------------------------------------------------------------------
+SHARD_BLOCK = 128   # classes per block of a shard boundary and of the forward's partial sums (dsk_aam_shard_partials)
+
+
+def class_shards(C: int, R: int):
+    """The contiguous class ranges [(c0, c1)] of R ranks over C classes: interior boundaries on multiples of 128
+    classes, range sizes that differ by at most 128 (the ranges holding one block more are the last ones, so the last
+    range's partial block does not widen the spread).  All K sub-centres of a class stay with its rank (a class's cosine
+    is the max over them).  ValueError when C < 128 R."""
+    for v, name in ((C, "C"), (R, "R")):
+        if isinstance(v, bool) or not isinstance(v, int):
+            raise ValueError(f"{name} must be an int, got {v!r}")
+    if R < 1 or C < SHARD_BLOCK * R:
+        raise ValueError(f"class_shards: {R} ranks need R >= 1 and at least {SHARD_BLOCK} classes each (C >= "
+                         f"{SHARD_BLOCK * max(R, 1)}), got C = {C}")
+    nb = -(-C // SHARD_BLOCK)
+    base, extra = divmod(nb, R)
+    out, c0 = [], 0
+    for r in range(R):
+        c1 = min(c0 + (base + (r >= R - extra)) * SHARD_BLOCK, C)
+        out.append((c0, c1))
+        c0 = c1
+    return out
+
+
+def shard_record_blocks(C: int, R: int) -> int:
+    """Blocks per row of a rank's partial-sum record: the largest range's ceil(size / 128), the same on every rank."""
+    return max(-(-(c1 - c0) // SHARD_BLOCK) for c0, c1 in class_shards(C, R))
+
+
+def emulated_gather(local):
+    """The forward exchange of R ranks emulated in one process: every rank receives the concatenation, in rank order,
+    of all ranks' records (what ``gather_records`` delivers under a process group)."""
+    cat = torch.cat([t.reshape(-1) for t in local])
+    return [cat] * len(local)
+
+
+def emulated_all_to_all(local):
+    """The backward exchange of R ranks emulated in one process: ``local[q]`` is rank q's (N, D) partial gradient of
+    all N = R n rows; rank r receives rows [r n, (r + 1) n) of every rank's partial, in rank order."""
+    R = len(local)
+    n = local[0].shape[0] // R
+    return [torch.cat([p[r * n:(r + 1) * n] for p in local]) for r in range(R)]
+
+
+def _all_to_all_rows(local, process_group=None):
+    """The backward exchange of a process group: ``all_to_all_single`` of each (N, D) partial (rows [q n, (q + 1) n)
+    to rank q), (R n, D) back in rank order.  Without a process group the local partials are returned."""
+    if not _distributed(process_group):
+        return list(local)
+    outs = []
+    for t in local:
+        t = t.contiguous()
+        out = torch.empty_like(t)
+        dist.all_to_all_single(out, t, group=process_group)
+        outs.append(out)
+    return outs
+
+
+class _ShardState:
+    """What the sharded forward leaves for its backward (all caller-owned device tensors)."""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+
+class _ShardedAAMFn(torch.autograd.Function):
+    """Forward: the four exchanged stages of ``ShardedAAMSoftmaxLoss.forward_stages``.  Backward: the shard's gW and
+    partial gE^, the all_to_all, this rank's rows of gE."""
+
+    @staticmethod
+    def forward(ctx, local_emb, weight, global_labels, head):
+        from .train import run_lockstep
+
+        st = run_lockstep([head.forward_stages(local_emb, global_labels)],
+                          lambda local: gather_records(local, head.group))[0]
+        ctx.head, ctx.st = head, st
+        return st.loss.reshape(())
+
+    @staticmethod
+    def backward(ctx, gl):
+        from .train import run_lockstep
+
+        head = ctx.head
+        gE, gW = run_lockstep([head.backward_stages(ctx.st, gl)], lambda local: _all_to_all_rows(local, head.group))[0]
+        ni = ctx.needs_input_grad
+        return (gE if ni[0] else None), (gW if ni[1] else None), None, None
+
+
+class ShardedAAMSoftmaxLoss:
+    """``AAMSoftmaxLoss`` (sub-centres, inter-top-k penalty) with its classes sharded over the ranks of
+    ``process_group``: a model-parallel classifier.  Rank r holds ``.weight``, the ``nn.Parameter`` W_r = rows
+    [c0 K, c1 K) of the (C K, D) weight for its ``.class_range`` (c0, c1) = ``class_shards(C, R)[r]``; no rank holds
+    the others.  Every rank holds the same n utterances (the precondition of ``GlobalGE2ELoss``).
+
+    ``forward(local_emb, global_labels)`` (labels from ``gather_labels``) returns the loss of ``AAMSoftmaxLoss`` on the
+    gathered batch with the full weight, a 0-dim device scalar with the same bits on every rank and for every R and
+    split; ``cos``, ``sub`` and ``top`` are the whole op's bits.  Its gradient w.r.t. ``local_emb`` is this rank's rows
+    of the global loss's gradient (the shards' parts added in rank order: within ~1e-6 of any other split) and w.r.t.
+    ``.weight`` the global loss's gradient for the shard (the same bits for every split).  Without a process group, or
+    at world size 1, the same stages run with R = 1, so a one-GPU run reproduces a multi-GPU run bit for bit.
+
+    ``weight_full_or_shape``: the full (C K, D) weight (this rank copies its rows: e.g. ``model.model.classifier.weight``
+    at K = 1), or its shape, for a weight drawn from N(0, 1/D) with the generator seeded by ``seed`` (the same on every
+    rank).  ``shard=(rank, R)`` without a process group runs the stages as rank ``rank`` of R emulated ranks: the caller
+    then drives ``forward_stages`` / ``backward_stages`` of all R heads with ``train.run_lockstep`` and the exchanges
+    ``emulated_gather`` / ``emulated_all_to_all``.
+
+    Collectives per step, N = R n rows, topk = k, nb = ``shard_record_blocks(C, R)``, bytes received per rank: forward
+    all_gathers of the embeddings (N D 4), the top-k keys (R N k 8, none at k = 0), the row maxima (R N 4) and the
+    partial-sum records (R N (2 nb + 2) 4, about N C / 16 bytes: R nb ~ C / 128 blocks of two floats per row); backward
+    one all_to_all of the embedding rows' gradients (n D 4 bytes per pair of ranks).  Each rank sends records for all N
+    rows, hence the factor R.  The weight, its gradient and its optimizer state never travel."""
+
+    def __init__(self, weight_full_or_shape, margin, scale, *, subcentres=1, topk=0, topk_margin=0.0,
+                 process_group=None, shard=None, seed=0, device=None):
+        if isinstance(weight_full_or_shape, torch.Tensor):
+            full = weight_full_or_shape.detach()
+            if full.dim() != 2:
+                raise ValueError(f"expected a (C * subcentres, D) weight, got shape {tuple(full.shape)}")
+            rows, D = full.shape
+        else:
+            full = None
+            rows, D = (int(v) for v in weight_full_or_shape)
+        self.C = _engine.aam_subcentre_args(rows, subcentres, topk, topk_margin)
+        for v, name in ((margin, "margin"), (scale, "scale")):
+            if not math.isfinite(float(v)):
+                raise ValueError(f"{name} must be finite, got {v!r}")
+        if float(margin) < 0.0 or not float(scale) > 0.0:
+            raise ValueError(f"need margin >= 0 and scale > 0, got {margin!r}, {scale!r}")
+        if D < 64 or D % 64:
+            raise ValueError(f"the embedding size must be a positive multiple of 64, got {D}")
+        self.margin, self.scale = float(margin), float(scale)
+        self.subcentres, self.topk, self.topk_margin = subcentres, topk, float(topk_margin)
+        self.group = process_group
+        if _distributed(process_group):
+            if shard is not None:
+                raise ValueError("shard= emulates ranks without a process group; the group gives the rank")
+            self.rank, self.world = dist.get_rank(process_group), dist.get_world_size(process_group)
+        elif shard is not None:
+            self.rank, self.world = (int(v) for v in shard)
+            if not 0 <= self.rank < self.world:
+                raise ValueError(f"shard must be (rank, R) with 0 <= rank < R, got {shard!r}")
+        else:
+            self.rank, self.world = 0, 1
+        self.shards = class_shards(self.C, self.world)
+        self.class_range = self.shards[self.rank]
+        self.record_blocks = shard_record_blocks(self.C, self.world)
+        c0, c1 = self.class_range
+        K = subcentres
+        if (c1 - c0) * K > _engine.L.DSK_AAM_MAX_C:
+            raise ValueError(f"the shard holds {(c1 - c0) * K} weight rows, above the per-rank cap "
+                             f"{_engine.L.DSK_AAM_MAX_C}: use more ranks or fewer sub-centres")
+        if device is None:
+            device = full.device if full is not None and full.is_cuda else torch.device("cuda", torch.cuda.current_device())
+        if full is None:
+            gen = torch.Generator().manual_seed(int(seed))
+            full = torch.randn(rows, D, generator=gen) / D ** 0.5
+        self.weight = torch.nn.Parameter(full[c0 * K:c1 * K].to(device=device, dtype=torch.float32).clone())
+
+    # -- the weight ---------------------------------------------------------------------------------------------------
+    def full_weight(self) -> torch.Tensor:
+        """The full (C K, D) weight in class order: an all_gather of the shards (for checkpoints, or to hand the weight
+        to a one-GPU ``AAMSoftmaxLoss``).  Collective: every rank must call it."""
+        w = self.weight.detach()
+        if not _distributed(self.group):
+            if self.world > 1:
+                raise RuntimeError("full_weight needs the process group; emulated shards hold only their own rows")
+            return w.clone()
+        K, D = self.subcentres, w.shape[1]
+        most = max(c1 - c0 for c0, c1 in self.shards) * K
+        pad = w.new_zeros(most, D)
+        pad[:w.shape[0]] = w
+        out = w.new_empty(self.world * most, D)
+        dist.all_gather_into_tensor(out, pad, group=self.group)
+        out = out.view(self.world, most, D)
+        return torch.cat([out[r, :(c1 - c0) * K] for r, (c0, c1) in enumerate(self.shards)])
+
+    @torch.no_grad()
+    def load_full_weight(self, W):
+        """Copies this rank's rows of the full (C K, D) weight W into ``.weight``."""
+        c0, c1 = self.class_range
+        K = self.subcentres
+        if tuple(W.shape) != (self.C * K, self.weight.shape[1]):
+            raise ValueError(f"expected a ({self.C * K}, {self.weight.shape[1]}) weight, got {tuple(W.shape)}")
+        self.weight.copy_(W[c0 * K:c1 * K])
+
+    # -- the stages -----------------------------------------------------------------------------------------------
+    def forward_stages(self, local_emb, global_labels):
+        """Generator of this rank's forward: yields its records four times (the fp32 embeddings, the top-k keys unless
+        topk = 0, the row maxima, the partial-sum records), each time receiving every rank's, concatenated in rank
+        order; returns the state ``backward_stages`` reads (StopIteration.value), with ``.loss`` (1,), ``.lse``,
+        ``.row_loss``, ``.cos``, ``.sub``, ``.top``."""
+        x = local_emb.detach().float().contiguous()
+        n, D = x.shape
+        E = (yield x).reshape(-1, D).contiguous()
+        labels = torch.as_tensor(global_labels).to(device=E.device, dtype=torch.int64).contiguous()
+        if labels.shape != (E.shape[0],):
+            raise ValueError(f"expected global labels of shape ({E.shape[0]},), got {tuple(labels.shape)}")
+        W = self.weight.detach().contiguous()
+        if W.device != E.device:
+            raise RuntimeError("ShardedAAMSoftmaxLoss: the weight and the embeddings must be on one device")
+        c0, c1 = self.class_range
+        R, C, K, k, nb = self.world, self.C, self.subcentres, self.topk, self.record_blocks
+        margins = (self.margin, self.scale, self.topk_margin)
+        cos, sub, keys = _engine.aam_shard_cos(E, W, labels, C, c0, c1, K, k)
+        keys_all = (yield keys) if k > 0 else None
+        top, thr, mloc = _engine.aam_shard_merge(cos, labels, keys_all, R, C, c0, c1, k, *margins)
+        maxima = yield mloc
+        m, rec = _engine.aam_shard_partials(cos, labels, thr, maxima, R, C, c0, c1, k, nb, *margins)
+        rec_all = yield rec
+        loss, lse, row_loss, den = _engine.aam_shard_finish(rec_all, m, labels, R, C, nb)
+        return _ShardState(E=E, W=W, labels=labels, n=n, cos=cos, sub=sub, top=top, thr=thr, m=m, den=den, loss=loss,
+                           lse=lse, row_loss=row_loss)
+
+    def backward_stages(self, st, grad_loss):
+        """Generator of this rank's backward from the forward's state: yields the shard's (N, D) partial gradient of
+        the normalised rows once and receives this rank's n rows of every rank's partial, (R n, D) in rank order;
+        returns (gE (n, D), gW of the shard), scaled by the device scalar ``grad_loss``."""
+        c0, c1 = self.class_range
+        gW, part = _engine.aam_shard_backward(st.E, st.W, st.labels, st.cos, st.sub, st.thr, st.m, st.den, self.C, c0,
+                                              c1, self.margin, self.scale, self.subcentres, self.topk, self.topk_margin,
+                                              grad_loss)
+        parts = yield part
+        r0 = self.rank * st.n
+        gE = _engine.aam_shard_backward_rows(st.E[r0:r0 + st.n].contiguous(), parts, self.world)
+        return gE, gW
+
+    def forward(self, local_emb, global_labels):
+        """local_emb (n, D) this rank's shard of the batch, global_labels (N,) int64 of the whole batch -> 0-dim
+        loss."""
+        if self.world > 1 and not _distributed(self.group):
+            raise RuntimeError("an emulated shard runs through forward_stages / backward_stages, not forward")
+        if local_emb.dim() != 2 or local_emb.shape[1] != self.weight.shape[1]:
+            raise ValueError(f"expected embeddings (n, {self.weight.shape[1]}), got {tuple(local_emb.shape)}")
+        if not local_emb.is_cuda:
+            raise RuntimeError("the sharded AAM-softmax loss needs CUDA tensors; there is no CPU fallback")
+        if tuple(global_labels.shape) != (self.world * local_emb.shape[0],):
+            raise ValueError(f"expected global labels of shape ({self.world * local_emb.shape[0]},) for {self.world} "
+                             f"ranks of {local_emb.shape[0]} embeddings, got {tuple(global_labels.shape)}")
+        return _ShardedAAMFn.apply(local_emb, self.weight, global_labels, self)
+
+    __call__ = forward

@@ -32,7 +32,7 @@ from .head import CrossEntropyLoss
 from .model import (AAMSoftmaxLoss, BatchHardTripletLoss, PairwiseDistance, TripletMarginLoss, batch_hard_valid_count,
                     select_hard_triplets)
 from .optim import FusedAdagrad
-from .parallel import GlobalBatchHardTripletLoss, GlobalGE2ELoss, _distributed, gather_labels
+from .parallel import GlobalBatchHardTripletLoss, GlobalGE2ELoss, GradBucket, _distributed, gather_labels
 
 _l2 = PairwiseDistance(2)   # train_triplet.py:119
 
@@ -197,6 +197,59 @@ def aam_softmax_step(model, optimizer, data, labels, *, margin, scale, bucket=No
     optimizer.zero_grad()
     loss.backward()
     _reduce_and_step(optimizer, bucket, None)
+    return {"loss": loss.detach()}
+
+
+def _held(opt):
+    if opt is None:
+        return []
+    if isinstance(opt, (FusedAdagrad, GradBucket)):
+        return list(opt.params)
+    return [p for g in opt.param_groups for p in g["params"]]
+
+
+def sharded_aam_softmax_step(model, optimizer, data, labels, *, head, head_optimizer, bucket=None):
+    """One AAM-softmax step with the class-sharded head ``head`` (``parallel.ShardedAAMSoftmaxLoss``): ONE train-mode
+    forward of this rank's n utterances, the sharded loss over the global batch, backward seeded with R, the network's
+    gradient reduction and step, then the shard's own step.  Returns ``{"loss": device scalar}``, the same on every
+    rank.
+
+    A step of its own rather than a ``head=`` argument of ``aam_softmax_step``: the two differ in everything after the
+    forward.  Here the labels are gathered, the loss issues collectives of its own, the backward is seeded with R, and
+    a second optimizer steps the shard with no collective; ``aam_softmax_step`` keeps its one all-reduce over the whole
+    weight and its signature.
+
+    ``optimizer`` (``FusedAdagrad`` or a torch optimizer with ``bucket``) holds the network's parameters and takes the
+    unchanged single mean all-reduce; ``head_optimizer`` holds ``head.weight`` only and steps it locally.  The backward's
+    seed R makes the shard's gradient R times the global loss's; the step undoes it: ``FusedAdagrad.step()`` without
+    ``allreduce()`` divides by R (build it with ``process_group=head.group``), and a torch optimizer gets the gradient
+    divided by R.  Both are exact at power-of-two R.  ValueError, on every rank before any collective, when
+    ``head.weight`` is in ``optimizer`` or ``bucket`` or not in ``head_optimizer``.  Runs unchanged on a model with
+    ``sync_batchnorm(group)``; without a process group it is the one-GPU step with R = 1."""
+    if not model.training:
+        raise RuntimeError("sharded_aam_softmax_step needs model.train()")
+    W = head.weight
+    if any(p is W for p in _held(optimizer) + _held(bucket)):
+        raise ValueError("sharded_aam_softmax_step: head.weight must not be in the network optimizer or the bucket "
+                         "(it is stepped by head_optimizer, with no collective)")
+    if not any(p is W for p in _held(head_optimizer)):
+        raise ValueError("sharded_aam_softmax_step: head_optimizer must hold head.weight")
+    world = head.world
+    if isinstance(head_optimizer, FusedAdagrad):
+        opt_world = dist.get_world_size(head_optimizer.group) if (dist.is_available() and dist.is_initialized()) else 1
+        if opt_world != world:
+            raise ValueError(f"sharded_aam_softmax_step: head_optimizer divides by its group's size {opt_world}, the "
+                             f"head has {world} ranks (build it with process_group=head.group)")
+    global_labels = gather_labels(_labels_to(labels, data.device), head.group)
+    emb = model(data)
+    loss = head.forward(emb, global_labels)
+    optimizer.zero_grad()
+    head_optimizer.zero_grad()
+    loss.backward(torch.full_like(loss, float(world)))       # R x this rank's share; the mean all-reduce divides by R
+    _reduce_and_step(optimizer, bucket, None)
+    if not isinstance(head_optimizer, FusedAdagrad):
+        W.grad.div_(world)
+    head_optimizer.step()
     return {"loss": loss.detach()}
 
 

@@ -414,6 +414,56 @@ int32_t dsk_aam_softmax_sc_bwd(dsk_handle h, const float* E, const float* W, con
 int32_t dsk_aam_subcentre_cos(const float* E, const float* W, const int64_t* labels, int32_t N, int32_t C, int32_t K,
                               int32_t D, float* out, void* stream);
 
+/* Class-sharded dsk_aam_softmax_sc (a model-parallel classifier): rank r of R holds the classes [c0, c1) of C, i.e. the
+ * rows [c0 K, c1 K) of the (C K, D) weight as W (local class c = global class c0 + c), and every rank holds the same
+ * N gathered rows E and global labels.  The loss, cos, sub, top and the formulas are those of dsk_aam_softmax_sc on
+ * the whole weight; only the placement of the work changes.  Four forward stages with an exchange between each
+ * (the caller moves the data: an all_gather in rank order, or a concatenation when one process emulates the ranks):
+ *   1. dsk_aam_shard_cos: cos (N, c1 - c0), sub (N, c1 - c0) uint8 (NULL when K = 1) over the shard, bit-identical to
+ *      those columns of the whole op's, and keys (N, topk) uint64: the row's local top-k candidates in rank order
+ *      (dsk_aam_softmax_sc's key: cosine bits, then the global class; the target excluded; 0 when the shard has fewer
+ *      than topk candidates).  Exchange: keys of all ranks, [R][N][topk] (none when topk = 0).
+ *   2. dsk_aam_shard_merge: top (N, topk) int32 (global class ids, the whole op's bits) and thr (N,) uint64 (the
+ *      last key) from the R topk candidates, then mloc (N,), the largest logit over the shard.  Exchange: mloc of all
+ *      ranks, [R][N].
+ *   3. dsk_aam_shard_partials: m (N,) the global max, and rec (N, 2 nb + 2) fp32: per 128-class block b of the shard
+ *      the sums S_b, S_other_b of exp(logit - m) (with and without the target; blocks past the shard are 0), then the
+ *      target logit s phi(cos) (on the rank that owns the class) and the flags (as float bits: 1 a NaN term, left out
+ *      of the sums; 2 the target is here; bits 8 and up the shard's block count).  nb must be the same on every
+ *      rank, >= ceil((c1 - c0) / 128).
+ *      Exchange: rec of all ranks, [R][N][2 nb + 2].
+ *   4. dsk_aam_shard_finish (no handle): the blocks summed in fp64 in an order fixed by the global block index alone
+ *      (one warp per row: lane g mod 32 adds blocks g in ascending order, then a fixed butterfly), so the result does
+ *      not depend on R or the split; lse = m + log S rounded once, row losses, loss (1,) (the fixed-order mean), and
+ *      den (N, 2) = (S, S_other) fp32 for the backward.  A NaN term makes the row's lse, loss and den NaN.
+ * Backward, with no exchange before the GEMMs: dsk_aam_shard_bwd writes gW (the shard's (c1 - c0) K rows; softmax
+ * exp(logit - m) / S, the target's softmax - 1 = -S_other / S, the margins' chain rules, the chosen sub-centre's
+ * column only) and gE_part (N, D), this shard's gradient w.r.t. the normalised rows e^ for all N rows.  Exchange:
+ * each rank receives the partials of its own n rows from every rank (an all_to_all), [R][n][D]; dsk_aam_shard_bwd_rows
+ * adds them in rank order and applies the normalize Jacobian: gE (n, D).  Caller-owned state between the stages:
+ * cos, sub, top, thr, m, den; the handle's plan (that of dsk_aam_softmax_sc for (N, (c1 - c0) K, D)) holds nothing
+ * across an exchange, so one handle may run the stages of several emulated ranks interleaved.  Deterministic, no float
+ * atomics.  Ranges: 0 <= c0 < c1 <= C, c0 and c1 (unless c1 = C) multiples of 128, (c1 - c0) K <= DSK_AAM_MAX_C; the
+ * other limits as dsk_aam_softmax_sc; else DSK_ERR_INVALID. */
+int32_t dsk_aam_shard_cos(dsk_handle h, const float* E, const float* W, const int64_t* labels, int32_t N, int32_t C,
+                          int32_t c0, int32_t c1, int32_t K, int32_t D, int32_t topk, float* cos, uint8_t* sub,
+                          uint64_t* keys, void* stream);
+int32_t dsk_aam_shard_merge(const float* cos, const int64_t* labels, const uint64_t* keys, int32_t R, int32_t N,
+                            int32_t C, int32_t c0, int32_t c1, int32_t topk, float margin, float scale,
+                            float topk_margin, int32_t* top, uint64_t* thr, float* mloc, void* stream);
+int32_t dsk_aam_shard_partials(const float* cos, const int64_t* labels, const uint64_t* thr, const float* maxima,
+                               int32_t R, int32_t N, int32_t C, int32_t c0, int32_t c1, int32_t topk, int32_t nb,
+                               float margin, float scale, float topk_margin, float* m, float* rec, void* stream);
+int32_t dsk_aam_shard_finish(const float* rec, const float* m, const int64_t* labels, int32_t R, int32_t N, int32_t C,
+                             int32_t nb, float* loss, float* lse, float* row_loss, float* den, void* stream);
+int32_t dsk_aam_shard_bwd(dsk_handle h, const float* E, const float* W, const int64_t* labels, const float* cos,
+                          const uint8_t* sub, const uint64_t* thr, const float* m, const float* den, int32_t N,
+                          int32_t C, int32_t c0, int32_t c1, int32_t K, int32_t D, float margin, float scale,
+                          int32_t topk, float topk_margin, const float* grad_loss, float* gW, float* gE_part,
+                          void* stream);
+int32_t dsk_aam_shard_bwd_rows(const float* E, const float* parts, int32_t R, int32_t n, int32_t D, float* gE,
+                               void* stream);
+
 /* Generalised end-to-end (GE2E) loss against in-batch speaker centroids (Wan et al., ICASSP 2018; no reference
  * implementation exists).  For embeddings E (N,D) and a batch of P speakers given as a CSR: speaker k's rows are
  * S_k = order[offsets[k] .. offsets[k+1]) (n_k of them, ascending row index within a speaker), col[i] = the speaker of
