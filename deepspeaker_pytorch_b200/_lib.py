@@ -168,7 +168,6 @@ SIGNATURES = {
     "dsk_bn_act_train_backward": (c_int32, [c_void_p] * 11 + [c_int64, c_int32, c_float, c_void_p]),
     "dsk_conv3x3_padded": (c_int32, [c_void_p] * 7 + [c_int32, c_int32, c_int32, c_int32, c_int32, c_float, c_int32, c_void_p]),
     "dsk_conv5x5s2_planar": (c_int32, [c_void_p] * 6 + [c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_float, c_void_p]),
-    "dsk_debug_set_trace": (c_int32, [c_void_p, c_void_p]),
     "dsk_debug_set_backward_capture": (c_int32, [c_void_p, POINTER(DskBackwardCapture)]),
     "dsk_padded_positions": (c_int64, [c_int32, c_int32, c_int32]),
     "dsk_pack_conv_weight": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]),

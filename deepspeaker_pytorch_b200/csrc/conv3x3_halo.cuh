@@ -7,7 +7,7 @@
 //   * activations live in a ZERO-PADDED NHWC layout: rows R = n*(H+1)+h+1 (row 0 and the row after every image are
 //     zero), W+1 pixels per row (column 0 is zero), so position Q = R*(W+1) + w+1 and the 3x3 neighbourhood of Q is
 //     Q + (r-1)*(W+1) + (s-1) for every pixel, including image borders (the pads are real zeros in memory);
-//   * an output tile is 128 (64 in the two-CTA shape) CONSECUTIVE padded positions; its A operand for one 64-channel
+//   * an output tile is 128 CONSECUTIVE padded positions; its A operand for one 64-channel
 //     chunk is ONE contiguous TMA box of tile + 2W + 4 rows (the halo), and every filter tap reads it through a wgmma descriptor whose start
 //     address is shifted by (r*(W+1)+s) rows (row-shifted SWIZZLE_128B descriptors: the swizzle follows the address);
 //   * weights arrive as one box per filter row (3 taps x N_TILE x 64 ch); with 64 channels all 9 taps stay resident;
@@ -20,9 +20,9 @@ namespace dsk {
 // The same kernel runs the 5x5 stride-2 stage-entry convs (model.py:98,102,106): their input is stored PARITY-PLANAR
 // (four planes (h&1, w&1), each a zero-padded grid at the OUTPUT resolution), so that every tap (r, s) reads plane
 // (r&1, s&1) at a fixed shift ((r-2)>>1, (s-2)>>1) of the output position: one halo box per (64-channel chunk, plane)
-// serves all taps of that plane.  The K loop is table driven: a sequence of weight BOXES (<= 3 taps each, packed
-// consecutively in plane-major tap order), each tap with its own row shift into the current plane's halo tile.
-constexpr int kHaloMaxBoxes = 25;
+// serves all taps of that plane.  The weight BOXES (<= 3 taps each, packed consecutively in plane-major tap order) are
+// listed in a table the producer walks; the consumers run the same sequence from a compile-time plan (HaloPlan).
+constexpr int kHaloMaxBoxes = 9;  // 5x5 s2: 3 + 2 + 2 + 2 three-tap boxes
 constexpr int kHaloMaxStages = 4;
 
 struct HaloParams {
@@ -34,16 +34,13 @@ struct HaloParams {
   // shared-memory carve (runtime): ring depths and buffer counts chosen by the host per layer
   int a_stage_bytes;      // halo tile rows * 128 rounded up to 1024
   int a_stages, b_stages; // <= kHaloMaxStages
-  int stg_bufs, res_bufs; // output staging buffers (1 or 2), residual prefetch buffers (0, 1 or 2)
+  int stg_bufs;           // output staging buffers (1 or 2)
   // K-loop table (per 64-channel chunk)
   int nboxes;
   int plane_positions;                     // positions per input plane (parity-planar input), 0 for a single plane
   int8_t box_plane[kHaloMaxBoxes];         // input plane of the box's taps
   int8_t box_first[kHaloMaxBoxes];         // first box of its plane group: load the plane's halo tile
-  int8_t box_last[kHaloMaxBoxes];          // last box of its plane group: release the halo tile
-  int8_t box_ntaps[kHaloMaxBoxes];
   int16_t box_wtap[kHaloMaxBoxes];         // first packed tap index of the box
-  int16_t tap_shift[kHaloMaxBoxes][3];     // halo-tile row offset of each tap
   // output: standard padded layout (TMA store) or parity-planar (3x3 only; staged, then copied out in 128-byte rows;
   // feeds a stride-2 conv)
   int out_planar;
@@ -57,39 +54,20 @@ struct HaloParams {
   // resource the MMA operand fetch already saturates
   float scale_c[512];
   float bias_c[512];
-  int plain3x3;           // MMA issuer plan: 1 = 3x3 (HaloPlan<1>), 2 = planar 5x5 s2 (HaloPlan<2>), 0 = walk the tables
-  int late_trigger;       // release the dependent kernel when this CTA starts its last tile instead of at entry
   int b_resident;         // all weight boxes of a CTA's channel tile fit the B ring: load once
   // floor(2^64/d)+1 for d = W+1 and H+1: q/d == __umul64hi(q, magic) for every q < 2^32 (the error of the rounded-up
   // reciprocal, q (magic d - 2^64) / (d 2^64) < q / 2^64, stays below 1/d).  A 32-bit reciprocal is exact only for
   // q < 2^32/d, which the image index R / (H+1) of a long batch of long utterances passes.
   unsigned long long pitch_magic, img_magic;
-  // stream-K (DESIGN.md): a layer of this network has 1.3-2.4 tiles per SM, so whole-tile scheduling leaves 20-36 % of
-  // the SM-time of stages 2-4 idle in the last wave.  With stream_k the K loop of the layer (tiles x chunks x weight
-  // boxes "units") is cut into gridDim.x EQUAL contiguous ranges: a CTA's range covers the tail of one tile, whole
-  // tiles, and the head of another.  The CTA that holds the HEAD of a tile (units 0..) owns its epilogue; the CTAs
-  // holding later parts (always the FIRST thing in their range) dump their fp32 accumulator to sk_partial[cta] and raise
-  // sk_flags[cta]; the owner adds those partials in fixed order before its usual epilogue (deterministic).
-  int stream_k;
-  int sk_q, sk_r;      // CTA i owns units [i*sk_q + min(i, sk_r), (i+1)*sk_q + min(i+1, sk_r)) of the num_tiles * units of the layer
-  float* sk_partial;   // [gridDim.x][accumulator register][consumer thread] fp32: each thread writes / reads its own column
-  int* sk_flags;       // [gridDim.x], zero outside a launch
   const uint16_t* res_ptr;  // residual tensor (padded layout, cout channels per position): read straight from global / L2
-                            // by the 4-epilogue-warp variant, which has no shared memory to spare for residual tiles
-  long long* trace;       // debug: per-role clock64 stamps of CTA 0 (nullptr = off); [role 0..2][512]
 };
-
-// role: 0 producer, 1 MMA, 2 epilogue
-#define DSK_TRACE(role, idx)                                                                  \
-  do {                                                                                        \
-    if (p.trace && blockIdx.x == 0 && (idx) < 512) p.trace[(role) * 512 + (idx)] = clock64(); \
-  } while (0)
 
 // Compile-time K-loop plans for the MMA issuer (the producer still walks the runtime tables, which say the same).
 // KIND 1: 3x3, one plane, boxes = filter rows.  KIND 2: planar 5x5 s2, packed tap n = 3*box + t, planes start at
 // packed taps 0 / 9 / 15 / 21 and have 3x3, 3x2, 2x3, 2x2 taps; tap (i, j) of a plane reads halo row i*(W+1) + j.
-template <int KIND, int TPB>  // TPB = taps per weight box (3, or 1 for the 256-channel tile)
+template <int KIND>
 struct HaloPlan {
+  static constexpr int TPB = 3;  // taps per weight box
   static constexpr int kTaps = KIND == 1 ? 9 : 25;
   static constexpr int kBoxes = (kTaps + TPB - 1) / TPB;  // plane starts 0/9/15/21 are multiples of 3: boxes never straddle planes
   __host__ __device__ static constexpr int plane_of(int n) { return KIND == 1 ? 0 : (n < 9 ? 0 : n < 15 ? 1 : n < 21 ? 2 : 3); }
@@ -107,22 +85,13 @@ struct HaloPlan {
   }
 };
 
-// Two CTA shapes of the same kernel (template parameter EW = consumer warps); every consumer warpgroup computes one
-// 64-row slice of a tile and holds its 64 x N_TILE fp32 accumulators in registers:
-//   EW = 8: 384 threads, the whole SM (up to 227 KB of shared memory, 3-tap weight boxes); 128-position tiles;
-//   EW = 4: 256 threads, <= 128 registers per thread and <= 112.5 KB of shared memory, so that TWO CTAs share an SM;
-//           64-position tiles and one-tap weight boxes (16 KB at 128 channels).  Opt-in through DSK_SMALL_CTA=1.
-template <int N_TILE, int EW = 8>
+// One CTA per SM: 384 threads, up to 227 KB of shared memory; each of the two consumer warpgroups computes one 64-row
+// slice of a tile and holds its 64 x N_TILE fp32 accumulators in registers.
+template <int N_TILE>
 struct HaloSmem {
-  static_assert(EW == 8 || EW == 4, "two consumer warpgroups (one CTA per SM) or one (two CTAs per SM)");
-  static constexpr bool kSmall = EW == 4;
-  static constexpr int kTileRows = 16 * EW;  // positions per tile: 64 per consumer warpgroup
-  static constexpr int kTapsPerBox = (N_TILE == 256 || kSmall) ? 1 : 3;  // weight box: 3 taps (48 KB at 128 channels) or 1
-  static constexpr int kBStageBytes = kTapsPerBox * N_TILE * 128;
+  static constexpr int kTileRows = 128;  // positions per tile: 64 per consumer warpgroup
+  static constexpr int kBStageBytes = 3 * N_TILE * 128;  // weight box: 3 taps (48 KB at 128 channels)
   static constexpr int kFixedBytes = 512 + 1024;  // barriers + alignment slack
-  static int total(int a_stage_bytes, int a_stages, int b_stages, int stg_bufs, int res_bufs) {
-    return a_stages * a_stage_bytes + b_stages * kBStageBytes + (stg_bufs + res_bufs) * kATileBytes + kFixedBytes;
-  }
 };
 
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
@@ -141,23 +110,20 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* s
 
 // tmIn : 2-D (C, positions) view of the padded input, box {64, kTileRows + 2W + 4}
 // tmW  : 3-D (cin, cout, 9 taps) packed weights, box {64, N_TILE, 3}
-// tmOut : 2-D (C, positions) view of the padded output, box {64, kTileRows}   (tmRes: unused since the residual is read from
-//         global memory through HaloParams::res_ptr; kept in the signature)
-constexpr int kHaloThreads = 384;  // EW = 8: one control warpgroup + two consumer warpgroups
-constexpr int halo_threads(int ew) { return 128 + 32 * ew; }
+// tmOut : 2-D (C, positions) view of the padded output, box {64, kTileRows}   (the residual is read from global memory
+//         through HaloParams::res_ptr)
+constexpr int kHaloThreads = 384;  // one control warpgroup + two consumer warpgroups
 
 // KIND: the compile-time tap plan the consumers run - 1 = 3x3 (HaloPlan<1>), 2 = parity-planar 5x5 s2 (HaloPlan<2>).
 // One plan per instantiation (and the resident-weights burst only where it can occur, 64-channel 3x3): each
 // instantiation carries only what it runs.
-template <int N_TILE, bool BF16, int EW = 8, bool SK = false, int KIND = 1>
-__global__ void __launch_bounds__(128 + 32 * EW, EW == 4 ? 2 : 1)
+template <int N_TILE, bool BF16, int KIND>
+__global__ void __launch_bounds__(kHaloThreads, 1)
 conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant__ CUtensorMap tmW,
-                    const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmRes,
-                    const HaloParams p) {
-  using S = HaloSmem<N_TILE, EW>;
-  constexpr int kEpiThreads = 32 * EW;
-  constexpr int kCG = EW / 4;   // consumer warpgroups
-  static_assert(!(EW == 4 && N_TILE == 256), "the two-CTA-per-SM shape runs 64- and 128-channel tiles");
+                    const __grid_constant__ CUtensorMap tmOut, const HaloParams p) {
+  using S = HaloSmem<N_TILE>;
+  constexpr int kEpiThreads = 256;
+  constexpr int kCG = 2;        // consumer warpgroups
   constexpr int kMW = 1;        // 64-row slices of the tile per consumer warpgroup
   constexpr int kTM = S::kTileRows;
   const int kAStages = p.a_stages, kBStages = p.b_stages;
@@ -168,7 +134,7 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem_a + kAStages * p.a_stage_bytes;
   uint8_t* smem_stg = smem_b + kBStages * S::kBStageBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_stg + (p.stg_bufs + p.res_bufs) * kATileBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_stg + p.stg_bufs * kATileBytes);
   uint64_t* a_full = bars;
   uint64_t* a_empty = a_full + kHaloMaxStages;
   uint64_t* b_full = a_empty + kHaloMaxStages;
@@ -176,8 +142,7 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) DSK_TRACE(0, 480);
-  if (!p.late_trigger) pdl_launch_dependents();
+  pdl_launch_dependents();
   const int pitch = p.W + 1;
   const int halo_rows = kTM + 2 * p.W + 4;
   const int num_tiles = p.tiles_m * p.tiles_c;
@@ -189,33 +154,8 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
     c0 = ct * N_TILE;
     q0 = p.q_begin + mt * kTM;
   };
-
-  // Work iteration shared by all roles.  Without stream-K a segment is a whole tile (tile = blockIdx.x + k * gridDim.x,
-  // units [0, units)); with it, consecutive pieces of this CTA's unit range [u_lo, u_hi).
+  // a CTA's tiles: blockIdx.x, blockIdx.x + gridDim.x, ...; each runs units (weight box b of chunk ch) 0 .. units-1
   const int units = p.chunks * p.nboxes;
-  constexpr bool sk = SK;  // a separate instantiation: the whole-tile kernel carries none of the stream-K code
-  // (32-bit arithmetic throughout: the host enables stream-K only while num_tiles * units fits comfortably)
-  auto sk_lo = [&](int i) -> int { return i * p.sk_q + (i < p.sk_r ? i : p.sk_r); };
-  const int u_lo = sk ? sk_lo(static_cast<int>(blockIdx.x)) : 0;
-  const int u_hi = sk ? sk_lo(static_cast<int>(blockIdx.x) + 1) : 0;
-  auto seg_begin = [&]() -> int { return sk ? u_lo : static_cast<int>(blockIdx.x); };
-  auto next_seg = [&](int& cur, int& tile, int& ub, int& ue) -> bool {
-    if (sk) {
-      if (cur >= u_hi) return false;
-      tile = cur / units;
-      ub = cur - tile * units;
-      const int rem = u_hi - cur;
-      ue = (units - ub) <= rem ? units : ub + rem;
-      cur += ue - ub;
-    } else {
-      if (cur >= num_tiles) return false;
-      tile = cur;
-      ub = 0;
-      ue = units;
-      cur += gridDim.x;
-    }
-    return true;
-  };
 
   // Prologue, split over two warps so that the two first-use descriptor fetches overlap: warp 0 sets up the weight ring
   // and issues the first weight boxes (parameters: no dependency wait), warp 3 sets up the halo ring and issues the first
@@ -229,28 +169,20 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
         mbar_init(&b_empty[i], kCG);  // one arrive per consumer warpgroup
       }
       fence_barrier_init();
-      DSK_TRACE(0, 484);
     }
     __syncwarp();
-    {
-      int cur0 = seg_begin();
-      int tile0, ub0, ue0;
-      if (next_seg(cur0, tile0, ub0, ue0)) {
-        int c0, q0;
-        decode(tile0, c0, q0);
-        const int seg_b = ue0 - ub0;  // weight boxes of the first segment
-        pre_b = seg_b < kBStages ? seg_b : kBStages;
-        if (elect_one_sync()) {
-          for (int i = 0; i < pre_b; ++i) {
-            const int u = ub0 + i;
-            const int ch = u / p.nboxes, b = u - ch * p.nboxes;
-            mbar_arrive_expect_tx(&b_full[i], S::kBStageBytes);
-            tma_load_3d(smem_b + i * S::kBStageBytes, &tmW, &b_full[i], ch * 64, c0, p.box_wtap[b]);
-          }
+    if (static_cast<int>(blockIdx.x) < num_tiles) {
+      int c0, q0;
+      decode(blockIdx.x, c0, q0);
+      pre_b = units < kBStages ? units : kBStages;
+      if (elect_one_sync()) {
+        for (int i = 0; i < pre_b; ++i) {
+          const int ch = i / p.nboxes, b = i - ch * p.nboxes;
+          mbar_arrive_expect_tx(&b_full[i], S::kBStageBytes);
+          tma_load_3d(smem_b + i * S::kBStageBytes, &tmW, &b_full[i], ch * 64, c0, p.box_wtap[b]);
         }
-        __syncwarp();
-        if (lane == 0) DSK_TRACE(0, 485);
       }
+      __syncwarp();
     }
   }
   if (warp == 3) {
@@ -263,45 +195,33 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
       fence_barrier_init();
     }
     __syncwarp();
-    {
-      int cur0 = seg_begin();
-      int tile0, ub0, ue0;
-      if (next_seg(cur0, tile0, ub0, ue0)) {
-        int c0, q0;
-        decode(tile0, c0, q0);
-        pdl_wait();  // activations of the previous kernel are read below
-        if (lane == 0) DSK_TRACE(0, 486);
-        if (elect_one_sync()) {
-          const int ch = ub0 / p.nboxes, b = ub0 - ch * p.nboxes;
-          mbar_arrive_expect_tx(&a_full[0], halo_rows * 128);
-          tma_load_2d(smem_a, &tmIn, &a_full[0], ch * 64, p.box_plane[b] * p.plane_positions + q0 - (p.W + 2));
-          DSK_TRACE(0, 0);
-        }
-        __syncwarp();
+    if (static_cast<int>(blockIdx.x) < num_tiles) {
+      int c0, q0;
+      decode(blockIdx.x, c0, q0);
+      pdl_wait();  // activations of the previous kernel are read below
+      if (elect_one_sync()) {
+        mbar_arrive_expect_tx(&a_full[0], halo_rows * 128);
+        tma_load_2d(smem_a, &tmIn, &a_full[0], 0, p.box_plane[0] * p.plane_positions + q0 - (p.W + 2));
       }
+      __syncwarp();
     }
   }
   if (warp == 1 && lane == 0) tma_prefetch_desc(&tmOut);
   __syncthreads();
-  if (threadIdx.x == 0) DSK_TRACE(0, 481);
   pdl_wait();  // everything above (but the producer's first halo tile) touched only parameters
-  if (threadIdx.x == 0) DSK_TRACE(0, 482);
 
   if (warp == 0) {
     // ===================== TMA producer (warp-converged loop, one elected lane issues) =====================
     int as = 0, bs = 0;
     uint32_t aph = 0, bph = 0;
     bool first = true;
-    int tcount = 1;
     bool a_pre = true;  // the first halo tile was issued in the prologue
-    int cur = seg_begin();
-    int tile, ub, ue;
-    while (next_seg(cur, tile, ub, ue)) {
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int c0, q0;
       decode(tile, c0, q0);
-      for (int u = ub; u < ue; ++u) {
+      for (int u = 0; u < units; ++u) {
         const int ch = u / p.nboxes, b = u - ch * p.nboxes;
-        if (p.box_first[b] || u == ub) {  // a plane's halo tile: at its first box, or where this segment enters the plane
+        if (p.box_first[b]) {  // a plane's halo tile: at its first box
           if (a_pre) {
             a_pre = false;
           } else {
@@ -310,8 +230,6 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
               mbar_arrive_expect_tx(&a_full[as], halo_rows * 128);
               tma_load_2d(smem_a + as * p.a_stage_bytes, &tmIn, &a_full[as], ch * 64,
                           p.box_plane[b] * p.plane_positions + q0 - (p.W + 2));
-              DSK_TRACE(0, tcount);
-              ++tcount;
             }
             __syncwarp();
           }
@@ -340,9 +258,9 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
       first = false;
     }
   } else if (warp >= 4) {
-    // ===================== consumers: MMA of a segment, then its epilogue ======================================
+    // ===================== consumers: MMA of a tile, then its epilogue ======================================
     // Warpgroup cg computes the 64-row slices cg*kMW .. cg*kMW + kMW - 1 of every tile (thread rows: frag_row() + 8*h
-    // of each slice).  A cut tile's later parts (stream-K) dump their accumulators for the CTA holding the tile's head.
+    // of each slice).
     const int cg = (warp >> 2) - 1;
     const int etid = threadIdx.x - 128;
     const bool wg_leader = (threadIdx.x & 127) == 0;
@@ -356,9 +274,6 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
     uint32_t aph = 0, bph = 0;
     bool first = true;
     int buf = 0;
-    int ecount = 0;
-    int cur = seg_begin();
-    int tile, ub, ue;
     // stages read by the last committed weight box: handed back to the producer once a later wait shows it complete
     int pend_b = -1, pend_a = -1;
     auto release_pending = [&]() {
@@ -384,12 +299,12 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
       }
       wgmma_commit();
     };
-    while (next_seg(cur, tile, ub, ue)) {
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int c0, q0;
       decode(tile, c0, q0);
-      // ---------------- MMA over units [ub, ue) of this tile ----------------
+      // ---------------- MMA over the units of this tile ----------------
       {
-        constexpr bool kResident = N_TILE == 64 && KIND == 1 && !S::kSmall;  // the only shape whose 9 taps fit the ring
+        constexpr bool kResident = N_TILE == 64 && KIND == 1;  // the only shape whose 9 taps fit the ring
         bool resident = false;
         if constexpr (kResident) resident = p.b_resident != 0;
         if (resident) {
@@ -420,24 +335,24 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
             aph ^= 1;
           }
         } else {
-          using Plan = HaloPlan<KIND, S::kTapsPerBox>;
-          // unit u = box b of chunk ch
-          for (int ch = ub / Plan::kBoxes; ch * Plan::kBoxes < ue; ++ch) {
+          using Plan = HaloPlan<KIND>;
+          // unit u = box b of chunk ch.  The host's table has Plan::kBoxes boxes per chunk, so u < units holds for every
+          // box; the per-box bound stays because without it ptxas gives the 64-channel forms some 20 more registers.
+          for (int ch = 0; ch * Plan::kBoxes < units; ++ch) {
             uint64_t da0 = 0;
 #pragma unroll
             for (int b = 0; b < Plan::kBoxes; ++b) {
-              const int u = ch * Plan::kBoxes + b;
-              if (u < ub || u >= ue) continue;
-              if (Plan::first(b) || u == ub) {
+              if (ch * Plan::kBoxes + b >= units) continue;
+              if (Plan::first(b)) {
                 mbar_wait(&a_full[as], aph);
                 da0 = gmma_desc_sw128(smem_u32(smem_a + as * p.a_stage_bytes));
               }
               mbar_wait(&b_full[bs], bph);
-              const bool rel_a = Plan::last(b) || u == ue - 1;
+              const bool rel_a = Plan::last(b);
               int16_t shifts[3];
 #pragma unroll
               for (int t = 0; t < Plan::ntaps(b); ++t) shifts[t] = static_cast<int16_t>(Plan::row_i(b, t) * pitch + Plan::col_j(b, t));
-              mma_box(da0, gmma_desc_sw128(smem_u32(smem_b + bs * S::kBStageBytes)), Plan::ntaps(b), shifts, u == ub);
+              mma_box(da0, gmma_desc_sw128(smem_u32(smem_b + bs * S::kBStageBytes)), Plan::ntaps(b), shifts, ch == 0 && b == 0);
               wgmma_wait<1>();  // the previous box's MMAs are done: its stages go back to the producer
               release_pending();
               pend_b = bs;
@@ -460,52 +375,6 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
         first = false;
 #pragma unroll
         for (int m = 0; m < kMW; ++m) wgmma_fence_acc(acc[m]);
-      }
-      // partial accumulators of stream-K: [cta][register][consumer thread] (what one thread writes, the same thread
-      // of the owner CTA reads back)
-      auto sk_slot = [&](int cta, int m, int i) -> float* {
-        return p.sk_partial + (static_cast<size_t>(cta) * (kMW * N_TILE / 2) + m * (N_TILE / 2) + i) * kEpiThreads + etid;
-      };
-      if (SK && ub > 0) {
-        // ---- stream-K: a later part of a tile.  Dump the raw fp32 accumulator for the tile's owner and raise this CTA's flag.
-#pragma unroll
-        for (int m = 0; m < kMW; ++m)
-#pragma unroll
-          for (int i = 0; i < N_TILE / 2; ++i) __stcg(sk_slot(blockIdx.x, m, i), acc[m][i]);
-        __threadfence();
-        named_bar_sync(3, kEpiThreads);  // every consumer thread's partial is written and fenced
-        if (etid == 0) st_release_gpu(p.sk_flags + blockIdx.x, 1);
-        continue;
-      }
-      // stream-K: the head of a cut tile owns its epilogue; the parts live in the next CTAs' ranges (each CTA's range
-      // starts with at most one such part, so CTA blockIdx.x + c holds part c)
-      int n_parts = 0;
-      if (SK && ue < units) {
-        const int tile_end = (tile + 1) * units;
-        while (static_cast<int>(blockIdx.x) + 1 + n_parts < static_cast<int>(gridDim.x) &&
-               sk_lo(static_cast<int>(blockIdx.x) + 1 + n_parts) < tile_end)
-          ++n_parts;
-      }
-      if (etid == 0) DSK_TRACE(2, ecount * 8 + 0);
-      if (p.late_trigger && (sk ? cur >= u_hi : cur >= num_tiles)) pdl_launch_dependents();
-      if (SK && n_parts > 0) {
-        if (etid == 0) {
-          const long long t_wait = clock64();
-          for (int c = 1; c <= n_parts; ++c)
-            while (ld_acquire_gpu(p.sk_flags + blockIdx.x + c) == 0) {
-              // a part that never arrives is a scheduling bug: fail the launch instead of hanging the device (~2 s)
-              if (clock64() - t_wait > (1ll << 32)) __trap();
-            }
-        }
-        named_bar_sync(3, kEpiThreads);
-        for (int c = 1; c <= n_parts; ++c)  // fixed order: own head part + part 1 + part 2 ...
-#pragma unroll
-          for (int m = 0; m < kMW; ++m)
-#pragma unroll
-            for (int i = 0; i < N_TILE / 2; ++i) acc[m][i] += __ldcg(sk_slot(blockIdx.x + c, m, i));
-        named_bar_sync(3, kEpiThreads);  // every thread has read the partials: the flags can go back to zero
-        if (etid == 0)
-          for (int c = 1; c <= n_parts; ++c) p.sk_flags[blockIdx.x + c] = 0;
       }
       // ---------------- epilogue ----------------
       // this thread's rows: slice m, half h -> tile row (cg*kMW + m)*64 + fr + 8h; padded position q0 + row
@@ -607,8 +476,6 @@ conv3x3_halo_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_const
           if (p.stg_bufs == 2) buf ^= 1;
         }
       }
-      if (etid == 0) DSK_TRACE(2, ecount * 8 + 7);
-      ++ecount;
     }
     if (etid == 0) tma_store_wait_all<0>();
   }

@@ -66,15 +66,7 @@ int fail(int code, const char* fmt, ...) {
 
 // Launch with the programmatic-stream-serialization attribute (PDL). Only for kernels that call pdl_wait().
 template <typename... KArgs, typename... Args>
-cudaError_t launch_opt(bool pdl, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args);
-
-template <typename... KArgs, typename... Args>
 cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
-  return launch_opt(true, kern, grid, block, smem, s, static_cast<Args&&>(args)...);
-}
-
-template <typename... KArgs, typename... Args>
-cudaError_t launch_opt(bool pdl, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
@@ -84,7 +76,7 @@ cudaError_t launch_opt(bool pdl, void (*kern)(KArgs...), dim3 grid, dim3 block, 
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl ? 1 : 0;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 
@@ -164,10 +156,10 @@ struct WgradLaunch {
 };
 
 struct HaloLaunch {
-  CUtensorMap tmIn, tmW, tmOut, tmRes;
+  CUtensorMap tmIn, tmW, tmOut;
   dsk::HaloParams p;
   int n_tile = 0;
-  int ew = 8;   // consumer warps: 8 = one CTA per SM, 4 = the two-CTAs-per-SM shape (conv3x3_halo.cuh)
+  int ksize = 3;  // 3: the 3x3 tap plan (HaloPlan<1>), 5: the parity-planar 5x5 s2 plan (HaloPlan<2>)
   int grid = 0;
   int smem = 0;
 };
@@ -339,8 +331,7 @@ struct dsk_handle_s {
     float* pooled = nullptr;
     float* fc_out = nullptr;
     float* fc_part = nullptr;  // [kFcSplit][B][E] K-slice partial sums of the fc layer
-    std::vector<ConvLaunch> conv;  // index = conv index (0 unused): the 5x5 s2 stage-entry convs
-    std::vector<HaloLaunch> halo;  // index = conv index: the 3x3 s1 block convs (padded layout)
+    std::vector<HaloLaunch> halo;  // index = conv index (0 unused): the 5x5 s2 and 3x3 s1 convs (padded layout)
     // The 15 launches of a forward as one CUDA graph (captured from the second call of a shape on; programmatic
     // dependent-launch edges included): one cudaGraphLaunch per forward instead of 15 kernel launches.  Only the input
     // and output pointers differ between calls: they are patched into the first / last kernel node.
@@ -356,7 +347,7 @@ struct dsk_handle_s {
     Plan(Plan&& o) noexcept { *this = std::move(o); }
     Plan& operator=(Plan&& o) noexcept {
       B = o.B; T = o.T; act = std::move(o.act); pooled = o.pooled; fc_out = o.fc_out; fc_part = o.fc_part;
-      conv = std::move(o.conv); halo = std::move(o.halo); warm = o.warm; graph_failed = o.graph_failed;
+      halo = std::move(o.halo); warm = o.warm; graph_failed = o.graph_failed;
       graph = o.graph; gexec = o.gexec; node_first = o.node_first; node_last = o.node_last; g_x = o.g_x; g_emb = o.g_emb;
       o.graph = nullptr; o.gexec = nullptr;
       return *this;
@@ -382,17 +373,7 @@ struct dsk_handle_s {
   Ge2ePlan ge2e;               // cached GE2E plan (its own slot: a step may sum the GE2E and AAM losses)
   ScorePlan score;             // cached cosine-scoring plan (its own slot: evaluation runs between training steps)
   ScorePlan search;            // cached gallery-search plan (its own slot: searches alternate with cohort statistics)
-  bool n256 = false;           // DSK_N256=1: 256-channel tiles for layers with >= n256_min_tiles such tiles
-  int n256_min_tiles = 80;
   bool use_graph = true;       // DSK_GRAPH=0: always launch the forward kernel by kernel
-  bool conv1_pdl = true;       // debug knob DSK_CONV1_PDL=0: launch conv1 with plain stream serialisation
-  bool late_trigger = false;   // debug knob DSK_LATE_TRIGGER=1: halo kernels release their dependents at the last tile
-  bool stream_k = false;       // DSK_STREAM_K=1: equal K ranges per CTA (conv3x3_halo.cuh) instead of whole tiles
-  float* sk_partial = nullptr; // stream-K partial accumulators [num_sms][128][256] fp32 and flags, one set per handle
-  int* sk_flags = nullptr;
-  bool small_cta = false;      // DSK_SMALL_CTA=1: 128-channel-tile halo convs as two 256-thread CTAs per SM (64-position tiles)
-  bool planar_s2 = true;       // eval forward: run the 5x5 s2 convs in the halo kernel's parity-planar form (DSK_PLANAR_S2=0: generic kernel)
-  long long* trace = nullptr;  // debug: device buffer [3][512] for conv3x3_halo_kernel clock stamps
   bool bwd_capture_on = false; // debug: dsk_debug_set_backward_capture
   dsk_backward_capture bwd_capture = {};
   // optional per-launch timing (dsk_set_profiling): events recorded around every kernel of a forward
@@ -731,34 +712,6 @@ long padded_positions(int N, int H, int W) {
   return rows * (W + 1);
 }
 size_t padded_bytes(int N, int H, int W, int C) { return static_cast<size_t>(padded_positions(N, H, W)) * C * 2; }
-const uint8_t* padded_origin(const void* base, int W, int C) {  // address of pixel (n=0, h=0, w=0)
-  return static_cast<const uint8_t*>(base) + (static_cast<size_t>(W + 1) + 1) * C * 2;
-}
-View5 padded_nhwc_view(const void* base, int N, int H, int W, int C) {
-  View5 v;
-  v.ptr = padded_origin(base, W, C);
-  v.dims[0] = C; v.dims[1] = W; v.dims[2] = 1; v.dims[3] = H; v.dims[4] = N;
-  v.str[0] = 2ull * C; v.str[1] = 2ull * (W + 1) * C; v.str[2] = 2ull * (W + 1) * C; v.str[3] = 2ull * (H + 1) * (W + 1) * C;
-  return v;
-}
-View5 padded_parity_view(const void* base, int N, int H, int W, int C) {
-  View5 v;
-  v.ptr = padded_origin(base, W, C);
-  v.dims[0] = 2ull * C; v.dims[1] = W / 2; v.dims[2] = 2; v.dims[3] = H / 2; v.dims[4] = N;
-  v.str[0] = 4ull * C; v.str[1] = 2ull * (W + 1) * C; v.str[2] = 4ull * (W + 1) * C; v.str[3] = 2ull * (H + 1) * (W + 1) * C;
-  return v;
-}
-
-// 5x5 s2 p2 conv reading and writing the padded layout (generic tap kernel, rectangular pixel tiles).
-int build_conv_s2_padded(const dsk_handle_s* h, ConvLaunch* L, const void* in, const void* wpk, const float* scale,
-                         const float* bias, void* out, int B, int Hin, int Win, int cin, int cout) {
-  TapTable tt;
-  for (int r = 0; r < 5; ++r)
-    for (int s = 0; s < 5; ++s) tt.add((s & 1) * cin, r * 5 + s, (s - 2) >> 1, r & 1, (r - 2) >> 1);
-  return build_conv_core(h, L, padded_parity_view(in, B, Hin, Win, cin), wpk, cin, cout, 25,
-                         padded_nhwc_view(out, B, Hin / 2, Win / 2, cout), nullptr, B, Hin / 2, Win / 2, tt, dsk::CONV_CLIP,
-                         20.0f, scale, bias, 0, 0);
-}
 
 // The GEMMs of the cached plans: O (rows_pad x n_total fp32) = A (rows_pad x K) B^T (n_total x K), both 16-bit row-major
 // images (f16: fp16 operands whatever the handle's type).  Rows of A are the "pixels" (W = 128, H = rows_pad / 128), rows
@@ -831,17 +784,12 @@ int build_halo(const dsk_handle_s* h, HaloLaunch* L, const void* in, const void*
   p.W = W; p.H = H; p.N = N;
   p.q_begin = W + 1;
   const long q_end = static_cast<long>(N) * (H + 1) * (W + 1);   // one past the last real pixel position
-  // 256-channel tiles halve the weight-operand shared-memory traffic per FLOP (the binding resource, DESIGN.md §6)
-  // but halve the tile count: used when the layer still has enough tiles to spread over the SMs
-  const int tiles_m_ = static_cast<int>((q_end - p.q_begin + 127) / 128);
-  const int n_tile = cout == 64 ? 64 : (h->n256 && cout % 256 == 0 && tiles_m_ * (cout / 256) >= h->n256_min_tiles) ? 256 : 128;
-  // 128-channel tiles optionally run as two 256-thread CTAs per SM, each with one consumer warpgroup and 64-position tiles
-  const bool small = h->small_cta && n_tile == 128;
-  const int tm = small ? 64 : 128;  // positions per tile (HaloSmem::kTileRows)
+  const int n_tile = cout == 64 ? 64 : 128;
+  const int tm = dsk::HaloSmem<128>::kTileRows;  // positions per tile
   p.tiles_m = static_cast<int>((q_end - p.q_begin + tm - 1) / tm);
-  const int tpb = (n_tile == 256 || small) ? 1 : 3;
+  const int tpb = 3;  // taps per weight box
   L->n_tile = n_tile;
-  L->ew = small ? 4 : 8;
+  L->ksize = ksize;
   p.tiles_c = cout / n_tile;
   p.chunks = cin / 64;
   p.cout = cout;
@@ -851,8 +799,6 @@ int build_halo(const dsk_handle_s* h, HaloLaunch* L, const void* in, const void*
     p.scale_c[i] = scale_host ? scale_host[i] : 1.0f;
     p.bias_c[i] = bias_host ? bias_host[i] : 0.0f;
   }
-  p.trace = h->trace;
-  p.late_trigger = h->late_trigger ? 1 : 0;
   p.pitch_magic = static_cast<unsigned long long>((static_cast<unsigned __int128>(1) << 64) / static_cast<unsigned>(W + 1)) + 1ull;
   p.img_magic = static_cast<unsigned long long>((static_cast<unsigned __int128>(1) << 64) / static_cast<unsigned>(H + 1)) + 1ull;
   const long npos = padded_positions(N, H, W);
@@ -867,19 +813,11 @@ int build_halo(const dsk_handle_s* h, HaloLaunch* L, const void* in, const void*
     for (int b = 0; b < p.nboxes; ++b) {
       p.box_plane[b] = 0;
       p.box_first[b] = b == 0;
-      p.box_last[b] = b == p.nboxes - 1;
-      p.box_ntaps[b] = (int8_t)tpb;
       p.box_wtap[b] = (int16_t)(tpb * b);
-      for (int t = 0; t < tpb; ++t) {
-        const int tap = tpb * b + t;
-        p.tap_shift[b][t] = (int16_t)((tap / 3) * (W + 1) + tap % 3);
-      }
     }
   } else {
     ntaps_total = 25;
     p.plane_positions = static_cast<int>(npos);
-    int perm[25];
-    planar_tap_order(perm);
     int slot = 0, nb = 0;
     for (int pl = 0; pl < 4; ++pl) {
       const int ph = pl >> 1, pw = pl & 1;
@@ -887,21 +825,13 @@ int build_halo(const dsk_handle_s* h, HaloLaunch* L, const void* in, const void*
       for (int t0 = 0; t0 < cnt; t0 += tpb, ++nb) {
         p.box_plane[nb] = (int8_t)pl;
         p.box_first[nb] = t0 == 0;
-        p.box_last[nb] = t0 + tpb >= cnt;
-        p.box_ntaps[nb] = (int8_t)(cnt - t0 < tpb ? cnt - t0 : tpb);
         p.box_wtap[nb] = (int16_t)(slot + t0);
-        for (int t = 0; t < p.box_ntaps[nb]; ++t) {
-          const int rs = perm[slot + t0 + t];
-          const int dh = ((rs / 5) - 2) >> 1, dw = ((rs % 5) - 2) >> 1;
-          p.tap_shift[nb][t] = (int16_t)((dh + 1) * (W + 1) + dw + 1);
-        }
       }
       slot += cnt;
     }
-    p.nboxes = nb;  // 3 + 2 + 2 + 2 = 9 three-tap boxes, or 25 single taps
+    p.nboxes = nb;  // 3 + 2 + 2 + 2 = 9 three-tap boxes
   }
   // all weight boxes of a CTA fit the B ring and every tile of the CTA uses the same ones: load them once
-  p.plain3x3 = ksize == 3 ? 1 : 2;
   p.b_resident = (p.chunks == 1 && p.tiles_c == 1 && p.nboxes <= 3 && n_tile == 64) ? 1 : 0;
   p.res_ptr = (flags & dsk::CONV_RESIDUAL) ? static_cast<const uint16_t*>(res) : nullptr;
   p.out_planar = out_planar;
@@ -910,70 +840,25 @@ int build_halo(const dsk_handle_s* h, HaloLaunch* L, const void* in, const void*
     p.out_plane_positions = static_cast<int>(padded_positions(N, H / 2, W / 2));
     p.out_C = cout;
   }
-  // shared-memory carve: weight boxes are the latency-critical stream (48 KB each at N_TILE = 128), so they get the
-  // deepest ring that fits in 227 KB; output staging / residual prefetch shrink to one buffer each when needed
+  // shared-memory carve: two output staging tiles; the residual is read from global memory (HaloParams::res_ptr), so
+  // everything else goes to the operand rings - weight boxes, the latency-critical stream, first (48 KB each at
+  // N_TILE = 128): the deepest ring that fits in 227 KB
   {
     const int halo_rows = tm + 2 * W + 4;
     p.a_stage_bytes = (halo_rows * 128 + 1023) / 1024 * 1024;
     const int b_bytes = tpb * n_tile * 128;
     const int fixed = dsk::HaloSmem<128>::kFixedBytes;  // the same for every tile width
-    if (small) {
-      // two CTAs per SM: (232448 B of shared memory per SM) / 2 minus the 1 KB the driver reserves per CTA
-      const int limit = 232448 / 2 - 1024;
-      p.a_stages = 2;
-      p.stg_bufs = 1;
-      p.res_bufs = 0;   // the residual is read from global memory (HaloParams::res_ptr)
-      int nb = (limit - fixed - p.a_stages * p.a_stage_bytes - p.stg_bufs * 16384) / b_bytes;
-      if (nb > dsk::kHaloMaxStages) nb = dsk::kHaloMaxStages;
-      if (nb < 2) return fail(DSK_ERR_INVALID, "halo conv (two CTAs per SM): shared memory does not fit");
-      p.b_stages = nb;
-      L->smem = p.a_stages * p.a_stage_bytes + p.b_stages * b_bytes + p.stg_bufs * 16384 + fixed;
-    } else {
-      // one CTA per SM: two output staging tiles; the residual is read from global memory (HaloParams::res_ptr), so
-    // everything else goes to the operand rings - weight boxes first (48 KB each at N_TILE = 128)
-      const int limit = 227 * 1024;
-      p.a_stages = n_tile == 64 ? 3 : 2;
-      p.stg_bufs = 2;
-      p.res_bufs = 0;
-      int nb = (limit - fixed - p.a_stages * p.a_stage_bytes - p.stg_bufs * 16384) / b_bytes;
-      p.b_stages = nb > dsk::kHaloMaxStages ? dsk::kHaloMaxStages : nb;
-      if (p.b_resident) p.b_stages = 3;
-      if (p.b_stages < 2) return fail(DSK_ERR_INVALID, "halo conv: shared memory does not fit");
-      L->smem = p.a_stages * p.a_stage_bytes + p.b_stages * b_bytes + p.stg_bufs * 16384 + fixed;
-    }
+    const int limit = 227 * 1024;
+    p.a_stages = n_tile == 64 ? 3 : 2;
+    p.stg_bufs = 2;
+    int nb = (limit - fixed - p.a_stages * p.a_stage_bytes - p.stg_bufs * 16384) / b_bytes;
+    p.b_stages = nb > dsk::kHaloMaxStages ? dsk::kHaloMaxStages : nb;
+    if (p.b_resident) p.b_stages = 3;
+    if (p.b_stages < 2) return fail(DSK_ERR_INVALID, "halo conv: shared memory does not fit");
+    L->smem = p.a_stages * p.a_stage_bytes + p.b_stages * b_bytes + p.stg_bufs * 16384 + fixed;
   }
   const int num_tiles = p.tiles_m * p.tiles_c;
-  const int slots = h->num_sms * (small ? 2 : 1);
-  L->grid = num_tiles < slots ? num_tiles : slots;
-  // stream-K: equal unit ranges per CTA instead of whole tiles when that shortens the longest CTA by > 5 %
-  p.stream_k = 0;
-  if (h->stream_k && !small && !p.b_resident && p.plain3x3 && n_tile != 64) {
-    const long units = static_cast<long>(p.chunks) * p.nboxes;
-    const long total = units * num_tiles;
-    long g = total / 6;  // at least 6 weight boxes per CTA
-    if (g > h->num_sms) g = h->num_sms;
-    if (g < 1) g = 1;
-    const long span_tiles = (num_tiles + L->grid - 1) / L->grid * units;
-    const long span_sk = (total + g - 1) / g;
-    if (span_sk * 105 < span_tiles * 100 && total < (1l << 28)) {
-      if (!h->sk_partial) {
-        dsk_handle_s* hh = const_cast<dsk_handle_s*>(h);
-        const size_t nb = static_cast<size_t>(h->num_sms) * 128 * 256 * sizeof(float);
-        if (cudaMalloc(reinterpret_cast<void**>(&hh->sk_partial), nb) != cudaSuccess ||
-            cudaMalloc(reinterpret_cast<void**>(&hh->sk_flags), h->num_sms * sizeof(int)) != cudaSuccess ||
-            cudaMemset(hh->sk_flags, 0, h->num_sms * sizeof(int)) != cudaSuccess) {
-          cudaGetLastError();
-          return fail(DSK_ERR_CUDA, "halo conv: stream-K workspace allocation failed");
-        }
-      }
-      p.stream_k = 1;
-      p.sk_q = static_cast<int>(total / g);
-      p.sk_r = static_cast<int>(total % g);
-      p.sk_partial = h->sk_partial;
-      p.sk_flags = h->sk_flags;
-      L->grid = static_cast<int>(g);
-    }
-  }
+  L->grid = num_tiles < h->num_sms ? num_tiles : h->num_sms;
   const uint64_t in_pos = static_cast<uint64_t>(npos) * (ksize == 5 ? 4 : 1);
   uint64_t idims[2] = {(uint64_t)cin, in_pos};
   uint64_t istr[1] = {2ull * cin};
@@ -985,46 +870,33 @@ int build_halo(const dsk_handle_s* h, HaloLaunch* L, const void* in, const void*
   uint32_t wb[3] = {64, (uint32_t)n_tile, (uint32_t)tpb};
   rc = make_tmap(&L->tmW, bf, wpk, 3, wd, ws, wb);
   if (rc) return rc;
-  // output / residual: standard padded layout of the output geometry (with a planar output the map is unused but
-  // must be valid: point it at the residual or the input)
+  // output: standard padded layout of the output geometry (with a planar output the map is unused but must be valid:
+  // point it at the residual or the input)
   uint64_t odims[2] = {(uint64_t)cout, (uint64_t)npos};
   uint64_t ostr[1] = {2ull * cout};
   uint32_t box_out[2] = {64, (uint32_t)tm};
-  const void* res_ptr = (flags & dsk::CONV_RESIDUAL) ? res : (out_planar ? in : out);
-  rc = make_tmap(&L->tmRes, bf, res_ptr, 2, odims, ostr, box_out);
-  if (rc) return rc;
-  return make_tmap(&L->tmOut, bf, out_planar ? res_ptr : out, 2, odims, ostr, box_out);
+  const void* out_map = out_planar ? ((flags & dsk::CONV_RESIDUAL) ? res : in) : out;
+  return make_tmap(&L->tmOut, bf, out_map, 2, odims, ostr, box_out);
 }
 
-template <int N_TILE, bool BF16, int EW, bool SK, int KIND>
+template <int N_TILE, bool BF16, int KIND>
 int launch_halo_t(const HaloLaunch& L, cudaStream_t s) {
-  auto kern = dsk::conv3x3_halo_kernel<N_TILE, BF16, EW, SK, KIND>;
-  if (int rc = ensure_smem_optin(reinterpret_cast<const void*>(kern), EW == 4 ? 232448 / 2 - 1024 : 227 * 1024)) return rc;
-  CUDA_TRY(launch_pdl(kern, dim3(L.grid), dim3(dsk::halo_threads(EW)), L.smem, s, L.tmIn, L.tmW, L.tmOut, L.tmRes, L.p));
+  auto kern = dsk::conv3x3_halo_kernel<N_TILE, BF16, KIND>;
+  if (int rc = ensure_smem_optin(reinterpret_cast<const void*>(kern), 227 * 1024)) return rc;
+  CUDA_TRY(launch_pdl(kern, dim3(L.grid), dim3(dsk::kHaloThreads), L.smem, s, L.tmIn, L.tmW, L.tmOut, L.p));
   return DSK_OK;
 }
 
-// one instantiation per (tile width, operand type, CTA shape, scheduling, tap plan): each carries only the code it runs
-template <int N_TILE, int EW, bool SK>
+// one instantiation per (tile width, operand type, tap plan): each carries only the code it runs
+template <int N_TILE>
 int launch_halo_v(const dsk_handle_s* h, const HaloLaunch& L, cudaStream_t s) {
-  const bool k5 = L.p.plain3x3 == 2;
-  if (h->bf16) return k5 ? launch_halo_t<N_TILE, true, EW, SK, 2>(L, s) : launch_halo_t<N_TILE, true, EW, SK, 1>(L, s);
-  return k5 ? launch_halo_t<N_TILE, false, EW, SK, 2>(L, s) : launch_halo_t<N_TILE, false, EW, SK, 1>(L, s);
+  const bool k5 = L.ksize == 5;
+  if (h->bf16) return k5 ? launch_halo_t<N_TILE, true, 2>(L, s) : launch_halo_t<N_TILE, true, 1>(L, s);
+  return k5 ? launch_halo_t<N_TILE, false, 2>(L, s) : launch_halo_t<N_TILE, false, 1>(L, s);
 }
 
 int launch_halo(const dsk_handle_s* h, const HaloLaunch& L, cudaStream_t s) {
-  if (L.p.plain3x3 != 1 && L.p.plain3x3 != 2) return fail(DSK_ERR_INVALID, "halo conv: unknown tap plan %d", L.p.plain3x3);
-  if (L.ew == 4) {
-    if (L.n_tile != 128 || L.p.stream_k) return fail(DSK_ERR_INVALID, "two-CTAs-per-SM halo conv: 128-channel whole tiles only");
-    return launch_halo_v<128, 4, false>(h, L, s);
-  }
-  if (L.p.stream_k) {
-    if (L.n_tile == 128) return launch_halo_v<128, 8, true>(h, L, s);
-    if (L.n_tile == 256) return launch_halo_v<256, 8, true>(h, L, s);
-    return fail(DSK_ERR_INVALID, "stream-K halo conv: 128- or 256-channel tiles only");
-  }
-  return L.n_tile == 64 ? launch_halo_v<64, 8, false>(h, L, s)
-                        : L.n_tile == 128 ? launch_halo_v<128, 8, false>(h, L, s) : launch_halo_v<256, 8, false>(h, L, s);
+  return L.n_tile == 64 ? launch_halo_v<64>(h, L, s) : launch_halo_v<128>(h, L, s);
 }
 
 int check_handle(dsk_handle h) {
@@ -1063,8 +935,8 @@ int get_plan(dsk_handle h, int B, int T, cudaStream_t s, dsk_handle_s::Plan** ou
     int H, W, C;
     act_shape(i, T, H, W, C);
     off[i] = bytes;
-    // optional: a block output that feeds a stride-2 conv (i = 2, 5, 8) stored parity-planar (4 planes at half res)
-    const bool planar = h->planar_s2 && (i % 3 == 2) && i < DSK_NUM_CONV - 1;
+    // a block output that feeds a stride-2 conv (i = 2, 5, 8) is stored parity-planar (4 planes at half res)
+    const bool planar = (i % 3 == 2) && i < DSK_NUM_CONV - 1;
     const size_t b = planar ? 4 * padded_bytes(B, H / 2, W / 2, C) : padded_bytes(B, H, W, C);
     bytes += ((b + 1023) / 1024) * 1024;
   }
@@ -1101,7 +973,6 @@ int get_plan(dsk_handle h, int B, int T, cudaStream_t s, dsk_handle_s::Plan** ou
   pl.pooled = reinterpret_cast<float*>(base + off_pooled);
   pl.fc_out = reinterpret_cast<float*>(base + off_fc);
   pl.fc_part = reinterpret_cast<float*>(base + off_fc_part);
-  pl.conv.resize(DSK_NUM_CONV);
   pl.halo.resize(DSK_NUM_CONV);
   if (!h->host_affine_valid) {  // once per weight load: host copy of the folded BN affine for the kernel parameters
     for (int i = 1; i < DSK_NUM_CONV; ++i) {
@@ -1112,24 +983,17 @@ int get_plan(dsk_handle h, int B, int T, cudaStream_t s, dsk_handle_s::Plan** ou
   }
   for (int i = 1; i < DSK_NUM_CONV; ++i) {
     const LayerCfg c = layer_cfg(i);
-    int Hi, Wi, Ci;
-    act_shape(i - 1, T, Hi, Wi, Ci);  // input of conv i is activation i-1
     const int k = i % 3;
     int Ho, Wo, Co;
     act_shape(i, T, Ho, Wo, Co);
     int rc;
-    if (k == 0 && h->planar_s2) {
+    if (k == 0) {
       rc = build_halo(h, &pl.halo[i], pl.act[i - 1], h->wpk_planar[i], h->scale_host[i].data(), h->bias_host[i].data(), nullptr, pl.act[i], B, Ho, Wo,
                       c.cin, c.cout, 5, dsk::CONV_CLIP, 20.0f, 0);
-    } else if (k == 0) {
-      // default: the generic tap kernel reads the padded input through its parity view (measured 4 % faster end to end
-      // than the planar form at batch 64: both are bound by operand delivery, and planar stores cost the producer)
-      rc = build_conv_s2_padded(h, &pl.conv[i], pl.act[i - 1], h->wpk[i], h->scale[i], h->bias[i], pl.act[i], B, Hi, Wi,
-                                c.cin, c.cout);
     } else {
       const void* res = (k == 2) ? pl.act[i - 2] : nullptr;  // block output adds the block input
       const int flags = dsk::CONV_CLIP | (k == 2 ? dsk::CONV_RESIDUAL : 0);
-      const int out_planar = (h->planar_s2 && k == 2 && i < DSK_NUM_CONV - 1) ? 1 : 0;
+      const int out_planar = (k == 2 && i < DSK_NUM_CONV - 1) ? 1 : 0;
       rc = build_halo(h, &pl.halo[i], pl.act[i - 1], h->wpk[i], h->scale_host[i].data(), h->bias_host[i].data(), res, pl.act[i], B, Ho, Wo, c.cin,
                       c.cout, 3, flags, 20.0f, out_planar);
     }
@@ -1164,22 +1028,8 @@ int32_t dsk_create(dsk_handle* out, int32_t device, int32_t operand) {
   h->bf16 = operand == DSK_BF16;
   h->num_sms = prop.multiProcessorCount;
   {
-    const char* e = getenv("DSK_PLANAR_S2");  // default on; DSK_PLANAR_S2=0 runs the 5x5 s2 convs in the generic tap kernel
-    h->planar_s2 = !(e && e[0] == '0');
-    e = getenv("DSK_SMALL_CTA");
-    if (e) h->small_cta = atoi(e) != 0;
-    e = getenv("DSK_STREAM_K");
-    if (e) h->stream_k = atoi(e) != 0;
-    e = getenv("DSK_N256");
-    h->n256 = e && e[0] == '1';
-    e = getenv("DSK_N256_MIN_TILES");
-    if (e) h->n256_min_tiles = atoi(e);
-    e = getenv("DSK_GRAPH");
+    const char* e = getenv("DSK_GRAPH");
     h->use_graph = !(e && e[0] == '0');
-    e = getenv("DSK_CONV1_PDL");
-    h->conv1_pdl = !(e && e[0] == '0');
-    e = getenv("DSK_LATE_TRIGGER");
-    h->late_trigger = e && e[0] == '1';
   }
   {
     std::vector<float> one(512, 1.0f);
@@ -1212,8 +1062,6 @@ int32_t dsk_destroy(dsk_handle h) {
     cudaFree(h->fc_wq);
   }
   cudaFree(h->ws);
-  cudaFree(h->sk_partial);
-  cudaFree(h->sk_flags);
   h->allpairs.release();
   h->aam.release();
   h->ge2e.release();
@@ -1433,17 +1281,17 @@ int enqueue_forward(dsk_handle h, dsk_handle_s::Plan* pl, const float* x, int B,
     if (rc) return rc;
     if (h->bf16) {
       if (int rc2 = ensure_smem_optin(reinterpret_cast<const void*>(dsk::conv1_umma_kernel<true>), dsk::kConv1SmemBytes)) return rc2;
-      CUDA_TRY(launch_opt(h->conv1_pdl, dsk::conv1_umma_kernel<true>, dim3(grid), dim3(dsk::kConv1Threads), dsk::kConv1SmemBytes, s, tmX,
+      CUDA_TRY(launch_pdl(dsk::conv1_umma_kernel<true>, dim3(grid), dim3(dsk::kConv1Threads), dsk::kConv1SmemBytes, s, tmX,
                           (const uint4*)h->conv1_img, (const float*)h->scale[0], (const float*)h->bias[0], (uint16_t*)pl->act[0], T, n_tiles, 20.0f));
     } else {
       if (int rc2 = ensure_smem_optin(reinterpret_cast<const void*>(dsk::conv1_umma_kernel<false>), dsk::kConv1SmemBytes)) return rc2;
-      CUDA_TRY(launch_opt(h->conv1_pdl, dsk::conv1_umma_kernel<false>, dim3(grid), dim3(dsk::kConv1Threads), dsk::kConv1SmemBytes, s, tmX,
+      CUDA_TRY(launch_pdl(dsk::conv1_umma_kernel<false>, dim3(grid), dim3(dsk::kConv1Threads), dsk::kConv1SmemBytes, s, tmX,
                           (const uint4*)h->conv1_img, (const float*)h->scale[0], (const float*)h->bias[0], (uint16_t*)pl->act[0], T, n_tiles, 20.0f));
     }
     mark(true);
   }
   for (int i = 1; i < DSK_NUM_CONV; ++i) {
-    rc = (i % 3 == 0 && !h->planar_s2) ? launch_conv(pl->conv[i], s) : launch_halo(h, pl->halo[i], s);
+    rc = launch_halo(h, pl->halo[i], s);
     if (rc) return rc;
     mark(i == DSK_NUM_CONV - 1);
   }
@@ -1590,7 +1438,7 @@ int32_t dsk_rescnn_forward(dsk_handle h, const float* x, int32_t B, int32_t T, f
   dsk_handle_s::Plan* pl;
   rc = get_plan(h, B, T, s, &pl);
   if (rc) return rc;
-  if (h->use_graph && !h->profiling && !h->trace && pl->warm) {
+  if (h->use_graph && !h->profiling && pl->warm) {
     cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
     if (cudaStreamIsCapturing(s, &cs) != cudaSuccess) cudaGetLastError();
     if (cs == cudaStreamCaptureStatusNone) {  // inside a caller's capture the plain launches are what gets recorded
@@ -2113,7 +1961,7 @@ int32_t dsk_debug_read_eval_activation(dsk_handle h, int32_t layer, void* dst, i
   int H, W, C;
   act_shape(layer, pl.T, H, W, C);
   // the layout get_plan chose for this buffer
-  const bool planar = h->planar_s2 && (layer % 3 == 2) && layer < DSK_NUM_CONV - 1;
+  const bool planar = (layer % 3 == 2) && layer < DSK_NUM_CONV - 1;
   const size_t bytes = planar ? 4 * padded_bytes(pl.B, H / 2, W / 2, C) : padded_bytes(pl.B, H, W, C);
   if (dst_bytes < 0 || static_cast<size_t>(dst_bytes) != bytes)
     return fail(DSK_ERR_INVALID, "dsk_debug_read_eval_activation: layer %d holds %zu bytes, dst_bytes is %lld", layer, bytes,
@@ -2458,12 +2306,6 @@ int32_t dsk_conv5x5s2_planar(dsk_handle h, const void* in_planar, const float* w
 }
 
 int64_t dsk_padded_positions(int32_t N, int32_t H, int32_t W) { return padded_positions(N, H, W); }
-
-int32_t dsk_debug_set_trace(dsk_handle h, void* device_buffer) {
-  if (!h) return fail(DSK_ERR_INVALID, "null handle");
-  h->trace = static_cast<long long*>(device_buffer);
-  return DSK_OK;
-}
 
 int32_t dsk_conv2d_nhwc(dsk_handle h, const void* in, const void* w_packed, const float* scale, const float* bias,
                         const void* res, void* out, int32_t B, int32_t Hin, int32_t Win, int32_t cin, int32_t cout,

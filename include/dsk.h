@@ -96,10 +96,9 @@ int32_t dsk_share_weights(dsk_handle h, dsk_handle src);
  * (train_triplet.py:332,347): x (B,1,T,64) fp32 contiguous -> emb (B,E) fp32 with ||emb||=10.
  * T must be a multiple of 16.
  * An utterance's embedding, and every activation of it, has the same bits whatever else is in the batch (its size,
- * order and content) under the default whole-tile scheduling; DSK_STREAM_K=1 cuts each tile's K loop where the tile
- * count puts it, which can move the last bits.  Nothing else bounds B and T: the workspace grows with B * T (130 MiB at
- * 64 x 160), and the halo convs' 32-bit position arithmetic is exact for every shape whose workspace fits in 80 GiB (a
- * layer past 2^31 padded positions fails with DSK_ERR_INVALID).
+ * order and content).  Nothing else bounds B and T: the workspace grows with B * T (130 MiB at 64 x 160), and the
+ * halo convs' 32-bit position arithmetic is exact for every shape whose workspace fits in 80 GiB (a layer past 2^31
+ * padded positions fails with DSK_ERR_INVALID).
  * Non-finite input: a NaN or +-inf element of x makes that utterance's embedding all NaN (every activation is NaN
  * exactly where a conv window reaches it, in every channel; the clamps keep NaN, as Hardtanh does) and leaves every
  * other utterance's bits unchanged; pads stay +0.  conv1 splits x into 16-bit halves x_hi + x_lo, so the finite input
@@ -242,9 +241,6 @@ int32_t dsk_conv5x5s2_planar(dsk_handle h, const void* in_planar, const float* w
                              const float* bias, void* out, int32_t N, int32_t Hout, int32_t Wout, int32_t cin,
                              int32_t cout, int32_t flags, float clip_hi, void* stream);
 int64_t dsk_padded_positions(int32_t N, int32_t H, int32_t W);
-/* Debug: device buffer of 3*512 int64 that dsk_conv3x3_padded fills with clock64 stamps of CTA 0
- * (producer / MMA / epilogue roles); NULL switches tracing off. */
-int32_t dsk_debug_set_trace(dsk_handle h, void* device_buffer);
 /* Debug / test: copies of the intermediate tensors of a train backward, which otherwise live in buffers that the next
  * layer overwrites.  Every non-NULL entry receives, by cudaMemcpyAsync on the backward's stream at the point where the
  * tensor is final, B*H*W*C contiguous values (B, T, C, H, W of the context; layer i as act_shape: C = 64 << i/3,

@@ -402,7 +402,7 @@ def test_eval_chain_at_embedding_size_128(cuda_dev):
     m.eval()
     with torch.no_grad():
         emb = m(x)
-        bufs = read_eval_activations(m, B, T, "fp16", True)
+        bufs = read_eval_activations(m, B, T, "fp16")
     torch.cuda.synchronize()
     check_eval_chain(f"eval fp16 E=128 B={B} T={T}", sd, "fp16", x, unpack_eval_activations(m._engine.lib, bufs, B, T), emb)
 

@@ -11,27 +11,13 @@ from deepspeaker_pytorch_b200 import _lib as L
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope="module", params=["one_cta_per_sm", "two_ctas_per_sm", "stream_k"])
-def hl(cuda_dev, request):
-    """The production shape of the halo kernel (384 threads, one CTA per SM, whole tiles) and its two opt-in variants
-    (csrc/conv3x3_halo.cuh): 256-thread CTAs sharing an SM, and stream-K scheduling; the handle reads the knobs when it
-    is created."""
-    import os
-
+@pytest.fixture(scope="module", params=["one_cta_per_sm"])
+def hl(cuda_dev):
+    """A handle for the halo kernel's one shape (384 threads, one CTA per SM, whole tiles; csrc/conv3x3_halo.cuh).
+    The parameter names that shape in the test ids."""
     lib = L.load()
     h = ctypes.c_void_p()
-    knobs = {"DSK_SMALL_CTA": "1" if request.param == "two_ctas_per_sm" else "0",
-             "DSK_STREAM_K": "1" if request.param == "stream_k" else "0"}
-    old = {k: os.environ.get(k) for k in knobs}
-    os.environ.update(knobs)
-    try:
-        L.check(lib.dsk_create(ctypes.byref(h), 0, L.DSK_F16), "dsk_create")
-    finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
+    L.check(lib.dsk_create(ctypes.byref(h), 0, L.DSK_F16), "dsk_create")
     yield lib, h
     lib.dsk_destroy(h)
 

@@ -187,13 +187,13 @@ def calibrated(sd, x):
     return out
 
 
-def read_eval_activations(m, B, T, dt, planar_s2):
+def read_eval_activations(m, B, T, dt):
     """The 12 activation buffers of the handle's last eval forward, byte for byte (dsk_debug_read_eval_activation)."""
     eng = m._engine
     out = []
     for i in range(12):
         C, H, W = act_geometry(i, T)
-        planar = planar_s2 and i % 3 == 2 and i < 11
+        planar = i % 3 == 2 and i < 11
         if planar:
             npl = eng.lib.dsk_padded_positions(B, H // 2, W // 2)
             buf = torch.empty(4, npl // (W // 2 + 1), W // 2 + 1, C, dtype=TD[dt], device="cuda")
@@ -255,7 +255,6 @@ def eval_case(dt, B, T, env, seed=300, shape_switch=False):
     xs = [O.make_input(B, T, seed + j, 4.0).cuda() for j in range(3)]
     sd = calibrated(sd0, xs[2])
     m = _fresh_model(sd, env, dt)
-    planar_s2 = env.get("DSK_PLANAR_S2", "1") != "0"
     side, cur = torch.cuda.Stream(), torch.cuda.current_stream()
     side.wait_stream(cur)
     # three forwards back to back on one non-legacy stream: plain launches, graph capture, then a graph replay re-pointed
@@ -263,7 +262,7 @@ def eval_case(dt, B, T, env, seed=300, shape_switch=False):
     with torch.no_grad(), torch.cuda.stream(side):
         for x in xs:
             emb = m(x)
-        bufs = read_eval_activations(m, B, T, dt, planar_s2)
+        bufs = read_eval_activations(m, B, T, dt)
     cur.wait_stream(side)
     torch.cuda.synchronize()
     tag = f"eval {dt} B={B} T={T} {' '.join(f'{k}={v}' for k, v in env.items()) or 'default'}"
@@ -272,7 +271,7 @@ def eval_case(dt, B, T, env, seed=300, shape_switch=False):
         with torch.no_grad(), torch.cuda.stream(side):
             m(O.make_input(3, 32, seed + 7, 4.0).cuda())
             emb = m(xs[2])
-            bufs = read_eval_activations(m, B, T, dt, planar_s2)
+            bufs = read_eval_activations(m, B, T, dt)
         cur.wait_stream(side)
         torch.cuda.synchronize()
         for i, (_, pads) in enumerate(unpack_eval_activations(m._engine.lib, bufs, B, T)):
@@ -280,8 +279,6 @@ def eval_case(dt, B, T, env, seed=300, shape_switch=False):
 
 
 EVAL_CASES = [("fp16", 64, 160), ("fp16", 64, 32), ("fp16", 1, 16), ("fp16", 33, 48), ("bf16", 64, 160)]
-KNOBS = [{"DSK_STREAM_K": "1"}, {"DSK_PLANAR_S2": "0"}, {"DSK_SMALL_CTA": "1"}, {"DSK_N256": "1", "DSK_N256_MIN_TILES": "1"},
-         {"DSK_LATE_TRIGGER": "1", "DSK_CONV1_PDL": "0"}, {"DSK_GRAPH": "0"}]
 
 
 @pytest.mark.gpu
@@ -291,9 +288,10 @@ def test_eval_chain_layer_by_layer(cuda_dev, dt, B, T):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("env", KNOBS, ids=lambda e: "+".join(f"{k}={v}" for k, v in e.items()))
-def test_eval_chain_layer_by_layer_knobs(cuda_dev, env):
-    eval_case("fp16", 64, 160, env)
+@pytest.mark.parametrize("dt,B,T", EVAL_CASES + [("bf16", 33, 48)])
+def test_eval_chain_layer_by_layer_kernel_by_kernel(cuda_dev, dt, B, T):
+    """The same checks with the forward launched kernel by kernel (DSK_GRAPH=0) instead of as one CUDA graph."""
+    eval_case(dt, B, T, {"DSK_GRAPH": "0"})
 
 
 # ---- train chain --------------------------------------------------------------------------------------------------

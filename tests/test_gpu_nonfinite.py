@@ -27,7 +27,7 @@ from oracle import rescnn_oracle as O
 from oracle import vad_oracle as V
 from tests.test_fbank import synth
 from tests.test_gpu_forward import _fresh_model
-from tests.test_gpu_layer_parity import KNOBS, calibrated, read_eval_activations, unpack_eval_activations
+from tests.test_gpu_layer_parity import calibrated, read_eval_activations, unpack_eval_activations
 from tests.test_nonfinite_host import check_nan_layer, nan_footprint, nonfinite_indicator
 
 pytestmark = pytest.mark.gpu
@@ -72,12 +72,12 @@ def _poisons(T):
             ("-inf", at(T // 5, 9, -INF)), ("1e5", at(T - 3, 50, 1e5))]
 
 
-def _forward_and_read(m, x, dt, planar_s2):
+def _forward_and_read(m, x, dt):
     side, cur = torch.cuda.Stream(), torch.cuda.current_stream()
     side.wait_stream(cur)
     with torch.no_grad(), torch.cuda.stream(side):
         emb = m(x).clone()
-        bufs = read_eval_activations(m, x.shape[0], x.shape[2], dt, planar_s2)
+        bufs = read_eval_activations(m, x.shape[0], x.shape[2], dt)
     cur.wait_stream(side)
     torch.cuda.synchronize()
     return emb.cpu(), unpack_eval_activations(m._engine.lib, bufs, x.shape[0], x.shape[2])
@@ -86,9 +86,8 @@ def _forward_and_read(m, x, dt, planar_s2):
 def eval_nonfinite_case(dt, B, T, env):
     sd = calibrated(O.make_state_dict(4, 16), O.make_input(B, T, 301, 4.0).cuda())
     m = _fresh_model(sd, env, dt)
-    planar_s2 = env.get("DSK_PLANAR_S2", "1") != "0"
     clean = O.make_input(B, T, 300, 4.0).cuda()
-    emb0, acts0 = _forward_and_read(m, clean, dt, planar_s2)
+    emb0, acts0 = _forward_and_read(m, clean, dt)
     assert torch.isfinite(emb0).all()
     slots = [0, B // 2, B - 1]
     poisons = _poisons(T)
@@ -99,7 +98,7 @@ def eval_nonfinite_case(dt, B, T, env):
             poison(x[slot])
         tag = f"{dt} B={B} T={T} {'+'.join(f'{k}={v}' for k, v in env.items()) or 'default'} " \
               f"{[name for name, _ in group]}"
-        emb, acts = _forward_and_read(m, x, dt, planar_s2)
+        emb, acts = _forward_and_read(m, x, dt)
         masks = nan_footprint(nonfinite_indicator(x.cpu(), fp16=dt == "fp16"))
         poisoned = nonfinite_indicator(x.cpu(), fp16=dt == "fp16").flatten(1).any(1)
         keep = torch.ones(B, dtype=torch.bool)
@@ -114,15 +113,18 @@ def eval_nonfinite_case(dt, B, T, env):
         print(f"[{tag}] poisoned {poisoned.nonzero().flatten().tolist()}: footprints exact, others bit-identical")
 
 
-@pytest.mark.parametrize("dt,B,T", [("fp16", 7, 160), ("fp16", 64, 160), ("bf16", 7, 160), ("bf16", 64, 160),
-                                    ("fp16", 5, 800)])
+NONFINITE_CASES = [("fp16", 7, 160), ("fp16", 64, 160), ("bf16", 7, 160), ("bf16", 64, 160), ("fp16", 5, 800)]
+
+
+@pytest.mark.parametrize("dt,B,T", NONFINITE_CASES)
 def test_eval_nonfinite_footprints(cuda_dev, dt, B, T):
     eval_nonfinite_case(dt, B, T, {})
 
 
-@pytest.mark.parametrize("env", KNOBS, ids=lambda e: "+".join(f"{k}={v}" for k, v in e.items()))
-def test_eval_nonfinite_footprints_knobs(cuda_dev, env):
-    eval_nonfinite_case("fp16", 64, 160, env)
+@pytest.mark.parametrize("dt,B,T", NONFINITE_CASES + [("bf16", 5, 800)])
+def test_eval_nonfinite_footprints_kernel_by_kernel(cuda_dev, dt, B, T):
+    """The same footprints with the forward launched kernel by kernel (DSK_GRAPH=0) instead of as one CUDA graph."""
+    eval_nonfinite_case(dt, B, T, {"DSK_GRAPH": "0"})
 
 
 def test_nan_crop_from_a_bad_cuda_index(cuda_dev):

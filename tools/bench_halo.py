@@ -22,7 +22,7 @@ sys.path.insert(0, ROOT)
 from bench import make_model  # noqa: E402
 from tools.bench_batch_hard import gpu_info  # noqa: E402
 
-TILE = 128  # padded positions per tile (HaloSmem<N, 8>::kTileRows)
+TILE = 128  # padded positions per tile (HaloSmem<N>::kTileRows)
 
 
 def conv_layers(T):
