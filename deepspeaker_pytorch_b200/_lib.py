@@ -27,6 +27,7 @@ DSK_NORM_NONE, DSK_NORM_LENGTH, DSK_NORM_PLDA = 0, 1, 2
 DSK_F64_MAX_DIM = 4096
 DSK_PLDA_MAX_ROWS = 4194240
 DSK_VBX_MAX_SPEAKERS = 128
+DSK_SC_MAX_SPEAKERS, DSK_SC_MAX_P = 32, 64
 DSK_SPEED_MAX_DEN, DSK_SPEED_TAPS, DSK_SPEED_MAX_FACTORS = 32, 50, 8
 DSK_AAM_MAX_C, DSK_AAM_MAX_SUBCENTRES, DSK_AAM_MAX_TOPK = 65536, 16, 64
 
@@ -224,6 +225,8 @@ SIGNATURES = {
     "dsk_class_centroids": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),
     "dsk_ahc": (c_int32, [c_void_p, c_int32, c_int64, c_int32, c_int32, c_double, c_void_p, POINTER(c_int32), c_void_p,
                           POINTER(c_int32), c_void_p]),
+    "dsk_spectral_cluster": (c_int32, [c_void_p, c_int32, c_int64, c_void_p, c_int32, c_int32, c_int32, c_int32]
+                             + [c_void_p] * 8),
     "dsk_class_sums_f64": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
                                      c_void_p]),
     "dsk_gram_f64": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),

@@ -32,6 +32,7 @@
 #include "plda_kernels.cuh"
 #include "score_kernels.cuh"
 #include "simt_kernels.cuh"
+#include "spectral_kernels.cuh"
 #include "train_kernels.cuh"
 #include "vbx_kernels.cuh"
 #include "wgrad_umma.cuh"
@@ -3756,6 +3757,177 @@ int32_t dsk_ahc(const float* S, int32_t N, int64_t ld, int32_t linkage, int32_t 
   ahc_assemble(rec, N, keep, Z, labels);
   *n_merges = keep;
   if (n_rounds) *n_rounds = hs.round;
+  return DSK_OK;
+}
+
+// ---- spectral clustering -----------------------------------------------------------------------------------------
+static_assert(dsk::kScMaxB >= DSK_SC_MAX_SPEAKERS + 1 + dsk::kScGuard && DSK_SC_MAX_P <= 64,
+              "spectral: block and grid limits");
+
+int32_t dsk_spectral_cluster(const float* S, int32_t N, int64_t ld, const int32_t* p_values, int32_t n_p,
+                             int32_t max_speakers, int32_t num_speakers, int32_t kmeans_iters, int32_t* labels,
+                             int32_t* k_out, int32_t* p_index_out, double* eigenvalues, double* lambda_max,
+                             double* ratio, double* embedding, void* stream) {
+  bool ok = S && p_values && labels && k_out && p_index_out && eigenvalues && lambda_max && ratio && N >= 2 &&
+            N <= DSK_AHC_MAX_N && ld >= N && n_p >= 1 && n_p <= DSK_SC_MAX_P && max_speakers >= 1 &&
+            max_speakers <= DSK_SC_MAX_SPEAKERS && num_speakers >= 0 &&
+            num_speakers <= std::min<int32_t>(N - 1, DSK_SC_MAX_SPEAKERS) && kmeans_iters >= 1;
+  for (int32_t t = 0; ok && t < n_p; ++t)
+    ok = p_values[t] >= 1 && p_values[t] <= N - 1 && (t == 0 || p_values[t] > p_values[t - 1]);
+  if (!ok)
+    return fail(DSK_ERR_INVALID, "dsk_spectral_cluster: bad arguments (need non-null S, p_values and outputs, "
+                "2 <= N <= %d, ld >= N, 1 <= n_p <= %d, p_values strictly increasing in [1, N - 1], 1 <= max_speakers "
+                "<= %d, 0 <= num_speakers <= min(N - 1, %d), kmeans_iters >= 1; got N %d, ld %lld, n_p %d, "
+                "max_speakers %d, num_speakers %d, kmeans_iters %d)", DSK_AHC_MAX_N, DSK_SC_MAX_P,
+                DSK_SC_MAX_SPEAKERS, DSK_SC_MAX_SPEAKERS, N, static_cast<long long>(ld), n_p, max_speakers,
+                num_speakers, kmeans_iters);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int m = num_speakers ? num_speakers + 1 : std::min(max_speakers + 1, static_cast<int>(N));
+  const int B = std::min(std::max(m + dsk::kScGuard, dsk::kScMinB), static_cast<int>(N)), P = 2 * n_p;
+  const int splits = (N + dsk::kScSplitRows - 1) / dsk::kScSplitRows, tiles = (N + dsk::kScRows - 1) / dsk::kScRows;
+  const size_t n2 = static_cast<size_t>(N) * N, blk = static_cast<size_t>(P) * N * B;
+  const size_t mb2 = dsk::kScMaxB * dsk::kScMaxB;
+  // workspace: codes (N^2 bytes), W (N^2 uint16), deg (n_p N), four blocks (P N B), partials (P splits 48^2), the
+  // small matrices (P 48^2), theta (P 48), the problems, the outputs of step 4 and the flags
+  const size_t sizes[] = {n2, n2 * 2, static_cast<size_t>(n_p) * N * 8, blk * 8, blk * 8, blk * 8, blk * 8,
+                          static_cast<size_t>(P) * splits * mb2 * 8, P * mb2 * 8, P * dsk::kScMaxB * 8,
+                          P * sizeof(dsk::ScProb), static_cast<size_t>(n_p) * m * 8, static_cast<size_t>(n_p) * 8,
+                          static_cast<size_t>(n_p) * 8, static_cast<size_t>(N) * 8, static_cast<size_t>(N) * 4,
+                          static_cast<size_t>(n_p) * 4, 16};
+  constexpr int n_buf = sizeof(sizes) / sizeof(sizes[0]);
+  size_t total = 0, offs[n_buf];
+  for (int i = 0; i < n_buf; ++i) {
+    offs[i] = total;
+    total += (sizes[i] + 255) / 256 * 256;
+  }
+  uint8_t* ws = nullptr;
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&ws), total, s));
+  uint8_t* code = ws + offs[0];
+  uint16_t* W = reinterpret_cast<uint16_t*>(ws + offs[1]);
+  double* deg = reinterpret_cast<double*>(ws + offs[2]);
+  double* buf[4];
+  for (int i = 0; i < 4; ++i) buf[i] = reinterpret_cast<double*>(ws + offs[3 + i]);
+  double* part = reinterpret_cast<double*>(ws + offs[7]);
+  double* mat = reinterpret_cast<double*>(ws + offs[8]);
+  double* theta = reinterpret_cast<double*>(ws + offs[9]);
+  dsk::ScProb* probs = reinterpret_cast<dsk::ScProb*>(ws + offs[10]);
+  double* d_eig = reinterpret_cast<double*>(ws + offs[11]);
+  double* d_lmax = reinterpret_cast<double*>(ws + offs[12]);
+  double* d_ratio = reinterpret_cast<double*>(ws + offs[13]);
+  double* scratch = reinterpret_cast<double*>(ws + offs[14]);
+  int32_t* d_labels = reinterpret_cast<int32_t*>(ws + offs[15]);
+  int32_t* d_pv = reinterpret_cast<int32_t*>(ws + offs[16]);
+  int32_t* flags = reinterpret_cast<int32_t*>(ws + offs[17]);  // [0] bad, [1..2] the selection (k, t)
+  int rc = DSK_OK;
+  std::vector<dsk::ScProb> hp(P);
+  int32_t hsel[3] = {0, 0, 0};
+  do {
+    cudaError_t e = cudaMemcpyAsync(d_pv, p_values, n_p * sizeof(int32_t), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaMemsetAsync(flags, 0, 16, s);
+    const size_t rank_smem = static_cast<size_t>(N) * 4;
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(dsk::sc_rank_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               static_cast<int>(rank_smem));
+    if (e == cudaSuccess) {
+      dsk::sc_rank_kernel<<<N, dsk::kScThreads, rank_smem, s>>>(S, N, ld, d_pv, n_p, code, flags);
+      e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(hsel, flags, sizeof(int32_t), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) {
+      rc = fail(DSK_ERR_CUDA, "dsk_spectral_cluster: %s", cudaGetErrorString(e));
+      break;
+    }
+    if (hsel[0]) {
+      rc = fail(DSK_ERR_INVALID, "dsk_spectral_cluster: bad arguments (a non-finite off-diagonal similarity in S)");
+      break;
+    }
+    const int t32 = (N + 31) / 32;
+    dsk::sc_pair_kernel<<<dim3(t32, t32), dim3(32, 8), 0, s>>>(code, N, W);
+    dsk::sc_degree_kernel<<<N, dsk::kScThreads, 0, s>>>(W, N, n_p, deg);
+    dsk::sc_setup_kernel<<<P, dsk::kScThreads, 0, s>>>(deg, N, n_p, m, B, probs);
+    dsk::sc_init_kernel<<<dim3(static_cast<unsigned>((static_cast<size_t>(N) * B + 255) / 256), P), 256, 0, s>>>(
+        buf[0], N, B, probs);
+    int src = 0;  // the buffer holding every active problem's block
+    bool done = false;
+    for (int it = 0; it < dsk::kScMaxOuter && !done && rc == DSK_OK; ++it) {
+      // orthonormalise by three CholeskyQR passes, src -> x -> y -> 0 (x, y the two other scratch buffers): the first
+      // may need the shift, the others restore orthogonality to rounding (shifted CholeskyQR3)
+      const int x = src == 1 ? 2 : 1, y = src == 0 ? 2 : 3;  // src 0: 1, 2; src 1: 2, 3; src 2: 1, 3
+      const int from[3] = {src, x, y}, to[3] = {x, y, 0};
+      for (int pass = 0; pass < 3; ++pass) {
+        dsk::sc_gram_kernel<<<dim3(P, splits), dsk::kScThreads, 0, s>>>(buf[from[pass]], buf[from[pass]], N, B, probs,
+                                                                        part);
+        dsk::sc_small_kernel<<<P, dsk::kScThreads, 0, s>>>(part, splits, N, probs, dsk::kScModeChol, mat, theta);
+        dsk::sc_apply_kernel<<<dim3(P, tiles), dsk::kScThreads, 0, s>>>(buf[from[pass]], buf[to[pass]], N, B, probs,
+                                                                        mat);
+      }
+      // Rayleigh-Ritz: Z = Op X (buffer 1), H = X^T Z, X Q -> 2, Z Q -> 3, then the residuals
+      dsk::sc_matvec_kernel<<<dim3(P, tiles), dsk::kScThreads, 0, s>>>(W, deg, probs, N, B, -1, buf[0], nullptr,
+                                                                       buf[1]);
+      dsk::sc_gram_kernel<<<dim3(P, splits), dsk::kScThreads, 0, s>>>(buf[0], buf[1], N, B, probs, part);
+      dsk::sc_small_kernel<<<P, dsk::kScThreads, 0, s>>>(part, splits, N, probs, dsk::kScModeRR, mat, theta);
+      dsk::sc_apply_kernel<<<dim3(P, tiles), dsk::kScThreads, 0, s>>>(buf[0], buf[2], N, B, probs, mat);
+      dsk::sc_apply_kernel<<<dim3(P, tiles), dsk::kScThreads, 0, s>>>(buf[1], buf[3], N, B, probs, mat);
+      dsk::sc_resid_kernel<<<dim3(P, splits), dsk::kScMaxB, 0, s>>>(buf[2], buf[3], N, B, probs, theta, part);
+      dsk::sc_small_kernel<<<P, dsk::kScThreads, 0, s>>>(part, splits, N, probs, dsk::kScModeRes, mat, theta);
+      e = cudaGetLastError();
+      if (e == cudaSuccess) e = cudaMemcpyAsync(hp.data(), probs, P * sizeof(dsk::ScProb), cudaMemcpyDeviceToHost, s);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+      if (e != cudaSuccess) {
+        rc = fail(DSK_ERR_CUDA, "dsk_spectral_cluster: %s", cudaGetErrorString(e));
+        break;
+      }
+      int max_deg = 0;
+      done = true;
+      for (const dsk::ScProb& p : hp) {
+        if (p.failed) {
+          rc = fail(DSK_ERR_STATE, "dsk_spectral_cluster: the %s eigenpairs at p = %d did not converge in %d "
+                    "iterations (residual %.3g of the spectrum bound)", p.top ? "largest" : "smallest",
+                    p_values[p.t], dsk::kScMaxOuter, p.res);
+          break;
+        }
+        if (!p.conv) {
+          done = false;
+          max_deg = std::max(max_deg, p.deg);
+        }
+      }
+      if (rc || done) break;
+      // Chebyshev filter from the Ritz vectors in 2, rotating through 2 -> 0 -> 1 -> 2 ...
+      int cur = 2, prev = 2;
+      for (int k = 0; k < max_deg; ++k) {
+        const int nxt = (cur + 1) % 3;
+        dsk::sc_matvec_kernel<<<dim3(P, tiles), dsk::kScThreads, 0, s>>>(W, deg, probs, N, B, k, buf[cur], buf[prev],
+                                                                         buf[nxt]);
+        prev = cur;
+        cur = nxt;
+      }
+      src = cur;
+    }
+    if (rc) break;
+    if (!done) {
+      rc = fail(DSK_ERR_STATE, "dsk_spectral_cluster: no convergence in %d iterations", dsk::kScMaxOuter);
+      break;
+    }
+    // the final Ritz vectors and values of every problem are in buffer 2 and theta
+    dsk::sc_select_kernel<<<1, 1, 0, s>>>(probs, theta, n_p, m, N, d_pv, num_speakers, d_eig, d_lmax, d_ratio,
+                                          flags + 1);
+    dsk::sc_kmeans_kernel<<<1, dsk::kScKmThreads, 0, s>>>(buf[2], N, B, flags + 1, kmeans_iters, scratch, d_labels,
+                                                          embedding, m - 1);
+    e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(hsel, flags, 3 * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(labels, d_labels, N * sizeof(int32_t), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(eigenvalues, d_eig, n_p * m * sizeof(double), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(lambda_max, d_lmax, n_p * sizeof(double), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ratio, d_ratio, n_p * sizeof(double), cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) rc = fail(DSK_ERR_CUDA, "dsk_spectral_cluster: %s", cudaGetErrorString(e));
+  } while (false);
+  const cudaError_t fe = cudaFreeAsync(ws, s);
+  if (rc) return rc;
+  if (fe != cudaSuccess) return fail(DSK_ERR_CUDA, "dsk_spectral_cluster: cudaFreeAsync failed: %s", cudaGetErrorString(fe));
+  *k_out = hsel[1];
+  *p_index_out = hsel[2];
   return DSK_OK;
 }
 

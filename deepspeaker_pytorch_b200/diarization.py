@@ -22,6 +22,12 @@ With ``plda`` and ``vbx`` (a dict of ``vbx`` options, ``{}`` for the defaults) t
 emission model is the PLDA itself (Landini et al., 2022), so neighbouring windows tend to share a speaker and surplus
 initial clusters lose their windows.  ``der`` scores per-frame labels against a reference.
 
+With ``spectral`` (a dict of ``spectral`` options, ``{}`` for the defaults) every recording is clustered by spectral
+clustering instead of AHC, with the number of speakers estimated by the normalised maximum eigengap (NME-SC, Park et
+al., IEEE SPL 2020) unless ``num_speakers`` fixes it: no threshold and no PLDA are needed, since NME-SC reads only
+the ranks of each window's affinities (cosines, or PLDA LLRs with ``plda``).  ``engine.spectral_cluster`` solves the
+eigenproblems of every pruning level of the grid in one call on the device.
+
 Overlapped speech and re-segmentation are not part of this module: a frame gets at most one speaker.
 """
 from __future__ import annotations
@@ -183,6 +189,75 @@ def der(ref, hyp):
     return DER((miss + fa + conf) / n, miss / n, fa / n, conf / n, mapping)
 
 
+class SpectralResult(NamedTuple):
+    """``spectral``'s result: ``labels`` (N,) int32 device tensor numbered by each cluster's smallest member, ``k`` the
+    number of speakers, ``p`` the index of the chosen pruning level into ``p_values`` (None when no eigenproblem was
+    solved), ``eigenvalues`` (n_p, m) fp64 the m smallest eigenvalues of every level's Laplacian, ``lambda_max`` and
+    ``ratio`` (n_p,) its largest eigenvalue and NME ratio r_p."""
+    labels: torch.Tensor
+    k: int
+    p: int
+    p_values: np.ndarray
+    eigenvalues: np.ndarray
+    lambda_max: np.ndarray
+    ratio: np.ndarray
+
+
+SPECTRAL_OPTIONS = ("max_speakers", "p_max_frac", "p_steps", "kmeans_iters")
+
+
+def p_grid(N: int, p_max_frac: float = 0.25, p_steps: int = 30) -> np.ndarray:
+    """The pruning levels tried for N items: the unique integers of linspace(1, max(1, floor(p_max_frac (N - 1))),
+    p_steps)."""
+    top = max(1, int(np.floor(float(p_max_frac) * (int(N) - 1))))
+    return np.unique(np.linspace(1, top, int(p_steps)).astype(np.int64))
+
+
+def spectral(S, max_speakers: int = 8, num_speakers=None, p_max_frac: float = 0.25, p_steps: int = 30,
+             kmeans_iters: int = 100) -> SpectralResult:
+    """Spectral clustering of N items from their similarities S (N, N) fp32 CUDA (cosines or PLDA LLRs; only each
+    row's ranks matter) with NME-SC speaker counting (oracle/spectral_oracle.py): for every pruning level p of
+    ``p_grid(N, p_max_frac, p_steps)`` the graph keeping each item's p nearest neighbours, the eigengap count and the
+    NME ratio r_p; the level of least r_p gives the count (at most ``max_speakers``, or ``num_speakers`` when given)
+    and the k-means partition of its spectral embedding.  ``num_speakers >= N`` gives one speaker per item without
+    solving anything; a count or ``max_speakers`` above DSK_SC_MAX_SPEAKERS (32) is otherwise a ValueError.  The defaults are the starting values of NeMo's diarization configs; they are NOT tuned for
+    this model."""
+    N = int(S.shape[0])
+    if not 0 < p_max_frac <= 1 or int(p_steps) < 1:
+        raise ValueError(f"spectral: need 0 < p_max_frac <= 1 and p_steps >= 1, got {p_max_frac}, {p_steps}")
+    if num_speakers is not None and int(num_speakers) < 1:
+        raise ValueError(f"spectral: num_speakers must be >= 1, got {num_speakers}")
+    if not 1 <= int(max_speakers) <= L.DSK_SC_MAX_SPEAKERS:
+        raise ValueError(f"spectral: max_speakers must be in [1, {L.DSK_SC_MAX_SPEAKERS}] (DSK_SC_MAX_SPEAKERS), got "
+                         f"{max_speakers}")
+    if num_speakers is not None and L.DSK_SC_MAX_SPEAKERS < int(num_speakers) < N:
+        raise ValueError(f"spectral: num_speakers must be <= {L.DSK_SC_MAX_SPEAKERS} (DSK_SC_MAX_SPEAKERS) or >= the "
+                         f"{N} items, got {num_speakers}")
+    pv = p_grid(N, p_max_frac, p_steps)
+    if N < 2 or (num_speakers is not None and int(num_speakers) >= N):
+        empty = np.zeros((0,), np.float64)
+        return SpectralResult(torch.arange(N, dtype=torch.int32, device=S.device), N, None, pv,
+                              np.zeros((0, 0)), empty, empty)
+    lab, k, t, eig, lmax, ratio = engine.spectral_cluster(S, pv, max_speakers, num_speakers, kmeans_iters)
+    return SpectralResult(lab, k, t, pv, eig, lmax, ratio)
+
+
+def _spectral_options(spectral, threshold, vbx):
+    if spectral is None:
+        return None
+    if not isinstance(spectral, dict):
+        raise ValueError(f"diarize: spectral must be None or a dict of options, got {type(spectral).__name__}")
+    unknown = sorted(set(spectral) - set(SPECTRAL_OPTIONS))
+    if unknown:
+        raise ValueError(f"diarize: unknown spectral options {unknown}; known: {list(SPECTRAL_OPTIONS)}")
+    if threshold is not None:
+        raise ValueError("diarize: spectral clustering takes no threshold (it estimates the count, or num_speakers "
+                         "fixes it)")
+    if vbx is not None:
+        raise ValueError("diarize: give at most one of vbx and spectral")
+    return dict(spectral)
+
+
 def _vbx_options(vbx, plda):
     if vbx is None:
         return None
@@ -246,9 +321,10 @@ def _smallest_hop(last, rec, R, hop):
     return lo
 
 
-def _cluster(E, plda, threshold, linkage, k):
+def _cluster(E, plda, threshold, linkage, k, sc_opts=None):
     """AHC of one recording's window embeddings E: on their cosines, or with a PLDA backend on the LLRs of their
-    transformed rows (a threshold on LLRs s is the threshold 1 - s on ahc's distance 1 - S)."""
+    transformed rows (a threshold on LLRs s is the threshold 1 - s on ahc's distance 1 - S).  With ``spectral``
+    options ``sc_opts``, spectral clustering of the same affinity instead (k None: estimated), and an empty linkage matrix."""
     if plda is None:
         S = engine.cosine_matrix(E, E)
     else:
@@ -256,12 +332,18 @@ def _cluster(E, plda, threshold, linkage, k):
         S = plda.score_matrix(Y, Y)
         if threshold is not None:
             threshold = 1.0 - float(threshold)
+    if sc_opts is not None:
+        return np.zeros((0, 4)), spectral(S, num_speakers=k, **sc_opts).labels
     if threshold is not None:
         return engine.ahc(S, linkage, threshold=threshold)
     return engine.ahc(S, linkage, num_clusters=k)
 
 
-def _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batch, plda, vbx):
+def _count(ks, r, W):
+    return None if ks[r] is None else min(int(ks[r]), W)
+
+
+def _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batch, plda, vbx, spectral):
     R = u.size
     table, runs, run_off, kept = bank._run_table(speech, u, "diarize")
     rec, first, end = table[:, 0], table[:, 1], table[:, 2]
@@ -289,7 +371,7 @@ def _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batc
         elif W == 1:
             wl, Z = np.zeros(1, np.int32), np.zeros((0, 4))
         else:
-            Z, lab = _cluster(emb[a:b], plda, threshold, linkage, min(int(ks[r]), W) if threshold is None else None)
+            Z, lab = _cluster(emb[a:b], plda, threshold, linkage, _count(ks, r, W), spectral)
             wl = lab.cpu().numpy()
         spans.append((a, b))
         wls.append(wl)
@@ -309,7 +391,7 @@ def _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batc
 
 
 def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40, num_speakers=None, threshold=None,
-            linkage: str = "average", batch: int = 256, speech=None, plda=None, vbx=None) -> list:
+            linkage: str = "average", batch: int = 256, speech=None, plda=None, vbx=None, spectral=None) -> list:
     """Diarize the recordings ``utt`` (indices into ``bank``) -> [Recording] in the order of ``utt``.  Give exactly
     one of ``num_speakers`` (an int, or one per recording; a recording with fewer windows gets one speaker per window)
     and ``threshold`` (a cosine distance 1 - cos: windows merge while the linkage distance is <= threshold), else
@@ -330,8 +412,15 @@ def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40,
     call refines the window labels of every recording of more than one window (with ``speech``, all speech windows of
     a recording in time order form one sequence).  ``window_labels`` are VBx's, renumbered by first window; frame
     labels and segments follow from them as above; ``Z`` stays the AHC tree.  More than DSK_VBX_MAX_SPEAKERS initial
-    clusters in a recording is a ValueError."""
-    if (num_speakers is None) == (threshold is None):
+    clusters in a recording is a ValueError.
+
+    ``spectral``: None (AHC, as above), or a dict of options of ``spectral`` (``{}`` for its defaults): every recording
+    of more than one window is then clustered by spectral clustering of the same affinity (cosines, or PLDA LLRs with
+    ``plda``), with or without ``speech``.  ``num_speakers`` becomes optional: None estimates each recording's count,
+    an int or a per-recording list fixes it.  ``threshold`` or ``vbx`` with ``spectral``, and an unknown option, are
+    ValueErrors.  ``Z`` is then an empty (0, 4) array."""
+    spectral = _spectral_options(spectral, threshold, vbx)
+    if spectral is None and (num_speakers is None) == (threshold is None):
         raise ValueError("diarize: give exactly one of num_speakers and threshold")
     if linkage not in engine.LINKAGES:
         raise ValueError(f"diarize: linkage must be one of {sorted(engine.LINKAGES)}, got {linkage!r}")
@@ -345,7 +434,7 @@ def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40,
     if num_speakers is not None and any(int(k) < 1 for k in ks):
         raise ValueError(f"diarize: num_speakers must be >= 1, got {num_speakers}")
     if speech is not None:
-        return _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batch, plda, vbx)
+        return _diarize_speech(model, bank, u, speech, T, hop, ks, threshold, linkage, batch, plda, vbx, spectral)
     _, _, win_off = bank.windows(u, T, hop)
     counts = np.diff(win_off.numpy())
     if counts.max() > MAX_WINDOWS:
@@ -361,7 +450,7 @@ def diarize(model, bank: frontend.FeatureBank, utt, T: int = 160, hop: int = 40,
         if W == 1:
             wl, Z = np.zeros(1, np.int32), np.zeros((0, 4))
         else:
-            Z, lab = _cluster(emb[a:b], plda, threshold, linkage, min(int(ks[r]), W) if threshold is None else None)
+            Z, lab = _cluster(emb[a:b], plda, threshold, linkage, _count(ks, r, W), spectral)
             wl = lab.cpu().numpy()
         spans.append((a, b))
         wls.append(wl)

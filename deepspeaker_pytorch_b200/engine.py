@@ -976,6 +976,42 @@ def ahc(S, linkage="average", num_clusters=None, threshold=None, return_rounds=F
     return out + (rounds.value,) if return_rounds else out
 
 
+def spectral_cluster(S, p_values, max_speakers=8, num_speakers=None, kmeans_iters=100, return_embedding=False):
+    """dsk_spectral_cluster: spectral clustering of N items from their similarities S (N, N) fp32 on the device (higher
+    = closer; both triangles are read, the diagonal never, the row stride is kept) with NME-SC speaker counting over
+    the pruning levels ``p_values`` (strictly increasing in [1, N - 1]).  ``num_speakers``: None estimates the count
+    (at most ``max_speakers``), an int fixes it.  -> (labels torch.int32 (N,) on S's device numbered by each cluster's
+    smallest member, k, p_index into p_values, eigenvalues np.float64 (n_p, m), lambda_max (n_p,), ratio (n_p,)), plus
+    the (N, m - 1) fp64 device embedding (its first k columns the eigenvectors) with ``return_embedding``.
+    RuntimeError on a non-finite off-diagonal similarity or on bad arguments."""
+    if not S.is_cuda:
+        raise RuntimeError("spectral_cluster needs a CUDA tensor; there is no CPU fallback")
+    if S.dim() != 2 or S.shape[0] != S.shape[1] or S.dtype != torch.float32 or S.stride(1) != 1:
+        raise RuntimeError(f"spectral_cluster: expected a row-major fp32 (N, N) tensor, got {S.dtype} {tuple(S.shape)}")
+    N = S.shape[0]
+    pv = np.ascontiguousarray(np.asarray(p_values, np.int64).reshape(-1).astype(np.int32))
+    ns = 0 if num_speakers is None else int(num_speakers)
+    m = ns + 1 if ns else min(int(max_speakers) + 1, max(N, 1))
+    labels = np.empty(max(N, 1), np.int32)
+    eig = np.empty((max(pv.size, 1), max(m, 1)), np.float64)
+    lmax = np.empty(max(pv.size, 1), np.float64)
+    ratio = np.empty(max(pv.size, 1), np.float64)
+    k, t = ctypes.c_int32(0), ctypes.c_int32(0)
+    emb = torch.zeros((max(N, 1), max(m - 1, 1)), dtype=torch.float64, device=S.device) if return_embedding else None
+
+    def host(a):
+        return a.ctypes.data_as(ctypes.c_void_p)
+
+    with torch.cuda.device(S.device):
+        L.check(L.load().dsk_spectral_cluster(S.data_ptr(), N, S.stride(0), host(pv), pv.size, int(max_speakers), ns,
+                                              int(kmeans_iters), host(labels), ctypes.byref(k), ctypes.byref(t),
+                                              host(eig), host(lmax), host(ratio),
+                                              emb.data_ptr() if emb is not None else None, L.cur_stream()),
+                "dsk_spectral_cluster")
+    out = (torch.from_numpy(labels).to(S.device), k.value, t.value, eig, lmax, ratio)
+    return out + (emb,) if return_embedding else out
+
+
 # ---------------------------------------------------------------------------------------------------
 # PLDA backend: fp64 fit statistics, transforms, LLR scoring
 # ---------------------------------------------------------------------------------------------------

@@ -633,6 +633,39 @@ int32_t dsk_class_centroids(const float* X, int32_t U, int32_t D, const int64_t*
 int32_t dsk_ahc(const float* S, int32_t N, int64_t ld, int32_t linkage, int32_t stop_k, double stop_height, double* Z,
                 int32_t* n_merges, int32_t* labels, int32_t* n_rounds, void* stream);
 
+/* Diarization without a threshold: spectral clustering with NME-SC speaker counting (Park, Han, Kumar, Narayanan, IEEE
+ * SPL 2020; no reference implementation exists, oracle/spectral_oracle.py defines the algorithm).  S (N x N fp32,
+ * device, row stride ld floats) holds similarities, higher meaning closer; both triangles are read, the diagonal never.
+ *   Ranks: per row i the columns j != i in descending S[i][j], ties to the lower column (dsk_topk_indices's order);
+ *     A_p[i][j] = ([rank_ij < p] + [rank_ji < p]) / 2, L_p = diag(A_p 1) - A_p, for every p of p_values (HOST,
+ *     strictly increasing in [1, N - 1]).  Only the ranks matter: S and a S + b (a > 0) give the same outputs.
+ *   Eigenvalues: per p the m smallest (m = min(max_speakers + 1, N), or num_speakers + 1 when num_speakers > 0) and
+ *     the largest, lambda_N, by Chebyshev-filtered subspace iteration on blocks of min(max(m + 8, 40), N) and min(8, N) columns
+ *     (every p in the same launches; fp64 on the CUDA cores; CholeskyQR2 and a Jacobi Rayleigh-Ritz per iteration).
+ *     Leading converged columns are locked (the filter leaves them, and CholeskyQR, run three times with them first,
+ *     projects them out of the others).  Every wanted pair ends with |L y - lambda y| <= 1e-10 * 2 max_i d_i; a p
+ *     that does not within 1000 iterations fails the call with DSK_ERR_STATE and a message naming p.
+ *   Selection: k_p = the first i in [1, m - 1] maximising lambda_{i+1} - lambda_i (num_speakers when > 0),
+ *     g_p = (lambda_{k+1} - lambda_k) / (lambda_N + 1e-10), ratio r_p = (p / N) / (g_p + 1e-10); p-hat is the first p
+ *     of least r_p.  k-means (fp64, one CTA) on the rows of the eigenvectors of lambda_1 .. lambda_k of L_p-hat:
+ *     maximin initialisation, at most kmeans_iters Lloyd iterations; labels numbered by each cluster's smallest member.
+ *   Outputs: labels (N) int32, *k_out, *p_index_out (into p_values), eigenvalues (n_p, m) fp64 ascending, lambda_max
+ *     (n_p), ratio (n_p), all HOST memory (the call synchronises the stream); embedding (N, m - 1) fp64 DEVICE (may be
+ *     NULL): the k eigenvectors of L_p-hat in its first k columns, zeros after them.
+ *   No float atomics and fixed-order sums: the same bits on every call.  Workspace (stream-ordered): 3 N^2 bytes
+ *   (codes and W), 8 n_p N bytes (degrees), 64 n_p N B bytes (four blocks of 2 n_p problems, B = min(max(m + 8, 40),
+ *   N) columns each), 18 KiB per problem per 256 rows (the Gram partials, 48 x 48 fp64 each) and O(n_p + N) more.
+ *   2 <= N <= DSK_AHC_MAX_N, ld >= N, 1 <= n_p <= DSK_SC_MAX_P, 1 <= max_speakers <= DSK_SC_MAX_SPEAKERS,
+ *   0 <= num_speakers <= min(N - 1, DSK_SC_MAX_SPEAKERS), kmeans_iters >= 1, non-null pointers (but embedding), else
+ *   DSK_ERR_INVALID before any device work; a non-finite off-diagonal similarity gives DSK_ERR_INVALID after one
+ *   validation pass. */
+#define DSK_SC_MAX_SPEAKERS 32
+#define DSK_SC_MAX_P 64
+int32_t dsk_spectral_cluster(const float* S, int32_t N, int64_t ld, const int32_t* p_values, int32_t n_p,
+                             int32_t max_speakers, int32_t num_speakers, int32_t kmeans_iters, int32_t* labels,
+                             int32_t* k_out, int32_t* p_index_out, double* eigenvalues, double* lambda_max,
+                             double* ratio, double* embedding, void* stream);
+
 /* PLDA backend: the N-sized passes of an LDA + two-covariance PLDA fit (the Kaldi x-vector recipe) and PLDA
  * log-likelihood-ratio scoring (no reference implementation exists; oracle/plda_oracle.py defines the model).  Inputs
  * are fp32 rows, every statistic is fp64, no float atomics: each output is the same bits on every call.  All pointers
