@@ -1,4 +1,4 @@
-"""ctypes binding of libdsk.so (the C ABI in include/dsk.h) and the in-tree nvcc build recipe.
+"""ctypes binding of libdsk.so, read from the C ABI in include/dsk.h, and the in-tree nvcc build recipe.
 
 The product path has no fallback: if the shared library is missing or an entry point fails, a
 RuntimeError is raised (north star: "no CPU fallback, no multi-backend dispatch").
@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes
 import os
+import re
 import shutil
 import subprocess
 from ctypes import POINTER, c_char_p, c_double, c_float, c_int32, c_int64, c_void_p
@@ -16,20 +17,7 @@ CSRC = os.path.join(_HERE, "csrc")
 LIB_DIR = os.path.join(_HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libdsk.so")
 INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
-
-NUM_CONV = 12
-DSK_F16, DSK_BF16 = 0, 1
-DSK_EVAL, DSK_TRAIN = 0, 1
-DSK_GE2E_SOFTMAX, DSK_GE2E_CONTRAST = 0, 1
-DSK_LINKAGE_AVERAGE, DSK_LINKAGE_COMPLETE = 0, 1
-DSK_AHC_MAX_N = 32768
-DSK_NORM_NONE, DSK_NORM_LENGTH, DSK_NORM_PLDA = 0, 1, 2
-DSK_F64_MAX_DIM = 4096
-DSK_PLDA_MAX_ROWS = 4194240
-DSK_VBX_MAX_SPEAKERS = 128
-DSK_SC_MAX_SPEAKERS, DSK_SC_MAX_P = 32, 64
-DSK_SPEED_MAX_DEN, DSK_SPEED_TAPS, DSK_SPEED_MAX_FACTORS = 32, 50, 8
-DSK_AAM_MAX_C, DSK_AAM_MAX_SUBCENTRES, DSK_AAM_MAX_TOPK = 65536, 16, 64
+HEADER = os.path.join(INCLUDE, "dsk.h")
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -38,9 +26,7 @@ NVCC_FLAGS = [
 
 
 def _sources():
-    return sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cu", ".cuh"))) + [
-        os.path.join(INCLUDE, "dsk.h")
-    ]
+    return sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cu", ".cuh"))) + [HEADER]
 
 
 HASH_PATH = LIB_PATH + ".srchash"
@@ -100,184 +86,84 @@ def build(force: bool = False, verbose: bool = False) -> str:
     return LIB_PATH
 
 
-class DskWeights(ctypes.Structure):
-    _fields_ = [
-        ("conv_w", c_void_p * NUM_CONV),
-        ("bn_gamma", c_void_p * NUM_CONV),
-        ("bn_beta", c_void_p * NUM_CONV),
-        ("bn_running_mean", c_void_p * NUM_CONV),
-        ("bn_running_var", c_void_p * NUM_CONV),
-        ("fc_w", c_void_p),
-        ("fc_b", c_void_p),
-        ("embedding_size", c_int32),
-    ]
+# ---- the binding, read from include/dsk.h at import -------------------------------------------------------------------
+# The header is the only statement of the C ABI: its integer #defines and enum members become module constants
+# (DSK_NUM_CONV, DSK_F16, ...), its structs ctypes Structures (dsk_weights -> DskWeights) and its prototypes the
+# (restype, argtypes) pairs that load() applies.  The compiler holds csrc/dsk_api.cu to the same header.
+
+def _ctype(decl: str, structs: dict, handles: set, where: str, ret: bool = False):
+    """The ctypes type of a header type; the one place where the binding names a ctypes scalar type.  A pointer is
+    c_void_p (device arrays are passed as data_ptr() integers, host out-parameters by byref() or as arrays), except a
+    pointer to a header struct, to a pointer or to a handle.  ValueError naming ``where`` for any other type."""
+    t = " ".join(decl.replace("*", " * ").split()).replace(" *", "*")
+    if ret and t == "const char*":
+        return c_char_p
+    t = t.removeprefix("const ")
+    if t.endswith("*"):
+        pointee = t[:-1].removeprefix("const ")
+        if pointee.endswith("*") or pointee in handles:
+            return POINTER(c_void_p)
+        return POINTER(structs[pointee]) if pointee in structs else c_void_p
+    if t in handles:
+        return c_void_p
+    scalars = {"int32_t": c_int32, "int64_t": c_int64, "float": c_float, "double": c_double}
+    if t not in scalars:
+        raise ValueError(f"{where}: no ctypes type for '{t}'")
+    return scalars[t]
 
 
-class DskGrads(ctypes.Structure):
-    _fields_ = [
-        ("conv_w", c_void_p * NUM_CONV),
-        ("bn_gamma", c_void_p * NUM_CONV),
-        ("bn_beta", c_void_p * NUM_CONV),
-        ("fc_w", c_void_p),
-        ("fc_b", c_void_p),
-    ]
+def _declarator(decl: str, where: str):
+    """(type, name, array extent or None) of a parameter or a struct field: ``const float* conv_w[DSK_NUM_CONV]``."""
+    m = re.fullmatch(r"\s*(\S.*?)\s*\b(\w+)\s*(?:\[\s*(\w+)\s*\])?\s*", decl, flags=re.S)
+    if not m:
+        raise ValueError(f"{where}: cannot read '{' '.join(decl.split())}'")
+    return m.groups()
 
 
-class DskBackwardCapture(ctypes.Structure):
-    _fields_ = [
-        ("gy", c_void_p * NUM_CONV),
-        ("G", c_void_p * NUM_CONV),
-        ("gres", c_void_p * NUM_CONV),
-        ("g_fc", c_void_p),
-        ("fc_out", c_void_p),
-        ("dP", c_void_p),
-        ("loss_scale", c_void_p),
-    ]
+def read_header(text: str):
+    """(constants, structs, prototypes) of a C header written as include/dsk.h is.  constants: every
+    ``#define DSK_<NAME> <integer>`` and enum member, by name; structs: every ``typedef struct {...} dsk_x;`` as a
+    ctypes.Structure named DskX, by typedef name; prototypes: every ``ret dsk_name(params);`` as (restype, argtypes),
+    by name.  ``typedef struct X* name;`` declares an opaque handle.  ValueError for anything else it meets."""
+    src = re.sub(r"/\*.*?\*/|//[^\n]*", " ", text, flags=re.S)
+    src = re.sub(r"#ifdef __cplusplus.*?#endif", "", src, flags=re.S)  # the extern "C" wrapper
+    consts = {n: int(v) for n, v in re.findall(r"^\s*#\s*define\s+(DSK_\w+)\s+(-?\d+)\s*$", src, flags=re.M)}
+    src = re.sub(r"^\s*#.*$", "", src, flags=re.M)
+    for body in re.findall(r"typedef\s+enum\s*\{([^}]*)\}\s*\w+\s*;", src):
+        for item in body.split(","):
+            m = re.fullmatch(r"\s*(DSK_\w+)\s*=\s*(-?\d+)\s*", item)
+            if not m:
+                raise ValueError(f"cannot read enum member '{item.strip()}' (each needs an explicit value)")
+            consts[m[1]] = int(m[2])
+    handles = set(re.findall(r"typedef\s+struct\s+\w+\s*\*\s*(\w+)\s*;", src))
+    structs = {}
+    for body, name in re.findall(r"typedef\s+struct\s*\{([^}]*)\}\s*(\w+)\s*;", src):
+        fields = []
+        for field in filter(str.strip, body.split(";")):
+            t, f, n = _declarator(field, name)
+            t = _ctype(t, structs, handles, f"{name}.{f}")
+            fields.append((f, t * (consts[n] if n in consts else int(n)) if n else t))
+        camel = "".join(w.capitalize() for w in name.split("_"))
+        structs[name] = type(camel, (ctypes.Structure,), {"_fields_": fields})
+    *decls, rest = re.sub(r"typedef\s[^;{]*(\{[^}]*\})?[^;]*;", "", src).split(";")
+    if rest.strip():
+        raise ValueError(f"cannot read '{' '.join(rest.split())}'")
+    prototypes = {}
+    for decl in decls:
+        m = re.fullmatch(r"\s*(.+?)\s*\b(dsk_\w+)\s*\((.*)\)\s*", decl, flags=re.S)
+        if not m:
+            raise ValueError(f"cannot read '{' '.join(decl.split())}'")
+        ret, name, params = m.groups()
+        params = [] if params.strip() == "void" else [_declarator(p, name)[0] for p in params.split(",")]
+        prototypes[name] = (_ctype(ret, structs, handles, name, ret=True),
+                            [_ctype(p, structs, handles, name) for p in params])
+    return consts, structs, prototypes
 
 
-# name -> (restype, argtypes); must list every symbol declared in include/dsk.h
-SIGNATURES = {
-    "dsk_last_error": (c_char_p, []),
-    "dsk_version": (c_int32, []),
-    "dsk_create": (c_int32, [POINTER(c_void_p), c_int32, c_int32]),
-    "dsk_destroy": (c_int32, [c_void_p]),
-    "dsk_load_weights": (c_int32, [c_void_p, POINTER(DskWeights), c_void_p]),
-    "dsk_load_weights_train": (c_int32, [c_void_p, POINTER(DskWeights), c_void_p]),
-    "dsk_share_weights": (c_int32, [c_void_p, c_void_p]),
-    "dsk_rescnn_forward": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int32, c_void_p]),
-    "dsk_rescnn_forward_train": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, POINTER(c_void_p), c_void_p]),
-    "dsk_rescnn_backward": (c_int32, [c_void_p, c_void_p, c_void_p, POINTER(DskGrads), c_void_p]),
-    "dsk_train_ctx_read": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p]),
-    "dsk_debug_backward_plan": (c_int32, [c_void_p, c_void_p, c_int32, POINTER(c_int32)]),
-    "dsk_debug_read_eval_activation": (c_int32, [c_void_p, c_int32, c_void_p, c_int64, POINTER(c_int32), c_void_p]),
-    "dsk_train_ctx_release": (c_int32, [c_void_p, c_void_p]),
-    "dsk_set_loss_scale": (c_int32, [c_void_p, c_float]),
-    "dsk_sync_forward_begin": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, POINTER(c_void_p), c_void_p]),
-    "dsk_sync_backward_begin": (c_int32, [c_void_p, c_void_p, c_void_p, POINTER(DskGrads), c_void_p]),
-    "dsk_sync_records": (c_int32, [c_void_p, c_void_p, POINTER(c_void_p), POINTER(c_int64)]),
-    "dsk_sync_stage": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, POINTER(c_int32), c_void_p]),
-    "dsk_bn_act_sync_train_forward": (c_int32, [c_void_p] * 10 + [c_int32, c_int32, c_int32, c_void_p]),
-    "dsk_set_profiling": (c_int32, [c_void_p, c_int32]),
-    "dsk_get_launch_times": (c_int32, [c_void_p, c_void_p, c_int32, POINTER(c_int32)]),
-    "dsk_conv2d_nhwc": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32,
-                                  c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_float, c_void_p]),
-    "dsk_conv2d_dgrad_nhwc": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32,
-                                        c_int32, c_int32, c_int32, c_int32, c_void_p]),
-    "dsk_conv2d_wgrad_nhwc": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32,
-                                        c_int32, c_int32, c_int32, c_float, c_void_p]),
-    "dsk_bn_act_train_forward": (c_int32, [c_void_p] * 10 + [c_int64, c_int32, c_void_p]),
-    "dsk_bn_act_train_backward": (c_int32, [c_void_p] * 11 + [c_int64, c_int32, c_float, c_void_p]),
-    "dsk_conv3x3_padded": (c_int32, [c_void_p] * 7 + [c_int32, c_int32, c_int32, c_int32, c_int32, c_float, c_int32, c_void_p]),
-    "dsk_conv5x5s2_planar": (c_int32, [c_void_p] * 6 + [c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_float, c_void_p]),
-    "dsk_debug_set_backward_capture": (c_int32, [c_void_p, POINTER(DskBackwardCapture)]),
-    "dsk_padded_positions": (c_int64, [c_int32, c_int32, c_int32]),
-    "dsk_pack_conv_weight": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p]),
-    "dsk_nchw_f32_to_nhwc16": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p]),
-    "dsk_nhwc16_to_nchw_f32": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p]),
-    "dsk_pairwise_distance": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p]),
-    "dsk_pairwise_distance_bwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p,
-                                            c_void_p, c_void_p]),
-    "dsk_triplet_loss": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float, c_void_p, c_void_p,
-                                   c_void_p, c_void_p]),
-    "dsk_triplet_loss_bwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32,
-                                       c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "dsk_margin_select": (c_int32, [c_void_p, c_void_p, c_int32, c_float, c_void_p, c_void_p, c_void_p]),
-    "dsk_gather_rows": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int64, c_void_p, c_void_p]),
-    "dsk_allpairs_topk_tc": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
-    "dsk_allpairs_topk": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
-    "dsk_batch_hard_triplet": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_float] + [c_void_p] * 7),
-    "dsk_batch_hard_triplet_bwd": (c_int32, [c_void_p] * 5 + [c_int32, c_int32, c_float, c_void_p, c_void_p, c_void_p,
-                                                              c_void_p]),
-    "dsk_batch_hard_select_rows": (c_int32, [c_void_p] * 3 + [c_int32] * 4 + [c_void_p] * 6),
-    "dsk_batch_hard_mean": (c_int32, [c_void_p] * 3 + [c_int32, c_float, c_void_p, c_void_p]),
-    "dsk_batch_hard_triplet_bwd_rows": (c_int32, [c_void_p] * 6 + [c_int32] * 4 + [c_float] + [c_void_p] * 3),
-    "dsk_aam_softmax": (c_int32, [c_void_p] * 4 + [c_int32] * 3 + [c_float, c_float] + [c_void_p] * 4),
-    "dsk_aam_softmax_bwd": (c_int32, [c_void_p] * 6 + [c_int32] * 3 + [c_float, c_float] + [c_void_p] * 4),
-    "dsk_aam_softmax_sc": (c_int32, [c_void_p] * 4 + [c_int32] * 4 + [c_float, c_float, c_int32, c_float]
-                           + [c_void_p] * 6),
-    "dsk_aam_softmax_sc_bwd": (c_int32, [c_void_p] * 8 + [c_int32] * 4 + [c_float, c_float, c_int32, c_float]
-                               + [c_void_p] * 4),
-    "dsk_aam_subcentre_cos": (c_int32, [c_void_p] * 3 + [c_int32] * 4 + [c_void_p] * 2),
-    "dsk_aam_shard_cos": (c_int32, [c_void_p] * 4 + [c_int32] * 7 + [c_void_p] * 4),
-    "dsk_aam_shard_merge": (c_int32, [c_void_p] * 3 + [c_int32] * 6 + [c_float] * 3 + [c_void_p] * 4),
-    "dsk_aam_shard_partials": (c_int32, [c_void_p] * 4 + [c_int32] * 7 + [c_float] * 3 + [c_void_p] * 3),
-    "dsk_aam_shard_finish": (c_int32, [c_void_p] * 3 + [c_int32] * 4 + [c_void_p] * 5),
-    "dsk_aam_shard_bwd": (c_int32, [c_void_p] * 9 + [c_int32] * 6 + [c_float, c_float, c_int32, c_float]
-                          + [c_void_p] * 4),
-    "dsk_aam_shard_bwd_rows": (c_int32, [c_void_p] * 2 + [c_int32] * 3 + [c_void_p] * 2),
-    "dsk_ge2e": (c_int32, [c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 3 + [c_int32, c_int32] + [c_void_p] * 2
-                 + [c_int32] + [c_void_p] * 4),
-    "dsk_ge2e_bwd": (c_int32, [c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 3 + [c_int32, c_int32]
-                     + [c_void_p] * 2 + [c_int32] + [c_void_p] * 7),
-    "dsk_ge2e_rows": (c_int32, [c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 3 + [c_int32, c_int32]
-                      + [c_void_p] * 2 + [c_int32] * 3 + [c_void_p] * 4),
-    "dsk_ge2e_mean": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p]),
-    "dsk_ge2e_dcos_rows": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p,
-                                     c_void_p, c_int32, c_void_p, c_int32, c_int32] + [c_void_p] * 5),
-    "dsk_ge2e_bwd_rows": (c_int32, [c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 3 + [c_int32]
-                          + [c_void_p] * 2 + [c_int32] * 2 + [c_void_p] * 2),
-    "dsk_cosine_matrix": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_void_p]),
-    "dsk_topk_mean_std": (c_int32, [c_void_p, c_int32, c_int32, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
-    "dsk_cohort_stats": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_int32] + [c_void_p] * 3),
-    "dsk_score_trials": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_int64] + [c_void_p] * 5),
-    "dsk_topk_indices": (c_int32, [c_void_p, c_int32, c_int32, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
-    "dsk_cosine_topk": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_int32, c_int32] + [c_void_p] * 3),
-    "dsk_class_centroids": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),
-    "dsk_ahc": (c_int32, [c_void_p, c_int32, c_int64, c_int32, c_int32, c_double, c_void_p, POINTER(c_int32), c_void_p,
-                          POINTER(c_int32), c_void_p]),
-    "dsk_spectral_cluster": (c_int32, [c_void_p, c_int32, c_int64, c_void_p, c_int32, c_int32, c_int32, c_int32]
-                             + [c_void_p] * 8),
-    "dsk_class_sums_f64": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
-                                     c_void_p]),
-    "dsk_gram_f64": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p]),
-    "dsk_affine_norm_f64": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_void_p,
-                                      c_void_p, c_void_p, c_void_p]),
-    "dsk_plda_score_trials": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_int64, c_void_p,
-                                        c_void_p]),
-    "dsk_plda_score_matrix": (c_int32, [c_void_p, c_int32, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_int64,
-                                        c_void_p]),
-    "dsk_vbx": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_double, c_double,
-                          c_double, c_double, c_int32, c_double] + [c_void_p] * 6),
-    "dsk_linear_forward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
-    "dsk_linear_backward": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p,
-                                      c_void_p, c_void_p]),
-    "dsk_cross_entropy": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "dsk_cross_entropy_bwd": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p]),
-    "dsk_adagrad_step": (c_int32, [c_void_p, c_void_p, c_void_p, c_int64, c_double, c_double, c_double, c_double,
-                                   c_int64, c_float, c_void_p, c_void_p]),
-    "dsk_set_defer_running_stats": (c_int32, [c_void_p, c_int32]),
-    "dsk_train_ctx_commit_stats": (c_int32, [c_void_p, c_void_p, c_void_p]),
-    "dsk_pipeline_create": (c_int32, [POINTER(c_void_p), c_void_p, c_int32, c_int32]),
-    "dsk_pipeline_destroy": (c_int32, [c_void_p]),
-    "dsk_pipeline_submit": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, POINTER(c_int64)]),
-    "dsk_pipeline_submit_device": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p, POINTER(c_int64)]),
-    "dsk_pipeline_join": (c_int32, [c_void_p, c_void_p]),
-    "dsk_pipeline_wait": (c_int32, [c_void_p, c_int64]),
-    "dsk_pipeline_sync": (c_int32, [c_void_p]),
-    "dsk_pipeline_lane_stream": (c_int32, [c_void_p, c_int32, POINTER(c_void_p)]),
-    "dsk_fbank_num_frames": (c_int64, [c_int64, c_int32]),
-    "dsk_fbank": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
-    "dsk_fbank_frame_offsets": (c_int32, [c_void_p, c_int32, c_int32, c_void_p]),
-    "dsk_fbank_batch": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]),
-    "dsk_fbank_crops": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int32,
-                                  c_void_p, c_int32, c_void_p, c_void_p]),
-    "dsk_fbank_batch_vad": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_double, c_double,
-                                      c_int32, c_double, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "dsk_frame_runs": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int64, c_int64, c_void_p,
-                                 c_void_p, c_void_p, c_void_p]),
-    "dsk_gather_runs": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p,
-                                  c_void_p]),
-    "dsk_fbank_filterbank": (c_int32, [c_int32, c_void_p]),
-    "dsk_wave_augment": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p,
-                                   c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_int32] + [c_void_p] * 5),
-    "dsk_speed_filter": (c_int32, [c_int32, c_int32, c_void_p]),
-    "dsk_wave_augment_speed": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p,
-                                         c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_int32]
-                               + [c_void_p] * 5 + [c_int32] + [c_void_p] * 3),
-    "dsk_fbank_segments": (c_int32, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_int32,
-                                     c_void_p, c_int32, c_void_p, c_void_p]),
-    "dsk_threshold_counts": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
-}
+with open(HEADER) as _f:
+    CONSTANTS, STRUCTS, PROTOTYPES = read_header(_f.read())
+globals().update(CONSTANTS)
+globals().update({s.__name__: s for s in STRUCTS.values()})
 
 _lib = None
 
@@ -300,7 +186,7 @@ def load() -> ctypes.CDLL:
             warnings.warn(f"libdsk.so was built from DIFFERENT sources than csrc/ and the rebuild failed ({e}); "
                           f"loading the stale library (set DSK_STRICT_BUILD=1 to make this an error)", RuntimeWarning)
     lib = ctypes.CDLL(LIB_PATH)
-    for name, (res, args) in SIGNATURES.items():
+    for name, (res, args) in PROTOTYPES.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported
         fn.restype = res
         fn.argtypes = args

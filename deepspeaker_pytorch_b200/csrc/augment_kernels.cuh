@@ -12,10 +12,12 @@
 #pragma once
 #include <stdint.h>
 
+#include "../../include/dsk.h"
+
 namespace dsk {
 
-constexpr int kAugMaxSources = 8;      // DSK_AUG_MAX_SOURCES
-constexpr int kAugMaxRir = 65536;      // DSK_AUG_MAX_RIR
+constexpr int kAugMaxSources = DSK_AUG_MAX_SOURCES;
+constexpr int kAugMaxRir = DSK_AUG_MAX_RIR;
 constexpr int kAugPart = 1024;         // partition length P
 constexpr int kAugFft = 2 * kAugPart;  // N = 2P-point complex FFT
 constexpr int kAugLogFft = 11;
@@ -24,9 +26,9 @@ constexpr int kAugFftThreads = 512;
 constexpr int kAugGatherThreads = 256;
 constexpr int kAugGatherPerBlock = 4 * kAugGatherThreads;
 constexpr int kAugMixThreads = 256;
-constexpr int kSpeedMaxDen = 32;                 // DSK_SPEED_MAX_DEN
-constexpr int kSpeedTaps = 50;                   // DSK_SPEED_TAPS: d = -24 .. 25
-constexpr int kSpeedMaxFactors = 8;              // DSK_SPEED_MAX_FACTORS
+constexpr int kSpeedMaxDen = DSK_SPEED_MAX_DEN;
+constexpr int kSpeedTaps = DSK_SPEED_TAPS;       // d = -24 .. 25
+constexpr int kSpeedMaxFactors = DSK_SPEED_MAX_FACTORS;
 constexpr int kSpeedTapStride = 51;              // odd, so rows of different phases start in different bank pairs
 constexpr int kSpeedMaxSpan = 2 * (kAugGatherPerBlock - 1) + 1 + kSpeedTaps;   // inputs of one tile at alpha = 2
 

@@ -3259,7 +3259,7 @@ int32_t dsk_topk_indices(const float* S, int32_t rows, int32_t cols, int64_t ld,
 }
 
 // Gallery columns per search chunk: every selection runs on a row staged in shared memory
-static_assert(dsk::kSearchMaxK == DSK_SEARCH_MAX_K && dsk::kSearchMaxK <= dsk::kTopkStageCols,
+static_assert(dsk::kSearchMaxK <= dsk::kTopkStageCols,
               "the first gallery chunk holds at least k columns");
 
 int32_t dsk_cosine_topk(dsk_handle h, const float* Q, int32_t M, const float* G, int32_t Ng, int32_t D, int32_t k,

@@ -10,6 +10,8 @@
 #pragma once
 #include <stdint.h>
 
+#include "../../include/dsk.h"
+
 namespace dsk {
 
 constexpr int kTopkThreads = 256;       // one CTA per row
@@ -189,7 +191,7 @@ score_trials_kernel(const float* __restrict__ X, int U, int D, const int64_t* __
 // ---- identification: exact top-k with indices, the merge of two sorted lists, class centroids ----------------------
 // The search order: a ranks above b <=> skey(a) > skey(b), or the keys are equal and a has the lower column.  -0 is
 // taken as +0 and every NaN ranks below every number (-inf included).
-constexpr int kSearchMaxK = 1024;  // DSK_SEARCH_MAX_K
+constexpr int kSearchMaxK = DSK_SEARCH_MAX_K;
 
 // Order-preserving key of the search: score_key for numbers (-inf has 0x007fffff), 0 for every NaN
 __device__ __forceinline__ uint32_t search_key(float x) {

@@ -52,23 +52,20 @@ def _ptr64(a):
     return a.ctypes.data_as(ctypes.c_void_p)
 
 
-# The rates the front-end frames: a 10 ms step of at least one sample and a 25 ms frame within NFFT = 512 (dsk.h)
-FBANK_MIN_RATE, FBANK_MAX_RATE = 50, 20499
-
-
 def _fbank_step(sample_rate, what="fbank"):
-    """(flen, step) of ``sample_rate``; ValueError unless it is an integer in [FBANK_MIN_RATE, FBANK_MAX_RATE]."""
+    """(flen, step) of ``sample_rate``; ValueError unless it is an integer in
+    [DSK_FBANK_MIN_RATE, DSK_FBANK_MAX_RATE]."""
     sr = float(sample_rate)
-    if not sr.is_integer() or not FBANK_MIN_RATE <= sr <= FBANK_MAX_RATE:
-        raise ValueError(f"{what}: sample_rate must be an integer in [{FBANK_MIN_RATE}, {FBANK_MAX_RATE}] Hz (a 10 ms "
-                         f"step of at least one sample, a 25 ms frame of at most 512), got {sample_rate}")
+    if not sr.is_integer() or not L.DSK_FBANK_MIN_RATE <= sr <= L.DSK_FBANK_MAX_RATE:
+        raise ValueError(f"{what}: sample_rate must be an integer in [{L.DSK_FBANK_MIN_RATE}, {L.DSK_FBANK_MAX_RATE}] Hz "
+                         f"(a 10 ms step of at least one sample, a 25 ms frame of at most 512), got {sample_rate}")
     return int(np.floor(0.025 * sr + 0.5)), int(np.floor(0.01 * sr + 0.5))
 
 
 def fbank_frame_offsets(lengths, sample_rate: int = 16000) -> np.ndarray:
     """Host only: frame offsets (U + 1,) int64 of utterances of ``lengths`` samples; utterance u gets
     ``dsk_fbank_num_frames(lengths[u], sample_rate)`` frames.  ValueError for an empty list, a length outside
-    [1, 2^31) or a sample rate outside [FBANK_MIN_RATE, FBANK_MAX_RATE]."""
+    [1, 2^31) or a sample rate outside [DSK_FBANK_MIN_RATE, DSK_FBANK_MAX_RATE]."""
     _fbank_step(sample_rate, "fbank_frame_offsets")
     lens = _host_int64(lengths, "fbank_frame_offsets")
     if lens.size == 0:
@@ -115,7 +112,7 @@ def mk_mfb_batch(audio: torch.Tensor, lengths, sample_rate: int = 16000, use_log
     -> ``(feats (F, 64) fp32 CUDA, offsets (U + 1,) int64 CPU)``: rows ``offsets[u]:offsets[u+1]`` are utterance u's,
     bit-identical to ``mk_mfb`` on that waveform alone.  One launch sequence and one host synchronisation per call.
     RuntimeError for a CPU tensor; ValueError for a zero length, lengths that do not add up to ``audio`` or a sample
-    rate outside [FBANK_MIN_RATE, FBANK_MAX_RATE] = [50, 20499] Hz, before any launch."""
+    rate outside [DSK_FBANK_MIN_RATE, DSK_FBANK_MAX_RATE] = [50, 20499] Hz, before any launch."""
     return _fbank_batch(audio, lengths, sample_rate, use_logscale, subtract_mean, None, "mk_mfb_batch")
 
 
@@ -443,16 +440,12 @@ def _filterbank(dev, sample_rate: int) -> torch.Tensor:
 
 def segment_samples(T: int, sample_rate: int = 16000) -> int:
     """Samples L = flen + (T - 1) step of a segment whose log-fbank has exactly T frames (25 840 at 16 kHz, T = 160).
-    ValueError for a sample rate outside [FBANK_MIN_RATE, FBANK_MAX_RATE] = [50, 20499] Hz."""
+    ValueError for a sample rate outside [DSK_FBANK_MIN_RATE, DSK_FBANK_MAX_RATE] = [50, 20499] Hz."""
     flen, step = _fbank_step(sample_rate, "segment_samples")
     return flen + (int(T) - 1) * step
 
 
 # ---- waveform augmentation ---------------------------------------------------------------------------------------------
-AUG_MAX_SOURCES = 8
-AUG_MAX_RIR = 65536
-
-
 def _bank_samples(samples, dtype, what):
     if not isinstance(samples, torch.Tensor) or samples.dim() != 1 or samples.dtype != dtype or samples.numel() == 0:
         raise ValueError(f"{what}: expected a non-empty 1-D {dtype} tensor")
@@ -566,8 +559,8 @@ class WaveBank:
                     or snr.shape != noise_idx.shape:
                 raise ValueError(f"segments: noise_idx, noise_start, snr_db must be (B, M) with B = {B}")
             M = int(noise_idx.shape[1])
-            if M > AUG_MAX_SOURCES:
-                raise ValueError(f"segments: at most {AUG_MAX_SOURCES} noise sources, got {M}")
+            if M > _lib.DSK_AUG_MAX_SOURCES:
+                raise ValueError(f"segments: at most {_lib.DSK_AUG_MAX_SOURCES} noise sources, got {M}")
             if M and noise_bank is None:
                 raise ValueError("segments: the plan adds noise but no noise_bank is given")
         speed_idx, K = plan.get("speed_idx"), 0
@@ -632,7 +625,8 @@ class WaveBank:
         """(B, 1, T, 64) fp32 training input: ``mk_mfb`` of each augmented segment of ``segment_samples(T)`` samples
         (``segments``), the mean subtracted over the segment's own T frames, then the SpecAugment masks exactly as
         ``FeatureBank.crops`` applies them.  ``start`` counts samples.  No host synchronisation once the filterbank of
-        ``sample_rate`` is on the device.  ValueError for a sample rate outside [FBANK_MIN_RATE, FBANK_MAX_RATE]."""
+        ``sample_rate`` is on the device.  ValueError for a sample rate outside
+        [DSK_FBANK_MIN_RATE, DSK_FBANK_MAX_RATE]."""
         _fbank_step(sample_rate, "augmented_crops")
         Ls = segment_samples(T, sample_rate)
         if T < 1 or L.load().dsk_fbank_num_frames(Ls, int(sample_rate)) != T:
@@ -659,8 +653,8 @@ class RirBank:
         self.samples = _bank_samples(samples, torch.float32, "RirBank")
         off = _bank_offsets(offsets, self.samples.numel(), "RirBank")
         self.lengths = np.diff(off)
-        if self.lengths.max() > AUG_MAX_RIR:
-            raise ValueError(f"RirBank: a RIR has {self.lengths.max()} taps, more than {AUG_MAX_RIR}")
+        if self.lengths.max() > L.DSK_AUG_MAX_RIR:
+            raise ValueError(f"RirBank: a RIR has {self.lengths.max()} taps, more than {L.DSK_AUG_MAX_RIR}")
         self.max_len = int(self.lengths.max())
         self.device = _bank_device(self.samples, device)
         self.offsets = torch.from_numpy(off).to(self.device)
@@ -679,8 +673,8 @@ class RirBank:
             e = float(np.sqrt(np.sum(a * a))) if a.size else 0.0
             if a.size == 0 or not np.isfinite(e) or e == 0.0:
                 raise ValueError("RirBank.from_arrays: every RIR must be non-empty, finite and not all zero")
-            if a.size > AUG_MAX_RIR:
-                raise ValueError(f"RirBank.from_arrays: a RIR has {a.size} taps, more than {AUG_MAX_RIR}")
+            if a.size > L.DSK_AUG_MAX_RIR:
+                raise ValueError(f"RirBank.from_arrays: a RIR has {a.size} taps, more than {L.DSK_AUG_MAX_RIR}")
             arrs.append((a / e).astype(np.float32))
         if not arrs:
             raise ValueError("RirBank.from_arrays: no RIRs")
@@ -728,9 +722,10 @@ def augment_plan(B: int, L: int, generator=None, rir_bank=None, p_reverb: float 
             raise ValueError("augment_plan: noise groups need a noise_bank")
         if ids.size == 0 or ids.min() < 0 or ids.max() >= noise_bank.num_utterances:
             raise ValueError(f"augment_plan: a group's utterances must be a non-empty subset of [0, {noise_bank.num_utterances})")
-        if not (1 <= clo <= chi <= AUG_MAX_SOURCES) or not (np.isfinite(slo) and np.isfinite(shi) and slo <= shi) or w < 0:
-            raise ValueError(f"augment_plan: need 1 <= count_lo <= count_hi <= {AUG_MAX_SOURCES}, finite snr_lo <= snr_hi "
-                             "and weight >= 0")
+        if not (1 <= clo <= chi <= _lib.DSK_AUG_MAX_SOURCES) or not (np.isfinite(slo) and np.isfinite(shi) and slo <= shi) \
+                or w < 0:
+            raise ValueError(f"augment_plan: need 1 <= count_lo <= count_hi <= {_lib.DSK_AUG_MAX_SOURCES}, finite "
+                             "snr_lo <= snr_hi and weight >= 0")
         groups.append((ids, float(slo), float(shi), int(clo), int(chi), float(w)))
     if p_reverb > 0 and rir_bank is None:
         raise ValueError("augment_plan: p_reverb > 0 needs a rir_bank")
@@ -763,11 +758,6 @@ def augment_plan(B: int, L: int, generator=None, rir_bank=None, p_reverb: float 
 
 
 # ---- speed perturbation ------------------------------------------------------------------------------------------------
-SPEED_MAX_DEN = 32
-SPEED_TAPS = 50
-SPEED_MAX_FACTORS = 8
-
-
 def speed_factor(a) -> Fraction:
     """The exact ratio of a speed factor: a float through its shortest decimal form (0.9 -> 9/10), an int or a
     ``Fraction`` as is.  ValueError unless 1/2 <= alpha <= 2 with a denominator of at most 32."""
@@ -779,8 +769,8 @@ def speed_factor(a) -> Fraction:
         f = Fraction(str(float(a)))
     else:
         f = Fraction(a)
-    if not (Fraction(1, 2) <= f <= 2) or f.denominator > SPEED_MAX_DEN:
-        raise ValueError(f"speed factor {a} = {f}: need 1/2 <= p / q <= 2 and q <= {SPEED_MAX_DEN}")
+    if not (Fraction(1, 2) <= f <= 2) or f.denominator > L.DSK_SPEED_MAX_DEN:
+        raise ValueError(f"speed factor {a} = {f}: need 1/2 <= p / q <= 2 and q <= {L.DSK_SPEED_MAX_DEN}")
     return f
 
 
@@ -788,15 +778,15 @@ def _speed_factors(speeds, what):
     if speeds is None:
         raise ValueError(f"{what}: speed_idx needs the plan's speeds")
     out = tuple(speed_factor(a) for a in speeds)
-    if not 1 <= len(out) <= SPEED_MAX_FACTORS:
-        raise ValueError(f"{what}: need 1 .. {SPEED_MAX_FACTORS} speed factors, got {len(out)}")
+    if not 1 <= len(out) <= L.DSK_SPEED_MAX_FACTORS:
+        raise ValueError(f"{what}: need 1 .. {L.DSK_SPEED_MAX_FACTORS} speed factors, got {len(out)}")
     return out
 
 
 def speed_filter(alpha) -> np.ndarray:
     """Host: the (q, 50) fp32 polyphase taps of the factor alpha = p / q (``dsk_speed_filter``)."""
     f = speed_factor(alpha)
-    taps = np.empty((f.denominator, SPEED_TAPS), np.float32)
+    taps = np.empty((f.denominator, L.DSK_SPEED_TAPS), np.float32)
     L.check(L.load().dsk_speed_filter(f.numerator, f.denominator, taps.ctypes.data_as(ctypes.c_void_p)),
             "dsk_speed_filter")
     return taps
@@ -811,7 +801,7 @@ def _speed_table(dev, speeds):
     key = (dev.index, tuple(speeds))
     if key not in _SPEED_CACHE:
         ratio = np.array([[a.numerator, a.denominator] for a in speeds], np.int32)
-        taps = np.zeros((len(speeds), SPEED_MAX_DEN, SPEED_TAPS), np.float32)
+        taps = np.zeros((len(speeds), L.DSK_SPEED_MAX_DEN, L.DSK_SPEED_TAPS), np.float32)
         for k, a in enumerate(speeds):
             taps[k, :a.denominator] = speed_filter(a)
         _SPEED_CACHE[key] = (torch.from_numpy(ratio).to(dev), torch.from_numpy(taps).to(dev))

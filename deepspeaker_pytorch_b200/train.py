@@ -85,7 +85,7 @@ def _forward_one(engine, x, params, need_grad):
 def _grads_struct(views):
     """The ``dsk_grads`` output pointers of a backward: the 38 gradient tensors in ``_train_params`` order."""
     g = L.DskGrads()
-    for i in range(L.NUM_CONV):
+    for i in range(L.DSK_NUM_CONV):
         g.conv_w[i] = views[3 * i].data_ptr()
         g.bn_gamma[i] = views[3 * i + 1].data_ptr()
         g.bn_beta[i] = views[3 * i + 2].data_ptr()

@@ -197,7 +197,7 @@ def test_sample_rates_outside_50_to_20499_are_rejected_by_every_entry_point():
 
 
 @pytest.mark.parametrize("sr", [50, 20499])
-def test_sample_rates_at_the_ends_of_the_range_are_accepted(sr):
+def test_sample_rates_at_the_ends_of_the_header_range_are_accepted(sr):
     lib = L.load()
     flen, step = FB.geometry(sr)
     assert (flen, step) == {50: (1, 1), 20499: (512, 205)}[sr]
@@ -212,4 +212,5 @@ def test_sample_rates_at_the_ends_of_the_range_are_accepted(sr):
     assert lib.dsk_fbank_num_frames(F.segment_samples(160, sr), sr) == 160
     # the range is exactly the rates with a step of at least one sample and a frame of at most 512
     ok = [r for r in range(1, 30000) if FB.geometry(r)[1] >= 1 and FB.geometry(r)[0] <= 512]
-    assert (ok[0], ok[-1], len(ok)) == (F.FBANK_MIN_RATE, F.FBANK_MAX_RATE, F.FBANK_MAX_RATE - F.FBANK_MIN_RATE + 1)
+    assert (ok[0], ok[-1], len(ok)) == (L.DSK_FBANK_MIN_RATE, L.DSK_FBANK_MAX_RATE,
+                                        L.DSK_FBANK_MAX_RATE - L.DSK_FBANK_MIN_RATE + 1)
