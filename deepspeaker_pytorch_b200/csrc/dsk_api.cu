@@ -1950,6 +1950,30 @@ int32_t dsk_debug_backward_plan(dsk_handle h, dsk_train_ctx c, int32_t layer, in
   return DSK_OK;
 }
 
+int32_t dsk_debug_train_tiles(dsk_handle h, dsk_train_ctx c, int32_t layer, int32_t* out) {
+  int rc = check_handle(h);
+  if (rc) return rc;
+  if (!c || !c->B) return fail(DSK_ERR_STATE, "dsk_debug_train_tiles: context is not bound to a batch");
+  if (layer < 0 || layer >= DSK_NUM_CONV || !out) return fail(DSK_ERR_INVALID, "dsk_debug_train_tiles: bad arguments");
+  for (int k = 0; k < 6; ++k) out[k] = 0;
+  if (layer == 0) return DSK_OK;
+  const dsk::ConvParams& f = c->conv[layer].p;
+  for (int k = 0; k < c->n_dgrad[layer]; ++k) {  // built on the forward's output grid: the same box, or a bug
+    const dsk::ConvParams& d = c->dgrad[layer][k].p;
+    if (d.wt != f.wt || d.hb != f.hb || d.nb != f.nb)
+      return fail(DSK_ERR_STATE, "dsk_debug_train_tiles: layer %d data-gradient conv %d tiles %dx%dx%d, forward %dx%dx%d",
+                  layer, k, d.wt, d.hb, d.nb, f.wt, f.hb, f.nb);
+  }
+  const dsk::WgradParams& w = c->wgrad[layer].p;
+  out[0] = f.wt;
+  out[1] = f.hb;
+  out[2] = f.nb;
+  out[3] = w.wt;
+  out[4] = w.hb;
+  out[5] = w.nb;
+  return DSK_OK;
+}
+
 int32_t dsk_debug_read_eval_activation(dsk_handle h, int32_t layer, void* dst, int64_t dst_bytes, int32_t* planar_out,
                                        void* stream) {
   int rc = check_handle(h);

@@ -144,6 +144,11 @@ int32_t dsk_train_ctx_read(dsk_handle h, dsk_train_ctx ctx, int32_t which, int32
  * out[2] = partial-sum blocks per 64-channel group of the BatchNorm reductions (forward statistics and backward sums of
  * the unsynchronised path).  Host-only: no device work. */
 int32_t dsk_debug_backward_plan(dsk_handle h, dsk_train_ctx ctx, int32_t layer, int32_t* out);
+/* Debug / test: the 128-pixel boxes (width, rows, utterances) the train convs of `ctx` (as bound by its last forward) tile
+ * conv layer `layer` (1..11) with: out[0..2] = (wt, hb, nb) of the forward conv and of its data-gradient convs (built
+ * on the same output grid; DSK_ERR_STATE if one is not), out[3..5] = (wt, hb, nb) of the weight-gradient GEMM's K
+ * chunks.  All six 0 for conv1, which is not tiled.  Host-only: no device work. */
+int32_t dsk_debug_train_tiles(dsk_handle h, dsk_train_ctx ctx, int32_t layer, int32_t* out);
 /* Debug / test read-back: activation `layer` (0..11: output of conv `layer` after BN, residual and clip) of this handle's
  * most recent dsk_rescnn_forward, byte for byte as stored: 16-bit zero-padded NHWC (dsk_padded_positions(B,H,W) * C),
  * or parity-planar (4 planes of dsk_padded_positions(B,H/2,W/2) * C) for the block outputs that feed a stride-2 conv.

@@ -32,6 +32,7 @@ from oracle import rescnn_oracle as O
 from tests.test_gpu_forward import _fresh_model
 from tests.test_gpu_halo_conv import from_padded, from_planar
 from tests.test_gpu_train_parity import read_saved_activations
+from tests.train_plan import reduce_chain, stat_blocks
 
 U = {"fp16": 2.0 ** -11, "bf16": 2.0 ** -8}         # unit roundoff of the 16-bit storage
 TD = {"fp16": torch.float16, "bf16": torch.bfloat16}
@@ -150,24 +151,39 @@ def batch_stats(raw):
     return mean, var
 
 
-def stat_eps(mean, var):
-    """Error of the engine's batch mean (relative to std) and variance (relative to var) per channel: fp32 chains of at
-    most 64 additions (2^-18 = 64 * 2^-24) of terms up to (mean^2 + var) in size.  The engine sums x itself while
-    mean^2 <= 1024 var and x - pivot beyond that (bn_finalize_kernel), so mean^2 / var counts up to 1024."""
-    return 2.0 ** -18 * (2 + (mean * mean / var.clamp_min(1e-300)).clamp(max=1024))
+def stat_eps(mean, var, n):
+    """Error of the engine's batch mean (relative to std) and variance (relative to var) per channel: fp32 chains of n
+    additions (n 2^-24; stat_chains gives n per layer) of terms up to (mean^2 + var) in size.  The engine sums x itself
+    while mean^2 <= 1024 var and x - pivot beyond that (bn_finalize_kernel; the synchronised records always sum around
+    each utterance's first pixel), so mean^2 / var counts up to 1024."""
+    return n * 2.0 ** -24 * (2 + (mean * mean / var.clamp_min(1e-300)).clamp(max=1024))
 
 
-def running_stats_check(name, rm0, rv0, rm1, rv1, mean, var, M):
-    """Running statistics after one train forward against the fp64 momentum update (unbiased variance)."""
+def running_stats_check(name, rm0, rv0, rm1, rv1, mean, var, M, n):
+    """Running statistics after one train forward against the fp64 momentum update (unbiased variance); n: the length
+    of the reductions' fp32 chains."""
     unb = var * M / max(M - 1, 1)
-    eps = stat_eps(mean, var)
+    eps = stat_eps(mean, var, n)
     em = 0.9 * rm0 + 0.1 * mean
     ev = 0.9 * rv0 + 0.1 * unb
     tm = 2.0 ** -22 * (rm0.abs() + mean.abs()) + 0.1 * eps * var.sqrt() + 1e-30
     tv = 2.0 ** -22 * (rv0.abs() + unb) + 0.1 * eps * unb + 1e-30
     r = max(((rm1 - em).abs() / tm).max().item(), ((rv1 - ev).abs() / tv).max().item())
-    print(f"  {name:<12} running stats max err/bound {r:.3f}")
+    print(f"  {name:<12} running stats max err/bound {r:.3f} (chains of {n})")
     return r
+
+
+def stat_chains(eng, tctx, B, T, sync):
+    """Per layer, the longest fp32 chain of the BatchNorm reductions of the forward (and backward) `tctx` is bound to:
+    the unsynchronised path's partial-block count gx as the library planned it (dsk_debug_backward_plan), or the
+    synchronised path's per-utterance records."""
+    out = []
+    for i in range(12):
+        C, H, W = act_geometry(i, T)
+        v = (ctypes.c_int32 * 3)()
+        L.check(eng.lib.dsk_debug_backward_plan(eng.handle, tctx, i, v), "dsk_debug_backward_plan")
+        out.append(reduce_chain(B * H * W, H * W, v[2], sync))
+    return out
 
 
 # ---- eval chain ---------------------------------------------------------------------------------------------------
@@ -295,44 +311,51 @@ def test_eval_chain_layer_by_layer_kernel_by_kernel(cuda_dev, dt, B, T):
 
 
 # ---- train chain --------------------------------------------------------------------------------------------------
-def check_train_chain(tag, sd, dt, x, raw, y, emb, rm0, rv0, rm1, rv1):
+def check_train_chain(tag, sd, dt, x, raw, y, emb, rm0, rv0, rm1, rv1, chains):
     """raw[0] against fp64 conv1 of x, raw[i] against fp64 conv(y[i-1], w16), y[i] against the clipped BatchNorm of the
-    engine's raw[i] with fp64 batch statistics (+ y[i-2]), the running statistics, and the tail."""
+    engine's raw[i] with fp64 batch statistics (+ y[i-2]), the running statistics, and the tail.  chains[i]: the length
+    of layer i's BatchNorm reduction chains (stat_chains).  Each layer's fp64 tensors are dropped before the next."""
     u = U[dt]
     dev = x.device
     one = lambda C: torch.ones(C, dtype=torch.float64, device=dev)
     zero = lambda C: torch.zeros(C, dtype=torch.float64, device=dev)
-    rw = [raw[i].double() for i in range(12)]
-    yy = [y[i].double() for i in range(12)]
     print(f"[{tag}]")
     worst_stats = 0.0
     for i in range(12):
         wkey, prefix, k, stride = CONV[i]
-        C = rw[i].shape[1]
+        rw, yy = raw[i].double(), y[i].double()
+        C = rw.shape[1]
         w = sd[wkey].to(dev).double()
-        a = x.double() if i == 0 else yy[i - 1]
+        a = x.double() if i == 0 else y[i - 1].double()
         ref, bound = conv_ref(a, w if i == 0 else rn16(w, dt), one(C), zero(C), zero(C), None, stride, k // 2, 0.0,
                               tiny=1e-30)
-        assert_layer(f"raw {i}", rw[i], ref, bound, saturating=False)
-        mean, var = batch_stats(rw[i])
+        del a
+        assert_layer(f"raw {i}", rw, ref, bound, saturating=False)
+        del ref, bound
+        mean, var = batch_stats(rw)
         g, be = sd[prefix + ".weight"].to(dev).double(), sd[prefix + ".bias"].to(dev).double()
         v = lambda t: t.view(1, -1, 1, 1)
         sc = g / torch.sqrt(var + O.BN_EPS)
-        xhat = (rw[i] - v(mean)) / v(torch.sqrt(var + O.BN_EPS))
+        xhat = (rw - v(mean)) / v(torch.sqrt(var + O.BN_EPS))
         pre = v(g) * xhat + v(be)
-        side = (rw[i] * v(sc)).abs() + v((mean * sc).abs() + be.abs())
+        side = (rw * v(sc)).abs() + v((mean * sc).abs() + be.abs())
         if i % 3 == 2:
-            pre = pre + yy[i - 2]
-            side = side + yy[i - 2].abs()
+            res = y[i - 2].double()
+            pre = pre + res
+            side = side + res.abs()
+            del res
         ref = pre.clamp(0, 20)
+        del pre
         # fp32 scale / shift and their fused multiply-add, then the batch statistics' own error
-        delta = 2.0 ** -21 * side + v(stat_eps(mean, var) * g.abs()) * (1 + xhat.abs())
-        assert_layer(f"y {i}", yy[i], ref, u * (ref.abs() + delta) + TINY + delta)
-        M = rw[i].numel() // C
+        delta = 2.0 ** -21 * side + v(stat_eps(mean, var, chains[i]) * g.abs()) * (1 + xhat.abs())
+        del side, xhat
+        assert_layer(f"y {i}", yy, ref, u * (ref.abs() + delta) + TINY + delta)
+        del ref, delta, rw, yy
+        M = raw[i].numel() // C
         worst_stats = max(worst_stats, running_stats_check(f"bn {i}", rm0[i].double(), rv0[i].double(), rm1[i].double(),
-                                                           rv1[i].double(), mean, var, M))
+                                                           rv1[i].double(), mean, var, M, chains[i]))
     assert worst_stats <= 1.0, f"{tag}: running statistics off by {worst_stats:.3g} x their bound"
-    eref, ebound = tail_ref(yy[11], sd["model.fc.weight"].to(dev), sd["model.fc.bias"].to(dev))
+    eref, ebound = tail_ref(y[11].double(), sd["model.fc.weight"].to(dev), sd["model.fc.bias"].to(dev))
     msg, _, _ = check("tail", emb.detach().double().view(*eref.shape, 1, 1), eref.view(*eref.shape, 1, 1),
                       ebound.view(*eref.shape, 1, 1), saturating=False)
     assert msg is None, f"{tag} tail: {msg}"
@@ -348,7 +371,8 @@ def train_forward_and_check(tag, m, sd, dt, x, T):
     torch.cuda.synchronize()
     rm1 = [bn.running_mean.detach().clone() for bn in bns]
     rv1 = [bn.running_var.detach().clone() for bn in bns]
-    check_train_chain(tag, sd, dt, x, raw, y, emb, rm0, rv0, rm1, rv1)
+    chains = stat_chains(m._engine, emb.grad_fn.guard.tctx, x.shape[0], T, sync=False)
+    check_train_chain(tag, sd, dt, x, raw, y, emb, rm0, rv0, rm1, rv1, chains)
     return emb
 
 
@@ -468,12 +492,15 @@ def test_checker_pins_the_conv1_lo_half(lo):
         assert frac > 0.02
 
 
-def emulate_bn_stats(raw, pivot):
+def emulate_bn_stats(raw, pivot, gx=None, defect=None):
     """Batch mean / biased variance of an [M][C] fp32 tensor by bn_stats_partial_kernel + bn_finalize_kernel's
     summation order: per-thread fp32 chains over rows m = 32*bx + p + k*32*gx, a 32-term fp32 sum per block, the block
-    partials added in fp64.  pivot=False: the plain sums E[x^2] - mean^2; pivot=True: sums of x - x[0]."""
+    partials added in fp64.  pivot=False: the plain sums E[x^2] - mean^2; pivot=True: sums of x - x[0].  gx: the
+    partial blocks (default: the library's stat_blocks); defect "drop_block": the last block's partials are lost.
+    -> (mean, var, the chains' length)."""
     M, C = raw.shape
-    gx = max(1, min(592 // (C // 64), (M + 31) // 32))
+    if gx is None:
+        gx = stat_blocks(M, C)
     k = raw[0].astype(np.float32) if pivot else np.zeros(C, np.float32)
     n1 = -(-M // (32 * gx))
     pad = np.zeros((n1 * 32 * gx, C), np.float32)
@@ -493,24 +520,105 @@ def emulate_bn_stats(raw, pivot):
     for p in range(32):
         bs = (bs + s[:, p]).astype(np.float32)
         bss = (bss + ss[:, p]).astype(np.float32)
+    if defect == "drop_block":
+        bs, bss = bs[:-1], bss[:-1]
     S, SS = bs.astype(np.float64).sum(0), bss.astype(np.float64).sum(0)
     dm = S / M
-    return k.astype(np.float64) + dm, SS / M - dm * dm
+    return k.astype(np.float64) + dm, SS / M - dm * dm, reduce_chain(M, 0, gx, False)
 
 
-@pytest.mark.parametrize("pivot", [True, False])
-def test_checker_catches_unshifted_bn_statistics(pivot):
-    """Batch variance at mean/std 1000 (M = 128*80*32 rows): from unshifted fp32 sums the running-variance check fails,
-    from sums around a per-channel pivot it passes."""
-    g = np.random.RandomState(3)
-    M, C = 128 * 80 * 32, 64
-    raw = (g.standard_normal((M, C)) + 1000.0).astype(np.float32)
-    mean_e, var_e = emulate_bn_stats(raw, pivot)
+def emulate_record_stats(raw, N, defect=None):
+    """The synchronised path's statistics of N utterances of HW = M / N rows each (bn_utt_record_kernel +
+    bn_record_finalize_kernel): per utterance, fp32 sums of x - k_u (k_u its first row) by 32 lanes striding over the
+    rows, a 5-level tree over the lanes; the records combined in fp64 around K = k_0.  defect "drop_record": the last
+    utterance's record is lost.  -> (mean, var, the chains' length)."""
+    M, C = raw.shape
+    HW = M // N
+    u = raw.reshape(N, HW, C)
+    k = u[:, 0].astype(np.float32)                                  # (N, C)
+    n1 = -(-HW // 32)
+    pad = np.zeros((N, n1 * 32, C), np.float32)
+    pad[:, :HW] = u - k[:, None]
+    d = pad.reshape(N, n1, 32, C)                                   # lane p walks rows p, p + 32, ...
+    s = np.zeros((N, 32, C), np.float32)
+    ss = np.zeros((N, 32, C), np.float32)
+    for i in range(n1):
+        s = (s + d[:, i]).astype(np.float32)
+        ss = (ss + d[:, i] * d[:, i]).astype(np.float32)
+    half = 16
+    while half:
+        s = (s[:, :half] + s[:, half:2 * half]).astype(np.float32)
+        ss = (ss[:, :half] + ss[:, half:2 * half]).astype(np.float32)
+        half >>= 1
+    keep = N - 1 if defect == "drop_record" else N
+    sd, ssd = s[:keep, 0].astype(np.float64), ss[:keep, 0].astype(np.float64)
+    dk = k[:keep].astype(np.float64) - k[0].astype(np.float64)
+    S1 = (sd + HW * dk).sum(0)
+    S2 = (ssd + 2 * dk * sd + HW * dk * dk).sum(0)
+    Mk = keep * HW
+    dm = S1 / Mk
+    return k[0].astype(np.float64) + dm, S2 / Mk - dm * dm, reduce_chain(M, HW, 0, True)
+
+
+# (how the statistics are summed, rows M, partial blocks gx or utterances N): the library's plan at 128 x 80 x 32 rows
+# (chains of 50), and chains of 400 and more: the unsynchronised reductions when M / gx is large, the synchronised records
+# of long utterances (2 x 12800 pixels)
+STAT_SETUPS = {"plain M=327680": ("blocks", 128 * 80 * 32, None), "plain M=47104 gx=4": ("blocks", 47104, 4),
+               "records N=2 HW=12800": ("records", 2 * 12800, 2)}
+
+
+def _emulated_stats(setup, raw, pivot, defect=None):
+    kind, _, arg = STAT_SETUPS[setup]
+    if kind == "records":
+        return emulate_record_stats(raw, arg, defect)
+    return emulate_bn_stats(raw, pivot, arg, defect)
+
+
+def _running_check(name, raw, mean_e, var_e, n):
+    M, C = raw.shape
     r64 = torch.from_numpy(raw.astype(np.float64))
     mean, var = r64.mean(0), r64.var(0, unbiased=False)
     rm0, rv0 = torch.zeros(C, dtype=torch.float64), torch.ones(C, dtype=torch.float64)
     unb_e = torch.from_numpy(var_e) * M / (M - 1)
     rm1 = (0.9 * rm0 + 0.1 * torch.from_numpy(mean_e)).float().double()
     rv1 = (0.9 * rv0 + 0.1 * unb_e).float().double()
-    r = running_stats_check(f"pivot={pivot}", rm0, rv0, rm1, rv1, mean, var, M)
+    return running_stats_check(name, rm0, rv0, rm1, rv1, mean, var, M, n)
+
+
+@pytest.mark.parametrize("pivot", [True, False])
+def test_checker_catches_unshifted_bn_statistics(pivot):
+    """Batch variance at mean/std 1000 (M = 128*80*32 rows, the library's gx: chains of 50): from unshifted fp32 sums
+    the running-variance check fails, from sums around a per-channel pivot it passes."""
+    unshifted_case("plain M=327680", pivot)
+
+
+@pytest.mark.parametrize("setup,pivot", [("plain M=47104 gx=4", True), ("plain M=47104 gx=4", False),
+                                         ("records N=2 HW=12800", True)])
+def test_checker_catches_unshifted_bn_statistics_at_long_chains(setup, pivot):
+    """The same at chains of 400 and more (the synchronised records always sum around a pivot)."""
+    assert unshifted_case(setup, pivot) >= 400
+
+
+def unshifted_case(setup, pivot):
+    g = np.random.RandomState(3)
+    M, C = STAT_SETUPS[setup][1], 64
+    raw = (g.standard_normal((M, C)) + 1000.0).astype(np.float32)
+    mean_e, var_e, n = _emulated_stats(setup, raw, pivot)
+    r = _running_check(f"pivot={pivot}", raw, mean_e, var_e, n)
     assert (r <= 1.0) == pivot, r
+    return n
+
+
+@pytest.mark.parametrize("setup", STAT_SETUPS)
+@pytest.mark.parametrize("defect", [None, "drop"])
+def test_checker_passes_long_bn_chains_and_catches_a_dropped_partial(setup, defect):
+    """Channels of mean/std from 0 to 30 (the plain sums) summed in fp32 by the kernels' order, at chains of 50 to 405
+    terms: within the n-dependent bound; with one partial block (synchronised: one utterance's record) lost, not."""
+    g = np.random.RandomState(5)
+    M, C = STAT_SETUPS[setup][1], 64
+    raw = (g.standard_normal((M, C)) * np.linspace(0.5, 2, C) + np.linspace(0, 30, C)).astype(np.float32)
+    kind = STAT_SETUPS[setup][0]
+    d = None if defect is None else ("drop_record" if kind == "records" else "drop_block")
+    mean_e, var_e, n = _emulated_stats(setup, raw, False, d)
+    r = _running_check(f"{setup} defect={defect}", raw, mean_e, var_e, n)
+    assert (r <= 1.0) == (defect is None), r

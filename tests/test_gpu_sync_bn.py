@@ -20,7 +20,7 @@ from deepspeaker_pytorch_b200.engine import conv_bn_modules
 from oracle import rescnn_oracle as O
 from tests.helpers import rel_l2
 from tests.test_gpu_backward_ops import TD, U
-from tests.test_gpu_layer_parity import check_train_chain
+from tests.test_gpu_layer_parity import check_train_chain, stat_chains
 
 pytestmark = pytest.mark.gpu
 
@@ -123,7 +123,8 @@ def test_one_shard_forward_passes_the_layer_checker(cuda_dev, dt, B, T):
     torch.cuda.synchronize()
     rm1 = [bn.running_mean.detach().clone() for _, bn in conv_bn_modules(m)]
     rv1 = [bn.running_var.detach().clone() for _, bn in conv_bn_modules(m)]
-    check_train_chain(f"sync {dt} B={B} T={T}", sd, dt, x, raw, y, emb, rm0, rv0, rm1, rv1)
+    chains = stat_chains(m._engine, tctx, B, T, sync=True)
+    check_train_chain(f"sync {dt} B={B} T={T}", sd, dt, x, raw, y, emb, rm0, rv0, rm1, rv1, chains)
 
 
 @pytest.mark.parametrize("dt", ["fp16", "bf16"])
