@@ -33,6 +33,7 @@
 #include "score_kernels.cuh"
 #include "simt_kernels.cuh"
 #include "spectral_kernels.cuh"
+#include "supcon_kernels.cuh"
 #include "train_kernels.cuh"
 #include "vbx_kernels.cuh"
 #include "wgrad_umma.cuh"
@@ -372,6 +373,7 @@ struct dsk_handle_s {
   AllpairsPlan allpairs;       // cached all-pairs Gram plan (the batch-hard and tensor-core top-k ops)
   AamPlan aam;                 // cached AAM-softmax plan (its own slot: a step may use both ops)
   Ge2ePlan ge2e;               // cached GE2E plan (its own slot: a step may sum the GE2E and AAM losses)
+  AamPlan supcon;              // cached supervised-contrastive plan: the AAM plan for (N, N, D), in a slot of its own
   ScorePlan score;             // cached cosine-scoring plan (its own slot: evaluation runs between training steps)
   ScorePlan search;            // cached gallery-search plan (its own slot: searches alternate with cohort statistics)
   bool use_graph = true;       // DSK_GRAPH=0: always launch the forward kernel by kernel
@@ -1066,6 +1068,7 @@ int32_t dsk_destroy(dsk_handle h) {
   h->allpairs.release();
   h->aam.release();
   h->ge2e.release();
+  h->supcon.release();
   h->score.release();
   h->search.release();
   cudaFree(h->ones);
@@ -3136,6 +3139,73 @@ int32_t dsk_ge2e_bwd(dsk_handle h, const float* E, int32_t N, int32_t D, const i
   rc = ge2e_dcos_run(cos, rec, offsets, col, P, V, w, b, method, grad_loss, 0, N, nullptr, G->tdc, gw, gb, G->part, G,
                      s);
   return rc ? rc : ge2e_bwd_rows_run(h, E, N, D, order, offsets, col, P, nullptr, G->tdc, 0, N, gE, s);
+}
+
+// ---- supervised-contrastive loss ----------------------------------------------------------------------------------
+static int supcon_check(dsk_handle h, bool ptrs_ok, int N, int D, int V, float tau, const char* what) {
+  if (!ptrs_ok || N < 2 || N > DSK_SUPCON_MAX_N || D < 64 || D % 64 || V < 1 || V > N || !std::isfinite(tau) ||
+      !(tau > 0.f))
+    return fail(DSK_ERR_INVALID, "%s: bad arguments (need non-null pointers, 2 <= N <= %d, D a positive multiple of 64, "
+                "1 <= V <= N and a finite tau > 0; got N %d, D %d, V %d, tau %g)", what, DSK_SUPCON_MAX_N, N, D, V, tau);
+  return check_handle(h);
+}
+
+// The handle's supervised-contrastive plan (the AAM plan for (N, N, D) in its own slot) and E's norms and operand
+// images, on both sides of its GEMMs (forward: row-major; backward: transposed)
+static int supcon_prep(dsk_handle h, const float* E, int N, int D, bool backward, cudaStream_t s, AamPlan** out) {
+  if (int rc = aam_plan(h, h->supcon, N, N, D, s, out)) return rc;
+  AamPlan& P = **out;
+  const CosRows a{E, N, P.Np, P.nrm_e, true, backward ? nullptr : P.ea, backward ? P.et : nullptr};
+  const CosRows b{E, N, P.Cp, P.nrm_e, false, backward ? nullptr : P.wb, backward ? P.wt : nullptr};
+  return cos_prep(D, &a, &b, s);
+}
+
+int32_t dsk_supcon(dsk_handle h, const float* E, const int64_t* labels, int32_t N, int32_t D, int32_t V, float tau,
+                   float* loss, float* cos, float* lse, void* stream) {
+  int rc = supcon_check(h, E && labels && loss && cos && lse, N, D, V, tau, "dsk_supcon");
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  AamPlan* P = nullptr;
+  if ((rc = supcon_prep(h, E, N, D, false, s, &P))) return rc;
+  for (const ConvLaunch& L : P->fwd)
+    if ((rc = launch_conv(L, s))) return rc;
+  dsk::supcon_rows_kernel<<<N, 256, 0, s>>>(P->gcos, P->Cp, E, D, labels, N, 1.0 / tau, cos, lse, P->row_loss);
+  KERNEL_CHECK();
+  dsk::mean_rows_kernel<<<1, 1024, 0, s>>>(P->row_loss, N, V, loss);
+  KERNEL_CHECK();
+  return DSK_OK;
+}
+
+int32_t dsk_supcon_bwd(dsk_handle h, const float* E, const int64_t* labels, const float* cos, const float* lse,
+                       int32_t N, int32_t D, int32_t V, float tau, const float* grad_loss, float* gE, void* stream) {
+  int rc = supcon_check(h, E && labels && cos && lse && grad_loss && gE, N, D, V, tau, "dsk_supcon_bwd");
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  AamPlan* P = nullptr;
+  if ((rc = supcon_prep(h, E, N, D, true, s, &P))) return rc;
+  dsk::supcon_dcos_kernel<<<P->Np, 256, 0, s>>>(cos, lse, labels, N, V, 1.0 / tau, grad_loss, P->Cp, P->dcos, P->da,
+                                                P->rinv);
+  KERNEL_CHECK();
+  dsk::aam_dcos_t_kernel<<<P->Cp / 32, 256, 0, s>>>(P->dcos, P->Np, P->Cp, P->dt, P->cinv);
+  KERNEL_CHECK();
+  for (const ConvLaunch& L : P->ge_gemm)  // dC E^
+    if ((rc = launch_conv(L, s))) return rc;
+  for (const ConvLaunch& L : P->gw_gemm)  // dC^T E^
+    if ((rc = launch_conv(L, s))) return rc;
+  // the two products un-scaled into parts [2][N][D] (dC E^ first), added in that order by the Jacobian kernel
+  const size_t nd = static_cast<size_t>(N) * D;
+  float* parts = nullptr;
+  CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&parts), 2 * nd * sizeof(float), s));
+  const unsigned grid = static_cast<unsigned>((nd + 255) / 256);
+  dsk::aam_shard_gpart_kernel<<<grid, 256, 0, s>>>(P->ge, P->sc, static_cast<size_t>(P->Np) * D, P->rinv, N, D, parts);
+  KERNEL_CHECK();
+  dsk::aam_shard_gpart_kernel<<<grid, 256, 0, s>>>(P->gw, P->sn, static_cast<size_t>(P->Cp) * D, P->cinv, N, D,
+                                                   parts + nd);
+  KERNEL_CHECK();
+  dsk::aam_shard_rows_bwd_kernel<<<(N + 7) / 8, 256, 0, s>>>(E, parts, 2, N, D, gE);
+  KERNEL_CHECK();
+  CUDA_TRY(cudaFreeAsync(parts, s));
+  return DSK_OK;
 }
 
 // ---- cosine scoring, cohort statistics (AS-norm) ------------------------------------------------------------------

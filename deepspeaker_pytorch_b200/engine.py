@@ -810,6 +810,70 @@ class GE2EFn(torch.autograd.Function):
 
 
 # ---------------------------------------------------------------------------------------------------
+# supervised-contrastive loss (NT-Xent with one label per utterance)
+# ---------------------------------------------------------------------------------------------------
+def _labels_on(labels, N, dev):
+    labels = torch.as_tensor(labels)
+    if labels.dtype.is_floating_point or labels.dtype == torch.bool:
+        raise ValueError(f"supervised-contrastive labels must be integers, got {labels.dtype}")
+    if labels.shape != (N,):
+        raise RuntimeError(f"expected labels of shape ({N},), got {tuple(labels.shape)}")
+    if not labels.is_cuda:   # a pageable copy would wait for the stream; a pinned one is queued like a kernel
+        return labels.to(torch.int64).contiguous().pin_memory().to(dev, non_blocking=True)
+    return labels.to(device=dev, dtype=torch.int64).contiguous()
+
+
+def supcon(E, labels, V, tau):
+    """dsk_supcon: (E, labels as the op read them, loss (1,), cos (N, N), lse (N,)) on E's device.  ``V`` is the number
+    of valid rows (``model.supcon_valid_count`` of the labels), ``tau`` the temperature."""
+    if not E.is_cuda:
+        raise RuntimeError("the supervised-contrastive loss needs CUDA tensors; there is no CPU fallback")
+    if E.dim() != 2:
+        raise RuntimeError(f"expected embeddings (N, D), got {tuple(E.shape)}")
+    E = E.detach().float().contiguous()
+    N, D = E.shape
+    dev = E.device
+    labels = _labels_on(labels, N, dev)
+    loss = torch.empty(1, device=dev, dtype=torch.float32)
+    cos = torch.empty(N, N, device=dev, dtype=torch.float32)
+    lse = torch.empty(N, device=dev, dtype=torch.float32)
+    with torch.cuda.device(dev):
+        L.check(L.load().dsk_supcon(_allpairs_handle(dev), E.data_ptr(), labels.data_ptr(), N, D, int(V), float(tau),
+                                    loss.data_ptr(), cos.data_ptr(), lse.data_ptr(), L.cur_stream()), "dsk_supcon")
+    return E, labels, loss, cos, lse
+
+
+def supcon_backward(E, labels, V, tau, cos, lse, grad_loss):
+    """dsk_supcon_bwd: gE (N, D) = d loss / d E scaled by the device scalar ``grad_loss``, from the forward's cos and
+    lse."""
+    N, D = E.shape
+    gl = grad_loss.float().reshape(1).contiguous()
+    gE = torch.empty_like(E)
+    with torch.cuda.device(E.device):
+        L.check(L.load().dsk_supcon_bwd(_allpairs_handle(E.device), E.data_ptr(), labels.data_ptr(), cos.data_ptr(),
+                                        lse.data_ptr(), N, D, int(V), float(tau), gl.data_ptr(), gE.data_ptr(),
+                                        L.cur_stream()), "dsk_supcon_bwd")
+    return gE
+
+
+class SupConFn(torch.autograd.Function):
+    """Supervised-contrastive loss over the batch's cosine matrix; the loss is a device scalar.  ``V`` and ``tau`` as in
+    ``supcon``."""
+
+    @staticmethod
+    def forward(ctx, E, labels, V, tau):
+        Ec, lab, loss, cos, lse = supcon(E, labels, V, tau)
+        ctx.save_for_backward(Ec, lab, cos, lse)
+        ctx.V, ctx.tau = V, tau
+        return loss.reshape(())
+
+    @staticmethod
+    def backward(ctx, gl):
+        E, lab, cos, lse = ctx.saved_tensors
+        return supcon_backward(E, lab, ctx.V, ctx.tau, cos, lse, gl), None, None, None
+
+
+# ---------------------------------------------------------------------------------------------------
 # cosine scoring and cohort statistics (AS-norm)
 # ---------------------------------------------------------------------------------------------------
 def _score_rows(X, what):

@@ -356,6 +356,53 @@ def batch_hard_valid_count(labels):
     return int(counts[counts >= 2].sum())
 
 
+def supcon_valid_count(labels):
+    """V, the number of valid rows of a supervised-contrastive loss, from the labels alone (host-side: no device sync
+    when the labels are a CPU tensor): rows whose label occurs at least twice.  Unlike ``batch_hard_valid_count`` a
+    batch of one label counts in full.  ValueError for non-integer labels."""
+    lab = torch.as_tensor(labels).detach().cpu().reshape(-1)
+    if lab.dtype.is_floating_point or lab.dtype == torch.bool:
+        raise ValueError(f"supervised-contrastive labels must be integers, got {lab.dtype}")
+    _, counts = torch.unique(lab, return_counts=True)
+    return int(counts[counts >= 2].sum())
+
+
+class SupConLoss:
+    """Supervised-contrastive loss (Khosla et al., "Supervised Contrastive Learning", NeurIPS 2020, the L_out form; no
+    reference implementation) over the batch's own cosine matrix at temperature ``temperature``: for each row with
+    another row of its label, the log-softmax over every other row of cos / temperature, averaged over the row's
+    positives; the loss is the mean over those rows.  A row whose label occurs once adds no term but is a negative in
+    every other row.  The definition is stated in full in ``include/dsk.h``.
+
+    With labels = the utterance index of each view (two augmented crops of each of B utterances, labels
+    ``arange(B).repeat(2)``) it is the NT-Xent loss of SimCLR (Chen et al., ICML 2020): self-supervised training
+    without speaker labels (see ``steps.supcon_step``).  With speaker labels it takes every positive pair in the batch.
+    ``temperature`` must be finite and > 0 (ValueError)."""
+
+    def __init__(self, temperature=0.1):
+        t = float(temperature)
+        if not math.isfinite(t) or t <= 0.0:
+            raise ValueError(f"SupConLoss: temperature must be finite and > 0, got {temperature!r}")
+        self.temperature = t
+
+    def forward(self, embeddings, labels):
+        """embeddings (N, D) CUDA (D a multiple of 64), labels (N,) int -> 0-dim device scalar; back-propagates into the
+        embeddings.  V comes from the labels on the host: with CPU labels, as a data loader yields them, nothing is read
+        back from the device; CUDA labels are read back once.  Raises ValueError when no row has a positive (V = 0) and
+        RuntimeError for a label count that does not match the embeddings, before any launch."""
+        V = supcon_valid_count(labels)
+        if V == 0:
+            raise ValueError("SupConLoss: no row has a positive (every label occurs once)")
+        n = torch.as_tensor(labels).numel()
+        if embeddings.dim() != 2 or n != embeddings.shape[0]:
+            raise RuntimeError(f"SupConLoss: {n} labels for embeddings of shape {tuple(embeddings.shape)}")
+        if not embeddings.is_cuda:
+            raise RuntimeError("SupConLoss needs CUDA embeddings; there is no CPU fallback")
+        return _engine.SupConFn.apply(embeddings, labels, V, self.temperature)
+
+    __call__ = forward
+
+
 def select_hard_triplets(d_p, d_n, margin):
     """Device-side restatement of train_triplet.py:251-262: returns (idx int64 (B,), count int32 (1,)) on the
     GPU; idx[:count] equals np.where((d_n - d_p < margin) == 1)[0].  No host synchronisation."""

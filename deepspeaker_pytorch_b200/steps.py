@@ -29,8 +29,8 @@ import torch.distributed as dist
 from . import engine as _engine
 from . import train as _train
 from .head import CrossEntropyLoss
-from .model import (AAMSoftmaxLoss, BatchHardTripletLoss, PairwiseDistance, TripletMarginLoss, batch_hard_valid_count,
-                    select_hard_triplets)
+from .model import (AAMSoftmaxLoss, BatchHardTripletLoss, PairwiseDistance, SupConLoss, TripletMarginLoss,
+                    batch_hard_valid_count, select_hard_triplets, supcon_valid_count)
 from .optim import FusedAdagrad
 from .parallel import GlobalBatchHardTripletLoss, GlobalGE2ELoss, GradBucket, _distributed, gather_labels
 
@@ -317,3 +317,38 @@ def _global_ge2e_step(model, optimizer, data, labels, loss, bucket):
     out.backward(torch.full_like(out, float(world)))         # R x this rank's share; the mean all-reduce divides by R
     _reduce_and_step(optimizer, bucket, None)
     return {"loss": out.detach(), "valid": V}
+
+
+def supcon_step(model, optimizer, data, labels, *, temperature, bucket=None):
+    """One supervised-contrastive step (``SupConLoss``): ONE train-mode forward of all N crops, the loss over the batch's
+    cosine matrix at ``temperature``, backward, optimizer step.  Returns ``{"loss": device scalar, "valid": V}``; raises
+    ValueError for a batch in which no row has a positive (V = 0).  V comes from the labels on the host: with CPU labels
+    the step reads nothing back from the device.  Runs unchanged on a model with ``sync_batchnorm()``.  Under data
+    parallelism (``bucket`` or a ``FusedAdagrad`` optimizer; ``data`` / ``labels`` this rank's shard, the same size on
+    every rank) each rank contrasts within its own shard and its gradient is weighted by its V_r, as in ``ge2e_step``.
+
+    Self-supervised training (SimCLR's NT-Xent; no speaker labels) takes two independently augmented views of each of
+    B utterances and labels each view with its utterance.  With a ``WaveBank`` ``bank``, a numpy generator ``g`` and
+    the utterance ids ``u`` (B,) of the batch::
+
+        utt = torch.cat([u, u])                                   # 2B examples, view v of utterance b at v B + b
+        L = segment_samples(T)
+        plan = augment_plan(2 * B, L, g, rir_bank=rirs, noise_bank=noises, noise_groups=groups, speeds=(0.9, 1.0, 1.1))
+        start = bank.random_starts(utt, L, g, plan)               # every example draws its own start and augmentation
+        x = bank.augmented_crops(utt, start, T, plan, rirs, noises)
+        supcon_step(model, opt, x, torch.arange(B).repeat(2), temperature=0.1)
+
+    With speaker labels instead, every pair of rows of one speaker is a positive."""
+    if not model.training:
+        raise RuntimeError("supcon_step needs model.train()")
+    crit = SupConLoss(temperature)
+    labels = torch.as_tensor(labels).detach().cpu()     # CUDA labels: the one read-back
+    V = supcon_valid_count(labels)
+    if V == 0:
+        raise ValueError("supcon_step: no row has a positive (every label occurs once)")
+    emb = model(data)
+    loss = crit.forward(emb, labels)
+    optimizer.zero_grad()
+    loss.backward()
+    _reduce_and_step(optimizer, bucket, torch.tensor(float(V)))
+    return {"loss": loss.detach(), "valid": V}

@@ -539,6 +539,43 @@ int32_t dsk_ge2e_bwd_rows(dsk_handle h, const float* E, int32_t N, int32_t D, co
                           const int64_t* offsets, const int64_t* col, int32_t P, const float* dcos, const float* tdc,
                           int32_t row0, int32_t rows, float* gE_rows, void* stream);
 
+/* Supervised-contrastive loss over the batch's own cosine matrix (Khosla et al., NeurIPS 2020, the L_out form; no
+ * reference implementation exists, and parity with any published one is unpinned).  With labels = the utterance index of
+ * each view it is the NT-Xent loss of SimCLR (Chen et al., ICML 2020): self-supervised training on augmented views of
+ * unlabelled speech.  For embeddings E (N,D), int64 labels y (any values) and a temperature tau:
+ *   e^_i = e_i / max(||e_i||, 1e-12) (F.normalize);  cos (N,N): cos_ij = e^_i . e^_j;  s_ij = cos_ij / tau;
+ *   P(i) = { j != i : y_j = y_i };  row i is valid iff P(i) is non-empty, V = the number of valid rows (unlike the
+ *   batch-hard rule, no second label is needed: a batch of one label is valid throughout);
+ *   lse_i = log sum_{j != i} exp(s_ij)  (the diagonal excluded, the positives included);
+ *   l_i = lse_i - (1/|P(i)|) sum_{p in P(i)} s_ip;  loss (1,) = (1/V) sum over valid i of l_i, summed in a fixed order.
+ *   A singleton row (no positive) has no loss term, but it is a negative in every other row.
+ * cos and lse are caller-owned outputs that dsk_supcon_bwd reads; V comes from the host (the labels' count, as for
+ * dsk_ge2e), so nothing is read back.  cos holds the GEMM's cosines, the diagonal (read by nothing) included.
+ * Accuracy: the cosines run on the AAM-softmax op's hi/lo fp16 tensor-core GEMM (fp16 whatever the handle's operand
+ * type: a bf16 handle gives the same bits), within ~1e-6 of fp64 (the truncated accumulation errs most where |cos| is
+ * near 1: ~1.6e-6 at D = 512); the positive pairs' cosines, where two views of one utterance sit close, are recomputed
+ * in fp64 from the fp32 rows and rounded once (cost O(sum_i |P(i)| D): N D for two views per utterance).  Each row's
+ * softmax denominator and positive sum are fp64 sums in a fixed order, lse and l_i rounded once.
+ * Non-finite input: a NaN or infinite element in row i makes cos row i and column i NaN, so every lse and the loss are
+ * NaN; the call still returns DSK_OK.
+ * The plan is the AAM op's for (N, N, D), cached in h in a slot of its own (the AAM, GE2E, scoring, search and all-pairs
+ * plans are untouched); a change of (N, D) rebuilds it, which synchronises the stream.  Its device memory at
+ * N = DSK_SUPCON_MAX_N, D = 512 is 7 717 847 040 bytes (7.19 GiB: 20 N^2 + N^2 D / 64 + 24 N D + 20 N bytes for N a
+ * multiple of 512), and the backward takes a stream-ordered workspace of 8 N D bytes (64 MiB there).
+ * 2 <= N <= DSK_SUPCON_MAX_N, D a positive multiple of 64, 1 <= V <= N, tau finite and > 0, non-null pointers, else
+ * DSK_ERR_INVALID before any launch, outputs untouched. */
+#define DSK_SUPCON_MAX_N 16384
+int32_t dsk_supcon(dsk_handle h, const float* E, const int64_t* labels, int32_t N, int32_t D, int32_t V, float tau,
+                   float* loss, float* cos, float* lse, void* stream);
+/* Its backward: gE (N,D) = d loss / d E scaled by grad_loss (device scalar), WRITTEN not accumulated.  On valid rows,
+ * for j != i: dS_ij = grad_loss / V * (exp(s_ij - lse_i) - [j in P(i)] / |P(i)|), taken at the forward's cos with the
+ * probabilities normalised by their own sum (the rounding of the saved lse cancels); dS is exactly 0 on the diagonal
+ * and on invalid rows; dC = dS / tau.  In e^-space g^ = dC E^ + dC^T E^ (the AAM plan's two backward GEMMs in fixed K
+ * slices, the two products added in that order), then gE_i = (g^_i - e^_i (e^_i . g^_i)) / max(||e_i||, 1e-12).
+ * Deterministic: no float atomics, two calls give the same bits.  Limits as dsk_supcon. */
+int32_t dsk_supcon_bwd(dsk_handle h, const float* E, const int64_t* labels, const float* cos, const float* lse,
+                       int32_t N, int32_t D, int32_t V, float tau, const float* grad_loss, float* gE, void* stream);
+
 /* Cosine scoring of verification trials with adaptive symmetric score normalisation (AS-norm) against an impostor
  * cohort (no reference implementation exists; the reference scores Euclidean distances, eval_metrics.py:5-50).  Rows are
  * normalised as in F.normalize, x^ = x / max(||x||, 1e-12).
